@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — headline benchmark of blance_b200 (contract: see the task statement).
+"""bench.py — headline benchmark of blance_b200.
 
 Metric (BASELINE.json): partition-assignments/sec on the 1 048 576-partition x
 1 024-node synthetic cluster (configs[3]: heterogeneous node + partition weights,
@@ -13,7 +13,8 @@ complete PlanNextMapEx (all convergence iterations, plan.go:23-58).
               all kernels, D2H inside the timed region
   roofline    of the dominant kernel k_assign_pass_spec: algorithmic bytes per findBestNodes
               step (SURVEY.md section 8d: 16*N + (N/8)(1+R*k) + 8*slots + 12) x steps /
-              its device time, against the measured HBM copy bandwidth
+              its device time, against the HBM bandwidth (MEASURED_PEAKS.json when present,
+              else the H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline  the literal C++ restatement of the Go planner (oracle/literal.cpp: string
               hash maps + comparison sort, the reference's asymptotics) on a bounded
               sample of the same cluster shape, 1 core (the reference planner is
@@ -28,6 +29,10 @@ previous step wrote), so one plan does not shard; N ranks plan the SAME cluster,
 per GPU — "replicas only", weak scaling, no collective in the data path;
 torch.distributed(nccl) is used for the barrier and the max over ranks.  What shards is the
 batch: tools/bench_cfg5.py runs config 5 over 1/2/4/8 GPUs through blance_ctx_create_multi.
+
+--dump-outputs DIR: after the timed steps, the arrays the timed path computed in its last step (the
+next map's rows, shapes and warnings, plus its iteration and step counts) go to DIR/<name>.npy as float32 /
+float64, so that two builds can be compared output for output on identical seeded inputs.
 
 --impl reference: the CPU arm — slices of the real workload's first inner plan through the
 literal oracle on the box's host cores (rank 0 only).
@@ -59,7 +64,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -154,15 +159,18 @@ def cpu_fast_sample(parts):
     return r.steps, time.perf_counter() - t0
 
 
-def ncu_traffic(steps_per_launch):
-    """DRAM bytes per k_assign_pass launch from the committed ncu --set full capture
-    (profiles/ncu_traffic.json: dram read+write bytes per step of one captured launch), scaled to
-    the bench's steps per launch; None when no capture is committed."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return float(json.load(f)["dram_bytes_per_step"]) * steps_per_launch
-    except Exception:
-        return None
+def dump_outputs(out_dir, res):
+    """What a caller of the resident plan receives from blance_plan_fetch after the last timed run: the next map as
+    rows (node ids, -1 = empty slot), per-state list shapes and warning flags, and the iteration count, the
+    convergence flag and the number of findBestNodes steps.  Node ids are
+    below 2^24, so float32 holds them exactly; the whole dump of the headline cluster is 28 MB."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"next_rows": res.next_rows.astype(np.float32), "next_shape": res.next_shape.astype(np.float32),
+              "warn": res.warn.astype(np.float32),
+              "counters": np.array([res.iters_run, res.converged, res.steps], np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def shared_config(n_parts, n_nodes):
@@ -213,7 +221,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-string-api", action="store_true")
     ap.add_argument("--no-batch", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32 / float64); GPU path only")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes what the GPU path computed; --impl reference has no such outputs")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -244,7 +258,7 @@ def main():
     t = synth.make_rebalance(CFG, P=args.parts)
     ctx = tables.Context(local_rank)
     plan = ctx.upload(t)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > L2 (126 MB)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > L2 (50 MB on H100)
 
     for _ in range(max(args.warmup, 3)):
         ctx.run(plan)
@@ -268,6 +282,8 @@ def main():
     barrier()
     launches = ctx.kernel_launches() - launches0
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ctx.fetch(plan, tables.PlanResult(t)))
     total_ms = sum(kernel_ms)
     tt = torch.tensor([total_ms, sum(pass_ms)], dtype=torch.float64, device=dev)
     if dist is not None:
@@ -304,8 +320,9 @@ def main():
     # ---- CalcPartitionMoves over the whole map (prev -> next), through the C ABI with host buffers -----
     ctx.calc_partition_moves(t.state_slot_off, t.prev_rows, out.next_rows, False)
     t0 = time.perf_counter()
-    mv = ctx.calc_partition_moves(t.state_slot_off, t.prev_rows, out.next_rows, False)
-    moves_s = time.perf_counter() - t0
+    for _ in range(args.steps):
+        mv = ctx.calc_partition_moves(t.state_slot_off, t.prev_rows, out.next_rows, False)
+    moves_s = (time.perf_counter() - t0) / args.steps
     moves_ops = int(mv[3].sum())
 
     # ---- outside every timed region: the result's digest next to the oracle's (profiles/parity_cfg4.json, written by
@@ -330,17 +347,19 @@ def main():
         removed = np.nonzero(t.node_removed)[0].tolist()
         added = np.nonzero(t.node_added)[0].tolist()
         reps = []
-        for _ in range(2):       # the first call pays the page faults of its fresh allocations
+        for _ in range(1 + args.steps):       # the first call pays the page faults of its fresh allocations: not timed
             d = blance_b200._host.bench_string_api(t.prev_rows, t.n_nodes, [int(x) for x in t.state_constraints], removed, added,
                                                    t.node_weight, t.part_weight, t.part_has_weight, [int(x) for x in t.state_stickiness], 10)
             reps.append(d)
-        d = reps[-1]
-        string_api = {"value": t.n_parts / (d["total_ms"] / 1e3), "unit": UNIT, "ms": d["total_ms"], "first_call_ms": reps[0]["total_ms"],
-                      "intern_ms": d["intern_ms"], "c_abi_call_ms": d["call_ms"], "unintern_ms": d["unintern_ms"],
-                      "caller_map_mutation_ms": d["mutate_ms"], "host_threads": d["host_threads"],
+
+        def mean(key):
+            return statistics.mean(r[key] for r in reps[1:])
+        string_api = {"value": t.n_parts / (mean("total_ms") / 1e3), "unit": UNIT, "ms": mean("total_ms"), "first_call_ms": reps[0]["total_ms"],
+                      "intern_ms": mean("intern_ms"), "c_abi_call_ms": mean("call_ms"), "unintern_ms": mean("unintern_ms"),
+                      "caller_map_mutation_ms": mean("mutate_ms"), "host_threads": d["host_threads"],
                       "result_equals_resident_run": bool(np.array_equal(d["next_rows"], res.next_rows)),
                       "note": "blance.PlanNextMapEx of the C++ host twin (host_api.cpp) on %d string partitions; what a Go host "
-                              "pays when it does not keep its maps interned" % t.n_parts}
+                              "pays when it does not keep its maps interned; mean of --steps calls after one untimed call" % t.n_parts}
 
     # ---- BASELINE config 5 on this GPU: 1 024 independent instances (multi-tenant fan-out) in one batch call; the struct
     # arrays are built once, the timed call is blance_plan_next_map_batch alone (H2D, all kernels, D2H inside)
@@ -354,7 +373,7 @@ def main():
         prep2 = ctx.prepare_batch(rebs)
         ctx.run_batch(prep2)                                  # warm-up
         ts_ = []
-        for _ in range(3):
+        for _ in range(args.steps):
             t0 = time.perf_counter()
             r5 = ctx.run_batch(prep2)
             ts_.append(time.perf_counter() - t0)
@@ -363,7 +382,7 @@ def main():
         batch = {"workload": "cfg5: %d independent PlanNextMapEx instances (1024 partitions x 64 nodes, rack rules), rebalance stage" % n_inst,
                  "value": parts5 / best, "unit": UNIT, "ms": 1e3 * best, "instances_per_s": n_inst / best,
                  "device_ms": float(r5[0].device_ms), "n_gpus": 1,
-                 "note": "wall time of the C call with host buffers; multi-GPU sharding of the batch: tools/bench_cfg5.py, profiles/"}
+                 "note": "wall time of the C call with host buffers; multi-GPU sharding of the batch: tools/bench_cfg5.py"}
 
     if rank == 0:
         P, N = t.n_parts, t.n_nodes
@@ -391,14 +410,13 @@ def main():
                     "ms_per_step": 1e3 * e2e_total / args.steps, "result_equals_resident_run": same},
             "calc_partition_moves": {"partitions_per_s": P / moves_s, "ms": 1e3 * moves_s, "ops": moves_ops,
                                      "note": "moves.go:41-119 for all partitions in one launch, prevMap -> nextMap, host buffers "
-                                             "(H2D of both maps and D2H of the op lists inside the timed call)"},
+                                             "(H2D of both maps and D2H of the op lists inside the timed call); mean of --steps calls"},
             "e2e_string_api": string_api,
             "batch_cfg5": batch,
             "gpu_launches": int(launches),
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "k_assign_pass_spec (the speculative assign pass; k_assign_pass runs the passes that do not qualify)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": ncu_traffic(steps_per_plan * args.steps / max(1, pass_launches)),
-                         "peak_source": peak_src, "bytes_per_findBestNodes_step": bytes_per_step,
+                         "frac": (achieved / peak) if achieved else None, "peak_source": peak_src, "bytes_per_findBestNodes_step": bytes_per_step,
                          "steps_per_launch": steps_per_plan * args.steps / max(1, pass_launches),
                          "t_step_ns": 1e9 * pass_s / (steps_per_plan * args.steps),
                          "note": "the pass is a loop-carried dependency chain (latency bound), not a streaming kernel; "

@@ -1,4 +1,4 @@
-"""blance_b200 — a B200-native (sm_100a) drop-in for the hot path of couchbase/blance:
+"""blance_b200 — an H100-native (sm_90a) drop-in for the hot path of couchbase/blance:
 PlanNextMapEx (api.go:147-157; plan.go:23-331) and CalcPartitionMoves (moves.go:41-119).
 
 The product is the C-ABI library `blance_b200/lib/libblance_b200.so`

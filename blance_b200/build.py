@@ -1,7 +1,7 @@
-"""In-tree build of the native pieces (no JIT cache: the .so files must travel to
-the GPU box with the repo snapshot).
+"""In-tree build of the native pieces (no JIT cache: the .so files live in the source tree, so that a
+copy of the built tree runs on another machine without compiling again).
 
-    libblance_b200.so   nvcc, sm_100a only: the CUDA kernels + the C ABI (include/blance_b200.h)
+    libblance_b200.so   nvcc, sm_90a (H100) only: the CUDA kernels + the C ABI (include/blance_b200.h)
     _host*.so           g++: the C++ host mirror of blance's api.go (pybind11 face), linked
                         against libblance_b200.so
 
@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 INCLUDE = os.path.join(ROOT, "include")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-fmad=false",           # the score of plan.go:634-689 is never fused
               "-Xcompiler", "-fPIC", "-shared", "-cudart", "static"]
 

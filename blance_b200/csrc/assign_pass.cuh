@@ -4,7 +4,7 @@
 // The pass is a loop-carried chain: every step reads the node counts the previous
 // step wrote (plan.go:286-301), so partitions are walked strictly in the
 // reference's order by ONE CTA per plan instance, while the N candidate nodes of a
-// step are scored in parallel.  Measured (profiles/): the chain is bound by the
+// step are scored in parallel.  The chain is bound by the
 // latency of the serial instruction path of one step, not by memory or issue
 // bandwidth, so the kernel is organised to keep that path short:
 //

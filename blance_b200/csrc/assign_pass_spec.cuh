@@ -63,7 +63,10 @@ namespace blance_dev {
 #define SP_SCAN2 1
 #endif
 #ifndef SP_LB
-#define SP_LB 512            // launch bound (the register budget follows from it: 544 -> 96, 512 -> 128, 384 -> 168)
+// launch bound = the widest launch (12 warps); the register budget follows from it: 512 -> 128, 384 -> 168.  On
+// sm_90a 128 registers spill ~180 bytes per thread; 168 keeps ~16 and is 1.9 % faster on the headline plan (H100 SXM,
+// profiles/README.md).
+#define SP_LB 384
 #endif
 #ifndef SP_U
 #define SP_U 1               // groups of 32 steps the leader examines per scan (independent instruction streams)

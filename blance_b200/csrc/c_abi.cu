@@ -35,7 +35,7 @@ static size_t g_spec_dyn[64][4];     // [device][K - 1], k_assign_pass_spec
 
 struct blance_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   std::string err;
   std::mutex mu;

@@ -82,8 +82,7 @@ __device__ __noinline__ double q_over_p_slow(int32_t q, double Pd, double Py);
 __device__ __noinline__ double q_over_p_slow(int32_t q, double Pd, double Py) { return div_exact((double)q, Pd, Py); }
 
 // atomic add without a return value.  atomicAdd() with an unused result compiles to ATOMG ... RZ here, not RED: the
-// warp then holds a scoreboard for the L2 round trip and stalls on it at its next branch (37 % of the leader's scan
-// time in the ncu source view).  red.* is the same relaxed, device-scope atomic and nothing waits for it.
+// warp then holds a scoreboard for the L2 round trip and stalls on it at its next branch.  red.* is the same relaxed, device-scope atomic and nothing waits for it.
 __device__ __forceinline__ void red_add(int32_t* p, int32_t v) {
   asm volatile("red.relaxed.gpu.global.add.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
 }

@@ -1,4 +1,4 @@
-/* include/blance_b200.h — C ABI of libblance_b200.so (B200 / sm_100a).
+/* include/blance_b200.h — C ABI of libblance_b200.so (H100 / sm_90a).
  *
  * This is the drop-in boundary for blance's planner hot path.  The reference
  * (couchbase/blance, pure Go) has no FFI of its own: its boundary is the

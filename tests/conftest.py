@@ -1,6 +1,6 @@
 """pytest configuration: registers the `gpu` marker and makes the repo root and
 oracle/ importable.  `-m "not gpu"` runs on the CPU-only builder; `-m gpu` runs
-on a B200 box and goes through the C ABI of libblance_b200.so."""
+on an H100 and goes through the C ABI of libblance_b200.so."""
 import os
 import sys
 
@@ -11,4 +11,4 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu on a GPU machine")

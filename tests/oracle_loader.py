@@ -1,6 +1,6 @@
 """Loads the CPU oracles (oracle/ — TEST INFRASTRUCTURE).  Builds them on demand
 with oracle/Makefile when the shared objects are missing (they are git-ignored
-but travel to the GPU box with the gpurun snapshot)."""
+build products that __graft_entry__.build() normally leaves in oracle/)."""
 import glob
 import importlib
 import os

@@ -2,7 +2,7 @@
 libblance_b200.so (directly, or underneath the C++ host mirror), against the
 reference's golden vectors and against the CPU oracle on identical tables.
 Integer/index work: the bar is bit-exact rows, shapes, warnings, iteration and step
-counts.  Needs a B200; run with `-m gpu`."""
+counts.  Needs an H100; run with `-m gpu`."""
 import copy
 import ctypes
 

@@ -2,10 +2,10 @@
 
 * no value-less atomic compiled WITH a return value (`ATOMG ... PT, RZ`): the pass kernels' atomicAdd calls whose
   result nobody reads were emitted that way, and the speculative kernel's leader then waited for an L2 round trip at
-  its next branch - 37 % of its scan time (profiles/r2_spec_experiments.md).  They go through red_add()
+  its next branch.  They go through red_add()
   (pass_common.cuh) now; this guards the next edit.
 * the speculative pass kernel is fed by TMA bulk copies completing on an mbarrier (UBLKCP / SYNCS) and reduces
-  with redux.sync (CREDUX): the sm_100a instructions DESIGN.md section 3 describes are really in the binary."""
+  with redux.sync (REDUX): the sm_90a instructions DESIGN.md section 3 describes are really in the binary."""
 import re
 import shutil
 import subprocess
@@ -46,5 +46,5 @@ def test_speculative_pass_kernel_uses_tma_mbarrier_redux_and_red(kernels):
     assert len(spec) == 4                                  # K = 1 .. 4
     for k, ls in spec.items():
         body = "\n".join(ls)
-        for op in ("UBLKCP", "SYNCS", "CREDUX", "REDG"):
+        for op in ("UBLKCP", "SYNCS", "REDUX", "REDG"):
             assert op in body, (k, op)

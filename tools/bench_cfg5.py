@@ -4,7 +4,7 @@ one host thread per device, no collective.  The struct arrays are built once; th
 blance_plan_next_map_batch alone (host buffers: H2D, all kernels, D2H inside).  Every instance of the last run is
 compared with the array oracle on 32 sampled instances (the -m gpu test checks all of a 160-instance batch).
 
-    python tools/bench_cfg5.py [--gpus 1,2,4,8] [--instances 1024] > profiles/r2_cfg5_scale.json
+    python tools/bench_cfg5.py [--gpus 1,2,4,8] [--instances 1024] > cfg5_scale.json
 """
 import argparse, ctypes, json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -5,6 +5,6 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; shift
 mkdir -p tools/_timing
-${NVCC:-/usr/local/cuda/bin/nvcc} -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -fmad=false \
+${NVCC:-/usr/local/cuda/bin/nvcc} -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false \
   -Xcompiler -fPIC -shared -cudart static -DBLANCE_SPEC_TIMING "$@" -Iinclude -Iblance_b200/csrc \
   blance_b200/csrc/c_abi.cu -o tools/_timing/lib_$name.so
