@@ -18,8 +18,8 @@ from . import build as _build
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
 _API_NAMES = ("BOOSTER_CBGT_MAX", "BOOSTER_NONE", "BlanceError", "CalcPartitionMoves", "CalcPartitionMovesMap",
-              "NodeStateOp", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "capi")
-__all__ = ["PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "CalcPartitionMoves", "CalcPartitionMovesMap",
+              "NodeStateOp", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "capi")
+__all__ = ["PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "CalcPartitionMoves", "CalcPartitionMovesMap",
            "NodeStateOp", "BlanceError", "BOOSTER_NONE", "BOOSTER_CBGT_MAX", "capi"]
 
 

@@ -33,9 +33,22 @@ class _PlanOut(ctypes.Structure):
                 ("sticky_steps", ctypes.c_int64)]
 
 
+class _Scenario(ctypes.Structure):     # struct blance_scenario
+    _fields_ = [("node_removed", ctypes.c_void_p), ("node_added", ctypes.c_void_p), ("add_is_nil", ctypes.c_int32),
+                ("has_node_weights", ctypes.c_int32), ("node_weight", ctypes.c_void_p), ("node_has_weight", ctypes.c_void_p)]
+
+
+class _ScenarioOut(ctypes.Structure):  # struct blance_scenario_out
+    _fields_ = [("next_rows", ctypes.c_void_p), ("next_shape", ctypes.c_void_p), ("warn", ctypes.c_void_p),
+                ("node_ops", ctypes.c_void_p), ("state_node_load", ctypes.c_void_p),
+                ("iters_run", ctypes.c_int32), ("converged", ctypes.c_int32), ("steps", ctypes.c_int64),
+                ("sticky_steps", ctypes.c_int64), ("parts_moved", ctypes.c_int64), ("ops_total", ctypes.c_int64),
+                ("warn_parts", ctypes.c_int64)]
+
+
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available", "blance_moves_free")
 
 
@@ -57,6 +70,7 @@ def capi():
         lib.blance_plan_in_check.argtypes = [vp, ctypes.c_char_p, i32]
         lib.blance_plan_next_map.argtypes = [vp, vp, vp]
         lib.blance_plan_next_map_batch.argtypes = [vp, i32, vp, vp]
+        lib.blance_plan_scenarios.argtypes = [vp, vp, i32, vp, i32, i32, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
         lib.blance_plan_run.argtypes = [vp, vp]
         lib.blance_plan_fetch.argtypes = [vp, vp, vp]
@@ -76,3 +90,5 @@ def capi():
 
 PlanIn = _PlanIn
 PlanOut = _PlanOut
+Scenario = _Scenario
+ScenarioOut = _ScenarioOut

@@ -72,6 +72,52 @@ def PlanNextMap(prevMap, partitionsToAssign, nodesAll, nodesToRemove, nodesToAdd
                                             nodeHierarchy, hierarchyRules))
 
 
+def _scenario_tuples(scenarios):
+    out = []
+    for i, sc in enumerate(scenarios):
+        missing = {"nodesToRemove", "nodesToAdd"} - set(sc)
+        if missing:
+            raise ValueError("scenario %d lacks %s" % (i, ", ".join(sorted(missing))))
+        rm, ad = sc["nodesToRemove"], sc["nodesToAdd"]
+        out.append((None if rm is None else list(rm), None if ad is None else list(ad), "nodeWeights" in sc,
+                    None if sc.get("nodeWeights") is None else dict(sc["nodeWeights"])))
+    return out
+
+
+def _option_kwargs(o):
+    return dict(model_state_constraints=o.ModelStateConstraints, partition_weights=o.PartitionWeights,
+                state_stickiness=o.StateStickiness, node_weights=o.NodeWeights, node_hierarchy=o.NodeHierarchy,
+                hierarchy_rules=None if o.HierarchyRules is None else {k: [tuple(x) for x in v] for k, v in o.HierarchyRules.items()},
+                booster=o.NodeScoreBooster, max_iterations=o.MaxIterationsPerPlan, engine=o.Engine)
+
+
+def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=None, scenarios=(), favorMinNodes=False,
+                         wantMaps=(), maxConcurrent=0):
+    """What-if variants of one cluster, planned side by side on the device.  Scenario i is
+    PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, sc["nodesToRemove"], sc["nodesToAdd"], model, options with
+    NodeWeights = sc["nodeWeights"]): both node-set keys are required (None = nil); a missing "nodeWeights" key
+    inherits options.NodeWeights, None means nil.  The caller's maps are NOT mutated.
+
+    Returns one dict per scenario: iterations, converged, steps, sticky_steps, parts_moved, ops_total, warn_parts,
+    node_ops {node: {op: count}} and state_node_load {state: {node: load}} (nonzero entries only), plus next_map and
+    warnings for the indices in wantMaps."""
+    o = options or PlanNextMapOptions()
+    same = prevMap is partitionsToAssign
+    return _host.PlanNextMapScenarios(prevMap, None if same else partitionsToAssign, list(nodesAll),
+                                      {k: tuple(v) for k, v in model.items()}, _scenario_tuples(scenarios),
+                                      bool(favorMinNodes), [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o))
+
+
+def intern_scenario(prevMap, partitionsToAssign, nodesAll, model, options, scenarios, index):
+    """The blance_plan_in of scenario `index` of PlanNextMapScenarios as an interned plan (_host.InternedPlan), for
+    running a CPU oracle on exactly the tables the device plans."""
+    o = options or PlanNextMapOptions()
+    same = prevMap is partitionsToAssign
+    return _host.intern_scenario(prevMap, None if same else partitionsToAssign, list(nodesAll),
+                                 {k: tuple(v) for k, v in model.items()}, _scenario_tuples(scenarios), int(index),
+                                 **_option_kwargs(o))
+
+
 def CalcPartitionMoves(states, begNodesByState, endNodesByState, favorMinNodes):
     return [NodeStateOp(*t) for t in _host.CalcPartitionMoves(list(states), begNodesByState, endNodesByState,
                                                               bool(favorMinNodes))]
@@ -84,4 +130,4 @@ def CalcPartitionMovesMap(states, begMap, endMap, favorMinNodes):
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------
-from .abi import EXPORTS, PlanIn, PlanOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401
+from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401

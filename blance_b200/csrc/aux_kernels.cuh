@@ -379,7 +379,37 @@ __global__ void k_next_iter(DPool pool, int n_inst, int* any_active) {
   atomicAdd(any_active, 1);
 }
 
-// ---- CalcPartitionMoves (moves.go:41-136), one thread per partition ------------------------------------------
+// ---- CalcPartitionMoves (moves.go:41-136) of one partition ----------------------------------------------------
+// beg / end: rows of the slot layout slot_off (SL slots are scanned for set membership).  Calls
+// emit(node, state, kind) for every candidate op in the reference's order; emit applies addMoves' "seen" rule.
+template <class Emit>
+__device__ __forceinline__ void calc_moves_row(const int32_t* beg, const int32_t* end, const int32_t* slot_off, int SL,
+                                               int n_visit, int favor_min, Emit&& emit) {
+  auto in_row = [&](const int32_t* row, int32_t node) { bool r = false; for (int i = 0; i < SL; ++i) r |= (row[i] == node); return r; };
+  for (int step = 0; step < n_visit; ++step) {
+    const int si = favor_min ? n_visit - 1 - step : step;
+    const int lo = slot_off[si], hi = slot_off[si + 1];
+    for (int phase = 0; phase < 4; ++phase) {
+      // !favorMinNodes: promote, demote, add, del (moves.go:66-90); favorMinNodes: del, demote, promote, add (:92-116)
+      const int what = favor_min ? (phase == 0 ? 3 : phase == 1 ? 1 : phase == 2 ? 0 : 2) : phase;
+      if (what <= 1) {                      // findStateChanges, moves.go:121-136
+        const int jlo = what == 0 ? si + 1 : 0, jhi = what == 0 ? n_visit : si;
+        for (int i = lo; i < hi && end[i] != BLANCE_NO_NODE; ++i)
+          for (int j = jlo; j < jhi; ++j)
+            for (int b = slot_off[j]; b < slot_off[j + 1] && beg[b] != BLANCE_NO_NODE; ++b)
+              if (beg[b] == end[i]) emit(end[i], si, what == 0 ? BLANCE_OP_PROMOTE : BLANCE_OP_DEMOTE);
+      } else if (what == 2) {               // end[s] \ beg[s], restricted to adds = endAll \ begAll
+        for (int i = lo; i < hi && end[i] != BLANCE_NO_NODE; ++i)
+          if (!in_row(beg, end[i])) emit(end[i], si, BLANCE_OP_ADD);
+      } else {                              // beg[s] \ end[s], restricted to dels = begAll \ endAll
+        for (int i = lo; i < hi && beg[i] != BLANCE_NO_NODE; ++i)
+          if (!in_row(end, beg[i])) emit(beg[i], BLANCE_OP_STATE_NONE, BLANCE_OP_DEL);
+      }
+    }
+  }
+}
+
+// one thread per partition
 __global__ void k_calc_moves(int32_t n_parts, int32_t n_states, int32_t n_visit, const int32_t* __restrict__ slot_off,
                              const int32_t* __restrict__ beg_rows, const int32_t* __restrict__ end_rows,
                              int32_t favor_min, int32_t max_ops, int32_t* __restrict__ op_node,
@@ -388,39 +418,118 @@ __global__ void k_calc_moves(int32_t n_parts, int32_t n_states, int32_t n_visit,
   const int SL = slot_off[n_states];
   for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < n_parts;
        p += (long long)gridDim.x * blockDim.x) {
-    const int32_t* beg = beg_rows + p * SL;
-    const int32_t* end = end_rows + p * SL;
     int32_t* on = op_node + p * max_ops;
     uint8_t* os = op_state + p * max_ops;
     uint8_t* ok = op_kind + p * max_ops;
     int cnt = 0;
-    auto in_row = [&](const int32_t* row, int32_t node) { bool r = false; for (int i = 0; i < SL; ++i) r |= (row[i] == node); return r; };
-    auto emit = [&](int32_t node, int st, int kind) {                 // addMoves + seen, moves.go:51-58
-      for (int j = 0; j < cnt; ++j) if (on[j] == node) return;
+    calc_moves_row(beg_rows + p * SL, end_rows + p * SL, slot_off, SL, n_visit, favor_min, [&](int32_t node, int st, int kind) {
+      for (int j = 0; j < cnt; ++j) if (on[j] == node) return;       // addMoves + seen, moves.go:51-58
       if (cnt < max_ops) { on[cnt] = node; os[cnt] = (uint8_t)st; ok[cnt] = (uint8_t)kind; ++cnt; }
-    };
-    for (int step = 0; step < n_visit; ++step) {
-      const int si = favor_min ? n_visit - 1 - step : step;
-      const int lo = slot_off[si], hi = slot_off[si + 1];
-      for (int phase = 0; phase < 4; ++phase) {
-        // !favorMinNodes: promote, demote, add, del (moves.go:66-90); favorMinNodes: del, demote, promote, add (:92-116)
-        const int what = favor_min ? (phase == 0 ? 3 : phase == 1 ? 1 : phase == 2 ? 0 : 2) : phase;
-        if (what <= 1) {                      // findStateChanges, moves.go:121-136
-          const int jlo = what == 0 ? si + 1 : 0, jhi = what == 0 ? n_visit : si;
-          for (int i = lo; i < hi && end[i] != BLANCE_NO_NODE; ++i)
-            for (int j = jlo; j < jhi; ++j)
-              for (int b = slot_off[j]; b < slot_off[j + 1] && beg[b] != BLANCE_NO_NODE; ++b)
-                if (beg[b] == end[i]) emit(end[i], si, what == 0 ? BLANCE_OP_PROMOTE : BLANCE_OP_DEMOTE);
-        } else if (what == 2) {               // end[s] \ beg[s], restricted to adds = endAll \ begAll
-          for (int i = lo; i < hi && end[i] != BLANCE_NO_NODE; ++i)
-            if (!in_row(beg, end[i])) emit(end[i], si, BLANCE_OP_ADD);
-        } else {                              // beg[s] \ end[s], restricted to dels = begAll \ endAll
-          for (int i = lo; i < hi && beg[i] != BLANCE_NO_NODE; ++i)
-            if (!in_row(end, beg[i])) emit(beg[i], BLANCE_OP_STATE_NONE, BLANCE_OP_DEL);
-        }
-      }
-    }
+    });
     op_count[p] = cnt;
+  }
+}
+
+// ---- what-if scenarios of one cluster (blance_plan_scenarios) -----------------------------------------------
+// The base's partition slices, unpacked once per device, are copied into every instance of a wave.  Base arrays
+// are indexed by the base partition; instance i owns partitions [i * PU, (i + 1) * PU) of the wave.
+__global__ void k_scenario_replicate(int32_t* __restrict__ rows_init, int32_t* __restrict__ prev_rows_init,
+                                     uint32_t* __restrict__ pmeta_init, uint32_t* __restrict__ prev_meta_init,
+                                     uint8_t* __restrict__ pflags_init, int32_t* __restrict__ pweight,
+                                     int32_t* __restrict__ rank, int32_t* __restrict__ inst,
+                                     const int32_t* __restrict__ b_rows, const int32_t* __restrict__ b_prev_rows,
+                                     const uint32_t* __restrict__ b_pmeta, const uint32_t* __restrict__ b_prev_meta,
+                                     const uint8_t* __restrict__ b_pflags, const int32_t* __restrict__ b_pweight,
+                                     const int32_t* __restrict__ b_rank, int32_t PU, int32_t SLP, long long n_parts_total) {
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < n_parts_total;
+       g += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(g / PU);
+    const long long p = g - (long long)i * PU;
+    for (int c = 0; c < SLP; ++c) {
+      rows_init[g * SLP + c] = b_rows[p * SLP + c];
+      prev_rows_init[g * SLP + c] = b_prev_rows[p * SLP + c];
+    }
+    pmeta_init[g] = b_pmeta[p];
+    prev_meta_init[g] = b_prev_meta[p];
+    pflags_init[g] = b_pflags[p];
+    pweight[g] = b_pweight[p];
+    rank[g] = b_rank[p];
+    inst[g] = i;
+  }
+}
+
+// Per instance: CalcPartitionMoves(prev row as uploaded -> next row) of every assigned partition, counted per
+// node and op kind; countStateNodes of the final map per state and node; partitions with an op / a warning.
+// out[i] = node_ops [NU][4] | state_node_load [S][NU] | parts_moved, ops_total, warn_parts  (int64, stride
+// `stride`).  Grid: x strides over the partitions of instance blockIdx.y.  SMEM: the node tables of one instance
+// live in shared memory (ops as u32, loads as i64) and are flushed once per CTA.
+template <bool SMEM>
+__global__ void k_scenario_summary(DPool pool, const int32_t* __restrict__ prev_rows_init, const uint8_t* __restrict__ pflags_init,
+                                   int32_t favor_min, long long stride, long long* __restrict__ out) {
+  extern __shared__ __align__(8) unsigned char sm[];
+  const int inst = blockIdx.y;
+  const DInst& D = pool.insts[inst];
+  const int NU = D.NU, S = D.S;
+  long long* o = out + (long long)inst * stride;
+  uint32_t* s_ops = reinterpret_cast<uint32_t*>(sm);
+  long long* s_load = reinterpret_cast<long long*>(sm + (((size_t)NU * 4 * sizeof(uint32_t) + 7) & ~(size_t)7));
+  if (SMEM) {
+    for (int x = threadIdx.x; x < NU * 4; x += blockDim.x) s_ops[x] = 0;
+    for (int x = threadIdx.x; x < S * NU; x += blockDim.x) s_load[x] = 0;
+    __syncthreads();
+  }
+  uint32_t moved = 0, n_ops = 0, warned = 0;
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < D.PU; p += (long long)gridDim.x * blockDim.x) {
+    const long long g = D.part_off + p;
+    const uint8_t f = pflags_init[g];
+    const bool assigned = (f & PF_IN_ASSIGN) != 0;
+    if (!assigned && !(f & PF_IN_PREV)) continue;
+    const int32_t* next = pool.rows + D.rows_off + p * D.SLP;
+    const int32_t* prev = prev_rows_init + D.rows_off + p * D.SLP;
+    const int32_t* fin = assigned ? next : prev;               // the final map: prevMap with the assigned rows replaced
+    const long long w = (D.has_part_weights && (f & PF_HAS_WEIGHT)) ? (long long)pool.pweight[g] : 1ll;
+    for (int s = 0; s < S; ++s)                                // countStateNodes, plan.go:374-399
+      for (int c = D.state_slot_off[s]; c < D.state_slot_off[s + 1] && fin[c] != BLANCE_NO_NODE; ++c) {
+        if (fin[c] < 0 || fin[c] >= NU) continue;
+        if (SMEM) atomicAdd(reinterpret_cast<unsigned long long*>(&s_load[s * NU + fin[c]]), (unsigned long long)w);
+        else atomicAdd(reinterpret_cast<unsigned long long*>(&o[4ll * NU + (long long)s * NU + fin[c]]), (unsigned long long)w);
+      }
+    if (!assigned) continue;
+    warned += ((pool.pmeta[g] >> 16) & 0xFFu) ? 1u : 0u;
+    int32_t seen[2 * BL_SLP_MAX];
+    int cnt = 0;
+    auto emit = [&](int32_t node, int, int kind) {
+      for (int j = 0; j < cnt; ++j) if (seen[j] == node) return;   // addMoves + seen, moves.go:51-58
+      seen[cnt++] = node;
+      if (node < 0 || node >= NU) return;
+      if (SMEM) atomicAdd(&s_ops[node * 4 + kind], 1u);
+      else atomicAdd(reinterpret_cast<unsigned long long*>(&o[(long long)node * 4 + kind]), 1ull);
+    };
+    if (f & PF_IN_PREV) calc_moves_row(prev, next, D.state_slot_off, D.SL, S, favor_min, emit);
+    else {                                                     // absent from prevMap: an empty beg row
+      int32_t blank[BL_SLP_MAX];
+      for (int c = 0; c < BL_SLP_MAX; ++c) blank[c] = BLANCE_NO_NODE;
+      calc_moves_row(blank, next, D.state_slot_off, D.SL, S, favor_min, emit);
+    }
+    moved += cnt > 0 ? 1u : 0u;
+    n_ops += (uint32_t)cnt;
+  }
+  // warp-aggregated scalars: one atomic per warp and counter
+  moved = __reduce_add_sync(0xFFFFFFFFu, moved);
+  n_ops = __reduce_add_sync(0xFFFFFFFFu, n_ops);
+  warned = __reduce_add_sync(0xFFFFFFFFu, warned);
+  if ((threadIdx.x & 31) == 0) {
+    long long* sc = o + 4ll * NU + (long long)S * NU;
+    if (moved) atomicAdd(reinterpret_cast<unsigned long long*>(&sc[0]), (unsigned long long)moved);
+    if (n_ops) atomicAdd(reinterpret_cast<unsigned long long*>(&sc[1]), (unsigned long long)n_ops);
+    if (warned) atomicAdd(reinterpret_cast<unsigned long long*>(&sc[2]), (unsigned long long)warned);
+  }
+  if (SMEM) {
+    __syncthreads();
+    for (int x = threadIdx.x; x < NU * 4; x += blockDim.x)
+      if (s_ops[x]) atomicAdd(reinterpret_cast<unsigned long long*>(&o[x]), (unsigned long long)s_ops[x]);
+    for (int x = threadIdx.x; x < S * NU; x += blockDim.x)
+      if (s_load[x]) atomicAdd(reinterpret_cast<unsigned long long*>(&o[4ll * NU + x]), (unsigned long long)s_load[x]);
   }
 }
 

@@ -337,24 +337,21 @@ static int grid_for(const blance_ctx* ctx, long long n, int block) {
   return (int)want;
 }
 
-static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan** out_plan) {
-  *out_plan = nullptr;
-  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "batch size must be positive");
-  for (int i = 0; i < n; ++i) {
-    int st = validate(ctx, &ins[i], i);
-    if (st != BLANCE_OK) return st;
-  }
-  CK(cudaSetDevice(ctx->device));
-  {
-    cudaError_t stale = cudaGetLastError();      // never let an earlier, unrelated error be blamed on this call
-    if (stale != cudaSuccess) return fail(ctx, BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
-  }
-  blance_plan* pl = new blance_plan();
+// Upload targets of the tables that DPool holds as const (the kernels only read them).
+struct PlanBufs {
+  int32_t *pweight = nullptr, *rank = nullptr, *inst = nullptr, *nw = nullptr, *ef = nullptr, *er = nullptr;
+  uint8_t *rm = nullptr, *ad = nullptr, *hw = nullptr;
+  uint32_t* mask = nullptr;
+};
+
+// Host side of a batch: the per-instance descriptors, their offsets into the pooled arrays and the totals.
+static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off) {
   pl->n_inst = n;
   pl->h_insts.resize(n);
   pl->raw_rows_off.resize(n + 1);
   pl->raw_shape_off.resize(n + 1);
-  std::vector<int> seg_off(n + 1);
+  seg_off.assign(n + 1, 0);
+  int n_prev = 0, n_assign = 0;
   for (int i = 0; i < n; ++i) {
     const blance_plan_in& in = ins[i];
     DInst& D = pl->h_insts[i];
@@ -378,8 +375,14 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
     }
     D.state_slot_off[in.n_states] = in.n_slots;
     D.rule_off[in.n_states] = in.has_hier_rules ? in.rule_off[in.n_states] : 0;
-    int n_prev = 0, n_assign = 0, n_valid = 0, rm_active = 0;
-    for (int p = 0; p < in.n_parts; ++p) { n_prev += in.part_in_prev[p] != 0; n_assign += in.part_in_assign[p] != 0; }
+    int n_valid = 0, rm_active = 0;
+    // (the instances of a scenario wave share their partition tables: counted once)
+    const bool same_parts = i > 0 && in.n_parts == ins[i - 1].n_parts && in.part_in_prev == ins[i - 1].part_in_prev &&
+                            in.part_in_assign == ins[i - 1].part_in_assign;
+    if (!same_parts) {
+      n_prev = 0; n_assign = 0;
+      for (int p = 0; p < in.n_parts; ++p) { n_prev += in.part_in_prev[p] != 0; n_assign += in.part_in_assign[p] != 0; }
+    }
     for (int q = 0; q < in.n_nodes; ++q) n_valid += in.node_removed[q] == 0;
     for (int q = 0; q < in.n_node_ids; ++q) rm_active |= in.node_removed[q] != 0;
     D.n_assign = n_assign; D.n_valid = n_valid;
@@ -398,7 +401,6 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
   }
   seg_off[n] = (int)pl->PT;
   pl->raw_rows_off[n] = pl->RRT; pl->raw_shape_off[n] = pl->RST;
-  if (pl->PT >= (1LL << 29)) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch"); }
   {
     int top_bits = 1, inst_bits = 1;
     while ((1ll << top_bits) < (long long)pl->max_NU + 2) ++top_bits;
@@ -406,17 +408,19 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
     pl->pair_inst_shift = 13 + top_bits;
     pl->pair_end_bit = pl->pair_inst_shift + inst_bits;
   }
+}
 
-  // ---- carve one device arena ------------------------------------------------------------
-  struct Slice { void** ptr; size_t bytes; };
+// The slices of a batch's device arena (sizes from layout()); `b` receives the const-in-DPool ones.
+struct Slice { void** ptr; size_t bytes; };
+static std::vector<Slice> arena_slices(blance_plan* pl, int n, PlanBufs& b) {
   std::vector<Slice> slices;
   DPool& P = pl->pool;
   const size_t PT = (size_t)pl->PT + 1, RT = (size_t)pl->RT + 4, NT = (size_t)pl->NT + 1, NUT = (size_t)pl->NUT + 1;
   const size_t CT = (size_t)pl->CT + 1, N2T = (size_t)pl->N2T + 1, MT = (size_t)pl->MT + 1;
   const size_t RRT = (size_t)pl->RRT + 1, RST = (size_t)pl->RST + 1;
-  const int32_t *c_pweight, *c_rank, *c_inst, *c_nw, *c_ef, *c_er;
-  const uint8_t *c_rm, *c_ad, *c_hw;
-  const uint32_t* c_mask;
+  int32_t *&c_pweight = b.pweight, *&c_rank = b.rank, *&c_inst = b.inst, *&c_nw = b.nw, *&c_ef = b.ef, *&c_er = b.er;
+  uint8_t *&c_rm = b.rm, *&c_ad = b.ad, *&c_hw = b.hw;
+  uint32_t*& c_mask = b.mask;
 #define SL_(p, T, cnt) slices.push_back(Slice{(void**)&(p), sizeof(T) * (cnt)})
   SL_(P.rows, int32_t, RT); SL_(P.prev_rows, int32_t, RT); SL_(pl->rows_init, int32_t, RT); SL_(pl->prev_rows_init, int32_t, RT);
   SL_(P.pmeta, uint32_t, PT); SL_(P.prev_meta, uint32_t, PT); SL_(pl->pmeta_init, uint32_t, PT); SL_(pl->prev_meta_init, uint32_t, PT);
@@ -435,11 +439,23 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
   SL_(pl->d_raw_rows_off, long long, (size_t)n + 1); SL_(pl->d_raw_shape_off, long long, (size_t)n + 1);
   SL_(pl->d_seg_off, int, (size_t)n + 1);
 #undef SL_
+  return slices;
+}
+
+static size_t slices_bytes(const std::vector<Slice>& slices) {
   size_t total = 0;
   for (auto& s : slices) total += align_up(s.bytes, 256);
+  return total;
+}
+
+// Allocates and carves the arena of a laid-out batch.  On failure the plan is released.
+static int carve_arena(blance_ctx* ctx, blance_plan* pl, int n, PlanBufs& b) {
+  std::vector<Slice> slices = arena_slices(pl, n, b);
+  const size_t total = slices_bytes(slices);
   // stream-ordered allocation: the context's memory pool keeps the arena of the previous call around
   cudaError_t e = cudaMallocAsync(&pl->arena, total, ctx->stream);
   if (e != cudaSuccess) {
+    cudaGetLastError();
     plan_release(pl, ctx);
     return fail(ctx, BLANCE_ERR_NOMEM, std::string("cudaMalloc of the plan arena failed: ") + cudaGetErrorString(e));
   }
@@ -448,9 +464,71 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
     size_t off = 0;
     for (auto& s : slices) { *s.ptr = (char*)pl->arena + off; off += align_up(s.bytes, 256); }
   }
-  P.pweight = c_pweight; P.name_rank = c_rank; P.part_inst = c_inst;
-  P.node_removed = c_rm; P.node_added = c_ad; P.node_weight = c_nw; P.node_has_weight = c_hw;
-  P.extra_first = c_ef; P.extra_rest = c_er; P.ie_mask = c_mask;
+  DPool& P = pl->pool;
+  P.pweight = b.pweight; P.name_rank = b.rank; P.part_inst = b.inst;
+  P.node_removed = b.rm; P.node_added = b.ad; P.node_weight = b.nw; P.node_has_weight = b.hw;
+  P.extra_first = b.ef; P.extra_rest = b.er; P.ie_mask = b.mask;
+  return BLANCE_OK;
+}
+
+// Device bytes of the radix sorts' scratch for a batch of PT partitions in n segments (a size query only).
+static size_t sort_scratch_bytes(long long PT, int n, cudaStream_t st) {
+  size_t need = 0, need2 = 0, need3 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, need, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int32_t*)nullptr,
+                                  (int32_t*)nullptr, (int)PT, 0, 64, st);
+  cub::DeviceSegmentedRadixSort::SortPairs(nullptr, need2, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int32_t*)nullptr,
+                                           (int32_t*)nullptr, (int)PT, n, (int*)nullptr, (int*)nullptr, 0, 64, st);
+  cub::DeviceRadixSort::SortPairs(nullptr, need3, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (uint32_t*)nullptr,
+                                  (uint32_t*)nullptr, (int)(4 * PT), 0, 64, st);
+  return std::max(need, std::max(need2, need3));
+}
+
+// Grows the context's sort scratch to what the batch needs, then waits for the uploads.  On failure the plan is released.
+static int finish_upload(blance_ctx* ctx, blance_plan* pl) {
+  const size_t need = sort_scratch_bytes(pl->PT, pl->n_inst, ctx->stream);
+  cudaError_t e;
+  if (need > ctx->cub_tmp_bytes) {
+    if (ctx->cub_tmp) cudaFree(ctx->cub_tmp);
+    ctx->cub_tmp = nullptr; ctx->cub_tmp_bytes = 0;
+    e = cudaMalloc(&ctx->cub_tmp, need);
+    if (e != cudaSuccess) { cudaGetLastError(); plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the sort scratch failed"); }
+    ctx->cub_tmp_bytes = need;
+  }
+  e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("upload sync failed: ") + cudaGetErrorString(e)); }
+  return BLANCE_OK;
+}
+
+static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan** out_plan) {
+  *out_plan = nullptr;
+  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "batch size must be positive");
+  for (int i = 0; i < n; ++i) {
+    int st = validate(ctx, &ins[i], i);
+    if (st != BLANCE_OK) return st;
+  }
+  CK(cudaSetDevice(ctx->device));
+  {
+    cudaError_t stale = cudaGetLastError();      // never let an earlier, unrelated error be blamed on this call
+    if (stale != cudaSuccess) return fail(ctx, BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
+  }
+  blance_plan* pl = new blance_plan();
+  std::vector<int> seg_off;
+  layout(pl, n, ins, seg_off);
+  if (pl->PT >= (1LL << 29)) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch"); }
+
+  // ---- carve one device arena ------------------------------------------------------------
+  PlanBufs bufs;
+  {
+    const int st = carve_arena(ctx, pl, n, bufs);
+    if (st != BLANCE_OK) return st;
+  }
+  DPool& P = pl->pool;
+  const size_t PT = (size_t)pl->PT + 1, NT = (size_t)pl->NT + 1, NUT = (size_t)pl->NUT + 1;
+  const size_t MT = (size_t)pl->MT + 1, RRT = (size_t)pl->RRT + 1, RST = (size_t)pl->RST + 1;
+  const int32_t *c_pweight = bufs.pweight, *c_rank = bufs.rank, *c_inst = bufs.inst, *c_nw = bufs.nw, *c_ef = bufs.ef, *c_er = bufs.er;
+  const uint8_t *c_rm = bufs.rm, *c_ad = bufs.ad, *c_hw = bufs.hw;
+  const uint32_t* c_mask = bufs.mask;
+  cudaError_t e = cudaSuccess;
 
   // ---- host side of the copy.  A batch is concatenated in caller layout into one pinned staging buffer;
   // a single instance is copied straight from the caller's arrays (no staging, no pinned allocation).
@@ -574,26 +652,10 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
     if (e == cudaSuccess) e = cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("upload failed: ") + cudaGetErrorString(e)); }
   }
-  // sort scratch
-  size_t need = 0, need2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, need, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT, 0, 64, st);
-  cub::DeviceSegmentedRadixSort::SortPairs(nullptr, need2, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT, n,
-                                           pl->d_seg_off, pl->d_seg_off + 1, 0, 64, st);
-  need = std::max(need, need2);
   {
-    size_t need3 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, need3, P.pair_keys_alt, P.pair_keys, P.pair_vals_alt, P.pair_vals, (int)(4 * pl->PT), 0, 64, st);
-    need = std::max(need, need3);
+    const int rc = finish_upload(ctx, pl);
+    if (rc != BLANCE_OK) return rc;
   }
-  if (need > ctx->cub_tmp_bytes) {
-    if (ctx->cub_tmp) cudaFree(ctx->cub_tmp);
-    ctx->cub_tmp = nullptr; ctx->cub_tmp_bytes = 0;
-    e = cudaMalloc(&ctx->cub_tmp, need);
-    if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the sort scratch failed"); }
-    ctx->cub_tmp_bytes = need;
-  }
-  e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("upload sync failed: ") + cudaGetErrorString(e)); }
   *out_plan = pl;
   return BLANCE_OK;
 }
@@ -967,6 +1029,257 @@ extern "C" int blance_plan_next_map(blance_ctx* ctx, const blance_plan_in* in, b
 
 extern "C" int blance_plan_next_map_batch(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out) {
   return plan_batch(ctx, n, in, out);
+}
+
+// ---------------------------------------------------------------------------------------
+// What-if scenarios of one cluster (blance_plan_scenarios): the base is uploaded once per device, each wave of
+// scenarios is a batch whose partition slices are replicated from it on the device.
+
+static blance_plan_in scenario_in(const blance_plan_in& base, const blance_scenario& sc) {
+  blance_plan_in in = base;
+  in.node_removed = sc.node_removed; in.node_added = sc.node_added; in.add_is_nil = sc.add_is_nil;
+  in.has_node_weights = sc.has_node_weights; in.node_weight = sc.node_weight; in.node_has_weight = sc.node_has_weight;
+  return in;
+}
+
+// int64 words of one scenario's summary: node_ops [NU][4] | state_node_load [S][NU] | 3 scalars
+static long long summary_stride(const blance_plan_in& base) {
+  return 4ll * base.n_node_ids + (long long)base.n_states * base.n_node_ids + 3;
+}
+
+// The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).
+static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, int n_dev, int max_concurrent, size_t* per_scenario) {
+  blance_plan probe;
+  std::vector<int> seg;
+  layout(&probe, 1, &in0, seg);
+  PlanBufs b;
+  const size_t per = slices_bytes(arena_slices(&probe, 1, b)) + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
+                     sizeof(long long) * (size_t)summary_stride(in0);
+  *per_scenario = per;
+  if (max_concurrent > 0) return std::min(n_dev, max_concurrent);
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return 1; }
+  const size_t headroom = std::max<size_t>(1ull << 30, total_b / 16);     // the device is shared: leave room
+  const long long fit = free_b > headroom ? (long long)((free_b - headroom) / std::max<size_t>(per, 1)) : 0;
+  int w = (int)std::min<long long>(n_dev, fit);
+  // above the 3-scout speculative kernel's node limit a wide batch would drop to lock-step (run(): 2n <= sm_count)
+  if (in0.n_nodes > std::min(2048, 32 * 3 * SP_NPTS)) w = std::min(w, std::max(1, ctx->sm_count / 2));
+  return w;
+}
+
+static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
+                               int favor_min, int max_concurrent, blance_scenario_out* out) {
+  std::lock_guard<std::mutex> g(ctx->mu);
+  CK(cudaSetDevice(ctx->device));
+  {
+    cudaError_t stale = cudaGetLastError();
+    if (stale != cudaSuccess) return fail(ctx, BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
+  }
+  cudaStream_t st = ctx->stream;
+  const int n_dev = (int)idx.size();
+  const blance_plan_in in0 = scenario_in(*base, sc[idx[0]]);
+  {
+    cudaMemPool_t pool;                // measure free memory without this context's cached arenas
+    if (max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
+      cudaStreamSynchronize(st);
+      cudaMemPoolTrimTo(pool, 0);
+    }
+  }
+  // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
+  blance_plan* pb = nullptr;
+  {
+    const int rc = upload(ctx, 1, &in0, &pb);
+    if (rc != BLANCE_OK) return rc;
+  }
+  size_t per = 0;
+  int W = wave_size(ctx, in0, n_dev, max_concurrent, &per);
+  if (W < 1) {
+    plan_release(pb, ctx);
+    return fail(ctx, BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
+  }
+  const bool auto_wave = max_concurrent <= 0;
+  const bool times = getenv("BLANCE_SCENARIO_TIMES") != nullptr;
+  const long long stride = summary_stride(*base);
+  const int PU = base->n_parts, NU = base->n_node_ids, S = base->n_states;
+  int rc = BLANCE_OK;
+  for (int w0 = 0; w0 < n_dev && rc == BLANCE_OK;) {
+    const int nw = std::min(W, n_dev - w0);
+    std::vector<blance_plan_in> ins((size_t)nw);
+    for (int j = 0; j < nw; ++j) ins[(size_t)j] = scenario_in(*base, sc[idx[(size_t)(w0 + j)]]);
+    // a device's only scenario is the base upload itself: nothing to replicate
+    const bool lone = n_dev == 1;
+    blance_plan* pl = lone ? pb : new blance_plan();
+    std::vector<int> seg_off;
+    if (!lone) layout(pl, nw, ins.data(), seg_off);
+    if (!lone && pl->PT >= (1LL << 29)) {
+      plan_release(pl, ctx);
+      if (nw > 1) { W = nw / 2; continue; }
+      rc = fail(ctx, BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
+      break;
+    }
+    PlanBufs b;
+    if (!lone) {
+      rc = carve_arena(ctx, pl, nw, b);
+      if (rc == BLANCE_ERR_NOMEM && auto_wave && nw > 1) { rc = BLANCE_OK; W = nw / 2; continue; }   // the free memory moved
+      if (rc != BLANCE_OK) break;
+    }
+    long long* d_sum = nullptr;
+    if (cudaMallocAsync((void**)&d_sum, sizeof(long long) * (size_t)(stride * nw), st) != cudaSuccess) {
+      cudaGetLastError();
+      if (!lone) plan_release(pl, ctx);
+      if (auto_wave && nw > 1) { W = nw / 2; continue; }
+      rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the scenario summaries failed");
+      break;
+    }
+    auto step = [&](cudaError_t e, const char* what) {
+      if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+    // the node tables of the wave's scenarios (small host copies); the hierarchy masks and extra counts of the base
+    if (!lone) {
+      const size_t NT = (size_t)pl->NT, NUT = (size_t)pl->NUT, MT = (size_t)pl->MT;
+      std::vector<uint8_t> rm(NUT + 1, 0), ad(NUT + 1, 0), hw(NT + 1, 0);
+      std::vector<int32_t> nwt(NT + 1, 0), ef(NT + 1, 0), er(NT + 1, 0);
+      std::vector<uint32_t> mask(MT + 1, 0);
+      for (int j = 0; j < nw; ++j) {
+        const blance_plan_in& in = ins[(size_t)j];
+        const DInst& D = pl->h_insts[(size_t)j];
+        if (D.NU) { std::memcpy(&rm[(size_t)D.nodeid_off], in.node_removed, (size_t)D.NU); std::memcpy(&ad[(size_t)D.nodeid_off], in.node_added, (size_t)D.NU); }
+        for (int q = 0; q < D.N; ++q) {
+          nwt[(size_t)D.node_off + q] = in.has_node_weights ? in.node_weight[q] : 0;
+          hw[(size_t)D.node_off + q] = in.has_node_weights ? in.node_has_weight[q] : 0;
+          ef[(size_t)D.node_off + q] = in.extra_tot_first ? in.extra_tot_first[q] : 0;
+          er[(size_t)D.node_off + q] = in.extra_tot_rest ? in.extra_tot_rest[q] : 0;
+        }
+        const size_t mw = (size_t)D.n_rules * (D.NU + 1) * D.HW;
+        if (mw) std::memcpy(&mask[(size_t)D.mask_off], in.ie_mask, sizeof(uint32_t) * mw);
+      }
+      step(cudaMemcpyAsync(b.rm, rm.data(), NUT + 1, cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.ad, ad.data(), NUT + 1, cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.hw, hw.data(), NT + 1, cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.nw, nwt.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.ef, ef.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.er, er.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(b.mask, mask.data(), sizeof(uint32_t) * (MT + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaMemcpyAsync(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
+      step(cudaStreamSynchronize(st), "H2D sync");          // the host vectors die at the end of this block
+    }
+    if (!lone && rc == BLANCE_OK && pl->PT > 0) {
+      const int SLP = pl->h_insts[0].SLP;
+      k_scenario_replicate<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(
+          pl->rows_init, pl->prev_rows_init, pl->pmeta_init, pl->prev_meta_init, pl->pflags_init, b.pweight, b.rank, b.inst,
+          pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init, pb->pflags_init, pb->pool.pweight,
+          pb->pool.name_rank, PU, SLP, pl->PT);
+      ctx->launches++;
+      step(cudaGetLastError(), "k_scenario_replicate");
+    }
+    if (!lone && rc == BLANCE_OK) {
+      rc = finish_upload(ctx, pl);
+      if (rc != BLANCE_OK) { cudaFreeAsync(d_sum, st); break; }          // (the plan is released)
+    }
+    step(cudaEventRecord(ctx->ev[0], st), "event");
+    if (rc == BLANCE_OK) rc = run(ctx, pl);
+    // summaries, then the requested rows
+    float sum_ms = 0.f;
+    if (rc == BLANCE_OK) {
+      step(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), st), "memset");
+      step(cudaEventRecord(ctx->ev[1], st), "event");
+      if (PU > 0) {
+        const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
+        const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
+        const dim3 grid((unsigned)bx, (unsigned)nw);
+        if (smem <= 48 * 1024) k_scenario_summary<true><<<grid, 256, smem, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
+        else k_scenario_summary<false><<<grid, 256, 0, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
+        ctx->launches++;
+        step(cudaGetLastError(), "k_scenario_summary");
+      }
+      step(cudaEventRecord(ctx->ev[2], st), "event");
+      bool any_rows = false;
+      for (int j = 0; j < nw; ++j) {
+        const blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+        any_rows |= o.next_rows || o.next_shape || o.warn;
+      }
+      if (any_rows && pl->PT > 0) {
+        k_pack<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(pl->pool, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
+                                                          pl->d_raw_shape_off, pl->PT);
+        ctx->launches++;
+        step(cudaGetLastError(), "k_pack");
+      }
+      std::vector<long long> h_sum((size_t)(stride * nw));
+      std::vector<DInst> fin((size_t)nw);
+      step(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st), "D2H");
+      step(cudaMemcpyAsync(fin.data(), pl->pool.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st), "D2H");
+      for (int j = 0; j < nw && rc == BLANCE_OK; ++j) {
+        blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+        const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
+        if (rr && o.next_rows) step(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st), "D2H");
+        if (rs && o.next_shape) step(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st), "D2H");
+        if (rs && o.warn) step(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st), "D2H");
+      }
+      step(cudaStreamSynchronize(st), "sync");
+      if (rc == BLANCE_OK) cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
+      for (int j = 0; j < nw && rc == BLANCE_OK; ++j) {
+        if (fin[(size_t)j].spec_abort) { rc = fail(ctx, BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)"); break; }
+        blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+        const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
+        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
+        if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
+        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
+        o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
+        o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
+      }
+    }
+    if (times && rc == BLANCE_OK) {
+      float wave_ms = 0.f;
+      cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
+      std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms\n",
+                   w0, nw, W, per, wave_ms, sum_ms);
+    }
+    cudaFreeAsync(d_sum, st);
+    if (!lone) plan_release(pl, ctx);
+    w0 += nw;
+  }
+  cudaStreamSynchronize(st);
+  plan_release(pb, ctx);
+  return rc;
+}
+
+extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                     int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
+  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: n must be positive");
+  if (!base || !sc || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: base, sc or out is NULL");
+  // every scenario is checked before any device work
+  for (int i = 0; i < n; ++i) {
+    std::string why;
+    if (sc[i].add_is_nil != 0 && sc[i].add_is_nil != 1) why = "add_is_nil is neither 0 nor 1";
+    else if (sc[i].has_node_weights != 0 && sc[i].has_node_weights != 1) why = "has_node_weights is neither 0 nor 1";
+    else {
+      const blance_plan_in in = scenario_in(*base, sc[i]);
+      const int st = check_structure(&in, why);
+      if (st != BLANCE_OK) return fail(ctx, st, "blance_plan_scenarios: scenario " + std::to_string(i) + ": " + why);
+    }
+    if (!why.empty()) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: scenario " + std::to_string(i) + ": " + why);
+  }
+  const int G = ctx->children.empty() ? 1 : (int)std::min<size_t>(ctx->children.size(), (size_t)n);
+  std::vector<std::vector<int>> idx((size_t)G);
+  for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
+  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, favor_min_nodes, max_concurrent, out);
+  // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
+  std::vector<int> status((size_t)G, BLANCE_OK);
+  std::vector<std::thread> th;
+  for (int d = 0; d < G; ++d)
+    th.emplace_back([&, d]() {
+      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, favor_min_nodes, max_concurrent, out);
+    });
+  for (auto& t : th) t.join();
+  for (int d = 0; d < G; ++d)
+    if (status[(size_t)d] != BLANCE_OK) {
+      ctx->err = "device " + std::to_string(ctx->children[(size_t)d]->device) + ": " + ctx->children[(size_t)d]->err;
+      return status[(size_t)d];
+    }
+  return BLANCE_OK;
 }
 
 extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,

@@ -233,6 +233,14 @@ int32_t checked_i32(long long v, const char* what) {
   return int32_t(v);
 }
 
+// plan.go:544-545 dereferences prevMap[name] whenever nodesToRemove is non-empty
+void check_remove_needs_prev(const InternedPlan& ip, const OptStrs& nodesToRemove, const std::string& who) {
+  if (deref(nodesToRemove).empty()) return;
+  for (size_t p = 0; p < ip.part_in_assign.size(); ++p)
+    if (ip.part_in_assign[p] && !ip.part_in_prev[p])
+      invalid(who + "partition '" + ip.part_names[p] + "' is being assigned with nodesToRemove set but is missing from prevMap (the reference panics, plan.go:544)");
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------
@@ -496,11 +504,7 @@ std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const Part
       ip->node_has_weight[size_t(id)] = 1;
     }
 
-  // plan.go:544-545 dereferences prevMap[name] whenever nodesToRemove is non-empty
-  if (!deref(nodesToRemove).empty())
-    for (int32_t p = 0; p < PU; ++p)
-      if (ip->part_in_assign[size_t(p)] && !ip->part_in_prev[size_t(p)])
-        invalid("partition '" + ip->part_names[size_t(p)] + "' is being assigned with nodesToRemove set but is missing from prevMap (the reference panics, plan.go:544)");
+  check_remove_needs_prev(*ip, nodesToRemove, "");
 
   // ---- counts under non-model states
   ip->extra_tot_first.assign(size_t(N), 0);
@@ -871,6 +875,138 @@ PartitionMap PlanNextMapEx(PartitionMap& prevMap, PartitionMap& partitionsToAssi
   if (ob.out.iters_run >= 2 || !ob.out.converged) ReplayCallerMutation(next, prevMap, partitionsToAssign);
   if (stats) { stats->unintern_ms = ms(t2, t3); stats->mutate_ms = ms(t3, clk::now()); }
   return next;
+}
+
+// ------------------------------------------------------------------------------------
+// What-if scenarios of one cluster
+
+namespace {
+
+// The base tables of a scenario sweep.  The node-id space holds every name of every scenario's nodesToRemove and
+// nodesToAdd (a removed name outside nodesAll still makes len(nodesToRemove) > 0, plan.go:543); the base's own node
+// flags and weights are replaced per scenario.
+std::unique_ptr<InternedPlan> intern_scenario_base(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                                   const Strs& nodesAll, const PartitionModel& model,
+                                                   const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios) {
+  Strs names;
+  for (const auto& sc : scenarios) {
+    for (const auto& n : deref(sc.NodesToRemove)) names.push_back(n);
+    for (const auto& n : deref(sc.NodesToAdd)) names.push_back(n);
+  }
+  return InternPlan(prevMap, partitionsToAssign, nodesAll, std::nullopt, OptStrs(std::move(names)), model, options);
+}
+
+struct ScenarioTables {
+  std::vector<uint8_t> removed, added, has_weight;
+  std::vector<int32_t> weight;
+  int32_t add_is_nil = 0, has_node_weights = 0;
+};
+
+ScenarioTables scenario_tables(const InternedPlan& ip, const Scenario& sc, const PlanNextMapOptions& options, size_t index) {
+  check_remove_needs_prev(ip, sc.NodesToRemove, "scenario " + std::to_string(index) + ": ");
+  const int32_t N = ip.in.n_nodes, NU = ip.in.n_node_ids;
+  std::unordered_map<std::string, int32_t> id;
+  id.reserve(size_t(NU));
+  for (int32_t q = 0; q < NU; ++q) id.emplace(ip.node_names[size_t(q)], q);
+  ScenarioTables t;
+  t.removed.assign(size_t(NU) + 1, 0);
+  t.added.assign(size_t(NU) + 1, 0);
+  for (const auto& n : deref(sc.NodesToRemove)) t.removed[size_t(id.at(n))] = 1;
+  for (const auto& n : deref(sc.NodesToAdd)) t.added[size_t(id.at(n))] = 1;
+  t.add_is_nil = sc.NodesToAdd ? 0 : 1;
+  const auto& weights = sc.NodeWeights ? *sc.NodeWeights : options.NodeWeights;
+  t.weight.assign(size_t(N) + 1, 0);
+  t.has_weight.assign(size_t(N) + 1, 0);
+  t.has_node_weights = weights ? 1 : 0;
+  if (weights)
+    for (const auto& kv : *weights) {
+      auto it = id.find(kv.first);
+      if (it == id.end() || it->second >= N) continue;
+      t.weight[size_t(it->second)] = kv.second;
+      t.has_weight[size_t(it->second)] = 1;
+    }
+  return t;
+}
+
+}  // namespace
+
+std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                             const Strs& nodesAll, const PartitionModel& model,
+                                             const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
+                                             size_t index) {
+  if (index >= scenarios.size()) invalid("InternScenario: scenario index out of range");
+  auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
+  ScenarioTables t = scenario_tables(*ip, scenarios[index], options, index);
+  ip->node_removed = std::move(t.removed);
+  ip->node_added = std::move(t.added);
+  ip->node_weight = std::move(t.weight);
+  ip->node_has_weight = std::move(t.has_weight);
+  blance_plan_in& in = ip->in;
+  in.node_removed = ip->node_removed.data();
+  in.node_added = ip->node_added.data();
+  in.node_weight = ip->node_weight.data();
+  in.node_has_weight = ip->node_has_weight.data();
+  in.add_is_nil = t.add_is_nil;
+  in.has_node_weights = t.has_node_weights;
+  return ip;
+}
+
+std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                                 const Strs& nodesAll, const PartitionModel& model,
+                                                 const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
+                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent) {
+  if (scenarios.empty()) invalid("PlanNextMapScenarios: no scenarios");
+  auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
+  const size_t n = scenarios.size();
+  std::vector<ScenarioTables> tabs(n);
+  for (size_t i = 0; i < n; ++i) tabs[i] = scenario_tables(*ip, scenarios[i], options, i);
+  std::vector<bool> want(n, false);
+  for (int i : wantMaps) {
+    if (i < 0 || size_t(i) >= n) invalid("PlanNextMapScenarios: wantMaps index " + std::to_string(i) + " out of range");
+    want[size_t(i)] = true;
+  }
+  const int32_t NU = ip->in.n_node_ids, S = ip->in.n_states;
+  std::vector<blance_scenario> sc(n);
+  std::vector<blance_scenario_out> out(n);
+  std::vector<std::vector<int64_t>> ops(n, std::vector<int64_t>(size_t(NU) * 4 + 1)), load(n, std::vector<int64_t>(size_t(S) * size_t(NU) + 1));
+  std::vector<std::unique_ptr<PlanOutBuffers>> maps(n);
+  for (size_t i = 0; i < n; ++i) {
+    sc[i] = blance_scenario{tabs[i].removed.data(), tabs[i].added.data(), tabs[i].add_is_nil, tabs[i].has_node_weights,
+                            tabs[i].weight.data(), tabs[i].has_weight.data()};
+    out[i] = blance_scenario_out{};
+    out[i].node_ops = ops[i].data();
+    out[i].state_node_load = load[i].data();
+    if (want[i]) {
+      maps[i] = std::make_unique<PlanOutBuffers>(*ip);
+      out[i].next_rows = maps[i]->next_rows.data();
+      out[i].next_shape = maps[i]->next_shape.data();
+      out[i].warn = maps[i]->warn.data();
+    }
+  }
+  blance_ctx* ctx = DefaultContext();
+  const int st = blance_plan_scenarios(ctx, &ip->in, int32_t(n), sc.data(), favorMinNodes ? 1 : 0, maxConcurrent, out.data());
+  if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_scenarios failed: ") + blance_last_error(ctx));
+  static const char* kOps[] = {"add", "del", "promote", "demote"};
+  std::vector<ScenarioResult> res(n);
+  for (size_t i = 0; i < n; ++i) {
+    ScenarioResult& r = res[i];
+    const blance_scenario_out& o = out[i];
+    r.iters_run = o.iters_run; r.converged = o.converged; r.steps = o.steps; r.sticky_steps = o.sticky_steps;
+    r.parts_moved = o.parts_moved; r.ops_total = o.ops_total; r.warn_parts = o.warn_parts;
+    for (int32_t q = 0; q < NU; ++q)
+      for (int k = 0; k < 4; ++k)
+        if (ops[i][size_t(q) * 4 + size_t(k)]) r.NodeOps[ip->node_names[size_t(q)]][kOps[k]] = ops[i][size_t(q) * 4 + size_t(k)];
+    for (int32_t s = 0; s < S; ++s)
+      for (int32_t q = 0; q < NU; ++q)
+        if (load[i][size_t(s) * size_t(NU) + size_t(q)])
+          r.StateNodeLoad[ip->state_names[size_t(s)]][ip->node_names[size_t(q)]] = load[i][size_t(s) * size_t(NU) + size_t(q)];
+    if (want[i]) {
+      r.HasMap = true;
+      maps[i]->out.iters_run = o.iters_run;
+      if (o.iters_run > 0) r.NextMap = UninternPlan(*ip, *maps[i], &r.NextWarnings);   // MaxIterationsPerPlan <= 0: plan.go:32,57
+    }
+  }
+  return res;
 }
 
 // ------------------------------------------------------------------------------------

@@ -92,6 +92,37 @@ PartitionMap PlanNextMapEx(PartitionMap& prevMap, PartitionMap& partitionsToAssi
                            const PartitionModel& model, const PlanNextMapOptions& options,
                            Warnings* warnings, PlanStats* stats = nullptr);
 
+// ---- what-if scenarios of one cluster (blance_plan_scenarios) ----------------------------------------------------
+struct Scenario {
+  OptStrs NodesToRemove;               // nullopt = nil
+  OptStrs NodesToAdd;                  // nullopt = nil (plan.go:554)
+  // outer nullopt: the options' NodeWeights; inner nullopt: nil
+  std::optional<std::optional<std::unordered_map<std::string, int>>> NodeWeights;
+};
+
+struct ScenarioResult {
+  int iters_run = 0, converged = 0;
+  int64_t steps = 0, sticky_steps = 0, parts_moved = 0, ops_total = 0, warn_parts = 0;
+  // CalcPartitionMoves(prevMap row -> next row) of every assigned partition, counted per node and op name
+  // ("add", "del", "promote", "demote"); nonzero counts only
+  std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> NodeOps;
+  // countStateNodes (plan.go:374-399) of the final map per model state and node; nonzero loads only
+  std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> StateNodeLoad;
+  bool HasMap = false;                 // the scenario was listed in wantMaps
+  PartitionMap NextMap;                // as PlanNextMapEx returns it
+  Warnings NextWarnings;
+};
+
+// Scenario i is PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, NodesToRemove_i, NodesToAdd_i, model, options
+// with NodeWeights_i).  Unlike PlanNextMapEx (plan.go:49-52), the caller's maps are NOT mutated: a what-if has no
+// side effects.  The maps are interned once; a scenario the reference would panic on (plan.go:544) throws
+// BlanceError naming its index before any device work.  NextMap / NextWarnings are filled for the indices in
+// wantMaps; maxConcurrent as in blance_plan_scenarios.
+std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                                 const Strs& nodesAll, const PartitionModel& model,
+                                                 const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
+                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent);
+
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 
 // moves.go:41-46 for one partition (a batch of one on the device).
@@ -140,6 +171,13 @@ struct PlanOutBuffers {
 
 // rows -> PartitionMap of the assigned partitions, plus the warning strings.
 PartitionMap UninternPlan(const InternedPlan& ip, const PlanOutBuffers& ob, Warnings* warnings);
+
+// The blance_plan_in of scenario `index` of PlanNextMapScenarios: the shared base tables with that scenario's node
+// fields substituted (so a CPU oracle can run on exactly the tables the device plans).
+std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                             const Strs& nodesAll, const PartitionModel& model,
+                                             const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
+                                             size_t index);
 
 // plan.go:49-52: store the partitions of `next` into the caller's maps (they may be the same object).
 void ReplayCallerMutation(const PartitionMap& next, PartitionMap& prevMap, PartitionMap& partitionsToAssign);

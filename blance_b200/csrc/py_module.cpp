@@ -302,6 +302,75 @@ PYBIND11_MODULE(_host, m) {
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10,
       py::arg("engine") = 0);
 
+  // what-if scenarios: (nodes_to_remove, nodes_to_add, has_node_weights_key, node_weights) per scenario
+  using PyScenario = std::tuple<OptStrs, OptStrs, bool, std::optional<IntMap>>;
+  auto to_scenarios = [](const std::vector<PyScenario>& v) {
+    std::vector<Scenario> out;
+    for (const auto& t : v) {
+      Scenario s;
+      s.NodesToRemove = std::get<0>(t);
+      s.NodesToAdd = std::get<1>(t);
+      if (std::get<2>(t)) s.NodeWeights = std::get<3>(t);
+      out.push_back(std::move(s));
+    }
+    return out;
+  };
+
+  m.def(
+      "PlanNextMapScenarios",
+      [to_scenarios](const PyPartitionMap& prev, const std::optional<PyPartitionMap>& assign, const Strs& nodes_all,
+                     const PyModel& model, const std::vector<PyScenario>& scenarios, bool favor_min_nodes,
+                     const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
+                     const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
+                     const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
+                     int engine) {
+        PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
+        const PartitionMap prev_map = to_map(prev);
+        const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
+        const std::vector<Scenario> scs = to_scenarios(scenarios);
+        std::vector<ScenarioResult> res;
+        {
+          py::gil_scoped_release rel;
+          res = PlanNextMapScenarios(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, scs,
+                                     favor_min_nodes, want_maps, max_concurrent);
+        }
+        py::list out;
+        for (const auto& r : res) {
+          py::dict d;
+          d["iterations"] = r.iters_run; d["converged"] = r.converged; d["steps"] = r.steps;
+          d["sticky_steps"] = r.sticky_steps; d["parts_moved"] = r.parts_moved; d["ops_total"] = r.ops_total;
+          d["warn_parts"] = r.warn_parts; d["node_ops"] = r.NodeOps; d["state_node_load"] = r.StateNodeLoad;
+          if (r.HasMap) { d["next_map"] = from_map(r.NextMap); d["warnings"] = r.NextWarnings; }
+          out.append(d);
+        }
+        return out;
+      },
+      py::arg("prev_map"), py::arg("partitions_to_assign"), py::arg("nodes_all"), py::arg("model"), py::arg("scenarios"),
+      py::arg("favor_min_nodes") = false, py::arg("want_maps") = std::vector<int>{}, py::arg("max_concurrent") = 0,
+      py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
+      py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
+      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+
+  // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
+  m.def(
+      "intern_scenario",
+      [to_scenarios](const PyPartitionMap& prev, const std::optional<PyPartitionMap>& assign, const Strs& nodes_all,
+                     const PyModel& model, const std::vector<PyScenario>& scenarios, size_t index,
+                     const std::optional<IntMap>& msc, const std::optional<IntMap>& pw, const std::optional<IntMap>& ss,
+                     const std::optional<IntMap>& nw, const std::optional<StrMap>& nh, const std::optional<PyRules>& hr,
+                     int booster, int max_iterations, int engine) {
+        PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
+        const PartitionMap prev_map = to_map(prev);
+        const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
+        PyInterned r;
+        r.ip = InternScenario(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, to_scenarios(scenarios), index);
+        return r;
+      },
+      py::arg("prev_map"), py::arg("partitions_to_assign"), py::arg("nodes_all"), py::arg("model"), py::arg("scenarios"),
+      py::arg("index"), py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
+      py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
+      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+
   m.def("plan_out", [](const PyInterned& ip) {
     PyOut o;
     o.ob = std::make_unique<PlanOutBuffers>(*ip.ip);

@@ -2,6 +2,7 @@
 blance_plan_out of include/blance_b200.h, for callers that already hold ids
 instead of strings (bench.py, the large parity tests).  The arrays are plain host
 memory; PlanTables.struct() returns the ctypes struct whose pointers alias them."""
+import copy
 import ctypes
 
 import numpy as np
@@ -104,6 +105,42 @@ class PlanResult:
     pass_ms = property(lambda self: self.out.pass_ms)
 
 
+SCENARIO_FIELDS = ("node_removed", "node_added", "add_is_nil", "has_node_weights", "node_weight", "node_has_weight")
+
+
+class ScenarioResult:
+    """Output buffers of a blance_scenario_out: the summaries always, the next map's tables when requested."""
+
+    def __init__(self, t, want_rows):
+        self.node_ops = np.zeros((t.n_node_ids, 4), np.int64)
+        self.state_node_load = np.zeros((t.n_states, t.n_node_ids), np.int64)
+        self.next_rows = np.full((t.n_parts, t.n_slots), NO_NODE, np.int32) if want_rows else None
+        self.next_shape = np.zeros((t.n_parts, t.n_states), np.uint8) if want_rows else None
+        self.warn = np.zeros((t.n_parts, t.n_states), np.uint8) if want_rows else None
+        self.out = api.ScenarioOut()
+        for f in ("node_ops", "state_node_load", "next_rows", "next_shape", "warn"):
+            a = getattr(self, f)
+            setattr(self.out, f, a.ctypes.data if a is not None and a.size else None)
+
+    iters_run = property(lambda self: self.out.iters_run)
+    converged = property(lambda self: self.out.converged)
+    steps = property(lambda self: self.out.steps)
+    sticky_steps = property(lambda self: self.out.sticky_steps)
+    parts_moved = property(lambda self: self.out.parts_moved)
+    ops_total = property(lambda self: self.out.ops_total)
+    warn_parts = property(lambda self: self.out.warn_parts)
+
+
+def scenario_tables(base, scenario):
+    """The PlanTables of one scenario: `base` with the scenario's node fields substituted (a shallow copy; the
+    partition arrays are shared).  A field missing from the scenario dict keeps the base's value."""
+    t = copy.copy(base)
+    for f in SCENARIO_FIELDS:
+        if f in scenario:
+            setattr(t, f, scenario[f])
+    return t
+
+
 class Context:
     """A blance_ctx* (one per process/GPU)."""
 
@@ -139,6 +176,32 @@ class Context:
         ins = (api.PlanIn * n)(*[t.struct() for t in tables_list])
         outs = (api.PlanOut * n)(*[r.out for r in results])
         self._check(self.lib.blance_plan_next_map_batch(self.ptr, n, ins, outs), "blance_plan_next_map_batch")
+        for r, o in zip(results, outs):
+            r.out = o
+        return results
+
+    def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=()):
+        """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
+        (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
+        are copied out.  Returns one ScenarioResult per scenario."""
+        n = len(scenarios)
+        want = set(want_rows)
+        base = base_tables.struct()
+        keep, scs = [], (api.Scenario * max(1, n))()
+        for i, sc in enumerate(scenarios):
+            t = scenario_tables(base_tables, sc)
+            for f in SCENARIO_FIELDS:
+                v = getattr(t, f)
+                if f in ("add_is_nil", "has_node_weights"):
+                    setattr(scs[i], f, int(v))
+                    continue
+                a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
+                keep.append(a)
+                setattr(scs[i], f, a.ctypes.data if a.size else None)
+        results = [ScenarioResult(base_tables, i in want) for i in range(n)]
+        outs = (api.ScenarioOut * max(1, n))(*[r.out for r in results])
+        self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),
+                                                   int(max_concurrent), outs), "blance_plan_scenarios")
         for r, o in zip(results, outs):
             r.out = o
         return results

@@ -179,6 +179,58 @@ int blance_plan_next_map(blance_ctx* ctx, const blance_plan_in* in, blance_plan_
  * context spreads them over its GPUs. */
 int blance_plan_next_map_batch(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out);
 
+/* ---- what-if scenarios of one cluster ----------------------------------------------------------------------
+ * One variant of a base instance: exactly the inputs of PlanNextMapEx that a what-if changes.  Every field is
+ * required; the base's own node_removed / node_added / add_is_nil / has_node_weights / node_weight /
+ * node_has_weight are ignored by blance_plan_scenarios. */
+typedef struct blance_scenario {
+  const uint8_t* node_removed;     /* [n_node_ids]  nodesToRemove of this variant */
+  const uint8_t* node_added;       /* [n_node_ids]  nodesToAdd of this variant */
+  int32_t add_is_nil;              /* nodesToAdd == nil (plan.go:554); 0 or 1 */
+  int32_t has_node_weights;        /* NodeWeights != nil (plan.go:675); 0 or 1 */
+  const int32_t* node_weight;      /* [n_nodes], read when has_node_weights */
+  const uint8_t* node_has_weight;  /* [n_nodes], read when has_node_weights */
+} blance_scenario;
+
+/* enum blance_op_kind indexes the second dimension of node_ops */
+typedef struct blance_scenario_out {
+  int32_t* next_rows;  uint8_t* next_shape;  uint8_t* warn;  /* as blance_plan_out; each may be NULL (not copied) */
+  int64_t* node_ops;          /* [n_node_ids][4] ops per node by enum blance_op_kind; may be NULL */
+  int64_t* state_node_load;   /* [n_states][n_node_ids]; may be NULL */
+  int32_t iters_run, converged;
+  int64_t steps, sticky_steps;
+  int64_t parts_moved, ops_total, warn_parts;
+} blance_scenario_out;
+
+/* Plans n variants of one cluster: scenario i is the plan of `base` with sc[i]'s six node fields substituted,
+ * i.e. PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, nodesToRemove_i, nodesToAdd_i, model, options with
+ * NodeWeights_i) on private copies of the two maps.  out[i].next_rows / next_shape / warn / iters_run /
+ * converged / steps equal what blance_plan_next_map returns for that substituted instance, whatever n,
+ * max_concurrent, the engine or the number of devices.
+ *
+ * Summaries (computed on the device; only they, the scalars and the requested row tables are copied out):
+ *   node_ops[q][kind], ops_total, parts_moved: for every partition with part_in_assign,
+ *     CalcPartitionMoves(states = all model states in state order, beg = its prev_rows row as passed in (a
+ *     partition with part_in_prev == 0 starts from an empty row), end = its next row, favor_min_nodes) - the
+ *     per-partition call OrchestrateMoves makes (orchestrate.go:273-287).  Each op counts at its node and kind;
+ *     ops_total is their sum; parts_moved counts the partitions with at least one op.
+ *   state_node_load[s][q]: countStateNodes (plan.go:374-399) over the model states of the final map (prevMap
+ *     with every assigned partition replaced by its next row), each entry weighted with the partition's weight
+ *     when has_part_weights is set and it has one, else 1.  Removed nodes keep what unassigned partitions hold.
+ *   warn_parts: assigned partitions with at least one warning bit.
+ *
+ * Errors: n <= 0, a NULL sc / out, or a bad scenario (the first one fails the call; the message names its
+ * index) is BLANCE_ERR_INVALID_ARG, checked before any device work.  BLANCE_ERR_NOMEM when one scenario does
+ * not fit in device memory.
+ *
+ * Scheduling: the base's partition tables are uploaded once per device and replicated on the device into each
+ * scenario of a wave; a wave is one batch through the convergence loop.  max_concurrent > 0 caps the wave size;
+ * 0 picks the largest wave that fits the free device memory, and at most sm_count / 2 when the cluster has more
+ * than 768 nodes (so every scenario keeps the wide speculative kernel).  A multi-device context sends scenario i
+ * to device i mod G, each device with its own copy of the base (DESIGN.md section 8). */
+int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                          int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out);
+
 /* Device-resident variant used by benchmarks and by callers that chain plans:
  * uploads `in` once and returns a handle; blance_plan_run() replays the whole
  * plan on the resident tables (inputs are restored on device before each run);

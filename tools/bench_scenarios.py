@@ -1,0 +1,195 @@
+"""What-if sweeps through blance_plan_scenarios against the same scenarios planned one by one with
+blance_plan_next_map, alternating in the same process, with sampled correctness checks.  Prints one JSON object
+and writes it to --out.
+
+    python tools/bench_scenarios.py [--ks 1,8,33,66,132] [--cfgs 4,3] [--out profiles/h100_scenarios.json]
+
+Clusters: synth.make_rebalance(4) (1 M partitions x 1 024 nodes) and synth.make_rebalance(3) (65 536 x 256 with
+zone and rack rules; its previous map is the fresh stage's plan).  Scenario j keeps the configuration's own
+removals and additions and also fails live node j; cfg 3 adds one scenario per rack that fails the whole rack.
+Timings are host wall clock around calls that end in a device synchronise; the wave size, device bytes per
+scenario and the summary kernel's time come from the library's BLANCE_SCENARIO_TIMES report (CUDA events)."""
+import argparse
+import json
+import os
+import re
+import subprocess
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from blance_b200 import synth, tables  # noqa: E402
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
+        name, power = [x.strip() for x in out.splitlines()[0].split(",")]
+        return dict(gpu=name, power_limit=power)
+    except Exception as e:   # noqa: BLE001 - recorded, not fatal
+        return dict(gpu="unknown (%s)" % e, power_limit="unknown")
+
+
+class CaptureStderr:
+    """Collects what the library writes to fd 2 (its BLANCE_SCENARIO_TIMES lines)."""
+
+    def __enter__(self):
+        sys.stderr.flush()
+        self.f = tempfile.TemporaryFile(mode="w+")
+        self.saved = os.dup(2)
+        os.dup2(self.f.fileno(), 2)
+        os.environ["BLANCE_SCENARIO_TIMES"] = "1"
+        return self
+
+    def __exit__(self, *a):
+        os.environ.pop("BLANCE_SCENARIO_TIMES", None)
+        sys.stderr.flush()
+        os.dup2(self.saved, 2)
+        os.close(self.saved)
+        self.f.seek(0)
+        self.text = self.f.read()
+        self.f.close()
+
+
+WAVE_RE = re.compile(r"scenario wave at \d+: (\d+) scenarios \(wave size (\d+), (\d+) device bytes each\), ([\d.]+) ms, summary ([\d.]+) ms")
+
+
+def parse_waves(text):
+    waves = [dict(n=int(m[0]), wave=int(m[1]), bytes=int(m[2]), ms=float(m[3]), summary_ms=float(m[4])) for m in WAVE_RE.findall(text)]
+    return dict(wave_size=max(w["wave"] for w in waves) if waves else None, waves=len(waves),
+                device_bytes_per_scenario=waves[0]["bytes"] if waves else None,
+                wave_ms=round(sum(w["ms"] for w in waves), 3), summary_ms=round(sum(w["summary_ms"] for w in waves), 3))
+
+
+def live_nodes(t):
+    return [q for q in range(t.n_nodes) if not t.node_removed[q] and not t.node_added[q]]
+
+
+def failure_scenarios(t, k):
+    out = []
+    for q in live_nodes(t)[:k]:
+        rm = t.node_removed.copy()
+        rm[q] = 1
+        out.append(dict(node_removed=rm))
+    return out
+
+
+def rack_scenarios(t, rack=8):
+    out = []
+    for r in range(t.n_nodes // rack):
+        rm = t.node_removed.copy()
+        rm[r * rack:(r + 1) * rack] = 1
+        out.append(dict(node_removed=rm))
+    return out
+
+
+def sweep(ctx, t, scs, max_concurrent=0):
+    with CaptureStderr() as cap:
+        t0 = time.perf_counter()
+        res = ctx.plan_scenarios(t, scs, False, max_concurrent=max_concurrent)
+        wall = time.perf_counter() - t0
+    return res, wall, parse_waves(cap.text)
+
+
+def one_by_one(ctx, t, scs):
+    t0 = time.perf_counter()
+    outs = [ctx.plan_next_map(tables.scenario_tables(t, sc)) for sc in scs]
+    return outs, time.perf_counter() - t0
+
+
+def numpy_summary(ctx, t, next_rows):
+    """The summaries recomputed on the host from the flat tables (moves from blance_calc_partition_moves)."""
+    a = t.part_in_assign != 0
+    beg = np.where((t.part_in_prev != 0)[:, None], t.prev_rows, -1)[a]
+    node, _state, kind, count = ctx.calc_partition_moves(t.state_slot_off, beg, next_rows[a], False)
+    valid = np.arange(node.shape[1])[None, :] < count[:, None]
+    ops = np.zeros((t.n_node_ids, 4), np.int64)
+    np.add.at(ops, (node[valid], kind[valid]), 1)
+    final = np.where(a[:, None], next_rows, t.prev_rows)
+    w = np.where((t.has_part_weights != 0) & (t.part_has_weight != 0), t.part_weight, 1).astype(np.int64)
+    load = np.zeros((t.n_states, t.n_node_ids), np.int64)
+    for s in range(t.n_states):
+        blk = final[:, t.state_slot_off[s]:t.state_slot_off[s + 1]]
+        ok = blk >= 0
+        load[s] = np.bincount(blk[ok], weights=np.broadcast_to(w[:, None], blk.shape)[ok], minlength=t.n_node_ids).astype(np.int64)
+    return ops, load, int((count > 0).sum()), int(count.sum())
+
+
+def check_sample(ctx, t, scs, res, rng):
+    """2 sampled scenarios: rows equal blance_plan_next_map on the substituted tables; summary equals numpy."""
+    ok = True
+    for i in sorted(set(rng.choice(len(scs), size=min(2, len(scs)), replace=False).tolist())):
+        st = tables.scenario_tables(t, scs[i])
+        ref = ctx.plan_next_map(st)
+        got = ctx.plan_scenarios(t, [scs[i]], False, want_rows=[0])[0]
+        ok &= bool(np.array_equal(got.next_rows, ref.next_rows) and np.array_equal(got.warn, ref.warn) and
+                   (got.iters_run, got.converged, got.steps) == (ref.iters_run, ref.converged, ref.steps))
+        ops, load, moved, total = numpy_summary(ctx, st, ref.next_rows)
+        ok &= bool(np.array_equal(res[i].node_ops, ops) and np.array_equal(res[i].state_node_load, load) and
+                   (res[i].parts_moved, res[i].ops_total) == (moved, total) and res[i].steps == ref.steps)
+    return ok
+
+
+def run_cfg(ctx, cfg, ks, rng):
+    if cfg == 3:
+        t = synth.make_rebalance(3, prev_rows=ctx.plan_next_map(synth.make_fresh(3)).next_rows)
+    else:
+        t = synth.make_rebalance(cfg)
+    ctx.plan_scenarios(t, failure_scenarios(t, 2), False)            # warm-up of every kernel the sweep uses
+    ctx.plan_next_map(t)
+    rows = []
+    for k in ks:
+        scs = failure_scenarios(t, k) + (rack_scenarios(t) if cfg == 3 else [])
+        res, wall_a, info = sweep(ctx, t, scs)
+        _, serial = one_by_one(ctx, t, scs)
+        _, wall_b, _ = sweep(ctx, t, scs)
+        wall = min(wall_a, wall_b)
+        row = dict(cfg=cfg, K=k, scenarios=len(scs), sweep_s=[round(wall_a, 3), round(wall_b, 3)],
+                   scenarios_per_s=round(len(scs) / wall, 3), one_by_one_s=round(serial, 3),
+                   one_by_one_scenarios_per_s=round(len(scs) / serial, 3), speedup=round(serial / wall, 3),
+                   summary_share=round(info["summary_ms"] / info["wave_ms"], 5) if info["wave_ms"] else None,
+                   correct=check_sample(ctx, t, scs, res, rng), **info)
+        print(json.dumps(row), flush=True)
+        rows.append(row)
+    return t, rows
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--ks", default="1,8,33,66,132")
+    ap.add_argument("--cfgs", default="4,3")
+    ap.add_argument("--wave-ks", default="33,66,132", help="explicit max_concurrent values tried on cfg 4 at the largest K")
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    ks = [int(x) for x in a.ks.split(",")]
+    rng = np.random.default_rng(0)
+    rec = dict(tool="tools/bench_scenarios.py", **gpu_info())
+    ctx = tables.Context()
+    rec["sm_count_note"] = "auto wave: free device memory, and at most sm_count / 2 above 768 nodes"
+    rec["results"] = []
+    for cfg in [int(x) for x in a.cfgs.split(",")]:
+        t, rows = run_cfg(ctx, cfg, ks, rng)
+        rec["results"] += rows
+        if cfg == 4 and a.wave_ks:
+            scs = failure_scenarios(t, max(ks))
+            waves = []
+            for mc in [0] + [int(x) for x in a.wave_ks.split(",")]:
+                _, wall, info = sweep(ctx, t, scs, max_concurrent=mc)
+                waves.append(dict(max_concurrent=mc, sweep_s=round(wall, 3), scenarios_per_s=round(len(scs) / wall, 3), **info))
+                print(json.dumps(waves[-1]), flush=True)
+            rec["cfg4_wave_sizes"] = dict(K=max(ks), runs=waves)
+    ctx.close()
+    print(json.dumps(rec))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(rec, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
