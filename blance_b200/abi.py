@@ -46,9 +46,21 @@ class _ScenarioOut(ctypes.Structure):  # struct blance_scenario_out
                 ("warn_parts", ctypes.c_int64)]
 
 
+OPT_CONSTRAINTS, OPT_STICKINESS, OPT_PART_WEIGHTS, OPT_HIERARCHY = 1, 2, 4, 8   # enum blance_scenario_opt_set
+
+
+class _ScenarioOpts(ctypes.Structure):  # struct blance_scenario_opts
+    _fields_ = [("set", ctypes.c_uint32), ("state_constraints", ctypes.c_void_p), ("state_stickiness", ctypes.c_void_p),
+                ("state_has_stickiness", ctypes.c_void_p), ("has_part_weights", ctypes.c_int32),
+                ("n_weight_overrides", ctypes.c_int32), ("ow_part", ctypes.c_void_p), ("ow_weight", ctypes.c_void_p),
+                ("ow_has", ctypes.c_void_p), ("extra_tot_first", ctypes.c_void_p), ("extra_tot_rest", ctypes.c_void_p),
+                ("has_hier_rules", ctypes.c_int32), ("n_rules", ctypes.c_int32), ("n_hier_bits", ctypes.c_int32),
+                ("rule_off", ctypes.c_void_p), ("ie_mask", ctypes.c_void_p)]
+
+
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available", "blance_moves_free")
 
 
@@ -71,6 +83,7 @@ def capi():
         lib.blance_plan_next_map.argtypes = [vp, vp, vp]
         lib.blance_plan_next_map_batch.argtypes = [vp, i32, vp, vp]
         lib.blance_plan_scenarios.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+        lib.blance_plan_scenarios_ex.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
         lib.blance_plan_run.argtypes = [vp, vp]
         lib.blance_plan_fetch.argtypes = [vp, vp, vp]
@@ -91,4 +104,5 @@ def capi():
 PlanIn = _PlanIn
 PlanOut = _PlanOut
 Scenario = _Scenario
+ScenarioOpts = _ScenarioOpts
 ScenarioOut = _ScenarioOut

@@ -72,6 +72,15 @@ def PlanNextMap(prevMap, partitionsToAssign, nodesAll, nodesToRemove, nodesToAdd
                                             nodeHierarchy, hierarchyRules))
 
 
+def _rules_arg(rules):
+    return None if rules is None else {k: [tuple(x) for x in v] for k, v in rules.items()}
+
+
+# the optional per-scenario option keys, in the order _host expects their (has_key, value) pairs
+_SCENARIO_OPTION_KEYS = (("nodeWeights", dict), ("modelStateConstraints", dict), ("stateStickiness", dict),
+                         ("partitionWeights", dict), ("nodeHierarchy", dict), ("hierarchyRules", _rules_arg))
+
+
 def _scenario_tuples(scenarios):
     out = []
     for i, sc in enumerate(scenarios):
@@ -79,8 +88,10 @@ def _scenario_tuples(scenarios):
         if missing:
             raise ValueError("scenario %d lacks %s" % (i, ", ".join(sorted(missing))))
         rm, ad = sc["nodesToRemove"], sc["nodesToAdd"]
-        out.append((None if rm is None else list(rm), None if ad is None else list(ad), "nodeWeights" in sc,
-                    None if sc.get("nodeWeights") is None else dict(sc["nodeWeights"])))
+        t = [None if rm is None else list(rm), None if ad is None else list(ad)]
+        for key, conv in _SCENARIO_OPTION_KEYS:
+            t += [key in sc, None if sc.get(key) is None else conv(sc[key])]
+        out.append(tuple(t))
     return out
 
 
@@ -95,8 +106,10 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
                          wantMaps=(), maxConcurrent=0):
     """What-if variants of one cluster, planned side by side on the device.  Scenario i is
     PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, sc["nodesToRemove"], sc["nodesToAdd"], model, options with
-    NodeWeights = sc["nodeWeights"]): both node-set keys are required (None = nil); a missing "nodeWeights" key
-    inherits options.NodeWeights, None means nil.  The caller's maps are NOT mutated.
+    the scenario's plan options substituted): both node-set keys are required (None = nil).  The optional keys
+    "nodeWeights", "modelStateConstraints", "stateStickiness", "partitionWeights", "nodeHierarchy" and
+    "hierarchyRules" replace the options field of the same name; a missing key inherits it, None means nil.
+    The caller's maps are NOT mutated.
 
     Returns one dict per scenario: iterations, converged, steps, sticky_steps, parts_moved, ops_total, warn_parts,
     node_ops {node: {op: count}} and state_node_load {state: {node: load}} (nonzero entries only), plus next_map and
@@ -130,4 +143,4 @@ def CalcPartitionMovesMap(states, begMap, endMap, favorMinNodes):
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------
-from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401
+from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401

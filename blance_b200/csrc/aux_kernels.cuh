@@ -458,6 +458,19 @@ __global__ void k_scenario_replicate(int32_t* __restrict__ rows_init, int32_t* _
   }
 }
 
+// Partition-weight overrides of a wave's scenarios (blance_scenario_opts), one thread per override: ow[j] is the
+// wave-global partition index, ow[n + j] its weight, ow[2n + j] its presence.  The indices are distinct (checked on
+// the host before any device work), so every word is written by one thread and plain stores suffice.
+__global__ void k_scenario_weights(int32_t* __restrict__ pweight, uint8_t* __restrict__ pflags_init,
+                                   const int32_t* __restrict__ ow, int32_t n) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const int32_t g = ow[j];
+    pweight[g] = ow[n + j];
+    const uint8_t f = pflags_init[g];
+    pflags_init[g] = ow[2 * n + j] ? (uint8_t)(f | PF_HAS_WEIGHT) : (uint8_t)(f & ~PF_HAS_WEIGHT);
+  }
+}
+
 // Per instance: CalcPartitionMoves(prev row as uploaded -> next row) of every assigned partition, counted per
 // node and op kind; countStateNodes of the final map per state and node; partitions with an op / a warning.
 // out[i] = node_ops [NU][4] | state_node_load [S][NU] | parts_moved, ops_total, warn_parts  (int64, stride

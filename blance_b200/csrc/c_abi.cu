@@ -5,7 +5,9 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -1035,11 +1037,69 @@ extern "C" int blance_plan_next_map_batch(blance_ctx* ctx, int32_t n, const blan
 // What-if scenarios of one cluster (blance_plan_scenarios): the base is uploaded once per device, each wave of
 // scenarios is a batch whose partition slices are replicated from it on the device.
 
-static blance_plan_in scenario_in(const blance_plan_in& base, const blance_scenario& sc) {
+// The substituted instance of one scenario.  The partition weights of its overrides are not in it: they are
+// applied on the device (k_scenario_weights) after the base is replicated.
+static blance_plan_in scenario_in(const blance_plan_in& base, const blance_scenario& sc, const blance_scenario_opts* o) {
   blance_plan_in in = base;
   in.node_removed = sc.node_removed; in.node_added = sc.node_added; in.add_is_nil = sc.add_is_nil;
   in.has_node_weights = sc.has_node_weights; in.node_weight = sc.node_weight; in.node_has_weight = sc.node_has_weight;
+  if (!o) return in;
+  if (o->set & BLANCE_OPT_CONSTRAINTS) in.state_constraints = o->state_constraints;
+  if (o->set & BLANCE_OPT_STICKINESS) { in.state_stickiness = o->state_stickiness; in.state_has_stickiness = o->state_has_stickiness; }
+  if (o->set & BLANCE_OPT_PART_WEIGHTS) {
+    in.has_part_weights = o->has_part_weights;
+    if (o->extra_tot_first) in.extra_tot_first = o->extra_tot_first;
+    if (o->extra_tot_rest) in.extra_tot_rest = o->extra_tot_rest;
+  }
+  if (o->set & BLANCE_OPT_HIERARCHY) {
+    in.has_hier_rules = o->has_hier_rules; in.n_rules = o->n_rules; in.n_hier_bits = o->n_hier_bits;
+    in.rule_off = o->rule_off; in.ie_mask = o->ie_mask;
+  }
   return in;
+}
+
+static const blance_scenario_opts* opts_of(const blance_scenario_opts* opts, int i) { return opts ? &opts[i] : nullptr; }
+
+static int n_overrides(const blance_scenario_opts* o) {
+  return o && (o->set & BLANCE_OPT_PART_WEIGHTS) ? o->n_weight_overrides : 0;
+}
+
+// The option checks of one scenario that check_structure cannot make (flags, override lists, the int32 bound).
+// base_sum: sum over the base's partitions of |weight| (1 where it has none), computed once by the caller.
+static int check_opts(const blance_plan_in& base, const blance_scenario_opts& o, long long base_sum, std::string& why) {
+  auto bad = [&](const std::string& what, int st = BLANCE_ERR_INVALID_ARG) { why = what; return st; };
+  const uint32_t all = BLANCE_OPT_CONSTRAINTS | BLANCE_OPT_STICKINESS | BLANCE_OPT_PART_WEIGHTS | BLANCE_OPT_HIERARCHY;
+  if (o.set & ~all) return bad("opts.set has an unknown bit");
+  if ((o.set & BLANCE_OPT_STICKINESS) && o.state_has_stickiness)
+    for (int s = 0; s < base.n_states; ++s)
+      if (o.state_has_stickiness[s] > 1) return bad("state_has_stickiness is neither 0 nor 1");
+  if ((o.set & BLANCE_OPT_HIERARCHY) && o.has_hier_rules != 0 && o.has_hier_rules != 1) return bad("has_hier_rules is neither 0 nor 1");
+  if (!(o.set & BLANCE_OPT_PART_WEIGHTS)) return BLANCE_OK;
+  if (o.has_part_weights != 0 && o.has_part_weights != 1) return bad("has_part_weights is neither 0 nor 1");
+  const int k = o.n_weight_overrides;
+  if (k < 0) return bad("n_weight_overrides is negative");
+  if (k > 0 && (!o.ow_part || !o.ow_weight || !o.ow_has)) return bad("weight override arrays are NULL");
+  std::vector<int32_t> seen(o.ow_part, o.ow_part + k);
+  std::sort(seen.begin(), seen.end());
+  if (k > 0 && (seen.front() < 0 || seen.back() >= base.n_parts)) return bad("a weight override's partition is outside [0, n_parts)");
+  if (std::adjacent_find(seen.begin(), seen.end()) != seen.end()) return bad("a partition has two weight overrides");
+  long long sum = base_sum;                 // sum |w_p| with the overrides applied (as if PartitionWeights != nil)
+  for (int j = 0; j < k; ++j) {
+    if (o.ow_has[j] > 1) return bad("ow_has is neither 0 nor 1");
+    if (o.ow_has[j] && o.ow_weight[j] > 999999999)      // the "%10d" rule of plan.go:539, as blance_plan_in_check
+      return bad("partition weight above 999999999 in override " + std::to_string(j), BLANCE_ERR_UNSUPPORTED);
+    const int32_t p = o.ow_part[j];
+    const long long old_w = base.part_has_weight[p] ? std::llabs((long long)base.part_weight[p]) : 1;
+    sum += (o.ow_has[j] ? std::llabs((long long)o.ow_weight[j]) : 1) - old_w;
+  }
+  const long long bound = (o.has_part_weights ? sum : (long long)base.n_parts) * std::max(1, base.n_slots);
+  if (bound > INT32_MAX) return bad("sum of partition weights x slots exceeds int32 (the device keeps int32 counts)", BLANCE_ERR_UNSUPPORTED);
+  return BLANCE_OK;
+}
+
+// uint32 words of one instance's hierarchy masks
+static long long mask_words(const blance_plan_in& in) {
+  return in.has_hier_rules ? (long long)in.n_rules * (in.n_node_ids + 1) * ((in.n_hier_bits + 31) / 32) : 0;
 }
 
 // int64 words of one scenario's summary: node_ops [NU][4] | state_node_load [S][NU] | 3 scalars
@@ -1047,14 +1107,17 @@ static long long summary_stride(const blance_plan_in& base) {
   return 4ll * base.n_node_ids + (long long)base.n_states * base.n_node_ids + 3;
 }
 
-// The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).
-static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, int n_dev, int max_concurrent, size_t* per_scenario) {
+// The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
+// their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and override list of any.
+static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
+                     int max_concurrent, size_t* per_scenario) {
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
   PlanBufs b;
   const size_t per = slices_bytes(arena_slices(&probe, 1, b)) + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
-                     sizeof(long long) * (size_t)summary_stride(in0);
+                     sizeof(long long) * (size_t)summary_stride(in0) +
+                     sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides;
   *per_scenario = per;
   if (max_concurrent > 0) return std::min(n_dev, max_concurrent);
   size_t free_b = 0, total_b = 0;
@@ -1068,7 +1131,7 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, int n_dev, int 
 }
 
 static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
-                               int favor_min, int max_concurrent, blance_scenario_out* out) {
+                               const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out) {
   std::lock_guard<std::mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
   {
@@ -1077,7 +1140,13 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
   }
   cudaStream_t st = ctx->stream;
   const int n_dev = (int)idx.size();
-  const blance_plan_in in0 = scenario_in(*base, sc[idx[0]]);
+  const blance_plan_in in0 = scenario_in(*base, sc[idx[0]], opts_of(opts, idx[0]));
+  long long max_mask = 0;
+  int max_ow = 0;
+  for (int i : idx) {
+    max_mask = std::max(max_mask, mask_words(scenario_in(*base, sc[i], opts_of(opts, i))));
+    max_ow = std::max(max_ow, n_overrides(opts_of(opts, i)));
+  }
   {
     cudaMemPool_t pool;                // measure free memory without this context's cached arenas
     if (max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
@@ -1092,7 +1161,7 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
     if (rc != BLANCE_OK) return rc;
   }
   size_t per = 0;
-  int W = wave_size(ctx, in0, n_dev, max_concurrent, &per);
+  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, &per);
   if (W < 1) {
     plan_release(pb, ctx);
     return fail(ctx, BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
@@ -1105,8 +1174,8 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
   for (int w0 = 0; w0 < n_dev && rc == BLANCE_OK;) {
     const int nw = std::min(W, n_dev - w0);
     std::vector<blance_plan_in> ins((size_t)nw);
-    for (int j = 0; j < nw; ++j) ins[(size_t)j] = scenario_in(*base, sc[idx[(size_t)(w0 + j)]]);
-    // a device's only scenario is the base upload itself: nothing to replicate
+    for (int j = 0; j < nw; ++j) ins[(size_t)j] = scenario_in(*base, sc[idx[(size_t)(w0 + j)]], opts_of(opts, idx[(size_t)(w0 + j)]));
+    // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
     const bool lone = n_dev == 1;
     blance_plan* pl = lone ? pb : new blance_plan();
     std::vector<int> seg_off;
@@ -1173,6 +1242,37 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
           pb->pool.name_rank, PU, SLP, pl->PT);
       ctx->launches++;
       step(cudaGetLastError(), "k_scenario_replicate");
+    }
+    // the wave's partition-weight overrides over its replicated slices (lone: over the base upload), as
+    // wave-global partition indices: ow = index[k] | weight[k] | presence[k]
+    std::vector<int32_t> ow;
+    for (int pass = 0; pass < 3; ++pass)
+      for (int j = 0; j < nw; ++j) {
+        const blance_scenario_opts* o = opts_of(opts, idx[(size_t)(w0 + j)]);
+        for (int k = 0; k < n_overrides(o); ++k)
+          ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
+      }
+    if (rc == BLANCE_OK && !ow.empty()) {
+      const int k = (int)(ow.size() / 3);
+      int32_t* d_ow = nullptr;
+      if (cudaMallocAsync((void**)&d_ow, sizeof(int32_t) * ow.size(), st) != cudaSuccess) {
+        cudaGetLastError();
+        rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the weight overrides failed");
+      } else {
+        step(cudaMemcpyAsync(d_ow, ow.data(), sizeof(int32_t) * ow.size(), cudaMemcpyHostToDevice, st), "H2D");
+        int32_t* pweight = lone ? const_cast<int32_t*>(pb->pool.pweight) : b.pweight;   // (the base upload is this scenario's own)
+        if (rc == BLANCE_OK) {
+          k_scenario_weights<<<grid_for(ctx, k, 256), 256, 0, st>>>(pweight, pl->pflags_init, d_ow, k);
+          ctx->launches++;
+          step(cudaGetLastError(), "k_scenario_weights");
+        }
+        cudaFreeAsync(d_ow, st);
+      }
+      if (rc != BLANCE_OK) {
+        cudaFreeAsync(d_sum, st);
+        if (!lone) plan_release(pl, ctx);
+        break;
+      }
     }
     if (!lone && rc == BLANCE_OK) {
       rc = finish_upload(ctx, pl);
@@ -1245,33 +1345,41 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
   return rc;
 }
 
-extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
-                                     int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
+static int plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                          const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
   if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: n must be positive");
-  if (!base || !sc || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: base, sc or out is NULL");
+  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
+  if (!base || !sc || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
   // every scenario is checked before any device work
+  long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
   for (int i = 0; i < n; ++i) {
     std::string why;
+    int st = BLANCE_OK;
+    const blance_scenario_opts* o = opts_of(opts, i);
     if (sc[i].add_is_nil != 0 && sc[i].add_is_nil != 1) why = "add_is_nil is neither 0 nor 1";
     else if (sc[i].has_node_weights != 0 && sc[i].has_node_weights != 1) why = "has_node_weights is neither 0 nor 1";
     else {
-      const blance_plan_in in = scenario_in(*base, sc[i]);
-      const int st = check_structure(&in, why);
-      if (st != BLANCE_OK) return fail(ctx, st, "blance_plan_scenarios: scenario " + std::to_string(i) + ": " + why);
+      const blance_plan_in in = scenario_in(*base, sc[i], o);
+      st = check_structure(&in, why);
+      if (st == BLANCE_OK && o && (o->set & BLANCE_OPT_PART_WEIGHTS) && base_sum < 0) {
+        base_sum = 0;
+        for (int p = 0; p < base->n_parts; ++p) base_sum += base->part_has_weight[p] ? std::llabs((long long)base->part_weight[p]) : 1;
+      }
+      if (st == BLANCE_OK && o) st = check_opts(*base, *o, base_sum, why);
     }
-    if (!why.empty()) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_plan_scenarios: scenario " + std::to_string(i) + ": " + why);
+    if (st == BLANCE_OK && !why.empty()) st = BLANCE_ERR_INVALID_ARG;
+    if (st != BLANCE_OK) return fail(ctx, st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
   }
   const int G = ctx->children.empty() ? 1 : (int)std::min<size_t>(ctx->children.size(), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
-  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, favor_min_nodes, max_concurrent, out);
+  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, opts, favor_min_nodes, max_concurrent, out);
   // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
   std::vector<int> status((size_t)G, BLANCE_OK);
   std::vector<std::thread> th;
   for (int d = 0; d < G; ++d)
     th.emplace_back([&, d]() {
-      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, favor_min_nodes, max_concurrent, out);
+      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out);
     });
   for (auto& t : th) t.join();
   for (int d = 0; d < G; ++d)
@@ -1280,6 +1388,17 @@ extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base
       return status[(size_t)d];
     }
   return BLANCE_OK;
+}
+
+extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                     int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
+  return plan_scenarios(ctx, "blance_plan_scenarios", base, n, sc, nullptr, favor_min_nodes, max_concurrent, out);
+}
+
+extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                        const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                        blance_scenario_out* out) {
+  return plan_scenarios(ctx, "blance_plan_scenarios_ex", base, n, sc, opts, favor_min_nodes, max_concurrent, out);
 }
 
 extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,

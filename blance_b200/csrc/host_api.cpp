@@ -233,6 +233,53 @@ int32_t checked_i32(long long v, const char* what) {
   return int32_t(v);
 }
 
+// The hierarchy bit sets of blance_plan_in (plan.go:174-226, 703-774): rule_off over the states of `state_names`,
+// and ie_mask[r][a] for every node id a of `node_names` plus the "" anchor.  `ids` maps node_names to their ids;
+// the first N are nodesAll.
+void hierarchy_tables(const Strs& state_names, const Strs& node_names, const std::unordered_map<std::string, int32_t>& ids,
+                      int32_t N, const std::optional<HierarchyRules>& rules_opt,
+                      const std::optional<std::unordered_map<std::string, std::string>>& parents, std::vector<int32_t>* rule_off,
+                      std::vector<uint32_t>* ie_mask, int32_t* n_rules, int32_t* n_hier_bits) {
+  const int32_t S = int32_t(state_names.size()), NU = int32_t(node_names.size());
+  rule_off->assign(size_t(S) + 1, 0);
+  ie_mask->clear();
+  *n_rules = 0;
+  *n_hier_bits = N;
+  if (!rules_opt) return;
+  std::vector<HierarchyRule> rules;
+  for (int32_t s = 0; s < S; ++s) {
+    auto it = rules_opt->find(state_names[size_t(s)]);
+    if (it != rules_opt->end())
+      for (const auto& r : it->second) rules.push_back(r);
+    (*rule_off)[size_t(s) + 1] = int32_t(rules.size());
+  }
+  *n_rules = int32_t(rules.size());
+  if (*n_rules == 0) return;
+  Hierarchy h(parents ? &*parents : nullptr);
+  // pass 1: the lists, and the leaf names outside nodesAll
+  Interner extra_bits;
+  std::vector<std::vector<int32_t>> lists(size_t(*n_rules) * size_t(NU + 1));
+  for (int32_t r = 0; r < *n_rules; ++r)
+    for (int32_t a = 0; a <= NU; ++a) {
+      const std::string anchor = a < NU ? node_names[size_t(a)] : std::string();
+      const Strs& inc = h.leaves(h.ancestor(anchor, rules[size_t(r)].IncludeLevel));
+      const Strs& exc = h.leaves(h.ancestor(anchor, rules[size_t(r)].ExcludeLevel));
+      std::unordered_set<std::string> ex(exc.begin(), exc.end());
+      auto& out = lists[size_t(r) * size_t(NU + 1) + size_t(a)];
+      for (const auto& leaf : inc) {
+        if (ex.count(leaf)) continue;                          // plan.go:733
+        auto id = ids.find(leaf);
+        if (id != ids.end() && id->second < N) out.push_back(id->second);
+        else out.push_back(N + extra_bits.get(leaf));
+      }
+    }
+  *n_hier_bits = N + int32_t(extra_bits.names.size());
+  const size_t HW = size_t((*n_hier_bits + 31) / 32);
+  ie_mask->assign(size_t(*n_rules) * size_t(NU + 1) * HW, 0u);
+  for (size_t i = 0; i < lists.size(); ++i)
+    for (int32_t b : lists[i]) (*ie_mask)[i * HW + size_t(b >> 5)] |= 1u << (b & 31);
+}
+
 // plan.go:544-545 dereferences prevMap[name] whenever nodesToRemove is non-empty
 void check_remove_needs_prev(const InternedPlan& ip, const OptStrs& nodesToRemove, const std::string& who) {
   if (deref(nodesToRemove).empty()) return;
@@ -245,10 +292,13 @@ void check_remove_needs_prev(const InternedPlan& ip, const OptStrs& nodesToRemov
 
 // ------------------------------------------------------------------------------------
 
-std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
-                                         const Strs& nodesAll, const OptStrs& nodesToRemove,
-                                         const OptStrs& nodesToAdd, const PartitionModel& model,
-                                         const PlanNextMapOptions& options) {
+// InternPlan, with each state's slot range at least min_width[state name] wide (when given): the shared layout of a
+// scenario sweep whose scenarios raise constraints.
+static std::unique_ptr<InternedPlan> intern_plan(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                                 const Strs& nodesAll, const OptStrs& nodesToRemove,
+                                                 const OptStrs& nodesToAdd, const PartitionModel& model,
+                                                 const PlanNextMapOptions& options,
+                                                 const std::unordered_map<std::string, int>* min_width) {
   auto ip = std::make_unique<InternedPlan>();
   blance_plan_in& in = ip->in;
 
@@ -405,7 +455,13 @@ std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const Part
   // filled in ONE pass over the maps assuming the constraints are wide enough; a longer list (rare) only
   // records the width it needs and the pass is repeated with the right layout.
   std::vector<int32_t> cap(size_t(S), 0);
-  for (int32_t s = 0; s < S; ++s) cap[size_t(s)] = std::max(0, ip->state_constraints[size_t(s)]);
+  for (int32_t s = 0; s < S; ++s) {
+    cap[size_t(s)] = std::max(0, ip->state_constraints[size_t(s)]);
+    if (min_width) {
+      auto it = min_width->find(ip->state_names[size_t(s)]);
+      if (it != min_width->end()) cap[size_t(s)] = std::max(cap[size_t(s)], it->second);
+    }
+  }
   struct Extra { int32_t part; int32_t node; };
   struct Unknown { size_t pos; int which; const std::string* name; };   // a row cell (or extras entry) naming a node outside nodesAll
   std::vector<Extra> extras;   // prevMap entries under non-model states (only feed tot)
@@ -509,7 +565,11 @@ std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const Part
   // ---- counts under non-model states
   ip->extra_tot_first.assign(size_t(N), 0);
   ip->extra_tot_rest.assign(size_t(N), 0);
+  ip->extra_part.clear();
+  ip->extra_node.clear();
   for (const auto& e : extras) {
+    ip->extra_part.push_back(e.part);
+    ip->extra_node.push_back(e.node);
     if (e.node >= N) continue;
     long long w = (options.PartitionWeights && ip->part_has_weight[size_t(e.part)]) ? ip->part_weight[size_t(e.part)] : 1;
     ip->extra_tot_first[size_t(e.node)] = checked_i32((long long)ip->extra_tot_first[size_t(e.node)] + w, "count");
@@ -528,43 +588,9 @@ std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const Part
   }
 
   // ---- hierarchy bit sets
-  ip->rule_off.assign(size_t(S) + 1, 0);
   int32_t n_rules = 0, n_hier_bits = N;
-  if (options.HierarchyRules) {
-    std::vector<HierarchyRule> rules;
-    for (int32_t s = 0; s < S; ++s) {
-      auto it = options.HierarchyRules->find(ip->state_names[size_t(s)]);
-      if (it != options.HierarchyRules->end())
-        for (const auto& r : it->second) rules.push_back(r);
-      ip->rule_off[size_t(s) + 1] = int32_t(rules.size());
-    }
-    n_rules = int32_t(rules.size());
-    if (n_rules > 0) {
-      Hierarchy h(options.NodeHierarchy ? &*options.NodeHierarchy : nullptr);
-      // pass 1: the lists, and the leaf names outside nodesAll
-      Interner extra_bits;
-      std::vector<std::vector<int32_t>> lists(size_t(n_rules) * size_t(NU + 1));
-      for (int32_t r = 0; r < n_rules; ++r)
-        for (int32_t a = 0; a <= NU; ++a) {
-          const std::string anchor = a < NU ? nodes.names[size_t(a)] : std::string();
-          const Strs& inc = h.leaves(h.ancestor(anchor, rules[size_t(r)].IncludeLevel));
-          const Strs& exc = h.leaves(h.ancestor(anchor, rules[size_t(r)].ExcludeLevel));
-          std::unordered_set<std::string> ex(exc.begin(), exc.end());
-          auto& out = lists[size_t(r) * size_t(NU + 1) + size_t(a)];
-          for (const auto& leaf : inc) {
-            if (ex.count(leaf)) continue;                          // plan.go:733
-            int32_t id = nodes.find(leaf);
-            if (id >= 0 && id < N) out.push_back(id);
-            else out.push_back(N + extra_bits.get(leaf));
-          }
-        }
-      n_hier_bits = N + int32_t(extra_bits.names.size());
-      const size_t HW = size_t((n_hier_bits + 31) / 32);
-      ip->ie_mask.assign(size_t(n_rules) * size_t(NU + 1) * HW, 0u);
-      for (size_t i = 0; i < lists.size(); ++i)
-        for (int32_t b : lists[i]) ip->ie_mask[i * HW + size_t(b >> 5)] |= 1u << (b & 31);
-    }
-  }
+  hierarchy_tables(ip->state_names, nodes.names, nodes.ids, N, options.HierarchyRules, options.NodeHierarchy, &ip->rule_off,
+                   &ip->ie_mask, &n_rules, &n_hier_bits);
 
   ip->node_names = nodes.names;
 
@@ -604,6 +630,13 @@ std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const Part
   return ip;
 }
 
+std::unique_ptr<InternedPlan> InternPlan(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                         const Strs& nodesAll, const OptStrs& nodesToRemove,
+                                         const OptStrs& nodesToAdd, const PartitionModel& model,
+                                         const PlanNextMapOptions& options) {
+  return intern_plan(prevMap, partitionsToAssign, nodesAll, nodesToRemove, nodesToAdd, model, options, nullptr);
+}
+
 PlanOutBuffers::PlanOutBuffers(const InternedPlan& ip) {
   next_rows.assign(size_t(ip.in.n_parts) * size_t(ip.in.n_slots) + 1, BLANCE_NO_NODE);
   next_shape.assign(size_t(ip.in.n_parts) * size_t(ip.in.n_states) + 1, 0);
@@ -613,7 +646,14 @@ PlanOutBuffers::PlanOutBuffers(const InternedPlan& ip) {
   out.warn = warn.data();
 }
 
+static PartitionMap unintern_plan(const InternedPlan& ip, const PlanOutBuffers& ob, Warnings* warnings, const int32_t* constraints);
+
 PartitionMap UninternPlan(const InternedPlan& ip, const PlanOutBuffers& ob, Warnings* warnings) {
+  return unintern_plan(ip, ob, warnings, ip.state_constraints.data());
+}
+
+// UninternPlan whose warnings name `constraints` (a scenario's own) instead of the tables' constraints
+static PartitionMap unintern_plan(const InternedPlan& ip, const PlanOutBuffers& ob, Warnings* warnings, const int32_t* constraints) {
   const blance_plan_in& in = ip.in;
   // the assigned partitions (plan.go:326-330), built in parallel, then moved into the map
   std::vector<int32_t> ids;
@@ -646,7 +686,7 @@ PartitionMap UninternPlan(const InternedPlan& ip, const PlanOutBuffers& ob, Warn
       for (int32_t s = 0; s < in.n_states; ++s)
         if (ob.warn[size_t(p) * size_t(in.n_states) + size_t(s)]) {
           char buf[32];                                              // plan.go:231-234
-          std::snprintf(buf, sizeof buf, "%d", ip.state_constraints[size_t(s)]);
+          std::snprintf(buf, sizeof buf, "%d", constraints[s]);
           (*warnings)[parts[i].Name].push_back(std::string("could not meet constraints: ") + buf +
                                                ", stateName: " + ip.state_names[size_t(s)] +
                                                ", partitionName: " + parts[i].Name);
@@ -882,29 +922,102 @@ PartitionMap PlanNextMapEx(PartitionMap& prevMap, PartitionMap& partitionsToAssi
 
 namespace {
 
+constexpr int kMaxConstraints = 16;   // BL_K_MAX of the device (device_types.cuh)
+
+// ModelStateConstraints of `state` in scenario `sc` (plan.go:308-319 on the substituted options)
+int scenario_constraint(const PartitionModel& model, const PlanNextMapOptions& options, const Scenario& sc, const std::string& state) {
+  int k = model.at(state).Constraints;
+  const auto& msc = sc.ModelStateConstraints ? *sc.ModelStateConstraints : options.ModelStateConstraints;
+  if (msc) {
+    auto it = msc->find(state);
+    if (it != msc->end()) k = it->second;
+  }
+  return k;
+}
+
 // The base tables of a scenario sweep.  The node-id space holds every name of every scenario's nodesToRemove and
 // nodesToAdd (a removed name outside nodesAll still makes len(nodesToRemove) > 0, plan.go:543); the base's own node
-// flags and weights are replaced per scenario.
+// flags and weights are replaced per scenario.  Every state's slot range holds the largest constraint of any
+// scenario: all scenarios share one row layout.
 std::unique_ptr<InternedPlan> intern_scenario_base(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                    const Strs& nodesAll, const PartitionModel& model,
                                                    const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios) {
   Strs names;
-  for (const auto& sc : scenarios) {
+  std::unordered_map<std::string, int> width;
+  for (size_t i = 0; i < scenarios.size(); ++i) {
+    const Scenario& sc = scenarios[i];
     for (const auto& n : deref(sc.NodesToRemove)) names.push_back(n);
     for (const auto& n : deref(sc.NodesToAdd)) names.push_back(n);
+    if (!sc.ModelStateConstraints) continue;
+    for (const auto& kv : model) {
+      const int k = scenario_constraint(model, options, sc, kv.first);
+      if (k > kMaxConstraints)
+        throw BlanceError(BLANCE_ERR_UNSUPPORTED, "blance: scenario " + std::to_string(i) + ": constraints " + std::to_string(k) +
+                                                      " of state '" + kv.first + "' are above 16, the device's limit");
+      int& w = width[kv.first];
+      w = std::max(w, k);
+    }
   }
-  return InternPlan(prevMap, partitionsToAssign, nodesAll, std::nullopt, OptStrs(std::move(names)), model, options);
+  return intern_plan(prevMap, partitionsToAssign, nodesAll, std::nullopt, OptStrs(std::move(names)), model, options, &width);
 }
 
+// One scenario's substitutions of the base tables: its node fields, and the option groups it sets
+// (blance_scenario_opts; the arrays live here, scenario_opts() points at them).
 struct ScenarioTables {
   std::vector<uint8_t> removed, added, has_weight;
   std::vector<int32_t> weight;
   int32_t add_is_nil = 0, has_node_weights = 0;
+  uint32_t set = 0;
+  std::vector<int32_t> constraints, stickiness;
+  std::vector<uint8_t> has_stickiness;
+  int32_t has_part_weights = 0;
+  std::vector<int32_t> ow_part, ow_weight;          // weight overrides, ascending partition
+  std::vector<uint8_t> ow_has;
+  std::vector<int32_t> extra_first, extra_rest;     // empty: the base's
+  int32_t has_hier_rules = 0, n_rules = 0, n_hier_bits = 0;
+  std::vector<int32_t> rule_off;
+  std::vector<uint32_t> ie_mask;
 };
 
-ScenarioTables scenario_tables(const InternedPlan& ip, const Scenario& sc, const PlanNextMapOptions& options, size_t index) {
-  check_remove_needs_prev(ip, sc.NodesToRemove, "scenario " + std::to_string(index) + ": ");
-  const int32_t N = ip.in.n_nodes, NU = ip.in.n_node_ids;
+blance_scenario_opts scenario_opts(const ScenarioTables& t) {
+  blance_scenario_opts o{};
+  o.set = t.set;
+  o.state_constraints = t.constraints.data();
+  o.state_stickiness = t.stickiness.data();
+  o.state_has_stickiness = t.has_stickiness.data();
+  o.has_part_weights = t.has_part_weights;
+  o.n_weight_overrides = int32_t(t.ow_part.size());
+  o.ow_part = t.ow_part.data();
+  o.ow_weight = t.ow_weight.data();
+  o.ow_has = t.ow_has.data();
+  o.extra_tot_first = t.extra_first.empty() ? nullptr : t.extra_first.data();
+  o.extra_tot_rest = t.extra_rest.empty() ? nullptr : t.extra_rest.data();
+  o.has_hier_rules = t.has_hier_rules;
+  o.n_rules = t.n_rules;
+  o.n_hier_bits = t.n_hier_bits;
+  o.rule_off = t.rule_off.data();
+  o.ie_mask = t.ie_mask.empty() ? nullptr : t.ie_mask.data();
+  return o;
+}
+
+// partition name -> index of the base tables, built on first use (only scenarios with their own weights need it)
+struct PartIndex {
+  const InternedPlan& ip;
+  std::unordered_map<std::string_view, int32_t> id;
+  const std::unordered_map<std::string_view, int32_t>& get() {
+    if (id.empty() && !ip.part_names.empty()) {
+      id.reserve(ip.part_names.size());
+      for (size_t p = 0; p < ip.part_names.size(); ++p) id.emplace(ip.part_names[p], int32_t(p));
+    }
+    return id;
+  }
+};
+
+ScenarioTables scenario_tables(const InternedPlan& ip, const PartitionModel& model, const Scenario& sc,
+                               const PlanNextMapOptions& options, size_t index, PartIndex& parts) {
+  const std::string who = "scenario " + std::to_string(index) + ": ";
+  check_remove_needs_prev(ip, sc.NodesToRemove, who);
+  const int32_t N = ip.in.n_nodes, NU = ip.in.n_node_ids, S = ip.in.n_states;
   std::unordered_map<std::string, int32_t> id;
   id.reserve(size_t(NU));
   for (int32_t q = 0; q < NU; ++q) id.emplace(ip.node_names[size_t(q)], q);
@@ -925,6 +1038,75 @@ ScenarioTables scenario_tables(const InternedPlan& ip, const Scenario& sc, const
       t.weight[size_t(it->second)] = kv.second;
       t.has_weight[size_t(it->second)] = 1;
     }
+
+  if (sc.ModelStateConstraints) {
+    t.set |= BLANCE_OPT_CONSTRAINTS;
+    for (int32_t s = 0; s < S; ++s) t.constraints.push_back(scenario_constraint(model, options, sc, ip.state_names[size_t(s)]));
+  }
+  if (sc.StateStickiness) {
+    t.set |= BLANCE_OPT_STICKINESS;
+    t.stickiness.assign(size_t(S), 0);
+    t.has_stickiness.assign(size_t(S), 0);
+    if (*sc.StateStickiness)
+      for (int32_t s = 0; s < S; ++s) {
+        auto it = (*sc.StateStickiness)->find(ip.state_names[size_t(s)]);
+        if (it != (*sc.StateStickiness)->end()) { t.stickiness[size_t(s)] = it->second; t.has_stickiness[size_t(s)] = 1; }
+      }
+  }
+  if (sc.PartitionWeights) {
+    t.set |= BLANCE_OPT_PART_WEIGHTS;
+    const auto& pw = *sc.PartitionWeights;
+    t.has_part_weights = pw ? 1 : 0;
+    std::unordered_map<int32_t, int32_t> mine;      // the partitions of the maps this scenario weighs
+    if (pw) {
+      const auto& pid = parts.get();
+      for (const auto& kv : *pw) {
+        auto it = pid.find(kv.first);
+        if (it == pid.end()) continue;                 // names outside the maps are ignored, as InternPlan does
+        if (kv.second > 999999999)                     // the "%10d" rule of plan.go:539
+          throw BlanceError(BLANCE_ERR_UNSUPPORTED, "blance: " + who + "partition weight of '" + kv.first + "' is above 999999999");
+        mine.emplace(it->second, kv.second);
+      }
+      // overrides: partitions whose weight or presence differs from the base's (without weights the flags are unread)
+      std::vector<std::pair<int32_t, int32_t>> diff;   // (partition, weight); presence below
+      for (const auto& kv : mine)
+        if (!ip.part_has_weight[size_t(kv.first)] || ip.part_weight[size_t(kv.first)] != kv.second) diff.emplace_back(kv.first, kv.second);
+      for (int32_t p = 0; p < ip.in.n_parts; ++p)
+        if (ip.part_has_weight[size_t(p)] && !mine.count(p)) diff.emplace_back(p, 1);
+      std::sort(diff.begin(), diff.end());
+      for (const auto& d : diff) {
+        t.ow_part.push_back(d.first);
+        t.ow_weight.push_back(d.second);
+        t.ow_has.push_back(mine.count(d.first) ? 1 : 0);
+      }
+    }
+    // extra_tot_* (host_api.cpp's counts of non-model states) only change when such a partition changes its weight
+    auto w_base = [&](int32_t p) { return ip.in.has_part_weights && ip.part_has_weight[size_t(p)] ? ip.part_weight[size_t(p)] : 1; };
+    auto w_mine = [&](int32_t p) {
+      if (!pw) return 1;
+      auto it = mine.find(p);
+      return it == mine.end() ? 1 : it->second;
+    };
+    bool moved = false;
+    for (int32_t p : ip.extra_part) moved |= w_base(p) != w_mine(p);
+    if (moved) {
+      t.extra_first.assign(size_t(N), 0);
+      t.extra_rest.assign(size_t(N), 0);
+      for (size_t e = 0; e < ip.extra_part.size(); ++e) {
+        const int32_t p = ip.extra_part[e], q = ip.extra_node[e];
+        if (q >= N) continue;
+        t.extra_first[size_t(q)] = checked_i32((long long)t.extra_first[size_t(q)] + w_mine(p), "count");
+        if (!ip.part_in_assign[size_t(p)]) t.extra_rest[size_t(q)] = checked_i32((long long)t.extra_rest[size_t(q)] + w_mine(p), "count");
+      }
+    }
+  }
+  if (sc.NodeHierarchy || sc.HierarchyRules) {
+    t.set |= BLANCE_OPT_HIERARCHY;
+    const auto& rules = sc.HierarchyRules ? *sc.HierarchyRules : options.HierarchyRules;
+    const auto& parents = sc.NodeHierarchy ? *sc.NodeHierarchy : options.NodeHierarchy;
+    t.has_hier_rules = rules ? 1 : 0;
+    hierarchy_tables(ip.state_names, ip.node_names, id, N, rules, parents, &t.rule_off, &t.ie_mask, &t.n_rules, &t.n_hier_bits);
+  }
   return t;
 }
 
@@ -936,18 +1118,43 @@ std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const 
                                              size_t index) {
   if (index >= scenarios.size()) invalid("InternScenario: scenario index out of range");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
-  ScenarioTables t = scenario_tables(*ip, scenarios[index], options, index);
+  PartIndex parts{*ip, {}};
+  ScenarioTables t = scenario_tables(*ip, model, scenarios[index], options, index, parts);
   ip->node_removed = std::move(t.removed);
   ip->node_added = std::move(t.added);
   ip->node_weight = std::move(t.weight);
   ip->node_has_weight = std::move(t.has_weight);
   blance_plan_in& in = ip->in;
+  in.add_is_nil = t.add_is_nil;
+  in.has_node_weights = t.has_node_weights;
+  if (t.set & BLANCE_OPT_CONSTRAINTS) ip->state_constraints = t.constraints;
+  if (t.set & BLANCE_OPT_STICKINESS) { ip->state_stickiness = t.stickiness; ip->state_has_stickiness = t.has_stickiness; }
+  if (t.set & BLANCE_OPT_PART_WEIGHTS) {
+    in.has_part_weights = t.has_part_weights;
+    for (size_t j = 0; j < t.ow_part.size(); ++j) {
+      ip->part_weight[size_t(t.ow_part[j])] = t.ow_weight[j];
+      ip->part_has_weight[size_t(t.ow_part[j])] = t.ow_has[j];
+    }
+    if (!t.extra_first.empty()) { ip->extra_tot_first = t.extra_first; ip->extra_tot_rest = t.extra_rest; }
+  }
+  if (t.set & BLANCE_OPT_HIERARCHY) {
+    ip->rule_off = t.rule_off;
+    ip->ie_mask = t.ie_mask;
+    in.has_hier_rules = t.has_hier_rules; in.n_rules = t.n_rules; in.n_hier_bits = t.n_hier_bits;
+  }
   in.node_removed = ip->node_removed.data();
   in.node_added = ip->node_added.data();
   in.node_weight = ip->node_weight.data();
   in.node_has_weight = ip->node_has_weight.data();
-  in.add_is_nil = t.add_is_nil;
-  in.has_node_weights = t.has_node_weights;
+  in.state_constraints = ip->state_constraints.data();
+  in.state_stickiness = ip->state_stickiness.data();
+  in.state_has_stickiness = ip->state_has_stickiness.data();
+  in.part_weight = ip->part_weight.data();
+  in.part_has_weight = ip->part_has_weight.data();
+  in.extra_tot_first = ip->extra_tot_first.data();
+  in.extra_tot_rest = ip->extra_tot_rest.data();
+  in.rule_off = ip->rule_off.data();
+  in.ie_mask = ip->ie_mask.empty() ? nullptr : ip->ie_mask.data();
   return ip;
 }
 
@@ -958,8 +1165,9 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
   if (scenarios.empty()) invalid("PlanNextMapScenarios: no scenarios");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
   const size_t n = scenarios.size();
+  PartIndex parts{*ip, {}};
   std::vector<ScenarioTables> tabs(n);
-  for (size_t i = 0; i < n; ++i) tabs[i] = scenario_tables(*ip, scenarios[i], options, i);
+  for (size_t i = 0; i < n; ++i) tabs[i] = scenario_tables(*ip, model, scenarios[i], options, i, parts);
   std::vector<bool> want(n, false);
   for (int i : wantMaps) {
     if (i < 0 || size_t(i) >= n) invalid("PlanNextMapScenarios: wantMaps index " + std::to_string(i) + " out of range");
@@ -967,12 +1175,14 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
   }
   const int32_t NU = ip->in.n_node_ids, S = ip->in.n_states;
   std::vector<blance_scenario> sc(n);
+  std::vector<blance_scenario_opts> opts(n);
   std::vector<blance_scenario_out> out(n);
   std::vector<std::vector<int64_t>> ops(n, std::vector<int64_t>(size_t(NU) * 4 + 1)), load(n, std::vector<int64_t>(size_t(S) * size_t(NU) + 1));
   std::vector<std::unique_ptr<PlanOutBuffers>> maps(n);
   for (size_t i = 0; i < n; ++i) {
     sc[i] = blance_scenario{tabs[i].removed.data(), tabs[i].added.data(), tabs[i].add_is_nil, tabs[i].has_node_weights,
                             tabs[i].weight.data(), tabs[i].has_weight.data()};
+    opts[i] = scenario_opts(tabs[i]);
     out[i] = blance_scenario_out{};
     out[i].node_ops = ops[i].data();
     out[i].state_node_load = load[i].data();
@@ -984,7 +1194,8 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     }
   }
   blance_ctx* ctx = DefaultContext();
-  const int st = blance_plan_scenarios(ctx, &ip->in, int32_t(n), sc.data(), favorMinNodes ? 1 : 0, maxConcurrent, out.data());
+  const int st = blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                          out.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_scenarios failed: ") + blance_last_error(ctx));
   static const char* kOps[] = {"add", "del", "promote", "demote"};
   std::vector<ScenarioResult> res(n);
@@ -1003,7 +1214,8 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     if (want[i]) {
       r.HasMap = true;
       maps[i]->out.iters_run = o.iters_run;
-      if (o.iters_run > 0) r.NextMap = UninternPlan(*ip, *maps[i], &r.NextWarnings);   // MaxIterationsPerPlan <= 0: plan.go:32,57
+      const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
+      if (o.iters_run > 0) r.NextMap = unintern_plan(*ip, *maps[i], &r.NextWarnings, k);   // MaxIterationsPerPlan <= 0: plan.go:32,57
     }
   }
   return res;

@@ -93,11 +93,18 @@ PartitionMap PlanNextMapEx(PartitionMap& prevMap, PartitionMap& partitionsToAssi
                            Warnings* warnings, PlanStats* stats = nullptr);
 
 // ---- what-if scenarios of one cluster (blance_plan_scenarios) ----------------------------------------------------
+template <class T>
+using ScenarioOpt = std::optional<std::optional<T>>;   // outer nullopt: the options' value; inner nullopt: nil
+
 struct Scenario {
   OptStrs NodesToRemove;               // nullopt = nil
   OptStrs NodesToAdd;                  // nullopt = nil (plan.go:554)
-  // outer nullopt: the options' NodeWeights; inner nullopt: nil
-  std::optional<std::optional<std::unordered_map<std::string, int>>> NodeWeights;
+  ScenarioOpt<std::unordered_map<std::string, int>> NodeWeights;
+  ScenarioOpt<std::unordered_map<std::string, int>> ModelStateConstraints;
+  ScenarioOpt<std::unordered_map<std::string, int>> StateStickiness;
+  ScenarioOpt<std::unordered_map<std::string, int>> PartitionWeights;   // names outside the maps are ignored
+  ScenarioOpt<std::unordered_map<std::string, std::string>> NodeHierarchy;
+  ScenarioOpt<::blance::HierarchyRules> HierarchyRules;
 };
 
 struct ScenarioResult {
@@ -114,10 +121,13 @@ struct ScenarioResult {
 };
 
 // Scenario i is PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, NodesToRemove_i, NodesToAdd_i, model, options
-// with NodeWeights_i).  Unlike PlanNextMapEx (plan.go:49-52), the caller's maps are NOT mutated: a what-if has no
-// side effects.  The maps are interned once; a scenario the reference would panic on (plan.go:544) throws
-// BlanceError naming its index before any device work.  NextMap / NextWarnings are filled for the indices in
-// wantMaps; maxConcurrent as in blance_plan_scenarios.
+// with the scenario's NodeWeights, ModelStateConstraints, StateStickiness, PartitionWeights, NodeHierarchy and
+// HierarchyRules substituted where it sets them).  Unlike PlanNextMapEx (plan.go:49-52), the caller's maps are NOT
+// mutated: a what-if has no side effects.  The maps are interned once, each state's slot range as wide as the
+// largest constraint of any scenario; a scenario's partition weights travel as the per-partition difference to the
+// options' weights (blance_plan_scenarios_ex).  A scenario the reference would panic on (plan.go:544) or the device
+// cannot plan (constraints above 16) throws BlanceError naming its index before any device work.  NextMap /
+// NextWarnings are filled for the indices in wantMaps; maxConcurrent as in blance_plan_scenarios.
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
@@ -152,6 +162,7 @@ struct InternedPlan {
   std::vector<int32_t> prev_rows, cur_rows;
   std::vector<uint8_t> prev_shape, cur_shape;
   std::vector<int32_t> extra_tot_first, extra_tot_rest;
+  std::vector<int32_t> extra_part, extra_node;   // the prevMap entries under non-model states behind extra_tot_*
   std::vector<int32_t> rule_off;
   std::vector<uint32_t> ie_mask;
   blance_plan_in in{};    // points into the vectors above
@@ -173,7 +184,8 @@ struct PlanOutBuffers {
 PartitionMap UninternPlan(const InternedPlan& ip, const PlanOutBuffers& ob, Warnings* warnings);
 
 // The blance_plan_in of scenario `index` of PlanNextMapScenarios: the shared base tables with that scenario's node
-// fields substituted (so a CPU oracle can run on exactly the tables the device plans).
+// fields and plan options substituted, its weight overrides applied (so a CPU oracle can run on exactly the tables
+// the device plans).
 std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                              const Strs& nodesAll, const PartitionModel& model,
                                              const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,

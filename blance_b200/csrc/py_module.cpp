@@ -302,8 +302,12 @@ PYBIND11_MODULE(_host, m) {
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10,
       py::arg("engine") = 0);
 
-  // what-if scenarios: (nodes_to_remove, nodes_to_add, has_node_weights_key, node_weights) per scenario
-  using PyScenario = std::tuple<OptStrs, OptStrs, bool, std::optional<IntMap>>;
+  // what-if scenarios: (nodes_to_remove, nodes_to_add, then a (has_key, value) pair for each of node_weights,
+  // model_state_constraints, state_stickiness, partition_weights, node_hierarchy, hierarchy_rules) per scenario;
+  // has_key false inherits the options' value, a None value is nil
+  using PyScenario = std::tuple<OptStrs, OptStrs, bool, std::optional<IntMap>, bool, std::optional<IntMap>, bool,
+                                std::optional<IntMap>, bool, std::optional<IntMap>, bool, std::optional<StrMap>, bool,
+                                std::optional<PyRules>>;
   auto to_scenarios = [](const std::vector<PyScenario>& v) {
     std::vector<Scenario> out;
     for (const auto& t : v) {
@@ -311,6 +315,21 @@ PYBIND11_MODULE(_host, m) {
       s.NodesToRemove = std::get<0>(t);
       s.NodesToAdd = std::get<1>(t);
       if (std::get<2>(t)) s.NodeWeights = std::get<3>(t);
+      if (std::get<4>(t)) s.ModelStateConstraints = std::get<5>(t);
+      if (std::get<6>(t)) s.StateStickiness = std::get<7>(t);
+      if (std::get<8>(t)) s.PartitionWeights = std::get<9>(t);
+      if (std::get<10>(t)) s.NodeHierarchy = std::get<11>(t);
+      if (std::get<12>(t)) {
+        std::optional<HierarchyRules> rules;
+        if (const auto& hr = std::get<13>(t)) {
+          rules.emplace();
+          for (const auto& kv : *hr) {
+            auto& dst = (*rules)[kv.first];
+            for (const auto& r : kv.second) dst.push_back(HierarchyRule{r.first, r.second});
+          }
+        }
+        s.HierarchyRules = std::move(rules);
+      }
       out.push_back(std::move(s));
     }
     return out;

@@ -131,14 +131,85 @@ class ScenarioResult:
     warn_parts = property(lambda self: self.out.warn_parts)
 
 
-def scenario_tables(base, scenario):
-    """The PlanTables of one scenario: `base` with the scenario's node fields substituted (a shallow copy; the
-    partition arrays are shared).  A field missing from the scenario dict keeps the base's value."""
+def scenario_tables(base, scenario, opts=None):
+    """The PlanTables of one scenario: `base` with the scenario's node fields substituted and, when `opts` (a dict
+    of OPT_GROUPS keys) is given, its plan options: the PlanNextMapEx instance blance_plan_scenarios_ex plans.  A
+    field missing from the dicts keeps the base's value.  A shallow copy: the row tables are shared with `base`,
+    the weight arrays are copied when the scenario has weight overrides."""
     t = copy.copy(base)
     for f in SCENARIO_FIELDS:
         if f in scenario:
             setattr(t, f, scenario[f])
+    for f, v in (opts or {}).items():
+        if f not in _OPT_KEYS:
+            raise KeyError("unknown scenario option %r" % f)
+        if f == "weight_overrides":
+            part, weight, has = (np.asarray(a) for a in v)
+            t.part_weight = np.array(base.part_weight, np.int32)
+            t.part_has_weight = np.array(base.part_has_weight, np.uint8)
+            t.part_weight[part] = weight
+            t.part_has_weight[part] = has
+        elif v is not None:                  # (extra_tot_* None: the base's)
+            setattr(t, f, v)
     return t
+
+
+def widen_layout(t, widths):
+    """A copy of `t` whose state s has a slot range of at least widths[s] (the row tables re-laid out, padded with
+    NO_NODE): the shared layout of scenarios that raise a state's constraints."""
+    caps = np.maximum(np.diff(t.state_slot_off), np.asarray(widths, np.int64)).astype(np.int32)
+    off = np.concatenate([[0], np.cumsum(caps)]).astype(np.int32)
+    w = copy.copy(t)
+    w.state_slot_off, w.n_slots = off, int(off[-1])
+    for f in ("prev_rows", "cur_rows"):
+        old = np.asarray(getattr(t, f)).reshape(t.n_parts, t.n_slots)
+        new = np.full((t.n_parts, w.n_slots), NO_NODE, np.int32)
+        for s in range(t.n_states):
+            lo, hi = int(t.state_slot_off[s]), int(t.state_slot_off[s + 1])
+            new[:, off[s]:off[s] + hi - lo] = old[:, lo:hi]
+        setattr(w, f, new)
+    return w
+
+
+# blance_scenario_opts in dict form: the keys of each group (a group is set when any of its keys is given)
+OPT_GROUPS = {api.OPT_CONSTRAINTS: ("state_constraints",),
+              api.OPT_STICKINESS: ("state_stickiness", "state_has_stickiness"),
+              api.OPT_PART_WEIGHTS: ("has_part_weights", "weight_overrides", "extra_tot_first", "extra_tot_rest"),
+              api.OPT_HIERARCHY: ("has_hier_rules", "n_rules", "n_hier_bits", "rule_off", "ie_mask")}
+_OPT_KEYS = {k for keys in OPT_GROUPS.values() for k in keys}
+
+
+def _opts_struct(base, o, keep):
+    """blance_scenario_opts of one option dict (weight_overrides = (partitions, weights, presence))."""
+    s = api.ScenarioOpts()
+    for bit, keys in OPT_GROUPS.items():
+        if any(k in o for k in keys):
+            s.set |= bit
+
+    def ptr(v, dt):
+        a = np.ascontiguousarray(v, dtype=dt)
+        keep.append(a)
+        return a.ctypes.data if a.size else None
+    if s.set & api.OPT_CONSTRAINTS:
+        s.state_constraints = ptr(o["state_constraints"], np.int32)
+    if s.set & api.OPT_STICKINESS:
+        s.state_stickiness = ptr(o.get("state_stickiness", base.state_stickiness), np.int32)
+        s.state_has_stickiness = ptr(o.get("state_has_stickiness", base.state_has_stickiness), np.uint8)
+    if s.set & api.OPT_PART_WEIGHTS:
+        s.has_part_weights = int(o.get("has_part_weights", base.has_part_weights))
+        part, weight, has = o.get("weight_overrides", ((), (), ()))
+        s.n_weight_overrides = len(part)
+        s.ow_part, s.ow_weight, s.ow_has = ptr(part, np.int32), ptr(weight, np.int32), ptr(has, np.uint8)
+        for f in ("extra_tot_first", "extra_tot_rest"):
+            if o.get(f) is not None:
+                setattr(s, f, ptr(o[f], np.int32))
+    if s.set & api.OPT_HIERARCHY:
+        s.has_hier_rules = int(o.get("has_hier_rules", base.has_hier_rules))
+        s.n_rules = int(o.get("n_rules", base.n_rules))
+        s.n_hier_bits = int(o.get("n_hier_bits", base.n_hier_bits))
+        s.rule_off = ptr(o.get("rule_off", base.rule_off), np.int32)
+        s.ie_mask = ptr(o.get("ie_mask", base.ie_mask), np.uint32)
+    return s
 
 
 class Context:
@@ -180,10 +251,11 @@ class Context:
             r.out = o
         return results
 
-    def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=()):
+    def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None):
         """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
         (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
-        are copied out.  Returns one ScenarioResult per scenario."""
+        are copied out.  opts (None, or one dict of OPT_GROUPS keys per scenario) calls blance_plan_scenarios_ex
+        with those plan options.  Returns one ScenarioResult per scenario."""
         n = len(scenarios)
         want = set(want_rows)
         base = base_tables.struct()
@@ -200,8 +272,13 @@ class Context:
                 setattr(scs[i], f, a.ctypes.data if a.size else None)
         results = [ScenarioResult(base_tables, i in want) for i in range(n)]
         outs = (api.ScenarioOut * max(1, n))(*[r.out for r in results])
-        self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),
-                                                   int(max_concurrent), outs), "blance_plan_scenarios")
+        if opts is None:
+            self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),
+                                                       int(max_concurrent), outs), "blance_plan_scenarios")
+        else:
+            ops = (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
+            self._check(self.lib.blance_plan_scenarios_ex(self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)),
+                                                          int(max_concurrent), outs), "blance_plan_scenarios_ex")
         for r, o in zip(results, outs):
             r.out = o
         return results

@@ -231,6 +231,68 @@ typedef struct blance_scenario_out {
 int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                           int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out);
 
+/* Plan options of one scenario (blance_plan_scenarios_ex).  `set` says which groups replace the base's fields;
+ * a group whose bit is clear inherits the base and its fields are not read.  Arrays are [n_states] unless noted.
+ *
+ *   BLANCE_OPT_CONSTRAINTS   ModelStateConstraints (plan.go:308-319): state_constraints.  Every value must fit
+ *                            the base's slot range of that state (state_slot_off[s+1] - state_slot_off[s]), so all
+ *                            scenarios share the base's row layout.  A binding that lets a scenario raise a
+ *                            constraint widens the base's slot ranges up front to the largest constraint of any
+ *                            scenario (PlanNextMapScenarios does).
+ *   BLANCE_OPT_STICKINESS    StateStickiness: state_stickiness, state_has_stickiness.
+ *   BLANCE_OPT_PART_WEIGHTS  PartitionWeights: has_part_weights, and a sparse list of per-partition changes to the
+ *                            base's part_weight / part_has_weight: partition ow_part[j] (distinct, in [0, n_parts))
+ *                            gets weight ow_weight[j] and presence ow_has[j], each [n_weight_overrides].
+ *                            extra_tot_first / extra_tot_rest ([n_nodes], NULL = the base's) replace the counts of
+ *                            non-model states (see blance_plan_in): a caller that reweights a partition holding such
+ *                            entries must supply them, the device cannot derive them.
+ *   BLANCE_OPT_HIERARCHY     NodeHierarchy and HierarchyRules: has_hier_rules, n_rules, n_hier_bits, rule_off,
+ *                            ie_mask, with the meaning they have in blance_plan_in. */
+enum blance_scenario_opt_set {
+  BLANCE_OPT_CONSTRAINTS = 1,
+  BLANCE_OPT_STICKINESS = 2,
+  BLANCE_OPT_PART_WEIGHTS = 4,
+  BLANCE_OPT_HIERARCHY = 8
+};
+
+typedef struct blance_scenario_opts {
+  uint32_t set;                         /* OR of enum blance_scenario_opt_set */
+  const int32_t* state_constraints;     /* BLANCE_OPT_CONSTRAINTS */
+  const int32_t* state_stickiness;      /* BLANCE_OPT_STICKINESS */
+  const uint8_t* state_has_stickiness;
+  int32_t has_part_weights;             /* BLANCE_OPT_PART_WEIGHTS: 0 or 1 */
+  int32_t n_weight_overrides;
+  const int32_t* ow_part;
+  const int32_t* ow_weight;
+  const uint8_t* ow_has;                /* 0 or 1 */
+  const int32_t* extra_tot_first;       /* [n_nodes] or NULL */
+  const int32_t* extra_tot_rest;        /* [n_nodes] or NULL */
+  int32_t has_hier_rules;               /* BLANCE_OPT_HIERARCHY: 0 or 1 */
+  int32_t n_rules;
+  int32_t n_hier_bits;
+  const int32_t* rule_off;              /* [n_states+1] */
+  const uint32_t* ie_mask;              /* [n_rules][n_node_ids+1][hier_words] */
+} blance_scenario_opts;
+
+/* blance_plan_scenarios with plan options per scenario: scenario i is PlanNextMapEx(prevMap, partitionsToAssign,
+ * nodesAll, nodesToRemove_i, nodesToAdd_i, model, options_i), where options_i is the base's options with
+ * NodeWeights from sc[i] and the groups of opts[i] replaced.  Everything blance_plan_scenarios promises holds here
+ * on the substituted tables (rows, shapes, warnings, iters_run, converged and steps equal blance_plan_next_map;
+ * state_node_load weights by the scenario's own partition weights).  opts NULL: no options vary, exactly
+ * blance_plan_scenarios.  NodeScoreBooster, MaxIterationsPerPlan, nodesAll and the maps stay shared.
+ *
+ * Errors, all before any device work, naming the scenario's index: the substituted blance_plan_in fails the
+ * checks of blance_plan_next_map (e.g. constraints > 16 or beyond the slot range, rules x constraints > 32, a
+ * hierarchy universe above 4096 bits); an unknown bit in `set`; a flag that is neither 0 nor 1; an override index
+ * outside [0, n_parts) or listed twice; NULL override arrays (BLANCE_ERR_INVALID_ARG).  An override weight above
+ * 999999999 (plan.go:539) or a sum of |partition weight| x n_slots at or above 2^31 is BLANCE_ERR_UNSUPPORTED.
+ *
+ * Scheduling as blance_plan_scenarios; the automatic wave size is priced by the wave's largest scenario (its
+ * hierarchy masks), and the overrides are applied on the device after each wave is replicated from the base. */
+int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                             const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                             blance_scenario_out* out);
+
 /* Device-resident variant used by benchmarks and by callers that chain plans:
  * uploads `in` once and returns a handle; blance_plan_run() replays the whole
  * plan on the resident tables (inputs are restored on device before each run);

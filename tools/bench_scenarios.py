@@ -3,6 +3,11 @@ blance_plan_next_map, alternating in the same process, with sampled correctness 
 and writes it to --out.
 
     python tools/bench_scenarios.py [--ks 1,8,33,66,132] [--cfgs 4,3] [--out profiles/h100_scenarios.json]
+    python tools/bench_scenarios.py --sweep stickiness,replicas [--out profiles/h100_option_sweeps.json]
+
+--sweep plans option variants of the cfg 4 cluster instead (StateStickiness {0, 1, 2, 3, 5, 8}, or replicas
+{1, 2, 3, 4} on a base widened to 4 replica slots) through blance_plan_scenarios_ex, against the same variants one
+by one, and checks every variant's plan against its one-by-one plan.
 
 Clusters: synth.make_rebalance(4) (1 M partitions x 1 024 nodes) and synth.make_rebalance(3) (65 536 x 256 with
 zone and rack rules; its previous map is the fresh stage's plan).  Scenario j keeps the configuration's own
@@ -159,17 +164,73 @@ def run_cfg(ctx, cfg, ks, rng):
     return t, rows
 
 
+def option_variants(t, kind):
+    """The option sweeps of the 1 M x 1 024 cluster (blance_scenario_opts as dicts): StateStickiness of every state
+    in {0, 1, 2, 3, 5, 8}, or the replica count in {1, 2, 3, 4} on a base widened to 4 replica slots."""
+    S = t.n_states
+    if kind == "stickiness":
+        vals = [0, 1, 2, 3, 5, 8]
+        return t, [dict(state_stickiness=np.full(S, v, np.int32), state_has_stickiness=np.ones(S, np.uint8)) for v in vals], vals
+    vals = [1, 2, 3, 4]
+    w = tables.widen_layout(t, [int(t.state_constraints[0]), max(vals)])
+    return w, [dict(state_constraints=np.array([t.state_constraints[0], v], np.int32)) for v in vals], vals
+
+
+def run_option_sweep(ctx, kind):
+    """K option variants as one blance_plan_scenarios_ex call against the same variants planned one by one with
+    blance_plan_next_map, alternating (sweep, one by one, sweep).  Every variant's rows, warnings, iterations and
+    steps are compared with its one-by-one plan."""
+    t, opts, vals = option_variants(synth.make_rebalance(4), kind)
+    scs = [{} for _ in opts]
+    ctx.plan_scenarios(t, scs[:2], False, opts=opts[:2])               # warm-up of every kernel the sweep uses
+    ctx.plan_next_map(tables.scenario_tables(t, {}, opts[0]))
+
+    def sweep_once():
+        with CaptureStderr() as cap:
+            t0 = time.perf_counter()
+            res = ctx.plan_scenarios(t, scs, False, want_rows=range(len(scs)), opts=opts)
+            wall = time.perf_counter() - t0
+        return res, wall, parse_waves(cap.text)
+    res, wall_a, info = sweep_once()
+    t0 = time.perf_counter()
+    serial = [ctx.plan_next_map(tables.scenario_tables(t, {}, o)) for o in opts]
+    serial_s = time.perf_counter() - t0
+    _, wall_b, _ = sweep_once()
+    wall = min(wall_a, wall_b)
+    same = [bool(np.array_equal(r.next_rows, s.next_rows) and np.array_equal(r.warn, s.warn) and
+                 (r.iters_run, r.converged, r.steps) == (s.iters_run, s.converged, s.steps)) for r, s in zip(res, serial)]
+    variants = [dict(value=v, matches_one_by_one=ok, iterations=r.iters_run, steps=r.steps, sticky_steps=r.sticky_steps,
+                     sticky_share=round(r.sticky_steps / r.steps, 4) if r.steps else None, parts_moved=r.parts_moved,
+                     ops_total=r.ops_total, warn_parts=r.warn_parts, one_by_one_device_ms=round(s.device_ms, 3),
+                     one_by_one_pass_ms=round(s.pass_ms, 3)) for v, r, s, ok in zip(vals, res, serial, same)]
+    row = dict(sweep=kind, cfg=4, K=len(opts), n_slots=t.n_slots, sweep_s=[round(wall_a, 3), round(wall_b, 3)],
+               one_by_one_s=round(serial_s, 3), speedup=round(serial_s / wall, 3), correct=all(same),
+               variants=variants, **info)
+    print(json.dumps(row), flush=True)
+    return row
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ks", default="1,8,33,66,132")
     ap.add_argument("--cfgs", default="4,3")
     ap.add_argument("--wave-ks", default="33,66,132", help="explicit max_concurrent values tried on cfg 4 at the largest K")
+    ap.add_argument("--sweep", default=None, help="option sweeps instead of node failures: stickiness, replicas, or both (comma separated)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     ks = [int(x) for x in a.ks.split(",")]
     rng = np.random.default_rng(0)
     rec = dict(tool="tools/bench_scenarios.py", **gpu_info())
     ctx = tables.Context()
+    if a.sweep:
+        rec["option_sweeps"] = [run_option_sweep(ctx, kind) for kind in a.sweep.split(",")]
+        ctx.close()
+        print(json.dumps(rec))
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(rec, f, indent=1)
+        return
     rec["sm_count_note"] = "auto wave: free device memory, and at most sm_count / 2 above 768 nodes"
     rec["results"] = []
     for cfg in [int(x) for x in a.cfgs.split(",")]:
