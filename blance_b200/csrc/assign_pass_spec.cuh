@@ -89,6 +89,9 @@ struct SpecCtl {
   int32_t epoch, front, cmd_seq, cmd_op, cmd_arg, cmd_epoch;
   int32_t res_n, res_same;
   int32_t res_chosen[BL_K_MAX];
+#ifdef BLANCE_SPEC_TIMING
+  int32_t probe;                     // timing builds: a store that waits for the resolve's n2n values
+#endif
 };
 
 __host__ __device__ inline size_t spec_dyn_smem_bytes(int N, int SW) {
@@ -585,8 +588,15 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
   int seq = 0;
   uint8_t* srank = pool.srank + D.part_off;
   long long n_fast = 0, n_res = 0, n_mov = 0, n_team = 0, n_reb = 0, n_wait = 0, n_stale = 0;
-  long long cyc[6] = {0, 0, 0, 0, 0, 0}, tc = clock64();
+  long long cyc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tc = clock64();   // the slots of DInst::spec_cyc
   const long long t_begin = tc;
+#ifdef BLANCE_SPEC_TIMING
+  long long cyc_n2n = 0, n_pfo = 0;
+  int pf_next = -1;                        // the next step the last resolve's scan showed as not accepted
+#define SP_PF_LOST() do { pf_next = -1; } while (0)
+#else
+#define SP_PF_LOST() do { } while (0)
+#endif
 #ifdef BLANCE_SPEC_TIMING
 #define SP_T(ix) do { const long long n_ = clock64(); cyc[ix] += n_ - tc; tc = n_; } while (0)
 #else
@@ -644,7 +654,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
 
   team_cmd(SP_OP_REBUILD, 0);
   adopt_list();
-  SP_T(4);
+  SP_T(6);
 
   int i = 0;
   uint32_t cslot = 0, cgen = 0;
@@ -731,6 +741,18 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
     if (!have_i) { ++n_wait; if (run == 0) __nanosleep(100); SP_T(1); continue; }        // its scout has not got there yet
     if (__shfl_sync(0xFFFFFFFFu, (int)stale_l, run & 31)) ++n_stale;
     ++n_res;
+#ifdef BLANCE_SPEC_TIMING
+    {
+      // prefetch opportunities: the previous resolve's ballot already named this step as the next one not accepted,
+      // and no team operation ran in between
+      if (i == pf_next) ++n_pfo;
+      uint32_t ok_i = okm[0];
+#pragma unroll
+      for (int g = 1; g < SP_U; ++g) if ((run >> 5) == g) ok_i = okm[g];
+      const uint32_t rest = ~ok_i & ~((2u << (run & 31)) - 1u);
+      pf_next = rest ? i + (__ffs(rest) - 1) - (run & 31) : -1;
+    }
+#endif
     {
       const uint32_t slot_i = cslot * 32u + (uint32_t)(i & 31);
       const uint32_t rb = rec_a + slot_i * RECB;
@@ -772,6 +794,17 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
         int32_t gq[SP_LPL + 1];
 #pragma unroll
         for (int u = 0; u <= SP_LPL; ++u) gq[u] = (cnode[u] >= 0 && have_p) ? ld_relaxed_gpu(Gt + cnode[u]) : 0;
+#ifdef BLANCE_SPEC_TIMING
+        {
+          // the part of the L2 round trip that nothing overlaps (the forced wait moves the mirror loads below behind it)
+          const long long t0 = clock64();
+          int32_t sum = 0;
+#pragma unroll
+          for (int u = 0; u <= SP_LPL; ++u) sum += gq[u];
+          sts32v((uint32_t)__cvta_generic_to_shared(&ctl.probe), sum);
+          cyc_n2n += clock64() - t0;
+        }
+#endif
         bool cur_ok = true;
         {
           // branch-free over the columns: independent FP64 chains that the scheduler can interleave (a lone warp pays
@@ -794,6 +827,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
             ck[u] = cnode[u] >= 0 ? k : ~0ull;
           }
         }
+        SP_T(2);
         if (__all_sync(0xFFFFFFFFu, cur_ok)) {
           unsigned long long lastk = 0;
           uint32_t lastp = 0;
@@ -832,10 +866,11 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           same = resolved && hit_all && n_ch == n_cur && n_cur == K;
         }
       }
-      SP_T(2);
+      SP_T(3);
       if (!resolved) {
         // ---- the team evaluates the step (and rebuilds the list if a count changed) ----------------------------------
         ++n_team;
+        SP_PF_LOST();
         team_cmd(SP_OP_FULL, i);
         n_ch = *(volatile int32_t*)&ctl.res_n;
         same = *(volatile int32_t*)&ctl.res_same != 0;
@@ -848,7 +883,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           orec[K] = n_ch;
         }
         if (!same) { adopt_list(); publish_epoch(); ++n_mov; }
-        SP_T(4);
+        SP_T(6);
       } else {
         int32_t* orec = ostream + (size_t)i * REC;
         if (lane == 0) {
@@ -921,6 +956,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
             ins = (fl & NF_VALID) && lex_lt(nk, (uint32_t)x, ubk, ubp);
           }
           __syncwarp();
+          SP_T(4);
           // list: drop the touched nodes, take the ones that are (still) below ub into free places
 #pragma unroll
           for (int u = 0; u < SP_LPL; ++u)
@@ -954,14 +990,15 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           for (int u = 0; u < SP_LPL; ++u) occ += __popc(__ballot_sync(0xFFFFFFFFu, Ln[u] >= 0));
           if (occ < SP_LMIN && ubp != 0xFFFFFFFFu) {
             publish_epoch();
-            SP_T(3);
+            SP_T(5);
+            SP_PF_LOST();
             team_cmd(SP_OP_REBUILD, 0);                                 // reads the mirror only
             adopt_list();
-            SP_T(4);
+            SP_T(6);
           } else {
             recompute_b0();
             publish_epoch();
-            SP_T(3);
+            SP_T(5);
           }
         }
       }
@@ -982,10 +1019,15 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
       printf("[blance] spec pass state %d K %d: steps %d accepted %lld resolved %lld movers %lld team %lld rebuilds %lld stale %lld waits %lld\n",
              s, K, n_assign, n_fast, n_res, n_mov, n_team, n_reb, n_stale, n_wait);
 #endif
-    cyc[5] = clock64() - t_begin;
-    for (int x = 0; x < 6; ++x) D.spec_cyc[x] += cyc[x];
+    cyc[7] = clock64() - t_begin;
+    for (int x = 0; x < 8; ++x) D.spec_cyc[x] += cyc[x];
+#ifdef BLANCE_SPEC_TIMING
+    D.spec_cyc_n2n += cyc_n2n;
+    D.spec_pf_opp += n_pfo;
+#endif
   }
 #undef SP_T
+#undef SP_PF_LOST
 }
 
 }  // namespace blance_dev

@@ -204,8 +204,18 @@ __global__ void k_gather_stream(DPool pool, int s, long long n_parts_total) {
     dst[D.SLP + 6] = n_cur;
     dst[D.SLP + 7] = clean ? 1 : 0;
     pool.srank[g] = 0;
-    if (clean && n_cur == D.state_constraints[s]) atomicAdd(&pool.insts[pool.part_inst[g]].n_elig, 1);
-    if (clean && n_cur <= D.state_constraints[s]) atomicAdd(&pool.insts[pool.part_inst[g]].n_clean, 1);
+    // warp-aggregated per instance: one atomic per warp and counter instead of one per row.  Every row of an
+    // instance adds to the same two words, and 1 M same-address atomics serialise at L2 (1.7 ms per call on an
+    // H100 SXM; 0.2 ms aggregated).
+    const int inst = pool.part_inst[g];
+    const unsigned act = __activemask();
+    const unsigned peers = __match_any_sync(act, inst);
+    const int n_e = __popc(__ballot_sync(act, clean && n_cur == D.state_constraints[s]) & peers);
+    const int n_c = __popc(__ballot_sync(act, clean && n_cur <= D.state_constraints[s]) & peers);
+    if ((threadIdx.x & 31) == __ffs(peers) - 1) {
+      if (n_e) atomicAdd(&pool.insts[inst].n_elig, n_e);
+      if (n_c) atomicAdd(&pool.insts[inst].n_clean, n_c);
+    }
   }
 }
 

@@ -915,8 +915,12 @@ static int fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
       std::fprintf(stderr, "[blance] inst %d: steps %lld accepted %lld | resolved by the leader %lld (stale results %lld) movers %lld team %lld rebuilds %lld waits %lld\n",
                    i, fin[i].steps, fin[i].fast_steps, fin[i].spec_resolved, fin[i].spec_stale, fin[i].spec_movers, fin[i].spec_team,
                    fin[i].spec_rebuilds, fin[i].spec_waits),
-      std::fprintf(stderr, "[blance]   leader cycles (-DBLANCE_SPEC_TIMING builds): scans %lld | waits %lld | resolves %lld | mover updates %lld | team %lld | passes total %lld\n",
-                   fin[i].spec_cyc[0], fin[i].spec_cyc[1], fin[i].spec_cyc[2], fin[i].spec_cyc[3], fin[i].spec_cyc[4], fin[i].spec_cyc[5]);
+      std::fprintf(stderr, "[blance]   leader cycles (-DBLANCE_SPEC_TIMING builds): scans %lld | waits %lld | resolve loads+keys %lld | resolve picks %lld"
+                           " | mover mirror %lld | mover list+publish %lld | team %lld | passes total %lld\n",
+                   fin[i].spec_cyc[0], fin[i].spec_cyc[1], fin[i].spec_cyc[2], fin[i].spec_cyc[3], fin[i].spec_cyc[4], fin[i].spec_cyc[5],
+                   fin[i].spec_cyc[6], fin[i].spec_cyc[7]),
+      std::fprintf(stderr, "[blance]   of the resolve loads+keys: waiting for n2n %lld | resolves whose step the previous ballot named next %lld\n",
+                   fin[i].spec_cyc_n2n, fin[i].spec_pf_opp);
   for (int i = 0; i < n; ++i) {
     const DInst& D = pl->h_insts[i];
     blance_plan_out& o = outs[i];

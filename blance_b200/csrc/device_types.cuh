@@ -59,6 +59,8 @@ struct DInst {
   // counters of the speculative kernel (whole plan)
   long long spec_resolved, spec_movers, spec_team, spec_rebuilds, spec_waits, spec_stale;
   long long spec_cyc[8];   // leader cycles: scans | waits | resolve loads+keys | resolve picks | mover mirror | mover list+publish | team | passes
+  long long spec_cyc_n2n;  // of resolve loads+keys: the cycles spent waiting for the n2n values (timing builds)
+  long long spec_pf_opp;   // resolves whose step the previous resolve's ballot had shown as the next one not accepted (timing builds)
   long long spec_abort;    // the speculative kernel's watchdog fired (a bug: the plan is reported as failed)
   long long spec_round2;   // resolves that had to look at the second list column
   long long spec_cwait;    // resolves that had to wait for the committer (a pending commit shared their top node)
