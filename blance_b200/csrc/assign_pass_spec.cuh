@@ -555,7 +555,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
 #pragma unroll
               for (int t = 0; t < K; ++t)
                 if (t != q && lex_lt(key[t], (uint32_t)cn[t], key[q], (uint32_t)cn[q])) ++rank;
-              ranks |= (uint32_t)rank << (2 * q);
+              ranks = srank_pack<K>(ranks, q, rank);
               if (rank == K - 1) worst = q;
             }
             T = key[0];
@@ -721,8 +721,8 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
         for (int q = 0; q < K; ++q)
           if (have_p) red_add(Gp[g][q], 1);
         // the outcome of an accepted step is "its current nodes in (score, position) order": one byte (0x80 | the
-        // ranks) in a dense array - one coalesced store per 32 steps - that k_scatter_stream expands
-        srank[i + 32 * g + lane] = (uint8_t)(0x80u | (((uint32_t)r[g].z >> 13) & 0xFFu));
+        // ranks, sticky_rank.cuh) in a dense array - one coalesced store per 32 steps - that k_scatter_stream expands
+        srank[i + 32 * g + lane] = srank_byte((uint32_t)r[g].z >> 13);
       }
     }
     cslot += (uint32_t)((i & 31) + run) >> 5;                           // i moves on by up to SP_U chunks

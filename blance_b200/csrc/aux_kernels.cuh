@@ -9,6 +9,7 @@
 
 #include "blance_b200.h"
 #include "device_types.cuh"
+#include "sticky_rank.cuh"
 
 namespace blance_dev {
 
@@ -299,14 +300,19 @@ __global__ void k_scatter_stream(DPool pool, int s, long long n_parts_total) {
     const int32_t p = in[D.SLP + 3];
     const uint32_t meta = (uint32_t)in[D.SLP];
     const int lo_s = D.state_slot_off[s], hi_s = D.state_slot_off[s + 1];
-    // a step the speculative kernel accepted as sticky keeps its k current nodes, in (score, position) order:
-    // srank = 0x80 | rank of current node q in bits 2q..2q+1
+    // a step the speculative kernel accepted as sticky keeps its k <= 4 current nodes, in (score, position) order
+    // (the outcome byte: sticky_rank.cuh)
     const uint32_t sr = pool.srank[g];
+    const bool accepted = srank_accepted(sr);
     int32_t sticky_out[4];
-    if (sr & 0x80u)
-      for (int q = 0; q < k && q < 4; ++q) sticky_out[(sr >> (2 * q)) & 3u] = in[lo_s + q];
-    const int32_t* out = (sr & 0x80u) ? sticky_out : out_rec;
-    const int n_chosen = (sr & 0x80u) ? k : out_rec[k];
+    if (accepted) {
+      if (k == 1) srank_expand<1>(sr, in + lo_s, sticky_out);
+      else if (k == 2) srank_expand<2>(sr, in + lo_s, sticky_out);
+      else if (k == 3) srank_expand<3>(sr, in + lo_s, sticky_out);
+      else srank_expand<4>(sr, in + lo_s, sticky_out);
+    }
+    const int32_t* out = accepted ? sticky_out : out_rec;
+    const int n_chosen = accepted ? k : out_rec[k];
     int32_t* row = pool.rows + D.rows_off + (long long)p * D.SLP;
     uint32_t nmeta = meta;
     bool have_higher_key = false;

@@ -85,7 +85,7 @@ struct DPool {
   // speculative pass: n2n's deviation from the all-sticky hypothesis, the per-step hypothesis counts
   // (qstat[step][4]) and the (top, node) pair sort that produces them
   int32_t* n2n_dev; int32_t* qstat;
-  uint8_t* srank;          // [sum PU] per step: 0x80 | ranks of its current nodes when the step was accepted as sticky
+  uint8_t* srank;          // [sum PU] per step: 0x80 | ranks of its current nodes when the step was accepted as sticky (sticky_rank.cuh)
   unsigned long long* pair_keys; unsigned long long* pair_keys_alt;
   uint32_t* pair_vals; uint32_t* pair_vals_alt;
   DInst* insts;

@@ -9,6 +9,7 @@
 
 #include "blance_b200.h"
 #include "device_types.cuh"
+#include "sticky_rank.cuh"
 
 namespace blance_dev {
 

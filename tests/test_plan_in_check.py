@@ -94,6 +94,21 @@ def test_each_invariant_is_caught():
     assert st == UNSUPPORTED and "999999999" in why
 
 
+@pytest.mark.parametrize("k,n_rules,ok", [(8, 4, True), (16, 2, True), (11, 3, False), (1, 33, False)])
+def test_hierarchy_picks_per_step_at_most_32(k, n_rules, ok):
+    """rules x constraints of one state is the number of hierarchy picks a step makes: 32 fit, 33 are rejected."""
+    t = synth.PlanTables(64, 1, 16, [0], [k])
+    t.has_hier_rules = 1
+    t.rule_off, mask = synth.hierarchy_masks(64, (8, 8), {0: [(2, 1)] * n_rules}, 1)
+    t.n_rules = mask.shape[0]
+    t.ie_mask = mask.reshape(-1)
+    st, why = check_tables(t)
+    if ok:
+        assert (st, why) == (OK, "")
+    else:
+        assert st == UNSUPPORTED and "rules x constraints" in why
+
+
 def test_structure_errors_come_first_and_null_is_safe():
     assert abi.capi().blance_plan_in_check(None, None, 0) == INVALID
     t = synth.make_fresh(1)

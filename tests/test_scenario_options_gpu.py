@@ -116,6 +116,8 @@ def random_base(seed):
     N = int(rng.integers(8, 160))
     S = int(rng.integers(1, 4))
     k = [int(rng.integers(1, 4)) if s < 2 else int(rng.integers(0, 2)) for s in range(S)]
+    if np.random.default_rng([seed, 4]).random() < 0.25:   # k = 4 from a stream of its own: other seeds keep their instances
+        k[0] = 4
     while sum(k) + S > N - 2:
         k = [max(1, x - 1) if s == 0 else max(0, x - 1) for s, x in enumerate(k)]
     P = int(rng.integers(70, 2500))
@@ -159,9 +161,7 @@ def random_option(t, rng):
     o = {}
     if rng.random() < 0.5:
         width = np.diff(t.state_slot_off)
-        # at most 3: with 4 the sticky pass kernels disagree with the lock-step kernel even for a single
-        # blance_plan_next_map (test_constraints_of_4_plan_as_lockstep below)
-        o["state_constraints"] = np.array([int(rng.integers(max(0, int(t.state_constraints[s]) - 1), min(3, int(width[s])) + 1))
+        o["state_constraints"] = np.array([int(rng.integers(max(0, int(t.state_constraints[s]) - 1), min(4, int(width[s])) + 1))
                                            for s in range(S)], np.int32)
         o["state_constraints"][0] = max(1, o["state_constraints"][0])
     if rng.random() < 0.5:
@@ -304,8 +304,6 @@ def test_cfg4_reduced_option_sweep(ctx):
     assert res[-1].sticky_steps > 0 and res[-2].sticky_steps > 0
 
 
-@pytest.mark.xfail(reason="known defect: with constraints of 4 the auto engine's sticky pass kernels plan other rows "
-                          "than the lock-step kernel and the oracle, also in blance_plan_next_map", strict=False)
 def test_constraints_of_4_plan_as_lockstep(ctx):
     t = tables.scenario_tables(tables.widen_layout(synth.make_rebalance(4, P=16384), [1, 4]), {},
                                dict(state_constraints=np.array([1, 4], np.int32)))
