@@ -46,6 +46,11 @@ class _ScenarioOut(ctypes.Structure):  # struct blance_scenario_out
                 ("warn_parts", ctypes.c_int64)]
 
 
+class _ScheduleOut(ctypes.Structure):  # struct blance_schedule_out
+    _fields_ = [("rounds", ctypes.c_int32), ("moves_done", ctypes.c_int64), ("stuck_parts", ctypes.c_int64),
+                ("max_batch", ctypes.c_int32), ("device_ms", ctypes.c_float)]
+
+
 OPT_CONSTRAINTS, OPT_STICKINESS, OPT_PART_WEIGHTS, OPT_HIERARCHY = 1, 2, 4, 8   # enum blance_scenario_opt_set
 
 
@@ -61,7 +66,8 @@ class _ScenarioOpts(ctypes.Structure):  # struct blance_scenario_opts
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
            "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
-           "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available", "blance_moves_free")
+           "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
+           "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_free")
 
 
 def capi():
@@ -95,6 +101,8 @@ def capi():
         lib.blance_moves_create.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int64)]
         lib.blance_moves_fetch.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.blance_moves_available.argtypes = [vp, vp, vp, vp, vp, vp]
+        lib.blance_moves_schedule.argtypes = [vp, vp, i32, vp, vp]
+        lib.blance_moves_schedule_fetch.argtypes = [vp, vp, vp, vp]
         lib.blance_moves_free.argtypes = [vp, vp]
         lib.blance_moves_free.restype = None
         _CAPI = lib
@@ -106,3 +114,4 @@ PlanOut = _PlanOut
 Scenario = _Scenario
 ScenarioOpts = _ScenarioOpts
 ScenarioOut = _ScenarioOut
+ScheduleOut = _ScheduleOut

@@ -5,6 +5,8 @@
     PlanNextMap(..., modelStateConstraints, partitionWeights, stateStickiness, nodeWeights,
                 nodeHierarchy, hierarchyRules) -> (nextMap, warnings)   api.go:109-132 (deprecated wrapper)
     CalcPartitionMoves(states, begNodesByState, endNodesByState, favorMinNodes) -> [NodeStateOp]   moves.go:41-46
+    OrchestrateSchedule(model, options, nodesAll, begMap, endMap) -> rounds of AssignPartitionsFunc calls
+        (the lock-step model of OrchestrateMoves, orchestrate.go:240-591; include/blance_b200.h)
 
 A PartitionMap is {partitionName: {stateName: [nodeName, ...] | None}}; a
 PartitionModel is {stateName: (priority, constraints)}; HierarchyRules is
@@ -142,5 +144,25 @@ def CalcPartitionMovesMap(states, begMap, endMap, favorMinNodes):
     return {k: [NodeStateOp(*t) for t in v] for k, v in r.items()}
 
 
+@dataclasses.dataclass
+class OrchestratorOptions:         # orchestrate.go:112-118
+    MaxConcurrentPartitionMovesPerNode: int = 0
+    FavorMinNodes: bool = False
+
+
+AssignPartitionsCall = collections.namedtuple("AssignPartitionsCall", ["Node", "Partitions", "States", "Ops"])
+
+
+def OrchestrateSchedule(model, options, nodesAll, begMap, endMap):
+    """The rebalance OrchestrateMoves(model, options, nodesAll, begMap, endMap, ..., LowestWeightPartitionMoveForNode)
+    runs, under the lock-step model of blance_moves_schedule, computed on the device: one list per round of
+    AssignPartitionsCall(Node, Partitions, States, Ops) in node-id order (nodesAll first), each in pick order.  A
+    node outside nodesAll has no mover: a partition whose next move is on it never advances."""
+    o = options or OrchestratorOptions()
+    r = _host.OrchestrateSchedule({k: tuple(v) for k, v in model.items()}, int(o.MaxConcurrentPartitionMovesPerNode),
+                                  bool(o.FavorMinNodes), list(nodesAll), begMap, endMap)
+    return [[AssignPartitionsCall(*c) for c in rnd] for rnd in r]
+
+
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------
-from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401
+from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, ScheduleOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401

@@ -17,6 +17,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
+#include <cub/device/device_select.cuh>
 
 #include "assign_pass.cuh"
 #include "assign_pass_seq.cuh"
@@ -24,6 +25,7 @@
 #include "aux_kernels.cuh"
 #include "blance_b200.h"
 #include "device_types.cuh"
+#include "schedule.cuh"
 
 using namespace blance_dev;
 
@@ -1477,6 +1479,10 @@ struct blance_moves {
   uint32_t *d_key = nullptr, *d_key2 = nullptr; int32_t *d_val = nullptr, *d_val2 = nullptr;   // [n_parts]
   int32_t* d_ncnt = nullptr; int32_t* d_noff = nullptr; unsigned long long* d_nbest = nullptr; int32_t* d_best = nullptr;   // per node
   void* d_tmp = nullptr; size_t tmp_bytes = 0;
+  // the last blance_moves_schedule: round_off [rounds + 1] and sched_op [moves_done] in one allocation
+  char* sched = nullptr;
+  int32_t sched_rounds = -1;         // -1: no schedule yet
+  long long sched_moves = 0;
 };
 
 extern "C" int blance_moves_create(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,
@@ -1600,6 +1606,143 @@ extern "C" int blance_moves_available(blance_ctx* ctx, blance_moves* mv, const i
   return BLANCE_OK;
 }
 
+// The lock-step schedule (include/blance_b200.h, schedule.cuh).  Rounds are enqueued in blocks of kSchedBlock; the
+// host reads the done flag and the active count once per block and bounds the next block's launches by that count.
+static const int kSchedBlock = 64;
+
+extern "C" int blance_moves_schedule(blance_ctx* ctx, blance_moves* mv, int32_t max_concurrent_per_node,
+                                     const uint8_t* node_has_mover, blance_schedule_out* out) {
+  if (!ctx || !mv || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule: ctx, moves or out is NULL");
+  if (!ctx->children.empty()) {
+    blance_ctx* c0 = ctx->children[0];
+    const int st = blance_moves_schedule(c0, mv, max_concurrent_per_node, node_has_mover, out);
+    if (st != BLANCE_OK) ctx->err = c0->err;
+    return st;
+  }
+  std::memset(out, 0, sizeof *out);
+  std::lock_guard<std::mutex> g(ctx->mu);
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const int32_t P = mv->n_parts, NN = mv->n_node_ids;
+  const long long T = mv->total_ops;
+  const int32_t count = max_concurrent_per_node <= 0 ? 1 : max_concurrent_per_node;   // orchestrate.go:484-487
+  int bits = 1;                                       // keys 0 .. NN (NN = past the active entries)
+  while (bits < 32 && (1ull << bits) <= (unsigned long long)NN) ++bits;
+  const size_t Pz = (size_t)std::max(P, 1), NNz = (size_t)std::max(NN, 1);
+  size_t sort_tmp = 0, sel_tmp = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
+                                  (int32_t*)nullptr, std::max(P, 1), 0, bits, st);
+  cub::DeviceSelect::Flagged(nullptr, sel_tmp, (const int32_t*)nullptr, (const uint8_t*)nullptr, (int32_t*)nullptr,
+                             (int32_t*)nullptr, std::max(P, 1), st);
+  const size_t tmp_bytes = std::max(sort_tmp, sel_tmp) + 256;
+  SchedState* d_st = nullptr;
+  int32_t *cur = nullptr, *act = nullptr, *act2 = nullptr, *list = nullptr, *cnt = nullptr, *noff = nullptr, *boff = nullptr;
+  uint32_t *key = nullptr, *key2 = nullptr;
+  uint8_t *flags = nullptr, *wl = nullptr, *mover = nullptr;
+  void* tmp = nullptr;
+  struct Sl { void** p; size_t bytes; };
+  std::vector<Sl> sl = {{(void**)&d_st, sizeof(SchedState)}, {(void**)&cur, sizeof(int32_t) * Pz}, {(void**)&act, sizeof(int32_t) * Pz},
+                        {(void**)&act2, sizeof(int32_t) * Pz}, {(void**)&list, sizeof(int32_t) * Pz}, {(void**)&key, sizeof(uint32_t) * Pz},
+                        {(void**)&key2, sizeof(uint32_t) * Pz}, {(void**)&flags, Pz}, {(void**)&wl, Pz},
+                        {(void**)&cnt, sizeof(int32_t) * NNz}, {(void**)&noff, sizeof(int32_t) * (NNz + 1)},
+                        {(void**)&boff, sizeof(int32_t) * (NNz + 1)}, {(void**)&mover, NNz}, {&tmp, tmp_bytes}};
+  size_t total = 0;
+  for (auto& x : sl) total += align_up(x.bytes, 256);
+  char* arena = nullptr;
+  if (cudaMallocAsync((void**)&arena, total, st) != cudaSuccess) return fail(ctx, BLANCE_ERR_NOMEM, "blance_moves_schedule: device allocation failed");
+  { size_t off = 0; for (auto& x : sl) { *x.p = arena + off; off += align_up(x.bytes, 256); } }
+  // results: round_off [T + 2] (R <= T) and sched_op [T], kept in the handle
+  if (mv->sched) { cudaFreeAsync(mv->sched, st); mv->sched = nullptr; }
+  mv->sched_rounds = -1;
+  const size_t ro_bytes = align_up(sizeof(long long) * (size_t)(T + 2), 256);
+  if (cudaMallocAsync((void**)&mv->sched, ro_bytes + sizeof(long long) * (size_t)std::max(T, 1ll), st) != cudaSuccess) {
+    mv->sched = nullptr;
+    cudaFreeAsync(arena, st);
+    return fail(ctx, BLANCE_ERR_NOMEM, "blance_moves_schedule: device allocation failed");
+  }
+  long long* round_off = (long long*)mv->sched;
+  long long* sched_op = (long long*)(mv->sched + ro_bytes);
+  int rc = BLANCE_OK;
+  auto step = [&](cudaError_t e, const char* what) {
+    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+  };
+  SchedState h{};
+  step(cudaEventRecord(ctx->ev[0], st), "event");
+  if (node_has_mover) step(cudaMemcpyAsync(mover, node_has_mover, (size_t)NN, cudaMemcpyHostToDevice, st), "H2D");
+  else step(cudaMemsetAsync(mover, 1, NNz, st), "memset");
+  step(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * NNz, st), "memset");
+  k_sched_init<<<grid_for(ctx, P, 256), 256, 0, st>>>(P, cur, act2, round_off, d_st);
+  ctx->launches += 1;
+  int32_t a_bound = 0;
+  if (P > 0) {                                        // the first compaction: partitions with a pickable first move
+    k_sched_flags<<<grid_for(ctx, P, 256), 256, 0, st>>>(P, act2, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
+    ctx->launches += 1;
+    size_t tb = tmp_bytes;
+    step(cub::DeviceSelect::Flagged(tmp, tb, act2, flags, act, &d_st->A, P, st), "select");
+    step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
+    step(cudaStreamSynchronize(st), "sync");
+    a_bound = h.A;
+  }
+  step(cudaGetLastError(), "k_sched_init / k_sched_flags");
+  const int pick_grid = (int)std::min<long long>((NNz + SCHED_PICK_THREADS / 32 - 1) / (SCHED_PICK_THREADS / 32), (long long)ctx->sm_count * 16);
+  long long launched = 0;
+  while (rc == BLANCE_OK && a_bound > 0) {
+    if (launched > T + kSchedBlock) { rc = fail(ctx, BLANCE_ERR_CUDA, "blance_moves_schedule: the schedule did not end (internal error)"); break; }
+    for (int r = 0; r < kSchedBlock && rc == BLANCE_OK; ++r) {
+      const int g = grid_for(ctx, a_bound, 256);
+      k_sched_keys<<<g, 256, 0, st>>>(a_bound, act, mv->d_off, mv->d_node, cur, NN, key, cnt, d_st);
+      size_t tb = tmp_bytes;
+      step(cub::DeviceRadixSort::SortPairs(tmp, tb, key, key2, act, list, a_bound, 0, bits, st), "sort");
+      k_sched_scan<<<1, SCHED_SCAN_THREADS, 0, st>>>(NN, count, cnt, noff, boff, round_off, d_st);
+      k_sched_pick<<<pick_grid, SCHED_PICK_THREADS, 0, st>>>(NN, count, noff, boff, list, wl, mv->d_off, mv->d_kind, cur, sched_op, d_st);
+      k_sched_flags<<<g, 256, 0, st>>>(a_bound, act, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
+      tb = tmp_bytes;
+      step(cub::DeviceSelect::Flagged(tmp, tb, act, flags, act2, &d_st->A, a_bound, st), "select");
+      ctx->launches += 4;
+      std::swap(act, act2);
+      ++launched;
+    }
+    step(cudaGetLastError(), "schedule round kernels");
+    step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
+    step(cudaStreamSynchronize(st), "sync");
+    if (h.done) break;
+    a_bound = h.A;
+  }
+  long long moves_done = 0;
+  step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
+  step(cudaStreamSynchronize(st), "sync");
+  if (rc == BLANCE_OK) step(cudaMemcpyAsync(&moves_done, round_off + h.rounds, sizeof moves_done, cudaMemcpyDeviceToHost, st), "D2H");
+  step(cudaEventRecord(ctx->ev[1], st), "event");
+  cudaFreeAsync(arena, st);
+  step(cudaStreamSynchronize(st), "sync");
+  if (rc != BLANCE_OK) return rc;
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
+  mv->sched_rounds = h.rounds;
+  mv->sched_moves = moves_done;
+  out->rounds = h.rounds;
+  out->moves_done = moves_done;
+  out->stuck_parts = (int64_t)h.stuck;
+  out->max_batch = h.max_batch;
+  out->device_ms = ms;
+  return BLANCE_OK;
+}
+
+extern "C" int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* mv, int64_t* round_off, int64_t* sched_op) {
+  if (!ctx || !mv) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: ctx or moves is NULL");
+  if (!ctx->children.empty()) ctx = ctx->children[0];
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (mv->sched_rounds < 0 || !mv->sched) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: no schedule was computed on this handle");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t ro_bytes = align_up(sizeof(long long) * (size_t)(mv->total_ops + 2), 256);
+  if (round_off) CK(cudaMemcpyAsync(round_off, mv->sched, sizeof(long long) * ((size_t)mv->sched_rounds + 1), cudaMemcpyDeviceToHost, st));
+  if (sched_op && mv->sched_moves > 0)
+    CK(cudaMemcpyAsync(sched_op, mv->sched + ro_bytes, sizeof(long long) * (size_t)mv->sched_moves, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return BLANCE_OK;
+}
+
 extern "C" void blance_moves_free(blance_ctx* ctx, blance_moves* mv) {
   if (!mv) return;
   if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
@@ -1607,7 +1750,11 @@ extern "C" void blance_moves_free(blance_ctx* ctx, blance_moves* mv) {
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaSetDevice(ctx->device);
     if (mv->arena) cudaFreeAsync(mv->arena, ctx->stream);
+    if (mv->sched) cudaFreeAsync(mv->sched, ctx->stream);
     cudaStreamSynchronize(ctx->stream);
-  } else if (mv->arena) cudaFree(mv->arena);
+  } else {
+    if (mv->arena) cudaFree(mv->arena);
+    if (mv->sched) cudaFree(mv->sched);
+  }
   delete mv;
 }

@@ -3,6 +3,7 @@
 #include "host_api.hpp"
 
 #include <algorithm>
+#include <functional>
 #include <chrono>
 #include <atomic>
 #include <cstdio>
@@ -1322,6 +1323,60 @@ std::unordered_map<std::string, std::vector<NodeStateOp>> CalcPartitionMovesMap(
   auto ops = run_moves(t, names.size(), favorMinNodes);
   std::unordered_map<std::string, std::vector<NodeStateOp>> out;
   for (size_t p = 0; p < names.size(); ++p) out.emplace(names[p], std::move(ops[p]));
+  return out;
+}
+
+std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const PartitionModel& model, const OrchestratorOptions& options,
+                                                                   const Strs& nodesAll, const PartitionMap& begMap,
+                                                                   const PartitionMap& endMap) {
+  if (begMap.size() != endMap.size()) throw BlanceError(BLANCE_ERR_INVALID_ARG, "mismatched begMap and endMap");   // orchestrate.go:250-252
+  const Strs states = sort_state_names(model);
+  Strs names;                                        // orchestrate.go:273: the partitions of begMap
+  for (const auto& kv : begMap) names.push_back(kv.first);
+  std::sort(names.begin(), names.end());
+  std::vector<const NodesByState*> begs, ends;
+  for (const auto& n : names) {
+    begs.push_back(&begMap.at(n).NodesByState);
+    auto e = endMap.find(n);
+    ends.push_back(e == endMap.end() ? nullptr : &e->second.NodesByState);
+  }
+  MovesTables t;
+  for (const auto& n : nodesAll) t.nodes.get(n);     // node ids: nodesAll first, so exactly they have a mover
+  const size_t n_movers = t.nodes.names.size();
+  intern_moves(states, begs, ends, &t);
+  const int32_t P = int32_t(names.size()), S = int32_t(t.state_names.size()), NN = int32_t(t.nodes.names.size());
+  std::vector<uint8_t> mover(size_t(NN) + 1, 0);
+  for (size_t i = 0; i < n_movers; ++i) mover[i] = 1;
+  blance_ctx* ctx = DefaultContext();
+  auto check = [&](int st, const char* what) {
+    if (st != BLANCE_OK) throw BlanceError(st, std::string(what) + " failed: " + blance_last_error(ctx));
+  };
+  blance_moves* h = nullptr;
+  int64_t total = 0;
+  check(blance_moves_create(ctx, P, S, t.n_visit, t.slot_off.data(), t.beg_rows.data(), t.end_rows.data(),
+                            options.FavorMinNodes ? 1 : 0, NN, &h, &total), "blance_moves_create");
+  std::unique_ptr<blance_moves, std::function<void(blance_moves*)>> guard(h, [ctx](blance_moves* m) { blance_moves_free(ctx, m); });
+  blance_schedule_out so{};
+  check(blance_moves_schedule(ctx, h, options.MaxConcurrentPartitionMovesPerNode, mover.data(), &so), "blance_moves_schedule");
+  std::vector<int64_t> round_off(size_t(so.rounds) + 1), sched(size_t(std::max<int64_t>(so.moves_done, 1)));
+  check(blance_moves_schedule_fetch(ctx, h, round_off.data(), sched.data()), "blance_moves_schedule_fetch");
+  std::vector<int64_t> op_off(size_t(P) + 1);
+  std::vector<int32_t> op_node(size_t(std::max<int64_t>(total, 1)));
+  std::vector<uint8_t> op_state(op_node.size()), op_kind(op_node.size());
+  check(blance_moves_fetch(ctx, h, op_off.data(), op_node.data(), op_state.data(), op_kind.data()), "blance_moves_fetch");
+  static const char* kOps[] = {"add", "del", "promote", "demote"};
+  std::vector<std::vector<AssignPartitionsCall>> out(size_t(so.rounds));
+  for (size_t r = 0; r < out.size(); ++r)
+    for (int64_t i = round_off[r]; i < round_off[r + 1]; ++i) {
+      const int64_t o = sched[size_t(i)];
+      const size_t p = size_t(std::upper_bound(op_off.begin(), op_off.end(), o) - op_off.begin()) - 1;
+      const auto& node = t.nodes.names[size_t(op_node[size_t(o)])];
+      if (out[r].empty() || out[r].back().Node != node) out[r].push_back(AssignPartitionsCall{node, {}, {}, {}});
+      auto& call = out[r].back();
+      call.Partitions.push_back(names[p]);
+      call.States.push_back(op_state[size_t(o)] == BLANCE_OP_STATE_NONE ? std::string() : t.state_names[op_state[size_t(o)]]);
+      call.Ops.push_back(kOps[op_kind[size_t(o)]]);
+    }
   return out;
 }
 

@@ -143,6 +143,27 @@ std::vector<NodeStateOp> CalcPartitionMoves(const Strs& states, const NodesBySta
 std::unordered_map<std::string, std::vector<NodeStateOp>> CalcPartitionMovesMap(
     const Strs& states, const PartitionMap& beg, const PartitionMap& end, bool favorMinNodes);
 
+struct OrchestratorOptions {           // orchestrate.go:112-118
+  int MaxConcurrentPartitionMovesPerNode = 0;
+  bool FavorMinNodes = false;
+};
+
+struct AssignPartitionsCall {          // the arguments of one AssignPartitionsFunc call (orchestrate.go:96-100)
+  std::string Node;
+  Strs Partitions, States, Ops;
+};
+
+// The rebalance OrchestrateMoves(model, options, nodesAll, begMap, endMap, assign, LowestWeightPartitionMoveForNode)
+// would run, under the lock-step model of blance_moves_schedule (include/blance_b200.h), computed on the device in
+// one call: result[r] lists round r's AssignPartitionsFunc calls in node-id order (nodesAll first, then the other
+// nodes in first-appearance order), each with its partitions, states and ops in pick order.  Partitions are
+// begMap's keys indexed in byte order of their names; move lists are CalcPartitionMoves(sortStateNames(model), ...)
+// as orchestrate.go:273-287 seeds them; a node outside nodesAll has no mover, so a partition whose next move is on
+// it never advances.  len(begMap) != len(endMap) throws BlanceError with OrchestrateMoves' message.
+std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const PartitionModel& model, const OrchestratorOptions& options,
+                                                                   const Strs& nodesAll, const PartitionMap& begMap,
+                                                                   const PartitionMap& endMap);
+
 // ---------------------------------------------------------------------------------
 // The interning layer, exposed so that tests can drive the SAME tables through the
 // CPU oracle and compare array for array.

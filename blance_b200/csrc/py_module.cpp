@@ -230,6 +230,23 @@ PYBIND11_MODULE(_host, m) {
     return out;
   });
 
+  m.def("OrchestrateSchedule", [](const PyModel& model, int max_concurrent, bool favor, const Strs& nodes_all,
+                                  const PyPartitionMap& beg, const PyPartitionMap& end) {
+    OrchestratorOptions o;
+    o.MaxConcurrentPartitionMovesPerNode = max_concurrent;
+    o.FavorMinNodes = favor;
+    const PartitionMap b = to_map(beg), e = to_map(end);
+    std::vector<std::vector<AssignPartitionsCall>> rounds;
+    {
+      py::gil_scoped_release rel;
+      rounds = OrchestrateSchedule(to_model(model), o, nodes_all, b, e);
+    }
+    std::vector<std::vector<std::tuple<std::string, Strs, Strs, Strs>>> out(rounds.size());
+    for (size_t r = 0; r < rounds.size(); ++r)
+      for (auto& c : rounds[r]) out[r].emplace_back(c.Node, c.Partitions, c.States, c.Ops);
+    return out;
+  });
+
   py::class_<PyInterned>(m, "InternedPlan")
       .def_property_readonly("in_ptr", [](const PyInterned& s) { return (uintptr_t)&s.ip->in; })
       .def_property_readonly("n_nodes", [](const PyInterned& s) { return s.ip->in.n_nodes; })

@@ -372,6 +372,24 @@ class Context:
                     "blance_moves_available")
         return node_off, node_parts[:node_off[-1]], best[:n_node_ids]
 
+    def moves_schedule(self, handle, max_concurrent, node_has_mover=None):
+        """blance_moves_schedule + blance_moves_schedule_fetch: the lock-step schedule of the handle's move lists
+        (include/blance_b200.h).  Returns (round_off [R+1], sched_op [moves_done], scalars) with scalars a dict of
+        rounds, moves_done, stuck_parts, max_batch and device_ms."""
+        h, _, n_node_ids = handle
+        mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
+        if mover is not None and mover.size != n_node_ids:
+            raise ValueError("node_has_mover must have n_node_ids = %d entries" % n_node_ids)
+        out = api.ScheduleOut()
+        self._check(self.lib.blance_moves_schedule(self.ptr, h, int(max_concurrent), None if mover is None else mover.ctypes.data,
+                                                   ctypes.byref(out)), "blance_moves_schedule")
+        round_off = np.zeros(out.rounds + 1, np.int64)
+        sched_op = np.zeros(max(1, out.moves_done), np.int64)
+        self._check(self.lib.blance_moves_schedule_fetch(self.ptr, h, round_off.ctypes.data, sched_op.ctypes.data),
+                    "blance_moves_schedule_fetch")
+        scalars = {f: getattr(out, f) for f, _ in api.ScheduleOut._fields_}
+        return round_off, sched_op[:out.moves_done], scalars
+
     def moves_free(self, handle):
         self.lib.blance_moves_free(self.ptr, handle[0])
 

@@ -347,6 +347,48 @@ int blance_moves_fetch(blance_ctx* ctx, blance_moves* moves, int64_t* op_off, in
  * when the node has no available move.  Any output pointer may be NULL. */
 int blance_moves_available(blance_ctx* ctx, blance_moves* moves, const int32_t* next, int32_t* node_off,
                            int32_t* node_parts, int32_t* best_part);
+
+/* ---- the orchestrator's whole schedule (orchestrate.go:482-504, 509-591, 749-763, 177-186) -----------------
+ * The Go orchestrator is goroutines and callbacks; Go's map order and its select between broadcastStopCh and
+ * nextDoneCh make every run's interleaving nondeterministic.  blance_moves_schedule() does not reproduce one run:
+ * it computes the schedule of a LOCK-STEP MODEL of the same statements:
+ *   1. every cursor starts at 0 (NextMoves.Next);
+ *   2. a round begins with findAvailableMovesUnlocked: every partition with next < len(moves) is appended to the
+ *      list of moves[next].Node, walking partitions in ASCENDING INDEX (the order of blance_moves_available);
+ *   3. for every node with a non-empty list, in ascending node id, filterNextPlausibleMovesForNode runs as
+ *      orchestrate.go:482-504: count = max(1, max_concurrent_per_node), capped at the list length; each pick is
+ *      LowestWeightPartitionMoveForNode - the FIRST index of minimal MoveOpWeight {promote 1, demote 2, add 3,
+ *      del 4} over the array as it stands - and the picked entry is replaced by the last one, the array shrinking
+ *      by one.  The picks, in pick order, are the node's batch (one AssignPartitionsFunc call);
+ *   4. every batch of the round completes before the next round (no errors, pause or stop); each picked
+ *      partition's cursor advances by one;
+ *   5. a move on a node without a mover (node_has_mover[n] == 0, or a node id outside [0, n_node_ids)) is never
+ *      picked: the reference would send on a nil channel and hang.  That partition never advances; the schedule
+ *      ends when no pickable move is left and stuck_parts counts the partitions left behind.
+ * FindMoveFunc is always LowestWeightPartitionMoveForNode and MoveOpWeight keeps its default values: Go func values
+ * and package variables cannot cross the ABI (the same policy as NodeScoreBooster).
+ *
+ * Result: R rounds; round_off[R+1] (int64, round_off[0] = 0) and sched_op[moves_done]: global op indices into the
+ * CSR arrays of blance_moves_fetch, ordered by round, then node id, then pick order.  Round r's ops are
+ * sched_op[round_off[r] .. round_off[r+1]); node, state and kind of each come from blance_moves_fetch.
+ *
+ * blance_moves_schedule computes the schedule on the device in one call (the host waits for the device once per
+ * 64 rounds) and keeps it in the handle until the next blance_moves_schedule or blance_moves_free;
+ * blance_moves_schedule_fetch copies it out (round_off: R+1 entries, sched_op: moves_done entries; either may be
+ * NULL).  Scratch is allocated and freed inside the call; blance_moves_available is not affected.  Repeated calls
+ * give identical results.  node_has_mover: [n_node_ids], NULL = every id has a mover.  Errors: NULL ctx, handle or
+ * out (BLANCE_ERR_INVALID_ARG); fetch before any schedule (BLANCE_ERR_INVALID_ARG). */
+typedef struct blance_schedule_out {
+  int32_t rounds;        /* R */
+  int64_t moves_done;    /* ops scheduled = length of sched_op = round_off[R] */
+  int64_t stuck_parts;   /* partitions whose next move is on a node without a mover */
+  int32_t max_batch;     /* largest batch of one node in one round */
+  float device_ms;       /* CUDA events around the whole call */
+} blance_schedule_out;
+
+int blance_moves_schedule(blance_ctx* ctx, blance_moves* moves, int32_t max_concurrent_per_node,
+                          const uint8_t* node_has_mover, blance_schedule_out* out);
+int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* moves, int64_t* round_off, int64_t* sched_op);
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
 #ifdef __cplusplus

@@ -676,4 +676,70 @@ func (m *movesB200) availableMovesB200(next map[string]int) (byNode map[string][
 	return byNode, best
 }
 
+// assignCallB200 holds the arguments of one AssignPartitionsFunc call of a scheduled round.
+type assignCallB200 struct {
+	Node                      string
+	Partitions, States, Ops []string
+}
+
+// scheduleB200 computes the whole rebalance the orchestrator would run (orchestrate.go:482-504, 509-591, 749-763,
+// 177-186) under the lock-step model of blance_moves_schedule (include/blance_b200.h): rounds[r] lists round r's
+// AssignPartitionsFunc calls in node-id order, each in pick order.  A node outside nodesAll has no mover, so a
+// partition whose next move is on it never advances.  states must be the list seedNextMovesB200 was given.
+// UNTESTED GO; the C ABI underneath is covered by tests/test_schedule_gpu.py.
+func (m *movesB200) scheduleB200(maxConcurrent int, nodesAll, states []string) ([][]assignCallB200, error) {
+	inAll := map[string]bool{}
+	for _, n := range nodesAll {
+		inAll[n] = true
+	}
+	mover := make([]C.uint8_t, m.nNodeIDs+1)
+	for i, n := range m.nodeNames {
+		if inAll[n] {
+			mover[i] = 1
+		}
+	}
+	var so C.blance_schedule_out
+	if st := C.blance_moves_schedule(b200(), m.h, C.int32_t(maxConcurrent), &mover[0], &so); st != C.BLANCE_OK {
+		return nil, fmt.Errorf("blance_moves_schedule: %d", int(st))
+	}
+	roundOff := make([]C.int64_t, int(so.rounds)+1)
+	sched := make([]C.int64_t, int(so.moves_done)+1)
+	if st := C.blance_moves_schedule_fetch(b200(), m.h, &roundOff[0], &sched[0]); st != C.BLANCE_OK {
+		return nil, fmt.Errorf("blance_moves_schedule_fetch: %d", int(st))
+	}
+	P := len(m.partNames)
+	opOff := make([]C.int64_t, P+1)
+	if st := C.blance_moves_fetch(b200(), m.h, &opOff[0], nil, nil, nil); st != C.BLANCE_OK {
+		return nil, fmt.Errorf("blance_moves_fetch: %d", int(st))
+	}
+	total := int(opOff[P])
+	opNode := make([]C.int32_t, total+1)
+	opState := make([]C.uint8_t, total+1)
+	opKind := make([]C.uint8_t, total+1)
+	if st := C.blance_moves_fetch(b200(), m.h, &opOff[0], &opNode[0], &opState[0], &opKind[0]); st != C.BLANCE_OK {
+		return nil, fmt.Errorf("blance_moves_fetch: %d", int(st))
+	}
+	kinds := [...]string{"add", "del", "promote", "demote"}
+	rounds := make([][]assignCallB200, int(so.rounds))
+	for r := range rounds {
+		for i := roundOff[r]; i < roundOff[r+1]; i++ {
+			o := sched[i]
+			p := sort.Search(P, func(q int) bool { return opOff[q+1] > o })
+			node := m.nodeNames[opNode[o]]
+			if len(rounds[r]) == 0 || rounds[r][len(rounds[r])-1].Node != node {
+				rounds[r] = append(rounds[r], assignCallB200{Node: node})
+			}
+			c := &rounds[r][len(rounds[r])-1]
+			st := ""
+			if opState[o] != C.BLANCE_OP_STATE_NONE {
+				st = states[opState[o]]
+			}
+			c.Partitions = append(c.Partitions, m.partNames[p])
+			c.States = append(c.States, st)
+			c.Ops = append(c.Ops, kinds[opKind[o]])
+		}
+	}
+	return rounds, nil
+}
+
 func (m *movesB200) free() { C.blance_moves_free(b200(), m.h) }
