@@ -51,6 +51,12 @@ class _ScheduleOut(ctypes.Structure):  # struct blance_schedule_out
                 ("max_batch", ctypes.c_int32), ("device_ms", ctypes.c_float)]
 
 
+class _ScenarioScheduleOut(ctypes.Structure):  # struct blance_scenario_schedule_out
+    _fields_ = [("rounds", ctypes.c_int32), ("moves_done", ctypes.c_int64), ("stuck_parts", ctypes.c_int64),
+                ("max_batch", ctypes.c_int32), ("node_rounds", ctypes.c_void_p), ("node_last_round", ctypes.c_void_p),
+                ("part_done_round", ctypes.c_void_p)]
+
+
 OPT_CONSTRAINTS, OPT_STICKINESS, OPT_PART_WEIGHTS, OPT_HIERARCHY = 1, 2, 4, 8   # enum blance_scenario_opt_set
 
 
@@ -65,7 +71,7 @@ class _ScenarioOpts(ctypes.Structure):  # struct blance_scenario_opts
 
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
            "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_free")
 
@@ -90,6 +96,7 @@ def capi():
         lib.blance_plan_next_map_batch.argtypes = [vp, i32, vp, vp]
         lib.blance_plan_scenarios.argtypes = [vp, vp, i32, vp, i32, i32, vp]
         lib.blance_plan_scenarios_ex.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp]
+        lib.blance_plan_scenarios_schedule.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
         lib.blance_plan_run.argtypes = [vp, vp]
         lib.blance_plan_fetch.argtypes = [vp, vp, vp]
@@ -115,3 +122,4 @@ Scenario = _Scenario
 ScenarioOpts = _ScenarioOpts
 ScenarioOut = _ScenarioOut
 ScheduleOut = _ScheduleOut
+ScenarioScheduleOut = _ScenarioScheduleOut

@@ -105,7 +105,7 @@ def _option_kwargs(o):
 
 
 def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=None, scenarios=(), favorMinNodes=False,
-                         wantMaps=(), maxConcurrent=0):
+                         wantMaps=(), maxConcurrent=0, scheduleConcurrency=()):
     """What-if variants of one cluster, planned side by side on the device.  Scenario i is
     PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, sc["nodesToRemove"], sc["nodesToAdd"], model, options with
     the scenario's plan options substituted): both node-set keys are required (None = nil).  The optional keys
@@ -115,12 +115,20 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
 
     Returns one dict per scenario: iterations, converged, steps, sticky_steps, parts_moved, ops_total, warn_parts,
     node_ops {node: {op: count}} and state_node_load {state: {node: load}} (nonzero entries only), plus next_map and
-    warnings for the indices in wantMaps."""
+    warnings for the indices in wantMaps.
+
+    scheduleConcurrency (a list of MaxConcurrentPartitionMovesPerNode values) adds a "schedules" list to every dict:
+    the lock-step rebalance schedule of OrchestrateSchedule over the moves node_ops counts, one dict per value with
+    MaxConcurrentPartitionMovesPerNode, Rounds, MovesDone, StuckParts, MaxBatch, and NodeRounds / NodeLastRound
+    {node: rounds with a batch / 1 + the last such round} (nonzero entries only).  The movers are the nodesAll names.
+    Partitions are walked in interning order (the name rule of plan.go:519-528) where OrchestrateSchedule walks them in
+    byte order: both are valid instances of Go's map order and agree whenever the names sort the same under both."""
     o = options or PlanNextMapOptions()
     same = prevMap is partitionsToAssign
     return _host.PlanNextMapScenarios(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                       {k: tuple(v) for k, v in model.items()}, _scenario_tuples(scenarios),
-                                      bool(favorMinNodes), [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o))
+                                      bool(favorMinNodes), [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o),
+                                      schedule_concurrency=[int(c) for c in scheduleConcurrency])
 
 
 def intern_scenario(prevMap, partitionsToAssign, nodesAll, model, options, scenarios, index):
@@ -165,4 +173,4 @@ def OrchestrateSchedule(model, options, nodesAll, begMap, endMap):
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------
-from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, ScheduleOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401
+from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, ScenarioScheduleOut, ScheduleOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401

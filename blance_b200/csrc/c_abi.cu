@@ -15,6 +15,7 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
 #include <cub/device/device_select.cuh>
@@ -26,6 +27,7 @@
 #include "blance_b200.h"
 #include "device_types.cuh"
 #include "schedule.cuh"
+#include "wave_schedule.cuh"
 
 using namespace blance_dev;
 
@@ -1113,18 +1115,76 @@ static long long summary_stride(const blance_plan_in& base) {
   return 4ll * base.n_node_ids + (long long)base.n_states * base.n_node_ids + 3;
 }
 
+// The schedules requested with blance_plan_scenarios_schedule: nc counts (>= 1), the movers ([n_node_ids]) and the
+// caller's outputs [n][nc].
+struct SchedReq {
+  int nc = 0;
+  std::vector<int32_t> count;
+  std::vector<uint8_t> mover;
+  blance_scenario_schedule_out* out = nullptr;
+};
+
+// The schedule state of a wave of nw scenarios (wave_schedule.cuh), sized from bounds known before planning: at most
+// MO = 2 x n_slots ops per partition, so at most PU x MO list entries and PU arrivals per instance.  With arena NULL
+// only the size is computed; else the slices are carved from it into W.
+static size_t wave_sched_layout(const blance_plan_in& base, int nw, int nc, char* arena, WSched* W, void** tmp,
+                                size_t* tmp_bytes, cudaStream_t st) {
+  const long long PU = base.n_parts, NU = base.n_node_ids, MO = std::max(1, 2 * base.n_slots);
+  const long long ni = (long long)nw * nc, nseg = ni * NU, cap = ni * PU * MO, nkeys = std::max(1ll, ni * PU);
+  int segbits = 1;
+  while ((1ll << segbits) <= nseg) ++segbits;
+  size_t sort_tmp = 0, scan_tmp = 0, red_tmp = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nkeys, 0, 64, st);
+  cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
+  cub::DeviceReduce::Sum(nullptr, red_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
+  *tmp_bytes = std::max(sort_tmp, std::max(scan_tmp, red_tmp)) + 256;
+  WSched w{};
+  struct Sl { void** p; size_t bytes; };
+  const std::vector<Sl> sl = {
+      {(void**)&w.count, sizeof(int32_t) * nc}, {(void**)&w.mover, (size_t)std::max(1ll, NU)}, {(void**)&w.op_n, (size_t)(nw * PU)},
+      {(void**)&w.op_node, sizeof(int32_t) * nw * PU * MO}, {(void**)&w.op_w, (size_t)(nw * PU * MO)},
+      {(void**)&w.cur, (size_t)(ni * PU)}, {(void**)&w.part_done, sizeof(int32_t) * ni * PU},
+      {(void**)&w.seg_off, sizeof(long long) * (nseg + 1)}, {(void**)&w.len, sizeof(int32_t) * (nseg + 1)},
+      {(void**)&w.kcnt, sizeof(int32_t) * (nseg + 1)}, {(void**)&w.poff, sizeof(long long) * (nseg + 1)},
+      {(void**)&w.astart, sizeof(int32_t) * nseg}, {(void**)&w.aend, sizeof(int32_t) * nseg},
+      {(void**)&w.node_rounds, sizeof(int32_t) * nseg}, {(void**)&w.node_last, sizeof(int32_t) * nseg},
+      {(void**)&w.buf0, sizeof(uint32_t) * cap}, {(void**)&w.buf1, sizeof(uint32_t) * cap}, {(void**)&w.scratch, sizeof(uint32_t) * cap},
+      {(void**)&w.keys_in, sizeof(unsigned long long) * nkeys}, {(void**)&w.keys_out, sizeof(unsigned long long) * nkeys},
+      {(void**)&w.scal, sizeof(unsigned long long) * 4 * ni}, {(void**)&w.overflow, sizeof(int32_t)},
+      {(void**)&w.esum, sizeof(long long)}, {tmp, *tmp_bytes}};
+  size_t total = 0;
+  for (const Sl& x : sl) {
+    if (arena) *x.p = arena + total;
+    total += align_up(std::max<size_t>(x.bytes, 1), 256);
+  }
+  if (arena) {
+    w.nw = nw; w.nc = nc; w.PU = (int32_t)PU; w.NU = (int32_t)NU; w.MO = (int32_t)MO; w.nseg = nseg;
+    w.PB = 1;
+    while (w.PB < WAVE_PART_BITS && (1ll << w.PB) < PU) ++w.PB;
+    *W = w;
+  }
+  return total;
+}
+
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
 // their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and override list of any.
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
-                     int max_concurrent, size_t* per_scenario) {
+                     int max_concurrent, const SchedReq* sr, size_t* per_scenario) {
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
   PlanBufs b;
-  const size_t per = slices_bytes(arena_slices(&probe, 1, b)) + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
-                     sizeof(long long) * (size_t)summary_stride(in0) +
-                     sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides;
+  size_t per = slices_bytes(arena_slices(&probe, 1, b)) + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
+               sizeof(long long) * (size_t)summary_stride(in0) +
+               sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides;
+  if (sr) {
+    void* tmp = nullptr;
+    size_t tb = 0;
+    per += wave_sched_layout(in0, 1, sr->nc, nullptr, nullptr, &tmp, &tb, ctx->stream);
+  }
   *per_scenario = per;
+  if (sr)            // the first round's arrival slots (nc x n_parts per scenario) are int32 positions
+    n_dev = (int)std::min<long long>(n_dev, std::max(1ll, (long long)INT32_MAX / ((long long)sr->nc * std::max(1, in0.n_parts))));
   if (max_concurrent > 0) return std::min(n_dev, max_concurrent);
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return 1; }
@@ -1136,8 +1196,114 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   return w;
 }
 
+// The schedules of a planned wave (wave_schedule.cuh): scenario j of the wave is caller scenario idx[j]; h_sum holds
+// the wave's summaries (node_ops carve the segments).  Rounds are enqueued in blocks of kWaveBlock; after each block
+// the host reads the entries left and sizes the next block's sorts by min(picks bound, entries).
+static const int kWaveBlock = 64;
+
+static int wave_schedule(blance_ctx* ctx, blance_plan* pl, int nw, const blance_plan_in& base, int favor_min, const SchedReq& sr,
+                         WSched W, void* tmp, size_t tmp_bytes, const long long* h_sum, long long stride, const int* idx) {
+  cudaStream_t st = ctx->stream;
+  const int nc = sr.nc, NU = base.n_node_ids, PU = base.n_parts;
+  const long long ni = (long long)nw * nc, nseg = W.nseg;
+  int rc = BLANCE_OK;
+  auto step = [&](cudaError_t e, const char* what) {
+    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+  };
+  // segments: capacity = the node's ops in the scenario (0 without a mover: nothing ever waits there)
+  std::vector<long long> seg_off((size_t)nseg + 1, 0);
+  long long pick_bound = 0, max_ops = 0;
+  for (long long i = 0; i < ni; ++i) {
+    const long long* ops = h_sum + (i / nc) * stride;
+    const int c = sr.count[(size_t)(i % nc)];
+    max_ops = std::max(max_ops, ops[stride - 2]);
+    for (int q = 0; q < NU; ++q) {
+      const long long s = i * NU + q;
+      const long long capq = sr.mover[(size_t)q] ? ops[4ll * q] + ops[4ll * q + 1] + ops[4ll * q + 2] + ops[4ll * q + 3] : 0;
+      seg_off[(size_t)s + 1] = seg_off[(size_t)s] + capq;
+      pick_bound += std::min<long long>(c, capq);
+    }
+  }
+  const long long nkeys = ni * PU;
+  const int end_bit = std::min(64, W.PB + [&] { int b = 1; while ((1ll << b) <= nseg) ++b; return b; }());
+  step(cudaMemcpyAsync((void*)W.count, sr.count.data(), sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st), "H2D");
+  step(cudaMemcpyAsync((void*)W.mover, sr.mover.data(), (size_t)NU, cudaMemcpyHostToDevice, st), "H2D");
+  step(cudaMemcpyAsync((void*)W.seg_off, seg_off.data(), sizeof(long long) * seg_off.size(), cudaMemcpyHostToDevice, st), "H2D");
+  step(cudaMemsetAsync(W.len, 0, sizeof(int32_t) * (nseg + 1), st), "memset");
+  step(cudaMemsetAsync(W.kcnt, 0, sizeof(int32_t) * (nseg + 1), st), "memset");
+  step(cudaMemsetAsync(W.astart, 0, sizeof(int32_t) * nseg, st), "memset");
+  step(cudaMemsetAsync(W.aend, 0, sizeof(int32_t) * nseg, st), "memset");
+  step(cudaMemsetAsync(W.node_rounds, 0, sizeof(int32_t) * nseg, st), "memset");
+  step(cudaMemsetAsync(W.node_last, 0, sizeof(int32_t) * nseg, st), "memset");
+  step(cudaMemsetAsync(W.scal, 0, sizeof(unsigned long long) * 4 * ni, st), "memset");
+  step(cudaMemsetAsync(W.overflow, 0, sizeof(int32_t), st), "memset");
+  const int seg_grid = grid_for(ctx, (nseg + WAVE_THREADS / 32 - 1) / (WAVE_THREADS / 32) * WAVE_THREADS, WAVE_THREADS);
+  auto sort = [&](long long n) {
+    size_t tb = tmp_bytes;
+    if (n > 0) step(cub::DeviceRadixSort::SortKeys(tmp, tb, W.keys_in, const_cast<unsigned long long*>(W.keys_out), (int)n, 0, end_bit, st), "sort");
+    k_wave_bounds<<<grid_for(ctx, std::max(1ll, n), 256), 256, 0, st>>>(W, n);
+  };
+  // the lists: every partition's first op, sorted into its segment
+  if (PU > 0 && rc == BLANCE_OK) {
+    const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
+    k_wave_moves<<<dim3((unsigned)bx, (unsigned)nw), 256, 0, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, W);
+    sort(nkeys);
+    k_wave_merge<<<seg_grid, WAVE_THREADS, 0, st>>>(W, -1);
+    ctx->launches += 3;
+  }
+  long long E = 0;
+  int32_t overflow = 0;
+  auto entries = [&]() {
+    size_t tb = tmp_bytes;
+    step(cub::DeviceReduce::Sum(tmp, tb, W.len, W.esum, (int)(nseg + 1), st), "reduce");
+    step(cudaMemcpyAsync(&E, W.esum, sizeof E, cudaMemcpyDeviceToHost, st), "D2H");
+    step(cudaMemcpyAsync(&overflow, W.overflow, sizeof overflow, cudaMemcpyDeviceToHost, st), "D2H");
+    step(cudaStreamSynchronize(st), "sync");
+    if (rc == BLANCE_OK && overflow) rc = fail(ctx, BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: a round had more picks than its bound (internal error)");
+  };
+  step(cudaGetLastError(), "k_wave_moves / k_wave_merge");
+  entries();
+  int32_t r = 0;
+  while (rc == BLANCE_OK && E > 0) {
+    // every instance with entries picks at least one op per round: no instance has more rounds than ops
+    if (r > max_ops + kWaveBlock) { rc = fail(ctx, BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: the schedule did not end (internal error)"); break; }
+    const long long n_sort = std::min(pick_bound, E);
+    for (int b = 0; b < kWaveBlock && rc == BLANCE_OK; ++b, ++r) {
+      size_t tb = tmp_bytes;
+      step(cub::DeviceScan::ExclusiveSum(tmp, tb, W.kcnt, const_cast<long long*>(W.poff), (int)(nseg + 1), st), "scan");
+      step(cudaMemsetAsync(W.keys_in, 0xFF, sizeof(unsigned long long) * (size_t)n_sort, st), "memset");
+      k_wave_pick<<<seg_grid, WAVE_THREADS, 0, st>>>(W, r, n_sort);
+      sort(n_sort);
+      k_wave_merge<<<seg_grid, WAVE_THREADS, 0, st>>>(W, r);
+      ctx->launches += 3;
+    }
+    step(cudaGetLastError(), "schedule round kernels");
+    entries();
+  }
+  if (rc != BLANCE_OK) return rc;
+  // results
+  std::vector<unsigned long long> scal((size_t)(4 * ni));
+  step(cudaMemcpyAsync(scal.data(), W.scal, sizeof(unsigned long long) * scal.size(), cudaMemcpyDeviceToHost, st), "D2H");
+  for (long long i = 0; i < ni; ++i) {
+    blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    if (o.node_rounds && NU) step(cudaMemcpyAsync(o.node_rounds, W.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st), "D2H");
+    if (o.node_last_round && NU) step(cudaMemcpyAsync(o.node_last_round, W.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st), "D2H");
+    if (o.part_done_round && PU) step(cudaMemcpyAsync(o.part_done_round, W.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st), "D2H");
+  }
+  step(cudaStreamSynchronize(st), "sync");
+  for (long long i = 0; rc == BLANCE_OK && i < ni; ++i) {
+    blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    o.rounds = (int32_t)scal[(size_t)(4 * i)];
+    o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
+    o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
+    o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
+  }
+  return rc;
+}
+
 static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
-                               const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out) {
+                               const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
+                               const SchedReq* sr) {
   std::lock_guard<std::mutex> g(ctx->mu);
   CK(cudaSetDevice(ctx->device));
   {
@@ -1167,7 +1333,7 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
     if (rc != BLANCE_OK) return rc;
   }
   size_t per = 0;
-  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, &per);
+  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, &per);
   if (W < 1) {
     plan_release(pb, ctx);
     return fail(ctx, BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
@@ -1205,6 +1371,23 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
       if (auto_wave && nw > 1) { W = nw / 2; continue; }
       rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the scenario summaries failed");
       break;
+    }
+    // the schedule state, allocated with the wave so that a plan is never lost for want of it
+    char* sched_arena = nullptr;
+    WSched wsch{};
+    void* wtmp = nullptr;
+    size_t wtmp_bytes = 0;
+    if (sr) {
+      const size_t bytes = wave_sched_layout(*base, nw, sr->nc, nullptr, nullptr, &wtmp, &wtmp_bytes, st);
+      if (cudaMallocAsync((void**)&sched_arena, bytes, st) != cudaSuccess) {
+        cudaGetLastError();
+        cudaFreeAsync(d_sum, st);
+        if (!lone) plan_release(pl, ctx);
+        if (auto_wave && nw > 1) { W = nw / 2; continue; }
+        rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the scenario schedules failed");
+        break;
+      }
+      wave_sched_layout(*base, nw, sr->nc, sched_arena, &wsch, &wtmp, &wtmp_bytes, st);
     }
     auto step = [&](cudaError_t e, const char* what) {
       if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
@@ -1276,18 +1459,23 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
       }
       if (rc != BLANCE_OK) {
         cudaFreeAsync(d_sum, st);
+        if (sched_arena) cudaFreeAsync(sched_arena, st);
         if (!lone) plan_release(pl, ctx);
         break;
       }
     }
     if (!lone && rc == BLANCE_OK) {
       rc = finish_upload(ctx, pl);
-      if (rc != BLANCE_OK) { cudaFreeAsync(d_sum, st); break; }          // (the plan is released)
+      if (rc != BLANCE_OK) {                                              // (the plan is released)
+        cudaFreeAsync(d_sum, st);
+        if (sched_arena) cudaFreeAsync(sched_arena, st);
+        break;
+      }
     }
     step(cudaEventRecord(ctx->ev[0], st), "event");
     if (rc == BLANCE_OK) rc = run(ctx, pl);
     // summaries, then the requested rows
-    float sum_ms = 0.f;
+    float sum_ms = 0.f, sched_ms = 0.f;
     if (rc == BLANCE_OK) {
       step(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), st), "memset");
       step(cudaEventRecord(ctx->ev[1], st), "event");
@@ -1335,13 +1523,23 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
         o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
         o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
       }
+      if (sr && rc == BLANCE_OK) {
+        step(cudaEventRecord(ctx->ev[3], st), "event");
+        rc = wave_schedule(ctx, pl, nw, *base, favor_min, *sr, wsch, wtmp, wtmp_bytes, h_sum.data(), stride, idx.data() + w0);
+        step(cudaEventRecord(ctx->ev[1], st), "event");
+        step(cudaEventSynchronize(ctx->ev[1]), "sync");
+        if (rc == BLANCE_OK) cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
+      }
     }
     if (times && rc == BLANCE_OK) {
       float wave_ms = 0.f;
       cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
-      std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms\n",
+      std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
                    w0, nw, W, per, wave_ms, sum_ms);
+      if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
+      std::fprintf(stderr, "\n");
     }
+    if (sched_arena) cudaFreeAsync(sched_arena, st);
     cudaFreeAsync(d_sum, st);
     if (!lone) plan_release(pl, ctx);
     w0 += nw;
@@ -1352,7 +1550,8 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
 }
 
 static int plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
-                          const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
+                          const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
+                          const SchedReq* sr = nullptr) {
   if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
   if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
   if (!base || !sc || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
@@ -1379,13 +1578,13 @@ static int plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_i
   const int G = ctx->children.empty() ? 1 : (int)std::min<size_t>(ctx->children.size(), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
-  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, opts, favor_min_nodes, max_concurrent, out);
+  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, opts, favor_min_nodes, max_concurrent, out, sr);
   // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
   std::vector<int> status((size_t)G, BLANCE_OK);
   std::vector<std::thread> th;
   for (int d = 0; d < G; ++d)
     th.emplace_back([&, d]() {
-      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out);
+      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr);
     });
   for (auto& t : th) t.join();
   for (int d = 0; d < G; ++d)
@@ -1405,6 +1604,35 @@ extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* b
                                         const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                         blance_scenario_out* out) {
   return plan_scenarios(ctx, "blance_plan_scenarios_ex", base, n, sc, opts, favor_min_nodes, max_concurrent, out);
+}
+
+extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                              const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                              int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                              blance_scenario_out* out, blance_scenario_schedule_out* sched) {
+  const char* name = "blance_plan_scenarios_schedule";
+  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+  if (n_move_conc < 1 || !move_conc || !sched)
+    return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
+  if (base && base->n_parts >= (1 << WAVE_PART_BITS))
+    return fail(ctx, BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
+  if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
+    return fail(ctx, BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
+  SchedReq sr;
+  sr.nc = n_move_conc;
+  sr.out = sched;
+  for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
+  if (base && base->n_node_ids > 0) {
+    sr.mover.assign((size_t)base->n_node_ids, 0);
+    for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
+  }
+  if (n > 0 && sc && out)
+    for (int i = 0; i < n; ++i)
+      for (int k = 0; k < n_move_conc; ++k) {
+        blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
+        o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
+      }
+  return plan_scenarios(ctx, name, base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr);
 }
 
 extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,

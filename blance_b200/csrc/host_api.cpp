@@ -1162,7 +1162,8 @@ std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const 
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
-                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent) {
+                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
+                                                 const std::vector<int>& scheduleConcurrency) {
   if (scenarios.empty()) invalid("PlanNextMapScenarios: no scenarios");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
   const size_t n = scenarios.size();
@@ -1194,9 +1195,19 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
       out[i].warn = maps[i]->warn.data();
     }
   }
+  const size_t nc = scheduleConcurrency.size();
+  std::vector<blance_scenario_schedule_out> sched(n * nc);
+  std::vector<int32_t> node_rounds(n * nc * size_t(NU) + 1), node_last(n * nc * size_t(NU) + 1);
+  for (size_t x = 0; x < sched.size(); ++x) {
+    sched[x] = blance_scenario_schedule_out{};
+    sched[x].node_rounds = node_rounds.data() + x * size_t(NU);
+    sched[x].node_last_round = node_last.data() + x * size_t(NU);
+  }
   blance_ctx* ctx = DefaultContext();
-  const int st = blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
-                                          out.data());
+  const int st = nc ? blance_plan_scenarios_schedule(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                                     int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), sched.data())
+                    : blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                               out.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_scenarios failed: ") + blance_last_error(ctx));
   static const char* kOps[] = {"add", "del", "promote", "demote"};
   std::vector<ScenarioResult> res(n);
@@ -1217,6 +1228,17 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
       maps[i]->out.iters_run = o.iters_run;
       const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
       if (o.iters_run > 0) r.NextMap = unintern_plan(*ip, *maps[i], &r.NextWarnings, k);   // MaxIterationsPerPlan <= 0: plan.go:32,57
+    }
+    for (size_t k = 0; k < nc; ++k) {
+      const blance_scenario_schedule_out& so = sched[i * nc + k];
+      ScenarioSchedule s;
+      s.MaxConcurrentPartitionMovesPerNode = scheduleConcurrency[k];
+      s.Rounds = so.rounds; s.MovesDone = so.moves_done; s.StuckParts = so.stuck_parts; s.MaxBatch = so.max_batch;
+      for (int32_t q = 0; q < NU; ++q) {
+        if (so.node_rounds[q]) s.NodeRounds[ip->node_names[size_t(q)]] = so.node_rounds[q];
+        if (so.node_last_round[q]) s.NodeLastRound[ip->node_names[size_t(q)]] = so.node_last_round[q];
+      }
+      r.Schedules.push_back(std::move(s));
     }
   }
   return res;

@@ -107,6 +107,16 @@ struct Scenario {
   ScenarioOpt<::blance::HierarchyRules> HierarchyRules;
 };
 
+// The rebalance schedule of one scenario at one MaxConcurrentPartitionMovesPerNode (blance_plan_scenarios_schedule):
+// the lock-step model of blance_moves_schedule over the moves NodeOps counts; per node (by name, nonzero entries
+// only) the rounds with a batch and 1 + the last such round.
+struct ScenarioSchedule {
+  int MaxConcurrentPartitionMovesPerNode = 0;
+  int Rounds = 0, MaxBatch = 0;
+  int64_t MovesDone = 0, StuckParts = 0;
+  std::unordered_map<std::string, int> NodeRounds, NodeLastRound;
+};
+
 struct ScenarioResult {
   int iters_run = 0, converged = 0;
   int64_t steps = 0, sticky_steps = 0, parts_moved = 0, ops_total = 0, warn_parts = 0;
@@ -118,6 +128,7 @@ struct ScenarioResult {
   bool HasMap = false;                 // the scenario was listed in wantMaps
   PartitionMap NextMap;                // as PlanNextMapEx returns it
   Warnings NextWarnings;
+  std::vector<ScenarioSchedule> Schedules;   // one per scheduleConcurrency value; empty without them
 };
 
 // Scenario i is PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, NodesToRemove_i, NodesToAdd_i, model, options
@@ -128,10 +139,16 @@ struct ScenarioResult {
 // options' weights (blance_plan_scenarios_ex).  A scenario the reference would panic on (plan.go:544) or the device
 // cannot plan (constraints above 16) throws BlanceError naming its index before any device work.  NextMap /
 // NextWarnings are filled for the indices in wantMaps; maxConcurrent as in blance_plan_scenarios.
+// scheduleConcurrency non-empty: each result's Schedules holds the rebalance schedule at each value
+// (blance_plan_scenarios_schedule), with the nodesAll names as the movers, as OrchestrateSchedule has them.  One
+// difference to OrchestrateSchedule: partitions are walked in interning order (the name rule of plan.go:519-528), where
+// OrchestrateSchedule walks them in byte order of their names.  Both are valid instances of Go's map order, and they
+// agree whenever the names sort the same under both rules.
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
-                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent);
+                                                 bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
+                                                 const std::vector<int>& scheduleConcurrency = {});
 
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 

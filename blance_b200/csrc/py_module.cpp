@@ -359,7 +359,7 @@ PYBIND11_MODULE(_host, m) {
                      const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
                      const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
                      const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
-                     int engine) {
+                     int engine, const std::vector<int>& schedule_concurrency) {
         PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
         const PartitionMap prev_map = to_map(prev);
         const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
@@ -368,7 +368,7 @@ PYBIND11_MODULE(_host, m) {
         {
           py::gil_scoped_release rel;
           res = PlanNextMapScenarios(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, scs,
-                                     favor_min_nodes, want_maps, max_concurrent);
+                                     favor_min_nodes, want_maps, max_concurrent, schedule_concurrency);
         }
         py::list out;
         for (const auto& r : res) {
@@ -377,6 +377,17 @@ PYBIND11_MODULE(_host, m) {
           d["sticky_steps"] = r.sticky_steps; d["parts_moved"] = r.parts_moved; d["ops_total"] = r.ops_total;
           d["warn_parts"] = r.warn_parts; d["node_ops"] = r.NodeOps; d["state_node_load"] = r.StateNodeLoad;
           if (r.HasMap) { d["next_map"] = from_map(r.NextMap); d["warnings"] = r.NextWarnings; }
+          if (!schedule_concurrency.empty()) {
+            py::list sl;
+            for (const auto& s : r.Schedules) {
+              py::dict sd;
+              sd["MaxConcurrentPartitionMovesPerNode"] = s.MaxConcurrentPartitionMovesPerNode;
+              sd["Rounds"] = s.Rounds; sd["MovesDone"] = s.MovesDone; sd["StuckParts"] = s.StuckParts;
+              sd["MaxBatch"] = s.MaxBatch; sd["NodeRounds"] = s.NodeRounds; sd["NodeLastRound"] = s.NodeLastRound;
+              sl.append(sd);
+            }
+            d["schedules"] = sl;
+          }
           out.append(d);
         }
         return out;
@@ -385,7 +396,8 @@ PYBIND11_MODULE(_host, m) {
       py::arg("favor_min_nodes") = false, py::arg("want_maps") = std::vector<int>{}, py::arg("max_concurrent") = 0,
       py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
-      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
+      py::arg("schedule_concurrency") = std::vector<int>{});
 
   // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
   m.def(

@@ -11,8 +11,9 @@
 //   k_sched_flags  + select: the active list compacted in order (finished and stuck partitions dropped)
 // Every kernel reads the active count and the done flag from SchedState, so the host can enqueue a block of
 // rounds and look at the flag once per block.  The work of a round is proportional to the bound on the active
-// entries the host last read, plus n_node_ids for the scan - never to n_parts.  A later caller can run one such
-// sequence per scenario instance: nothing here is global to the context.
+// entries the host last read, plus n_node_ids for the scan - never to n_parts.  The schedules of a scenario wave
+// (blance_plan_scenarios_schedule) run on wave_schedule.cuh instead, which shares the picks (sched_pick_node) but
+// keeps the per-node lists between rounds rather than sorting every active entry each round.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -146,10 +147,29 @@ __global__ void __launch_bounds__(SCHED_SCAN_THREADS) k_sched_scan(int32_t n_nod
   }
 }
 
-// One warp per node: filterNextPlausibleMovesForNode over the node's list L (ascending partition index).  Each
-// pick is the FIRST index of the minimal MoveOpWeight over L as it stands (a warp arg-min of (weight, index));
-// L[pick] = L[last] and L shrinks.  Lists of any length and counts up to the length are exact: every pick scans
-// the whole remaining list.  wl holds the weights next to L so that the scans touch two arrays only.
+// filterNextPlausibleMovesForNode over one node's list of m entries, run by one warp: k picks, each the FIRST index
+// of the minimal MoveOpWeight over the list as it stands (a warp arg-min of (weight, index)).  weight(i) reads entry
+// i's weight; lane 0 calls take(j, i, last) for pick j at index i, and take must replace entry i by entry `last`
+// (the swap-remove; the list then shrinks by one).  Lists of any length and counts up to the length are exact:
+// every pick scans the whole remaining list.
+template <class Weight, class Take>
+__device__ __forceinline__ void sched_pick_node(int32_t m, int32_t k, int lane, Weight&& weight, Take&& take) {
+  for (int32_t j = 0; j < k; ++j) {
+    uint32_t bw = 8, bi = 0xFFFFFFFFu;
+    for (int32_t i = lane; i < m; i += 32) {            // ascending i: the strict < keeps this lane's first minimum
+      const uint32_t w = weight(i);
+      if (w < bw) { bw = w; bi = (uint32_t)i; }
+    }
+    const uint32_t wmin = __reduce_min_sync(0xFFFFFFFFu, bw);
+    const int32_t imin = (int32_t)__reduce_min_sync(0xFFFFFFFFu, bw == wmin ? bi : 0xFFFFFFFFu);
+    if (lane == 0) take(j, imin, m - 1);
+    __syncwarp();
+    --m;
+  }
+}
+
+// One warp per node: sched_pick_node over the node's list L (ascending partition index).  wl holds the weights
+// next to L so that the scans touch two arrays only.
 constexpr int SCHED_PICK_THREADS = 256;
 
 __global__ void __launch_bounds__(SCHED_PICK_THREADS) k_sched_pick(int32_t n_node_ids, int32_t count,
@@ -175,24 +195,13 @@ __global__ void __launch_bounds__(SCHED_PICK_THREADS) k_sched_pick(int32_t n_nod
     __syncwarp();
     const int32_t k = m < count ? m : count;
     long long* out = sched_op + base + boff[n];
-    for (int32_t j = 0; j < k; ++j) {
-      uint32_t bw = 8, bi = 0xFFFFFFFFu;
-      for (int32_t i = lane; i < m; i += 32) {          // ascending i: the strict < keeps this lane's first minimum
-        const uint32_t w = W[i];
-        if (w < bw) { bw = w; bi = (uint32_t)i; }
-      }
-      const uint32_t wmin = __reduce_min_sync(0xFFFFFFFFu, bw);
-      const int32_t imin = (int32_t)__reduce_min_sync(0xFFFFFFFFu, bw == wmin ? bi : 0xFFFFFFFFu);
-      if (lane == 0) {
-        const int32_t p = L[imin];
-        out[j] = off[p] + cur[p];
-        cur[p] += 1;
-        L[imin] = L[m - 1];
-        W[imin] = W[m - 1];
-      }
-      __syncwarp();
-      --m;
-    }
+    sched_pick_node(m, k, lane, [&](int32_t i) { return (uint32_t)W[i]; }, [&](int32_t j, int32_t imin, int32_t last) {
+      const int32_t p = L[imin];
+      out[j] = off[p] + cur[p];
+      cur[p] += 1;
+      L[imin] = L[last];
+      W[imin] = W[last];
+    });
   }
 }
 

@@ -126,9 +126,29 @@ class ScenarioResult:
     converged = property(lambda self: self.out.converged)
     steps = property(lambda self: self.out.steps)
     sticky_steps = property(lambda self: self.out.sticky_steps)
+    schedules = None          # blance_plan_scenarios_schedule: one ScenarioSchedule per count
     parts_moved = property(lambda self: self.out.parts_moved)
     ops_total = property(lambda self: self.out.ops_total)
     warn_parts = property(lambda self: self.out.warn_parts)
+
+
+class ScenarioSchedule:
+    """Output buffers of a blance_scenario_schedule_out: the schedule's summaries at one count."""
+
+    def __init__(self, t, count):
+        self.count = count
+        self.node_rounds = np.zeros(t.n_node_ids, np.int32)
+        self.node_last_round = np.zeros(t.n_node_ids, np.int32)
+        self.part_done_round = np.zeros(t.n_parts, np.int32)
+        self.out = api.ScenarioScheduleOut()
+        for f in ("node_rounds", "node_last_round", "part_done_round"):
+            a = getattr(self, f)
+            setattr(self.out, f, a.ctypes.data if a.size else None)
+
+    rounds = property(lambda self: self.out.rounds)
+    moves_done = property(lambda self: self.out.moves_done)
+    stuck_parts = property(lambda self: self.out.stuck_parts)
+    max_batch = property(lambda self: self.out.max_batch)
 
 
 def scenario_tables(base, scenario, opts=None):
@@ -251,11 +271,15 @@ class Context:
             r.out = o
         return results
 
-    def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None):
+    def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None,
+                       schedule=None, node_has_mover=None):
         """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
         (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
         are copied out.  opts (None, or one dict of OPT_GROUPS keys per scenario) calls blance_plan_scenarios_ex
-        with those plan options.  Returns one ScenarioResult per scenario."""
+        with those plan options.  schedule (None, or a list of MaxConcurrentPartitionMovesPerNode values) calls
+        blance_plan_scenarios_schedule instead, with node_has_mover ([n_node_ids], None = the ids < n_nodes), and
+        sets each result's `schedules` to one ScenarioSchedule per value.  Returns one ScenarioResult per
+        scenario."""
         n = len(scenarios)
         want = set(want_rows)
         base = base_tables.struct()
@@ -272,7 +296,23 @@ class Context:
                 setattr(scs[i], f, a.ctypes.data if a.size else None)
         results = [ScenarioResult(base_tables, i in want) for i in range(n)]
         outs = (api.ScenarioOut * max(1, n))(*[r.out for r in results])
-        if opts is None:
+        if schedule is not None:
+            counts = np.ascontiguousarray(schedule, np.int32)
+            mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
+            if mover is not None and mover.size != base_tables.n_node_ids:
+                raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
+            for r in results:
+                r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+            sch = (api.ScenarioScheduleOut * max(1, n * counts.size))(*[s.out for r in results for s in r.schedules])
+            ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
+            self._check(self.lib.blance_plan_scenarios_schedule(
+                self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent), int(counts.size),
+                counts.ctypes.data if counts.size else None, None if mover is None else mover.ctypes.data, outs, sch),
+                "blance_plan_scenarios_schedule")
+            for i, r in enumerate(results):
+                for k, s in enumerate(r.schedules):
+                    s.out = sch[i * counts.size + k]
+        elif opts is None:
             self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),
                                                        int(max_concurrent), outs), "blance_plan_scenarios")
         else:

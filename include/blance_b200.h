@@ -293,6 +293,59 @@ int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_
                              const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                              blance_scenario_out* out);
 
+/* ---- the rebalance schedule of every scenario (blance_plan_scenarios_schedule) --------------------------------
+ * Summaries of the lock-step schedule of blance_moves_schedule (rules 1-5 below) of one scenario's moves at one
+ * MaxConcurrentPartitionMovesPerNode.  Every array may be NULL (not copied). */
+typedef struct blance_scenario_schedule_out {
+  int32_t  rounds;           /* R, as blance_schedule_out */
+  int64_t  moves_done;       /* ops scheduled */
+  int64_t  stuck_parts;      /* partitions whose next move is on a node without a mover */
+  int32_t  max_batch;        /* largest batch of one node in one round */
+  int32_t* node_rounds;      /* [n_node_ids] rounds in which the node has a batch */
+  int32_t* node_last_round;  /* [n_node_ids] 1 + last round with a batch on the node, 0 = none */
+  int32_t* part_done_round;  /* [n_parts] 1 + round of the partition's last op; 0 = no ops; -1 = stuck */
+} blance_scenario_schedule_out;
+
+/* blance_plan_scenarios_ex, and how long each scenario's rebalance takes.
+ *
+ * Plans are unchanged: out[i] equals what blance_plan_scenarios_ex returns for the same arguments (rows, shapes,
+ * warnings, scalars, node_ops and state_node_load).
+ *
+ * sched[i * n_move_conc + k] is the lock-step schedule of blance_moves_schedule (rules 1-5 there, unchanged) at
+ * MaxConcurrentPartitionMovesPerNode = move_conc[k] (values <= 0 mean 1, orchestrate.go:484-487) of exactly the
+ * move lists node_ops counts: for every partition with part_in_assign, CalcPartitionMoves over all model states in
+ * state order from its prev row as passed in to its next row (a partition with part_in_prev == 0 starts from an
+ * empty row); every other partition has no ops.  In orchestrator terms: OrchestrateMoves(model, {move_conc[k],
+ * favor_min_nodes}, nodesAll, begMap = prevMap plus an empty entry for every assigned partition it lacks,
+ * endMap = the final map).  So moves_done + the ops left on stuck partitions = ops_total.
+ *
+ * Partitions are walked in ascending partition index.  node_has_mover ([n_node_ids]) NULL means that exactly the ids
+ * < n_nodes (nodesAll) have a mover, as in OrchestrateSchedule, where a node outside nodesAll has none.
+ *
+ * Summaries, read from the schedule's round_off / sched_op (blance_moves_schedule_fetch):
+ *   node_rounds[q]      number of rounds r with an op on node q in round r;
+ *   node_last_round[q]  1 + the last such r, 0 if none;
+ *   part_done_round[p]  1 + the round of partition p's last op if all its ops were scheduled and it has any; 0 if it
+ *                       has no ops; -1 if it is stuck (its next op is on a node without a mover);
+ *   rounds, moves_done, stuck_parts and max_batch as blance_schedule_out.
+ * Every value equals blance_moves_create (favor_min_nodes, all states visited) + blance_moves_schedule on that
+ * scenario's prev and next rows, and none depends on n, max_concurrent, the wave size, the engine, the number of
+ * devices or the other values of move_conc.
+ *
+ * Errors, before any device work, naming the scenario or the index k: everything blance_plan_scenarios_ex rejects;
+ * n_move_conc < 1, a NULL move_conc or a NULL sched (BLANCE_ERR_INVALID_ARG); 2^29 or more partitions
+ * (BLANCE_ERR_UNSUPPORTED).  BLANCE_ERR_NOMEM when one scenario together with its schedules does not fit in device
+ * memory.
+ *
+ * Scheduling as blance_plan_scenarios_ex.  A scenario's schedule state is priced into the wave size from a bound
+ * known before planning (2 x n_slots ops per partition, per count) and allocated with the wave, so the automatic
+ * wave never fails for memory because of it; all counts of all scenarios of a wave run in one lock-step sequence
+ * on the wave's device (DESIGN.md section 10). */
+int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                   const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                   int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                   blance_scenario_out* out, blance_scenario_schedule_out* sched);
+
 /* Device-resident variant used by benchmarks and by callers that chain plans:
  * uploads `in` once and returns a handle; blance_plan_run() replays the whole
  * plan on the resident tables (inputs are restored on device before each run);

@@ -4,6 +4,14 @@ and writes it to --out.
 
     python tools/bench_scenarios.py [--ks 1,8,33,66,132] [--cfgs 4,3] [--out profiles/h100_scenarios.json]
     python tools/bench_scenarios.py --sweep stickiness,replicas [--out profiles/h100_option_sweeps.json]
+    python tools/bench_scenarios.py --schedule 1,2,4 [--ks 8,66] [--cap 4] [--out profiles/h100_scenario_schedule.json]
+
+--schedule times, on cfg 4 node-failure sweeps, the plain sweep (blance_plan_scenarios), the sweep with the
+rebalance schedules at those MaxConcurrentPartitionMovesPerNode values (blance_plan_scenarios_schedule) and the
+only alternative without it (rows copied out, then blance_moves_create + blance_moves_schedule per scenario and per
+value), alternating in one process.  The alternative runs on the first --cap scenarios and is extrapolated to K.
+Sampled scenarios' schedule summaries are checked against the serial oracle (tests/schedule_oracle.c).  It also
+times the wave engine as a wave of one on the headline rebalance next to blance_moves_schedule on the same moves.
 
 --sweep plans option variants of the cfg 4 cluster instead (StateStickiness {0, 1, 2, 3, 5, 8}, or replicas
 {1, 2, 3, 4} on a base widened to 4 replica slots) through blance_plan_scenarios_ex, against the same variants one
@@ -164,6 +172,104 @@ def run_cfg(ctx, cfg, ks, rng):
     return t, rows
 
 
+WAVE_SCHED_RE = re.compile(r"schedule ([\d.]+) ms")
+
+
+def schedule_summary_of(off, node, kind, n_node_ids, c, mover):
+    """The serial oracle's schedule at count c, reduced to the summaries of blance_plan_scenarios_schedule."""
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import schedule_oracle as SO
+    from test_scenario_schedule import schedule_summaries
+    ro, so, _ = SO.schedule(off, node, kind, n_node_ids, c, mover)
+    return schedule_summaries(off, node, n_node_ids, ro, so)
+
+
+def scenario_moves(ctx, t, next_rows):
+    """The CSR move lists the scenario schedule runs over (blance_moves_create on beg / end rows)."""
+    a = t.part_in_assign != 0
+    beg = np.where(((t.part_in_prev != 0) & a)[:, None], t.prev_rows, -1).astype(np.int32)
+    beg[~a] = next_rows[~a]
+    return beg
+
+
+def run_schedule_sweeps(ctx, counts, ks, cap, rng):
+    t = synth.make_rebalance(4)
+    mover = (np.arange(t.n_node_ids) < t.n_nodes).astype(np.uint8)
+    warm = failure_scenarios(t, 2)
+    ctx.plan_scenarios(t, warm, False)                                     # warm-up of every kernel the runs use
+    ctx.plan_scenarios(t, warm, False, schedule=counts)
+    rows = []
+    for k in ks:
+        scs = failure_scenarios(t, k)
+
+        def timed(**kw):
+            with CaptureStderr() as cap_err:
+                t0 = time.perf_counter()
+                res = ctx.plan_scenarios(t, scs, False, **kw)
+                wall = time.perf_counter() - t0
+            return res, wall, parse_waves(cap_err.text), sum(float(x) for x in WAVE_SCHED_RE.findall(cap_err.text))
+
+        def alternative():
+            n = min(cap, len(scs))
+            t0 = time.perf_counter()
+            res = ctx.plan_scenarios(t, scs[:n], False, want_rows=range(n))
+            t1 = time.perf_counter()
+            out = []
+            for r in res:
+                h, _ = ctx.moves_create(t.state_slot_off, scenario_moves(ctx, t, r.next_rows), r.next_rows, False, t.n_node_ids)
+                out.append([ctx.moves_schedule(h, c, mover)[2] for c in counts])
+                ctx.moves_free(h)
+            t2 = time.perf_counter()
+            return n, t1 - t0, t2 - t1, out
+
+        plain_a, plain_s_a, _, _ = timed()
+        sched_a, sched_s_a, info, sched_ms_a = timed(schedule=counts)
+        n_alt, alt_plan_s, alt_sched_s, _ = alternative()
+        _, plain_s_b, _, _ = timed()
+        _, sched_s_b, _, sched_ms_b = timed(schedule=counts)
+        plain_s, sched_s = min(plain_s_a, plain_s_b), min(sched_s_a, sched_s_b)
+        # the alternative at K: the plain sweep with rows out, plus the per-scenario schedules extrapolated from n_alt
+        alt_s = plain_s + alt_sched_s * len(scs) / n_alt
+        ok = True
+        for i in sorted(set(rng.choice(len(scs), size=min(2, len(scs)), replace=False).tolist())):
+            r = ctx.plan_scenarios(t, [scs[i]], False, want_rows=[0])[0]
+            h, total = ctx.moves_create(t.state_slot_off, scenario_moves(ctx, t, r.next_rows), r.next_rows, False, t.n_node_ids)
+            off, node, _, kind = ctx.moves_fetch(h, total)
+            ctx.moves_free(h)
+            for c, s in zip(counts, sched_a[i].schedules):
+                want = schedule_summary_of(off, node, kind, t.n_node_ids, c, mover)
+                ok &= all(getattr(s, f) == want[f] for f in ("rounds", "moves_done", "stuck_parts", "max_batch"))
+                ok &= all(np.array_equal(getattr(s, f), want[f]) for f in ("node_rounds", "node_last_round", "part_done_round"))
+            ok &= bool(sched_a[i].ops_total == plain_a[i].ops_total == r.ops_total)
+        row = dict(cfg=4, K=k, counts=counts, plain_sweep_s=[round(plain_s_a, 3), round(plain_s_b, 3)],
+                   schedule_sweep_s=[round(sched_s_a, 3), round(sched_s_b, 3)],
+                   schedule_device_ms=[round(sched_ms_a, 3), round(sched_ms_b, 3)],
+                   added_over_plain=round((sched_s - plain_s) / plain_s, 4),
+                   alternative=dict(scenarios_measured=n_alt, plan_with_rows_s=round(alt_plan_s, 3),
+                                    schedules_s=round(alt_sched_s, 3), extrapolated_to_K_s=round(alt_s, 3)),
+                   speedup_vs_alternative=round(alt_s / sched_s, 3), rounds=[[s.rounds for s in r.schedules] for r in sched_a[:4]],
+                   correct=bool(ok), **info)
+        print(json.dumps(row), flush=True)
+        rows.append(row)
+    # the wave engine as a wave of one on the headline rebalance, next to blance_moves_schedule on the same moves
+    one = []
+    r = ctx.plan_scenarios(t, [{}], False, want_rows=[0])[0]
+    h, _ = ctx.moves_create(t.state_slot_off, scenario_moves(ctx, t, r.next_rows), r.next_rows, False, t.n_node_ids)
+    for c in counts:
+        ms = []
+        for _ in range(2):
+            with CaptureStderr() as cap_err:
+                w = ctx.plan_scenarios(t, [{}], False, schedule=[c])[0].schedules[0]
+            ms.append(float(WAVE_SCHED_RE.findall(cap_err.text)[0]))
+        dev = [ctx.moves_schedule(h, c, mover)[2] for _ in range(2)]
+        one.append(dict(c=c, rounds=w.rounds, wave_of_one_ms=[round(x, 3) for x in ms],
+                        moves_schedule_ms=[round(d["device_ms"], 3) for d in dev], same_rounds=dev[0]["rounds"] == w.rounds,
+                        same_max_batch=dev[0]["max_batch"] == w.max_batch))
+        print(json.dumps(one[-1]), flush=True)
+    ctx.moves_free(h)
+    return dict(sweeps=rows, headline_wave_of_one=one)
+
+
 def option_variants(t, kind):
     """The option sweeps of the 1 M x 1 024 cluster (blance_scenario_opts as dicts): StateStickiness of every state
     in {0, 1, 2, 3, 5, 8}, or the replica count in {1, 2, 3, 4} on a base widened to 4 replica slots."""
@@ -216,12 +322,25 @@ def main():
     ap.add_argument("--cfgs", default="4,3")
     ap.add_argument("--wave-ks", default="33,66,132", help="explicit max_concurrent values tried on cfg 4 at the largest K")
     ap.add_argument("--sweep", default=None, help="option sweeps instead of node failures: stickiness, replicas, or both (comma separated)")
+    ap.add_argument("--schedule", default=None, help="MaxConcurrentPartitionMovesPerNode values, e.g. 1,2,4: time the sweeps with schedules")
+    ap.add_argument("--cap", type=int, default=4, help="--schedule: scenarios the one-by-one alternative runs on before extrapolating")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     ks = [int(x) for x in a.ks.split(",")]
     rng = np.random.default_rng(0)
     rec = dict(tool="tools/bench_scenarios.py", **gpu_info())
     ctx = tables.Context()
+    if a.schedule:
+        rec["schedule"] = run_schedule_sweeps(ctx, [int(x) for x in a.schedule.split(",")],
+                                              [int(x) for x in (a.ks if a.ks != ap.get_default("ks") else "8,66").split(",")], a.cap, rng)
+        rec["command"] = "python tools/bench_scenarios.py " + " ".join(sys.argv[1:])
+        ctx.close()
+        print(json.dumps(rec))
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(rec, f, indent=1)
+        return
     if a.sweep:
         rec["option_sweeps"] = [run_option_sweep(ctx, kind) for kind in a.sweep.split(",")]
         ctx.close()
