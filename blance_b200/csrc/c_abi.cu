@@ -9,9 +9,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -35,9 +37,66 @@ static std::string g_create_error;
 
 // Opted-in dynamic shared memory of k_assign_pass_seq<1|2|4|8>, per device.  The attribute belongs to the
 // (function, device) pair, not to a blance_ctx, and must only ever be raised.
-static std::mutex g_seq_dyn_mu;
+static std::mutex g_dyn_smem_mu;
 static size_t g_seq_dyn[64][4][4];   // [device][NPT index][K - 1]
 static size_t g_spec_dyn[64][4];     // [device][K - 1], k_assign_pass_spec
+
+// A failure inside this file.  It is thrown, and entry() / fan_out() turn it into a status and a message.
+struct Error {
+  int status;
+  std::string msg;
+};
+
+[[noreturn]] static void throw_err(int status, const std::string& msg) { throw Error{status, msg}; }
+
+static void cuda_check(cudaError_t e, const char* call) {
+  if (e != cudaSuccess) throw_err(BLANCE_ERR_CUDA, std::string(call) + " failed: " + cudaGetErrorString(e));
+}
+#define CUDA(call) cuda_check((call), #call)
+
+static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// One stream-ordered device allocation carved into slices, each aligned to 256 bytes.  The slice list alone
+// gives the size, so a layout is priced without allocating it; carve() lays the same list over a host buffer.
+class Arena {
+ public:
+  Arena() = default;
+  Arena(const Arena&) = delete;
+  Arena& operator=(const Arena&) = delete;
+  ~Arena() {
+    if (base_) cudaFreeAsync(base_, stream_);       // back to the pool (stream ordered)
+  }
+  template <class T> void add(T*& p, size_t count) { slices_.push_back(Slice{(void**)&p, sizeof(T) * count}); }
+  void add(void*& p, size_t bytes) { slices_.push_back(Slice{&p, bytes}); }
+  size_t bytes() const {
+    size_t total = 0;
+    for (const Slice& s : slices_) total += span(s);
+    return total;
+  }
+  void carve(void* base) const {
+    char* p = (char*)base;
+    for (const Slice& s : slices_) { *s.ptr = p; p += span(s); }
+  }
+  // The context's memory pool keeps the arena of the previous call around.
+  void alloc(cudaStream_t st, const char* what) {
+    void* p = nullptr;
+    const cudaError_t e = cudaMallocAsync(&p, bytes(), st);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      throw_err(BLANCE_ERR_NOMEM, std::string("cudaMalloc of ") + what + " failed: " + cudaGetErrorString(e));
+    }
+    base_ = p;
+    stream_ = st;
+    carve(p);
+  }
+
+ private:
+  struct Slice { void** ptr; size_t bytes; };
+  static size_t span(const Slice& s) { return align_up(std::max<size_t>(s.bytes, 1), 256); }   // no two slices alias
+  std::vector<Slice> slices_;
+  void* base_ = nullptr;
+  cudaStream_t stream_ = nullptr;
+};
 
 struct blance_ctx {
   int device = 0;
@@ -57,20 +116,95 @@ struct blance_ctx {
   std::vector<blance_ctx*> children; // blance_ctx_create_multi: one single-device context per GPU
 };
 
-#define CK(call)                                                                           \
-  do {                                                                                     \
-    cudaError_t e_ = (call);                                                               \
-    if (e_ != cudaSuccess) {                                                               \
-      char b_[512];                                                                        \
-      std::snprintf(b_, sizeof b_, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-      ctx->err = b_;                                                                       \
-      return BLANCE_ERR_CUDA;                                                              \
-    }                                                                                      \
-  } while (0)
-
 static int fail(blance_ctx* ctx, int st, const std::string& msg) {
   if (ctx) ctx->err = msg; else g_create_error = msg;
   return st;
+}
+
+// The entry ritual on the context that does a call's work: its lock is taken, its device made current, and an
+// earlier CUDA error still pending on this thread is reported instead of being blamed on this call's first launch.
+static std::unique_lock<std::mutex> enter(blance_ctx* dev) {
+  std::unique_lock<std::mutex> lock(dev->mu);
+  CUDA(cudaSetDevice(dev->device));
+  const cudaError_t stale = cudaGetLastError();
+  if (stale != cudaSuccess)
+    throw_err(BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
+  return lock;
+}
+
+// device() takes the entry ritual on the context that does the work (the first device of a multi-device context)
+// and returns it.  An entry point calls it after the argument checks that need no device.
+struct Device {
+  blance_ctx* ctx;
+  std::unique_lock<std::mutex> lock;
+  blance_ctx* operator()() {
+    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    blance_ctx* dev = ctx->children.empty() ? ctx : ctx->children[0];
+    lock = enter(dev);
+    return dev;
+  }
+};
+
+// The boundary of every entry point that reports into a context: runs body(device) and turns what it throws into
+// the status and the message of the context the caller passed (of blance_last_error(NULL) when that is NULL).
+template <class F>
+static int entry(blance_ctx* ctx, F&& body) noexcept {
+  Device device{ctx, {}};
+  try {
+    body(device);
+    return BLANCE_OK;
+  } catch (const Error& e) {
+    return fail(ctx, e.status, e.msg);
+  } catch (const std::exception& e) {                   // host memory or threads
+    return fail(ctx, BLANCE_ERR_NOMEM, std::string("host resources exhausted: ") + e.what());
+  }
+}
+
+// Runs work(d, dev) on devices d = 0 .. G-1 of ctx (ctx itself when it is a single-device context, with G = 1),
+// one host thread per device, each after the entry ritual.  The first failing device's error is rethrown as
+// "device N: ...".
+template <class F>
+static void fan_out(blance_ctx* ctx, int G, F&& work) {
+  if (ctx->children.empty()) {
+    auto lock = enter(ctx);
+    work(0, ctx);
+    return;
+  }
+  std::vector<Error> err((size_t)G, Error{BLANCE_OK, std::string()});
+  auto one = [&](int d) {
+    blance_ctx* dev = ctx->children[(size_t)d];
+    try {
+      auto lock = enter(dev);
+      work(d, dev);
+    } catch (const Error& e) {
+      err[(size_t)d] = e;
+    } catch (const std::exception& e) {
+      err[(size_t)d] = Error{BLANCE_ERR_NOMEM, std::string("host resources exhausted: ") + e.what()};
+    }
+  };
+  std::vector<std::thread> th;
+  for (int d = 0; d < G; ++d) th.emplace_back(one, d);
+  for (auto& t : th) t.join();
+  for (int d = 0; d < G; ++d)
+    if (err[(size_t)d].status != BLANCE_OK)
+      throw_err(err[(size_t)d].status, "device " + std::to_string(ctx->children[(size_t)d]->device) + ": " + err[(size_t)d].msg);
+}
+
+// Launches a kernel of this library on the context's stream, counts it and checks the launch.
+template <class... P, class... A>
+static void launch(blance_ctx* ctx, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  kernel<<<grid, block, smem, ctx->stream>>>(std::forward<A>(args)...);
+  ++ctx->launches;
+  CUDA(cudaGetLastError());
+}
+
+// Raises a kernel's dynamic shared memory opt-in on the current device to `bytes` (it is never lowered).
+// `configured` is the (kernel, device) pair's current opt-in.
+static void opt_in_smem(const void* kernel, size_t* configured, size_t bytes) {
+  std::lock_guard<std::mutex> g(g_dyn_smem_mu);
+  if (bytes <= *configured) return;
+  CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  *configured = bytes;
 }
 
 extern "C" int blance_version(void) { return 100; }
@@ -130,7 +264,8 @@ extern "C" int blance_ctx_create(blance_ctx** out, int device_id) {
 
 // One context over several GPUs of the node (SURVEY.md section 8b: blance_ctx_create(gpu_ids, n_gpus)).  A batch
 // (blance_plan_next_map_batch) is sharded instance i -> device i mod n, one host thread per device, no collective:
-// plan instances are independent.  Everything else runs on the first device.
+// plan instances are independent; scenarios are sharded the same way (fan_out()).  Everything else runs on the
+// first device (entry()).
 extern "C" int blance_ctx_create_multi(blance_ctx** out, const int* device_ids, int n_devices) {
   if (!out) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "blance_ctx_create_multi: out is NULL");
   *out = nullptr;
@@ -185,8 +320,7 @@ struct blance_plan {
   int max_N = 0, max_S = 0, max_NU = 0;
   int pair_inst_shift = 0, pair_end_bit = 64;   // key layout of the (top, node) pair sort (k_pair_keys)
   bool any_state_active[BL_S_MAX] = {};
-  void* arena = nullptr;               // one device allocation, carved below
-  size_t arena_bytes = 0;
+  Arena arena;                         // one device allocation, carved by plan_slices()
   DPool pool{};
   // immutable copies of the mutable state, to replay the plan (blance_plan_run)
   int32_t *rows_init = nullptr, *prev_rows_init = nullptr;
@@ -197,14 +331,18 @@ struct blance_plan {
   uint8_t *rawsh_a = nullptr, *rawsh_b = nullptr;       // cur/prev shape in, next shape (a) / warn (b) out
   long long *d_raw_rows_off = nullptr, *d_raw_shape_off = nullptr;
   int* d_seg_off = nullptr;            // [n_inst+1] partition offsets for the segmented sort
-  // pinned host staging (batch concatenation and results)
-  void* h_stage = nullptr;
-  size_t h_stage_bytes = 0;
+  // where a staged batch's results land in the context's pinned buffer (upload() carves them; unused by a
+  // single instance, whose results are copied straight to the caller)
+  int32_t* h_rows = nullptr;
+  uint8_t *h_shape = nullptr, *h_warn = nullptr;
   float last_kernel_ms = 0, last_pass_ms = 0;
   int pass_launches = 0;
 };
+using PlanPtr = std::unique_ptr<blance_plan>;
 
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// A batch of one instance is copied between the caller's arrays and the device directly; a larger batch goes
+// through the pinned staging buffer.
+static bool direct(const blance_plan* pl) { return pl->n_inst == 1; }
 
 // sizes, pointers and limits of one instance (no table contents: those are blance_plan_in_check's)
 static int check_structure(const blance_plan_in* in, std::string& why) {
@@ -252,13 +390,10 @@ static int check_structure(const blance_plan_in* in, std::string& why) {
   return BLANCE_OK;
 }
 
-static int validate(blance_ctx* ctx, const blance_plan_in* in, int idx) {
+static void validate(const blance_plan_in* in, int idx) {
   std::string why;
   const int st = check_structure(in, why);
-  if (st == BLANCE_OK) return st;
-  char b[256];
-  std::snprintf(b, sizeof b, "instance %d: %s", idx, why.c_str());
-  return fail(ctx, st, b);
+  if (st != BLANCE_OK) throw_err(st, "instance " + std::to_string(idx) + ": " + why);
 }
 
 /* The contents of the tables, for bindings that do not trust their own marshalling (the planning entry points
@@ -326,15 +461,6 @@ extern "C" int blance_plan_in_check(const blance_plan_in* in, char* msg, int32_t
   return done(BLANCE_OK);
 }
 
-static void plan_release(blance_plan* pl, blance_ctx* ctx = nullptr) {
-  if (!pl) return;
-  if (pl->arena) {
-    if (ctx) cudaFreeAsync(pl->arena, ctx->stream);     // back to the pool (stream ordered)
-    else cudaFree(pl->arena);
-  }
-  delete pl;                         // (the pinned staging buffer belongs to the context)
-}
-
 static int grid_for(const blance_ctx* ctx, long long n, int block) {
   long long want = (n + block - 1) / block;
   long long cap = (long long)ctx->sm_count * 8;      // multiples of the SM count; kernels are grid-stride
@@ -342,13 +468,6 @@ static int grid_for(const blance_ctx* ctx, long long n, int block) {
   if (want < 1) want = 1;
   return (int)want;
 }
-
-// Upload targets of the tables that DPool holds as const (the kernels only read them).
-struct PlanBufs {
-  int32_t *pweight = nullptr, *rank = nullptr, *inst = nullptr, *nw = nullptr, *ef = nullptr, *er = nullptr;
-  uint8_t *rm = nullptr, *ad = nullptr, *hw = nullptr;
-  uint32_t* mask = nullptr;
-};
 
 // Host side of a batch: the per-instance descriptors, their offsets into the pooled arrays and the totals.
 static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off) {
@@ -416,65 +535,28 @@ static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vecto
   }
 }
 
-// The slices of a batch's device arena (sizes from layout()); `b` receives the const-in-DPool ones.
-struct Slice { void** ptr; size_t bytes; };
-static std::vector<Slice> arena_slices(blance_plan* pl, int n, PlanBufs& b) {
-  std::vector<Slice> slices;
+// Adds the device slices of a laid-out batch (sizes from layout()) to an arena.
+static void plan_slices(Arena& a, blance_plan* pl, int n) {
   DPool& P = pl->pool;
   const size_t PT = (size_t)pl->PT + 1, RT = (size_t)pl->RT + 4, NT = (size_t)pl->NT + 1, NUT = (size_t)pl->NUT + 1;
   const size_t CT = (size_t)pl->CT + 1, N2T = (size_t)pl->N2T + 1, MT = (size_t)pl->MT + 1;
   const size_t RRT = (size_t)pl->RRT + 1, RST = (size_t)pl->RST + 1;
-  int32_t *&c_pweight = b.pweight, *&c_rank = b.rank, *&c_inst = b.inst, *&c_nw = b.nw, *&c_ef = b.ef, *&c_er = b.er;
-  uint8_t *&c_rm = b.rm, *&c_ad = b.ad, *&c_hw = b.hw;
-  uint32_t*& c_mask = b.mask;
-#define SL_(p, T, cnt) slices.push_back(Slice{(void**)&(p), sizeof(T) * (cnt)})
-  SL_(P.rows, int32_t, RT); SL_(P.prev_rows, int32_t, RT); SL_(pl->rows_init, int32_t, RT); SL_(pl->prev_rows_init, int32_t, RT);
-  SL_(P.pmeta, uint32_t, PT); SL_(P.prev_meta, uint32_t, PT); SL_(pl->pmeta_init, uint32_t, PT); SL_(pl->prev_meta_init, uint32_t, PT);
-  SL_(P.pflags, uint8_t, PT); SL_(pl->pflags_init, uint8_t, PT);
-  SL_(c_pweight, int32_t, PT); SL_(c_rank, int32_t, PT); SL_(c_inst, int32_t, PT);
-  SL_(P.stream, int32_t, (size_t)pl->ST + 4); SL_(P.ostream, int32_t, (size_t)pl->ST + 4);
-  SL_(P.keys, unsigned long long, PT); SL_(P.keys_alt, unsigned long long, PT); SL_(P.order, int32_t, PT); SL_(P.order_alt, int32_t, PT);
-  SL_(c_rm, uint8_t, NUT); SL_(c_ad, uint8_t, NUT); SL_(c_nw, int32_t, NT); SL_(c_hw, uint8_t, NT);
-  SL_(c_ef, int32_t, NT); SL_(c_er, int32_t, NT);
-  SL_(P.counts, int32_t, CT); SL_(P.n2n, int32_t, N2T); SL_(c_mask, uint32_t, MT);
-  SL_(P.n2n_dev, int32_t, N2T); SL_(P.qstat, int32_t, 4 * PT); SL_(P.srank, uint8_t, PT);
-  SL_(P.pair_keys, unsigned long long, 4 * PT); SL_(P.pair_keys_alt, unsigned long long, 4 * PT);
-  SL_(P.pair_vals, uint32_t, 4 * PT); SL_(P.pair_vals_alt, uint32_t, 4 * PT);
-  SL_(P.insts, DInst, (size_t)n);
-  SL_(pl->raw_a, int32_t, RRT); SL_(pl->raw_b, int32_t, RRT); SL_(pl->rawsh_a, uint8_t, RST); SL_(pl->rawsh_b, uint8_t, RST);
-  SL_(pl->d_raw_rows_off, long long, (size_t)n + 1); SL_(pl->d_raw_shape_off, long long, (size_t)n + 1);
-  SL_(pl->d_seg_off, int, (size_t)n + 1);
-#undef SL_
-  return slices;
-}
-
-static size_t slices_bytes(const std::vector<Slice>& slices) {
-  size_t total = 0;
-  for (auto& s : slices) total += align_up(s.bytes, 256);
-  return total;
-}
-
-// Allocates and carves the arena of a laid-out batch.  On failure the plan is released.
-static int carve_arena(blance_ctx* ctx, blance_plan* pl, int n, PlanBufs& b) {
-  std::vector<Slice> slices = arena_slices(pl, n, b);
-  const size_t total = slices_bytes(slices);
-  // stream-ordered allocation: the context's memory pool keeps the arena of the previous call around
-  cudaError_t e = cudaMallocAsync(&pl->arena, total, ctx->stream);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    plan_release(pl, ctx);
-    return fail(ctx, BLANCE_ERR_NOMEM, std::string("cudaMalloc of the plan arena failed: ") + cudaGetErrorString(e));
-  }
-  pl->arena_bytes = total;
-  {
-    size_t off = 0;
-    for (auto& s : slices) { *s.ptr = (char*)pl->arena + off; off += align_up(s.bytes, 256); }
-  }
-  DPool& P = pl->pool;
-  P.pweight = b.pweight; P.name_rank = b.rank; P.part_inst = b.inst;
-  P.node_removed = b.rm; P.node_added = b.ad; P.node_weight = b.nw; P.node_has_weight = b.hw;
-  P.extra_first = b.ef; P.extra_rest = b.er; P.ie_mask = b.mask;
-  return BLANCE_OK;
+  a.add(P.rows, RT); a.add(P.prev_rows, RT); a.add(pl->rows_init, RT); a.add(pl->prev_rows_init, RT);
+  a.add(P.pmeta, PT); a.add(P.prev_meta, PT); a.add(pl->pmeta_init, PT); a.add(pl->prev_meta_init, PT);
+  a.add(P.pflags, PT); a.add(pl->pflags_init, PT);
+  a.add(P.pweight, PT); a.add(P.name_rank, PT); a.add(P.part_inst, PT);
+  a.add(P.stream, (size_t)pl->ST + 4); a.add(P.ostream, (size_t)pl->ST + 4);
+  a.add(P.keys, PT); a.add(P.keys_alt, PT); a.add(P.order, PT); a.add(P.order_alt, PT);
+  a.add(P.node_removed, NUT); a.add(P.node_added, NUT); a.add(P.node_weight, NT); a.add(P.node_has_weight, NT);
+  a.add(P.extra_first, NT); a.add(P.extra_rest, NT);
+  a.add(P.counts, CT); a.add(P.n2n, N2T); a.add(P.ie_mask, MT);
+  a.add(P.n2n_dev, N2T); a.add(P.qstat, 4 * PT); a.add(P.srank, PT);
+  a.add(P.pair_keys, 4 * PT); a.add(P.pair_keys_alt, 4 * PT);
+  a.add(P.pair_vals, 4 * PT); a.add(P.pair_vals_alt, 4 * PT);
+  a.add(P.insts, (size_t)n);
+  a.add(pl->raw_a, RRT); a.add(pl->raw_b, RRT); a.add(pl->rawsh_a, RST); a.add(pl->rawsh_b, RST);
+  a.add(pl->d_raw_rows_off, (size_t)n + 1); a.add(pl->d_raw_shape_off, (size_t)n + 1);
+  a.add(pl->d_seg_off, (size_t)n + 1);
 }
 
 // Device bytes of the radix sorts' scratch for a batch of PT partitions in n segments (a size query only).
@@ -489,132 +571,109 @@ static size_t sort_scratch_bytes(long long PT, int n, cudaStream_t st) {
   return std::max(need, std::max(need2, need3));
 }
 
-// Grows the context's sort scratch to what the batch needs, then waits for the uploads.  On failure the plan is released.
-static int finish_upload(blance_ctx* ctx, blance_plan* pl) {
+// Grows the context's sort scratch to what the batch needs, then waits for the uploads.
+static void finish_upload(blance_ctx* ctx, const blance_plan* pl) {
   const size_t need = sort_scratch_bytes(pl->PT, pl->n_inst, ctx->stream);
-  cudaError_t e;
   if (need > ctx->cub_tmp_bytes) {
     if (ctx->cub_tmp) cudaFree(ctx->cub_tmp);
     ctx->cub_tmp = nullptr; ctx->cub_tmp_bytes = 0;
-    e = cudaMalloc(&ctx->cub_tmp, need);
-    if (e != cudaSuccess) { cudaGetLastError(); plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the sort scratch failed"); }
+    const cudaError_t e = cudaMalloc(&ctx->cub_tmp, need);
+    if (e != cudaSuccess) { cudaGetLastError(); throw_err(BLANCE_ERR_NOMEM, "cudaMalloc of the sort scratch failed"); }
     ctx->cub_tmp_bytes = need;
   }
-  e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("upload sync failed: ") + cudaGetErrorString(e)); }
-  return BLANCE_OK;
+  CUDA(cudaStreamSynchronize(ctx->stream));
 }
 
-static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan** out_plan) {
-  *out_plan = nullptr;
-  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "batch size must be positive");
-  for (int i = 0; i < n; ++i) {
-    int st = validate(ctx, &ins[i], i);
-    if (st != BLANCE_OK) return st;
+// Host arrays of a batch's node tables, extra counts and hierarchy masks, in the pooled layout of layout().
+struct NodeTables {
+  uint8_t *rm, *ad, *hw;
+  int32_t *nw, *ef, *er;
+  uint32_t* mask;
+};
+
+// Writes instance `in` (descriptor D) into its slices of t.
+static void stage_nodes(const blance_plan_in& in, const DInst& D, const NodeTables& t) {
+  if (D.NU) { std::memcpy(t.rm + D.nodeid_off, in.node_removed, (size_t)D.NU); std::memcpy(t.ad + D.nodeid_off, in.node_added, (size_t)D.NU); }
+  for (int q = 0; q < D.N; ++q) {
+    t.nw[D.node_off + q] = in.has_node_weights ? in.node_weight[q] : 0;
+    t.hw[D.node_off + q] = in.has_node_weights ? in.node_has_weight[q] : 0;
+    t.ef[D.node_off + q] = in.extra_tot_first ? in.extra_tot_first[q] : 0;
+    t.er[D.node_off + q] = in.extra_tot_rest ? in.extra_tot_rest[q] : 0;
   }
-  CK(cudaSetDevice(ctx->device));
-  {
-    cudaError_t stale = cudaGetLastError();      // never let an earlier, unrelated error be blamed on this call
-    if (stale != cudaSuccess) return fail(ctx, BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
-  }
-  blance_plan* pl = new blance_plan();
+  const size_t mw = (size_t)D.n_rules * (D.NU + 1) * D.HW;
+  if (mw) std::memcpy(t.mask + D.mask_off, in.ie_mask, sizeof(uint32_t) * mw);
+}
+
+static uint8_t part_flags(const blance_plan_in& in, int p) {
+  return (uint8_t)((in.part_in_prev[p] ? PF_IN_PREV : 0) | ((in.part_in_prev[p] & 2) ? PF_PREV_EXTRA : 0) |
+                   (in.part_in_assign[p] ? PF_IN_ASSIGN : 0) | (in.part_has_weight[p] ? PF_HAS_WEIGHT : 0));
+}
+
+static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins) {
+  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, "batch size must be positive");
+  for (int i = 0; i < n; ++i) validate(&ins[i], i);
+  PlanPtr pl(new blance_plan());
   std::vector<int> seg_off;
-  layout(pl, n, ins, seg_off);
-  if (pl->PT >= (1LL << 29)) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch"); }
-
-  // ---- carve one device arena ------------------------------------------------------------
-  PlanBufs bufs;
-  {
-    const int st = carve_arena(ctx, pl, n, bufs);
-    if (st != BLANCE_OK) return st;
-  }
+  layout(pl.get(), n, ins, seg_off);
+  if (pl->PT >= (1LL << 29)) throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch");
+  plan_slices(pl->arena, pl.get(), n);
+  pl->arena.alloc(ctx->stream, "the plan arena");
   DPool& P = pl->pool;
-  const size_t PT = (size_t)pl->PT + 1, NT = (size_t)pl->NT + 1, NUT = (size_t)pl->NUT + 1;
-  const size_t MT = (size_t)pl->MT + 1, RRT = (size_t)pl->RRT + 1, RST = (size_t)pl->RST + 1;
-  const int32_t *c_pweight = bufs.pweight, *c_rank = bufs.rank, *c_inst = bufs.inst, *c_nw = bufs.nw, *c_ef = bufs.ef, *c_er = bufs.er;
-  const uint8_t *c_rm = bufs.rm, *c_ad = bufs.ad, *c_hw = bufs.hw;
-  const uint32_t* c_mask = bufs.mask;
-  cudaError_t e = cudaSuccess;
 
-  // ---- host side of the copy.  A batch is concatenated in caller layout into one pinned staging buffer;
-  // a single instance is copied straight from the caller's arrays (no staging, no pinned allocation).
-  const bool direct = (n == 1);
+  // ---- host side of the copy: a single instance straight from the caller's arrays, a batch concatenated in
+  // caller layout into the context's pinned staging buffer
   const int32_t *h_cur = nullptr, *h_prev = nullptr, *h_pw = nullptr, *h_rank = nullptr, *h_inst = nullptr;
   const int32_t *h_nw = nullptr, *h_ef = nullptr, *h_er = nullptr;
   const uint8_t *h_csh = nullptr, *h_psh = nullptr, *h_flags = nullptr, *h_rm = nullptr, *h_ad = nullptr, *h_hw = nullptr;
   const uint32_t* h_mask = nullptr;
   std::vector<uint8_t> v_flags;
-  if (direct) {
+  if (direct(pl.get())) {
     const blance_plan_in& in = ins[0];
-    const DInst& D = pl->h_insts[0];
-    v_flags.resize((size_t)D.PU + 1);
-    for (int p = 0; p < D.PU; ++p)
-      v_flags[p] = (uint8_t)((in.part_in_prev[p] ? PF_IN_PREV : 0) | ((in.part_in_prev[p] & 2) ? PF_PREV_EXTRA : 0) | (in.part_in_assign[p] ? PF_IN_ASSIGN : 0) |
-                             (in.part_has_weight[p] ? PF_HAS_WEIGHT : 0));
+    v_flags.resize((size_t)in.n_parts + 1);
+    for (int p = 0; p < in.n_parts; ++p) v_flags[(size_t)p] = part_flags(in, p);
     h_cur = in.cur_rows; h_prev = in.prev_rows; h_csh = in.cur_shape; h_psh = in.prev_shape;
     h_flags = v_flags.data(); h_pw = in.part_weight; h_rank = in.part_name_rank;     // h_inst stays NULL: all zero
     h_rm = in.node_removed; h_ad = in.node_added;
     if (in.has_node_weights) { h_nw = in.node_weight; h_hw = in.node_has_weight; }
     h_ef = in.extra_tot_first; h_er = in.extra_tot_rest; h_mask = in.ie_mask;
   } else {
-  const size_t stage_bytes = align_up(sizeof(int32_t) * RRT, 256) * 2 + align_up(RST, 256) * 2 + align_up(PT, 256) +
-                             align_up(sizeof(int32_t) * PT, 256) * 3 + align_up(NUT, 256) * 2 +
-                             align_up(sizeof(int32_t) * NT, 256) * 3 + align_up(NT, 256) + align_up(sizeof(uint32_t) * MT, 256);
-  if (stage_bytes > ctx->h_stage_bytes) {          // grow-only, kept by the context between calls
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-    ctx->h_stage = nullptr; ctx->h_stage_bytes = 0;
-    e = cudaMallocHost(&ctx->h_stage, stage_bytes + stage_bytes / 4);
-    if (e != cudaSuccess) {
-      plan_release(pl, ctx);
-      return fail(ctx, BLANCE_ERR_NOMEM, std::string("cudaMallocHost of the staging buffer failed: ") + cudaGetErrorString(e));
+    const size_t PT = (size_t)pl->PT + 1, NT = (size_t)pl->NT + 1, NUT = (size_t)pl->NUT + 1;
+    const size_t MT = (size_t)pl->MT + 1, RRT = (size_t)pl->RRT + 1, RST = (size_t)pl->RST + 1;
+    int32_t *s_cur, *s_prev, *s_pw, *s_rank, *s_inst;
+    uint8_t *s_csh, *s_psh, *s_flags;
+    NodeTables s;
+    Arena stage;                // carved over the pinned buffer; fetch() reads the results from s_cur / s_csh / s_psh
+    stage.add(s_cur, RRT); stage.add(s_prev, RRT); stage.add(s_csh, RST); stage.add(s_psh, RST);
+    stage.add(s_flags, PT); stage.add(s_pw, PT); stage.add(s_rank, PT); stage.add(s_inst, PT);
+    stage.add(s.rm, NUT); stage.add(s.ad, NUT); stage.add(s.nw, NT); stage.add(s.ef, NT); stage.add(s.er, NT);
+    stage.add(s.hw, NT); stage.add(s.mask, MT);
+    const size_t stage_bytes = stage.bytes();
+    if (stage_bytes > ctx->h_stage_bytes) {          // grow-only, kept by the context between calls
+      if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
+      ctx->h_stage = nullptr; ctx->h_stage_bytes = 0;
+      const cudaError_t e = cudaMallocHost(&ctx->h_stage, stage_bytes + stage_bytes / 4);
+      if (e != cudaSuccess)
+        throw_err(BLANCE_ERR_NOMEM, std::string("cudaMallocHost of the staging buffer failed: ") + cudaGetErrorString(e));
+      ctx->h_stage_bytes = stage_bytes + stage_bytes / 4;
     }
-    ctx->h_stage_bytes = stage_bytes + stage_bytes / 4;
-  }
-  pl->h_stage = ctx->h_stage;
-  pl->h_stage_bytes = stage_bytes;
-  char* hp = (char*)pl->h_stage;
-  auto carve = [&](size_t bytes) { char* r = hp; hp += align_up(bytes, 256); return r; };
-  int32_t* s_cur = (int32_t*)carve(sizeof(int32_t) * RRT);
-  int32_t* s_prev = (int32_t*)carve(sizeof(int32_t) * RRT);
-  uint8_t* s_csh = (uint8_t*)carve(RST);
-  uint8_t* s_psh = (uint8_t*)carve(RST);
-  uint8_t* s_flags = (uint8_t*)carve(PT);
-  int32_t* s_pw = (int32_t*)carve(sizeof(int32_t) * PT);
-  int32_t* s_rank = (int32_t*)carve(sizeof(int32_t) * PT);
-  int32_t* s_inst = (int32_t*)carve(sizeof(int32_t) * PT);
-  uint8_t* s_rm = (uint8_t*)carve(NUT);
-  uint8_t* s_ad = (uint8_t*)carve(NUT);
-  int32_t* s_nw = (int32_t*)carve(sizeof(int32_t) * NT);
-  int32_t* s_ef = (int32_t*)carve(sizeof(int32_t) * NT);
-  int32_t* s_er = (int32_t*)carve(sizeof(int32_t) * NT);
-  uint8_t* s_hw = (uint8_t*)carve(NT);
-  uint32_t* s_mask = (uint32_t*)carve(sizeof(uint32_t) * MT);
-  auto stage_one = [&](int i) {
-    const blance_plan_in& in = ins[i];
-    const DInst& D = pl->h_insts[i];
-    const size_t rr = (size_t)D.PU * D.SL, rs = (size_t)D.PU * D.S;
-    if (rr) { std::memcpy(s_cur + pl->raw_rows_off[i], in.cur_rows, sizeof(int32_t) * rr);
-              std::memcpy(s_prev + pl->raw_rows_off[i], in.prev_rows, sizeof(int32_t) * rr); }
-    if (rs) { std::memcpy(s_csh + pl->raw_shape_off[i], in.cur_shape, rs); std::memcpy(s_psh + pl->raw_shape_off[i], in.prev_shape, rs); }
-    for (int p = 0; p < D.PU; ++p) {
-      const size_t g = (size_t)D.part_off + p;
-      s_flags[g] = (uint8_t)((in.part_in_prev[p] ? PF_IN_PREV : 0) | ((in.part_in_prev[p] & 2) ? PF_PREV_EXTRA : 0) | (in.part_in_assign[p] ? PF_IN_ASSIGN : 0) |
-                             (in.part_has_weight[p] ? PF_HAS_WEIGHT : 0));
-      s_pw[g] = in.part_weight[p];
-      s_rank[g] = in.part_name_rank[p];
-      s_inst[g] = i;
-    }
-    if (D.NU) { std::memcpy(s_rm + D.nodeid_off, in.node_removed, D.NU); std::memcpy(s_ad + D.nodeid_off, in.node_added, D.NU); }
-    for (int q = 0; q < D.N; ++q) {
-      s_nw[D.node_off + q] = in.has_node_weights ? in.node_weight[q] : 0;
-      s_hw[D.node_off + q] = in.has_node_weights ? in.node_has_weight[q] : 0;
-      s_ef[D.node_off + q] = in.extra_tot_first ? in.extra_tot_first[q] : 0;
-      s_er[D.node_off + q] = in.extra_tot_rest ? in.extra_tot_rest[q] : 0;
-    }
-    const size_t mw = (size_t)D.n_rules * (D.NU + 1) * D.HW;
-    if (mw) std::memcpy(s_mask + D.mask_off, in.ie_mask, sizeof(uint32_t) * mw);
-  };
-  {
+    stage.carve(ctx->h_stage);
+    pl->h_rows = s_cur; pl->h_shape = s_csh; pl->h_warn = s_psh;
+    auto stage_one = [&](int i) {
+      const blance_plan_in& in = ins[i];
+      const DInst& D = pl->h_insts[i];
+      const size_t rr = (size_t)D.PU * D.SL, rs = (size_t)D.PU * D.S;
+      if (rr) { std::memcpy(s_cur + pl->raw_rows_off[i], in.cur_rows, sizeof(int32_t) * rr);
+                std::memcpy(s_prev + pl->raw_rows_off[i], in.prev_rows, sizeof(int32_t) * rr); }
+      if (rs) { std::memcpy(s_csh + pl->raw_shape_off[i], in.cur_shape, rs); std::memcpy(s_psh + pl->raw_shape_off[i], in.prev_shape, rs); }
+      for (int p = 0; p < D.PU; ++p) {
+        const size_t g = (size_t)D.part_off + p;
+        s_flags[g] = part_flags(in, p);
+        s_pw[g] = in.part_weight[p];
+        s_rank[g] = in.part_name_rank[p];
+        s_inst[g] = i;
+      }
+      stage_nodes(in, D, s);
+    };
     // instances are staged by a few host threads (a 1 024-instance fan-out is ~1 M partitions of flag packing)
     int T = (int)std::min<long long>(8, std::max<long long>(1, pl->PT / 65536));
     T = std::min(T, std::max(1, (int)std::thread::hardware_concurrency()));
@@ -624,46 +683,37 @@ static int upload(blance_ctx* ctx, int n, const blance_plan_in* ins, blance_plan
       for (int t = 0; t < T; ++t) th.emplace_back([&, t]() { for (int i = t; i < n; i += T) stage_one(i); });
       for (auto& x : th) x.join();
     }
-  }
-  h_cur = s_cur; h_prev = s_prev; h_csh = s_csh; h_psh = s_psh; h_flags = s_flags; h_pw = s_pw; h_rank = s_rank;
-  h_inst = s_inst; h_rm = s_rm; h_ad = s_ad; h_nw = s_nw; h_hw = s_hw; h_ef = s_ef; h_er = s_er; h_mask = s_mask;
+    h_cur = s_cur; h_prev = s_prev; h_csh = s_csh; h_psh = s_psh; h_flags = s_flags; h_pw = s_pw; h_rank = s_rank;
+    h_inst = s_inst; h_rm = s.rm; h_ad = s.ad; h_nw = s.nw; h_hw = s.hw; h_ef = s.ef; h_er = s.er; h_mask = s.mask;
   }
   cudaStream_t st = ctx->stream;
-#define H2D(dst, src, bytes) do { if ((bytes) > 0) { \
-    e = (src) ? cudaMemcpyAsync((void*)(dst), (src), (bytes), cudaMemcpyHostToDevice, st) : cudaMemsetAsync((void*)(dst), 0, (bytes), st); \
-    if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("H2D copy failed: ") + cudaGetErrorString(e)); } } } while (0)
-  H2D(pl->raw_a, h_cur, sizeof(int32_t) * (size_t)pl->RRT); H2D(pl->raw_b, h_prev, sizeof(int32_t) * (size_t)pl->RRT);
-  H2D(pl->rawsh_a, h_csh, (size_t)pl->RST); H2D(pl->rawsh_b, h_psh, (size_t)pl->RST);
-  H2D(pl->pflags_init, h_flags, (size_t)pl->PT); H2D(c_pweight, h_pw, sizeof(int32_t) * (size_t)pl->PT);
-  H2D(c_rank, h_rank, sizeof(int32_t) * (size_t)pl->PT); H2D(c_inst, h_inst, sizeof(int32_t) * (size_t)pl->PT);
-  H2D(c_rm, h_rm, (size_t)pl->NUT); H2D(c_ad, h_ad, (size_t)pl->NUT);
-  H2D(c_nw, h_nw, sizeof(int32_t) * (size_t)pl->NT); H2D(c_hw, h_hw, (size_t)pl->NT);
-  H2D(c_ef, h_ef, sizeof(int32_t) * (size_t)pl->NT); H2D(c_er, h_er, sizeof(int32_t) * (size_t)pl->NT);
-  H2D(c_mask, h_mask, sizeof(uint32_t) * (size_t)pl->MT);
-  H2D(P.insts, pl->h_insts.data(), sizeof(DInst) * (size_t)n);
-  H2D(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(n + 1));
-  H2D(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(n + 1));
-  H2D(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(n + 1));
-#undef H2D
+  auto h2d = [&](const void* dst, const void* src, size_t bytes) {      // a NULL source uploads zeros
+    if (bytes > 0)
+      cuda_check(src ? cudaMemcpyAsync((void*)dst, src, bytes, cudaMemcpyHostToDevice, st) : cudaMemsetAsync((void*)dst, 0, bytes, st), "H2D copy");
+  };
+  h2d(pl->raw_a, h_cur, sizeof(int32_t) * (size_t)pl->RRT); h2d(pl->raw_b, h_prev, sizeof(int32_t) * (size_t)pl->RRT);
+  h2d(pl->rawsh_a, h_csh, (size_t)pl->RST); h2d(pl->rawsh_b, h_psh, (size_t)pl->RST);
+  h2d(pl->pflags_init, h_flags, (size_t)pl->PT); h2d(P.pweight, h_pw, sizeof(int32_t) * (size_t)pl->PT);
+  h2d(P.name_rank, h_rank, sizeof(int32_t) * (size_t)pl->PT); h2d(P.part_inst, h_inst, sizeof(int32_t) * (size_t)pl->PT);
+  h2d(P.node_removed, h_rm, (size_t)pl->NUT); h2d(P.node_added, h_ad, (size_t)pl->NUT);
+  h2d(P.node_weight, h_nw, sizeof(int32_t) * (size_t)pl->NT); h2d(P.node_has_weight, h_hw, (size_t)pl->NT);
+  h2d(P.extra_first, h_ef, sizeof(int32_t) * (size_t)pl->NT); h2d(P.extra_rest, h_er, sizeof(int32_t) * (size_t)pl->NT);
+  h2d(P.ie_mask, h_mask, sizeof(uint32_t) * (size_t)pl->MT);
+  h2d(P.insts, pl->h_insts.data(), sizeof(DInst) * (size_t)n);
+  h2d(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(n + 1));
+  h2d(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(n + 1));
+  h2d(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(n + 1));
   // device layout of the rows / shapes, into the *_init copies via the working arrays
   if (pl->PT > 0) {
-    k_unpack<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(P, pl->raw_a, pl->raw_b, pl->rawsh_a, pl->rawsh_b,
-                                                        pl->d_raw_rows_off, pl->d_raw_shape_off, pl->PT);
-    ctx->launches++;
-    e = cudaGetLastError();
-    if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("k_unpack launch failed: ") + cudaGetErrorString(e)); }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(pl->rows_init, P.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(pl->prev_rows_init, P.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(pl->pmeta_init, P.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) { plan_release(pl, ctx); return fail(ctx, BLANCE_ERR_CUDA, std::string("upload failed: ") + cudaGetErrorString(e)); }
+    launch(ctx, k_unpack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->raw_b, pl->rawsh_a, pl->rawsh_b,
+           pl->d_raw_rows_off, pl->d_raw_shape_off, pl->PT);
+    CUDA(cudaMemcpyAsync(pl->rows_init, P.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_rows_init, P.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->pmeta_init, P.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
   }
-  {
-    const int rc = finish_upload(ctx, pl);
-    if (rc != BLANCE_OK) return rc;
-  }
-  *out_plan = pl;
-  return BLANCE_OK;
+  finish_upload(ctx, pl.get());
+  return pl;
 }
 
 static cudaEvent_t get_event(blance_ctx* ctx, size_t idx) {
@@ -675,53 +725,27 @@ static cudaEvent_t get_event(blance_ctx* ctx, size_t idx) {
   return ctx->events[idx];
 }
 
-template <int NPT, int MAXT>
-static void launch_pass(const DPool& P, int n_inst, int T, int s, bool hier, cudaStream_t st) {
-  if (hier) k_assign_pass<NPT, true, MAXT><<<n_inst, T, 0, st>>>(P, s);
-  else k_assign_pass<NPT, false, MAXT><<<n_inst, T, 0, st>>>(P, s);
-}
-
-// the sequencer variant, one instantiation per constraint count K; CTAs whose instance picked the other
-// kernel (or has a different K for this state) exit at once
-template <int NPT, int K, int MAXT>
-static cudaError_t launch_pass_seq_k(size_t* configured, const DPool& P, int n_inst, int TC, int W, int s, size_t dyn, cudaStream_t st) {
-  {
-    std::lock_guard<std::mutex> g(g_seq_dyn_mu);
-    if (dyn > *configured) {
-      cudaError_t e = cudaFuncSetAttribute(k_assign_pass_seq<NPT, K, MAXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-      if (e != cudaSuccess) return e;
-      *configured = dyn;
-    }
+// Calls f(std::integral_constant<int, NPT>()) for the pass kernel's nodes per thread npt (1, 2, 4, 8 or 16).
+template <class F>
+static void dispatch_npt(int npt, F&& f) {
+  switch (npt) {
+    case 1: f(std::integral_constant<int, 1>()); break;
+    case 2: f(std::integral_constant<int, 2>()); break;
+    case 4: f(std::integral_constant<int, 4>()); break;
+    case 8: f(std::integral_constant<int, 8>()); break;
+    default: f(std::integral_constant<int, 16>()); break;
   }
-  k_assign_pass_seq<NPT, K, MAXT><<<n_inst, TC + 32 * W, dyn, st>>>(P, s, TC);
-  return cudaSuccess;
 }
 
-// kmask: bit K set when some instance of the batch has constraints == K for state s
-template <int NPT, int MAXT>
-static cudaError_t launch_pass_seq(size_t* configured, const DPool& P, int n_inst, int TC, int W, int s, int max_n, unsigned kmask, cudaStream_t st) {
-  const size_t dyn = seq_dyn_smem_bytes(max_n, W);
-  cudaError_t e = cudaSuccess;
-  if (e == cudaSuccess && (kmask & 2u)) e = launch_pass_seq_k<NPT, 1, MAXT>(configured + 0, P, n_inst, TC, W, s, dyn, st);
-  if (e == cudaSuccess && (kmask & 4u)) e = launch_pass_seq_k<NPT, 2, MAXT>(configured + 1, P, n_inst, TC, W, s, dyn, st);
-  if (e == cudaSuccess && (kmask & 8u)) e = launch_pass_seq_k<NPT, 3, MAXT>(configured + 2, P, n_inst, TC, W, s, dyn, st);
-  if (e == cudaSuccess && (kmask & 16u)) e = launch_pass_seq_k<NPT, 4, MAXT>(configured + 3, P, n_inst, TC, W, s, dyn, st);
-  return e;
-}
-
-// the speculative variant, one instantiation per constraint count K (CTAs of other modes / other K exit at once)
-template <int K>
-static cudaError_t launch_pass_spec_k(size_t* configured, const DPool& P, int n_inst, int nw, int sw, unsigned idle_mask, int shift, int s, size_t dyn, cudaStream_t st) {
-  {
-    std::lock_guard<std::mutex> g(g_seq_dyn_mu);
-    if (dyn > *configured) {
-      cudaError_t e = cudaFuncSetAttribute(k_assign_pass_spec<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-      if (e != cudaSuccess) return e;
-      *configured = dyn;
-    }
-  }
-  k_assign_pass_spec<K><<<n_inst, 32 * nw, dyn, st>>>(P, s, sw, idle_mask, shift);
-  return cudaSuccess;
+// Calls f(std::integral_constant<int, K>()) for K = 1 .. 4 in ascending order where bit K of kmask is set: the
+// sequencer and speculative kernels have one instantiation per constraint count K.  CTAs whose instance picked
+// another kernel (or has a different K for this state) exit at once.
+template <class F>
+static void for_each_k(unsigned kmask, F&& f) {
+  if (kmask & 2u) f(std::integral_constant<int, 1>());
+  if (kmask & 4u) f(std::integral_constant<int, 2>());
+  if (kmask & 8u) f(std::integral_constant<int, 3>());
+  if (kmask & 16u) f(std::integral_constant<int, 4>());
 }
 
 static int next_pow2(int v) { int p = 1; while (p < v) p <<= 1; return p; }
@@ -730,7 +754,6 @@ static int next_pow2(int v) { int p = 1; while (p < v) p <<= 1; return p; }
 // thread for the pass kernel.  The chain is latency bound, so prefer many warps with few nodes each.
 static void pass_shape(int max_n, int* TC, int* npt) {
   int want = max_n > 512 ? 2 : 1;
-  if (const char* e = getenv("BLANCE_PASS_NPT")) { int v = atoi(e); if (v == 1 || v == 2 || v == 4 || v == 8) want = v; }
   if (max_n > 3968) want = 8;
   int t = next_pow2((std::max(1, max_n) + want - 1) / want);
   if (t < 32) t = 32;
@@ -740,21 +763,20 @@ static void pass_shape(int max_n, int* TC, int* npt) {
   *TC = t;
 }
 
-static int run(blance_ctx* ctx, blance_plan* pl) {
-  CK(cudaSetDevice(ctx->device));
+static void run(blance_ctx* ctx, blance_plan* pl) {
   cudaStream_t st = ctx->stream;
   DPool& P = pl->pool;
   const int n = pl->n_inst;
   // restore the mutable state
   if (pl->PT > 0) {
-    CK(cudaMemcpyAsync(P.rows, pl->rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(P.prev_rows, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(P.pmeta, pl->pmeta_init, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(P.prev_meta, pl->prev_meta_init, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(P.pflags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(P.rows, pl->rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(P.prev_rows, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(P.pmeta, pl->pmeta_init, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(P.prev_meta, pl->prev_meta_init, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(P.pflags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
   }
-  CK(cudaMemcpyAsync(P.insts, pl->h_insts.data(), sizeof(DInst) * (size_t)n, cudaMemcpyHostToDevice, st));
-  CK(cudaEventRecord(ctx->ev[1], st));
+  CUDA(cudaMemcpyAsync(P.insts, pl->h_insts.data(), sizeof(DInst) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CUDA(cudaEventRecord(ctx->ev[1], st));
 
   int T = 32, npt = 1;
   pass_shape(pl->max_N, &T, &npt);
@@ -766,38 +788,32 @@ static int run(blance_ctx* ctx, blance_plan* pl) {
   const int grid = grid_for(ctx, pl->PT, blk);
   size_t n_ev = 0;
   pl->pass_launches = 0;
-  const bool smem_hist = (n == 1) && ((size_t)pl->h_insts[0].S * pl->h_insts[0].N * sizeof(int32_t) <= 40 * 1024);
+  const size_t hist_smem = (size_t)pl->h_insts[0].S * pl->h_insts[0].N * sizeof(int32_t);
+  const bool smem_hist = (n == 1) && hist_smem <= 40 * 1024;
   int guard = 0;
   while (any_active > 0) {
-    if (++guard > 100000) return fail(ctx, BLANCE_ERR_CUDA, "convergence loop did not terminate");
+    if (++guard > 100000) throw_err(BLANCE_ERR_CUDA, "convergence loop did not terminate");
     if (pl->PT == 0) {          // no partitions at all: the loop of plan.go:32-45 still runs once and matches
-      CK(cudaMemsetAsync(ctx->d_any_active, 0, sizeof(int), st));
-      k_next_iter<<<(n + 127) / 128, 128, 0, st>>>(P, n, ctx->d_any_active);
-      ctx->launches++;
+      CUDA(cudaMemsetAsync(ctx->d_any_active, 0, sizeof(int), st));
+      launch(ctx, k_next_iter, (n + 127) / 128, 128, 0, P, n, ctx->d_any_active);
       break;
     }
-    k_prepare_rows<<<grid, blk, 0, st>>>(P, pl->PT);
-    ctx->launches += 2;   // + k_count_prev below
-    CK(cudaMemsetAsync(P.counts, 0, sizeof(int32_t) * (size_t)(pl->CT + 1), st));
-    if (smem_hist)
-      k_count_prev<true><<<std::min(grid, ctx->sm_count * 2), blk, (size_t)pl->h_insts[0].S * pl->h_insts[0].N * sizeof(int32_t), st>>>(P, pl->PT);
-    else
-      k_count_prev<false><<<grid, blk, 0, st>>>(P, pl->PT);
+    launch(ctx, k_prepare_rows, grid, blk, 0, P, pl->PT);
+    CUDA(cudaMemsetAsync(P.counts, 0, sizeof(int32_t) * (size_t)(pl->CT + 1), st));
+    if (smem_hist) launch(ctx, k_count_prev<true>, std::min(grid, ctx->sm_count * 2), blk, hist_smem, P, pl->PT);
+    else launch(ctx, k_count_prev<false>, grid, blk, 0, P, pl->PT);
     for (int s = 0; s < pl->max_S; ++s) {
       if (!pl->any_state_active[s]) continue;
-      k_build_keys<<<grid, blk, 0, st>>>(P, s, pl->PT);
-      ctx->launches += 2;   // + k_assign_pass below
+      launch(ctx, k_build_keys, grid, blk, 0, P, s, pl->PT);
       size_t tmp = ctx->cub_tmp_bytes;
       if (n == 1)
-        CK(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp, tmp, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT, 0, 64, st));
+        CUDA(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp, tmp, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT, 0, 64, st));
       else
-        CK(cub::DeviceSegmentedRadixSort::SortPairs(ctx->cub_tmp, tmp, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT,
-                                                    n, pl->d_seg_off, pl->d_seg_off + 1, 0, 64, st));
-      k_gather_stream<<<grid, blk, 0, st>>>(P, s, pl->PT);
+        CUDA(cub::DeviceSegmentedRadixSort::SortPairs(ctx->cub_tmp, tmp, P.keys_alt, P.keys, P.order_alt, P.order, (int)pl->PT,
+                                                      n, pl->d_seg_off, pl->d_seg_off + 1, 0, 64, st));
+      launch(ctx, k_gather_stream, grid, blk, 0, P, s, pl->PT);
       unsigned kmask = 0;
       for (int i = 0; i < n; ++i) { const int kk = pl->h_insts[i].S > s ? pl->h_insts[i].state_constraints[s] : 0; if (kk >= 1 && kk <= 4) kmask |= 1u << kk; }
-      // speculative kernel: 9 scout warps + the leader (warps 4 and 8 stay away from the leader's scheduler) when the
-      // GPU has SMs to spare, 3 scouts per CTA for wide batches
       // speculative kernel: warp 0 leads, 9 scout warps (warps 4 and 8 exit at once: the leader has its scheduler to
       // itself) when the GPU has SMs to spare; leader + 3 scouts per CTA for wide batches
       const bool spec_wide = 2 * n <= ctx->sm_count;
@@ -808,67 +824,59 @@ static int run(blance_ctx* ctx, blance_plan* pl) {
       bool any_auto = false;
       for (int i = 0; i < n; ++i) any_auto |= pl->h_insts[i].engine == BLANCE_ENGINE_AUTO;
       const bool spec_allowed = any_auto && kmask != 0 && pl->pair_end_bit <= 62 && !getenv("BLANCE_NO_SPEC");
-      k_pick_mode<<<(n + 127) / 128, 128, 0, st>>>(P, s, n, (npt <= 8 && !getenv("BLANCE_NO_SEQ")) ? 1 : 0, spec_allowed ? 1 : 0, spec_max_n);
+      launch(ctx, k_pick_mode, (n + 127) / 128, 128, 0, P, s, n, (npt <= 8 && !getenv("BLANCE_NO_SEQ")) ? 1 : 0,
+             spec_allowed ? 1 : 0, spec_max_n);
       if (spec_allowed) {
         // the all-sticky hypothesis counts (qstat) of the instances that picked the speculative kernel
-        k_pair_keys<<<grid, blk, 0, st>>>(P, s, pl->PT, pl->pair_inst_shift);
+        launch(ctx, k_pair_keys, grid, blk, 0, P, s, pl->PT, pl->pair_inst_shift);
         size_t tmp2 = ctx->cub_tmp_bytes;
-        CK(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp, tmp2, P.pair_keys_alt, P.pair_keys, P.pair_vals_alt, P.pair_vals,
-                                           (int)(4 * pl->PT), 0, pl->pair_end_bit + 1, st));
-        k_pair_rank<<<grid_for(ctx, 4 * pl->PT, blk), blk, 0, st>>>(P, 4 * pl->PT);
-        CK(cudaMemsetAsync(P.n2n_dev, 0, sizeof(int32_t) * (size_t)(pl->N2T + 1), st));
-        ctx->launches += 2;
+        CUDA(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp, tmp2, P.pair_keys_alt, P.pair_keys, P.pair_vals_alt, P.pair_vals,
+                                             (int)(4 * pl->PT), 0, pl->pair_end_bit + 1, st));
+        launch(ctx, k_pair_rank, grid_for(ctx, 4 * pl->PT, blk), blk, 0, P, 4 * pl->PT);
+        CUDA(cudaMemsetAsync(P.n2n_dev, 0, sizeof(int32_t) * (size_t)(pl->N2T + 1), st));
       }
-      CK(cudaMemsetAsync(P.n2n, 0, sizeof(int32_t) * (size_t)(pl->N2T + 1), st));     // plan.go:266
+      CUDA(cudaMemsetAsync(P.n2n, 0, sizeof(int32_t) * (size_t)(pl->N2T + 1), st));     // plan.go:266
       cudaEvent_t e0 = get_event(ctx, n_ev), e1 = get_event(ctx, n_ev + 1);
-      if (e0 && e1 && n_ev < 256) CK(cudaEventRecord(e0, st));
-      if (npt == 1) launch_pass<1, 544>(P, n, T + 32, s, any_hier, st);
-      else if (npt == 2) launch_pass<2, 544>(P, n, T + 32, s, any_hier, st);
-      else if (npt == 4) launch_pass<4, 544>(P, n, T + 32, s, any_hier, st);
-      else if (npt == 8) launch_pass<8, 544>(P, n, T + 32, s, any_hier, st);
-      else launch_pass<16, 544>(P, n, T + 32, s, any_hier, st);
-      cudaError_t se = cudaSuccess;
+      if (e0 && e1 && n_ev < 256) CUDA(cudaEventRecord(e0, st));
       // sequencer warps per CTA: wide windows when the GPU has SMs to spare, one warp for wide batches
-      int seq_w = (2 * n <= ctx->sm_count) ? SEQ_W_MAX : 1;
-      if (const char* ev = getenv("BLANCE_SEQ_W")) { const int v = atoi(ev); if (v >= 1 && v <= SEQ_W_MAX) seq_w = v; }   // experiments
-      if (npt == 1) se = (launch_pass_seq<1, 640>)(g_seq_dyn[ctx->device & 63][0], P, n, T, seq_w, s, pl->max_N, kmask, st);
-      else if (npt == 2) se = (launch_pass_seq<2, 640>)(g_seq_dyn[ctx->device & 63][1], P, n, T, seq_w, s, pl->max_N, kmask, st);
-      else if (npt == 4) se = (launch_pass_seq<4, 640>)(g_seq_dyn[ctx->device & 63][2], P, n, T, seq_w, s, pl->max_N, kmask, st);
-      else if (npt == 8) se = (launch_pass_seq<8, 640>)(g_seq_dyn[ctx->device & 63][3], P, n, T, seq_w, s, pl->max_N, kmask, st);
-      CK(se);
-      CK(cudaGetLastError());
-      ctx->launches += 1 + (npt <= 8 ? __builtin_popcount(kmask) : 0);   // k_pick_mode + the sequencer kernel(s)
+      const int seq_w = (2 * n <= ctx->sm_count) ? SEQ_W_MAX : 1;
+      dispatch_npt(npt, [&](auto npt_c) {
+        constexpr int NPT = decltype(npt_c)::value;
+        launch(ctx, any_hier ? k_assign_pass<NPT, true, 544> : k_assign_pass<NPT, false, 544>, n, T + 32, 0, P, s);
+        if constexpr (NPT <= 8) {
+          const size_t dyn = seq_dyn_smem_bytes(pl->max_N, seq_w);
+          for_each_k(kmask, [&](auto k_c) {
+            constexpr int K = decltype(k_c)::value;
+            opt_in_smem((const void*)k_assign_pass_seq<NPT, K, 640>, &g_seq_dyn[ctx->device & 63][__builtin_ctz(NPT)][K - 1], dyn);
+            launch(ctx, k_assign_pass_seq<NPT, K, 640>, n, T + 32 * seq_w, dyn, P, s, T);
+          });
+        }
+      });
       if (spec_allowed) {
         const size_t sdyn = spec_dyn_smem_bytes(std::min(pl->max_N, spec_max_n), spec_sw);
-        size_t* cfgd = g_spec_dyn[ctx->device & 63];
-        cudaError_t pe = cudaSuccess;
-        if (pe == cudaSuccess && (kmask & 2u)) pe = launch_pass_spec_k<1>(cfgd + 0, P, n, spec_nw, spec_sw, spec_idle, spec_shift, s, sdyn, st);
-        if (pe == cudaSuccess && (kmask & 4u)) pe = launch_pass_spec_k<2>(cfgd + 1, P, n, spec_nw, spec_sw, spec_idle, spec_shift, s, sdyn, st);
-        if (pe == cudaSuccess && (kmask & 8u)) pe = launch_pass_spec_k<3>(cfgd + 2, P, n, spec_nw, spec_sw, spec_idle, spec_shift, s, sdyn, st);
-        if (pe == cudaSuccess && (kmask & 16u)) pe = launch_pass_spec_k<4>(cfgd + 3, P, n, spec_nw, spec_sw, spec_idle, spec_shift, s, sdyn, st);
-        CK(pe);
-        ctx->launches += __builtin_popcount(kmask);
+        for_each_k(kmask, [&](auto k_c) {
+          constexpr int K = decltype(k_c)::value;
+          opt_in_smem((const void*)k_assign_pass_spec<K>, &g_spec_dyn[ctx->device & 63][K - 1], sdyn);
+          launch(ctx, k_assign_pass_spec<K>, n, 32 * spec_nw, sdyn, P, s, spec_sw, spec_idle, spec_shift);
+        });
       }
-      CK(cudaGetLastError());
-      if (e0 && e1 && n_ev < 256) { CK(cudaEventRecord(e1, st)); n_ev += 2; }
+      if (e0 && e1 && n_ev < 256) { CUDA(cudaEventRecord(e1, st)); n_ev += 2; }
       pl->pass_launches++;
-      k_scatter_stream<<<grid, blk, 0, st>>>(P, s, pl->PT);
-      ctx->launches += 2;   // gather + scatter
+      launch(ctx, k_scatter_stream, grid, blk, 0, P, s, pl->PT);
     }
-    k_compare<<<grid, blk, 0, st>>>(P, pl->PT);
-    ctx->launches += 3;   // + k_commit, k_next_iter
-    k_commit<<<grid, blk, 0, st>>>(P, pl->PT);
-    CK(cudaMemsetAsync(ctx->d_any_active, 0, sizeof(int), st));
-    k_next_iter<<<(n + 127) / 128, 128, 0, st>>>(P, n, ctx->d_any_active);
-    CK(cudaMemcpyAsync(ctx->h_any_active, ctx->d_any_active, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
+    launch(ctx, k_compare, grid, blk, 0, P, pl->PT);
+    launch(ctx, k_commit, grid, blk, 0, P, pl->PT);
+    CUDA(cudaMemsetAsync(ctx->d_any_active, 0, sizeof(int), st));
+    launch(ctx, k_next_iter, (n + 127) / 128, 128, 0, P, n, ctx->d_any_active);
+    CUDA(cudaMemcpyAsync(ctx->h_any_active, ctx->d_any_active, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    CUDA(cudaGetLastError());
     any_active = *ctx->h_any_active;
   }
-  CK(cudaEventRecord(ctx->ev[2], st));
-  CK(cudaStreamSynchronize(st));
+  CUDA(cudaEventRecord(ctx->ev[2], st));
+  CUDA(cudaStreamSynchronize(st));
   float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
+  CUDA(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
   pl->last_kernel_ms = ms;
   float pass = 0.f;
   const bool show = getenv("BLANCE_PASS_TIMES") != nullptr;
@@ -878,42 +886,26 @@ static int run(blance_ctx* ctx, blance_plan* pl) {
     if (show) std::fprintf(stderr, "[blance] assign pass %zu: %.3f ms\n", i / 2, t);
   }
   pl->last_pass_ms = pass;
-  return BLANCE_OK;
 }
 
-static int fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
-  CK(cudaSetDevice(ctx->device));
+static void fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
   cudaStream_t st = ctx->stream;
   const int n = pl->n_inst;
-  if (pl->PT > 0) {
-    k_pack<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(pl->pool, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
-                                                      pl->d_raw_shape_off, pl->PT);
-    CK(cudaGetLastError());
-    ctx->launches++;
-  }
-  // a single instance is copied straight into the caller's buffers; a batch lands in the pinned staging
-  // buffer first (its head is large enough: it held cur+prev rows)
-  int32_t* h_rows = nullptr;
-  uint8_t *h_shape = nullptr, *h_warn = nullptr;
-  const bool direct = pl->h_stage == nullptr;
-  if (direct) {
-    h_rows = outs[0].next_rows; h_shape = outs[0].next_shape; h_warn = outs[0].warn;
-  } else {
-    char* hp = (char*)pl->h_stage;
-    h_rows = (int32_t*)hp;
-    hp += align_up(sizeof(int32_t) * ((size_t)pl->RRT + 1), 256) * 2;
-    h_shape = (uint8_t*)hp;
-    hp += align_up((size_t)pl->RST + 1, 256);
-    h_warn = (uint8_t*)hp;
-  }
-  if (pl->RRT && h_rows) CK(cudaMemcpyAsync(h_rows, pl->raw_a, sizeof(int32_t) * (size_t)pl->RRT, cudaMemcpyDeviceToHost, st));
-  if (pl->RST && h_shape) CK(cudaMemcpyAsync(h_shape, pl->rawsh_a, (size_t)pl->RST, cudaMemcpyDeviceToHost, st));
-  if (pl->RST && h_warn) CK(cudaMemcpyAsync(h_warn, pl->rawsh_b, (size_t)pl->RST, cudaMemcpyDeviceToHost, st));
+  if (pl->PT > 0)
+    launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, pl->pool, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
+           pl->d_raw_shape_off, pl->PT);
+  const bool dir = direct(pl);
+  int32_t* h_rows = dir ? outs[0].next_rows : pl->h_rows;
+  uint8_t* h_shape = dir ? outs[0].next_shape : pl->h_shape;
+  uint8_t* h_warn = dir ? outs[0].warn : pl->h_warn;
+  if (pl->RRT && h_rows) CUDA(cudaMemcpyAsync(h_rows, pl->raw_a, sizeof(int32_t) * (size_t)pl->RRT, cudaMemcpyDeviceToHost, st));
+  if (pl->RST && h_shape) CUDA(cudaMemcpyAsync(h_shape, pl->rawsh_a, (size_t)pl->RST, cudaMemcpyDeviceToHost, st));
+  if (pl->RST && h_warn) CUDA(cudaMemcpyAsync(h_warn, pl->rawsh_b, (size_t)pl->RST, cudaMemcpyDeviceToHost, st));
   std::vector<DInst> fin(n);
-  CK(cudaMemcpyAsync(fin.data(), pl->pool.insts, sizeof(DInst) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  CUDA(cudaMemcpyAsync(fin.data(), pl->pool.insts, sizeof(DInst) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i)
-    if (fin[i].spec_abort) return fail(ctx, BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
+    if (fin[i].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
   if (getenv("BLANCE_SPEC_STATS"))
     for (int i = 0; i < n && i < 4; ++i)
       std::fprintf(stderr, "[blance] inst %d: steps %lld accepted %lld | resolved by the leader %lld (stale results %lld) movers %lld team %lld rebuilds %lld waits %lld\n",
@@ -929,7 +921,7 @@ static int fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
     const DInst& D = pl->h_insts[i];
     blance_plan_out& o = outs[i];
     const size_t rr = (size_t)D.PU * D.SL, rs = (size_t)D.PU * D.S;
-    if (!direct) {
+    if (!dir) {
       if (rr && o.next_rows) std::memcpy(o.next_rows, h_rows + pl->raw_rows_off[i], sizeof(int32_t) * rr);
       if (rs && o.next_shape) std::memcpy(o.next_shape, h_shape + pl->raw_shape_off[i], rs);
       if (rs && o.warn) std::memcpy(o.warn, h_warn + pl->raw_shape_off[i], rs);
@@ -942,29 +934,29 @@ static int fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
     o.pass_ms = pl->last_pass_ms;
     o.device_ms = 0.f;
   }
-  return BLANCE_OK;
 }
 
 extern "C" int blance_plan_upload(blance_ctx* ctx, const blance_plan_in* in, blance_plan** plan) {
-  if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (!plan) return fail(ctx, BLANCE_ERR_INVALID_ARG, "plan is NULL");
-  std::lock_guard<std::mutex> g(ctx->mu);
-  return upload(ctx, 1, in, plan);
+  return entry(ctx, [&](Device& device) {
+    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    if (!plan) throw_err(BLANCE_ERR_INVALID_ARG, "plan is NULL");
+    *plan = nullptr;
+    *plan = upload(device(), 1, in).release();
+  });
 }
 
 extern "C" int blance_plan_run(blance_ctx* ctx, blance_plan* plan) {
-  if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
-  if (!ctx || !plan) return fail(ctx, BLANCE_ERR_INVALID_ARG, "ctx or plan is NULL");
-  std::lock_guard<std::mutex> g(ctx->mu);
-  return run(ctx, plan);
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !plan) throw_err(BLANCE_ERR_INVALID_ARG, "ctx or plan is NULL");
+    run(device(), plan);
+  });
 }
 
 extern "C" int blance_plan_fetch(blance_ctx* ctx, blance_plan* plan, blance_plan_out* out) {
-  if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
-  if (!ctx || !plan || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "ctx, plan or out is NULL");
-  std::lock_guard<std::mutex> g(ctx->mu);
-  return fetch(ctx, plan, out);
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !plan || !out) throw_err(BLANCE_ERR_INVALID_ARG, "ctx, plan or out is NULL");
+    fetch(device(), plan, out);
+  });
 }
 
 extern "C" int blance_plan_timing(const blance_plan* plan, float* kernel_ms, float* pass_ms, int32_t* pass_launches) {
@@ -976,69 +968,44 @@ extern "C" int blance_plan_timing(const blance_plan* plan, float* kernel_ms, flo
 }
 
 extern "C" void blance_plan_free(blance_ctx* ctx, blance_plan* plan) {
-  if (!plan) return;
-  if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
-  if (ctx) { std::lock_guard<std::mutex> g(ctx->mu); cudaSetDevice(ctx->device); cudaStreamSynchronize(ctx->stream); plan_release(plan, ctx); }
-  else plan_release(plan);
+  PlanPtr owner(plan);               // freed on the stream it was allocated on, also when ctx is NULL
+  if (ctx && plan) entry(ctx, [&](Device& device) { CUDA(cudaStreamSynchronize(device()->stream)); owner.reset(); });
 }
 
-static int plan_batch_one(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out) {
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  CK(cudaEventRecord(ctx->ev[0], ctx->stream));
-  blance_plan* pl = nullptr;
-  int st = upload(ctx, n, in, &pl);
-  if (st != BLANCE_OK) return st;
-  st = run(ctx, pl);
-  if (st == BLANCE_OK) st = fetch(ctx, pl, out);
-  if (st == BLANCE_OK) {
-    cudaEventRecord(ctx->ev[3], ctx->stream);
-    cudaEventSynchronize(ctx->ev[3]);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]);
-    for (int i = 0; i < n; ++i) out[i].device_ms = ms;
-  }
-  plan_release(pl, ctx);
-  return st;
+static void plan_on_device(blance_ctx* ctx, int n, const blance_plan_in* in, blance_plan_out* out) {
+  CUDA(cudaEventRecord(ctx->ev[0], ctx->stream));
+  PlanPtr pl = upload(ctx, n, in);
+  run(ctx, pl.get());
+  fetch(ctx, pl.get(), out);
+  cudaEventRecord(ctx->ev[3], ctx->stream);
+  cudaEventSynchronize(ctx->ev[3]);
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]);
+  for (int i = 0; i < n; ++i) out[i].device_ms = ms;
 }
 
-static int plan_batch(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out) {
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (!in || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "in or out is NULL");
-  if (ctx->children.empty()) return plan_batch_one(ctx, n, in, out);
-  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, "batch size must be positive");
-  // ---- several GPUs: instance i -> device i mod G, one host thread per device, no collective -------------------
-  const int G = (int)std::min<size_t>(ctx->children.size(), (size_t)n);
-  if (G == 1) {
-    const int st = plan_batch_one(ctx->children[0], n, in, out);
-    if (st != BLANCE_OK) ctx->err = ctx->children[0]->err;
-    return st;
-  }
+// Several GPUs: instance i -> device i mod G, one host thread per device, no collective.
+static void plan_batch(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out) {
+  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+  if (!in || !out) throw_err(BLANCE_ERR_INVALID_ARG, "in or out is NULL");
+  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, "batch size must be positive");
+  const int G = (int)std::min<size_t>(std::max<size_t>(1, blance_ctx_device_count(ctx)), (size_t)n);
+  if (G == 1) return fan_out(ctx, 1, [&](int, blance_ctx* dev) { plan_on_device(dev, n, in, out); });
   std::vector<std::vector<blance_plan_in>> ins((size_t)G);
   std::vector<std::vector<blance_plan_out>> outs((size_t)G);
   for (int i = 0; i < n; ++i) { ins[(size_t)(i % G)].push_back(in[i]); outs[(size_t)(i % G)].push_back(out[i]); }
-  std::vector<int> status((size_t)G, BLANCE_OK);
-  std::vector<std::thread> th;
-  for (int d = 0; d < G; ++d)
-    th.emplace_back([&, d]() {
-      status[(size_t)d] = plan_batch_one(ctx->children[(size_t)d], (int32_t)ins[(size_t)d].size(), ins[(size_t)d].data(), outs[(size_t)d].data());
-    });
-  for (auto& t : th) t.join();
-  for (int d = 0; d < G; ++d)
-    if (status[(size_t)d] != BLANCE_OK) {
-      ctx->err = "device " + std::to_string(ctx->children[(size_t)d]->device) + ": " + ctx->children[(size_t)d]->err;
-      return status[(size_t)d];
-    }
+  fan_out(ctx, G, [&](int d, blance_ctx* dev) {
+    plan_on_device(dev, (int)ins[(size_t)d].size(), ins[(size_t)d].data(), outs[(size_t)d].data());
+  });
   for (int i = 0; i < n; ++i) out[i] = outs[(size_t)(i % G)][(size_t)(i / G)];
-  return BLANCE_OK;
 }
 
 extern "C" int blance_plan_next_map(blance_ctx* ctx, const blance_plan_in* in, blance_plan_out* out) {
-  return plan_batch(ctx, 1, in, out);
+  return entry(ctx, [&](Device&) { plan_batch(ctx, 1, in, out); });
 }
 
 extern "C" int blance_plan_next_map_batch(blance_ctx* ctx, int32_t n, const blance_plan_in* in, blance_plan_out* out) {
-  return plan_batch(ctx, n, in, out);
+  return entry(ctx, [&](Device&) { plan_batch(ctx, n, in, out); });
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1125,45 +1092,31 @@ struct SchedReq {
 };
 
 // The schedule state of a wave of nw scenarios (wave_schedule.cuh), sized from bounds known before planning: at most
-// MO = 2 x n_slots ops per partition, so at most PU x MO list entries and PU arrivals per instance.  With arena NULL
-// only the size is computed; else the slices are carved from it into W.
-static size_t wave_sched_layout(const blance_plan_in& base, int nw, int nc, char* arena, WSched* W, void** tmp,
-                                size_t* tmp_bytes, cudaStream_t st) {
+// MO = 2 x n_slots ops per partition, so at most PU x MO list entries and PU arrivals per instance.  Adds its slices
+// to `a`, the sorts' scratch (`tmp`, tmp_bytes) last, and sets W's sizes.
+static void sched_slices(Arena& a, const blance_plan_in& base, int nw, int nc, WSched& w, void*& tmp, size_t& tmp_bytes,
+                         cudaStream_t st) {
   const long long PU = base.n_parts, NU = base.n_node_ids, MO = std::max(1, 2 * base.n_slots);
   const long long ni = (long long)nw * nc, nseg = ni * NU, cap = ni * PU * MO, nkeys = std::max(1ll, ni * PU);
-  int segbits = 1;
-  while ((1ll << segbits) <= nseg) ++segbits;
   size_t sort_tmp = 0, scan_tmp = 0, red_tmp = 0;
   cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nkeys, 0, 64, st);
   cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
   cub::DeviceReduce::Sum(nullptr, red_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
-  *tmp_bytes = std::max(sort_tmp, std::max(scan_tmp, red_tmp)) + 256;
-  WSched w{};
-  struct Sl { void** p; size_t bytes; };
-  const std::vector<Sl> sl = {
-      {(void**)&w.count, sizeof(int32_t) * nc}, {(void**)&w.mover, (size_t)std::max(1ll, NU)}, {(void**)&w.op_n, (size_t)(nw * PU)},
-      {(void**)&w.op_node, sizeof(int32_t) * nw * PU * MO}, {(void**)&w.op_w, (size_t)(nw * PU * MO)},
-      {(void**)&w.cur, (size_t)(ni * PU)}, {(void**)&w.part_done, sizeof(int32_t) * ni * PU},
-      {(void**)&w.seg_off, sizeof(long long) * (nseg + 1)}, {(void**)&w.len, sizeof(int32_t) * (nseg + 1)},
-      {(void**)&w.kcnt, sizeof(int32_t) * (nseg + 1)}, {(void**)&w.poff, sizeof(long long) * (nseg + 1)},
-      {(void**)&w.astart, sizeof(int32_t) * nseg}, {(void**)&w.aend, sizeof(int32_t) * nseg},
-      {(void**)&w.node_rounds, sizeof(int32_t) * nseg}, {(void**)&w.node_last, sizeof(int32_t) * nseg},
-      {(void**)&w.buf0, sizeof(uint32_t) * cap}, {(void**)&w.buf1, sizeof(uint32_t) * cap}, {(void**)&w.scratch, sizeof(uint32_t) * cap},
-      {(void**)&w.keys_in, sizeof(unsigned long long) * nkeys}, {(void**)&w.keys_out, sizeof(unsigned long long) * nkeys},
-      {(void**)&w.scal, sizeof(unsigned long long) * 4 * ni}, {(void**)&w.overflow, sizeof(int32_t)},
-      {(void**)&w.esum, sizeof(long long)}, {tmp, *tmp_bytes}};
-  size_t total = 0;
-  for (const Sl& x : sl) {
-    if (arena) *x.p = arena + total;
-    total += align_up(std::max<size_t>(x.bytes, 1), 256);
-  }
-  if (arena) {
-    w.nw = nw; w.nc = nc; w.PU = (int32_t)PU; w.NU = (int32_t)NU; w.MO = (int32_t)MO; w.nseg = nseg;
-    w.PB = 1;
-    while (w.PB < WAVE_PART_BITS && (1ll << w.PB) < PU) ++w.PB;
-    *W = w;
-  }
-  return total;
+  tmp_bytes = std::max(sort_tmp, std::max(scan_tmp, red_tmp)) + 256;
+  a.add(w.count, (size_t)nc); a.add(w.mover, (size_t)std::max(1ll, NU)); a.add(w.op_n, (size_t)(nw * PU));
+  a.add(w.op_node, (size_t)(nw * PU * MO)); a.add(w.op_w, (size_t)(nw * PU * MO));
+  a.add(w.cur, (size_t)(ni * PU)); a.add(w.part_done, (size_t)(ni * PU));
+  a.add(w.seg_off, (size_t)(nseg + 1)); a.add(w.len, (size_t)(nseg + 1));
+  a.add(w.kcnt, (size_t)(nseg + 1)); a.add(w.poff, (size_t)(nseg + 1));
+  a.add(w.astart, (size_t)nseg); a.add(w.aend, (size_t)nseg);
+  a.add(w.node_rounds, (size_t)nseg); a.add(w.node_last, (size_t)nseg);
+  a.add(w.buf0, (size_t)cap); a.add(w.buf1, (size_t)cap); a.add(w.scratch, (size_t)cap);
+  a.add(w.keys_in, (size_t)nkeys); a.add(w.keys_out, (size_t)nkeys);
+  a.add(w.scal, (size_t)(4 * ni)); a.add(w.overflow, 1);
+  a.add(w.esum, 1); a.add(tmp, tmp_bytes);
+  w.nw = nw; w.nc = nc; w.PU = (int32_t)PU; w.NU = (int32_t)NU; w.MO = (int32_t)MO; w.nseg = nseg;
+  w.PB = 1;
+  while (w.PB < WAVE_PART_BITS && (1ll << w.PB) < PU) ++w.PB;
 }
 
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
@@ -1173,14 +1126,18 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
-  PlanBufs b;
-  size_t per = slices_bytes(arena_slices(&probe, 1, b)) + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
+  Arena one;
+  plan_slices(one, &probe, 1);
+  size_t per = one.bytes() + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
                sizeof(long long) * (size_t)summary_stride(in0) +
                sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides;
   if (sr) {
+    Arena sched;
+    WSched w{};
     void* tmp = nullptr;
     size_t tb = 0;
-    per += wave_sched_layout(in0, 1, sr->nc, nullptr, nullptr, &tmp, &tb, ctx->stream);
+    sched_slices(sched, in0, 1, sr->nc, w, tmp, tb, ctx->stream);
+    per += sched.bytes();
   }
   *per_scenario = per;
   if (sr)            // the first round's arrival slots (nc x n_parts per scenario) are int32 positions
@@ -1201,15 +1158,12 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
 // the host reads the entries left and sizes the next block's sorts by min(picks bound, entries).
 static const int kWaveBlock = 64;
 
-static int wave_schedule(blance_ctx* ctx, blance_plan* pl, int nw, const blance_plan_in& base, int favor_min, const SchedReq& sr,
-                         WSched W, void* tmp, size_t tmp_bytes, const long long* h_sum, long long stride, const int* idx) {
+static void wave_schedule(blance_ctx* ctx, const blance_plan* pl, int nw, const blance_plan_in& base, int favor_min,
+                          const SchedReq& sr, const WSched& W, void* tmp, size_t tmp_bytes, const long long* h_sum,
+                          long long stride, const int* idx) {
   cudaStream_t st = ctx->stream;
   const int nc = sr.nc, NU = base.n_node_ids, PU = base.n_parts;
   const long long ni = (long long)nw * nc, nseg = W.nseg;
-  int rc = BLANCE_OK;
-  auto step = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-  };
   // segments: capacity = the node's ops in the scenario (0 without a mover: nothing ever waits there)
   std::vector<long long> seg_off((size_t)nseg + 1, 0);
   long long pick_bound = 0, max_ops = 0;
@@ -1226,90 +1180,78 @@ static int wave_schedule(blance_ctx* ctx, blance_plan* pl, int nw, const blance_
   }
   const long long nkeys = ni * PU;
   const int end_bit = std::min(64, W.PB + [&] { int b = 1; while ((1ll << b) <= nseg) ++b; return b; }());
-  step(cudaMemcpyAsync((void*)W.count, sr.count.data(), sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st), "H2D");
-  step(cudaMemcpyAsync((void*)W.mover, sr.mover.data(), (size_t)NU, cudaMemcpyHostToDevice, st), "H2D");
-  step(cudaMemcpyAsync((void*)W.seg_off, seg_off.data(), sizeof(long long) * seg_off.size(), cudaMemcpyHostToDevice, st), "H2D");
-  step(cudaMemsetAsync(W.len, 0, sizeof(int32_t) * (nseg + 1), st), "memset");
-  step(cudaMemsetAsync(W.kcnt, 0, sizeof(int32_t) * (nseg + 1), st), "memset");
-  step(cudaMemsetAsync(W.astart, 0, sizeof(int32_t) * nseg, st), "memset");
-  step(cudaMemsetAsync(W.aend, 0, sizeof(int32_t) * nseg, st), "memset");
-  step(cudaMemsetAsync(W.node_rounds, 0, sizeof(int32_t) * nseg, st), "memset");
-  step(cudaMemsetAsync(W.node_last, 0, sizeof(int32_t) * nseg, st), "memset");
-  step(cudaMemsetAsync(W.scal, 0, sizeof(unsigned long long) * 4 * ni, st), "memset");
-  step(cudaMemsetAsync(W.overflow, 0, sizeof(int32_t), st), "memset");
+  CUDA(cudaMemcpyAsync((void*)W.count, sr.count.data(), sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)W.mover, sr.mover.data(), (size_t)NU, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)W.seg_off, seg_off.data(), sizeof(long long) * seg_off.size(), cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemsetAsync(W.len, 0, sizeof(int32_t) * (nseg + 1), st));
+  CUDA(cudaMemsetAsync(W.kcnt, 0, sizeof(int32_t) * (nseg + 1), st));
+  CUDA(cudaMemsetAsync(W.astart, 0, sizeof(int32_t) * nseg, st));
+  CUDA(cudaMemsetAsync(W.aend, 0, sizeof(int32_t) * nseg, st));
+  CUDA(cudaMemsetAsync(W.node_rounds, 0, sizeof(int32_t) * nseg, st));
+  CUDA(cudaMemsetAsync(W.node_last, 0, sizeof(int32_t) * nseg, st));
+  CUDA(cudaMemsetAsync(W.scal, 0, sizeof(unsigned long long) * 4 * ni, st));
+  CUDA(cudaMemsetAsync(W.overflow, 0, sizeof(int32_t), st));
   const int seg_grid = grid_for(ctx, (nseg + WAVE_THREADS / 32 - 1) / (WAVE_THREADS / 32) * WAVE_THREADS, WAVE_THREADS);
   auto sort = [&](long long n) {
     size_t tb = tmp_bytes;
-    if (n > 0) step(cub::DeviceRadixSort::SortKeys(tmp, tb, W.keys_in, const_cast<unsigned long long*>(W.keys_out), (int)n, 0, end_bit, st), "sort");
-    k_wave_bounds<<<grid_for(ctx, std::max(1ll, n), 256), 256, 0, st>>>(W, n);
+    if (n > 0) CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, W.keys_in, const_cast<unsigned long long*>(W.keys_out), (int)n, 0, end_bit, st));
+    launch(ctx, k_wave_bounds, grid_for(ctx, std::max(1ll, n), 256), 256, 0, W, n);
   };
   // the lists: every partition's first op, sorted into its segment
-  if (PU > 0 && rc == BLANCE_OK) {
+  if (PU > 0) {
     const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
-    k_wave_moves<<<dim3((unsigned)bx, (unsigned)nw), 256, 0, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, W);
+    launch(ctx, k_wave_moves, dim3((unsigned)bx, (unsigned)nw), 256, 0, pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, W);
     sort(nkeys);
-    k_wave_merge<<<seg_grid, WAVE_THREADS, 0, st>>>(W, -1);
-    ctx->launches += 3;
+    launch(ctx, k_wave_merge, seg_grid, WAVE_THREADS, 0, W, -1);
   }
   long long E = 0;
   int32_t overflow = 0;
   auto entries = [&]() {
     size_t tb = tmp_bytes;
-    step(cub::DeviceReduce::Sum(tmp, tb, W.len, W.esum, (int)(nseg + 1), st), "reduce");
-    step(cudaMemcpyAsync(&E, W.esum, sizeof E, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaMemcpyAsync(&overflow, W.overflow, sizeof overflow, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaStreamSynchronize(st), "sync");
-    if (rc == BLANCE_OK && overflow) rc = fail(ctx, BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: a round had more picks than its bound (internal error)");
+    CUDA(cub::DeviceReduce::Sum(tmp, tb, W.len, W.esum, (int)(nseg + 1), st));
+    CUDA(cudaMemcpyAsync(&E, W.esum, sizeof E, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaMemcpyAsync(&overflow, W.overflow, sizeof overflow, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    if (overflow) throw_err(BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: a round had more picks than its bound (internal error)");
   };
-  step(cudaGetLastError(), "k_wave_moves / k_wave_merge");
   entries();
   int32_t r = 0;
-  while (rc == BLANCE_OK && E > 0) {
+  while (E > 0) {
     // every instance with entries picks at least one op per round: no instance has more rounds than ops
-    if (r > max_ops + kWaveBlock) { rc = fail(ctx, BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: the schedule did not end (internal error)"); break; }
+    if (r > max_ops + kWaveBlock) throw_err(BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: the schedule did not end (internal error)");
     const long long n_sort = std::min(pick_bound, E);
-    for (int b = 0; b < kWaveBlock && rc == BLANCE_OK; ++b, ++r) {
+    for (int b = 0; b < kWaveBlock; ++b, ++r) {
       size_t tb = tmp_bytes;
-      step(cub::DeviceScan::ExclusiveSum(tmp, tb, W.kcnt, const_cast<long long*>(W.poff), (int)(nseg + 1), st), "scan");
-      step(cudaMemsetAsync(W.keys_in, 0xFF, sizeof(unsigned long long) * (size_t)n_sort, st), "memset");
-      k_wave_pick<<<seg_grid, WAVE_THREADS, 0, st>>>(W, r, n_sort);
+      CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, W.kcnt, const_cast<long long*>(W.poff), (int)(nseg + 1), st));
+      CUDA(cudaMemsetAsync(W.keys_in, 0xFF, sizeof(unsigned long long) * (size_t)n_sort, st));
+      launch(ctx, k_wave_pick, seg_grid, WAVE_THREADS, 0, W, r, n_sort);
       sort(n_sort);
-      k_wave_merge<<<seg_grid, WAVE_THREADS, 0, st>>>(W, r);
-      ctx->launches += 3;
+      launch(ctx, k_wave_merge, seg_grid, WAVE_THREADS, 0, W, r);
     }
-    step(cudaGetLastError(), "schedule round kernels");
     entries();
   }
-  if (rc != BLANCE_OK) return rc;
   // results
   std::vector<unsigned long long> scal((size_t)(4 * ni));
-  step(cudaMemcpyAsync(scal.data(), W.scal, sizeof(unsigned long long) * scal.size(), cudaMemcpyDeviceToHost, st), "D2H");
+  CUDA(cudaMemcpyAsync(scal.data(), W.scal, sizeof(unsigned long long) * scal.size(), cudaMemcpyDeviceToHost, st));
   for (long long i = 0; i < ni; ++i) {
     blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
-    if (o.node_rounds && NU) step(cudaMemcpyAsync(o.node_rounds, W.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st), "D2H");
-    if (o.node_last_round && NU) step(cudaMemcpyAsync(o.node_last_round, W.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st), "D2H");
-    if (o.part_done_round && PU) step(cudaMemcpyAsync(o.part_done_round, W.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st), "D2H");
+    if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, W.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+    if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, W.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+    if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, W.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
   }
-  step(cudaStreamSynchronize(st), "sync");
-  for (long long i = 0; rc == BLANCE_OK && i < ni; ++i) {
+  CUDA(cudaStreamSynchronize(st));
+  for (long long i = 0; i < ni; ++i) {
     blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
     o.rounds = (int32_t)scal[(size_t)(4 * i)];
     o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
     o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
     o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
   }
-  return rc;
 }
 
-static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
-                               const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
-                               const SchedReq* sr) {
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  {
-    cudaError_t stale = cudaGetLastError();
-    if (stale != cudaSuccess) return fail(ctx, BLANCE_ERR_CUDA, std::string("a previous CUDA call on this thread failed: ") + cudaGetErrorString(stale));
-  }
+static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
+                                const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
+                                const SchedReq* sr) {
   cudaStream_t st = ctx->stream;
   const int n_dev = (int)idx.size();
   const blance_plan_in in0 = scenario_in(*base, sc[idx[0]], opts_of(opts, idx[0]));
@@ -1327,110 +1269,28 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
     }
   }
   // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
-  blance_plan* pb = nullptr;
-  {
-    const int rc = upload(ctx, 1, &in0, &pb);
-    if (rc != BLANCE_OK) return rc;
-  }
+  const PlanPtr pb = upload(ctx, 1, &in0);
   size_t per = 0;
   int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, &per);
-  if (W < 1) {
-    plan_release(pb, ctx);
-    return fail(ctx, BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
-  }
+  if (W < 1)
+    throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
   const bool auto_wave = max_concurrent <= 0;
   const bool times = getenv("BLANCE_SCENARIO_TIMES") != nullptr;
   const long long stride = summary_stride(*base);
   const int PU = base->n_parts, NU = base->n_node_ids, S = base->n_states;
-  int rc = BLANCE_OK;
-  for (int w0 = 0; w0 < n_dev && rc == BLANCE_OK;) {
+  for (int w0 = 0; w0 < n_dev;) {
     const int nw = std::min(W, n_dev - w0);
     std::vector<blance_plan_in> ins((size_t)nw);
     for (int j = 0; j < nw; ++j) ins[(size_t)j] = scenario_in(*base, sc[idx[(size_t)(w0 + j)]], opts_of(opts, idx[(size_t)(w0 + j)]));
     // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
     const bool lone = n_dev == 1;
-    blance_plan* pl = lone ? pb : new blance_plan();
+    blance_plan wave_plan;
+    blance_plan* pl = lone ? pb.get() : &wave_plan;
     std::vector<int> seg_off;
     if (!lone) layout(pl, nw, ins.data(), seg_off);
     if (!lone && pl->PT >= (1LL << 29)) {
-      plan_release(pl, ctx);
       if (nw > 1) { W = nw / 2; continue; }
-      rc = fail(ctx, BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
-      break;
-    }
-    PlanBufs b;
-    if (!lone) {
-      rc = carve_arena(ctx, pl, nw, b);
-      if (rc == BLANCE_ERR_NOMEM && auto_wave && nw > 1) { rc = BLANCE_OK; W = nw / 2; continue; }   // the free memory moved
-      if (rc != BLANCE_OK) break;
-    }
-    long long* d_sum = nullptr;
-    if (cudaMallocAsync((void**)&d_sum, sizeof(long long) * (size_t)(stride * nw), st) != cudaSuccess) {
-      cudaGetLastError();
-      if (!lone) plan_release(pl, ctx);
-      if (auto_wave && nw > 1) { W = nw / 2; continue; }
-      rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the scenario summaries failed");
-      break;
-    }
-    // the schedule state, allocated with the wave so that a plan is never lost for want of it
-    char* sched_arena = nullptr;
-    WSched wsch{};
-    void* wtmp = nullptr;
-    size_t wtmp_bytes = 0;
-    if (sr) {
-      const size_t bytes = wave_sched_layout(*base, nw, sr->nc, nullptr, nullptr, &wtmp, &wtmp_bytes, st);
-      if (cudaMallocAsync((void**)&sched_arena, bytes, st) != cudaSuccess) {
-        cudaGetLastError();
-        cudaFreeAsync(d_sum, st);
-        if (!lone) plan_release(pl, ctx);
-        if (auto_wave && nw > 1) { W = nw / 2; continue; }
-        rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the scenario schedules failed");
-        break;
-      }
-      wave_sched_layout(*base, nw, sr->nc, sched_arena, &wsch, &wtmp, &wtmp_bytes, st);
-    }
-    auto step = [&](cudaError_t e, const char* what) {
-      if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-    // the node tables of the wave's scenarios (small host copies); the hierarchy masks and extra counts of the base
-    if (!lone) {
-      const size_t NT = (size_t)pl->NT, NUT = (size_t)pl->NUT, MT = (size_t)pl->MT;
-      std::vector<uint8_t> rm(NUT + 1, 0), ad(NUT + 1, 0), hw(NT + 1, 0);
-      std::vector<int32_t> nwt(NT + 1, 0), ef(NT + 1, 0), er(NT + 1, 0);
-      std::vector<uint32_t> mask(MT + 1, 0);
-      for (int j = 0; j < nw; ++j) {
-        const blance_plan_in& in = ins[(size_t)j];
-        const DInst& D = pl->h_insts[(size_t)j];
-        if (D.NU) { std::memcpy(&rm[(size_t)D.nodeid_off], in.node_removed, (size_t)D.NU); std::memcpy(&ad[(size_t)D.nodeid_off], in.node_added, (size_t)D.NU); }
-        for (int q = 0; q < D.N; ++q) {
-          nwt[(size_t)D.node_off + q] = in.has_node_weights ? in.node_weight[q] : 0;
-          hw[(size_t)D.node_off + q] = in.has_node_weights ? in.node_has_weight[q] : 0;
-          ef[(size_t)D.node_off + q] = in.extra_tot_first ? in.extra_tot_first[q] : 0;
-          er[(size_t)D.node_off + q] = in.extra_tot_rest ? in.extra_tot_rest[q] : 0;
-        }
-        const size_t mw = (size_t)D.n_rules * (D.NU + 1) * D.HW;
-        if (mw) std::memcpy(&mask[(size_t)D.mask_off], in.ie_mask, sizeof(uint32_t) * mw);
-      }
-      step(cudaMemcpyAsync(b.rm, rm.data(), NUT + 1, cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.ad, ad.data(), NUT + 1, cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.hw, hw.data(), NT + 1, cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.nw, nwt.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.ef, ef.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.er, er.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(b.mask, mask.data(), sizeof(uint32_t) * (MT + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaMemcpyAsync(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st), "H2D");
-      step(cudaStreamSynchronize(st), "H2D sync");          // the host vectors die at the end of this block
-    }
-    if (!lone && rc == BLANCE_OK && pl->PT > 0) {
-      const int SLP = pl->h_insts[0].SLP;
-      k_scenario_replicate<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(
-          pl->rows_init, pl->prev_rows_init, pl->pmeta_init, pl->prev_meta_init, pl->pflags_init, b.pweight, b.rank, b.inst,
-          pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init, pb->pflags_init, pb->pool.pweight,
-          pb->pool.name_rank, PU, SLP, pl->PT);
-      ctx->launches++;
-      step(cudaGetLastError(), "k_scenario_replicate");
+      throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
     }
     // the wave's partition-weight overrides over its replicated slices (lone: over the base upload), as
     // wave-global partition indices: ow = index[k] | weight[k] | presence[k]
@@ -1441,97 +1301,109 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
         for (int k = 0; k < n_overrides(o); ++k)
           ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
       }
-    if (rc == BLANCE_OK && !ow.empty()) {
+    // one allocation per wave, so that a plan is never lost for want of its summaries or schedule state: the
+    // wave's plan (lone: the base upload is the plan), the summaries, the schedule state, the weight overrides
+    Arena wave;
+    if (!lone) plan_slices(wave, pl, nw);
+    long long* d_sum = nullptr;
+    wave.add(d_sum, (size_t)(stride * nw));
+    WSched wsch{};
+    void* wtmp = nullptr;
+    size_t wtmp_bytes = 0;
+    if (sr) sched_slices(wave, *base, nw, sr->nc, wsch, wtmp, wtmp_bytes, st);
+    int32_t* d_ow = nullptr;
+    if (!ow.empty()) wave.add(d_ow, ow.size());
+    try {
+      wave.alloc(st, "a scenario wave");
+    } catch (const Error&) {
+      if (auto_wave && nw > 1) { W = nw / 2; continue; }      // the free memory moved
+      throw;
+    }
+    DPool& P = pl->pool;
+    // the node tables of the wave's scenarios (small host copies); the hierarchy masks and extra counts of the base
+    if (!lone) {
+      const size_t NT = (size_t)pl->NT, NUT = (size_t)pl->NUT, MT = (size_t)pl->MT;
+      std::vector<uint8_t> rm(NUT + 1, 0), ad(NUT + 1, 0), hw(NT + 1, 0);
+      std::vector<int32_t> nwt(NT + 1, 0), ef(NT + 1, 0), er(NT + 1, 0);
+      std::vector<uint32_t> mask(MT + 1, 0);
+      const NodeTables t{rm.data(), ad.data(), hw.data(), nwt.data(), ef.data(), er.data(), mask.data()};
+      for (int j = 0; j < nw; ++j) stage_nodes(ins[(size_t)j], pl->h_insts[(size_t)j], t);
+      CUDA(cudaMemcpyAsync((void*)P.node_removed, rm.data(), NUT + 1, cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.node_added, ad.data(), NUT + 1, cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.node_has_weight, hw.data(), NT + 1, cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.node_weight, nwt.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.extra_first, ef.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.extra_rest, er.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync((void*)P.ie_mask, mask.data(), sizeof(uint32_t) * (MT + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
+      CUDA(cudaStreamSynchronize(st));          // the host vectors die at the end of this block
+    }
+    if (!lone && pl->PT > 0)
+      launch(ctx, k_scenario_replicate, grid_for(ctx, pl->PT, 256), 256, 0, pl->rows_init, pl->prev_rows_init, pl->pmeta_init,
+             pl->prev_meta_init, pl->pflags_init, const_cast<int32_t*>(P.pweight), const_cast<int32_t*>(P.name_rank),
+             const_cast<int32_t*>(P.part_inst), pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init,
+             pb->pflags_init, pb->pool.pweight, pb->pool.name_rank, PU, pl->h_insts[0].SLP, pl->PT);
+    if (!ow.empty()) {
       const int k = (int)(ow.size() / 3);
-      int32_t* d_ow = nullptr;
-      if (cudaMallocAsync((void**)&d_ow, sizeof(int32_t) * ow.size(), st) != cudaSuccess) {
-        cudaGetLastError();
-        rc = fail(ctx, BLANCE_ERR_NOMEM, "cudaMalloc of the weight overrides failed");
-      } else {
-        step(cudaMemcpyAsync(d_ow, ow.data(), sizeof(int32_t) * ow.size(), cudaMemcpyHostToDevice, st), "H2D");
-        int32_t* pweight = lone ? const_cast<int32_t*>(pb->pool.pweight) : b.pweight;   // (the base upload is this scenario's own)
-        if (rc == BLANCE_OK) {
-          k_scenario_weights<<<grid_for(ctx, k, 256), 256, 0, st>>>(pweight, pl->pflags_init, d_ow, k);
-          ctx->launches++;
-          step(cudaGetLastError(), "k_scenario_weights");
-        }
-        cudaFreeAsync(d_ow, st);
-      }
-      if (rc != BLANCE_OK) {
-        cudaFreeAsync(d_sum, st);
-        if (sched_arena) cudaFreeAsync(sched_arena, st);
-        if (!lone) plan_release(pl, ctx);
-        break;
-      }
+      CUDA(cudaMemcpyAsync(d_ow, ow.data(), sizeof(int32_t) * ow.size(), cudaMemcpyHostToDevice, st));
+      launch(ctx, k_scenario_weights, grid_for(ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, d_ow, k);
     }
-    if (!lone && rc == BLANCE_OK) {
-      rc = finish_upload(ctx, pl);
-      if (rc != BLANCE_OK) {                                              // (the plan is released)
-        cudaFreeAsync(d_sum, st);
-        if (sched_arena) cudaFreeAsync(sched_arena, st);
-        break;
-      }
-    }
-    step(cudaEventRecord(ctx->ev[0], st), "event");
-    if (rc == BLANCE_OK) rc = run(ctx, pl);
+    if (!lone) finish_upload(ctx, pl);
+    CUDA(cudaEventRecord(ctx->ev[0], st));
+    run(ctx, pl);
     // summaries, then the requested rows
     float sum_ms = 0.f, sched_ms = 0.f;
-    if (rc == BLANCE_OK) {
-      step(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), st), "memset");
-      step(cudaEventRecord(ctx->ev[1], st), "event");
-      if (PU > 0) {
-        const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
-        const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
-        const dim3 grid((unsigned)bx, (unsigned)nw);
-        if (smem <= 48 * 1024) k_scenario_summary<true><<<grid, 256, smem, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
-        else k_scenario_summary<false><<<grid, 256, 0, st>>>(pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
-        ctx->launches++;
-        step(cudaGetLastError(), "k_scenario_summary");
-      }
-      step(cudaEventRecord(ctx->ev[2], st), "event");
-      bool any_rows = false;
-      for (int j = 0; j < nw; ++j) {
-        const blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-        any_rows |= o.next_rows || o.next_shape || o.warn;
-      }
-      if (any_rows && pl->PT > 0) {
-        k_pack<<<grid_for(ctx, pl->PT, 256), 256, 0, st>>>(pl->pool, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
-                                                          pl->d_raw_shape_off, pl->PT);
-        ctx->launches++;
-        step(cudaGetLastError(), "k_pack");
-      }
-      std::vector<long long> h_sum((size_t)(stride * nw));
-      std::vector<DInst> fin((size_t)nw);
-      step(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st), "D2H");
-      step(cudaMemcpyAsync(fin.data(), pl->pool.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st), "D2H");
-      for (int j = 0; j < nw && rc == BLANCE_OK; ++j) {
-        blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-        const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
-        if (rr && o.next_rows) step(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st), "D2H");
-        if (rs && o.next_shape) step(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st), "D2H");
-        if (rs && o.warn) step(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st), "D2H");
-      }
-      step(cudaStreamSynchronize(st), "sync");
-      if (rc == BLANCE_OK) cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
-      for (int j = 0; j < nw && rc == BLANCE_OK; ++j) {
-        if (fin[(size_t)j].spec_abort) { rc = fail(ctx, BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)"); break; }
-        blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-        const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
-        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
-        if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
-        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
-        o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
-        o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
-      }
-      if (sr && rc == BLANCE_OK) {
-        step(cudaEventRecord(ctx->ev[3], st), "event");
-        rc = wave_schedule(ctx, pl, nw, *base, favor_min, *sr, wsch, wtmp, wtmp_bytes, h_sum.data(), stride, idx.data() + w0);
-        step(cudaEventRecord(ctx->ev[1], st), "event");
-        step(cudaEventSynchronize(ctx->ev[1]), "sync");
-        if (rc == BLANCE_OK) cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
-      }
+    CUDA(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), st));
+    CUDA(cudaEventRecord(ctx->ev[1], st));
+    if (PU > 0) {
+      const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
+      const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
+      const dim3 grid((unsigned)bx, (unsigned)nw);
+      if (smem <= 48 * 1024) launch(ctx, k_scenario_summary<true>, grid, 256, smem, P, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
+      else launch(ctx, k_scenario_summary<false>, grid, 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
     }
-    if (times && rc == BLANCE_OK) {
+    CUDA(cudaEventRecord(ctx->ev[2], st));
+    bool any_rows = false;
+    for (int j = 0; j < nw; ++j) {
+      const blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+      any_rows |= o.next_rows || o.next_shape || o.warn;
+    }
+    if (any_rows && pl->PT > 0)
+      launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
+             pl->d_raw_shape_off, pl->PT);
+    std::vector<long long> h_sum((size_t)(stride * nw));
+    std::vector<DInst> fin((size_t)nw);
+    CUDA(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st));
+    CUDA(cudaMemcpyAsync(fin.data(), P.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st));
+    for (int j = 0; j < nw; ++j) {
+      blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+      const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
+      if (rr && o.next_rows) CUDA(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st));
+      if (rs && o.next_shape) CUDA(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+      if (rs && o.warn) CUDA(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
+    for (int j = 0; j < nw; ++j) {
+      if (fin[(size_t)j].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
+      blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
+      const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
+      if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
+      if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
+      o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
+      o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
+      o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
+    }
+    if (sr) {
+      CUDA(cudaEventRecord(ctx->ev[3], st));
+      wave_schedule(ctx, pl, nw, *base, favor_min, *sr, wsch, wtmp, wtmp_bytes, h_sum.data(), stride, idx.data() + w0);
+      CUDA(cudaEventRecord(ctx->ev[1], st));
+      CUDA(cudaEventSynchronize(ctx->ev[1]));
+      cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
+    }
+    if (times) {
       float wave_ms = 0.f;
       cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
       std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
@@ -1539,22 +1411,17 @@ static int scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, cons
       if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
       std::fprintf(stderr, "\n");
     }
-    if (sched_arena) cudaFreeAsync(sched_arena, st);
-    cudaFreeAsync(d_sum, st);
-    if (!lone) plan_release(pl, ctx);
     w0 += nw;
   }
   cudaStreamSynchronize(st);
-  plan_release(pb, ctx);
-  return rc;
 }
 
-static int plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
-                          const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
-                          const SchedReq* sr = nullptr) {
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (n <= 0) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
-  if (!base || !sc || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
+static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                           const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
+                           const SchedReq* sr = nullptr) {
+  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
+  if (!base || !sc || !out) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
   // every scenario is checked before any device work
   long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
   for (int i = 0; i < n; ++i) {
@@ -1573,125 +1440,101 @@ static int plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_i
       if (st == BLANCE_OK && o) st = check_opts(*base, *o, base_sum, why);
     }
     if (st == BLANCE_OK && !why.empty()) st = BLANCE_ERR_INVALID_ARG;
-    if (st != BLANCE_OK) return fail(ctx, st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
+    if (st != BLANCE_OK) throw_err(st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
   }
-  const int G = ctx->children.empty() ? 1 : (int)std::min<size_t>(ctx->children.size(), (size_t)n);
+  // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
+  const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
-  if (ctx->children.empty()) return scenarios_on_device(ctx, base, idx[0], sc, opts, favor_min_nodes, max_concurrent, out, sr);
-  // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
-  std::vector<int> status((size_t)G, BLANCE_OK);
-  std::vector<std::thread> th;
-  for (int d = 0; d < G; ++d)
-    th.emplace_back([&, d]() {
-      status[(size_t)d] = scenarios_on_device(ctx->children[(size_t)d], base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr);
-    });
-  for (auto& t : th) t.join();
-  for (int d = 0; d < G; ++d)
-    if (status[(size_t)d] != BLANCE_OK) {
-      ctx->err = "device " + std::to_string(ctx->children[(size_t)d]->device) + ": " + ctx->children[(size_t)d]->err;
-      return status[(size_t)d];
-    }
-  return BLANCE_OK;
+  fan_out(ctx, G, [&](int d, blance_ctx* dev) {
+    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr);
+  });
 }
 
 extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                      int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
-  return plan_scenarios(ctx, "blance_plan_scenarios", base, n, sc, nullptr, favor_min_nodes, max_concurrent, out);
+  return entry(ctx, [&](Device&) {
+    plan_scenarios(ctx, "blance_plan_scenarios", base, n, sc, nullptr, favor_min_nodes, max_concurrent, out);
+  });
 }
 
 extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                         const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                         blance_scenario_out* out) {
-  return plan_scenarios(ctx, "blance_plan_scenarios_ex", base, n, sc, opts, favor_min_nodes, max_concurrent, out);
+  return entry(ctx, [&](Device&) {
+    plan_scenarios(ctx, "blance_plan_scenarios_ex", base, n, sc, opts, favor_min_nodes, max_concurrent, out);
+  });
 }
 
 extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                               const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                               int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
                                               blance_scenario_out* out, blance_scenario_schedule_out* sched) {
-  const char* name = "blance_plan_scenarios_schedule";
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (n_move_conc < 1 || !move_conc || !sched)
-    return fail(ctx, BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
-  if (base && base->n_parts >= (1 << WAVE_PART_BITS))
-    return fail(ctx, BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
-  if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
-    return fail(ctx, BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
-  SchedReq sr;
-  sr.nc = n_move_conc;
-  sr.out = sched;
-  for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
-  if (base && base->n_node_ids > 0) {
-    sr.mover.assign((size_t)base->n_node_ids, 0);
-    for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
-  }
-  if (n > 0 && sc && out)
-    for (int i = 0; i < n; ++i)
-      for (int k = 0; k < n_move_conc; ++k) {
-        blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
-        o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
-      }
-  return plan_scenarios(ctx, name, base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr);
+  return entry(ctx, [&](Device&) {
+    const char* name = "blance_plan_scenarios_schedule";
+    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    if (n_move_conc < 1 || !move_conc || !sched)
+      throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
+    if (base && base->n_parts >= (1 << WAVE_PART_BITS))
+      throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
+    if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
+      throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
+    SchedReq sr;
+    sr.nc = n_move_conc;
+    sr.out = sched;
+    for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
+    if (base && base->n_node_ids > 0) {
+      sr.mover.assign((size_t)base->n_node_ids, 0);
+      for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
+    }
+    if (n > 0 && sc && out)
+      for (int i = 0; i < n; ++i)
+        for (int k = 0; k < n_move_conc; ++k) {
+          blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
+          o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
+        }
+    plan_scenarios(ctx, name, base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr);
+  });
 }
 
 extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,
                                            const int32_t* state_slot_off, const int32_t* beg_rows,
                                            const int32_t* end_rows, int32_t favor_min_nodes, int32_t max_ops,
                                            int32_t* op_node, uint8_t* op_state, uint8_t* op_kind, int32_t* op_count) {
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->children.empty()) {
-    blance_ctx* c0 = ctx->children[0];
-    const int st = blance_calc_partition_moves(c0, n_parts, n_states, n_visit_states, state_slot_off, beg_rows, end_rows,
-                                               favor_min_nodes, max_ops, op_node, op_state, op_kind, op_count);
-    if (st != BLANCE_OK) ctx->err = c0->err;
-    return st;
-  }
-  if (n_parts < 0 || n_states < 0 || n_states >= 255 || n_visit_states < 0 || n_visit_states > n_states || !state_slot_off || max_ops < 0)
-    return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_calc_partition_moves: bad sizes (at most 254 states: 0xFF is the \"\" state of a del op)");
-  if (max_ops < 2 * state_slot_off[n_states])
-    return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_calc_partition_moves: max_ops must be at least 2 * n_slots (no op may be dropped)");
-  if (n_parts == 0) return BLANCE_OK;
-  const int SL = state_slot_off[n_states];
-  if (SL > 0 && (!beg_rows || !end_rows)) return fail(ctx, BLANCE_ERR_INVALID_ARG, "rows are NULL");
-  if (!op_node || !op_state || !op_kind || !op_count) return fail(ctx, BLANCE_ERR_INVALID_ARG, "outputs are NULL");
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const size_t rows_b = sizeof(int32_t) * (size_t)n_parts * std::max(SL, 1), ops = (size_t)n_parts * std::max(max_ops, 1);
-  char* d = nullptr;
-  const size_t o_slot = 0, o_beg = align_up(sizeof(int32_t) * (n_states + 1), 256), o_end = o_beg + align_up(rows_b, 256),
-               o_node = o_end + align_up(rows_b, 256), o_state = o_node + align_up(sizeof(int32_t) * ops, 256),
-               o_kind = o_state + align_up(ops, 256), o_cnt = o_kind + align_up(ops, 256),
-               total = o_cnt + align_up(sizeof(int32_t) * (size_t)n_parts, 256);
-  if (cudaMallocAsync((void**)&d, total, st) != cudaSuccess)       // stream-ordered pool: no device-wide sync per call
-    return fail(ctx, BLANCE_ERR_NOMEM, "blance_calc_partition_moves: device allocation failed");
-  int rc = BLANCE_OK;
-  auto step = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-  };
-  step(cudaMemcpyAsync(d + o_slot, state_slot_off, sizeof(int32_t) * (n_states + 1), cudaMemcpyHostToDevice, st), "H2D");
-  if (SL > 0) {
-    step(cudaMemcpyAsync(d + o_beg, beg_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st), "H2D");
-    step(cudaMemcpyAsync(d + o_end, end_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st), "H2D");
-  }
-  if (rc == BLANCE_OK) {
-    k_calc_moves<<<grid_for(ctx, n_parts, 128), 128, 0, st>>>(n_parts, n_states, n_visit_states, (const int32_t*)(d + o_slot),
-                                                             (const int32_t*)(d + o_beg), (const int32_t*)(d + o_end),
-                                                             favor_min_nodes, max_ops, (int32_t*)(d + o_node),
-                                                             (uint8_t*)(d + o_state), (uint8_t*)(d + o_kind), (int32_t*)(d + o_cnt));
-    step(cudaGetLastError(), "k_calc_moves");
-    ctx->launches++;
-  }
-  if (max_ops > 0) {
-    step(cudaMemcpyAsync(op_node, d + o_node, sizeof(int32_t) * (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaMemcpyAsync(op_state, d + o_state, (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaMemcpyAsync(op_kind, d + o_kind, (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st), "D2H");
-  }
-  step(cudaMemcpyAsync(op_count, d + o_cnt, sizeof(int32_t) * (size_t)n_parts, cudaMemcpyDeviceToHost, st), "D2H");
-  cudaFreeAsync(d, st);
-  step(cudaStreamSynchronize(st), "sync");
-  return rc;
+  return entry(ctx, [&](Device& device) {
+    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    if (n_parts < 0 || n_states < 0 || n_states >= 255 || n_visit_states < 0 || n_visit_states > n_states || !state_slot_off || max_ops < 0)
+      throw_err(BLANCE_ERR_INVALID_ARG, "blance_calc_partition_moves: bad sizes (at most 254 states: 0xFF is the \"\" state of a del op)");
+    if (max_ops < 2 * state_slot_off[n_states])
+      throw_err(BLANCE_ERR_INVALID_ARG, "blance_calc_partition_moves: max_ops must be at least 2 * n_slots (no op may be dropped)");
+    if (n_parts == 0) return;
+    const int SL = state_slot_off[n_states];
+    if (SL > 0 && (!beg_rows || !end_rows)) throw_err(BLANCE_ERR_INVALID_ARG, "rows are NULL");
+    if (!op_node || !op_state || !op_kind || !op_count) throw_err(BLANCE_ERR_INVALID_ARG, "outputs are NULL");
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    const size_t rows = (size_t)n_parts * std::max(SL, 1), ops = (size_t)n_parts * std::max(max_ops, 1);
+    int32_t *d_slot, *d_beg, *d_end, *d_node, *d_cnt;
+    uint8_t *d_state, *d_kind;
+    Arena a;
+    a.add(d_slot, (size_t)n_states + 1); a.add(d_beg, rows); a.add(d_end, rows);
+    a.add(d_node, ops); a.add(d_state, ops); a.add(d_kind, ops); a.add(d_cnt, (size_t)n_parts);
+    a.alloc(st, "the partition moves");
+    CUDA(cudaMemcpyAsync(d_slot, state_slot_off, sizeof(int32_t) * (n_states + 1), cudaMemcpyHostToDevice, st));
+    if (SL > 0) {
+      CUDA(cudaMemcpyAsync(d_beg, beg_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync(d_end, end_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st));
+    }
+    launch(dev, k_calc_moves, grid_for(dev, n_parts, 128), 128, 0, n_parts, n_states, n_visit_states, d_slot, d_beg, d_end,
+           favor_min_nodes, max_ops, d_node, d_state, d_kind, d_cnt);
+    if (max_ops > 0) {
+      CUDA(cudaMemcpyAsync(op_node, d_node, sizeof(int32_t) * (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st));
+      CUDA(cudaMemcpyAsync(op_state, d_state, (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st));
+      CUDA(cudaMemcpyAsync(op_kind, d_kind, (size_t)n_parts * max_ops, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA(cudaMemcpyAsync(op_count, d_cnt, sizeof(int32_t) * (size_t)n_parts, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+  });
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1700,15 +1543,16 @@ extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int
 struct blance_moves {
   int32_t n_parts = 0, n_node_ids = 0;
   long long total_ops = 0;
-  char* arena = nullptr;             // one stream-ordered allocation
+  Arena arena;
   long long* d_off = nullptr;        // [n_parts + 1]
   int32_t* d_node = nullptr; uint8_t* d_state = nullptr; uint8_t* d_kind = nullptr;   // CSR ops
   int32_t* d_next = nullptr;         // [n_parts] cursors of the current round
   uint32_t *d_key = nullptr, *d_key2 = nullptr; int32_t *d_val = nullptr, *d_val2 = nullptr;   // [n_parts]
   int32_t* d_ncnt = nullptr; int32_t* d_noff = nullptr; unsigned long long* d_nbest = nullptr; int32_t* d_best = nullptr;   // per node
   void* d_tmp = nullptr; size_t tmp_bytes = 0;
-  // the last blance_moves_schedule: round_off [rounds + 1] and sched_op [moves_done] in one allocation
-  char* sched = nullptr;
+  // the last blance_moves_schedule: round_off [rounds + 1] and sched_op [moves_done]
+  std::unique_ptr<Arena> sched;
+  long long *round_off = nullptr, *sched_op = nullptr;
   int32_t sched_rounds = -1;         // -1: no schedule yet
   long long sched_moves = 0;
 };
@@ -1716,122 +1560,105 @@ struct blance_moves {
 extern "C" int blance_moves_create(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,
                                    const int32_t* state_slot_off, const int32_t* beg_rows, const int32_t* end_rows,
                                    int32_t favor_min_nodes, int32_t n_node_ids, blance_moves** out, int64_t* total_ops) {
-  if (!ctx) return fail(nullptr, BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->children.empty()) ctx = ctx->children[0];
-  if (!out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_create: out is NULL");
-  *out = nullptr;
-  if (n_parts < 0 || n_states < 0 || n_states >= 255 || n_visit_states < 0 || n_visit_states > n_states || !state_slot_off || n_node_ids < 0)
-    return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_create: bad sizes");
-  const int SL = state_slot_off[n_states];
-  if (n_parts > 0 && SL > 0 && (!beg_rows || !end_rows)) return fail(ctx, BLANCE_ERR_INVALID_ARG, "rows are NULL");
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const int max_ops = std::max(1, 2 * SL);
-  const size_t P = (size_t)std::max(n_parts, 1), NN = (size_t)std::max(n_node_ids, 1);
-  size_t scan_tmp = 0, sort_tmp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const int32_t*)nullptr, (long long*)nullptr, n_parts + 1, st);
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr, n_parts, 0, 32, st);
-  // scratch of the construction (rows, padded ops, counts) lives in the same arena and is simply left unused later
-  struct Sl { void** p; size_t bytes; };
-  blance_moves* mv = new blance_moves();
-  mv->n_parts = n_parts; mv->n_node_ids = n_node_ids;
-  int32_t *d_slot = nullptr, *d_beg = nullptr, *d_end = nullptr, *p_node = nullptr, *d_cnt = nullptr;
-  uint8_t *p_state = nullptr, *p_kind = nullptr;
-  mv->tmp_bytes = std::max(scan_tmp, sort_tmp) + 256;
-  std::vector<Sl> sl = {
-      {(void**)&mv->d_off, sizeof(long long) * (P + 2)}, {(void**)&mv->d_node, sizeof(int32_t) * P * max_ops},
-      {(void**)&mv->d_state, P * max_ops}, {(void**)&mv->d_kind, P * max_ops}, {(void**)&mv->d_next, sizeof(int32_t) * P},
-      {(void**)&mv->d_key, sizeof(uint32_t) * P}, {(void**)&mv->d_key2, sizeof(uint32_t) * P}, {(void**)&mv->d_val, sizeof(int32_t) * P},
-      {(void**)&mv->d_val2, sizeof(int32_t) * P}, {(void**)&mv->d_ncnt, sizeof(int32_t) * (NN + 1)}, {(void**)&mv->d_noff, sizeof(int32_t) * (NN + 2)},
-      {(void**)&mv->d_nbest, sizeof(unsigned long long) * NN}, {(void**)&mv->d_best, sizeof(int32_t) * NN}, {(void**)&mv->d_tmp, mv->tmp_bytes},
-      {(void**)&d_slot, sizeof(int32_t) * (n_states + 1)}, {(void**)&d_beg, sizeof(int32_t) * P * std::max(SL, 1)},
-      {(void**)&d_end, sizeof(int32_t) * P * std::max(SL, 1)}, {(void**)&p_node, sizeof(int32_t) * P * max_ops},
-      {(void**)&p_state, P * max_ops}, {(void**)&p_kind, P * max_ops}, {(void**)&d_cnt, sizeof(int32_t) * (P + 1)}};
-  size_t total = 0;
-  for (auto& x : sl) total += align_up(x.bytes, 256);
-  if (cudaMallocAsync((void**)&mv->arena, total, st) != cudaSuccess) { delete mv; return fail(ctx, BLANCE_ERR_NOMEM, "blance_moves_create: device allocation failed"); }
-  { size_t off = 0; for (auto& x : sl) { *x.p = mv->arena + off; off += align_up(x.bytes, 256); } }
-  int rc = BLANCE_OK;
-  auto step = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-  };
-  step(cudaMemcpyAsync(d_slot, state_slot_off, sizeof(int32_t) * (n_states + 1), cudaMemcpyHostToDevice, st), "H2D");
-  if (n_parts > 0 && SL > 0) {
-    step(cudaMemcpyAsync(d_beg, beg_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st), "H2D");
-    step(cudaMemcpyAsync(d_end, end_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st), "H2D");
-  }
-  step(cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * (P + 1), st), "memset");
-  if (rc == BLANCE_OK && n_parts > 0) {
-    k_calc_moves<<<grid_for(ctx, n_parts, 128), 128, 0, st>>>(n_parts, n_states, n_visit_states, d_slot, d_beg, d_end, favor_min_nodes,
-                                                             max_ops, p_node, p_state, p_kind, d_cnt);
-    size_t tb = mv->tmp_bytes;
-    step(cub::DeviceScan::ExclusiveSum(mv->d_tmp, tb, d_cnt, mv->d_off, n_parts + 1, st), "scan");
-    k_moves_compact<<<grid_for(ctx, n_parts, 128), 128, 0, st>>>(n_parts, max_ops, mv->d_off, d_cnt, p_node, p_state, p_kind,
-                                                                mv->d_node, mv->d_state, mv->d_kind);
-    step(cudaGetLastError(), "k_calc_moves / k_moves_compact");
-    ctx->launches += 2;
-    step(cudaMemcpyAsync(&mv->total_ops, mv->d_off + n_parts, sizeof(long long), cudaMemcpyDeviceToHost, st), "D2H");
-  } else {
-    step(cudaMemsetAsync(mv->d_off, 0, sizeof(long long) * (P + 2), st), "memset");
-  }
-  step(cudaStreamSynchronize(st), "sync");
-  if (rc != BLANCE_OK) { cudaFreeAsync(mv->arena, st); delete mv; return rc; }
-  if (total_ops) *total_ops = mv->total_ops;
-  *out = mv;
-  return BLANCE_OK;
+  return entry(ctx, [&](Device& device) {
+    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    if (!out) throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_create: out is NULL");
+    *out = nullptr;
+    if (n_parts < 0 || n_states < 0 || n_states >= 255 || n_visit_states < 0 || n_visit_states > n_states || !state_slot_off || n_node_ids < 0)
+      throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_create: bad sizes");
+    const int SL = state_slot_off[n_states];
+    if (n_parts > 0 && SL > 0 && (!beg_rows || !end_rows)) throw_err(BLANCE_ERR_INVALID_ARG, "rows are NULL");
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    const int max_ops = std::max(1, 2 * SL);
+    const size_t P = (size_t)std::max(n_parts, 1), NN = (size_t)std::max(n_node_ids, 1);
+    size_t scan_tmp = 0, sort_tmp = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const int32_t*)nullptr, (long long*)nullptr, n_parts + 1, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr, n_parts, 0, 32, st);
+    std::unique_ptr<blance_moves> mv(new blance_moves());
+    mv->n_parts = n_parts; mv->n_node_ids = n_node_ids;
+    mv->tmp_bytes = std::max(scan_tmp, sort_tmp) + 256;
+    // scratch of the construction (rows, padded ops, counts) lives in the same arena and is simply left unused later
+    int32_t *d_slot, *d_beg, *d_end, *p_node, *d_cnt;
+    uint8_t *p_state, *p_kind;
+    Arena& a = mv->arena;
+    a.add(mv->d_off, P + 2); a.add(mv->d_node, P * max_ops);
+    a.add(mv->d_state, P * max_ops); a.add(mv->d_kind, P * max_ops); a.add(mv->d_next, P);
+    a.add(mv->d_key, P); a.add(mv->d_key2, P); a.add(mv->d_val, P);
+    a.add(mv->d_val2, P); a.add(mv->d_ncnt, NN + 1); a.add(mv->d_noff, NN + 2);
+    a.add(mv->d_nbest, NN); a.add(mv->d_best, NN); a.add(mv->d_tmp, mv->tmp_bytes);
+    a.add(d_slot, (size_t)n_states + 1); a.add(d_beg, P * std::max(SL, 1));
+    a.add(d_end, P * std::max(SL, 1)); a.add(p_node, P * max_ops);
+    a.add(p_state, P * max_ops); a.add(p_kind, P * max_ops); a.add(d_cnt, P + 1);
+    a.alloc(st, "the move lists");
+    CUDA(cudaMemcpyAsync(d_slot, state_slot_off, sizeof(int32_t) * (n_states + 1), cudaMemcpyHostToDevice, st));
+    if (n_parts > 0 && SL > 0) {
+      CUDA(cudaMemcpyAsync(d_beg, beg_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st));
+      CUDA(cudaMemcpyAsync(d_end, end_rows, sizeof(int32_t) * (size_t)n_parts * SL, cudaMemcpyHostToDevice, st));
+    }
+    CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * (P + 1), st));
+    if (n_parts > 0) {
+      launch(dev, k_calc_moves, grid_for(dev, n_parts, 128), 128, 0, n_parts, n_states, n_visit_states, d_slot, d_beg, d_end,
+             favor_min_nodes, max_ops, p_node, p_state, p_kind, d_cnt);
+      size_t tb = mv->tmp_bytes;
+      CUDA(cub::DeviceScan::ExclusiveSum(mv->d_tmp, tb, d_cnt, mv->d_off, n_parts + 1, st));
+      launch(dev, k_moves_compact, grid_for(dev, n_parts, 128), 128, 0, n_parts, max_ops, mv->d_off, d_cnt, p_node, p_state,
+             p_kind, mv->d_node, mv->d_state, mv->d_kind);
+      CUDA(cudaMemcpyAsync(&mv->total_ops, mv->d_off + n_parts, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    } else {
+      CUDA(cudaMemsetAsync(mv->d_off, 0, sizeof(long long) * (P + 2), st));
+    }
+    CUDA(cudaStreamSynchronize(st));
+    if (total_ops) *total_ops = mv->total_ops;
+    *out = mv.release();
+  });
 }
 
 extern "C" int blance_moves_fetch(blance_ctx* ctx, blance_moves* mv, int64_t* op_off, int32_t* op_node, uint8_t* op_state, uint8_t* op_kind) {
-  if (!ctx || !mv) return fail(ctx, BLANCE_ERR_INVALID_ARG, "ctx or moves is NULL");
-  if (!ctx->children.empty()) ctx = ctx->children[0];
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  if (op_off) CK(cudaMemcpyAsync(op_off, mv->d_off, sizeof(long long) * ((size_t)mv->n_parts + 1), cudaMemcpyDeviceToHost, st));
-  if (mv->total_ops > 0) {
-    if (op_node) CK(cudaMemcpyAsync(op_node, mv->d_node, sizeof(int32_t) * (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
-    if (op_state) CK(cudaMemcpyAsync(op_state, mv->d_state, (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
-    if (op_kind) CK(cudaMemcpyAsync(op_kind, mv->d_kind, (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
-  return BLANCE_OK;
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !mv) throw_err(BLANCE_ERR_INVALID_ARG, "ctx or moves is NULL");
+    cudaStream_t st = device()->stream;
+    if (op_off) CUDA(cudaMemcpyAsync(op_off, mv->d_off, sizeof(long long) * ((size_t)mv->n_parts + 1), cudaMemcpyDeviceToHost, st));
+    if (mv->total_ops > 0) {
+      if (op_node) CUDA(cudaMemcpyAsync(op_node, mv->d_node, sizeof(int32_t) * (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
+      if (op_state) CUDA(cudaMemcpyAsync(op_state, mv->d_state, (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
+      if (op_kind) CUDA(cudaMemcpyAsync(op_kind, mv->d_kind, (size_t)mv->total_ops, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA(cudaStreamSynchronize(st));
+  });
 }
 
 extern "C" int blance_moves_available(blance_ctx* ctx, blance_moves* mv, const int32_t* next, int32_t* node_off, int32_t* node_parts,
                                       int32_t* best_part) {
-  if (!ctx || !mv || !next) return fail(ctx, BLANCE_ERR_INVALID_ARG, "ctx, moves or next is NULL");
-  if (!ctx->children.empty()) ctx = ctx->children[0];
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const int P = mv->n_parts, NN = mv->n_node_ids;
-  CK(cudaMemsetAsync(mv->d_ncnt, 0, sizeof(int32_t) * ((size_t)NN + 1), st));
-  CK(cudaMemsetAsync(mv->d_nbest, 0xFF, sizeof(unsigned long long) * (size_t)std::max(NN, 1), st));
-  if (P > 0) {
-    CK(cudaMemcpyAsync(mv->d_next, next, sizeof(int32_t) * (size_t)P, cudaMemcpyHostToDevice, st));
-    k_moves_next<<<grid_for(ctx, P, 256), 256, 0, st>>>(P, NN, mv->d_off, mv->d_node, mv->d_kind, mv->d_next, mv->d_key, mv->d_val,
-                                                       mv->d_ncnt, mv->d_nbest);
-    size_t tb = mv->tmp_bytes;
-    CK(cub::DeviceRadixSort::SortPairs(mv->d_tmp, tb, mv->d_key, mv->d_key2, mv->d_val, mv->d_val2, P, 0, 32, st));   // stable: partitions stay ascending
-    ctx->launches += 1;
-  }
-  {
-    size_t tb = mv->tmp_bytes;
-    CK(cub::DeviceScan::ExclusiveSum(mv->d_tmp, tb, mv->d_ncnt, mv->d_noff, NN + 1, st));
-  }
-  if (NN > 0) { k_moves_best<<<(NN + 255) / 256, 256, 0, st>>>(NN, mv->d_nbest, mv->d_best); ctx->launches += 1; }
-  CK(cudaGetLastError());
-  int32_t n_avail = 0;
-  CK(cudaMemcpyAsync(&n_avail, mv->d_noff + NN, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  if (node_off) CK(cudaMemcpyAsync(node_off, mv->d_noff, sizeof(int32_t) * ((size_t)NN + 1), cudaMemcpyDeviceToHost, st));
-  if (best_part && NN > 0) CK(cudaMemcpyAsync(best_part, mv->d_best, sizeof(int32_t) * (size_t)NN, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (node_parts && n_avail > 0) {
-    CK(cudaMemcpyAsync(node_parts, mv->d_val2, sizeof(int32_t) * (size_t)n_avail, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return BLANCE_OK;
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !mv || !next) throw_err(BLANCE_ERR_INVALID_ARG, "ctx, moves or next is NULL");
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    const int P = mv->n_parts, NN = mv->n_node_ids;
+    CUDA(cudaMemsetAsync(mv->d_ncnt, 0, sizeof(int32_t) * ((size_t)NN + 1), st));
+    CUDA(cudaMemsetAsync(mv->d_nbest, 0xFF, sizeof(unsigned long long) * (size_t)std::max(NN, 1), st));
+    if (P > 0) {
+      CUDA(cudaMemcpyAsync(mv->d_next, next, sizeof(int32_t) * (size_t)P, cudaMemcpyHostToDevice, st));
+      launch(dev, k_moves_next, grid_for(dev, P, 256), 256, 0, P, NN, mv->d_off, mv->d_node, mv->d_kind, mv->d_next, mv->d_key,
+             mv->d_val, mv->d_ncnt, mv->d_nbest);
+      size_t tb = mv->tmp_bytes;
+      CUDA(cub::DeviceRadixSort::SortPairs(mv->d_tmp, tb, mv->d_key, mv->d_key2, mv->d_val, mv->d_val2, P, 0, 32, st));   // stable: partitions stay ascending
+    }
+    {
+      size_t tb = mv->tmp_bytes;
+      CUDA(cub::DeviceScan::ExclusiveSum(mv->d_tmp, tb, mv->d_ncnt, mv->d_noff, NN + 1, st));
+    }
+    if (NN > 0) launch(dev, k_moves_best, (NN + 255) / 256, 256, 0, NN, mv->d_nbest, mv->d_best);
+    int32_t n_avail = 0;
+    CUDA(cudaMemcpyAsync(&n_avail, mv->d_noff + NN, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (node_off) CUDA(cudaMemcpyAsync(node_off, mv->d_noff, sizeof(int32_t) * ((size_t)NN + 1), cudaMemcpyDeviceToHost, st));
+    if (best_part && NN > 0) CUDA(cudaMemcpyAsync(best_part, mv->d_best, sizeof(int32_t) * (size_t)NN, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    if (node_parts && n_avail > 0) {
+      CUDA(cudaMemcpyAsync(node_parts, mv->d_val2, sizeof(int32_t) * (size_t)n_avail, cudaMemcpyDeviceToHost, st));
+      CUDA(cudaStreamSynchronize(st));
+    }
+  });
 }
 
 // The lock-step schedule (include/blance_b200.h, schedule.cuh).  Rounds are enqueued in blocks of kSchedBlock; the
@@ -1840,149 +1667,119 @@ static const int kSchedBlock = 64;
 
 extern "C" int blance_moves_schedule(blance_ctx* ctx, blance_moves* mv, int32_t max_concurrent_per_node,
                                      const uint8_t* node_has_mover, blance_schedule_out* out) {
-  if (!ctx || !mv || !out) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule: ctx, moves or out is NULL");
-  if (!ctx->children.empty()) {
-    blance_ctx* c0 = ctx->children[0];
-    const int st = blance_moves_schedule(c0, mv, max_concurrent_per_node, node_has_mover, out);
-    if (st != BLANCE_OK) ctx->err = c0->err;
-    return st;
-  }
-  std::memset(out, 0, sizeof *out);
-  std::lock_guard<std::mutex> g(ctx->mu);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const int32_t P = mv->n_parts, NN = mv->n_node_ids;
-  const long long T = mv->total_ops;
-  const int32_t count = max_concurrent_per_node <= 0 ? 1 : max_concurrent_per_node;   // orchestrate.go:484-487
-  int bits = 1;                                       // keys 0 .. NN (NN = past the active entries)
-  while (bits < 32 && (1ull << bits) <= (unsigned long long)NN) ++bits;
-  const size_t Pz = (size_t)std::max(P, 1), NNz = (size_t)std::max(NN, 1);
-  size_t sort_tmp = 0, sel_tmp = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, std::max(P, 1), 0, bits, st);
-  cub::DeviceSelect::Flagged(nullptr, sel_tmp, (const int32_t*)nullptr, (const uint8_t*)nullptr, (int32_t*)nullptr,
-                             (int32_t*)nullptr, std::max(P, 1), st);
-  const size_t tmp_bytes = std::max(sort_tmp, sel_tmp) + 256;
-  SchedState* d_st = nullptr;
-  int32_t *cur = nullptr, *act = nullptr, *act2 = nullptr, *list = nullptr, *cnt = nullptr, *noff = nullptr, *boff = nullptr;
-  uint32_t *key = nullptr, *key2 = nullptr;
-  uint8_t *flags = nullptr, *wl = nullptr, *mover = nullptr;
-  void* tmp = nullptr;
-  struct Sl { void** p; size_t bytes; };
-  std::vector<Sl> sl = {{(void**)&d_st, sizeof(SchedState)}, {(void**)&cur, sizeof(int32_t) * Pz}, {(void**)&act, sizeof(int32_t) * Pz},
-                        {(void**)&act2, sizeof(int32_t) * Pz}, {(void**)&list, sizeof(int32_t) * Pz}, {(void**)&key, sizeof(uint32_t) * Pz},
-                        {(void**)&key2, sizeof(uint32_t) * Pz}, {(void**)&flags, Pz}, {(void**)&wl, Pz},
-                        {(void**)&cnt, sizeof(int32_t) * NNz}, {(void**)&noff, sizeof(int32_t) * (NNz + 1)},
-                        {(void**)&boff, sizeof(int32_t) * (NNz + 1)}, {(void**)&mover, NNz}, {&tmp, tmp_bytes}};
-  size_t total = 0;
-  for (auto& x : sl) total += align_up(x.bytes, 256);
-  char* arena = nullptr;
-  if (cudaMallocAsync((void**)&arena, total, st) != cudaSuccess) return fail(ctx, BLANCE_ERR_NOMEM, "blance_moves_schedule: device allocation failed");
-  { size_t off = 0; for (auto& x : sl) { *x.p = arena + off; off += align_up(x.bytes, 256); } }
-  // results: round_off [T + 2] (R <= T) and sched_op [T], kept in the handle
-  if (mv->sched) { cudaFreeAsync(mv->sched, st); mv->sched = nullptr; }
-  mv->sched_rounds = -1;
-  const size_t ro_bytes = align_up(sizeof(long long) * (size_t)(T + 2), 256);
-  if (cudaMallocAsync((void**)&mv->sched, ro_bytes + sizeof(long long) * (size_t)std::max(T, 1ll), st) != cudaSuccess) {
-    mv->sched = nullptr;
-    cudaFreeAsync(arena, st);
-    return fail(ctx, BLANCE_ERR_NOMEM, "blance_moves_schedule: device allocation failed");
-  }
-  long long* round_off = (long long*)mv->sched;
-  long long* sched_op = (long long*)(mv->sched + ro_bytes);
-  int rc = BLANCE_OK;
-  auto step = [&](cudaError_t e, const char* what) {
-    if (e != cudaSuccess && rc == BLANCE_OK) rc = fail(ctx, BLANCE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-  };
-  SchedState h{};
-  step(cudaEventRecord(ctx->ev[0], st), "event");
-  if (node_has_mover) step(cudaMemcpyAsync(mover, node_has_mover, (size_t)NN, cudaMemcpyHostToDevice, st), "H2D");
-  else step(cudaMemsetAsync(mover, 1, NNz, st), "memset");
-  step(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * NNz, st), "memset");
-  k_sched_init<<<grid_for(ctx, P, 256), 256, 0, st>>>(P, cur, act2, round_off, d_st);
-  ctx->launches += 1;
-  int32_t a_bound = 0;
-  if (P > 0) {                                        // the first compaction: partitions with a pickable first move
-    k_sched_flags<<<grid_for(ctx, P, 256), 256, 0, st>>>(P, act2, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
-    ctx->launches += 1;
-    size_t tb = tmp_bytes;
-    step(cub::DeviceSelect::Flagged(tmp, tb, act2, flags, act, &d_st->A, P, st), "select");
-    step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaStreamSynchronize(st), "sync");
-    a_bound = h.A;
-  }
-  step(cudaGetLastError(), "k_sched_init / k_sched_flags");
-  const int pick_grid = (int)std::min<long long>((NNz + SCHED_PICK_THREADS / 32 - 1) / (SCHED_PICK_THREADS / 32), (long long)ctx->sm_count * 16);
-  long long launched = 0;
-  while (rc == BLANCE_OK && a_bound > 0) {
-    if (launched > T + kSchedBlock) { rc = fail(ctx, BLANCE_ERR_CUDA, "blance_moves_schedule: the schedule did not end (internal error)"); break; }
-    for (int r = 0; r < kSchedBlock && rc == BLANCE_OK; ++r) {
-      const int g = grid_for(ctx, a_bound, 256);
-      k_sched_keys<<<g, 256, 0, st>>>(a_bound, act, mv->d_off, mv->d_node, cur, NN, key, cnt, d_st);
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !mv || !out) throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_schedule: ctx, moves or out is NULL");
+    std::memset(out, 0, sizeof *out);
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    const int32_t P = mv->n_parts, NN = mv->n_node_ids;
+    const long long T = mv->total_ops;
+    const int32_t count = max_concurrent_per_node <= 0 ? 1 : max_concurrent_per_node;   // orchestrate.go:484-487
+    int bits = 1;                                       // keys 0 .. NN (NN = past the active entries)
+    while (bits < 32 && (1ull << bits) <= (unsigned long long)NN) ++bits;
+    const size_t Pz = (size_t)std::max(P, 1), NNz = (size_t)std::max(NN, 1);
+    size_t sort_tmp = 0, sel_tmp = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
+                                    (int32_t*)nullptr, std::max(P, 1), 0, bits, st);
+    cub::DeviceSelect::Flagged(nullptr, sel_tmp, (const int32_t*)nullptr, (const uint8_t*)nullptr, (int32_t*)nullptr,
+                               (int32_t*)nullptr, std::max(P, 1), st);
+    const size_t tmp_bytes = std::max(sort_tmp, sel_tmp) + 256;
+    SchedState* d_st;
+    int32_t *cur, *act, *act2, *list, *cnt, *noff, *boff;
+    uint32_t *key, *key2;
+    uint8_t *flags, *wl, *mover;
+    void* tmp;
+    Arena scratch;
+    scratch.add(d_st, 1); scratch.add(cur, Pz); scratch.add(act, Pz);
+    scratch.add(act2, Pz); scratch.add(list, Pz); scratch.add(key, Pz);
+    scratch.add(key2, Pz); scratch.add(flags, Pz); scratch.add(wl, Pz);
+    scratch.add(cnt, NNz); scratch.add(noff, NNz + 1);
+    scratch.add(boff, NNz + 1); scratch.add(mover, NNz); scratch.add(tmp, tmp_bytes);
+    scratch.alloc(st, "the schedule scratch");
+    // results: round_off [T + 2] (R <= T) and sched_op [T], kept in the handle
+    mv->sched.reset();
+    mv->sched_rounds = -1;
+    std::unique_ptr<Arena> res(new Arena());
+    res->add(mv->round_off, (size_t)(T + 2));
+    res->add(mv->sched_op, (size_t)std::max(T, 1ll));
+    res->alloc(st, "the schedule");
+    mv->sched = std::move(res);
+    long long* round_off = mv->round_off;
+    SchedState h{};
+    CUDA(cudaEventRecord(dev->ev[0], st));
+    if (node_has_mover) CUDA(cudaMemcpyAsync(mover, node_has_mover, (size_t)NN, cudaMemcpyHostToDevice, st));
+    else CUDA(cudaMemsetAsync(mover, 1, NNz, st));
+    CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * NNz, st));
+    launch(dev, k_sched_init, grid_for(dev, P, 256), 256, 0, P, cur, act2, round_off, d_st);
+    int32_t a_bound = 0;
+    if (P > 0) {                                        // the first compaction: partitions with a pickable first move
+      launch(dev, k_sched_flags, grid_for(dev, P, 256), 256, 0, P, act2, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
       size_t tb = tmp_bytes;
-      step(cub::DeviceRadixSort::SortPairs(tmp, tb, key, key2, act, list, a_bound, 0, bits, st), "sort");
-      k_sched_scan<<<1, SCHED_SCAN_THREADS, 0, st>>>(NN, count, cnt, noff, boff, round_off, d_st);
-      k_sched_pick<<<pick_grid, SCHED_PICK_THREADS, 0, st>>>(NN, count, noff, boff, list, wl, mv->d_off, mv->d_kind, cur, sched_op, d_st);
-      k_sched_flags<<<g, 256, 0, st>>>(a_bound, act, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
-      tb = tmp_bytes;
-      step(cub::DeviceSelect::Flagged(tmp, tb, act, flags, act2, &d_st->A, a_bound, st), "select");
-      ctx->launches += 4;
-      std::swap(act, act2);
-      ++launched;
+      CUDA(cub::DeviceSelect::Flagged(tmp, tb, act2, flags, act, &d_st->A, P, st));
+      CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
+      CUDA(cudaStreamSynchronize(st));
+      a_bound = h.A;
     }
-    step(cudaGetLastError(), "schedule round kernels");
-    step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
-    step(cudaStreamSynchronize(st), "sync");
-    if (h.done) break;
-    a_bound = h.A;
-  }
-  long long moves_done = 0;
-  step(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st), "D2H");
-  step(cudaStreamSynchronize(st), "sync");
-  if (rc == BLANCE_OK) step(cudaMemcpyAsync(&moves_done, round_off + h.rounds, sizeof moves_done, cudaMemcpyDeviceToHost, st), "D2H");
-  step(cudaEventRecord(ctx->ev[1], st), "event");
-  cudaFreeAsync(arena, st);
-  step(cudaStreamSynchronize(st), "sync");
-  if (rc != BLANCE_OK) return rc;
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
-  mv->sched_rounds = h.rounds;
-  mv->sched_moves = moves_done;
-  out->rounds = h.rounds;
-  out->moves_done = moves_done;
-  out->stuck_parts = (int64_t)h.stuck;
-  out->max_batch = h.max_batch;
-  out->device_ms = ms;
-  return BLANCE_OK;
+    const int pick_grid = (int)std::min<long long>((NNz + SCHED_PICK_THREADS / 32 - 1) / (SCHED_PICK_THREADS / 32), (long long)dev->sm_count * 16);
+    long long launched = 0;
+    while (a_bound > 0) {
+      if (launched > T + kSchedBlock) throw_err(BLANCE_ERR_CUDA, "blance_moves_schedule: the schedule did not end (internal error)");
+      for (int r = 0; r < kSchedBlock; ++r) {
+        const int g = grid_for(dev, a_bound, 256);
+        launch(dev, k_sched_keys, g, 256, 0, a_bound, act, mv->d_off, mv->d_node, cur, NN, key, cnt, d_st);
+        size_t tb = tmp_bytes;
+        CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, key, key2, act, list, a_bound, 0, bits, st));
+        launch(dev, k_sched_scan, 1, SCHED_SCAN_THREADS, 0, NN, count, cnt, noff, boff, round_off, d_st);
+        launch(dev, k_sched_pick, pick_grid, SCHED_PICK_THREADS, 0, NN, count, noff, boff, list, wl, mv->d_off, mv->d_kind, cur,
+               mv->sched_op, d_st);
+        launch(dev, k_sched_flags, g, 256, 0, a_bound, act, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
+        tb = tmp_bytes;
+        CUDA(cub::DeviceSelect::Flagged(tmp, tb, act, flags, act2, &d_st->A, a_bound, st));
+        std::swap(act, act2);
+        ++launched;
+      }
+      CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
+      CUDA(cudaStreamSynchronize(st));
+      if (h.done) break;
+      a_bound = h.A;
+    }
+    long long moves_done = 0;
+    CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    CUDA(cudaMemcpyAsync(&moves_done, round_off + h.rounds, sizeof moves_done, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaEventRecord(dev->ev[1], st));
+    CUDA(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, dev->ev[0], dev->ev[1]);
+    mv->sched_rounds = h.rounds;
+    mv->sched_moves = moves_done;
+    out->rounds = h.rounds;
+    out->moves_done = moves_done;
+    out->stuck_parts = (int64_t)h.stuck;
+    out->max_batch = h.max_batch;
+    out->device_ms = ms;
+  });
 }
 
 extern "C" int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* mv, int64_t* round_off, int64_t* sched_op) {
-  if (!ctx || !mv) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: ctx or moves is NULL");
-  if (!ctx->children.empty()) ctx = ctx->children[0];
-  std::lock_guard<std::mutex> g(ctx->mu);
-  if (mv->sched_rounds < 0 || !mv->sched) return fail(ctx, BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: no schedule was computed on this handle");
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const size_t ro_bytes = align_up(sizeof(long long) * (size_t)(mv->total_ops + 2), 256);
-  if (round_off) CK(cudaMemcpyAsync(round_off, mv->sched, sizeof(long long) * ((size_t)mv->sched_rounds + 1), cudaMemcpyDeviceToHost, st));
-  if (sched_op && mv->sched_moves > 0)
-    CK(cudaMemcpyAsync(sched_op, mv->sched + ro_bytes, sizeof(long long) * (size_t)mv->sched_moves, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return BLANCE_OK;
+  return entry(ctx, [&](Device& device) {
+    if (!ctx || !mv) throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: ctx or moves is NULL");
+    cudaStream_t st = device()->stream;
+    if (mv->sched_rounds < 0 || !mv->sched)
+      throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_schedule_fetch: no schedule was computed on this handle");
+    if (round_off) CUDA(cudaMemcpyAsync(round_off, mv->round_off, sizeof(long long) * ((size_t)mv->sched_rounds + 1), cudaMemcpyDeviceToHost, st));
+    if (sched_op && mv->sched_moves > 0)
+      CUDA(cudaMemcpyAsync(sched_op, mv->sched_op, sizeof(long long) * (size_t)mv->sched_moves, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+  });
 }
 
 extern "C" void blance_moves_free(blance_ctx* ctx, blance_moves* mv) {
-  if (!mv) return;
-  if (ctx && !ctx->children.empty()) ctx = ctx->children[0];
-  if (ctx) {
-    std::lock_guard<std::mutex> g(ctx->mu);
-    cudaSetDevice(ctx->device);
-    if (mv->arena) cudaFreeAsync(mv->arena, ctx->stream);
-    if (mv->sched) cudaFreeAsync(mv->sched, ctx->stream);
-    cudaStreamSynchronize(ctx->stream);
-  } else {
-    if (mv->arena) cudaFree(mv->arena);
-    if (mv->sched) cudaFree(mv->sched);
-  }
-  delete mv;
+  std::unique_ptr<blance_moves> owner(mv);   // freed on the stream it was allocated on, also when ctx is NULL
+  if (ctx && mv)
+    entry(ctx, [&](Device& device) {
+      blance_ctx* dev = device();
+      owner.reset();
+      CUDA(cudaStreamSynchronize(dev->stream));
+    });
 }

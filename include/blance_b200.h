@@ -72,7 +72,8 @@ typedef struct blance_ctx blance_ctx;   /* owns the device, streams, scratch buf
 int blance_ctx_create(blance_ctx** out, int device_id);
 /* One context over several GPUs of the node.  blance_plan_next_map_batch() shards its instances over them
  * (instance i -> device_ids[i mod n_devices], one host thread per device; plan instances are independent, so
- * there is no collective in the data path); every other entry point runs on device_ids[0]. */
+ * there is no collective in the data path), and the blance_plan_scenarios* calls shard their scenarios the same
+ * way; every other entry point runs on device_ids[0].  Errors are reported on this context either way. */
 int blance_ctx_create_multi(blance_ctx** out, const int* device_ids, int n_devices);
 int blance_ctx_device_count(const blance_ctx* ctx);
 void blance_ctx_destroy(blance_ctx* ctx);
