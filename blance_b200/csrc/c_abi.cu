@@ -20,7 +20,6 @@
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
-#include <cub/device/device_select.cuh>
 
 #include "assign_pass.cuh"
 #include "assign_pass_seq.cuh"
@@ -28,7 +27,6 @@
 #include "aux_kernels.cuh"
 #include "blance_b200.h"
 #include "device_types.cuh"
-#include "schedule.cuh"
 #include "wave_schedule.cuh"
 
 using namespace blance_dev;
@@ -1091,20 +1089,23 @@ struct SchedReq {
   blance_scenario_schedule_out* out = nullptr;
 };
 
-// The schedule state of a wave of nw scenarios (wave_schedule.cuh), sized from bounds known before planning: at most
-// MO = 2 x n_slots ops per partition, so at most PU x MO list entries and PU arrivals per instance.  Adds its slices
-// to `a`, the sorts' scratch (`tmp`, tmp_bytes) last, and sets W's sizes.
-static void sched_slices(Arena& a, const blance_plan_in& base, int nw, int nc, WSched& w, void*& tmp, size_t& tmp_bytes,
-                         cudaStream_t st) {
-  const long long PU = base.n_parts, NU = base.n_node_ids, MO = std::max(1, 2 * base.n_slots);
-  const long long ni = (long long)nw * nc, nseg = ni * NU, cap = ni * PU * MO, nkeys = std::max(1ll, ni * PU);
+// At most 2 x n_slots ops per partition of a scenario: the bound its schedule state is sized by before planning.
+static int scenario_ops(const blance_plan_in& base) { return std::max(1, 2 * base.n_slots); }
+
+// The schedule state of nw scenarios x nc counts over PU partitions and NU node ids (wave_schedule.cuh), with room for
+// `entries` list entries per instance and PU arrivals per instance.  MO > 0 adds the op table of MO ops per
+// partition; MO = 0 leaves the ops to the caller (a moves handle's CSR arrays).  Adds its slices to `a`, the sorts'
+// scratch (`tmp`, tmp_bytes) last, and sets W's sizes.
+static void sched_slices(Arena& a, int nw, int nc, long long PU, long long NU, int MO, long long entries, WSched& w,
+                         void*& tmp, size_t& tmp_bytes, cudaStream_t st) {
+  const long long ni = (long long)nw * nc, nseg = ni * NU, cap = ni * entries, nkeys = std::max(1ll, ni * PU);
   size_t sort_tmp = 0, scan_tmp = 0, red_tmp = 0;
   cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nkeys, 0, 64, st);
   cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
   cub::DeviceReduce::Sum(nullptr, red_tmp, (const int32_t*)nullptr, (long long*)nullptr, (int)(nseg + 1), st);
   tmp_bytes = std::max(sort_tmp, std::max(scan_tmp, red_tmp)) + 256;
-  a.add(w.count, (size_t)nc); a.add(w.mover, (size_t)std::max(1ll, NU)); a.add(w.op_n, (size_t)(nw * PU));
-  a.add(w.op_node, (size_t)(nw * PU * MO)); a.add(w.op_w, (size_t)(nw * PU * MO));
+  a.add(w.count, (size_t)nc); a.add(w.mover, (size_t)std::max(1ll, NU));
+  if (MO > 0) { a.add(w.op_n, (size_t)(nw * PU)); a.add(w.op_node, (size_t)(nw * PU * MO)); a.add(w.op_kind, (size_t)(nw * PU * MO)); }
   a.add(w.cur, (size_t)(ni * PU)); a.add(w.part_done, (size_t)(ni * PU));
   a.add(w.seg_off, (size_t)(nseg + 1)); a.add(w.len, (size_t)(nseg + 1));
   a.add(w.kcnt, (size_t)(nseg + 1)); a.add(w.poff, (size_t)(nseg + 1));
@@ -1136,7 +1137,8 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
     WSched w{};
     void* tmp = nullptr;
     size_t tb = 0;
-    sched_slices(sched, in0, 1, sr->nc, w, tmp, tb, ctx->stream);
+    sched_slices(sched, 1, sr->nc, in0.n_parts, in0.n_node_ids, scenario_ops(in0), (long long)in0.n_parts * scenario_ops(in0), w, tmp, tb,
+                 ctx->stream);
     per += sched.bytes();
   }
   *per_scenario = per;
@@ -1153,30 +1155,34 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   return w;
 }
 
-// The schedules of a planned wave (wave_schedule.cuh): scenario j of the wave is caller scenario idx[j]; h_sum holds
-// the wave's summaries (node_ops carve the segments).  Rounds are enqueued in blocks of kWaveBlock; after each block
-// the host reads the entries left and sizes the next block's sorts by min(picks bound, entries).
+// grid of a kernel striding over the PU partitions of each of nw scenarios (blockIdx.y = scenario)
+static dim3 wave_grid(const blance_ctx* ctx, int PU, int nw) {
+  return dim3((unsigned)std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw))), (unsigned)nw);
+}
+
+// The schedules of nw scenarios x sr.nc counts on W (wave_schedule.cuh), its ops in place: ops[j * NU + q] = the
+// ops of scenario j on node q carve the segments.  Rounds are enqueued in blocks of kWaveBlock; after each block the
+// host reads the entries left and sizes the next block's sorts by min(picks bound, entries).  Returns the
+// instances' scalars [ni][4]: rounds, moves_done, stuck_parts, max_batch.
 static const int kWaveBlock = 64;
 
-static void wave_schedule(blance_ctx* ctx, const blance_plan* pl, int nw, const blance_plan_in& base, int favor_min,
-                          const SchedReq& sr, const WSched& W, void* tmp, size_t tmp_bytes, const long long* h_sum,
-                          long long stride, const int* idx) {
+static std::vector<unsigned long long> wave_schedule(blance_ctx* ctx, const char* name, const SchedReq& sr, const WSched& W,
+                                                     void* tmp, size_t tmp_bytes, const long long* ops) {
   cudaStream_t st = ctx->stream;
-  const int nc = sr.nc, NU = base.n_node_ids, PU = base.n_parts;
-  const long long ni = (long long)nw * nc, nseg = W.nseg;
+  const int nc = sr.nc, NU = W.NU, PU = W.PU;
+  const long long ni = (long long)W.nw * nc, nseg = W.nseg;
   // segments: capacity = the node's ops in the scenario (0 without a mover: nothing ever waits there)
   std::vector<long long> seg_off((size_t)nseg + 1, 0);
   long long pick_bound = 0, max_ops = 0;
   for (long long i = 0; i < ni; ++i) {
-    const long long* ops = h_sum + (i / nc) * stride;
     const int c = sr.count[(size_t)(i % nc)];
-    max_ops = std::max(max_ops, ops[stride - 2]);
     for (int q = 0; q < NU; ++q) {
       const long long s = i * NU + q;
-      const long long capq = sr.mover[(size_t)q] ? ops[4ll * q] + ops[4ll * q + 1] + ops[4ll * q + 2] + ops[4ll * q + 3] : 0;
+      const long long capq = sr.mover[(size_t)q] ? ops[(i / nc) * NU + q] : 0;
       seg_off[(size_t)s + 1] = seg_off[(size_t)s] + capq;
       pick_bound += std::min<long long>(c, capq);
     }
+    max_ops = std::max(max_ops, seg_off[(size_t)(i + 1) * NU] - seg_off[(size_t)i * NU]);
   }
   const long long nkeys = ni * PU;
   const int end_bit = std::min(64, W.PB + [&] { int b = 1; while ((1ll << b) <= nseg) ++b; return b; }());
@@ -1191,6 +1197,7 @@ static void wave_schedule(blance_ctx* ctx, const blance_plan* pl, int nw, const 
   CUDA(cudaMemsetAsync(W.node_last, 0, sizeof(int32_t) * nseg, st));
   CUDA(cudaMemsetAsync(W.scal, 0, sizeof(unsigned long long) * 4 * ni, st));
   CUDA(cudaMemsetAsync(W.overflow, 0, sizeof(int32_t), st));
+  if (W.round_off) CUDA(cudaMemsetAsync(W.round_off, 0, sizeof(long long), st));
   const int seg_grid = grid_for(ctx, (nseg + WAVE_THREADS / 32 - 1) / (WAVE_THREADS / 32) * WAVE_THREADS, WAVE_THREADS);
   auto sort = [&](long long n) {
     size_t tb = tmp_bytes;
@@ -1199,8 +1206,7 @@ static void wave_schedule(blance_ctx* ctx, const blance_plan* pl, int nw, const 
   };
   // the lists: every partition's first op, sorted into its segment
   if (PU > 0) {
-    const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
-    launch(ctx, k_wave_moves, dim3((unsigned)bx, (unsigned)nw), 256, 0, pl->pool, pl->prev_rows_init, pl->pflags_init, favor_min, W);
+    launch(ctx, k_wave_first, wave_grid(ctx, PU, W.nw), 256, 0, W);
     sort(nkeys);
     launch(ctx, k_wave_merge, seg_grid, WAVE_THREADS, 0, W, -1);
   }
@@ -1212,41 +1218,27 @@ static void wave_schedule(blance_ctx* ctx, const blance_plan* pl, int nw, const 
     CUDA(cudaMemcpyAsync(&E, W.esum, sizeof E, cudaMemcpyDeviceToHost, st));
     CUDA(cudaMemcpyAsync(&overflow, W.overflow, sizeof overflow, cudaMemcpyDeviceToHost, st));
     CUDA(cudaStreamSynchronize(st));
-    if (overflow) throw_err(BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: a round had more picks than its bound (internal error)");
+    if (overflow) throw_err(BLANCE_ERR_CUDA, std::string(name) + ": a round had more picks than its bound (internal error)");
   };
   entries();
   int32_t r = 0;
   while (E > 0) {
     // every instance with entries picks at least one op per round: no instance has more rounds than ops
-    if (r > max_ops + kWaveBlock) throw_err(BLANCE_ERR_CUDA, "blance_plan_scenarios_schedule: the schedule did not end (internal error)");
+    if (r > max_ops + kWaveBlock) throw_err(BLANCE_ERR_CUDA, std::string(name) + ": the schedule did not end (internal error)");
     const long long n_sort = std::min(pick_bound, E);
     for (int b = 0; b < kWaveBlock; ++b, ++r) {
       size_t tb = tmp_bytes;
       CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, W.kcnt, const_cast<long long*>(W.poff), (int)(nseg + 1), st));
-      CUDA(cudaMemsetAsync(W.keys_in, 0xFF, sizeof(unsigned long long) * (size_t)n_sort, st));
       launch(ctx, k_wave_pick, seg_grid, WAVE_THREADS, 0, W, r, n_sort);
       sort(n_sort);
       launch(ctx, k_wave_merge, seg_grid, WAVE_THREADS, 0, W, r);
     }
     entries();
   }
-  // results
   std::vector<unsigned long long> scal((size_t)(4 * ni));
   CUDA(cudaMemcpyAsync(scal.data(), W.scal, sizeof(unsigned long long) * scal.size(), cudaMemcpyDeviceToHost, st));
-  for (long long i = 0; i < ni; ++i) {
-    blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
-    if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, W.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-    if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, W.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-    if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, W.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
-  }
   CUDA(cudaStreamSynchronize(st));
-  for (long long i = 0; i < ni; ++i) {
-    blance_scenario_schedule_out& o = sr.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
-    o.rounds = (int32_t)scal[(size_t)(4 * i)];
-    o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
-    o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
-    o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
-  }
+  return scal;
 }
 
 static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
@@ -1310,7 +1302,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     WSched wsch{};
     void* wtmp = nullptr;
     size_t wtmp_bytes = 0;
-    if (sr) sched_slices(wave, *base, nw, sr->nc, wsch, wtmp, wtmp_bytes, st);
+    if (sr) sched_slices(wave, nw, sr->nc, PU, NU, scenario_ops(*base), (long long)PU * scenario_ops(*base), wsch, wtmp, wtmp_bytes, st);
     int32_t* d_ow = nullptr;
     if (!ow.empty()) wave.add(d_ow, ow.size());
     try {
@@ -1398,7 +1390,23 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     }
     if (sr) {
       CUDA(cudaEventRecord(ctx->ev[3], st));
-      wave_schedule(ctx, pl, nw, *base, favor_min, *sr, wsch, wtmp, wtmp_bytes, h_sum.data(), stride, idx.data() + w0);
+      if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, wsch);
+      std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
+      for (size_t x = 0; x < ops.size(); ++x) {
+        const long long* s = h_sum.data() + (x / NU) * stride + 4 * (x % NU);
+        ops[x] = s[0] + s[1] + s[2] + s[3];
+      }
+      const std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
+      for (long long i = 0; i < (long long)nw * sr->nc; ++i) {
+        blance_scenario_schedule_out& o = sr->out[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
+        o.rounds = (int32_t)scal[(size_t)(4 * i)];
+        o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
+        o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
+        o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
+        if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+        if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+        if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
+      }
       CUDA(cudaEventRecord(ctx->ev[1], st));
       CUDA(cudaEventSynchronize(ctx->ev[1]));
       cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
@@ -1661,40 +1669,31 @@ extern "C" int blance_moves_available(blance_ctx* ctx, blance_moves* mv, const i
   });
 }
 
-// The lock-step schedule (include/blance_b200.h, schedule.cuh).  Rounds are enqueued in blocks of kSchedBlock; the
-// host reads the done flag and the active count once per block and bounds the next block's launches by that count.
-static const int kSchedBlock = 64;
-
+// The lock-step schedule (include/blance_b200.h) of the handle's CSR ops: one instance of the wave engine
+// (wave_schedule.cuh), which also writes round_off and sched_op into the handle.
 extern "C" int blance_moves_schedule(blance_ctx* ctx, blance_moves* mv, int32_t max_concurrent_per_node,
                                      const uint8_t* node_has_mover, blance_schedule_out* out) {
   return entry(ctx, [&](Device& device) {
     if (!ctx || !mv || !out) throw_err(BLANCE_ERR_INVALID_ARG, "blance_moves_schedule: ctx, moves or out is NULL");
     std::memset(out, 0, sizeof *out);
+    if (mv->n_parts >= (1 << WAVE_PART_BITS)) throw_err(BLANCE_ERR_UNSUPPORTED, "blance_moves_schedule: 2^29 or more partitions");
     blance_ctx* dev = device();
     cudaStream_t st = dev->stream;
     const int32_t P = mv->n_parts, NN = mv->n_node_ids;
     const long long T = mv->total_ops;
-    const int32_t count = max_concurrent_per_node <= 0 ? 1 : max_concurrent_per_node;   // orchestrate.go:484-487
-    int bits = 1;                                       // keys 0 .. NN (NN = past the active entries)
-    while (bits < 32 && (1ull << bits) <= (unsigned long long)NN) ++bits;
-    const size_t Pz = (size_t)std::max(P, 1), NNz = (size_t)std::max(NN, 1);
-    size_t sort_tmp = 0, sel_tmp = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                    (int32_t*)nullptr, std::max(P, 1), 0, bits, st);
-    cub::DeviceSelect::Flagged(nullptr, sel_tmp, (const int32_t*)nullptr, (const uint8_t*)nullptr, (int32_t*)nullptr,
-                               (int32_t*)nullptr, std::max(P, 1), st);
-    const size_t tmp_bytes = std::max(sort_tmp, sel_tmp) + 256;
-    SchedState* d_st;
-    int32_t *cur, *act, *act2, *list, *cnt, *noff, *boff;
-    uint32_t *key, *key2;
-    uint8_t *flags, *wl, *mover;
-    void* tmp;
+    SchedReq sr;
+    sr.nc = 1;
+    sr.count = {max_concurrent_per_node <= 0 ? 1 : max_concurrent_per_node};   // orchestrate.go:484-487
+    sr.mover.assign((size_t)NN, 1);
+    if (node_has_mover)
+      for (int q = 0; q < NN; ++q) sr.mover[(size_t)q] = node_has_mover[q] != 0;
+    WSched W{};
+    void* tmp = nullptr;
+    size_t tmp_bytes = 0;
+    unsigned long long* d_ops = nullptr;
     Arena scratch;
-    scratch.add(d_st, 1); scratch.add(cur, Pz); scratch.add(act, Pz);
-    scratch.add(act2, Pz); scratch.add(list, Pz); scratch.add(key, Pz);
-    scratch.add(key2, Pz); scratch.add(flags, Pz); scratch.add(wl, Pz);
-    scratch.add(cnt, NNz); scratch.add(noff, NNz + 1);
-    scratch.add(boff, NNz + 1); scratch.add(mover, NNz); scratch.add(tmp, tmp_bytes);
+    sched_slices(scratch, 1, 1, P, NN, 0, T, W, tmp, tmp_bytes, st);
+    scratch.add(d_ops, (size_t)std::max(NN, 1));
     scratch.alloc(st, "the schedule scratch");
     // results: round_off [T + 2] (R <= T) and sched_op [T], kept in the handle
     mv->sched.reset();
@@ -1704,59 +1703,26 @@ extern "C" int blance_moves_schedule(blance_ctx* ctx, blance_moves* mv, int32_t 
     res->add(mv->sched_op, (size_t)std::max(T, 1ll));
     res->alloc(st, "the schedule");
     mv->sched = std::move(res);
-    long long* round_off = mv->round_off;
-    SchedState h{};
+    W.op_off = mv->d_off; W.op_node = mv->d_node; W.op_kind = mv->d_kind;
+    W.round_off = mv->round_off; W.sched_op = mv->sched_op;
     CUDA(cudaEventRecord(dev->ev[0], st));
-    if (node_has_mover) CUDA(cudaMemcpyAsync(mover, node_has_mover, (size_t)NN, cudaMemcpyHostToDevice, st));
-    else CUDA(cudaMemsetAsync(mover, 1, NNz, st));
-    CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * NNz, st));
-    launch(dev, k_sched_init, grid_for(dev, P, 256), 256, 0, P, cur, act2, round_off, d_st);
-    int32_t a_bound = 0;
-    if (P > 0) {                                        // the first compaction: partitions with a pickable first move
-      launch(dev, k_sched_flags, grid_for(dev, P, 256), 256, 0, P, act2, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
-      size_t tb = tmp_bytes;
-      CUDA(cub::DeviceSelect::Flagged(tmp, tb, act2, flags, act, &d_st->A, P, st));
-      CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
-      CUDA(cudaStreamSynchronize(st));
-      a_bound = h.A;
-    }
-    const int pick_grid = (int)std::min<long long>((NNz + SCHED_PICK_THREADS / 32 - 1) / (SCHED_PICK_THREADS / 32), (long long)dev->sm_count * 16);
-    long long launched = 0;
-    while (a_bound > 0) {
-      if (launched > T + kSchedBlock) throw_err(BLANCE_ERR_CUDA, "blance_moves_schedule: the schedule did not end (internal error)");
-      for (int r = 0; r < kSchedBlock; ++r) {
-        const int g = grid_for(dev, a_bound, 256);
-        launch(dev, k_sched_keys, g, 256, 0, a_bound, act, mv->d_off, mv->d_node, cur, NN, key, cnt, d_st);
-        size_t tb = tmp_bytes;
-        CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, key, key2, act, list, a_bound, 0, bits, st));
-        launch(dev, k_sched_scan, 1, SCHED_SCAN_THREADS, 0, NN, count, cnt, noff, boff, round_off, d_st);
-        launch(dev, k_sched_pick, pick_grid, SCHED_PICK_THREADS, 0, NN, count, noff, boff, list, wl, mv->d_off, mv->d_kind, cur,
-               mv->sched_op, d_st);
-        launch(dev, k_sched_flags, g, 256, 0, a_bound, act, mv->d_off, mv->d_node, cur, mover, NN, flags, d_st);
-        tb = tmp_bytes;
-        CUDA(cub::DeviceSelect::Flagged(tmp, tb, act, flags, act2, &d_st->A, a_bound, st));
-        std::swap(act, act2);
-        ++launched;
-      }
-      CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
-      CUDA(cudaStreamSynchronize(st));
-      if (h.done) break;
-      a_bound = h.A;
-    }
-    long long moves_done = 0;
-    CUDA(cudaMemcpyAsync(&h, d_st, sizeof h, cudaMemcpyDeviceToHost, st));
+    // segment capacities: the ops on each node
+    std::vector<long long> ops((size_t)NN);
+    CUDA(cudaMemsetAsync(d_ops, 0, sizeof(unsigned long long) * (size_t)NN, st));
+    if (T > 0 && NN > 0) launch(dev, k_wave_node_ops, grid_for(dev, T, 256), 256, 0, T, mv->d_node, NN, d_ops);
+    CUDA(cudaMemcpyAsync(ops.data(), d_ops, sizeof(long long) * (size_t)NN, cudaMemcpyDeviceToHost, st));
     CUDA(cudaStreamSynchronize(st));
-    CUDA(cudaMemcpyAsync(&moves_done, round_off + h.rounds, sizeof moves_done, cudaMemcpyDeviceToHost, st));
+    const std::vector<unsigned long long> scal = wave_schedule(dev, "blance_moves_schedule", sr, W, tmp, tmp_bytes, ops.data());
     CUDA(cudaEventRecord(dev->ev[1], st));
     CUDA(cudaStreamSynchronize(st));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, dev->ev[0], dev->ev[1]);
-    mv->sched_rounds = h.rounds;
-    mv->sched_moves = moves_done;
-    out->rounds = h.rounds;
-    out->moves_done = moves_done;
-    out->stuck_parts = (int64_t)h.stuck;
-    out->max_batch = h.max_batch;
+    mv->sched_rounds = (int32_t)scal[0];
+    mv->sched_moves = (long long)scal[1];
+    out->rounds = (int32_t)scal[0];
+    out->moves_done = (int64_t)scal[1];
+    out->stuck_parts = (int64_t)scal[2];
+    out->max_batch = (int32_t)scal[3];
     out->device_ms = ms;
   });
 }

@@ -431,7 +431,8 @@ int blance_moves_available(blance_ctx* ctx, blance_moves* moves, const int32_t* 
  * blance_moves_schedule_fetch copies it out (round_off: R+1 entries, sched_op: moves_done entries; either may be
  * NULL).  Scratch is allocated and freed inside the call; blance_moves_available is not affected.  Repeated calls
  * give identical results.  node_has_mover: [n_node_ids], NULL = every id has a mover.  Errors: NULL ctx, handle or
- * out (BLANCE_ERR_INVALID_ARG); fetch before any schedule (BLANCE_ERR_INVALID_ARG). */
+ * out (BLANCE_ERR_INVALID_ARG); a handle with 2^29 or more partitions (BLANCE_ERR_UNSUPPORTED, before any device
+ * work); fetch before any schedule (BLANCE_ERR_INVALID_ARG). */
 typedef struct blance_schedule_out {
   int32_t rounds;        /* R */
   int64_t moves_done;    /* ops scheduled = length of sched_op = round_off[R] */

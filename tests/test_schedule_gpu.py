@@ -161,6 +161,13 @@ def test_edges(ctx):
     ro, so, sc = ctx.moves_schedule(h, 2, np.zeros(41, np.uint8))
     assert sc["rounds"] == 0 and sc["moves_done"] == 0 and sc["stuck_parts"] == P and ro.tolist() == [0]
     ctx.moves_free(h)
+    # 320 ops per partition: 160 slots per row, every node changing
+    perms = np.stack([rng.permutation(320) for _ in range(3)]).astype(np.int32)
+    h, total = ctx.moves_create(np.array([0, 160], np.int32), perms[:, :160], perms[:, 160:], False, 320)
+    for c in (1, 4):
+        off, _, _, _, _, _ = schedule_both(ctx, h, total, c)
+        assert np.diff(off).min() == 320
+    ctx.moves_free(h)
 
 
 def test_repeated_calls_leave_available_moves_alone(ctx):

@@ -199,9 +199,10 @@ def test_null_arguments_are_invalid_without_a_device():
 CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
 
 
-def test_schedule_kernels_issue_value_less_atomics_as_red():
-    """k_sched_keys (per-node list lengths) and k_sched_flags (stuck count) discard their atomics' results: they
-    must compile to RED, not to ATOM with a return value the warp would wait for."""
+def test_wave_kernels_issue_value_less_atomics_as_red():
+    """The schedule engine's kernels (k_wave_*, wave_schedule.cuh) discard their atomics' results: the per-node op
+    histogram, the stuck counts and the per-instance summaries must compile to RED, not to ATOM with a return value
+    the warp would wait for."""
     try:
         txt = subprocess.run([CUOBJDUMP, "-sass", build.lib_path()], stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=300).stdout
     except (OSError, subprocess.TimeoutExpired):
@@ -214,12 +215,12 @@ def test_schedule_kernels_issue_value_less_atomics_as_red():
             kernels[name] = []
         elif name and re.match(r"\s*/\*[0-9a-f]{4,6}\*/", line):
             kernels[name].append(line)
-    sched = {k: "\n".join(v) for k, v in kernels.items() if "k_sched_" in k}
+    sched = {k: "\n".join(v) for k, v in kernels.items() if "k_wave_" in k}
     if not sched:
         pytest.skip("cuobjdump printed no SASS")
-    assert len(sched) == 5, sorted(sched)
+    assert len(sched) == 6, sorted(sched)
     for k, body in sched.items():
         assert not re.search(r"ATOMG?\.\S+ PT, RZ,", body), k
-    for want in ("k_sched_keys", "k_sched_flags"):
+    for want in ("k_wave_pick", "k_wave_first", "k_wave_node_ops"):
         body = next(b for k, b in sched.items() if want in k)
         assert re.search(r"\bREDG?\.", body), want
