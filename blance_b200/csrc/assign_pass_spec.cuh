@@ -31,9 +31,12 @@
 //     that the K-th winner is below `ub` give the reference's first K nodes without looking at the other
 //     nodes.  A mover updates the mirror, the matrices, the list and the epoch - about a microsecond,
 //     against a CTA-wide N-way arg-min per pick in the other kernels.
-//   * Rows that are not clean, a failed proof and a list that has run dry go to the TEAM: the scouts stop
-//     sweeping and run the full evaluation / the list rebuild together (named barriers), exactly as the
-//     lock-step kernel would.
+//   * Every node's base key is CACHED in shared memory and rewritten by whoever changes the node.  A failed
+//     proof with K winners is still the leader's: it scans the cached keys for the few nodes between ub and
+//     the K-th winner and scores them too (the extended resolve).
+//   * Rows that are not clean, a failed proof with too many such nodes and a list that has run dry go to the
+//     TEAM: the scouts stop sweeping and run the full evaluation / the list rebuild together (named
+//     barriers), exactly as the lock-step kernel would.
 //
 // Exactness never depends on timing: a result is only used under the two tests above, anything else falls
 // through to an exact evaluation.  tools/spec_model.c checks these rules step by step inside the CPU oracle.
@@ -74,10 +77,19 @@ namespace blance_dev {
 #ifndef SP_LMIN
 #define SP_LMIN 4            // rebuild the list when fewer entries are left (and it is not complete)
 #endif
+#ifndef SP_XMAX
+#define SP_XMAX 64           // extended resolve: at most this many nodes beyond the list (SP_XMAX / 32 per leader lane); more: the team
+#endif
+#define SP_XPL (SP_XMAX / 32)
+#ifndef SP_XRES
+#define SP_XRES 1            // 0: failed proofs go to the team (no extended resolve)
+#endif
 
 enum : int { SPB_ALL = 8, SPB_GO = 9, SPB_DONE = 10, SPB_TEAM = 11 };
 enum : int32_t { SP_OP_EXIT = 1, SP_OP_REBUILD = 2, SP_OP_FULL = 3 };
 enum : uint32_t { SPZ_NEVER = 0x80000000u };
+// leader path counts of a pass (SpecCtl::stat): team commands by cause, extended resolves
+enum : int { SPS_FULL_PROOF = 0, SPS_FULL_OTHER = 1, SPS_REB_DRY = 2, SPS_FULL_MOVED = 3, SPS_XRES = 4, SPS_XOVER = 5, SPS_N = 8 };
 
 struct SpecCtl {
   uint4 xchg[2][32];                 // team arg-min partials
@@ -89,6 +101,8 @@ struct SpecCtl {
   int32_t epoch, front, cmd_seq, cmd_op, cmd_arg, cmd_epoch;
   int32_t res_n, res_same;
   int32_t res_chosen[BL_K_MAX];
+  int32_t xnode[SP_XMAX];            // extended resolve: the nodes found by the scan of the base keys
+  int32_t stat[SPS_N];               // leader path counts (lane 0 of the leader; SPS_*)
 #ifdef BLANCE_SPEC_TIMING
   int32_t probe;                     // timing builds: a store that waits for the resolve's n2n values
 #endif
@@ -97,7 +111,7 @@ struct SpecCtl {
 __host__ __device__ inline size_t spec_dyn_smem_bytes(int N, int SW) {
   const size_t H = (size_t)32 * SW * SP_D;
   const size_t Np = ((size_t)N + 3) & ~(size_t)3;        // every array starts 16-byte aligned
-  size_t b = Np * 32 + Np * 4 + Np * 4 + ((Np + 15) & ~(size_t)15);
+  size_t b = Np * 32 + Np * 8 + Np * 4 + Np * 4 + ((Np + 15) & ~(size_t)15);   // mirror, base keys, totals, stamps, flags
   b += H * 64 + H * 16 + H * 16;       // records (<= 16 words), qstat, results
   return b;
 }
@@ -114,6 +128,14 @@ __device__ __forceinline__ int32_t lds32v(uint32_t a) {
 }
 __device__ __forceinline__ void sts32v(uint32_t a, int32_t x) {
   asm volatile("st.volatile.shared.b32 [%0], %1;" :: "r"(a), "r"(x) : "memory");
+}
+__device__ __forceinline__ unsigned long long lds64u(uint32_t a) {
+  unsigned long long v;
+  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ void sts64u(uint32_t a, unsigned long long x) {
+  asm volatile("st.shared.b64 [%0], %1;" :: "r"(a), "l"(x) : "memory");
 }
 __device__ __forceinline__ void mbar_init(uint32_t a, int cnt) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(a), "r"(cnt) : "memory");
@@ -196,7 +218,8 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
   const uint32_t base_a = (uint32_t)__cvta_generic_to_shared(dyn_smem);
   const uint32_t Np = ((uint32_t)N + 3u) & ~3u;                  // (padded: every array starts 16-byte aligned)
   const uint32_t nd_a = base_a;                                  // mirror: {cd, ff, wd, wy} per node
-  const uint32_t tot_a = nd_a + 32u * Np;                        // all-state totals
+  const uint32_t bk_a = nd_a + 32u * Np;                         // base keys (~0 for removed nodes and the padding)
+  const uint32_t tot_a = bk_a + 8u * Np;                         // all-state totals
   const uint32_t chg_a = tot_a + 4u * Np;                        // lastchg
   const uint32_t flg_a = chg_a + 4u * Np;                        // NF_VALID | NF_BOOST
   const uint32_t rec_a = flg_a + ((Np + 15u) & ~15u);            // ring: records
@@ -233,15 +256,18 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
     const double ff = have_p ? div_exact(__dmul_rn(0.001, (double)t), Pd, Py) : 0.0;   // plan.go:650
     double* nd = reinterpret_cast<double*>(dyn_smem) + 4 * (size_t)n;
     nd[0] = cd; nd[1] = ff; nd[2] = wd; nd[3] = wy;
+    sts64u(bk_a + 8u * n, (fl & NF_VALID) ? sp_key(cd, ff, wd, wy, (fl & NF_BOOST) != 0, has_nw, 0, 0.0, have_p, Pd, Py) : ~0ull);
     sts32(tot_a + 4u * n, t);
     sts32(chg_a + 4u * n, 0);
     dyn_smem[(flg_a - base_a) + n] = (unsigned char)fl;
   }
+  for (int n = N + atid; n < (int)Np; n += NTA) sts64u(bk_a + 8u * n, ~0ull);
   for (int i = atid; i < H; i += NTA) sts128(dyn_a + 16u * i, 0u, 0u, (uint32_t)SP_GEN_MOD << 21, 0u);
   if (atid == 0) {
     for (int i = 0; i < SWD; ++i) mbar_init(mbar_a + 8u * i, 1);
     ctl.epoch = 0; ctl.front = 0; ctl.cmd_seq = 0; ctl.cmd_op = 0; ctl.cmd_arg = 0; ctl.cmd_epoch = 0;
     ctl.res_n = 0; ctl.res_same = 0;
+    for (int x = 0; x < SPS_N; ++x) ctl.stat[x] = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -422,10 +448,13 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
                   }
                   if (tk) { cd = __dadd_rn(cd, wpd); t += w_p; }
                   nd[0] = cd;
+                  double ff = nd[1];
                   if (t != t0) {
                     sts32(tot_a + 4u * n, t);
-                    if (have_p) nd[1] = div_exact(__dmul_rn(0.001, (double)t), Pd, Py);
+                    if (have_p) { ff = div_exact(__dmul_rn(0.001, (double)t), Pd, Py); nd[1] = ff; }
                   }
+                  const uint32_t fl = dyn_smem[(flg_a - base_a) + n];
+                  sts64u(bk_a + 8u * n, (fl & NF_VALID) ? sp_key(cd, ff, nd[2], nd[3], (fl & NF_BOOST) != 0, has_nw, 0, 0.0, have_p, Pd, Py) : ~0ull);
                   sts32(chg_a + 4u * n, E1);
                 }
               }
@@ -434,30 +463,16 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           }
           if (changed) {
             // ---- rebuild: every scout warp extracts its M_ext smallest base keys and a lower bound of the rest ---
+            // (from the cached base keys: whoever changes a node's mirror entry rewrites its key)
             unsigned long long bkey[SP_NPTS];
             uint32_t live = 0;
 #pragma unroll
-            for (int j = 0; j < SP_NPTS; ++j) bkey[j] = ~0ull;
-#pragma unroll
-            for (int h = 0; h < SP_NPTS; h += 4) {
-              if (SW * 32 * h >= N) break;                                                 // (uniform)
-              int4 ma[4], mb[4];
-              uint32_t fl[4];
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const int n = team_node(h + jj);
-                const uint32_t nx = n < N ? (uint32_t)n : 0u;
-                ma[jj] = lds128(nd_a + nx * 32u);
-                mb[jj] = lds128(nd_a + nx * 32u + 16u);
-                fl[jj] = dyn_smem[(flg_a - base_a) + nx];
-              }
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const int j = h + jj;
-                const unsigned long long k =
-                    sp_key(__hiloint2double(ma[jj].y, ma[jj].x), __hiloint2double(ma[jj].w, ma[jj].z), __hiloint2double(mb[jj].y, mb[jj].x),
-                           __hiloint2double(mb[jj].w, mb[jj].z), (fl[jj] & NF_BOOST) != 0, has_nw, 0, 0.0, have_p, Pd, Py);
-                if (team_node(j) < N && (fl[jj] & NF_VALID)) { bkey[j] = k; live |= 1u << j; }
+            for (int j = 0; j < SP_NPTS; ++j) {
+              const int n = team_node(j);
+              bkey[j] = ~0ull;
+              if (n < N) {
+                bkey[j] = lds64u(bk_a + 8u * (uint32_t)n);
+                if (dyn_smem[(flg_a - base_a) + n] & NF_VALID) live |= 1u << j;
               }
             }
             for (int r = 0; r <= M_ext; ++r) {
@@ -590,8 +605,11 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
   long long n_fast = 0, n_res = 0, n_mov = 0, n_team = 0, n_reb = 0, n_wait = 0, n_stale = 0;
   long long cyc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tc = clock64();   // the slots of DInst::spec_cyc
   const long long t_begin = tc;
+  // path counts kept in shared memory (no leader registers): only rare paths touch them
+  auto sp_bump = [&](int x) { if (lane == 0) { volatile int32_t* p = &ctl.stat[x]; *p = *p + 1; } };
 #ifdef BLANCE_SPEC_TIMING
-  long long cyc_n2n = 0, n_pfo = 0;
+  long long cyc_n2n = 0, n_pfo = 0, cyc_x = 0;
+  long long tcyc[4] = {0, 0, 0, 0};        // team cycles by cause (SPS_FULL_PROOF .. SPS_FULL_MOVED)
   int pf_next = -1;                        // the next step the last resolve's scan showed as not accepted
 #define SP_PF_LOST() do { pf_next = -1; } while (0)
 #else
@@ -622,7 +640,9 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
     for (int u = 0; u < SP_LPL; ++u)
       if (Ln[u] >= 0 && lex_lt(Lk[u], (uint32_t)Ln[u], bk, bp)) { bk = Lk[u]; bp = (uint32_t)Ln[u]; }
     const Best b = warp_argmin(Best{(uint32_t)(bk >> 32), (uint32_t)bk, bp});
-    if (b.pos != 0xFFFFFFFFu) { B0k = ((unsigned long long)b.hi << 32) | b.lo; B0p = b.pos; }
+    const unsigned long long lk = ((unsigned long long)b.hi << 32) | b.lo;
+    // (ub, when a mover found no room in the list, may lie below every listed key: B0 is the smaller of the two)
+    if (b.pos != 0xFFFFFFFFu && lex_lt(lk, b.pos, ubk, ubp)) { B0k = lk; B0p = b.pos; }
     else { B0k = ubk; B0p = ubp; }
   };
   auto adopt_list = [&]() {                 // after a team rebuild: cand[] / bound[] -> list, ub, B0
@@ -864,6 +884,113 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           }
 #endif
           same = resolved && hit_all && n_ch == n_cur && n_cur == K;
+          if (SP_XRES && !resolved && n_ch == K) {
+            // ---- extended resolve: the proof failed, W = (lastk, lastp) is the K-th winner among listed + current --------
+            // A node's exact score is never below its base key, and every node whose base key is below ub is listed.  So
+            // besides the listed and the current nodes only the nodes with ub <= (base key, node) <= W can be among the
+            // first K: any other node is beaten by the K candidates at or below W.  Their exact scores and K arg-mins over
+            // all three groups give the step.  One pass is enough: the new K-th winner is <= W, so no node beyond the
+            // set can enter.  (Listed nodes found by the scan - ub may have been lowered below them - appear twice with
+            // the same key; a pick clears every entry of its node.)  More than SP_XMAX such nodes: the team evaluates
+            // the step.
+#ifdef BLANCE_SPEC_TIMING
+            const long long tx0 = clock64();
+#endif
+            // the scan: lane l looks at nodes l + 32 j and sets bit j of xm for ub <= (k, n) <= W, i.e. k >= ubk (ubk + 1
+            // when n < ubp) and k <= lastk (lastk - 1 when n > lastp)
+            unsigned long long xm = 0;
+            const unsigned long long lastk1 = lastk - 1, ubk1 = ubk + 1;
+            for (int j0 = 0; 32 * j0 < N; j0 += 8) {
+              unsigned long long k[8];
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {                              // (all eight loads in flight together)
+                const int n = lane + 32 * (j0 + jj);
+                k[jj] = lds64u(bk_a + 8u * (uint32_t)(n < N ? n : 0));
+              }
+              uint32_t byte = 0;
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int n = lane + 32 * (j0 + jj);
+                const unsigned long long top = n <= (int)lastp ? lastk : lastk1, bot = (uint32_t)n >= ubp ? ubk : ubk1;
+                byte |= (n < N && k[jj] >= bot && k[jj] <= top) ? 1u << jj : 0u;
+              }
+              xm |= (unsigned long long)byte << j0;
+            }
+            const int xc = __popcll(xm);
+            int xpre = xc;                                                  // inclusive prefix sum over the lanes
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+              const int v = __shfl_up_sync(0xFFFFFFFFu, xpre, o);
+              if (lane >= o) xpre += v;
+            }
+            const int cnt = __shfl_sync(0xFFFFFFFFu, xpre, 31);
+            if (cnt <= SP_XMAX) {
+              for (int r = xpre - xc; xm; ++r) {                            // compact: lane + 32 u takes entry u
+                ctl.xnode[r] = lane + 32 * (__ffsll((long long)xm) - 1);
+                xm &= xm - 1;
+              }
+              __syncwarp();
+              int32_t xn[SP_XPL];
+#pragma unroll
+              for (int u = 0; u < SP_XPL; ++u) xn[u] = lane + 32 * u < cnt ? ctl.xnode[lane + 32 * u] : -1;
+              // the listed and current columns as they were before the picks (a pick clears its winner's entry)
+#pragma unroll
+              for (int u = 0; u < SP_LPL; ++u) cnode[u] = Ln[u];
+              cnode[SP_LPL] = lane < n_cur ? mycur : -1;
+#pragma unroll
+              for (int sl = 0; sl < 8; ++sl) {
+                const int32_t x = __shfl_sync(0xFFFFFFFFu, myslot, sl);
+                if ((slot_blocked >> sl) & 1u) {
+#pragma unroll
+                  for (int u = 0; u < SP_LPL; ++u) if (cnode[u] == x) cnode[u] = -1;
+#pragma unroll
+                  for (int u = 0; u < SP_XPL; ++u) if (xn[u] == x) xn[u] = -1;
+                }
+              }
+              int32_t xq[SP_XPL];
+#pragma unroll
+              for (int u = 0; u < SP_XPL; ++u) xq[u] = (xn[u] >= 0 && have_p) ? ld_relaxed_gpu(Gt + xn[u]) : 0;
+              unsigned long long xk[SP_XPL];
+#pragma unroll
+              for (int u = 0; u < SP_XPL; ++u) {
+                const uint32_t nx = xn[u] >= 0 ? (uint32_t)xn[u] : 0u;
+                const int4 ma = lds128(nd_a + nx * 32u), mb = lds128(nd_a + nx * 32u + 16u);
+                const uint32_t fl = dyn_smem[(flg_a - base_a) + nx];
+                const unsigned long long k =
+                    sp_key(__hiloint2double(ma.y, ma.x), __hiloint2double(ma.w, ma.z), __hiloint2double(mb.y, mb.x),
+                           __hiloint2double(mb.w, mb.z), (fl & NF_BOOST) != 0, has_nw, xq[u], 0.0, have_p, Pd, Py);
+                xk[u] = xn[u] >= 0 ? k : ~0ull;
+              }
+              n_ch = 0;
+              hit_all = true;
+              for (int t = 0; t < K; ++t) {
+                unsigned long long bk = ~0ull;
+                uint32_t bp = 0xFFFFFFFFu;
+#pragma unroll
+                for (int u = 0; u <= SP_LPL; ++u)
+                  if (cnode[u] >= 0 && lex_lt(ck[u], (uint32_t)cnode[u], bk, bp)) { bk = ck[u]; bp = (uint32_t)cnode[u]; }
+#pragma unroll
+                for (int u = 0; u < SP_XPL; ++u)
+                  if (xn[u] >= 0 && lex_lt(xk[u], (uint32_t)xn[u], bk, bp)) { bk = xk[u]; bp = (uint32_t)xn[u]; }
+                const Best b = warp_argmin(Best{(uint32_t)(bk >> 32), (uint32_t)bk, bp});
+                chosen[t] = (int32_t)b.pos;                                 // (K candidates are at or below W)
+                ++n_ch;
+                hit_all = hit_all && __any_sync(0xFFFFFFFFu, cnode[SP_LPL] == (int32_t)b.pos);
+#pragma unroll
+                for (int u = 0; u <= SP_LPL; ++u) if (cnode[u] == (int32_t)b.pos) cnode[u] = -1;
+#pragma unroll
+                for (int u = 0; u < SP_XPL; ++u) if (xn[u] == (int32_t)b.pos) xn[u] = -1;
+              }
+              resolved = true;
+              same = hit_all && n_ch == n_cur && n_cur == K;
+              sp_bump(SPS_XRES);
+            } else {
+              sp_bump(SPS_XOVER);
+            }
+#ifdef BLANCE_SPEC_TIMING
+            cyc_x += clock64() - tx0;
+#endif
+          }
         }
       }
       SP_T(3);
@@ -871,6 +998,11 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
         // ---- the team evaluates the step (and rebuilds the list if a count changed) ----------------------------------
         ++n_team;
         SP_PF_LOST();
+        const int why = n_ch == K ? SPS_FULL_PROOF : SPS_FULL_OTHER;     // (n_ch == K only after a failed proof)
+        sp_bump(why);
+#ifdef BLANCE_SPEC_TIMING
+        const long long tt0 = tc;
+#endif
         team_cmd(SP_OP_FULL, i);
         n_ch = *(volatile int32_t*)&ctl.res_n;
         same = *(volatile int32_t*)&ctl.res_same != 0;
@@ -882,8 +1014,12 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
           for (int t = 0; t < K; ++t) orec[t] = chosen[t];
           orec[K] = n_ch;
         }
-        if (!same) { adopt_list(); publish_epoch(); ++n_mov; }
+        if (!same) { adopt_list(); publish_epoch(); ++n_mov; sp_bump(SPS_FULL_MOVED); }
         SP_T(6);
+#ifdef BLANCE_SPEC_TIMING
+        tcyc[why] += tc - tt0;
+        if (!same) tcyc[SPS_FULL_MOVED] += tc - tt0;
+#endif
       } else {
         int32_t* orec = ostream + (size_t)i * REC;
         if (lane == 0) {
@@ -953,6 +1089,7 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
             nd[0] = cd; nd[1] = ff;
             sts32(chg_a + 4u * (uint32_t)x, E1);
             nk = sp_key(cd, ff, __hiloint2double(mb.y, mb.x), __hiloint2double(mb.w, mb.z), (fl & NF_BOOST) != 0, has_nw, 0, 0.0, have_p, Pd, Py);
+            sts64u(bk_a + 8u * (uint32_t)x, (fl & NF_VALID) ? nk : ~0ull);
             ins = (fl & NF_VALID) && lex_lt(nk, (uint32_t)x, ubk, ubp);
           }
           __syncwarp();
@@ -992,9 +1129,16 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
             publish_epoch();
             SP_T(5);
             SP_PF_LOST();
-            team_cmd(SP_OP_REBUILD, 0);                                 // reads the mirror only
+            sp_bump(SPS_REB_DRY);
+#ifdef BLANCE_SPEC_TIMING
+            const long long tt0 = tc;
+#endif
+            team_cmd(SP_OP_REBUILD, 0);                                 // reads the base keys only
             adopt_list();
             SP_T(6);
+#ifdef BLANCE_SPEC_TIMING
+            tcyc[SPS_REB_DRY] += tc - tt0;
+#endif
           } else {
             recompute_b0();
             publish_epoch();
@@ -1021,9 +1165,12 @@ __global__ void __launch_bounds__(SP_LB, 1) k_assign_pass_spec(DPool pool, int s
 #endif
     cyc[7] = clock64() - t_begin;
     for (int x = 0; x < 8; ++x) D.spec_cyc[x] += cyc[x];
+    for (int x = 0; x < 6; ++x) D.spec_path[x] += *(volatile int32_t*)&ctl.stat[x];
 #ifdef BLANCE_SPEC_TIMING
     D.spec_cyc_n2n += cyc_n2n;
     D.spec_pf_opp += n_pfo;
+    D.spec_cyc_x += cyc_x;
+    for (int x = 0; x < 4; ++x) D.spec_cyc_team[x] += tcyc[x];
 #endif
   }
 #undef SP_T

@@ -914,7 +914,12 @@ static void fetch(blance_ctx* ctx, blance_plan* pl, blance_plan_out* outs) {
                    fin[i].spec_cyc[0], fin[i].spec_cyc[1], fin[i].spec_cyc[2], fin[i].spec_cyc[3], fin[i].spec_cyc[4], fin[i].spec_cyc[5],
                    fin[i].spec_cyc[6], fin[i].spec_cyc[7]),
       std::fprintf(stderr, "[blance]   of the resolve loads+keys: waiting for n2n %lld | resolves whose step the previous ballot named next %lld\n",
-                   fin[i].spec_cyc_n2n, fin[i].spec_pf_opp);
+                   fin[i].spec_cyc_n2n, fin[i].spec_pf_opp),
+      std::fprintf(stderr, "[blance]   team: full after a failed proof %lld (%lld cycles) | full, other rows %lld (%lld cycles) | rebuild, list dry %lld"
+                           " (%lld cycles) | full that moved %lld (%lld cycles) | extended resolves %lld, too large %lld (%lld cycles)\n",
+                   fin[i].spec_path[0], fin[i].spec_cyc_team[0], fin[i].spec_path[1], fin[i].spec_cyc_team[1], fin[i].spec_path[2],
+                   fin[i].spec_cyc_team[2], fin[i].spec_path[3], fin[i].spec_cyc_team[3], fin[i].spec_path[4], fin[i].spec_path[5],
+                   fin[i].spec_cyc_x);
   for (int i = 0; i < n; ++i) {
     const DInst& D = pl->h_insts[i];
     blance_plan_out& o = outs[i];

@@ -61,6 +61,12 @@ struct DInst {
   long long spec_cyc[8];   // leader cycles: scans | waits | resolve loads+keys | resolve picks | mover mirror | mover list+publish | team | passes
   long long spec_cyc_n2n;  // of resolve loads+keys: the cycles spent waiting for the n2n values (timing builds)
   long long spec_pf_opp;   // resolves whose step the previous resolve's ballot had shown as the next one not accepted (timing builds)
+  long long spec_path[6];  // team evaluations after a failed proof (K winners) | other team evaluations (row not clean,
+                           // n_cur > k, a dead current node, too few candidates) | list rebuilds because the list ran
+                           // dry | team evaluations that moved data (and rebuilt the list) | extended resolves |
+                           // extended scans that found more than SP_XMAX nodes (then a team evaluation)
+  long long spec_cyc_team[4];  // of spec_cyc[6], by the first four causes of spec_path (the fourth is part of the first two; timing builds)
+  long long spec_cyc_x;    // of spec_cyc[3]: the extended scans and resolves (timing builds)
   long long spec_abort;    // the speculative kernel's watchdog fired (a bug: the plan is reported as failed)
   long long spec_round2;   // resolves that had to look at the second list column
   long long spec_cwait;    // resolves that had to wait for the committer (a pending commit shared their top node)

@@ -25,10 +25,19 @@ static void spec_pass(void* f, const void* order, int32_t lim, int32_t s);
 #define FO_PASS(f, order, lim, s) spec_pass((void*)(f), (const void*)(order), (lim), (s))
 #include "../oracle/fast.c"
 
+/* extended resolve of a failed bound proof (K winners found, the K-th not below ub): the exact scores of the unlisted,
+ * live, unblocked nodes whose base key is lex-below the K-th winner decide the step together with the listed and the
+ * current nodes.  xhist: how many such nodes there were, in buckets 0 | 1 | 2 | 3-4 | 5-8 | 9-16 | 17-32 | 33-64 |
+ * 65-128 | more. */
+#define XHIST 10
 typedef struct {
   long long steps, elig, fast, slow_sticky, movers, inelig, stale, t_ge_b0;
   long long list_ok, list_fail, list_rebuild, list_ok_sticky;
   long long asserts_failed;
+  long long list_fail_k;               /* of list_fail: K winners found (the extended resolve applies) */
+  long long xres_ok;                   /* extended resolves checked against the oracle's outcome */
+  long long xmax;                      /* the largest extended set */
+  long long xhist[XHIST];
 } spec_stats_t;
 static spec_stats_t g_st;
 static int g_H = 256, g_resweeps = 2, g_L = 32, g_Lmin = 6;
@@ -191,30 +200,64 @@ static void spec_pass(void* fv, const void* ov, int32_t lim, int32_t s) {
 
     /* list-based resolution of the steps the scouts did not decide */
     int list_pred = 0; int32_t list_ch[4]; int list_n = 0;
+    int x_pred = 0; int32_t x_ch[4];
     if (!predicted && r->elig && Llen > 0) {
       const int32_t* row = row_of(f->rows, f->SL, r->p);
+#define BLOCKED(n_, out_) do { \
+        out_ = 0; \
+        for (int q_ = 0; q_ < K; q_++) out_ |= (r->cur[q_] == (n_)); \
+        for (int s2_ = 0; s2_ < f->S; s2_++) \
+          if (((higher >> s2_) & 1u) && f->shape[(size_t)r->p * f->S + s2_] != BLANCE_SHAPE_ABSENT) \
+            out_ |= list_has(row, in->state_slot_off[s2_], in->state_slot_off[s2_ + 1], (n_)); } while (0)
       /* candidates: current nodes + listed nodes, minus nodes of higher-priority states, minus dead nodes */
-      int32_t cn[40]; double ck[40]; int nc = 0;
+      int32_t* cn = (int32_t*)malloc(sizeof(int32_t) * ((size_t)N + 8)); double* ck = (double*)malloc(sizeof(double) * ((size_t)N + 8));
+      uint8_t* used = (uint8_t*)calloc((size_t)N + 8, 1);
+      int nc = 0;
       for (int q = 0; q < K; q++) if (f->valid[r->cur[q]]) { cn[nc] = r->cur[q]; ck[nc] = score_q(f, s, r->cur[q], f->n2n[(size_t)r->top * N + r->cur[q]], r->stick); nc++; }
       for (int x = 0; x < Llen; x++) {
         const int32_t n = L[x].n;
-        int blocked = 0;
-        for (int q = 0; q < K; q++) blocked |= (r->cur[q] == n);
-        for (int s2 = 0; s2 < f->S; s2++)
-          if (((higher >> s2) & 1u) && f->shape[(size_t)r->p * f->S + s2] != BLANCE_SHAPE_ABSENT)
-            blocked |= list_has(row, in->state_slot_off[s2], in->state_slot_off[s2 + 1], n);
+        int blocked;
+        BLOCKED(n, blocked);
         if (blocked) continue;
         cn[nc] = n; ck[nc] = score_q(f, s, n, f->n2n[(size_t)r->top * N + n], 0.0); nc++;
       }
       /* current nodes held by a higher-priority state are not candidates either (row clean => cannot happen) */
-      uint8_t used[40] = {0};
+      double wk = 0.0; int32_t wn = -1;
       for (int t = 0; t < K && t < nc; t++) {
         int b = -1;
         for (int x = 0; x < nc; x++) if (!used[x] && (b < 0 || lex_lt(ck[x], cn[x], ck[b], cn[b]))) b = x;
         used[b] = 1; list_ch[list_n++] = cn[b];
+        wk = ck[b]; wn = cn[b];
         if (t == K - 1 && lex_lt(ck[b], cn[b], ubk, ubp)) list_pred = 1;
       }
       if (list_n < K) list_pred = 0;
+      if (!list_pred && list_n == K) {
+        /* the extended resolve: every node outside listed + current whose base key is lex-below the K-th winner W.
+         * A node's exact score is never below its base key, so a node whose base key is not below W cannot beat
+         * the K candidates already at or below W; the new K-th winner is <= W, so the set never has to grow. */
+        g_st.list_fail_k++;
+        int nx = 0;
+        for (int32_t n = 0; n < N; n++) {
+          if (!f->valid[n] || listed[n] || !lex_lt(base[n], n, wk, wn)) continue;
+          int blocked;
+          BLOCKED(n, blocked);
+          if (blocked) continue;
+          cn[nc] = n; ck[nc] = score_q(f, s, n, f->n2n[(size_t)r->top * N + n], 0.0); nc++; nx++;
+        }
+        int hb = 0;
+        while (hb < XHIST - 1 && nx > (hb == 0 ? 0 : (1 << (hb - 1)))) hb++;
+        g_st.xhist[hb]++;
+        if (nx > g_st.xmax) g_st.xmax = nx;
+        memset(used, 0, (size_t)nc);
+        for (int t = 0; t < K; t++) {
+          int b = -1;
+          for (int x = 0; x < nc; x++) if (!used[x] && (b < 0 || lex_lt(ck[x], cn[x], ck[b], cn[b]))) b = x;
+          used[b] = 1; x_ch[t] = cn[b];
+        }
+        x_pred = 1;
+      }
+#undef BLOCKED
+      free(cn); free(ck); free(used);
     }
 
     /* ---- the truth ---- */
@@ -244,6 +287,12 @@ static void spec_pass(void* fv, const void* ov, int32_t lim, int32_t s) {
         for (int q = 0; ok && q < n_ch; q++) if (chosen[q] != list_ch[q]) ok = 0;
         if (!ok) { g_st.asserts_failed++; if (g_st.asserts_failed < 10) fprintf(stderr, "MODEL: list resolution wrong at step %d\n", j); }
       } else g_st.list_fail++;
+    }
+    if (x_pred) {
+      int ok = (n_ch == K);
+      for (int q = 0; ok && q < K; q++) if (chosen[q] != x_ch[q]) ok = 0;
+      if (ok) g_st.xres_ok++;
+      else { g_st.asserts_failed++; if (g_st.asserts_failed < 10) fprintf(stderr, "MODEL: extended resolve wrong at step %d\n", j); }
     }
     /* ---- bookkeeping of a count change ---- */
     if (!same) {
