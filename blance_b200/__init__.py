@@ -17,10 +17,10 @@ from . import build as _build
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
-_API_NAMES = ("BOOSTER_CBGT_MAX", "BOOSTER_NONE", "BlanceError", "CalcPartitionMoves", "CalcPartitionMovesMap",
+_API_NAMES = ("AuditMap", "BOOSTER_CBGT_MAX", "BOOSTER_NONE", "BlanceError", "CalcPartitionMoves", "CalcPartitionMovesMap",
               "NodeStateOp", "OrchestrateSchedule", "OrchestratorOptions", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions",
               "PlanNextMapScenarios", "capi")
-__all__ = ["PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "CalcPartitionMoves", "CalcPartitionMovesMap",
+__all__ = ["AuditMap", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "CalcPartitionMoves", "CalcPartitionMovesMap",
            "NodeStateOp", "OrchestrateSchedule", "OrchestratorOptions", "BlanceError", "BOOSTER_NONE", "BOOSTER_CBGT_MAX", "capi"]
 
 

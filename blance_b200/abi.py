@@ -69,9 +69,25 @@ class _ScenarioOpts(ctypes.Structure):  # struct blance_scenario_opts
                 ("rule_off", ctypes.c_void_p), ("ie_mask", ctypes.c_void_p)]
 
 
+AUDIT_N2N = 1                                                                   # enum blance_audit_flags
+
+
+class _AuditOpts(ctypes.Structure):    # struct blance_audit_opts
+    _fields_ = [("flags", ctypes.c_uint32), ("n_domains", ctypes.c_int32), ("domain_parent", ctypes.c_void_p)]
+
+
+class _AuditOut(ctypes.Structure):     # struct blance_audit_out
+    _fields_ = [("short_slots", ctypes.c_void_p), ("over_slots", ctypes.c_void_p), ("rule_miss", ctypes.c_void_p),
+                ("rule_tested", ctypes.c_void_p), ("dom_top", ctypes.c_void_p), ("dom_all", ctypes.c_void_p),
+                ("dom_copies", ctypes.c_void_p), ("n2n", ctypes.c_void_p), ("part_flags", ctypes.c_void_p),
+                ("short_parts", ctypes.c_int64), ("rule_miss_parts", ctypes.c_int64), ("no_top_parts", ctypes.c_int64),
+                ("n2n_max", ctypes.c_int32), ("n2n_max_a", ctypes.c_int32), ("n2n_max_b", ctypes.c_int32),
+                ("kernel_ms", ctypes.c_float)]
+
+
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
            "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_free")
 
@@ -97,6 +113,9 @@ def capi():
         lib.blance_plan_scenarios.argtypes = [vp, vp, i32, vp, i32, i32, vp]
         lib.blance_plan_scenarios_ex.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp]
         lib.blance_plan_scenarios_schedule.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]
+        lib.blance_plan_scenarios_audit.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+        lib.blance_map_audit.argtypes = [vp, vp, vp, vp, vp, vp]
+        lib.blance_plan_audit.argtypes = [vp, vp, vp, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
         lib.blance_plan_run.argtypes = [vp, vp]
         lib.blance_plan_fetch.argtypes = [vp, vp, vp]
@@ -123,3 +142,5 @@ ScenarioOpts = _ScenarioOpts
 ScenarioOut = _ScenarioOut
 ScheduleOut = _ScheduleOut
 ScenarioScheduleOut = _ScenarioScheduleOut
+AuditOpts = _AuditOpts
+AuditOut = _AuditOut

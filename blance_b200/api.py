@@ -105,7 +105,7 @@ def _option_kwargs(o):
 
 
 def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=None, scenarios=(), favorMinNodes=False,
-                         wantMaps=(), maxConcurrent=0, scheduleConcurrency=()):
+                         wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None):
     """What-if variants of one cluster, planned side by side on the device.  Scenario i is
     PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, sc["nodesToRemove"], sc["nodesToAdd"], model, options with
     the scenario's plan options substituted): both node-set keys are required (None = nil).  The optional keys
@@ -122,13 +122,38 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
     MaxConcurrentPartitionMovesPerNode, Rounds, MovesDone, StuckParts, MaxBatch, and NodeRounds / NodeLastRound
     {node: rounds with a batch / 1 + the last such round} (nonzero entries only).  The movers are the nodesAll names.
     Partitions are walked in interning order (the name rule of plan.go:519-528) where OrchestrateSchedule walks them in
-    byte order: both are valid instances of Go's map order and agree whenever the names sort the same under both."""
+    byte order: both are valid instances of Go's map order and agree whenever the names sort the same under both.
+
+    audit (None = no audit, exactly the results above; or a dict with the optional key "failoverSpread") adds an
+    "audit" dict to every result: AuditMap of that scenario's final map (prevMap with every assigned partition
+    replaced by its next row) under the scenario's own constraints and hierarchy rules, computed inside the sweep
+    without copying the map out.  The fault domains are the options' NodeHierarchy for every scenario."""
     o = options or PlanNextMapOptions()
     same = prevMap is partitionsToAssign
     return _host.PlanNextMapScenarios(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                       {k: tuple(v) for k, v in model.items()}, _scenario_tuples(scenarios),
                                       bool(favorMinNodes), [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o),
-                                      schedule_concurrency=[int(c) for c in scheduleConcurrency])
+                                      schedule_concurrency=[int(c) for c in scheduleConcurrency],
+                                      audit=None if audit is None else bool(audit.get("failoverSpread", False)))
+
+
+def AuditMap(partitionMap, nodesAll, model, options=None, failoverSpread=False):
+    """What the planner never reports about a finished map (include/blance_b200.h, "auditing a partition map"),
+    counted on the device.  options (PlanNextMapOptions): ModelStateConstraints override the model's constraints;
+    HierarchyRules over NodeHierarchy are the rules checked; NodeHierarchy is also the fault-domain forest (a node
+    absent from it is its own root).  Returns a dict, zero counts left out:
+      short_slots / over_slots {state: slots}, short_parts;
+      rule_miss / rule_tested {state: [count per rule of that state]}, rule_miss_parts: placements the planner made by
+        its silent fallback (plan.go:214-220), e.g. a replica in its primary's rack;
+      dom_copies / dom_top / dom_all {node or hierarchy name: copies under it / partitions whose top node is under it /
+        partitions that live under it alone}, no_top_parts;
+      part_flags {partition: bit 0 short | bit 1 rule miss | bit 2 no top node};
+      with failoverSpread: failover_spread {a: {b: copies on b of partitions whose top node is a}} and failover_max
+        (count, a, b), the node that takes the most promotions when a fails."""
+    o = options or PlanNextMapOptions()
+    return _host.AuditMap(partitionMap, list(nodesAll), {k: tuple(v) for k, v in model.items()},
+                          model_state_constraints=o.ModelStateConstraints, node_hierarchy=o.NodeHierarchy,
+                          hierarchy_rules=_rules_arg(o.HierarchyRules), failover_spread=bool(failoverSpread))
 
 
 def intern_scenario(prevMap, partitionsToAssign, nodesAll, model, options, scenarios, index):
@@ -173,4 +198,4 @@ def OrchestrateSchedule(model, options, nodesAll, begMap, endMap):
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------
-from .abi import EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, ScenarioScheduleOut, ScheduleOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401
+from .abi import AUDIT_N2N, AuditOpts, AuditOut, EXPORTS, PlanIn, PlanOut, Scenario, ScenarioOpts, ScenarioOut, ScenarioScheduleOut, ScheduleOut, _I32_FIELDS, _PTR_FIELDS, capi  # noqa: E402,F401

@@ -24,6 +24,7 @@
 #include "assign_pass.cuh"
 #include "assign_pass_seq.cuh"
 #include "assign_pass_spec.cuh"
+#include "audit.cuh"
 #include "aux_kernels.cuh"
 #include "blance_b200.h"
 #include "device_types.cuh"
@@ -105,7 +106,7 @@ struct blance_ctx {
   void* cub_tmp = nullptr;
   size_t cub_tmp_bytes = 0;
   std::vector<cudaEvent_t> events;   // pool for pass timing
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [4], [5]: around the audit kernels
   int* d_any_active = nullptr;
   int* h_any_active = nullptr;       // pinned
   long long launches = 0;            // kernels of this library launched so far
@@ -1128,7 +1129,7 @@ static void sched_slices(Arena& a, int nw, int nc, long long PU, long long NU, i
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
 // their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and override list of any.
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
-                     int max_concurrent, const SchedReq* sr, size_t* per_scenario) {
+                     int max_concurrent, const SchedReq* sr, size_t audit_bytes, size_t* per_scenario) {
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
@@ -1136,7 +1137,8 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   plan_slices(one, &probe, 1);
   size_t per = one.bytes() + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
                sizeof(long long) * (size_t)summary_stride(in0) +
-               sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides;
+               sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides +
+               audit_bytes;
   if (sr) {
     Arena sched;
     WSched w{};
@@ -1246,17 +1248,228 @@ static std::vector<unsigned long long> wave_schedule(blance_ctx* ctx, const char
   return scal;
 }
 
+// ---------------------------------------------------------------------------------------
+// The audit of a partition map (audit.cuh; include/blance_b200.h).
+
+// The audits requested with one call: the checked options and the caller's outputs (one per audited map).
+struct AuditReq {
+  uint32_t flags = 0;
+  int n_domains = 0;
+  const int32_t* parent = nullptr;     // host, [n_node_ids + n_domains] or NULL
+  blance_audit_out* out = nullptr;
+};
+
+// What an audit reads of a model: sizes, the state tables and the hierarchy fields (not the partition tables).
+static void check_audit_model(const std::string& name, const blance_plan_in* m) {
+  auto bad = [&](const char* what, int st = BLANCE_ERR_INVALID_ARG) { throw_err(st, name + ": " + what); };
+  if (!m) bad("model is NULL");
+  if (m->n_nodes < 0 || m->n_node_ids < m->n_nodes || m->n_states < 0 || m->n_parts < 0 || m->n_slots < 0)
+    bad("negative size or n_node_ids < n_nodes");
+  if (m->n_states > BL_S_MAX) bad("more than 8 model states", BLANCE_ERR_UNSUPPORTED);
+  if (m->n_slots > BL_SLP_MAX) bad("more than 32 slots per row", BLANCE_ERR_UNSUPPORTED);
+  if (m->n_nodes > 8192) bad("more than 8192 nodes", BLANCE_ERR_UNSUPPORTED);
+  if (m->n_parts >= (1 << 30)) bad("2^30 or more partitions", BLANCE_ERR_UNSUPPORTED);
+  if (m->n_states > 0) {
+    if (!m->state_constraints || !m->state_slot_off) bad("state tables are NULL");
+    if (m->top_state < 0 || m->top_state >= m->n_states) bad("top_state out of range");
+    if (m->state_slot_off[0] != 0 || m->state_slot_off[m->n_states] != m->n_slots) bad("state_slot_off does not span [0, n_slots]");
+    for (int s = 0; s < m->n_states; ++s)
+      if (m->state_slot_off[s + 1] < m->state_slot_off[s]) bad("state_slot_off not monotone");
+  }
+  if (!m->has_hier_rules) return;
+  if (!m->rule_off) bad("rule_off is NULL");
+  if (m->n_rules < 0) bad("n_rules is negative");
+  if (m->n_rules > AUDIT_RULES_MAX) bad("more than 256 hierarchy rules", BLANCE_ERR_UNSUPPORTED);
+  if (m->n_rules > 0 && !m->ie_mask) bad("ie_mask is NULL");
+  if (m->n_hier_bits < m->n_nodes) bad("n_hier_bits < n_nodes");
+  if ((m->n_hier_bits + 31) / 32 > 32 * AUDIT_HW_LANE) bad("hierarchy universe above 4096 bits", BLANCE_ERR_UNSUPPORTED);
+  for (int s = 0; s <= m->n_states; ++s)
+    if (m->rule_off[s] < 0 || m->rule_off[s] > m->n_rules || (s > 0 && m->rule_off[s] < m->rule_off[s - 1]))
+      bad("rule_off is not a monotone offset table into the rules");
+}
+
+// The options of an audit over NU node ids, checked: flags, and a fault-domain forest without cycles, every vertex
+// at most AUDIT_DEPTH_MAX edges below its root.
+static AuditReq check_audit_opts(const std::string& name, const blance_audit_opts* o, int NU, blance_audit_out* out) {
+  AuditReq ar;
+  ar.out = out;
+  if (!out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": the audit output is NULL");
+  if (!o) return ar;
+  if (o->flags & ~(uint32_t)BLANCE_AUDIT_N2N) throw_err(BLANCE_ERR_INVALID_ARG, name + ": audit flags hold an unknown bit");
+  if (o->n_domains < 0 || o->n_domains > (1 << 24)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains outside [0, 2^24]");
+  if (!o->domain_parent && o->n_domains != 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains without domain_parent");
+  ar.flags = o->flags; ar.n_domains = o->n_domains; ar.parent = o->domain_parent;
+  if (!ar.parent) return ar;
+  const long long V = (long long)NU + o->n_domains;
+  for (long long v = 0; v < V; ++v)
+    if (ar.parent[v] < -1 || ar.parent[v] >= V)
+      throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent[" + std::to_string(v) + "] is outside [-1, n_node_ids + n_domains)");
+  for (long long v = 0; v < V; ++v) {
+    int d = 0;
+    for (long long u = ar.parent[v]; u >= 0; u = ar.parent[u])
+      if (++d > AUDIT_DEPTH_MAX)
+        throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent has a cycle or a vertex more than 16 edges below its root (vertex " + std::to_string(v) + ")");
+  }
+  return ar;
+}
+
+// Without a context there is nothing to run on: BLANCE_ERR_CUDA when that is because the machine has no usable
+// device (no context can be created then), an argument error otherwise.
+static void need_ctx(const blance_ctx* ctx) {
+  if (ctx) return;
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
+    cudaGetLastError();
+    throw_err(BLANCE_ERR_CUDA, "no CUDA device available; libblance_b200 has no CPU fallback");
+  }
+  throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+}
+
+// Device buffers of nw audits of maps with P partitions over NU node ids and N nodes: descriptors, the int64
+// result blocks (audit_out_words each, Rc rules), and on request the forest, the failover matrices and the
+// per-partition flags.  The forest is one array whatever nw; pricing a wave as nw times one audit counts it nw times,
+// an over-estimate of V x 4 bytes per scenario.
+struct AuditBufs {
+  AuditInst* insts = nullptr;
+  long long* out = nullptr;
+  int32_t* parent = nullptr;
+  int32_t* n2n = nullptr;
+  uint8_t* flags = nullptr;
+  int nw = 0, S = 0, Rc = 0, V = 0, N = 0, P = 0;
+  long long words = 0;
+};
+
+static void audit_slices(Arena& a, AuditBufs& b, const AuditReq& ar, int nw, int S, int Rc, int NU, int N, int P, bool want_flags) {
+  b.nw = nw; b.S = S; b.Rc = Rc; b.V = NU + ar.n_domains; b.N = N; b.P = P;
+  b.words = audit_out_words(S, Rc, b.V);
+  a.add(b.insts, (size_t)nw);
+  a.add(b.out, (size_t)(b.words * nw));
+  if (ar.parent) a.add(b.parent, (size_t)b.V);
+  if (ar.flags & BLANCE_AUDIT_N2N) a.add(b.n2n, (size_t)nw * N * N);
+  if (want_flags) a.add(b.flags, (size_t)nw * P);
+}
+
+// The model part of a descriptor, from an instance as laid out for the device / from the caller's tables.
+static AuditInst audit_inst(const DInst& D) {
+  AuditInst A{};
+  A.P = D.PU; A.N = D.N; A.NU = D.NU; A.S = D.S; A.top_state = D.top_state;
+  A.HW = D.HW; A.n_rules = D.has_hier_rules ? D.n_rules : 0;
+  for (int s = 0; s < D.S; ++s) { A.constraints[s] = D.state_constraints[s]; A.slot_off[s] = D.state_slot_off[s]; A.rule_off[s] = D.rule_off[s]; }
+  A.slot_off[D.S] = D.state_slot_off[D.S]; A.rule_off[D.S] = D.rule_off[D.S];
+  return A;
+}
+
+static AuditInst audit_inst(const blance_plan_in& m) {
+  AuditInst A{};
+  A.P = m.n_parts; A.N = m.n_nodes; A.NU = m.n_node_ids; A.S = m.n_states; A.top_state = m.top_state;
+  A.HW = m.has_hier_rules ? (m.n_hier_bits + 31) / 32 : 0; A.n_rules = m.has_hier_rules ? m.n_rules : 0;
+  for (int s = 0; s < m.n_states; ++s) {
+    A.constraints[s] = m.state_constraints[s]; A.slot_off[s] = m.state_slot_off[s];
+    A.rule_off[s] = m.has_hier_rules ? m.rule_off[s] : 0;
+  }
+  A.slot_off[m.n_states] = m.n_slots; A.rule_off[m.n_states] = m.has_hier_rules ? m.rule_off[m.n_states] : 0;
+  return A;
+}
+
+static void audit_kernels(blance_ctx* ctx, const AuditBufs& b, bool any_rules);
+
+// Enqueues the audits `insts` (map and model fields set by the caller) on b's buffers.
+static void audit_run(blance_ctx* ctx, const AuditBufs& b, const AuditReq& ar, std::vector<AuditInst>& insts) {
+  cudaStream_t st = ctx->stream;
+  const int nw = b.nw;
+  bool any_rules = false;
+  for (int j = 0; j < nw; ++j) {
+    AuditInst& A = insts[(size_t)j];
+    A.V = b.V; A.Rc = b.Rc; A.dom_parent = b.parent;
+    A.out = b.out + (long long)j * b.words;
+    A.n2n = b.n2n ? b.n2n + (size_t)j * b.N * b.N : nullptr;
+    A.part_flags = b.flags ? b.flags + (size_t)j * b.P : nullptr;
+    any_rules |= A.n_rules > 0;
+  }
+  CUDA(cudaMemcpyAsync(b.insts, insts.data(), sizeof(AuditInst) * (size_t)nw, cudaMemcpyHostToDevice, st));
+  if (b.parent) CUDA(cudaMemcpyAsync(b.parent, ar.parent, sizeof(int32_t) * (size_t)b.V, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemsetAsync(b.out, 0, sizeof(long long) * (size_t)(b.words * nw), st));
+  if (b.n2n) CUDA(cudaMemsetAsync(b.n2n, 0, sizeof(int32_t) * (size_t)nw * b.N * b.N, st));
+  if (b.flags) CUDA(cudaMemsetAsync(b.flags, 0, (size_t)nw * b.P, st));
+  CUDA(cudaEventRecord(ctx->ev[4], st));
+  audit_kernels(ctx, b, any_rules);
+  CUDA(cudaEventRecord(ctx->ev[5], st));
+}
+
+static void audit_kernels(blance_ctx* ctx, const AuditBufs& b, bool any_rules) {
+  const int nw = b.nw;
+  if (b.P <= 0) return;
+  const int per_sm = std::max(1, ctx->sm_count * 8 / nw);
+  const size_t smem = sizeof(uint32_t) * 3 * (size_t)b.V;
+  const dim3 grid((unsigned)std::max(1, std::min((b.P + 255) / 256, per_sm)), (unsigned)nw);
+  if (smem <= 44 * 1024) launch(ctx, k_map_audit<true>, grid, 256, smem, b.insts);
+  else launch(ctx, k_map_audit<false>, grid, 256, 0, b.insts);
+  if (any_rules)         // one warp per partition
+    launch(ctx, k_map_audit_rules, dim3((unsigned)std::max(1, std::min((b.P + 7) / 8, per_sm)), (unsigned)nw), 256, 0, b.insts);
+  if (b.n2n && b.N > 0)
+    launch(ctx, k_audit_n2n_max, dim3((unsigned)std::max(1, (int)std::min<long long>(((long long)b.N * b.N + 255) / 256, per_sm)), (unsigned)nw),
+           256, 0, b.insts);
+}
+
+// Copies the results of audit j of b into o (the caller synchronises the stream; `host` receives the int64 block
+// and must outlive that).
+static void audit_fetch(blance_ctx* ctx, const AuditBufs& b, int j, std::vector<long long>& host, blance_audit_out& o) {
+  cudaStream_t st = ctx->stream;
+  host.assign((size_t)b.words, 0);
+  CUDA(cudaMemcpyAsync(host.data(), b.out + (long long)j * b.words, sizeof(long long) * (size_t)b.words, cudaMemcpyDeviceToHost, st));
+  if (o.n2n && b.n2n && b.N > 0)
+    CUDA(cudaMemcpyAsync(o.n2n, b.n2n + (size_t)j * b.N * b.N, sizeof(int32_t) * (size_t)b.N * b.N, cudaMemcpyDeviceToHost, st));
+  if (o.part_flags && b.flags && b.P > 0)
+    CUDA(cudaMemcpyAsync(o.part_flags, b.flags + (size_t)j * b.P, (size_t)b.P, cudaMemcpyDeviceToHost, st));
+}
+
+// The int64 block of one audit (n_rules of its own) into the caller's arrays and scalars, after the stream was
+// synchronised; kernel_ms is the time between the events audit_run recorded.
+static void audit_unpack(blance_ctx* ctx, const AuditBufs& b, int n_rules, const std::vector<long long>& host, blance_audit_out& o) {
+  o.kernel_ms = 0.f;
+  cudaEventElapsedTime(&o.kernel_ms, ctx->ev[4], ctx->ev[5]);
+  const long long* h = host.data();
+  const int S = b.S, Rc = b.Rc, V = b.V;
+  auto put = [](int64_t* dst, const long long* src, int n) { if (dst && n > 0) std::memcpy(dst, src, sizeof(int64_t) * (size_t)n); };
+  put(o.short_slots, h, S); put(o.over_slots, h + S, S);
+  put(o.rule_miss, h + 2 * S, n_rules); put(o.rule_tested, h + 2 * S + Rc, n_rules);
+  const long long* d = h + 2 * S + 2 * Rc;
+  put(o.dom_top, d, V); put(o.dom_all, d + V, V); put(o.dom_copies, d + 2ll * V, V);
+  const long long* sc = d + 3ll * V;
+  o.short_parts = sc[0]; o.rule_miss_parts = sc[1]; o.no_top_parts = sc[2];
+  o.n2n_max = o.n2n_max_a = o.n2n_max_b = -1;
+  if (b.n2n) {
+    const unsigned long long key = (unsigned long long)sc[3];
+    o.n2n_max = (int32_t)(key >> 32);
+    if (key) {
+      const uint32_t idx = 0xFFFFFFFFu - (uint32_t)key;
+      o.n2n_max_a = (int32_t)(idx / (uint32_t)b.N); o.n2n_max_b = (int32_t)(idx % (uint32_t)b.N);
+    }
+  }
+}
+
 static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
                                 const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
-                                const SchedReq* sr) {
+                                const SchedReq* sr, const AuditReq* ar) {
   cudaStream_t st = ctx->stream;
   const int n_dev = (int)idx.size();
   const blance_plan_in in0 = scenario_in(*base, sc[idx[0]], opts_of(opts, idx[0]));
   long long max_mask = 0;
-  int max_ow = 0;
+  int max_ow = 0, max_rules = 0;
+  bool audit_flags = false;            // any caller wants the per-partition flags
   for (int i : idx) {
-    max_mask = std::max(max_mask, mask_words(scenario_in(*base, sc[i], opts_of(opts, i))));
+    const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
+    max_mask = std::max(max_mask, mask_words(in));
     max_ow = std::max(max_ow, n_overrides(opts_of(opts, i)));
+    max_rules = std::max(max_rules, in.has_hier_rules ? in.n_rules : 0);
+    audit_flags |= ar && ar->out[i].part_flags;
+  }
+  size_t audit_bytes = 0;              // one scenario's audit buffers, priced into the wave
+  if (ar) {
+    Arena one;
+    AuditBufs b;
+    audit_slices(one, b, *ar, 1, base->n_states, max_rules, base->n_node_ids, base->n_nodes, base->n_parts, audit_flags);
+    audit_bytes = one.bytes();
   }
   {
     cudaMemPool_t pool;                // measure free memory without this context's cached arenas
@@ -1268,7 +1481,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
   // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
   const PlanPtr pb = upload(ctx, 1, &in0);
   size_t per = 0;
-  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, &per);
+  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, audit_bytes, &per);
   if (W < 1)
     throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
   const bool auto_wave = max_concurrent <= 0;
@@ -1310,6 +1523,8 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     if (sr) sched_slices(wave, nw, sr->nc, PU, NU, scenario_ops(*base), (long long)PU * scenario_ops(*base), wsch, wtmp, wtmp_bytes, st);
     int32_t* d_ow = nullptr;
     if (!ow.empty()) wave.add(d_ow, ow.size());
+    AuditBufs abuf;
+    if (ar) audit_slices(wave, abuf, *ar, nw, S, max_rules, NU, base->n_nodes, PU, audit_flags);
     try {
       wave.alloc(st, "a scenario wave");
     } catch (const Error&) {
@@ -1362,6 +1577,23 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
       else launch(ctx, k_scenario_summary<false>, grid, 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
     }
     CUDA(cudaEventRecord(ctx->ev[2], st));
+    // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
+    std::vector<AuditInst> a_insts;
+    std::vector<std::vector<long long>> a_host((size_t)(ar ? nw : 0));
+    if (ar) {
+      for (int j = 0; j < nw; ++j) {
+        const DInst& D = pl->h_insts[(size_t)j];
+        AuditInst A = audit_inst(D);
+        A.rows = P.rows + D.rows_off; A.alt_rows = pl->prev_rows_init + D.rows_off;
+        A.meta = P.pmeta + D.part_off; A.alt_meta = pl->prev_meta_init + D.part_off;
+        A.pflags = pl->pflags_init + D.part_off;
+        A.ie_mask = P.ie_mask + D.mask_off;
+        A.stride = D.SLP;
+        a_insts.push_back(A);
+      }
+      audit_run(ctx, abuf, *ar, a_insts);
+      for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
+    }
     bool any_rows = false;
     for (int j = 0; j < nw; ++j) {
       const blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
@@ -1392,6 +1624,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
       o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
       o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
       o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
+      if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
     }
     if (sr) {
       CUDA(cudaEventRecord(ctx->ev[3], st));
@@ -1431,7 +1664,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
 
 static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                            const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
-                           const SchedReq* sr = nullptr) {
+                           const SchedReq* sr = nullptr, const AuditReq* ar = nullptr) {
   if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
   if (!base || !sc || !out) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
@@ -1460,7 +1693,7 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
   fan_out(ctx, G, [&](int d, blance_ctx* dev) {
-    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr);
+    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr, ar);
   });
 }
 
@@ -1479,6 +1712,33 @@ extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* b
   });
 }
 
+// The checked schedule request of blance_plan_scenarios_schedule's arguments; the scalars of sched are cleared.
+static SchedReq sched_req(const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc, const blance_scenario_out* out,
+                          int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                          blance_scenario_schedule_out* sched) {
+  if (n_move_conc < 1 || !move_conc || !sched)
+    throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
+  if (base && base->n_parts >= (1 << WAVE_PART_BITS))
+    throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
+  if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
+    throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
+  SchedReq sr;
+  sr.nc = n_move_conc;
+  sr.out = sched;
+  for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
+  if (base && base->n_node_ids > 0) {
+    sr.mover.assign((size_t)base->n_node_ids, 0);
+    for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
+  }
+  if (n > 0 && sc && out)
+    for (int i = 0; i < n; ++i)
+      for (int k = 0; k < n_move_conc; ++k) {
+        blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
+        o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
+      }
+  return sr;
+}
+
 extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                               const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                               int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
@@ -1486,27 +1746,92 @@ extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan
   return entry(ctx, [&](Device&) {
     const char* name = "blance_plan_scenarios_schedule";
     if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-    if (n_move_conc < 1 || !move_conc || !sched)
-      throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
-    if (base && base->n_parts >= (1 << WAVE_PART_BITS))
-      throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
-    if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
-      throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
-    SchedReq sr;
-    sr.nc = n_move_conc;
-    sr.out = sched;
-    for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
-    if (base && base->n_node_ids > 0) {
-      sr.mover.assign((size_t)base->n_node_ids, 0);
-      for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
-    }
-    if (n > 0 && sc && out)
-      for (int i = 0; i < n; ++i)
-        for (int k = 0; k < n_move_conc; ++k) {
-          blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
-          o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
-        }
+    const SchedReq sr = sched_req(name, base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
     plan_scenarios(ctx, name, base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr);
+  });
+}
+
+extern "C" int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                           const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                           int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                           blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                                           const blance_audit_opts* aopts, blance_audit_out* audit) {
+  return entry(ctx, [&](Device&) {
+    const std::string name = "blance_plan_scenarios_audit";
+    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base is NULL");
+    const AuditReq ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
+    const bool no_sched = n_move_conc == 0 && !move_conc && !sched;
+    SchedReq sr;
+    if (!no_sched) sr = sched_req(name.c_str(), base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
+    if (n > 0 && sc)
+      for (int i = 0; i < n; ++i) {
+        const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
+        check_audit_model(name + ": scenario " + std::to_string(i), &in);
+      }
+    need_ctx(ctx);
+    plan_scenarios(ctx, name.c_str(), base, n, sc, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, &ar);
+  });
+}
+
+// blance_map_audit / blance_plan_audit: one audit on buffers of its own.
+static void audit_one(blance_ctx* dev, const AuditBufs& b, const AuditReq& ar, const AuditInst& A) {
+  std::vector<AuditInst> insts{A};
+  audit_run(dev, b, ar, insts);
+  std::vector<long long> host;
+  audit_fetch(dev, b, 0, host, *ar.out);
+  CUDA(cudaStreamSynchronize(dev->stream));
+  audit_unpack(dev, b, A.n_rules, host, *ar.out);
+}
+
+extern "C" int blance_map_audit(blance_ctx* ctx, const blance_plan_in* model, const int32_t* rows, const uint8_t* shape,
+                                const blance_audit_opts* opts, blance_audit_out* out) {
+  return entry(ctx, [&](Device& device) {
+    const std::string name = "blance_map_audit";
+    check_audit_model(name, model);
+    const AuditReq ar = check_audit_opts(name, opts, model->n_node_ids, out);
+    const size_t P = (size_t)model->n_parts, SL = (size_t)model->n_slots, S = (size_t)model->n_states;
+    if (P * SL > 0 && !rows) throw_err(BLANCE_ERR_INVALID_ARG, name + ": rows is NULL");
+    if (P * S > 0 && !shape) throw_err(BLANCE_ERR_INVALID_ARG, name + ": shape is NULL");
+    need_ctx(ctx);
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    AuditInst A = audit_inst(*model);
+    int32_t* d_rows = nullptr;
+    uint8_t* d_shape = nullptr;
+    uint32_t* d_mask = nullptr;
+    const size_t mw = (size_t)mask_words(*model);
+    Arena a;
+    AuditBufs b;
+    a.add(d_rows, P * SL); a.add(d_shape, P * S); a.add(d_mask, mw);
+    audit_slices(a, b, ar, 1, model->n_states, A.n_rules, model->n_node_ids, model->n_nodes, model->n_parts, out->part_flags != nullptr);
+    a.alloc(st, "the audit");
+    if (P * SL) CUDA(cudaMemcpyAsync(d_rows, rows, sizeof(int32_t) * P * SL, cudaMemcpyHostToDevice, st));
+    if (P * S) CUDA(cudaMemcpyAsync(d_shape, shape, P * S, cudaMemcpyHostToDevice, st));
+    if (mw) CUDA(cudaMemcpyAsync(d_mask, model->ie_mask, sizeof(uint32_t) * mw, cudaMemcpyHostToDevice, st));
+    A.rows = d_rows; A.shape8 = d_shape; A.ie_mask = d_mask; A.stride = model->n_slots;
+    audit_one(dev, b, ar, A);
+  });
+}
+
+extern "C" int blance_plan_audit(blance_ctx* ctx, blance_plan* plan, const blance_audit_opts* opts, blance_audit_out* out) {
+  return entry(ctx, [&](Device& device) {
+    const std::string name = "blance_plan_audit";
+    if (!plan) throw_err(BLANCE_ERR_INVALID_ARG, name + ": plan is NULL");
+    if (plan->n_inst != 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": the plan is not a single instance");
+    const DInst& D = plan->h_insts[0];
+    if (D.has_hier_rules && D.n_rules > AUDIT_RULES_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 256 hierarchy rules");
+    if (D.has_hier_rules && (D.rule_off[0] < 0 || D.rule_off[D.S] > D.n_rules)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": rule_off points outside the rules");
+    const AuditReq ar = check_audit_opts(name, opts, D.NU, out);
+    need_ctx(ctx);
+    blance_ctx* dev = device();
+    AuditInst A = audit_inst(D);
+    A.rows = plan->pool.rows + D.rows_off; A.meta = plan->pool.pmeta + D.part_off;
+    A.ie_mask = plan->pool.ie_mask + D.mask_off; A.stride = D.SLP;
+    Arena a;
+    AuditBufs b;
+    audit_slices(a, b, ar, 1, D.S, A.n_rules, D.NU, D.N, D.PU, out->part_flags != nullptr);
+    a.alloc(dev->stream, "the audit");
+    audit_one(dev, b, ar, A);
   });
 }
 

@@ -1113,6 +1113,116 @@ ScenarioTables scenario_tables(const InternedPlan& ip, const PartitionModel& mod
 
 }  // namespace
 
+// ------------------------------------------------------------------------------------
+// The audit of a map, by name
+
+namespace {
+
+// The fault-domain forest of blance_audit_opts over ip's node ids: the node names are vertices 0 .. NU-1, every other
+// name of `parents` follows in byte order; a missing or "" parent is a root.
+struct Forest {
+  Strs names;                          // [V]
+  std::vector<int32_t> parent;         // [V]; empty = nodes only
+  blance_audit_opts opts{};
+};
+
+void build_forest(const InternedPlan& ip, const std::optional<std::unordered_map<std::string, std::string>>& parents, bool n2n, Forest* f) {
+  f->names = ip.node_names;
+  f->opts = blance_audit_opts{};
+  f->opts.flags = n2n ? BLANCE_AUDIT_N2N : 0;
+  if (!parents) return;
+  std::unordered_map<std::string, int32_t> id;
+  for (size_t i = 0; i < f->names.size(); ++i) id.emplace(f->names[i], int32_t(i));
+  Strs others;
+  for (const auto& kv : *parents) { others.push_back(kv.first); others.push_back(kv.second); }
+  std::sort(others.begin(), others.end());
+  for (const auto& n : others)
+    if (!n.empty() && id.emplace(n, int32_t(f->names.size())).second) f->names.push_back(n);
+  f->parent.assign(f->names.size(), -1);
+  for (const auto& kv : *parents)
+    if (!kv.first.empty() && !kv.second.empty()) f->parent[size_t(id[kv.first])] = id[kv.second];
+  f->opts.n_domains = int32_t(f->names.size() - ip.node_names.size());
+  f->opts.domain_parent = f->parent.data();
+}
+
+// Output buffers of one blance_audit_out over V vertices, R rules.
+struct AuditBuffers {
+  std::vector<int64_t> state, rule, dom;
+  std::vector<int32_t> n2n;
+  std::vector<uint8_t> flags;
+  blance_audit_out out{};
+  AuditBuffers(const InternedPlan& ip, size_t V, size_t R, bool want_n2n)
+      : state(2 * size_t(ip.in.n_states) + 1), rule(2 * R + 1), dom(3 * V + 1),
+        n2n(want_n2n ? size_t(ip.in.n_nodes) * size_t(ip.in.n_nodes) + 1 : 0), flags(size_t(ip.in.n_parts) + 1) {
+    const size_t S = size_t(ip.in.n_states);
+    out.short_slots = state.data(); out.over_slots = state.data() + S;
+    out.rule_miss = rule.data(); out.rule_tested = rule.data() + R;
+    out.dom_top = dom.data(); out.dom_all = dom.data() + V; out.dom_copies = dom.data() + 2 * V;
+    out.n2n = want_n2n ? n2n.data() : nullptr;
+    out.part_flags = flags.data();
+  }
+};
+
+MapAudit name_audit(const InternedPlan& ip, const Forest& f, const int32_t* rule_off, const AuditBuffers& b, bool want_n2n) {
+  MapAudit a;
+  const blance_audit_out& o = b.out;
+  const size_t S = size_t(ip.in.n_states), V = f.names.size(), N = size_t(ip.in.n_nodes);
+  for (size_t s = 0; s < S; ++s) {
+    if (o.short_slots[s]) a.ShortSlots[ip.state_names[s]] = o.short_slots[s];
+    if (o.over_slots[s]) a.OverSlots[ip.state_names[s]] = o.over_slots[s];
+    if (rule_off && rule_off[s + 1] > rule_off[s]) {
+      a.RuleMiss[ip.state_names[s]].assign(o.rule_miss + rule_off[s], o.rule_miss + rule_off[s + 1]);
+      a.RuleTested[ip.state_names[s]].assign(o.rule_tested + rule_off[s], o.rule_tested + rule_off[s + 1]);
+    }
+  }
+  for (size_t v = 0; v < V; ++v) {
+    if (o.dom_top[v]) a.DomTop[f.names[v]] = o.dom_top[v];
+    if (o.dom_all[v]) a.DomAll[f.names[v]] = o.dom_all[v];
+    if (o.dom_copies[v]) a.DomCopies[f.names[v]] = o.dom_copies[v];
+  }
+  a.ShortParts = o.short_parts; a.RuleMissParts = o.rule_miss_parts; a.NoTopParts = o.no_top_parts;
+  for (size_t p = 0; p < size_t(ip.in.n_parts); ++p)
+    if (o.part_flags[p]) a.PartFlags[ip.part_names[p]] = o.part_flags[p];
+  a.HasFailoverSpread = want_n2n;
+  if (want_n2n) {
+    for (size_t x = 0; x < N; ++x)
+      for (size_t y = 0; y < N; ++y)
+        if (o.n2n[x * N + y]) a.FailoverSpread[ip.node_names[x]][ip.node_names[y]] = o.n2n[x * N + y];
+    a.FailoverMax = std::max(0, o.n2n_max);
+    if (o.n2n_max_a >= 0) { a.FailoverMaxFrom = ip.node_names[size_t(o.n2n_max_a)]; a.FailoverMaxTo = ip.node_names[size_t(o.n2n_max_b)]; }
+  }
+  return a;
+}
+
+}  // namespace
+
+void AuditForest(const InternedPlan& ip, const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy,
+                 Strs* names, std::vector<int32_t>* parent) {
+  Forest f;
+  build_forest(ip, nodeHierarchy, false, &f);
+  *names = std::move(f.names);
+  *parent = std::move(f.parent);
+}
+
+MapAudit AuditMap(const PartitionMap& map, const Strs& nodesAll, const PartitionModel& model,
+                  const PlanNextMapOptions& options, bool failoverSpread) {
+  // the map interned as a prevMap with nothing to assign: each state's slot range holds its longest list, and state
+  // names outside the model are allowed there (they are no copies)
+  PlanNextMapOptions o;
+  o.ModelStateConstraints = options.ModelStateConstraints;
+  o.NodeHierarchy = options.NodeHierarchy;
+  o.HierarchyRules = options.HierarchyRules;
+  auto ip = InternPlan(map, PartitionMap{}, nodesAll, std::nullopt, std::nullopt, model, o);
+  Forest f;
+  build_forest(*ip, options.NodeHierarchy, failoverSpread, &f);
+  const size_t R = ip->in.has_hier_rules ? size_t(ip->in.n_rules) : 0;
+  AuditBuffers b(*ip, f.names.size(), R, failoverSpread);
+  blance_ctx* ctx = DefaultContext();
+  const int st = blance_map_audit(ctx, &ip->in, ip->prev_rows.data(), ip->prev_shape.data(), &f.opts, &b.out);
+  if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_map_audit failed: ") + blance_last_error(ctx));
+  return name_audit(*ip, f, ip->in.has_hier_rules ? ip->rule_off.data() : nullptr, b, failoverSpread);
+}
+
 std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                              const Strs& nodesAll, const PartitionModel& model,
                                              const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
@@ -1163,7 +1273,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
                                                  bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
-                                                 const std::vector<int>& scheduleConcurrency) {
+                                                 const std::vector<int>& scheduleConcurrency, const ScenarioAudit* audit) {
   if (scenarios.empty()) invalid("PlanNextMapScenarios: no scenarios");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
   const size_t n = scenarios.size();
@@ -1203,8 +1313,28 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     sched[x].node_rounds = node_rounds.data() + x * size_t(NU);
     sched[x].node_last_round = node_last.data() + x * size_t(NU);
   }
+  // the audits: one forest for all scenarios, each scenario's own rules
+  Forest forest;
+  std::vector<std::unique_ptr<AuditBuffers>> abuf;
+  std::vector<blance_audit_out> aout;
+  auto rules_of = [&](size_t i) -> const int32_t* {
+    if (tabs[i].set & BLANCE_OPT_HIERARCHY) return tabs[i].has_hier_rules ? tabs[i].rule_off.data() : nullptr;
+    return ip->in.has_hier_rules ? ip->rule_off.data() : nullptr;
+  };
+  if (audit) {
+    build_forest(*ip, options.NodeHierarchy, audit->FailoverSpread, &forest);
+    for (size_t i = 0; i < n; ++i) {
+      const int32_t R = (tabs[i].set & BLANCE_OPT_HIERARCHY) ? (tabs[i].has_hier_rules ? tabs[i].n_rules : 0)
+                                                             : (ip->in.has_hier_rules ? ip->in.n_rules : 0);
+      abuf.push_back(std::make_unique<AuditBuffers>(*ip, forest.names.size(), size_t(R), audit->FailoverSpread));
+      aout.push_back(abuf.back()->out);
+    }
+  }
   blance_ctx* ctx = DefaultContext();
-  const int st = nc ? blance_plan_scenarios_schedule(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+  const int st = audit ? blance_plan_scenarios_audit(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                                     int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
+                                                     nc ? sched.data() : nullptr, &forest.opts, aout.data())
+                 : nc ? blance_plan_scenarios_schedule(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                      int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), sched.data())
                     : blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                out.data());
@@ -1239,6 +1369,10 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
         if (so.node_last_round[q]) s.NodeLastRound[ip->node_names[size_t(q)]] = so.node_last_round[q];
       }
       r.Schedules.push_back(std::move(s));
+    }
+    if (audit) {
+      abuf[i]->out = aout[i];
+      r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[i], audit->FailoverSpread);
     }
   }
   return res;

@@ -117,6 +117,29 @@ struct ScenarioSchedule {
   std::unordered_map<std::string, int> NodeRounds, NodeLastRound;
 };
 
+// The audit of one map (include/blance_b200.h, "auditing a partition map"), by name; zero counts are left out.
+struct MapAudit {
+  std::unordered_map<std::string, int64_t> ShortSlots, OverSlots;                 // per model state
+  std::unordered_map<std::string, std::vector<int64_t>> RuleMiss, RuleTested;     // per state with rules: one entry per rule, in rule order
+  std::unordered_map<std::string, int64_t> DomTop, DomAll, DomCopies;             // per node or NodeHierarchy name
+  int64_t ShortParts = 0, RuleMissParts = 0, NoTopParts = 0;
+  bool HasFailoverSpread = false;      // the three fields below were asked for
+  std::unordered_map<std::string, std::unordered_map<std::string, int32_t>> FailoverSpread;   // n2n[a][b] by name
+  int32_t FailoverMax = 0;             // the largest entry, and the lowest (a, b) in node-id order that holds it
+  std::string FailoverMaxFrom, FailoverMaxTo;
+  std::unordered_map<std::string, int> PartFlags;                                 // bit 0 short, 1 rule miss, 2 no top node
+};
+
+// AuditMap audits `map` against `model` as PlanNextMapEx would read it with `options`: ModelStateConstraints
+// override the constraints, HierarchyRules over NodeHierarchy are the rules checked (none when HierarchyRules is
+// nil), and NodeHierarchy is also the fault-domain forest: the node names first, then every other name it mentions;
+// a node absent from it, or whose parent is "", is its own root (nil: every node is its own domain).  nodesAll says
+// which names are nodes the planner may pick (a node outside it never complies with a rule).  failoverSpread asks
+// for the failover matrix.  Throws BlanceError for what blance_map_audit rejects (a cycle in NodeHierarchy, a name
+// more than 16 levels below its root) and without a device.
+MapAudit AuditMap(const PartitionMap& map, const Strs& nodesAll, const PartitionModel& model,
+                  const PlanNextMapOptions& options, bool failoverSpread);
+
 struct ScenarioResult {
   int iters_run = 0, converged = 0;
   int64_t steps = 0, sticky_steps = 0, parts_moved = 0, ops_total = 0, warn_parts = 0;
@@ -129,7 +152,13 @@ struct ScenarioResult {
   PartitionMap NextMap;                // as PlanNextMapEx returns it
   Warnings NextWarnings;
   std::vector<ScenarioSchedule> Schedules;   // one per scheduleConcurrency value; empty without them
+  std::optional<MapAudit> Audit;       // with `audit`: the audit of the scenario's final map
 };
+
+// PlanNextMapScenarios' audit request: every result's Audit is AuditMap of that scenario's final map (prevMap with
+// every assigned partition replaced by its next row) under the scenario's own constraints and hierarchy rules
+// (blance_plan_scenarios_audit).  The fault-domain forest is the options' NodeHierarchy for every scenario.
+struct ScenarioAudit { bool FailoverSpread = false; };
 
 // Scenario i is PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, NodesToRemove_i, NodesToAdd_i, model, options
 // with the scenario's NodeWeights, ModelStateConstraints, StateStickiness, PartitionWeights, NodeHierarchy and
@@ -148,7 +177,8 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
                                                  bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
-                                                 const std::vector<int>& scheduleConcurrency = {});
+                                                 const std::vector<int>& scheduleConcurrency = {},
+                                                 const ScenarioAudit* audit = nullptr);
 
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 
@@ -237,6 +267,12 @@ void ReplayCallerMutation(const PartitionMap& next, PartitionMap& prevMap, Parti
 // or this call (0 = back to the default).  Results do not depend on the thread count.
 void SetHostThreads(int n);
 int HostThreads();
+
+// The fault-domain forest AuditMap passes as blance_audit_opts.domain_parent: vertex names (ip's node ids first, then
+// every other name of nodeHierarchy in byte order) and each vertex's parent index, -1 for a root (a name without a
+// parent, or whose parent is "").  nodeHierarchy nil: the node names and an empty parent array (nodes only).
+void AuditForest(const InternedPlan& ip, const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy,
+                 Strs* names, std::vector<int32_t>* parent);
 
 // The process-wide context the host API runs on (created on first use).
 blance_ctx* DefaultContext();

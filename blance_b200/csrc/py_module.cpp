@@ -78,6 +78,20 @@ static py::array_t<T> np_copy(const std::vector<T>& v, size_t n) {
   return a;
 }
 
+static py::dict audit_dict(const MapAudit& a) {
+  py::dict d;
+  d["short_slots"] = a.ShortSlots; d["over_slots"] = a.OverSlots;
+  d["rule_miss"] = a.RuleMiss; d["rule_tested"] = a.RuleTested;
+  d["dom_top"] = a.DomTop; d["dom_all"] = a.DomAll; d["dom_copies"] = a.DomCopies;
+  d["short_parts"] = a.ShortParts; d["rule_miss_parts"] = a.RuleMissParts; d["no_top_parts"] = a.NoTopParts;
+  d["part_flags"] = a.PartFlags;
+  if (a.HasFailoverSpread) {
+    d["failover_spread"] = a.FailoverSpread;
+    d["failover_max"] = py::make_tuple(a.FailoverMax, a.FailoverMaxFrom, a.FailoverMaxTo);
+  }
+  return d;
+}
+
 struct PyInterned { std::unique_ptr<InternedPlan> ip; };
 struct PyOut { std::unique_ptr<PlanOutBuffers> ob; const InternedPlan* ip; };
 
@@ -211,6 +225,22 @@ PYBIND11_MODULE(_host, m) {
   }, py::arg("rows"), py::arg("n_nodes"), py::arg("constraints"), py::arg("removed"), py::arg("added"),
      py::arg("node_weights") = py::none(), py::arg("part_weight") = py::none(), py::arg("part_has_weight") = py::none(),
      py::arg("state_stickiness") = py::none(), py::arg("max_iterations") = 10);
+
+  m.def(
+      "AuditMap",
+      [](const PyPartitionMap& map, const Strs& nodes_all, const PyModel& model, const std::optional<IntMap>& msc,
+         const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, bool failover_spread) {
+        PlanNextMapOptions o = to_options(msc, std::nullopt, std::nullopt, std::nullopt, nh, hr, 0, 10, 0);
+        const PartitionMap pm = to_map(map);
+        MapAudit a;
+        {
+          py::gil_scoped_release rel;
+          a = AuditMap(pm, nodes_all, to_model(model), o, failover_spread);
+        }
+        return audit_dict(a);
+      },
+      py::arg("map"), py::arg("nodes_all"), py::arg("model"), py::arg("model_state_constraints") = py::none(),
+      py::arg("node_hierarchy") = py::none(), py::arg("hierarchy_rules") = py::none(), py::arg("failover_spread") = false);
 
   m.def("CalcPartitionMoves", [](const Strs& states, const NodesByState& beg, const NodesByState& end, bool favor) {
     std::vector<std::tuple<std::string, std::string, std::string>> out;
@@ -359,16 +389,18 @@ PYBIND11_MODULE(_host, m) {
                      const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
                      const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
                      const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
-                     int engine, const std::vector<int>& schedule_concurrency) {
+                     int engine, const std::vector<int>& schedule_concurrency, const std::optional<bool>& audit) {
         PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
         const PartitionMap prev_map = to_map(prev);
         const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
         const std::vector<Scenario> scs = to_scenarios(scenarios);
         std::vector<ScenarioResult> res;
+        ScenarioAudit aud;
+        aud.FailoverSpread = audit.value_or(false);
         {
           py::gil_scoped_release rel;
           res = PlanNextMapScenarios(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, scs,
-                                     favor_min_nodes, want_maps, max_concurrent, schedule_concurrency);
+                                     favor_min_nodes, want_maps, max_concurrent, schedule_concurrency, audit ? &aud : nullptr);
         }
         py::list out;
         for (const auto& r : res) {
@@ -388,6 +420,7 @@ PYBIND11_MODULE(_host, m) {
             }
             d["schedules"] = sl;
           }
+          if (r.Audit) d["audit"] = audit_dict(*r.Audit);
           out.append(d);
         }
         return out;
@@ -397,7 +430,7 @@ PYBIND11_MODULE(_host, m) {
       py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
-      py::arg("schedule_concurrency") = std::vector<int>{});
+      py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none());
 
   // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
   m.def(
@@ -418,6 +451,14 @@ PYBIND11_MODULE(_host, m) {
       py::arg("index"), py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+
+  // test hook: the fault-domain forest AuditMap builds over an interned plan's node ids
+  m.def("audit_forest", [](const PyInterned& ip, const std::optional<StrMap>& nh) {
+    Strs names;
+    std::vector<int32_t> parent;
+    AuditForest(*ip.ip, nh, &names, &parent);
+    return py::make_tuple(names, parent);
+  });
 
   m.def("plan_out", [](const PyInterned& ip) {
     PyOut o;

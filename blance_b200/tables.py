@@ -127,6 +127,7 @@ class ScenarioResult:
     steps = property(lambda self: self.out.steps)
     sticky_steps = property(lambda self: self.out.sticky_steps)
     schedules = None          # blance_plan_scenarios_schedule: one ScenarioSchedule per count
+    audit = None              # blance_plan_scenarios_audit: the AuditResult of the final map
     parts_moved = property(lambda self: self.out.parts_moved)
     ops_total = property(lambda self: self.out.ops_total)
     warn_parts = property(lambda self: self.out.warn_parts)
@@ -149,6 +150,49 @@ class ScenarioSchedule:
     moves_done = property(lambda self: self.out.moves_done)
     stuck_parts = property(lambda self: self.out.stuck_parts)
     max_batch = property(lambda self: self.out.max_batch)
+
+
+class AuditResult:
+    """Output buffers of a blance_audit_out for a map of `t`'s sizes with n_rules rules: every array, the failover
+    matrix only with n2n."""
+
+    def __init__(self, t, n_rules, n_domains=0, n2n=False):
+        V = t.n_node_ids + n_domains
+        self.short_slots = np.zeros(t.n_states, np.int64)
+        self.over_slots = np.zeros(t.n_states, np.int64)
+        self.rule_miss = np.zeros(n_rules, np.int64)
+        self.rule_tested = np.zeros(n_rules, np.int64)
+        self.dom_top = np.zeros(V, np.int64)
+        self.dom_all = np.zeros(V, np.int64)
+        self.dom_copies = np.zeros(V, np.int64)
+        self.n2n = np.zeros((t.n_nodes, t.n_nodes), np.int32) if n2n else None
+        self.part_flags = np.zeros(t.n_parts, np.uint8)
+        self.out = api.AuditOut()
+        for f in ("short_slots", "over_slots", "rule_miss", "rule_tested", "dom_top", "dom_all", "dom_copies", "n2n", "part_flags"):
+            a = getattr(self, f)
+            setattr(self.out, f, a.ctypes.data if a is not None and a.size else None)
+
+    short_parts = property(lambda self: self.out.short_parts)
+    rule_miss_parts = property(lambda self: self.out.rule_miss_parts)
+    no_top_parts = property(lambda self: self.out.no_top_parts)
+    n2n_max = property(lambda self: (self.out.n2n_max, self.out.n2n_max_a, self.out.n2n_max_b))
+    kernel_ms = property(lambda self: self.out.kernel_ms)
+
+
+def _audit_opts(n2n, domain_parent, n_node_ids, keep):
+    """blance_audit_opts of (n2n, domain_parent [n_node_ids + n_domains] or None) and its n_domains."""
+    o = api.AuditOpts()
+    o.flags = api.AUDIT_N2N if n2n else 0
+    if domain_parent is not None:
+        a = np.ascontiguousarray(domain_parent, np.int32)
+        keep.append(a)
+        o.n_domains = a.size - n_node_ids
+        o.domain_parent = a.ctypes.data
+    return o, int(o.n_domains)
+
+
+def _n_rules(t):
+    return int(t.n_rules) if t.has_hier_rules else 0
 
 
 def scenario_tables(base, scenario, opts=None):
@@ -271,15 +315,39 @@ class Context:
             r.out = o
         return results
 
+    def map_audit(self, tables, rows, shape, n2n=False, domain_parent=None):
+        """blance_map_audit of the map (rows [n_parts][n_slots], shape [n_parts][n_states]) against the model and
+        hierarchy of `tables`.  Returns an AuditResult."""
+        keep = []
+        o, n_dom = _audit_opts(n2n, domain_parent, tables.n_node_ids, keep)
+        r = AuditResult(tables, _n_rules(tables), n_dom, n2n)
+        rows = np.ascontiguousarray(rows, np.int32)
+        shape = np.ascontiguousarray(shape, np.uint8)
+        s = tables.struct()
+        self._check(self.lib.blance_map_audit(self.ptr, ctypes.byref(s), rows.ctypes.data if rows.size else None,
+                                              shape.ctypes.data if shape.size else None, ctypes.byref(o), ctypes.byref(r.out)),
+                    "blance_map_audit")
+        return r
+
+    def plan_audit(self, plan, tables, n2n=False, domain_parent=None):
+        """blance_plan_audit of the resident plan `plan` (uploaded from `tables`)."""
+        keep = []
+        o, n_dom = _audit_opts(n2n, domain_parent, tables.n_node_ids, keep)
+        r = AuditResult(tables, _n_rules(tables), n_dom, n2n)
+        self._check(self.lib.blance_plan_audit(self.ptr, plan, ctypes.byref(o), ctypes.byref(r.out)), "blance_plan_audit")
+        return r
+
     def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None,
-                       schedule=None, node_has_mover=None):
+                       schedule=None, node_has_mover=None, audit=None):
         """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
         (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
         are copied out.  opts (None, or one dict of OPT_GROUPS keys per scenario) calls blance_plan_scenarios_ex
         with those plan options.  schedule (None, or a list of MaxConcurrentPartitionMovesPerNode values) calls
         blance_plan_scenarios_schedule instead, with node_has_mover ([n_node_ids], None = the ids < n_nodes), and
         sets each result's `schedules` to one ScenarioSchedule per value.  Returns one ScenarioResult per
-        scenario."""
+        scenario.  audit (None, or a dict with the optional keys n2n and domain_parent) calls
+        blance_plan_scenarios_audit (with the schedules when `schedule` is given) and sets each result's `audit` to
+        the AuditResult of that scenario's final map."""
         n = len(scenarios)
         want = set(want_rows)
         base = base_tables.struct()
@@ -296,21 +364,32 @@ class Context:
                 setattr(scs[i], f, a.ctypes.data if a.size else None)
         results = [ScenarioResult(base_tables, i in want) for i in range(n)]
         outs = (api.ScenarioOut * max(1, n))(*[r.out for r in results])
-        if schedule is not None:
-            counts = np.ascontiguousarray(schedule, np.int32)
+        if schedule is not None or audit is not None:
+            counts = np.ascontiguousarray([] if schedule is None else schedule, np.int32)
             mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
             if mover is not None and mover.size != base_tables.n_node_ids:
                 raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
-            for r in results:
-                r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
-            sch = (api.ScenarioScheduleOut * max(1, n * counts.size))(*[s.out for r in results for s in r.schedules])
+            sch = None
+            if schedule is not None:
+                for r in results:
+                    r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+                sch = (api.ScenarioScheduleOut * max(1, n * counts.size))(*[s.out for r in results for s in r.schedules])
             ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-            self._check(self.lib.blance_plan_scenarios_schedule(
-                self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent), int(counts.size),
-                counts.ctypes.data if counts.size else None, None if mover is None else mover.ctypes.data, outs, sch),
-                "blance_plan_scenarios_schedule")
+            args = (self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent), int(counts.size),
+                    counts.ctypes.data if counts.size else None, None if mover is None else mover.ctypes.data, outs, sch)
+            if audit is None:
+                self._check(self.lib.blance_plan_scenarios_schedule(*args), "blance_plan_scenarios_schedule")
+            else:
+                a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
+                for i, r in enumerate(results):
+                    t = scenario_tables(base_tables, scenarios[i], None if opts is None else opts[i])
+                    r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
+                auds = (api.AuditOut * max(1, n))(*[r.audit.out for r in results])
+                self._check(self.lib.blance_plan_scenarios_audit(*args, ctypes.byref(a_opts), auds), "blance_plan_scenarios_audit")
+                for r, a in zip(results, auds):
+                    r.audit.out = a
             for i, r in enumerate(results):
-                for k, s in enumerate(r.schedules):
+                for k, s in enumerate(r.schedules or ()):
                     s.out = sch[i * counts.size + k]
         elif opts is None:
             self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),

@@ -361,6 +361,117 @@ void blance_plan_free(blance_ctx* ctx, blance_plan* plan);
  * those were launched. */
 int blance_plan_timing(const blance_plan* plan, float* kernel_ms, float* pass_ms, int32_t* pass_launches);
 
+/* ---- auditing a partition map (blance_map_audit, blance_plan_audit, blance_plan_scenarios_audit) ---------------
+ * The planner reports one kind of problem, "could not meet constraints" (plan.go:228-235).  It is silent when a
+ * hierarchy rule's candidate set is empty and findBestNodes falls back to the flat best node (plan.go:214-220): a
+ * replica lands in its primary's rack and nothing says so.  An audit counts, over a finished map, the unmet
+ * constraints, the placements that miss a hierarchy rule and what each node or fault domain holds.  It audits the map
+ * against the rule as the planner applies it to a finished row; it does NOT replay the pass (the planner anchored
+ * the top state's own pass on the OLD primary, and carried one rule's picks into the next rule's prefix).
+ *
+ * Inputs: one map (rows + shapes in the layout of "Id spaces"), the model (n_states, state_slot_off,
+ * state_constraints, top_state), optionally the hierarchy rules (has_hier_rules, n_rules, n_hier_bits, rule_off,
+ * ie_mask) and optionally a fault-domain forest.  Only model states count.  For partition p, L_s is its list of
+ * state s: it HAS a list when shape[p][s] != BLANCE_SHAPE_ABSENT, and len(L_s) is the number of nodes before the
+ * first BLANCE_NO_NODE of the state's slot range (0 for a nil slice, whatever its slots hold).  Node ids must lie in
+ * [-1, n_node_ids) (blance_plan_in_check scans for that; the audit does not): an id outside that range counts
+ * towards len(L_s) but is no copy, never complies, and as a prefix element stands for "".  h is the first node of its list of
+ * top_state, or the "" anchor (id n_node_ids) when that list is absent or empty (plan.go:134-138).  A copy is one
+ * (state, position) entry of any list of p.
+ *
+ * Constraints (states with state_constraints[s] > 0, partitions that have a list for s; the static form of
+ * plan.go:228, which also sees partitions that were not assigned - `warn` never does):
+ *   short_slots[s] = sum over p of max(0, state_constraints[s] - len(L_s));  short_parts = partitions with any
+ *   shortfall;  over_slots[s] = sum over p of max(0, len(L_s) - state_constraints[s]).
+ *
+ * Hierarchy rules (has_hier_rules; states with rules and state_constraints[s] > 0).  Position j of L_s is TESTED
+ * when j < min(len(L_s), state_constraints[s]), except position 0 of top_state (it is the anchor).  For rule r of
+ * state s (global index rule_off[s] <= r < rule_off[s+1]) the node x = L_s[j] COMPLIES iff x < n_nodes (the planner
+ * picks from nodesNext only, plan.go:193-194) and bit x is set in
+ *   includeExcludeNodesIntersect([a] + L_s[0..j-1], r.IncludeLevel, r.ExcludeLevel)      (plan.go:738-753)
+ * read literally over the bit sets ie_mask[r][.]: rv starts empty; for every node y of the list in order, rv becomes
+ * ie_mask[r][y] when rv is empty (the replace-on-empty step of plan.go:746-749, over all n_hier_bits bits), else
+ * rv AND ie_mask[r][y].  The anchor a is h; when h is "" and j > 0 it is L_s[0] (plan.go:178-181); when h is "" and
+ * j = 0 it is "" itself.
+ *   rule_tested[r] = tested (partition, position) pairs;  rule_miss[r] = those that do not comply;
+ *   rule_miss_parts = partitions with at least one miss.
+ *
+ * Fault domains.  domain_parent[n_node_ids + n_domains]: vertices 0 .. n_node_ids-1 are the node ids, the rest are
+ * inner vertices (racks, zones); domain_parent[v] is v's parent vertex or -1 for a root; every vertex is at most 16
+ * edges below its root.  NULL (with n_domains = 0) means every node is its own domain.  A vertex contains itself.
+ *   dom_copies[v] = copies on nodes under v;
+ *   dom_top[v]    = partitions whose h lies under v (they need a promotion if v fails);
+ *   dom_all[v]    = partitions with at least one copy whose EVERY copy lies under v (they are lost if v fails): per
+ *                   partition the deepest common ancestor of its copies and every vertex from there to the root.
+ *   no_top_parts  = partitions whose h is "".
+ *
+ * Failover spread (BLANCE_AUDIT_N2N).  n2n[a][b] (a, b < n_nodes) = number of copies on b of partitions with h = a,
+ * b != a: the final-map form of the nodeToNodeCounts the score spreads (plan.go:238-245).  n2n_max is its largest
+ * entry and (n2n_max_a, n2n_max_b) the lowest (a, b) that holds it - the node that takes the most promotions when a
+ * fails; (-1, -1) when the matrix is all zero.  Without the flag no matrix exists on the device and the three
+ * scalars are -1.
+ *
+ * part_flags[p]: bit 0 = short, bit 1 = rule miss, bit 2 = h is "".
+ * All counts are unweighted; none depends on thread order, the wave size, the engine or the number of devices. */
+enum blance_audit_flags { BLANCE_AUDIT_N2N = 1 };
+
+typedef struct blance_audit_opts {
+  uint32_t flags;                 /* OR of enum blance_audit_flags */
+  int32_t n_domains;              /* inner vertices of the forest; 0 when domain_parent is NULL */
+  const int32_t* domain_parent;   /* [n_node_ids + n_domains] or NULL */
+} blance_audit_opts;
+
+/* Every array may be NULL (not copied).  V = n_node_ids + n_domains; n_rules is the audited instance's own (0
+ * without has_hier_rules). */
+typedef struct blance_audit_out {
+  int64_t* short_slots;           /* [n_states] */
+  int64_t* over_slots;            /* [n_states] */
+  int64_t* rule_miss;             /* [n_rules] */
+  int64_t* rule_tested;           /* [n_rules] */
+  int64_t* dom_top;               /* [V] */
+  int64_t* dom_all;               /* [V] */
+  int64_t* dom_copies;            /* [V] */
+  int32_t* n2n;                   /* [n_nodes][n_nodes], BLANCE_AUDIT_N2N only */
+  uint8_t* part_flags;            /* [n_parts] */
+  int64_t short_parts, rule_miss_parts, no_top_parts;
+  int32_t n2n_max, n2n_max_a, n2n_max_b;
+  float kernel_ms;                /* GPU time of the audit kernels (events around them); in a scenario wave, of the whole
+                                   * wave's audits, the same value in each of its scenarios */
+} blance_audit_out;
+
+/* Audits the map (rows [n_parts][n_slots], shape [n_parts][n_states]) against `model`, of which only the sizes, the
+ * state tables state_slot_off / state_constraints / top_state and the hierarchy fields are read; its own row and
+ * partition tables are ignored and may be NULL.  opts NULL = no flags, nodes only.
+ * Errors, all before any device work: a NULL model, out, rows or shape (with partitions and slots / states to
+ * read); sizes beyond the limits of blance_plan_next_map (8 states, 32 slots, 4096 hierarchy bits ->
+ * BLANCE_ERR_UNSUPPORTED), more than 256 rules (BLANCE_ERR_UNSUPPORTED); an unknown flag; n_domains < 0 or without
+ * domain_parent; a domain_parent entry outside [-1, V), a cycle or a vertex more than 16 edges below its root
+ * (BLANCE_ERR_INVALID_ARG).  Then, without a usable device, BLANCE_ERR_CUDA (also when ctx is NULL because none
+ * could be created). */
+int blance_map_audit(blance_ctx* ctx, const blance_plan_in* model, const int32_t* rows, const uint8_t* shape,
+                     const blance_audit_opts* opts, blance_audit_out* out);
+
+/* The same audit of a resident plan's map as it stands on the device - the result of the last blance_plan_run, the
+ * uploaded partitionsToAssign rows before any run - under the plan's own model and hierarchy, with no copy of the
+ * rows: equal to blance_map_audit on the rows and shapes blance_plan_fetch returns. */
+int blance_plan_audit(blance_ctx* ctx, blance_plan* plan, const blance_audit_opts* opts, blance_audit_out* out);
+
+/* blance_plan_scenarios_schedule, and an audit of every scenario's final map.
+ *
+ * out and sched equal what blance_plan_scenarios_schedule returns for the same arguments.  n_move_conc = 0 with a
+ * NULL move_conc and sched asks for no schedule (out then equals blance_plan_scenarios_ex).
+ * audit[i] (n entries) equals blance_map_audit of scenario i's FINAL MAP - prevMap with every assigned partition
+ * replaced by its next row, the map state_node_load is defined over; a partition in neither map has no lists -
+ * under scenario i's own constraints and hierarchy (blance_scenario_opts) and the shared `aopts`.  The audit runs
+ * inside the wave, next to the summaries and before anything is copied out; its buffers are priced into the wave
+ * size (a few KB per scenario, plus n_nodes x n_nodes x 4 bytes with BLANCE_AUDIT_N2N).
+ * Errors as blance_plan_scenarios_schedule and blance_map_audit, plus a NULL audit, all before any device work. */
+int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                                const blance_audit_opts* aopts, blance_audit_out* audit);
+
 /* ---- CalcPartitionMoves (moves.go:41-119), vectorised over partitions ------- */
 enum blance_op_kind { BLANCE_OP_ADD = 0, BLANCE_OP_DEL = 1, BLANCE_OP_PROMOTE = 2, BLANCE_OP_DEMOTE = 3 };
 #define BLANCE_OP_STATE_NONE 0xFF   /* the "" state of a del op (moves.go:87) */

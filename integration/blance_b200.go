@@ -743,3 +743,150 @@ func (m *movesB200) scheduleB200(maxConcurrent int, nodesAll, states []string) (
 }
 
 func (m *movesB200) free() { C.blance_moves_free(b200(), m.h) }
+
+// ---- auditing a map (blance_map_audit; include/blance_b200.h "auditing a partition map") ------------------------
+// What PlanNextMapEx never reports about a finished map: unmet constraints, copies / top copies / sole copies per
+// node and NodeHierarchy name, and the failover spread.  UNTESTED GO; the C ABI underneath is covered by
+// tests/test_audit_gpu.py and its C++ twin (host_api.cpp AuditMap) by tests/test_audit_host_gpu.py.
+type mapAuditB200 struct {
+	ShortSlots, OverSlots                  map[string]int64 // per model state
+	DomTop, DomAll, DomCopies              map[string]int64 // per node or hierarchy name
+	ShortParts, RuleMissParts, NoTopParts  int64
+	FailoverMax                            int32
+	FailoverMaxFrom, FailoverMaxTo         string
+}
+
+// auditMapB200 audits pmap against model (constraints as PlanNextMapEx would use them).  nodeHierarchy (may be nil) is
+// the fault-domain forest: node ids first, then its other names in byte order; a name without a parent, or whose
+// parent is "", is a root.  To have the hierarchy rules checked too, fill has_hier_rules / n_rules / n_hier_bits /
+// rule_off / ie_mask of the blance_plan_in exactly as planNextMapExB200 does and read rule_miss / rule_tested.
+func auditMapB200(pmap PartitionMap, nodesAll []string, model PartitionModel, nodeHierarchy map[string]string,
+	failoverSpread bool) (*mapAuditB200, error) {
+	var a cArena
+	defer a.free()
+	states := sortStateNames(model)
+	S := len(states)
+	it := &interner{ids: map[string]int32{}}
+	for _, n := range nodesAll {
+		it.get(n)
+	}
+	parts := partitionOrder(pmap, pmap)
+	// slot ranges: max(constraints, longest list) per state
+	width := make([]int, S)
+	for s, st := range states {
+		width[s] = model[st].Constraints
+		for _, p := range pmap {
+			if l := len(p.NodesByState[st]); l > width[s] {
+				width[s] = l
+			}
+		}
+		if width[s] < 0 {
+			width[s] = 0
+		}
+	}
+	cSlot, slot := a.i32(S+1, 0)
+	cK, k := a.i32(S, 0)
+	for s, st := range states {
+		slot[s+1] = slot[s] + int32(width[s])
+		k[s] = int32(model[st].Constraints)
+	}
+	SL := int(slot[S])
+	cRows, rows := a.i32(len(parts)*SL, -1)
+	cShape, shape := a.u8(len(parts) * S)
+	for pi, name := range parts {
+		for s, st := range states {
+			l, ok := pmap[name].NodesByState[st]
+			switch {
+			case !ok:
+				shape[pi*S+s] = C.BLANCE_SHAPE_ABSENT
+			case l == nil:
+				shape[pi*S+s] = C.BLANCE_SHAPE_NIL
+			default:
+				shape[pi*S+s] = C.BLANCE_SHAPE_LIST
+			}
+			for j, n := range l {
+				rows[pi*SL+int(slot[s])+j] = it.get(n)
+			}
+		}
+	}
+	NU := len(it.names)
+	// the forest
+	vertex := append([]string(nil), it.names...)
+	vid := map[string]int32{}
+	for i, n := range vertex {
+		vid[n] = int32(i)
+	}
+	var others []string
+	for c, p := range nodeHierarchy {
+		others = append(others, c, p)
+	}
+	sort.Strings(others)
+	for _, n := range others {
+		if _, ok := vid[n]; !ok && n != "" {
+			vid[n] = int32(len(vertex))
+			vertex = append(vertex, n)
+		}
+	}
+	var opts C.blance_audit_opts
+	if failoverSpread {
+		opts.flags = C.BLANCE_AUDIT_N2N
+	}
+	if nodeHierarchy != nil {
+		cPar, par := a.i32(len(vertex), -1)
+		for c, p := range nodeHierarchy {
+			if c != "" && p != "" {
+				par[vid[c]] = vid[p]
+			}
+		}
+		opts.n_domains = C.int32_t(len(vertex) - NU)
+		opts.domain_parent = cPar
+	}
+	var in C.blance_plan_in
+	in.n_nodes, in.n_node_ids = C.int32_t(len(nodesAll)), C.int32_t(NU)
+	in.n_states, in.n_parts, in.n_slots = C.int32_t(S), C.int32_t(len(parts)), C.int32_t(SL)
+	in.top_state = 0 // sortStateNames puts the top-priority state first (plan.go:126-132)
+	in.state_constraints, in.state_slot_off = cK, cSlot
+	V := len(vertex)
+	i64 := func(n int) (*C.int64_t, []int64) {
+		p := C.calloc(C.size_t(n+1), 8)
+		a.ptrs = append(a.ptrs, p)
+		return (*C.int64_t)(p), unsafe.Slice((*int64)(p), n+1)[:n]
+	}
+	var out C.blance_audit_out
+	var short, over, top, all, copies []int64
+	out.short_slots, short = i64(S)
+	out.over_slots, over = i64(S)
+	out.dom_top, top = i64(V)
+	out.dom_all, all = i64(V)
+	out.dom_copies, copies = i64(V)
+	if st := C.blance_map_audit(b200(), &in, cRows, cShape, &opts, &out); st != C.BLANCE_OK {
+		return nil, fmt.Errorf("blance_map_audit: %s", C.GoString(C.blance_last_error(b200())))
+	}
+	r := &mapAuditB200{ShortSlots: map[string]int64{}, OverSlots: map[string]int64{}, DomTop: map[string]int64{},
+		DomAll: map[string]int64{}, DomCopies: map[string]int64{},
+		ShortParts: int64(out.short_parts), RuleMissParts: int64(out.rule_miss_parts), NoTopParts: int64(out.no_top_parts)}
+	for s, st := range states {
+		if short[s] != 0 {
+			r.ShortSlots[st] = short[s]
+		}
+		if over[s] != 0 {
+			r.OverSlots[st] = over[s]
+		}
+	}
+	for v, n := range vertex {
+		if top[v] != 0 {
+			r.DomTop[n] = top[v]
+		}
+		if all[v] != 0 {
+			r.DomAll[n] = all[v]
+		}
+		if copies[v] != 0 {
+			r.DomCopies[n] = copies[v]
+		}
+	}
+	if failoverSpread && out.n2n_max_a >= 0 {
+		r.FailoverMax = int32(out.n2n_max)
+		r.FailoverMaxFrom, r.FailoverMaxTo = it.names[out.n2n_max_a], it.names[out.n2n_max_b]
+	}
+	return r, nil
+}
