@@ -47,7 +47,7 @@ def host_module_path():
 def build_cuda_lib(force=False, verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     srcs = [os.path.join(CSRC, "c_abi.cu")]
-    deps = srcs + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(INCLUDE, "blance_b200.h")]
+    deps = srcs + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(CSRC, "count_bound.hpp"), os.path.join(INCLUDE, "blance_b200.h")]
     out = lib_path()
     if force or _newer(deps, out):
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -62,7 +62,7 @@ def build_host_module(force=False):
     import pybind11
     out = host_module_path()
     srcs = [os.path.join(CSRC, "host_api.cpp"), os.path.join(CSRC, "py_module.cpp")]
-    deps = srcs + [os.path.join(CSRC, "host_api.hpp"), os.path.join(INCLUDE, "blance_b200.h"), lib_path()]
+    deps = srcs + [os.path.join(CSRC, "host_api.hpp"), os.path.join(CSRC, "count_bound.hpp"), os.path.join(INCLUDE, "blance_b200.h"), lib_path()]
     if force or _newer(deps, out):
         cxx = os.environ.get("CXX", "g++")
         cmd = [cxx, "-O2", "-std=c++17", "-pthread", "-fPIC", "-shared", "-fvisibility=hidden",

@@ -27,6 +27,7 @@
 #include "audit.cuh"
 #include "aux_kernels.cuh"
 #include "blance_b200.h"
+#include "count_bound.hpp"
 #include "device_types.cuh"
 #include "wave_schedule.cuh"
 
@@ -451,6 +452,7 @@ extern "C" int blance_plan_in_check(const blance_plan_in* in, char* msg, int32_t
       if (in->has_part_weights && in->part_has_weight[p] && in->part_weight[p] > 999999999)
         return bad("partition weight above 999999999 at partition " + std::to_string(p), BLANCE_ERR_UNSUPPORTED);
   }
+  if (!count_bound_fits(*in)) return bad(BLANCE_COUNT_BOUND_MSG, BLANCE_ERR_UNSUPPORTED);
   if (in->has_hier_rules)
     for (int s = 0; s <= in->n_states; ++s) {
       if (in->rule_off[s] < 0 || in->rule_off[s] > in->n_rules || (s > 0 && in->rule_off[s] < in->rule_off[s - 1]))
@@ -1043,9 +1045,8 @@ static int n_overrides(const blance_scenario_opts* o) {
   return o && (o->set & BLANCE_OPT_PART_WEIGHTS) ? o->n_weight_overrides : 0;
 }
 
-// The option checks of one scenario that check_structure cannot make (flags, override lists, the int32 bound).
-// base_sum: sum over the base's partitions of |weight| (1 where it has none), computed once by the caller.
-static int check_opts(const blance_plan_in& base, const blance_scenario_opts& o, long long base_sum, std::string& why) {
+// The option checks of one scenario that check_structure cannot make (flags, override lists, the "%10d" rule).
+static int check_opts(const blance_plan_in& base, const blance_scenario_opts& o, std::string& why) {
   auto bad = [&](const std::string& what, int st = BLANCE_ERR_INVALID_ARG) { why = what; return st; };
   const uint32_t all = BLANCE_OPT_CONSTRAINTS | BLANCE_OPT_STICKINESS | BLANCE_OPT_PART_WEIGHTS | BLANCE_OPT_HIERARCHY;
   if (o.set & ~all) return bad("opts.set has an unknown bit");
@@ -1062,18 +1063,35 @@ static int check_opts(const blance_plan_in& base, const blance_scenario_opts& o,
   std::sort(seen.begin(), seen.end());
   if (k > 0 && (seen.front() < 0 || seen.back() >= base.n_parts)) return bad("a weight override's partition is outside [0, n_parts)");
   if (std::adjacent_find(seen.begin(), seen.end()) != seen.end()) return bad("a partition has two weight overrides");
-  long long sum = base_sum;                 // sum |w_p| with the overrides applied (as if PartitionWeights != nil)
   for (int j = 0; j < k; ++j) {
     if (o.ow_has[j] > 1) return bad("ow_has is neither 0 nor 1");
     if (o.ow_has[j] && o.ow_weight[j] > 999999999)      // the "%10d" rule of plan.go:539, as blance_plan_in_check
       return bad("partition weight above 999999999 in override " + std::to_string(j), BLANCE_ERR_UNSUPPORTED);
-    const int32_t p = o.ow_part[j];
-    const long long old_w = base.part_has_weight[p] ? std::llabs((long long)base.part_weight[p]) : 1;
-    sum += (o.ow_has[j] ? std::llabs((long long)o.ow_weight[j]) : 1) - old_w;
   }
-  const long long bound = (o.has_part_weights ? sum : (long long)base.n_parts) * std::max(1, base.n_slots);
-  if (bound > INT32_MAX) return bad("sum of partition weights x slots exceeds int32 (the device keeps int32 counts)", BLANCE_ERR_UNSUPPORTED);
   return BLANCE_OK;
+}
+
+// The count bound (count_bound.hpp) of one scenario's substituted instance `in`, with its weight overrides applied.
+// base_sum: sum over the base's partitions of |weight| as if PartitionWeights != nil (1 where it has none), computed
+// once by the caller (< 0: not yet).
+static int check_counts(const blance_plan_in& base, const blance_plan_in& in, const blance_scenario_opts* o, long long& base_sum,
+                        std::string& why) {
+  long long sum = in.n_parts;
+  if (in.has_part_weights) {
+    if (base_sum < 0) {
+      blance_plan_in weighted = base;
+      weighted.has_part_weights = 1;
+      base_sum = count_bound_weight_sum(weighted);
+    }
+    sum = base_sum;
+    for (int j = 0; j < n_overrides(o); ++j) {
+      const int32_t p = o->ow_part[j];
+      sum += (o->ow_has[j] ? std::llabs((long long)o->ow_weight[j]) : 1) - (base.part_has_weight[p] ? std::llabs((long long)base.part_weight[p]) : 1);
+    }
+  }
+  if (count_bound_fits(sum, in.n_slots, count_bound_max_extra(in.n_nodes, in.extra_tot_first, in.extra_tot_rest))) return BLANCE_OK;
+  why = BLANCE_COUNT_BOUND_MSG;
+  return BLANCE_ERR_UNSUPPORTED;
 }
 
 // uint32 words of one instance's hierarchy masks
@@ -1665,10 +1683,9 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
 static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                            const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
                            const SchedReq* sr = nullptr, const AuditReq* ar = nullptr) {
-  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
   if (!base || !sc || !out) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
-  // every scenario is checked before any device work
+  // every scenario is checked before the context is used, so a NULL ctx checks the scenarios without a device
   long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
   for (int i = 0; i < n; ++i) {
     std::string why;
@@ -1679,15 +1696,13 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
     else {
       const blance_plan_in in = scenario_in(*base, sc[i], o);
       st = check_structure(&in, why);
-      if (st == BLANCE_OK && o && (o->set & BLANCE_OPT_PART_WEIGHTS) && base_sum < 0) {
-        base_sum = 0;
-        for (int p = 0; p < base->n_parts; ++p) base_sum += base->part_has_weight[p] ? std::llabs((long long)base->part_weight[p]) : 1;
-      }
-      if (st == BLANCE_OK && o) st = check_opts(*base, *o, base_sum, why);
+      if (st == BLANCE_OK && o) st = check_opts(*base, *o, why);
+      if (st == BLANCE_OK) st = check_counts(*base, in, o, base_sum, why);
     }
     if (st == BLANCE_OK && !why.empty()) st = BLANCE_ERR_INVALID_ARG;
     if (st != BLANCE_OK) throw_err(st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
   }
+  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
   // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
   const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);

@@ -1,6 +1,7 @@
 // blance_b200/csrc/host_api.cpp — see host_api.hpp.  Interning (strings -> flat
 // int32 tables), the calls into the CUDA library, and the way back to maps.
 #include "host_api.hpp"
+#include "count_bound.hpp"
 
 #include <algorithm>
 #include <functional>
@@ -229,8 +230,11 @@ struct Hierarchy {
   }
 };
 
-int32_t checked_i32(long long v, const char* what) {
-  if (v < INT32_MIN || v > INT32_MAX) invalid(std::string(what) + " does not fit int32");
+[[noreturn]] void counts_too_large() { throw BlanceError(BLANCE_ERR_UNSUPPORTED, std::string("blance: ") + BLANCE_COUNT_BOUND_MSG); }
+
+// a count of non-model states: beyond int32 the count bound (count_bound.hpp) fails as well
+int32_t count_i32(long long v) {
+  if (v < INT32_MIN || v > INT32_MAX) counts_too_large();
   return int32_t(v);
 }
 
@@ -573,19 +577,9 @@ static std::unique_ptr<InternedPlan> intern_plan(const PartitionMap& prevMap, co
     ip->extra_node.push_back(e.node);
     if (e.node >= N) continue;
     long long w = (options.PartitionWeights && ip->part_has_weight[size_t(e.part)]) ? ip->part_weight[size_t(e.part)] : 1;
-    ip->extra_tot_first[size_t(e.node)] = checked_i32((long long)ip->extra_tot_first[size_t(e.node)] + w, "count");
+    ip->extra_tot_first[size_t(e.node)] = count_i32((long long)ip->extra_tot_first[size_t(e.node)] + w);
     if (!ip->part_in_assign[size_t(e.part)])
-      ip->extra_tot_rest[size_t(e.node)] = checked_i32((long long)ip->extra_tot_rest[size_t(e.node)] + w, "count");
-  }
-
-  // int32 is wide enough for every count the device keeps: sum |w_p| * slots
-  {
-    long long bound = 0;
-    for (int32_t p = 0; p < PU; ++p) {
-      long long w = (options.PartitionWeights && ip->part_has_weight[size_t(p)]) ? ip->part_weight[size_t(p)] : 1;
-      bound += (w < 0 ? -w : w) * std::max<long long>(1, SL);
-    }
-    if (bound > INT32_MAX) invalid("sum of partition weights x slots exceeds int32 (the device keeps int32 counts)");
+      ip->extra_tot_rest[size_t(e.node)] = count_i32((long long)ip->extra_tot_rest[size_t(e.node)] + w);
   }
 
   // ---- hierarchy bit sets
@@ -628,6 +622,7 @@ static std::unique_ptr<InternedPlan> intern_plan(const PartitionMap& prevMap, co
   in.rule_off = ip->rule_off.data();
   in.ie_mask = ip->ie_mask.empty() ? nullptr : ip->ie_mask.data();
   in.engine = options.Engine;
+  if (!count_bound_fits(in)) counts_too_large();
   return ip;
 }
 
@@ -1096,8 +1091,8 @@ ScenarioTables scenario_tables(const InternedPlan& ip, const PartitionModel& mod
       for (size_t e = 0; e < ip.extra_part.size(); ++e) {
         const int32_t p = ip.extra_part[e], q = ip.extra_node[e];
         if (q >= N) continue;
-        t.extra_first[size_t(q)] = checked_i32((long long)t.extra_first[size_t(q)] + w_mine(p), "count");
-        if (!ip.part_in_assign[size_t(p)]) t.extra_rest[size_t(q)] = checked_i32((long long)t.extra_rest[size_t(q)] + w_mine(p), "count");
+        t.extra_first[size_t(q)] = count_i32((long long)t.extra_first[size_t(q)] + w_mine(p));
+        if (!ip.part_in_assign[size_t(p)]) t.extra_rest[size_t(q)] = count_i32((long long)t.extra_rest[size_t(q)] + w_mine(p));
       }
     }
   }

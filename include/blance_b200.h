@@ -164,10 +164,17 @@ typedef struct blance_plan_out {
 /* Checks one instance's tables without planning anything and without a device: sizes, pointers and limits (what
  * every planning entry point checks itself) AND the contents - state_slot_off[0] == 0, node ids of both row tables
  * in [-1, n_node_ids), each state's slots filled from the left, shape values, part_name_rank unique and below
- * 2^30, partition weights within the "%10d" rule of plan.go:539, rule_off monotone.  The planning entry points do
- * NOT scan the contents (it would sit in the timed path of every call): a binding that does not trust its own
- * marshalling calls this first.  Returns BLANCE_OK / BLANCE_ERR_INVALID_ARG / BLANCE_ERR_UNSUPPORTED; msg (may be
- * NULL) receives the reason, truncated to msg_cap bytes. */
+ * 2^30, partition weights within the "%10d" rule of plan.go:539, rule_off monotone, and the count bound below.
+ * The planning entry points do NOT scan the contents (it would sit in the timed path of every call): a binding that
+ * does not trust its own marshalling calls this first.
+ *
+ * The count bound: the reference counts in 64-bit ints, the device keeps every node's weighted count in int32.
+ *     sum_p |w_p| * max(1, n_slots) + max_n max(|extra_tot_first[n]|, |extra_tot_rest[n]|) <= INT32_MAX
+ * (w_p = part_weight[p] where has_part_weights and part_has_weight[p], else 1) bounds every such count; an instance
+ * above it is BLANCE_ERR_UNSUPPORTED here.  Planning such an instance is undefined: its counts wrap.
+ *
+ * Returns BLANCE_OK / BLANCE_ERR_INVALID_ARG / BLANCE_ERR_UNSUPPORTED; msg (may be NULL) receives the reason,
+ * truncated to msg_cap bytes. */
 int blance_plan_in_check(const blance_plan_in* in, char* msg, int32_t msg_cap);
 
 /* Host buffers in, host buffers out.  If prevMap and partitionsToAssign must be
@@ -221,7 +228,10 @@ typedef struct blance_scenario_out {
  *   warn_parts: assigned partitions with at least one warning bit.
  *
  * Errors: n <= 0, a NULL sc / out, or a bad scenario (the first one fails the call; the message names its
- * index) is BLANCE_ERR_INVALID_ARG, checked before any device work.  BLANCE_ERR_NOMEM when one scenario does
+ * index) is BLANCE_ERR_INVALID_ARG, checked before any device work.  A scenario above the count bound of
+ * blance_plan_in_check (on its own partition weights and non-model counts) is BLANCE_ERR_UNSUPPORTED.  Every
+ * scenario is checked before ctx is used: with ctx NULL the call returns the first scenario's error, or
+ * BLANCE_ERR_INVALID_ARG for the NULL ctx when every scenario passes.  BLANCE_ERR_NOMEM when one scenario does
  * not fit in device memory.
  *
  * Scheduling: the base's partition tables are uploaded once per device and replicated on the device into each
@@ -246,7 +256,8 @@ int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n
  *                            gets weight ow_weight[j] and presence ow_has[j], each [n_weight_overrides].
  *                            extra_tot_first / extra_tot_rest ([n_nodes], NULL = the base's) replace the counts of
  *                            non-model states (see blance_plan_in): a caller that reweights a partition holding such
- *                            entries must supply them, the device cannot derive them.
+ *                            entries must supply them, the device cannot derive them.  The scenario's weights and
+ *                            non-model counts must keep the count bound of blance_plan_in_check.
  *   BLANCE_OPT_HIERARCHY     NodeHierarchy and HierarchyRules: has_hier_rules, n_rules, n_hier_bits, rule_off,
  *                            ie_mask, with the meaning they have in blance_plan_in. */
 enum blance_scenario_opt_set {
@@ -286,7 +297,7 @@ typedef struct blance_scenario_opts {
  * checks of blance_plan_next_map (e.g. constraints > 16 or beyond the slot range, rules x constraints > 32, a
  * hierarchy universe above 4096 bits); an unknown bit in `set`; a flag that is neither 0 nor 1; an override index
  * outside [0, n_parts) or listed twice; NULL override arrays (BLANCE_ERR_INVALID_ARG).  An override weight above
- * 999999999 (plan.go:539) or a sum of |partition weight| x n_slots at or above 2^31 is BLANCE_ERR_UNSUPPORTED.
+ * 999999999 (plan.go:539) or a scenario above the count bound of blance_plan_in_check is BLANCE_ERR_UNSUPPORTED.
  *
  * Scheduling as blance_plan_scenarios; the automatic wave size is priced by the wave's largest scenario (its
  * hierarchy masks), and the overrides are applied on the device after each wave is replicated from the base. */

@@ -3,7 +3,8 @@ divisor's correctly rounded reciprocal plus one FMA-residual correction
 (assign_pass.cuh: div_exact).  This test runs the same sequence on the CPU (C, real
 fma(), no contraction) against true IEEE division on adversarial operands: exact
 multiples +- a few ulps, half-way quotients, planner-shaped values, integer divisors from
-3 to 2e9.  Zero mismatches allowed.  CPU only."""
+3 to 2^31 - 1 (node weights are int32), dividends of both signs (counts go negative under
+negative partition weights).  Zero mismatches allowed.  CPU only."""
 import os
 import subprocess
 import tempfile
@@ -20,8 +21,10 @@ static double div_exact(double a, double b, double y) { double q = a * y; double
 int main(void) {
   long bad = 0, n = 0;
   for (long it = 0; it < 40000000L; ++it) {
-    uint64_t a = rnd(), b = rnd();
-    double w = (it & 1) ? (double)(3 + (b % 5000)) : (double)(3 + (b % 2000000000ull));
+    uint64_t a = rnd(), b = rnd(), c = rnd();
+    double w = (it & 1) ? (double)(3 + (b % 5000))
+             : (c & 1) ? (double)(2000000000ull + (b % 147483648ull)) : (double)(3 + (b % 2000000000ull));
+    if ((c & 0xff0) == 0) w = 2147483647.0;
     double r;
     int mode = a & 3;
     if (mode == 0) { uint64_t m = (a >> 8) & ((1ull << 52) - 1); int e = (int)((a >> 60) % 70) - 40; r = ldexp(1.0 + (double)m / 4503599627370496.0, e); }
@@ -31,6 +34,7 @@ int main(void) {
     else { uint64_t m = (a >> 8) & ((1ull << 52) - 1); double q = 1.0 + (double)m / 4503599627370496.0; double h = q + ldexp(1.0, -53);
       r = (double)((long double)h * (long double)w); }
     if (!(r > 0)) continue;
+    if (c & 2) r = -r;
     double y = 1.0 / w;
     n++;
     if (div_exact(r, w, y) != r / w) bad++;
