@@ -19,8 +19,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 
 _API_NAMES = ("AuditMap", "BOOSTER_CBGT_MAX", "BOOSTER_NONE", "BlanceError", "CalcPartitionMoves", "CalcPartitionMovesMap",
               "NodeStateOp", "OrchestrateSchedule", "OrchestratorOptions", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions",
-              "PlanNextMapScenarios", "capi")
-__all__ = ["AuditMap", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "CalcPartitionMoves", "CalcPartitionMovesMap",
+              "PlanNextMapChains", "PlanNextMapScenarios", "capi")
+__all__ = ["AuditMap", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "PlanNextMapChains", "CalcPartitionMoves", "CalcPartitionMovesMap",
            "NodeStateOp", "OrchestrateSchedule", "OrchestratorOptions", "BlanceError", "BOOSTER_NONE", "BOOSTER_CBGT_MAX", "capi"]
 
 

@@ -57,6 +57,14 @@ class _ScenarioScheduleOut(ctypes.Structure):  # struct blance_scenario_schedule
                 ("part_done_round", ctypes.c_void_p)]
 
 
+class _ChainStage(ctypes.Structure):   # struct blance_chain_stage
+    _fields_ = [("nodes", _Scenario), ("node_in_all", ctypes.c_void_p)]
+
+
+class _ChainOut(ctypes.Structure):     # struct blance_chain_out
+    _fields_ = [("node_ops", ctypes.c_void_p), ("ops_total", ctypes.c_int64), ("parts_moved", ctypes.c_int64)]
+
+
 OPT_CONSTRAINTS, OPT_STICKINESS, OPT_PART_WEIGHTS, OPT_HIERARCHY = 1, 2, 4, 8   # enum blance_scenario_opt_set
 
 
@@ -87,7 +95,7 @@ class _AuditOut(ctypes.Structure):     # struct blance_audit_out
 
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_chains", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
            "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_free")
 
@@ -114,6 +122,7 @@ def capi():
         lib.blance_plan_scenarios_ex.argtypes = [vp, vp, i32, vp, vp, i32, i32, vp]
         lib.blance_plan_scenarios_schedule.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]
         lib.blance_plan_scenarios_audit.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+        lib.blance_plan_chains.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, vp, vp]
         lib.blance_map_audit.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.blance_plan_audit.argtypes = [vp, vp, vp, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
@@ -141,6 +150,8 @@ Scenario = _Scenario
 ScenarioOpts = _ScenarioOpts
 ScenarioOut = _ScenarioOut
 ScheduleOut = _ScheduleOut
+ChainStage = _ChainStage
+ChainOut = _ChainOut
 ScenarioScheduleOut = _ScenarioScheduleOut
 AuditOpts = _AuditOpts
 AuditOut = _AuditOut

@@ -137,6 +137,43 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
                                       audit=None if audit is None else bool(audit.get("failoverSpread", False)))
 
 
+def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None, chains=(), favorMinNodes=False,
+                      wantMaps=(), maxConcurrent=0):
+    """Chains of cluster changes, each stage planned on the map the stage before produced (blance_plan_chains).  Chain
+    i runs the Go loop `next = PlanNextMapEx(prev, assign, nodesAll_t, nodesToRemove_t, nodesToAdd_t, model, options_i_t);
+    prev = prev with every entry of next replaced; assign = next` over its stages.  nodesAll is the universe: a stage's
+    nodesAll is a subset of it, always in its order.  A chain is a dict with "stages" (a list) and the optional option
+    keys of PlanNextMapScenarios' scenarios ("nodeWeights", "modelStateConstraints", "stateStickiness",
+    "partitionWeights", "nodeHierarchy", "hierarchyRules": missing inherits the options, None means nil), shared by
+    its stages.  A stage is a dict with "nodesToRemove" and "nodesToAdd" (required, None = nil), an optional
+    "nodeWeights" and an optional "nodesAll"; without it, the previous stage's members minus its nodesToRemove plus
+    this stage's nodesToAdd (the first stage: the whole universe).  Every chain has the same number of stages.  The
+    caller's maps are NOT mutated.
+
+    Returns one dict per chain: "stages", one dict per stage with the keys of PlanNextMapScenarios' results (next_map
+    and warnings for the chains in wantMaps), and "net": node_ops, ops_total and parts_moved of CalcPartitionMoves
+    from the base prevMap to the last stage's map."""
+    o = options or PlanNextMapOptions()
+    same = prevMap is partitionsToAssign
+    cs = []
+    for i, c in enumerate(chains):
+        opts = {k: v for k, v in c.items() if k != "stages"}
+        opts.update(nodesToRemove=None, nodesToAdd=None)
+        stages = []
+        for t, st in enumerate(c["stages"]):
+            missing = {"nodesToRemove", "nodesToAdd"} - set(st)
+            if missing:
+                raise ValueError("chain %d, stage %d lacks %s" % (i, t, ", ".join(sorted(missing))))
+            rm, ad, na = st["nodesToRemove"], st["nodesToAdd"], st.get("nodesAll")
+            nw = st.get("nodeWeights")
+            stages.append((None if rm is None else list(rm), None if ad is None else list(ad), "nodeWeights" in st,
+                           None if nw is None else dict(nw), None if na is None else list(na)))
+        cs.append((_scenario_tuples([opts])[0], stages))
+    return _host.PlanNextMapChains(prevMap, None if same else partitionsToAssign, list(nodesAll),
+                                   {k: tuple(v) for k, v in model.items()}, cs, bool(favorMinNodes),
+                                   [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o))
+
+
 def AuditMap(partitionMap, nodesAll, model, options=None, failoverSpread=False):
     """What the planner never reports about a finished map (include/blance_b200.h, "auditing a partition map"),
     counted on the device.  options (PlanNextMapOptions): ModelStateConstraints override the model's constraints;

@@ -60,7 +60,7 @@ __global__ void k_pack(DPool pool, int32_t* __restrict__ raw_next, uint8_t* __re
 }
 
 // ---- start of an iteration (plan.go:83-88, 70) -------------------------------------------
-// Working rows = partitionsToAssign rows minus the to-be-removed nodes (order kept);
+// Working rows = partitionsToAssign rows minus the to-be-removed nodes (bit NR_REMOVE; order kept);
 // every present state list becomes a non-nil slice; warnings are reset.
 __global__ void k_prepare_rows(DPool pool, long long n_parts_total) {
   for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < n_parts_total;
@@ -78,7 +78,7 @@ __global__ void k_prepare_rows(DPool pool, long long n_parts_total) {
       for (int i = o; i < hi; ++i) {
         const int32_t x = row[i];
         if (x == BLANCE_NO_NODE) break;
-        if (!pool.node_removed[D.nodeid_off + x]) row[o++] = x;
+        if (!(pool.node_removed[D.nodeid_off + x] & NR_REMOVE)) row[o++] = x;
       }
       for (; o < hi; ++o) row[o] = BLANCE_NO_NODE;
     }
@@ -138,7 +138,7 @@ __global__ void k_build_keys(DPool pool, int s, long long n_parts_total) {
       for (int i = D.state_slot_off[s]; i < D.state_slot_off[s + 1]; ++i) {
         const int32_t x = prow[i];
         if (x == BLANCE_NO_NODE) break;
-        b0 |= pool.node_removed[D.nodeid_off + x] != 0;
+        b0 |= (pool.node_removed[D.nodeid_off + x] & NR_REMOVE) != 0;
       }
     }
     if (b0) bucket = 0;
@@ -198,7 +198,7 @@ __global__ void k_gather_stream(DPool pool, int s, long long n_parts_total) {
     bool clean = true;
     for (int a = lo; a < hi && row[a] != BLANCE_NO_NODE; ++a) {
       ++n_cur;
-      if (row[a] >= D.N) clean = false;
+      if (row[a] >= D.N || (D.masked && (pool.node_removed[D.nodeid_off + row[a]] & NR_OUTSIDE))) clean = false;
       for (int b = 0; b < D.SL; ++b)
         if (b != a && row[b] == row[a]) clean = false;
     }

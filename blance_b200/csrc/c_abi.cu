@@ -470,8 +470,29 @@ static int grid_for(const blance_ctx* ctx, long long n, int block) {
   return (int)want;
 }
 
+// The device code (NR_REMOVE | NR_OUTSIDE) of node id q of an instance.  A caller's node_removed says only "in
+// nodesToRemove", any nonzero value meaning yes; `coded` tables (blance_plan_chains' stages) already hold the code.
+static uint8_t rm_code(const blance_plan_in& in, int q, bool coded) {
+  const uint8_t v = in.node_removed[q];
+  return coded ? v : (uint8_t)(v ? NR_REMOVE : 0);
+}
+
+// The node fields of a descriptor that a scenario or a chain stage changes, and the loop state they start it in:
+// nodesNext's size, whether nodesToRemove is non-empty (also with ids outside nodesAll), nodesToAdd == nil.  n_prev =
+// len(prevMap).
+static void node_state(DInst& D, const blance_plan_in& in, bool coded, int n_prev) {
+  int n_valid = 0, rm_active = 0, masked = 0;
+  for (int q = 0; q < in.n_nodes; ++q) { n_valid += rm_code(in, q, coded) == 0; masked |= (rm_code(in, q, coded) & NR_OUTSIDE) != 0; }
+  for (int q = 0; q < in.n_node_ids; ++q) rm_active |= rm_code(in, q, coded) & NR_REMOVE;
+  D.has_node_weights = in.has_node_weights;
+  D.n_valid = n_valid; D.masked = masked;
+  D.P = n_prev; D.rm_active = rm_active; D.add_active = 1; D.add_is_nil = in.add_is_nil; D.use_rest = 0;
+  D.active = in.max_iters > 0 ? 1 : 0;
+  D.iters_run = 0; D.converged = 0; D.mismatch = 0;
+}
+
 // Host side of a batch: the per-instance descriptors, their offsets into the pooled arrays and the totals.
-static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off) {
+static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off, bool coded = false) {
   pl->n_inst = n;
   pl->h_insts.resize(n);
   pl->raw_rows_off.resize(n + 1);
@@ -501,7 +522,6 @@ static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vecto
     }
     D.state_slot_off[in.n_states] = in.n_slots;
     D.rule_off[in.n_states] = in.has_hier_rules ? in.rule_off[in.n_states] : 0;
-    int n_valid = 0, rm_active = 0;
     // (the instances of a scenario wave share their partition tables: counted once)
     const bool same_parts = i > 0 && in.n_parts == ins[i - 1].n_parts && in.part_in_prev == ins[i - 1].part_in_prev &&
                             in.part_in_assign == ins[i - 1].part_in_assign;
@@ -509,11 +529,8 @@ static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vecto
       n_prev = 0; n_assign = 0;
       for (int p = 0; p < in.n_parts; ++p) { n_prev += in.part_in_prev[p] != 0; n_assign += in.part_in_assign[p] != 0; }
     }
-    for (int q = 0; q < in.n_nodes; ++q) n_valid += in.node_removed[q] == 0;
-    for (int q = 0; q < in.n_node_ids; ++q) rm_active |= in.node_removed[q] != 0;
-    D.n_assign = n_assign; D.n_valid = n_valid;
-    D.P = n_prev; D.rm_active = rm_active; D.add_active = 1; D.add_is_nil = in.add_is_nil; D.use_rest = 0;
-    D.active = in.max_iters > 0 ? 1 : 0;
+    D.n_assign = n_assign;
+    node_state(D, in, coded, n_prev);
     D.part_off = pl->PT; D.rows_off = pl->RT; D.node_off = pl->NT; D.nodeid_off = pl->NUT;
     D.counts_off = pl->CT; D.n2n_off = pl->N2T; D.mask_off = pl->MT; D.stream_off = pl->ST;
     pl->raw_rows_off[i] = pl->RRT; pl->raw_shape_off[i] = pl->RST;
@@ -593,8 +610,9 @@ struct NodeTables {
 };
 
 // Writes instance `in` (descriptor D) into its slices of t.
-static void stage_nodes(const blance_plan_in& in, const DInst& D, const NodeTables& t) {
-  if (D.NU) { std::memcpy(t.rm + D.nodeid_off, in.node_removed, (size_t)D.NU); std::memcpy(t.ad + D.nodeid_off, in.node_added, (size_t)D.NU); }
+static void stage_nodes(const blance_plan_in& in, const DInst& D, const NodeTables& t, bool coded = false) {
+  for (int q = 0; q < D.NU; ++q) t.rm[D.nodeid_off + q] = rm_code(in, q, coded);
+  if (D.NU) std::memcpy(t.ad + D.nodeid_off, in.node_added, (size_t)D.NU);
   for (int q = 0; q < D.N; ++q) {
     t.nw[D.node_off + q] = in.has_node_weights ? in.node_weight[q] : 0;
     t.hw[D.node_off + q] = in.has_node_weights ? in.node_has_weight[q] : 0;
@@ -610,12 +628,12 @@ static uint8_t part_flags(const blance_plan_in& in, int p) {
                    (in.part_in_assign[p] ? PF_IN_ASSIGN : 0) | (in.part_has_weight[p] ? PF_HAS_WEIGHT : 0));
 }
 
-static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins) {
+static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins, bool coded = false) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, "batch size must be positive");
   for (int i = 0; i < n; ++i) validate(&ins[i], i);
   PlanPtr pl(new blance_plan());
   std::vector<int> seg_off;
-  layout(pl.get(), n, ins, seg_off);
+  layout(pl.get(), n, ins, seg_off, coded);
   if (pl->PT >= (1LL << 29)) throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch");
   plan_slices(pl->arena, pl.get(), n);
   pl->arena.alloc(ctx->stream, "the plan arena");
@@ -627,14 +645,16 @@ static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins) {
   const int32_t *h_nw = nullptr, *h_ef = nullptr, *h_er = nullptr;
   const uint8_t *h_csh = nullptr, *h_psh = nullptr, *h_flags = nullptr, *h_rm = nullptr, *h_ad = nullptr, *h_hw = nullptr;
   const uint32_t* h_mask = nullptr;
-  std::vector<uint8_t> v_flags;
+  std::vector<uint8_t> v_flags, v_rm;
   if (direct(pl.get())) {
     const blance_plan_in& in = ins[0];
     v_flags.resize((size_t)in.n_parts + 1);
     for (int p = 0; p < in.n_parts; ++p) v_flags[(size_t)p] = part_flags(in, p);
+    v_rm.resize((size_t)in.n_node_ids + 1);
+    for (int q = 0; q < in.n_node_ids; ++q) v_rm[(size_t)q] = rm_code(in, q, coded);
     h_cur = in.cur_rows; h_prev = in.prev_rows; h_csh = in.cur_shape; h_psh = in.prev_shape;
     h_flags = v_flags.data(); h_pw = in.part_weight; h_rank = in.part_name_rank;     // h_inst stays NULL: all zero
-    h_rm = in.node_removed; h_ad = in.node_added;
+    h_rm = v_rm.data(); h_ad = in.node_added;
     if (in.has_node_weights) { h_nw = in.node_weight; h_hw = in.node_has_weight; }
     h_ef = in.extra_tot_first; h_er = in.extra_tot_rest; h_mask = in.ie_mask;
   } else {
@@ -673,7 +693,7 @@ static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins) {
         s_rank[g] = in.part_name_rank[p];
         s_inst[g] = i;
       }
-      stage_nodes(in, D, s);
+      stage_nodes(in, D, s, coded);
     };
     // instances are staged by a few host threads (a 1 024-instance fan-out is ~1 M partitions of flag packing)
     int T = (int)std::min<long long>(8, std::max<long long>(1, pl->PT / 65536));
@@ -1147,7 +1167,7 @@ static void sched_slices(Arena& a, int nw, int nc, long long PU, long long NU, i
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
 // their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and override list of any.
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
-                     int max_concurrent, const SchedReq* sr, size_t audit_bytes, size_t* per_scenario) {
+                     int max_concurrent, const SchedReq* sr, size_t extra_bytes, size_t* per_scenario) {
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
@@ -1156,7 +1176,7 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   size_t per = one.bytes() + sort_scratch_bytes(probe.PT, 1, ctx->stream) +
                sizeof(long long) * (size_t)summary_stride(in0) +
                sizeof(uint32_t) * (size_t)(max_mask_words - mask_words(in0)) + 3 * sizeof(int32_t) * (size_t)max_overrides +
-               audit_bytes;
+               extra_bytes;
   if (sr) {
     Arena sched;
     WSched w{};
@@ -1466,28 +1486,98 @@ static void audit_unpack(blance_ctx* ctx, const AuditBufs& b, int n_rules, const
   }
 }
 
+// The chains requested with blance_plan_chains: T stages per chain, stages [n][T], net [n] or NULL.
+struct ChainReq {
+  int T = 1;
+  const blance_chain_stage* stages = nullptr;
+  blance_chain_out* net = nullptr;
+};
+
+// The node fields of scenario (or chain) i at stage t.
+static const blance_scenario& nodes_of(const blance_scenario* sc, const ChainReq* cr, int i, int t) {
+  return cr ? cr->stages[(size_t)i * cr->T + t].nodes : sc[i];
+}
+
+// The substituted instance of scenario / chain i at stage t.  A chain stage's node_removed is written in the device
+// code into `code` (NR_OUTSIDE for the ids below n_nodes that its node_in_all leaves out), and from stage 2 on the
+// non-model counts of iteration 1 are those of the later iterations: the assigned partitions' prevMap entries are
+// the previous stage's next rows, which hold model states only.
+static blance_plan_in stage_in(const blance_plan_in& base, const blance_scenario* sc, const blance_scenario_opts* opts,
+                               const ChainReq* cr, int i, int t, std::vector<uint8_t>& code) {
+  blance_plan_in in = scenario_in(base, nodes_of(sc, cr, i, t), opts_of(opts, i));
+  if (!cr) return in;
+  const blance_chain_stage& st = cr->stages[(size_t)i * cr->T + t];
+  code.assign((size_t)std::max(1, base.n_node_ids), 0);
+  for (int q = 0; q < base.n_node_ids; ++q)
+    code[(size_t)q] = (uint8_t)((st.nodes.node_removed[q] ? NR_REMOVE : 0) | (q < base.n_nodes && !st.node_in_all[q] ? NR_OUTSIDE : 0));
+  in.node_removed = code.data();
+  if (t > 0) in.extra_tot_first = in.extra_tot_rest;
+  return in;
+}
+
+// Uploads the node tables (node flags, weights, non-model counts, hierarchy masks) of the wave's instances `ins`
+// into pl's pool.
+static void upload_nodes(blance_ctx* ctx, blance_plan* pl, const std::vector<blance_plan_in>& ins, bool coded) {
+  cudaStream_t st = ctx->stream;
+  DPool& P = pl->pool;
+  const size_t NT = (size_t)pl->NT, NUT = (size_t)pl->NUT, MT = (size_t)pl->MT;
+  std::vector<uint8_t> rm(NUT + 1, 0), ad(NUT + 1, 0), hw(NT + 1, 0);
+  std::vector<int32_t> nwt(NT + 1, 0), ef(NT + 1, 0), er(NT + 1, 0);
+  std::vector<uint32_t> mask(MT + 1, 0);
+  const NodeTables t{rm.data(), ad.data(), hw.data(), nwt.data(), ef.data(), er.data(), mask.data()};
+  for (size_t j = 0; j < ins.size(); ++j) stage_nodes(ins[j], pl->h_insts[j], t, coded);
+  CUDA(cudaMemcpyAsync((void*)P.node_removed, rm.data(), NUT + 1, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.node_added, ad.data(), NUT + 1, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.node_has_weight, hw.data(), NT + 1, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.node_weight, nwt.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.extra_first, ef.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.extra_rest, er.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemcpyAsync((void*)P.ie_mask, mask.data(), sizeof(uint32_t) * (MT + 1), cudaMemcpyHostToDevice, st));
+  CUDA(cudaStreamSynchronize(st));          // the host vectors die here
+}
+
+// Scenario summaries (node_ops | state_node_load | 3 scalars per instance, `stride` int64 words) of the wave's plans
+// from the beg rows / flags `prev_rows` / `pflags` to the working rows.
+static void wave_summary(blance_ctx* ctx, blance_plan* pl, int nw, const int32_t* prev_rows, const uint8_t* pflags, int favor_min,
+                         long long stride, long long* d_sum) {
+  const DInst& D0 = pl->h_insts[0];
+  const int PU = D0.PU, NU = D0.NU, S = D0.S;
+  CUDA(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), ctx->stream));
+  if (PU <= 0) return;
+  const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
+  const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
+  const dim3 grid((unsigned)bx, (unsigned)nw);
+  if (smem <= 48 * 1024) launch(ctx, k_scenario_summary<true>, grid, 256, smem, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
+  else launch(ctx, k_scenario_summary<false>, grid, 256, 0, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
+}
+
+// Plans the scenarios idx (of sc / opts) on one device, in waves.  With cr each is a chain of cr->T stages, planned
+// in lock step: a stage boundary is an iteration boundary plus the next stage's node tables (DESIGN.md section 12).
 static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
                                 const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
-                                const SchedReq* sr, const AuditReq* ar) {
+                                const SchedReq* sr, const AuditReq* ar, const ChainReq* cr = nullptr) {
   cudaStream_t st = ctx->stream;
   const int n_dev = (int)idx.size();
-  const blance_plan_in in0 = scenario_in(*base, sc[idx[0]], opts_of(opts, idx[0]));
+  const int T = cr ? cr->T : 1;
+  const bool coded = cr != nullptr;
+  std::vector<uint8_t> code0;
+  const blance_plan_in in0 = stage_in(*base, sc, opts, cr, idx[0], 0, code0);
   long long max_mask = 0;
   int max_ow = 0, max_rules = 0;
   bool audit_flags = false;            // any caller wants the per-partition flags
   for (int i : idx) {
-    const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
+    const blance_plan_in in = scenario_in(*base, nodes_of(sc, cr, i, 0), opts_of(opts, i));
     max_mask = std::max(max_mask, mask_words(in));
     max_ow = std::max(max_ow, n_overrides(opts_of(opts, i)));
     max_rules = std::max(max_rules, in.has_hier_rules ? in.n_rules : 0);
     audit_flags |= ar && ar->out[i].part_flags;
   }
-  size_t audit_bytes = 0;              // one scenario's audit buffers, priced into the wave
+  size_t extra_bytes = 0;              // one scenario's audit buffers / one chain's net buffers, priced into the wave
   if (ar) {
     Arena one;
     AuditBufs b;
     audit_slices(one, b, *ar, 1, base->n_states, max_rules, base->n_node_ids, base->n_nodes, base->n_parts, audit_flags);
-    audit_bytes = one.bytes();
+    extra_bytes = one.bytes();
   }
   {
     cudaMemPool_t pool;                // measure free memory without this context's cached arenas
@@ -1497,25 +1587,37 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     }
   }
   // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
-  const PlanPtr pb = upload(ctx, 1, &in0);
+  const PlanPtr pb = upload(ctx, 1, &in0, coded);
+  const long long stride = summary_stride(*base);
+  const bool want_net = cr && cr->net;
+  if (want_net) {                      // the base's prev rows and flags, kept for the net summary, and its result
+    Arena one;
+    int32_t* r = nullptr;
+    uint8_t* f = nullptr;
+    long long* d = nullptr;
+    one.add(r, (size_t)pb->RT + 4); one.add(f, (size_t)pb->PT + 1); one.add(d, (size_t)stride);
+    extra_bytes += one.bytes();
+  }
   size_t per = 0;
-  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, audit_bytes, &per);
+  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, extra_bytes, &per);
   if (W < 1)
     throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
   const bool auto_wave = max_concurrent <= 0;
   const bool times = getenv("BLANCE_SCENARIO_TIMES") != nullptr;
-  const long long stride = summary_stride(*base);
   const int PU = base->n_parts, NU = base->n_node_ids, S = base->n_states;
+  int n_prev_later = 0;                // len(prevMap) from stage 2 on: the base's prevMap plus every assigned partition
+  for (int p = 0; cr && p < PU; ++p) n_prev_later += (base->part_in_prev[p] || base->part_in_assign[p]) ? 1 : 0;
   for (int w0 = 0; w0 < n_dev;) {
     const int nw = std::min(W, n_dev - w0);
     std::vector<blance_plan_in> ins((size_t)nw);
-    for (int j = 0; j < nw; ++j) ins[(size_t)j] = scenario_in(*base, sc[idx[(size_t)(w0 + j)]], opts_of(opts, idx[(size_t)(w0 + j)]));
+    std::vector<std::vector<uint8_t>> code((size_t)nw);
+    for (int j = 0; j < nw; ++j) ins[(size_t)j] = stage_in(*base, sc, opts, cr, idx[(size_t)(w0 + j)], 0, code[(size_t)j]);
     // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
     const bool lone = n_dev == 1;
     blance_plan wave_plan;
     blance_plan* pl = lone ? pb.get() : &wave_plan;
     std::vector<int> seg_off;
-    if (!lone) layout(pl, nw, ins.data(), seg_off);
+    if (!lone) layout(pl, nw, ins.data(), seg_off, coded);
     if (!lone && pl->PT >= (1LL << 29)) {
       if (nw > 1) { W = nw / 2; continue; }
       throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
@@ -1530,7 +1632,8 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
           ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
       }
     // one allocation per wave, so that a plan is never lost for want of its summaries or schedule state: the
-    // wave's plan (lone: the base upload is the plan), the summaries, the schedule state, the weight overrides
+    // wave's plan (lone: the base upload is the plan), the summaries, the schedule state, the weight overrides,
+    // the chains' net buffers
     Arena wave;
     if (!lone) plan_slices(wave, pl, nw);
     long long* d_sum = nullptr;
@@ -1543,6 +1646,10 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     if (!ow.empty()) wave.add(d_ow, ow.size());
     AuditBufs abuf;
     if (ar) audit_slices(wave, abuf, *ar, nw, S, max_rules, NU, base->n_nodes, PU, audit_flags);
+    int32_t* net_prev = nullptr;
+    uint8_t* net_flags = nullptr;
+    long long* d_net = nullptr;
+    if (want_net) { wave.add(net_prev, (size_t)pl->RT + 4); wave.add(net_flags, (size_t)pl->PT + 1); wave.add(d_net, (size_t)(stride * nw)); }
     try {
       wave.alloc(st, "a scenario wave");
     } catch (const Error&) {
@@ -1552,19 +1659,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     DPool& P = pl->pool;
     // the node tables of the wave's scenarios (small host copies); the hierarchy masks and extra counts of the base
     if (!lone) {
-      const size_t NT = (size_t)pl->NT, NUT = (size_t)pl->NUT, MT = (size_t)pl->MT;
-      std::vector<uint8_t> rm(NUT + 1, 0), ad(NUT + 1, 0), hw(NT + 1, 0);
-      std::vector<int32_t> nwt(NT + 1, 0), ef(NT + 1, 0), er(NT + 1, 0);
-      std::vector<uint32_t> mask(MT + 1, 0);
-      const NodeTables t{rm.data(), ad.data(), hw.data(), nwt.data(), ef.data(), er.data(), mask.data()};
-      for (int j = 0; j < nw; ++j) stage_nodes(ins[(size_t)j], pl->h_insts[(size_t)j], t);
-      CUDA(cudaMemcpyAsync((void*)P.node_removed, rm.data(), NUT + 1, cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.node_added, ad.data(), NUT + 1, cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.node_has_weight, hw.data(), NT + 1, cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.node_weight, nwt.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.extra_first, ef.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.extra_rest, er.data(), sizeof(int32_t) * (NT + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync((void*)P.ie_mask, mask.data(), sizeof(uint32_t) * (MT + 1), cudaMemcpyHostToDevice, st));
+      upload_nodes(ctx, pl, ins, coded);
       CUDA(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
       CUDA(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
       CUDA(cudaMemcpyAsync(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
@@ -1580,104 +1675,150 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
       CUDA(cudaMemcpyAsync(d_ow, ow.data(), sizeof(int32_t) * ow.size(), cudaMemcpyHostToDevice, st));
       launch(ctx, k_scenario_weights, grid_for(ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, d_ow, k);
     }
+    if (want_net && pl->PT > 0) {      // the stage boundary overwrites these (in the lone path, the base upload's own)
+      CUDA(cudaMemcpyAsync(net_prev, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+      CUDA(cudaMemcpyAsync(net_flags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    }
     if (!lone) finish_upload(ctx, pl);
-    CUDA(cudaEventRecord(ctx->ev[0], st));
-    run(ctx, pl);
-    // summaries, then the requested rows
-    float sum_ms = 0.f, sched_ms = 0.f;
-    CUDA(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), st));
-    CUDA(cudaEventRecord(ctx->ev[1], st));
-    if (PU > 0) {
-      const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
-      const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
-      const dim3 grid((unsigned)bx, (unsigned)nw);
-      if (smem <= 48 * 1024) launch(ctx, k_scenario_summary<true>, grid, 256, smem, P, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
-      else launch(ctx, k_scenario_summary<false>, grid, 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
-    }
-    CUDA(cudaEventRecord(ctx->ev[2], st));
-    // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
-    std::vector<AuditInst> a_insts;
-    std::vector<std::vector<long long>> a_host((size_t)(ar ? nw : 0));
-    if (ar) {
-      for (int j = 0; j < nw; ++j) {
-        const DInst& D = pl->h_insts[(size_t)j];
-        AuditInst A = audit_inst(D);
-        A.rows = P.rows + D.rows_off; A.alt_rows = pl->prev_rows_init + D.rows_off;
-        A.meta = P.pmeta + D.part_off; A.alt_meta = pl->prev_meta_init + D.part_off;
-        A.pflags = pl->pflags_init + D.part_off;
-        A.ie_mask = P.ie_mask + D.mask_off;
-        A.stride = D.SLP;
-        a_insts.push_back(A);
+    for (int t = 0; t < T; ++t) {
+      if (t > 0) {
+        // the stage boundary: what the convergence loop left in the working state is the next stage's input - the
+        // assigned partitions' prev and cur rows are their next rows, committed by k_commit (or equal to them when the
+        // stage converged) with their flags - then the next stage's node tables and a fresh loop state
+        if (pl->PT > 0) {
+          CUDA(cudaMemcpyAsync(pl->rows_init, P.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+          CUDA(cudaMemcpyAsync(pl->prev_rows_init, P.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+          CUDA(cudaMemcpyAsync(pl->pmeta_init, P.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+          CUDA(cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+          CUDA(cudaMemcpyAsync(pl->pflags_init, P.pflags, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+        }
+        for (int j = 0; j < nw; ++j) {
+          ins[(size_t)j] = stage_in(*base, sc, opts, cr, idx[(size_t)(w0 + j)], t, code[(size_t)j]);
+          node_state(pl->h_insts[(size_t)j], ins[(size_t)j], coded, n_prev_later);
+        }
+        upload_nodes(ctx, pl, ins, coded);
       }
-      audit_run(ctx, abuf, *ar, a_insts);
-      for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
-    }
-    bool any_rows = false;
-    for (int j = 0; j < nw; ++j) {
-      const blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-      any_rows |= o.next_rows || o.next_shape || o.warn;
-    }
-    if (any_rows && pl->PT > 0)
-      launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
-             pl->d_raw_shape_off, pl->PT);
-    std::vector<long long> h_sum((size_t)(stride * nw));
-    std::vector<DInst> fin((size_t)nw);
-    CUDA(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st));
-    CUDA(cudaMemcpyAsync(fin.data(), P.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st));
-    for (int j = 0; j < nw; ++j) {
-      blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-      const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
-      if (rr && o.next_rows) CUDA(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st));
-      if (rs && o.next_shape) CUDA(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
-      if (rs && o.warn) CUDA(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
-    }
-    CUDA(cudaStreamSynchronize(st));
-    cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
-    for (int j = 0; j < nw; ++j) {
-      if (fin[(size_t)j].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
-      blance_scenario_out& o = out[idx[(size_t)(w0 + j)]];
-      const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
-      if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
-      if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
-      o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
-      o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
-      o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
-      if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
-    }
-    if (sr) {
-      CUDA(cudaEventRecord(ctx->ev[3], st));
-      if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, wsch);
-      std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
-      for (size_t x = 0; x < ops.size(); ++x) {
-        const long long* s = h_sum.data() + (x / NU) * stride + 4 * (x % NU);
-        ops[x] = s[0] + s[1] + s[2] + s[3];
-      }
-      const std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
-      for (long long i = 0; i < (long long)nw * sr->nc; ++i) {
-        blance_scenario_schedule_out& o = sr->out[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
-        o.rounds = (int32_t)scal[(size_t)(4 * i)];
-        o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
-        o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
-        o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
-        if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-        if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-        if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
-      }
+      CUDA(cudaEventRecord(ctx->ev[0], st));
+      run(ctx, pl);
+      // summaries, then the requested rows
+      float sum_ms = 0.f, sched_ms = 0.f;
       CUDA(cudaEventRecord(ctx->ev[1], st));
-      CUDA(cudaEventSynchronize(ctx->ev[1]));
-      cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
+      wave_summary(ctx, pl, nw, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
+      if (want_net && t == T - 1) wave_summary(ctx, pl, nw, net_prev, net_flags, favor_min, stride, d_net);
+      CUDA(cudaEventRecord(ctx->ev[2], st));
+      // the output of wave member j at this stage
+      auto out_of = [&](int j) -> blance_scenario_out& { return out[(size_t)idx[(size_t)(w0 + j)] * T + t]; };
+      // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
+      std::vector<AuditInst> a_insts;
+      std::vector<std::vector<long long>> a_host((size_t)(ar ? nw : 0));
+      if (ar) {
+        for (int j = 0; j < nw; ++j) {
+          const DInst& D = pl->h_insts[(size_t)j];
+          AuditInst A = audit_inst(D);
+          A.rows = P.rows + D.rows_off; A.alt_rows = pl->prev_rows_init + D.rows_off;
+          A.meta = P.pmeta + D.part_off; A.alt_meta = pl->prev_meta_init + D.part_off;
+          A.pflags = pl->pflags_init + D.part_off;
+          A.ie_mask = P.ie_mask + D.mask_off;
+          A.stride = D.SLP;
+          a_insts.push_back(A);
+        }
+        audit_run(ctx, abuf, *ar, a_insts);
+        for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
+      }
+      bool any_rows = false;
+      for (int j = 0; j < nw; ++j) {
+        const blance_scenario_out& o = out_of(j);
+        any_rows |= o.next_rows || o.next_shape || o.warn;
+      }
+      if (any_rows && pl->PT > 0)
+        launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
+               pl->d_raw_shape_off, pl->PT);
+      std::vector<long long> h_sum((size_t)(stride * nw));
+      std::vector<DInst> fin((size_t)nw);
+      CUDA(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st));
+      CUDA(cudaMemcpyAsync(fin.data(), P.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st));
+      for (int j = 0; j < nw; ++j) {
+        blance_scenario_out& o = out_of(j);
+        const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
+        if (rr && o.next_rows) CUDA(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st));
+        if (rs && o.next_shape) CUDA(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+        if (rs && o.warn) CUDA(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+      }
+      CUDA(cudaStreamSynchronize(st));
+      cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
+      for (int j = 0; j < nw; ++j) {
+        if (fin[(size_t)j].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
+        blance_scenario_out& o = out_of(j);
+        const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
+        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
+        if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
+        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
+        o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
+        o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
+        if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
+      }
+      if (sr) {
+        CUDA(cudaEventRecord(ctx->ev[3], st));
+        if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, wsch);
+        std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
+        for (size_t x = 0; x < ops.size(); ++x) {
+          const long long* s = h_sum.data() + (x / NU) * stride + 4 * (x % NU);
+          ops[x] = s[0] + s[1] + s[2] + s[3];
+        }
+        const std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
+        for (long long i = 0; i < (long long)nw * sr->nc; ++i) {
+          blance_scenario_schedule_out& o = sr->out[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
+          o.rounds = (int32_t)scal[(size_t)(4 * i)];
+          o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
+          o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
+          o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
+          if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+          if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+          if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
+        }
+        CUDA(cudaEventRecord(ctx->ev[1], st));
+        CUDA(cudaEventSynchronize(ctx->ev[1]));
+        cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
+      }
+      if (times) {
+        float wave_ms = 0.f;
+        cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
+        std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
+                     w0, nw, W, per, wave_ms, sum_ms);
+        if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
+        std::fprintf(stderr, "\n");
+      }
     }
-    if (times) {
-      float wave_ms = 0.f;
-      cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
-      std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
-                   w0, nw, W, per, wave_ms, sum_ms);
-      if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
-      std::fprintf(stderr, "\n");
+    if (want_net) {
+      std::vector<long long> h_net((size_t)(stride * nw));
+      CUDA(cudaMemcpyAsync(h_net.data(), d_net, sizeof(long long) * h_net.size(), cudaMemcpyDeviceToHost, st));
+      CUDA(cudaStreamSynchronize(st));
+      for (int j = 0; j < nw; ++j) {
+        blance_chain_out& o = cr->net[idx[(size_t)(w0 + j)]];
+        const long long* s = h_net.data() + (size_t)j * (size_t)stride;
+        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
+        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2];
+      }
     }
     w0 += nw;
   }
   cudaStreamSynchronize(st);
+}
+
+// The checks of one scenario's substituted instance (base_sum: see check_counts).  Returns a status, `why` the reason.
+static int check_scenario(const blance_plan_in& base, const blance_scenario& sc, const blance_scenario_opts* o, long long& base_sum,
+                          std::string& why) {
+  int st = BLANCE_OK;
+  if (sc.add_is_nil != 0 && sc.add_is_nil != 1) why = "add_is_nil is neither 0 nor 1";
+  else if (sc.has_node_weights != 0 && sc.has_node_weights != 1) why = "has_node_weights is neither 0 nor 1";
+  else {
+    const blance_plan_in in = scenario_in(base, sc, o);
+    st = check_structure(&in, why);
+    if (st == BLANCE_OK && o) st = check_opts(base, *o, why);
+    if (st == BLANCE_OK) st = check_counts(base, in, o, base_sum, why);
+  }
+  if (st == BLANCE_OK && !why.empty()) st = BLANCE_ERR_INVALID_ARG;
+  return st;
 }
 
 static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
@@ -1689,17 +1830,7 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
   long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
   for (int i = 0; i < n; ++i) {
     std::string why;
-    int st = BLANCE_OK;
-    const blance_scenario_opts* o = opts_of(opts, i);
-    if (sc[i].add_is_nil != 0 && sc[i].add_is_nil != 1) why = "add_is_nil is neither 0 nor 1";
-    else if (sc[i].has_node_weights != 0 && sc[i].has_node_weights != 1) why = "has_node_weights is neither 0 nor 1";
-    else {
-      const blance_plan_in in = scenario_in(*base, sc[i], o);
-      st = check_structure(&in, why);
-      if (st == BLANCE_OK && o) st = check_opts(*base, *o, why);
-      if (st == BLANCE_OK) st = check_counts(*base, in, o, base_sum, why);
-    }
-    if (st == BLANCE_OK && !why.empty()) st = BLANCE_ERR_INVALID_ARG;
+    const int st = check_scenario(*base, sc[i], opts_of(opts, i), base_sum, why);
     if (st != BLANCE_OK) throw_err(st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
   }
   if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
@@ -1709,6 +1840,48 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
   fan_out(ctx, G, [&](int d, blance_ctx* dev) {
     scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr, ar);
+  });
+}
+
+// Chains of stages over one base (blance_plan_chains): chain i -> device i mod G, its stages planned in lock step
+// with the other chains of its wave.
+static void plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
+                        const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
+                        blance_chain_out* net) {
+  const std::string name = "blance_plan_chains";
+  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
+  if (n_stages < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_stages must be positive");
+  if (!base || !stages || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
+  if (n_stages > 1 && base->max_iters < 1)      // the stage would assign nothing and leave no next map to plan on
+    throw_err(BLANCE_ERR_INVALID_ARG, name + ": a chain of several stages needs max_iters >= 1");
+  // every stage is checked before the context is used, so a NULL ctx checks the chains without a device
+  long long base_sum = -1;
+  for (int i = 0; i < n; ++i)
+    for (int t = 0; t < n_stages; ++t) {
+      const blance_chain_stage& cs = stages[(size_t)i * n_stages + t];
+      std::string why;
+      int st = check_scenario(*base, cs.nodes, opts_of(opts, i), base_sum, why);
+      if (st == BLANCE_OK && base->n_nodes > 0 && !cs.node_in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
+      for (int q = 0; st == BLANCE_OK && q < base->n_nodes; ++q)
+        if (cs.node_in_all[q] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
+      if (st != BLANCE_OK) throw_err(st, name + ": chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": " + why);
+    }
+  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+  ChainReq cr;
+  cr.T = n_stages; cr.stages = stages; cr.net = net;
+  const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
+  std::vector<std::vector<int>> idx((size_t)G);
+  for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
+  fan_out(ctx, G, [&](int d, blance_ctx* dev) {
+    scenarios_on_device(dev, base, idx[(size_t)d], nullptr, opts, favor_min_nodes, max_concurrent, out, nullptr, nullptr, &cr);
+  });
+}
+
+extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                  const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
+                                  int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
+  return entry(ctx, [&](Device&) {
+    plan_chains(ctx, base, n, n_stages, stages, opts, favor_min_nodes, max_concurrent, out, net);
   });
 }
 

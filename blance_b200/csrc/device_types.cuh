@@ -30,6 +30,11 @@
 #define BL_PICK_MAX 32    // hierarchy picks per step (rules x constraints)
 #define BL_RING 8         // step-record ring depth in shared memory (records i .. i+3 live, i+4 in flight)
 
+// node_removed on the device: bit 0 = in nodesToRemove, bit 1 = outside this plan's nodesAll (a chain stage's
+// membership mask, blance_plan_chains).  Candidate tests read "!= 0"; the strip of plan.go:83-88 and the bucket-0
+// test of plan.go:544 read bit 0 only.  A caller's table is normalised to 0 / 1 when it is staged.
+enum : uint8_t { NR_REMOVE = 1, NR_OUTSIDE = 2 };
+
 enum : uint8_t { PF_IN_PREV = 1, PF_IN_ASSIGN = 2, PF_HAS_WEIGHT = 4,
                  PF_PREV_EXTRA = 8 };   // the prevMap entry has keys outside the model (until plan.go:49-52 replaces it)
 
@@ -71,6 +76,7 @@ struct DInst {
   long long spec_round2;   // resolves that had to look at the second list column
   long long spec_cwait;    // resolves that had to wait for the committer (a pending commit shared their top node)
   long long spec_why[4];   // team evaluations by cause: row not clean | current node dead | candidates ran out | bound test failed
+  int32_t masked;          // some node id below N is outside nodesAll (NR_OUTSIDE): such a current node makes a row unclean
 };
 
 struct DPool {

@@ -1009,10 +1009,11 @@ struct PartIndex {
   }
 };
 
+// who: "scenario i: " / "chain i, stage t: ".  check_prev: reject a removal with assigned partitions absent from
+// prevMap (plan.go:544); a chain's later stages plan on a prevMap that holds every assigned partition.
 ScenarioTables scenario_tables(const InternedPlan& ip, const PartitionModel& model, const Scenario& sc,
-                               const PlanNextMapOptions& options, size_t index, PartIndex& parts) {
-  const std::string who = "scenario " + std::to_string(index) + ": ";
-  check_remove_needs_prev(ip, sc.NodesToRemove, who);
+                               const PlanNextMapOptions& options, const std::string& who, PartIndex& parts, bool check_prev = true) {
+  if (check_prev) check_remove_needs_prev(ip, sc.NodesToRemove, who);
   const int32_t N = ip.in.n_nodes, NU = ip.in.n_node_ids, S = ip.in.n_states;
   std::unordered_map<std::string, int32_t> id;
   id.reserve(size_t(NU));
@@ -1225,7 +1226,7 @@ std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const 
   if (index >= scenarios.size()) invalid("InternScenario: scenario index out of range");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
   PartIndex parts{*ip, {}};
-  ScenarioTables t = scenario_tables(*ip, model, scenarios[index], options, index, parts);
+  ScenarioTables t = scenario_tables(*ip, model, scenarios[index], options, "scenario " + std::to_string(index) + ": ", parts);
   ip->node_removed = std::move(t.removed);
   ip->node_added = std::move(t.added);
   ip->node_weight = std::move(t.weight);
@@ -1264,6 +1265,41 @@ std::unique_ptr<InternedPlan> InternScenario(const PartitionMap& prevMap, const 
   return ip;
 }
 
+namespace {
+
+const char* const kOpNames[] = {"add", "del", "promote", "demote"};   // enum blance_op_kind
+
+// node_ops [NU][4] by node and op name, nonzero entries only
+std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> node_ops_by_name(const InternedPlan& ip, const int64_t* ops) {
+  std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> r;
+  for (int32_t q = 0; q < ip.in.n_node_ids; ++q)
+    for (int k = 0; k < 4; ++k)
+      if (ops[size_t(q) * 4 + size_t(k)]) r[ip.node_names[size_t(q)]][kOpNames[k]] = ops[size_t(q) * 4 + size_t(k)];
+  return r;
+}
+
+// One blance_scenario_out by name; `map` (rows copied out, or NULL) is uninterned under the constraints k.
+ScenarioResult scenario_result(const InternedPlan& ip, const blance_scenario_out& o, const std::vector<int64_t>& ops,
+                               const std::vector<int64_t>& load, PlanOutBuffers* map, const int32_t* k) {
+  const int32_t NU = ip.in.n_node_ids, S = ip.in.n_states;
+  ScenarioResult r;
+  r.iters_run = o.iters_run; r.converged = o.converged; r.steps = o.steps; r.sticky_steps = o.sticky_steps;
+  r.parts_moved = o.parts_moved; r.ops_total = o.ops_total; r.warn_parts = o.warn_parts;
+  r.NodeOps = node_ops_by_name(ip, ops.data());
+  for (int32_t s = 0; s < S; ++s)
+    for (int32_t q = 0; q < NU; ++q)
+      if (load[size_t(s) * size_t(NU) + size_t(q)])
+        r.StateNodeLoad[ip.state_names[size_t(s)]][ip.node_names[size_t(q)]] = load[size_t(s) * size_t(NU) + size_t(q)];
+  if (map) {
+    r.HasMap = true;
+    map->out.iters_run = o.iters_run;
+    if (o.iters_run > 0) r.NextMap = unintern_plan(ip, *map, &r.NextWarnings, k);   // MaxIterationsPerPlan <= 0: plan.go:32,57
+  }
+  return r;
+}
+
+}  // namespace
+
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
@@ -1274,7 +1310,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
   const size_t n = scenarios.size();
   PartIndex parts{*ip, {}};
   std::vector<ScenarioTables> tabs(n);
-  for (size_t i = 0; i < n; ++i) tabs[i] = scenario_tables(*ip, model, scenarios[i], options, i, parts);
+  for (size_t i = 0; i < n; ++i) tabs[i] = scenario_tables(*ip, model, scenarios[i], options, "scenario " + std::to_string(i) + ": ", parts);
   std::vector<bool> want(n, false);
   for (int i : wantMaps) {
     if (i < 0 || size_t(i) >= n) invalid("PlanNextMapScenarios: wantMaps index " + std::to_string(i) + " out of range");
@@ -1334,26 +1370,11 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
                     : blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                out.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_scenarios failed: ") + blance_last_error(ctx));
-  static const char* kOps[] = {"add", "del", "promote", "demote"};
   std::vector<ScenarioResult> res(n);
   for (size_t i = 0; i < n; ++i) {
     ScenarioResult& r = res[i];
-    const blance_scenario_out& o = out[i];
-    r.iters_run = o.iters_run; r.converged = o.converged; r.steps = o.steps; r.sticky_steps = o.sticky_steps;
-    r.parts_moved = o.parts_moved; r.ops_total = o.ops_total; r.warn_parts = o.warn_parts;
-    for (int32_t q = 0; q < NU; ++q)
-      for (int k = 0; k < 4; ++k)
-        if (ops[i][size_t(q) * 4 + size_t(k)]) r.NodeOps[ip->node_names[size_t(q)]][kOps[k]] = ops[i][size_t(q) * 4 + size_t(k)];
-    for (int32_t s = 0; s < S; ++s)
-      for (int32_t q = 0; q < NU; ++q)
-        if (load[i][size_t(s) * size_t(NU) + size_t(q)])
-          r.StateNodeLoad[ip->state_names[size_t(s)]][ip->node_names[size_t(q)]] = load[i][size_t(s) * size_t(NU) + size_t(q)];
-    if (want[i]) {
-      r.HasMap = true;
-      maps[i]->out.iters_run = o.iters_run;
-      const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
-      if (o.iters_run > 0) r.NextMap = unintern_plan(*ip, *maps[i], &r.NextWarnings, k);   // MaxIterationsPerPlan <= 0: plan.go:32,57
-    }
+    const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
+    r = scenario_result(*ip, out[i], ops[i], load[i], want[i] ? maps[i].get() : nullptr, k);
     for (size_t k = 0; k < nc; ++k) {
       const blance_scenario_schedule_out& so = sched[i * nc + k];
       ScenarioSchedule s;
@@ -1369,6 +1390,105 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
       abuf[i]->out = aout[i];
       r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[i], audit->FailoverSpread);
     }
+  }
+  return res;
+}
+
+std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                           const Strs& nodesAll, const PartitionModel& model,
+                                           const PlanNextMapOptions& options, const std::vector<Chain>& chains,
+                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent) {
+  if (chains.empty()) invalid("PlanNextMapChains: no chains");
+  const size_t n = chains.size(), T = chains[0].Stages.size();
+  if (T == 0) invalid("PlanNextMapChains: chain 0 has no stages");
+  for (size_t i = 0; i < n; ++i)
+    if (chains[i].Stages.size() != T)
+      invalid("PlanNextMapChains: chain " + std::to_string(i) + " has " + std::to_string(chains[i].Stages.size()) +
+              " stages, chain 0 has " + std::to_string(T) + " (chains of different lengths go in separate calls)");
+  // every stage as a scenario: its node sets and weights, the chain's option fields
+  std::vector<Scenario> flat(n * T);
+  for (size_t i = 0; i < n; ++i)
+    for (size_t t = 0; t < T; ++t) {
+      const ChainStage& cs = chains[i].Stages[t];
+      Scenario& sc = flat[i * T + t];
+      sc = chains[i].Options;
+      sc.NodesToRemove = cs.NodesToRemove;
+      sc.NodesToAdd = cs.NodesToAdd;
+      if (cs.NodeWeights) sc.NodeWeights = cs.NodeWeights;
+    }
+  auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, flat);
+  const int32_t N = ip->in.n_nodes, NU = ip->in.n_node_ids, S = ip->in.n_states;
+  std::unordered_map<std::string, int32_t> universe;
+  for (int32_t q = 0; q < N; ++q) universe.emplace(ip->node_names[size_t(q)], q);
+  PartIndex parts{*ip, {}};
+  std::vector<ScenarioTables> tabs(n * T);
+  std::vector<std::vector<uint8_t>> member(n * T);
+  for (size_t i = 0; i < n; ++i)
+    for (size_t t = 0; t < T; ++t) {
+      const std::string who = "chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": ";
+      tabs[i * T + t] = scenario_tables(*ip, model, flat[i * T + t], options, who, parts, t == 0);
+      const ChainStage& cs = chains[i].Stages[t];
+      std::vector<uint8_t>& m = member[i * T + t];
+      m.assign(size_t(N) + 1, 0);
+      if (cs.NodesAll) {
+        for (const auto& name : *cs.NodesAll) {
+          auto it = universe.find(name);
+          if (it == universe.end()) throw BlanceError(BLANCE_ERR_INVALID_ARG, "blance: " + who + "NodesAll name '" + name + "' is not in nodesAll");
+          m[size_t(it->second)] = 1;
+        }
+      } else if (t == 0) {
+        std::fill(m.begin(), m.begin() + N, uint8_t(1));
+      } else {                         // (previous members - previous NodesToRemove) U NodesToAdd
+        const std::vector<uint8_t>& pm = member[i * T + t - 1];
+        const ScenarioTables& pt = tabs[i * T + t - 1];
+        for (int32_t q = 0; q < N; ++q) m[size_t(q)] = (pm[size_t(q)] && !pt.removed[size_t(q)]) || tabs[i * T + t].added[size_t(q)];
+      }
+    }
+  std::vector<bool> want(n, false);
+  for (int i : wantMaps) {
+    if (i < 0 || size_t(i) >= n) invalid("PlanNextMapChains: wantMaps index " + std::to_string(i) + " out of range");
+    want[size_t(i)] = true;
+  }
+  std::vector<blance_chain_stage> stages(n * T);
+  std::vector<blance_scenario_opts> opts(n);
+  std::vector<blance_scenario_out> out(n * T);
+  std::vector<blance_chain_out> net(n);
+  std::vector<std::vector<int64_t>> ops(n * T, std::vector<int64_t>(size_t(NU) * 4 + 1)),
+      load(n * T, std::vector<int64_t>(size_t(S) * size_t(NU) + 1)), net_ops(n, std::vector<int64_t>(size_t(NU) * 4 + 1));
+  std::vector<std::unique_ptr<PlanOutBuffers>> maps(n * T);
+  for (size_t x = 0; x < n * T; ++x) {
+    const ScenarioTables& tb = tabs[x];
+    stages[x] = blance_chain_stage{blance_scenario{tb.removed.data(), tb.added.data(), tb.add_is_nil, tb.has_node_weights,
+                                                   tb.weight.data(), tb.has_weight.data()},
+                                   member[x].data()};
+    out[x] = blance_scenario_out{};
+    out[x].node_ops = ops[x].data();
+    out[x].state_node_load = load[x].data();
+    if (want[x / T]) {
+      maps[x] = std::make_unique<PlanOutBuffers>(*ip);
+      out[x].next_rows = maps[x]->next_rows.data();
+      out[x].next_shape = maps[x]->next_shape.data();
+      out[x].warn = maps[x]->warn.data();
+    }
+  }
+  for (size_t i = 0; i < n; ++i) {
+    opts[i] = scenario_opts(tabs[i * T]);     // the chain's option groups (its stages differ in node fields only)
+    net[i] = blance_chain_out{};
+    net[i].node_ops = net_ops[i].data();
+  }
+  blance_ctx* ctx = DefaultContext();
+  const int st = blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+                                    maxConcurrent, out.data(), net.data());
+  if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_chains failed: ") + blance_last_error(ctx));
+  std::vector<ChainResult> res(n);
+  for (size_t i = 0; i < n; ++i) {
+    const ScenarioTables& t0 = tabs[i * T];
+    const int32_t* k = (t0.set & BLANCE_OPT_CONSTRAINTS) ? t0.constraints.data() : ip->state_constraints.data();
+    for (size_t t = 0; t < T; ++t)
+      res[i].Stages.push_back(scenario_result(*ip, out[i * T + t], ops[i * T + t], load[i * T + t], maps[i * T + t].get(), k));
+    res[i].NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());
+    res[i].NetOpsTotal = net[i].ops_total;
+    res[i].NetPartsMoved = net[i].parts_moved;
   }
   return res;
 }

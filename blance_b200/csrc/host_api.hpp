@@ -180,6 +180,46 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
                                                  const std::vector<int>& scheduleConcurrency = {},
                                                  const ScenarioAudit* audit = nullptr);
 
+// ---- chains of cluster changes (blance_plan_chains) --------------------------------------------------------------
+struct ChainStage {
+  OptStrs NodesToRemove;               // nullopt = nil
+  OptStrs NodesToAdd;                  // nullopt = nil (plan.go:554)
+  ScenarioOpt<std::unordered_map<std::string, int>> NodeWeights;   // outer nullopt: the chain's / the options' value
+  // This stage's nodesAll, a subset of the universe (PlanNextMapChains' nodesAll); it is always used in universe order.
+  // nullopt: the previous stage's members minus its NodesToRemove, plus this stage's NodesToAdd that are in the
+  // universe; the first stage's default is the whole universe.
+  OptStrs NodesAll;
+};
+
+struct Chain {
+  // The plan options of every stage of the chain: the option fields of a Scenario (ModelStateConstraints,
+  // StateStickiness, PartitionWeights, NodeHierarchy, HierarchyRules, and NodeWeights unless a stage sets its own).
+  // Its NodesToRemove / NodesToAdd are not read.
+  Scenario Options;
+  std::vector<ChainStage> Stages;
+};
+
+struct ChainResult {
+  std::vector<ScenarioResult> Stages;  // one per stage, as PlanNextMapScenarios' results; "prev row" = that stage's prevMap
+  // CalcPartitionMoves from the base prevMap row (empty when absent) to the last stage's next row, every assigned
+  // partition: per node and op name (nonzero only), the total and the partitions with at least one op
+  std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> NetNodeOps;
+  int64_t NetOpsTotal = 0, NetPartsMoved = 0;
+};
+
+// Chain i is the Go loop of include/blance_b200.h over its stages: stage t is PlanNextMapEx(prev, assign, nodesAll_t,
+// NodesToRemove_t, NodesToAdd_t, model, options with chain i's option fields and stage t's NodeWeights), then prev =
+// prev with every entry of next replaced and assign = next.  nodesAll is the UNIVERSE: every stage's nodesAll is a
+// subset of it in its order, so a node that leaves and comes back keeps its position.  The caller's maps are NOT
+// mutated; they are interned once.  Every chain has the same number of stages (>= 1).  A stage the reference would
+// panic on (a removal in the first stage with assigned partitions absent from prevMap, plan.go:544), a NodesAll name
+// outside the universe or chains of different lengths throw BlanceError naming the chain and stage before any device
+// work.  Stage maps (NextMap / NextWarnings) are filled for the chains listed in wantMaps.
+std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
+                                           const Strs& nodesAll, const PartitionModel& model,
+                                           const PlanNextMapOptions& options, const std::vector<Chain>& chains,
+                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent);
+
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 
 // moves.go:41-46 for one partition (a batch of one on the device).

@@ -432,6 +432,67 @@ PYBIND11_MODULE(_host, m) {
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
       py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none());
 
+  // chains: per chain (its option fields as a scenario tuple - the node sets are not read -, its stages); per stage
+  // (nodes_to_remove, nodes_to_add, has_node_weights_key, node_weights, nodes_all or None for the default)
+  using PyStage = std::tuple<OptStrs, OptStrs, bool, std::optional<IntMap>, OptStrs>;
+  using PyChain = std::tuple<PyScenario, std::vector<PyStage>>;
+  m.def(
+      "PlanNextMapChains",
+      [to_scenarios](const PyPartitionMap& prev, const std::optional<PyPartitionMap>& assign, const Strs& nodes_all,
+                     const PyModel& model, const std::vector<PyChain>& chains, bool favor_min_nodes,
+                     const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
+                     const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
+                     const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
+                     int engine) {
+        PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
+        const PartitionMap prev_map = to_map(prev);
+        const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
+        std::vector<Chain> cs;
+        for (const auto& c : chains) {
+          Chain ch;
+          ch.Options = to_scenarios({std::get<0>(c)})[0];
+          for (const auto& st : std::get<1>(c)) {
+            ChainStage s;
+            s.NodesToRemove = std::get<0>(st);
+            s.NodesToAdd = std::get<1>(st);
+            if (std::get<2>(st)) s.NodeWeights = std::get<3>(st);
+            s.NodesAll = std::get<4>(st);
+            ch.Stages.push_back(std::move(s));
+          }
+          cs.push_back(std::move(ch));
+        }
+        std::vector<ChainResult> res;
+        {
+          py::gil_scoped_release rel;
+          res = PlanNextMapChains(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, cs, favor_min_nodes,
+                                  want_maps, max_concurrent);
+        }
+        py::list out;
+        for (const auto& c : res) {
+          py::list stages;
+          for (const auto& r : c.Stages) {
+            py::dict d;
+            d["iterations"] = r.iters_run; d["converged"] = r.converged; d["steps"] = r.steps;
+            d["sticky_steps"] = r.sticky_steps; d["parts_moved"] = r.parts_moved; d["ops_total"] = r.ops_total;
+            d["warn_parts"] = r.warn_parts; d["node_ops"] = r.NodeOps; d["state_node_load"] = r.StateNodeLoad;
+            if (r.HasMap) { d["next_map"] = from_map(r.NextMap); d["warnings"] = r.NextWarnings; }
+            stages.append(d);
+          }
+          py::dict net;
+          net["node_ops"] = c.NetNodeOps; net["ops_total"] = c.NetOpsTotal; net["parts_moved"] = c.NetPartsMoved;
+          py::dict d;
+          d["stages"] = stages;
+          d["net"] = net;
+          out.append(d);
+        }
+        return out;
+      },
+      py::arg("prev_map"), py::arg("partitions_to_assign"), py::arg("nodes_all"), py::arg("model"), py::arg("chains"),
+      py::arg("favor_min_nodes") = false, py::arg("want_maps") = std::vector<int>{}, py::arg("max_concurrent") = 0,
+      py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
+      py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
+      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+
   // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
   m.def(
       "intern_scenario",

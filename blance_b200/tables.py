@@ -133,6 +133,18 @@ class ScenarioResult:
     warn_parts = property(lambda self: self.out.warn_parts)
 
 
+class ChainNet:
+    """Output buffers of a blance_chain_out: the moves from a chain's base map to its last stage's map."""
+
+    def __init__(self, t):
+        self.node_ops = np.zeros((t.n_node_ids, 4), np.int64)
+        self.out = api.ChainOut()
+        self.out.node_ops = self.node_ops.ctypes.data if self.node_ops.size else None
+
+    ops_total = property(lambda self: self.out.ops_total)
+    parts_moved = property(lambda self: self.out.parts_moved)
+
+
 class ScenarioSchedule:
     """Output buffers of a blance_scenario_schedule_out: the schedule's summaries at one count."""
 
@@ -401,6 +413,48 @@ class Context:
         for r, o in zip(results, outs):
             r.out = o
         return results
+
+    def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True):
+        """blance_plan_chains: chains of cluster changes, each stage planned on the map the stage before produced.
+        chains is a list of chains of equal length; a stage is a dict of SCENARIO_FIELDS and node_in_all ([n_nodes],
+        missing = every node; missing scenario keys keep the base's value).  want_rows lists the (chain, stage) pairs
+        whose next rows, shapes and warnings are copied out.  opts: None, or one dict of OPT_GROUPS keys per chain.
+        Returns (results, nets): results[i][t] a ScenarioResult per stage, nets[i] a ChainNet (None without net)."""
+        n = len(chains)
+        T = len(chains[0]) if n else 0
+        if any(len(c) != T for c in chains):
+            raise ValueError("every chain of one call has the same number of stages")
+        want = set(want_rows)
+        base = base_tables.struct()
+        keep, sts = [], (api.ChainStage * max(1, n * T))()
+        for i, chain in enumerate(chains):
+            for t, stage in enumerate(chain):
+                st = sts[i * T + t]
+                sc = scenario_tables(base_tables, {k: v for k, v in stage.items() if k != "node_in_all"})
+                for f in SCENARIO_FIELDS:
+                    v = getattr(sc, f)
+                    if f in ("add_is_nil", "has_node_weights"):
+                        setattr(st.nodes, f, int(v))
+                        continue
+                    a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
+                    keep.append(a)
+                    setattr(st.nodes, f, a.ctypes.data if a.size else None)
+                m = np.ascontiguousarray(stage.get("node_in_all", np.ones(base_tables.n_nodes)), np.uint8)
+                keep.append(m)
+                st.node_in_all = m.ctypes.data if m.size else None
+        results = [[ScenarioResult(base_tables, (i, t) in want) for t in range(T)] for i in range(n)]
+        outs = (api.ScenarioOut * max(1, n * T))(*[r.out for rs in results for r in rs])
+        nets = [ChainNet(base_tables) for _ in range(n)] if net else None
+        net_arr = (api.ChainOut * max(1, n))(*[x.out for x in nets]) if net else None
+        ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
+        self._check(self.lib.blance_plan_chains(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
+                                                int(max_concurrent), outs, net_arr), "blance_plan_chains")
+        for i in range(n):
+            for t in range(T):
+                results[i][t].out = outs[i * T + t]
+            if net:
+                nets[i].out = net_arr[i]
+        return results, nets
 
     def prepare_batch(self, tables_list, results=None):
         """Builds the blance_plan_in / blance_plan_out arrays of a batch once; run_batch() is then only the

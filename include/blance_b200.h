@@ -106,7 +106,7 @@ typedef struct blance_plan_in {
   const uint8_t* state_has_stickiness;  /* key present */
 
   /* per node id, [n_node_ids] */
-  const uint8_t* node_removed;          /* in nodesToRemove */
+  const uint8_t* node_removed;          /* in nodesToRemove (any nonzero value means yes) */
   const uint8_t* node_added;            /* in nodesToAdd */
   /* per node, [n_nodes] */
   const int32_t* node_weight;           /* NodeWeights[n] */
@@ -304,6 +304,56 @@ typedef struct blance_scenario_opts {
 int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                              const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                              blance_scenario_out* out);
+
+/* ---- chains of cluster changes (blance_plan_chains) ---------------------------------------------------------
+ * A rolling upgrade, successive failures or repeated rebalances are SEQUENCES of plans, each on the map the one
+ * before produced.  Chain i has T = n_stages stages; stage t of chain i is the Go host loop
+ *
+ *     prev, assign := prevMap, partitionsToAssign              // the base's, never mutated
+ *     for t := 0; t < T; t++ {
+ *         next, warnings := PlanNextMapEx(prev, assign, nodesAll_t, nodesToRemove_t, nodesToAdd_t, model, options_i_t)
+ *         prev = prev with every entry of next replaced         // the stage's FINAL MAP
+ *         assign = next
+ *     }
+ *
+ * where nodesAll_t is the base's nodesAll IN BASE ORDER restricted to the ids q < n_nodes with node_in_all[q] = 1
+ * (a node that leaves and comes back keeps its position; ids >= n_nodes stay outside nodesAll), nodesToRemove_t /
+ * nodesToAdd_t / NodeWeights_t come from the stage's blance_scenario, and options_i_t is the base's options with
+ * chain i's opts groups substituted (as blance_plan_scenarios_ex) and NodeWeights_t.  In table terms stage t+1's
+ * instance is stage t's with, for every partition with part_in_assign, prev_rows = cur_rows = next_rows,
+ * prev_shape = cur_shape = next_shape and part_in_prev = 1 (bit 1 cleared); extra_tot_first = extra_tot_rest (a
+ * next row holds model states only: partitionsToAssign may not name other states); and the stage's node fields.
+ *
+ * out[i * n_stages + t] is a blance_scenario_out with exactly the meaning it has in blance_plan_scenarios, where the
+ * "prev row as passed in" is THAT STAGE's prevMap row.  With n_stages = 1 and every node_in_all set, out[i] equals
+ * blance_plan_scenarios_ex field for field.  net[i] (net may be NULL; its node_ops may be NULL) holds
+ * CalcPartitionMoves over the same states with the same favor_min_nodes from the BASE's prev row (empty when the
+ * partition is absent from prevMap) to the LAST stage's next row, for every assigned partition: node_ops, ops_total,
+ * parts_moved as in blance_scenario_out.  sum_t out[i * n_stages + t].ops_total - net[i].ops_total is what the
+ * sequence moves beyond one direct plan.  Nothing depends on n, max_concurrent, the engine or the number of devices.
+ * No schedules or audits per stage: blance_map_audit audits a copied-out row table.
+ *
+ * Errors, all before any device work: n <= 0, n_stages < 1, a NULL base / stages / out; n_stages > 1 with
+ * max_iters < 1 (a stage that plans nothing leaves no next map); a stage that blance_plan_scenarios_ex would reject,
+ * a NULL node_in_all, or a node_in_all entry that is neither 0 nor 1 - the message names "chain i, stage t".  With ctx
+ * NULL the call returns the first stage's error, or BLANCE_ERR_INVALID_ARG for the NULL ctx.  Scheduling as
+ * blance_plan_scenarios (chain i -> device i mod G); a wave's chains run stage by stage in lock step, the map never
+ * leaves the device between stages, and the net buffers are priced into the wave size (DESIGN.md section 12).
+ * The C++ twin over string maps is PlanNextMapChains (blance_b200/csrc/host_api.hpp). */
+typedef struct blance_chain_stage {
+  blance_scenario nodes;           /* the stage's nodesToRemove / nodesToAdd / NodeWeights, as a scenario */
+  const uint8_t* node_in_all;      /* [n_nodes] 1 = the node is in this stage's nodesAll, 0 = outside */
+} blance_chain_stage;
+
+typedef struct blance_chain_out {
+  int64_t* node_ops;               /* [n_node_ids][4] by enum blance_op_kind; may be NULL */
+  int64_t ops_total, parts_moved;
+} blance_chain_out;
+
+int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                       const blance_chain_stage* stages /* [n][n_stages] */, const blance_scenario_opts* opts /* [n] or NULL */,
+                       int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out /* [n][n_stages] */,
+                       blance_chain_out* net /* [n] or NULL */);
 
 /* ---- the rebalance schedule of every scenario (blance_plan_scenarios_schedule) --------------------------------
  * Summaries of the lock-step schedule of blance_moves_schedule (rules 1-5 below) of one scenario's moves at one
