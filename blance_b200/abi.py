@@ -93,11 +93,26 @@ class _AuditOut(ctypes.Structure):     # struct blance_audit_out
                 ("kernel_ms", ctypes.c_float)]
 
 
+EXPO_METRICS = ("NO_TOP", "MULTI_TOP", "SHORT", "ONE_COPY", "NO_COPY", "COPIES")   # enum blance_expo_metric order
+
+
+class _ExposureIn(ctypes.Structure):   # struct blance_exposure_in
+    _fields_ = [("state_constraints", ctypes.c_void_p), ("top_state", ctypes.c_int32), ("n_domains", ctypes.c_int32),
+                ("domain_parent", ctypes.c_void_p)]
+
+
+class _ExposureOut(ctypes.Structure):  # struct blance_exposure_out
+    _fields_ = [("rounds", ctypes.c_int32), ("series", ctypes.c_void_p), ("peak", ctypes.c_int64 * 6),
+                ("peak_round", ctypes.c_int32 * 6), ("area", ctypes.c_int64 * 6), ("dom_peak", ctypes.c_void_p),
+                ("dom_peak_round", ctypes.c_void_p), ("part_min_copies", ctypes.c_void_p), ("part_no_top", ctypes.c_void_p),
+                ("part_flags", ctypes.c_void_p), ("kernel_ms", ctypes.c_float)]
+
+
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
            "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_chains", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
-           "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_free")
+           "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_exposure", "blance_moves_free")
 
 
 def capi():
@@ -138,6 +153,7 @@ def capi():
         lib.blance_moves_available.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.blance_moves_schedule.argtypes = [vp, vp, i32, vp, vp]
         lib.blance_moves_schedule_fetch.argtypes = [vp, vp, vp, vp]
+        lib.blance_moves_exposure.argtypes = [vp, vp, vp, vp]
         lib.blance_moves_free.argtypes = [vp, vp]
         lib.blance_moves_free.restype = None
         _CAPI = lib
@@ -155,3 +171,5 @@ ChainOut = _ChainOut
 ScenarioScheduleOut = _ScenarioScheduleOut
 AuditOpts = _AuditOpts
 AuditOut = _AuditOut
+ExposureIn = _ExposureIn
+ExposureOut = _ExposureOut

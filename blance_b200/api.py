@@ -7,6 +7,8 @@
     CalcPartitionMoves(states, begNodesByState, endNodesByState, favorMinNodes) -> [NodeStateOp]   moves.go:41-46
     OrchestrateSchedule(model, options, nodesAll, begMap, endMap) -> rounds of AssignPartitionsFunc calls
         (the lock-step model of OrchestrateMoves, orchestrate.go:240-591; include/blance_b200.h)
+    OrchestrateExposure(model, options, nodesAll, begMap, endMap, nodeHierarchy) -> the maps those rounds pass
+        through, counted per round (blance_moves_exposure)
 
 A PartitionMap is {partitionName: {stateName: [nodeName, ...] | None}}; a
 PartitionModel is {stateName: (priority, constraints)}; HierarchyRules is
@@ -232,6 +234,23 @@ def OrchestrateSchedule(model, options, nodesAll, begMap, endMap):
     r = _host.OrchestrateSchedule({k: tuple(v) for k, v in model.items()}, int(o.MaxConcurrentPartitionMovesPerNode),
                                   bool(o.FavorMinNodes), list(nodesAll), begMap, endMap)
     return [[AssignPartitionsCall(*c) for c in rnd] for rnd in r]
+
+
+def OrchestrateExposure(model, options, nodesAll, begMap, endMap, nodeHierarchy=None):
+    """Is the data safe while the rebalance of OrchestrateSchedule(model, options, nodesAll, begMap, endMap) runs?  The
+    maps M_0 .. M_R it passes through under the lock-step model (M_t: after t rounds of AssignPartitionsFunc calls),
+    counted on the device (blance_moves_exposure, include/blance_b200.h).  Constraints are the model's, the top state
+    is the model's lowest priority (ties: first name), nodeHierarchy ({child: parent}, as NodeHierarchy) the
+    fault-domain forest (None: every node is its own domain).  Returns a dict:
+      rounds R;  series {metric: [R + 1 values]}, peak / peak_round / area {metric: ...} for every metric of
+        NO_TOP (no primary), MULTI_TOP (more primaries than the constraint), SHORT, ONE_COPY, NO_COPY, COPIES;
+      dom_peak / dom_peak_round {node or hierarchy name: most partitions it alone held at one round / first such
+        round}, part_min_copies / part_no_top / part_flags {partition: ...}: nonzero entries only;
+      kernel_ms."""
+    o = options or OrchestratorOptions()
+    return _host.OrchestrateExposure({k: tuple(v) for k, v in model.items()}, int(o.MaxConcurrentPartitionMovesPerNode),
+                                     bool(o.FavorMinNodes), list(nodesAll), begMap, endMap,
+                                     None if nodeHierarchy is None else dict(nodeHierarchy))
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------

@@ -69,22 +69,23 @@ __device__ __forceinline__ const int32_t* audit_row(const AuditInst& A, long lon
   return row;
 }
 
-__device__ __forceinline__ int audit_parent(const AuditInst& A, int v) { return A.dom_parent ? __ldg(A.dom_parent + v) : -1; }
+// The fault-domain forest (domain_parent, or NULL: every node its own root), shared with exposure.cuh.
+__device__ __forceinline__ int audit_parent(const int32_t* par, int v) { return par ? __ldg(par + v) : -1; }
 
-__device__ __forceinline__ int audit_depth(const AuditInst& A, int v) {
+__device__ __forceinline__ int audit_depth(const int32_t* par, int v) {
   int d = 0;
-  for (int u = audit_parent(A, v); u >= 0 && d < AUDIT_DEPTH_MAX; u = audit_parent(A, u)) ++d;
+  for (int u = audit_parent(par, v); u >= 0 && d < AUDIT_DEPTH_MAX; u = audit_parent(par, u)) ++d;
   return d;
 }
 
 // deepest common ancestor of two vertices, -1 when they are in different trees
-__device__ __forceinline__ int audit_dca(const AuditInst& A, int a, int b) {
-  if (a == b || !A.dom_parent) return a == b ? a : -1;
-  int da = audit_depth(A, a), db = audit_depth(A, b);
-  for (; da > db; --da) a = audit_parent(A, a);
-  for (; db > da; --db) b = audit_parent(A, b);
+__device__ __forceinline__ int audit_dca(const int32_t* par, int a, int b) {
+  if (a == b || !par) return a == b ? a : -1;
+  int da = audit_depth(par, a), db = audit_depth(par, b);
+  for (; da > db; --da) a = audit_parent(par, a);
+  for (; db > da; --db) b = audit_parent(par, b);
   for (int i = 0; a != b && i <= AUDIT_DEPTH_MAX; ++i) {
-    a = audit_parent(A, a); b = audit_parent(A, b);
+    a = audit_parent(par, a); b = audit_parent(par, b);
     if (a < 0 || b < 0) return -1;
   }
   return a == b ? a : -1;
@@ -126,8 +127,8 @@ __global__ void k_map_audit(const AuditInst* __restrict__ insts) {
         const int32_t x = row[c];
         if (x == BLANCE_NO_NODE) break;
         if (x < 0 || x >= NU) continue;
-        for (int v = x, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A, v), ++d) dom_add(2, v);
-        dca = dca == -2 ? x : dca == -1 ? -1 : audit_dca(A, dca, x);
+        for (int v = x, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A.dom_parent, v), ++d) dom_add(2, v);
+        dca = dca == -2 ? x : dca == -1 ? -1 : audit_dca(A.dom_parent, dca, x);
         if (A.n2n && h >= 0 && h < N && x < N && x != h) red_add32(A.n2n + (long long)h * N + x, 1);
       }
       const int k = A.constraints[s];
@@ -135,8 +136,8 @@ __global__ void k_map_audit(const AuditInst* __restrict__ insts) {
       if (len < k) { reds_add32(&s_state[s], (uint32_t)(k - len)); is_short = true; }
       if (len > k) reds_add32(&s_state[BL_S_MAX + s], (uint32_t)(len - k));
     }
-    for (int v = h, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A, v), ++d) dom_add(0, v);
-    for (int v = dca, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A, v), ++d) dom_add(1, v);
+    for (int v = h, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A.dom_parent, v), ++d) dom_add(0, v);
+    for (int v = dca, d = 0; v >= 0 && d <= AUDIT_DEPTH_MAX; v = audit_parent(A.dom_parent, v), ++d) dom_add(1, v);
     n_short += is_short ? 1u : 0u;
     n_notop += h < 0 ? 1u : 0u;
     if (A.part_flags) A.part_flags[p] = (uint8_t)((is_short ? 1 : 0) | (h < 0 ? 4 : 0));

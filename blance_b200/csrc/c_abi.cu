@@ -29,6 +29,7 @@
 #include "blance_b200.h"
 #include "count_bound.hpp"
 #include "device_types.cuh"
+#include "exposure.cuh"
 #include "wave_schedule.cuh"
 
 using namespace blance_dev;
@@ -1326,6 +1327,24 @@ static void check_audit_model(const std::string& name, const blance_plan_in* m) 
       bad("rule_off is not a monotone offset table into the rules");
 }
 
+// A fault-domain forest over NU node ids and n_domains inner vertices (parent NULL: none): n_domains in [0, 2^24], no
+// cycle, every vertex at most AUDIT_DEPTH_MAX edges below its root.
+static void check_forest(const std::string& name, int n_domains, const int32_t* parent, int NU) {
+  if (n_domains < 0 || n_domains > (1 << 24)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains outside [0, 2^24]");
+  if (!parent && n_domains != 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains without domain_parent");
+  if (!parent) return;
+  const long long V = (long long)NU + n_domains;
+  for (long long v = 0; v < V; ++v)
+    if (parent[v] < -1 || parent[v] >= V)
+      throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent[" + std::to_string(v) + "] is outside [-1, n_node_ids + n_domains)");
+  for (long long v = 0; v < V; ++v) {
+    int d = 0;
+    for (long long u = parent[v]; u >= 0; u = parent[u])
+      if (++d > AUDIT_DEPTH_MAX)
+        throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent has a cycle or a vertex more than 16 edges below its root (vertex " + std::to_string(v) + ")");
+  }
+}
+
 // The options of an audit over NU node ids, checked: flags, and a fault-domain forest without cycles, every vertex
 // at most AUDIT_DEPTH_MAX edges below its root.
 static AuditReq check_audit_opts(const std::string& name, const blance_audit_opts* o, int NU, blance_audit_out* out) {
@@ -1334,20 +1353,8 @@ static AuditReq check_audit_opts(const std::string& name, const blance_audit_opt
   if (!out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": the audit output is NULL");
   if (!o) return ar;
   if (o->flags & ~(uint32_t)BLANCE_AUDIT_N2N) throw_err(BLANCE_ERR_INVALID_ARG, name + ": audit flags hold an unknown bit");
-  if (o->n_domains < 0 || o->n_domains > (1 << 24)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains outside [0, 2^24]");
-  if (!o->domain_parent && o->n_domains != 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_domains without domain_parent");
   ar.flags = o->flags; ar.n_domains = o->n_domains; ar.parent = o->domain_parent;
-  if (!ar.parent) return ar;
-  const long long V = (long long)NU + o->n_domains;
-  for (long long v = 0; v < V; ++v)
-    if (ar.parent[v] < -1 || ar.parent[v] >= V)
-      throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent[" + std::to_string(v) + "] is outside [-1, n_node_ids + n_domains)");
-  for (long long v = 0; v < V; ++v) {
-    int d = 0;
-    for (long long u = ar.parent[v]; u >= 0; u = ar.parent[u])
-      if (++d > AUDIT_DEPTH_MAX)
-        throw_err(BLANCE_ERR_INVALID_ARG, name + ": domain_parent has a cycle or a vertex more than 16 edges below its root (vertex " + std::to_string(v) + ")");
-  }
+  check_forest(name, o->n_domains, o->domain_parent, NU);
   return ar;
 }
 
@@ -2069,7 +2076,9 @@ extern "C" int blance_calc_partition_moves(blance_ctx* ctx, int32_t n_parts, int
 struct blance_moves {
   int32_t n_parts = 0, n_node_ids = 0;
   long long total_ops = 0;
+  std::vector<int32_t> slot_off;     // [n_states + 1], host copy of the slot layout
   Arena arena;
+  int32_t* d_beg = nullptr;          // [n_parts][n_slots] the beg rows (blance_moves_exposure)
   long long* d_off = nullptr;        // [n_parts + 1]
   int32_t* d_node = nullptr; uint8_t* d_state = nullptr; uint8_t* d_kind = nullptr;   // CSR ops
   int32_t* d_next = nullptr;         // [n_parts] cursors of the current round
@@ -2103,9 +2112,11 @@ extern "C" int blance_moves_create(blance_ctx* ctx, int32_t n_parts, int32_t n_s
     cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr, n_parts, 0, 32, st);
     std::unique_ptr<blance_moves> mv(new blance_moves());
     mv->n_parts = n_parts; mv->n_node_ids = n_node_ids;
+    mv->slot_off.assign(state_slot_off, state_slot_off + n_states + 1);
     mv->tmp_bytes = std::max(scan_tmp, sort_tmp) + 256;
-    // scratch of the construction (rows, padded ops, counts) lives in the same arena and is simply left unused later
-    int32_t *d_slot, *d_beg, *d_end, *p_node, *d_cnt;
+    // scratch of the construction (end rows, padded ops, counts) lives in the same arena and is simply left unused
+    // later; the beg rows stay for blance_moves_exposure
+    int32_t *d_slot, *&d_beg = mv->d_beg, *d_end, *p_node, *d_cnt;
     uint8_t *p_state, *p_kind;
     Arena& a = mv->arena;
     a.add(mv->d_off, P + 2); a.add(mv->d_node, P * max_ops);
@@ -2255,6 +2266,138 @@ extern "C" int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* mv, in
     if (sched_op && mv->sched_moves > 0)
       CUDA(cudaMemcpyAsync(sched_op, mv->sched_op, sizeof(long long) * (size_t)mv->sched_moves, cudaMemcpyDeviceToHost, st));
     CUDA(cudaStreamSynchronize(st));
+  });
+}
+
+// The exposure of the handle's last schedule (exposure.cuh; include/blance_b200.h).
+extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const blance_exposure_in* in, blance_exposure_out* out) {
+  return entry(ctx, [&](Device& device) {
+    const std::string name = "blance_moves_exposure";
+    if (!ctx || !mv || !in || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": ctx, moves, in or out is NULL");
+    if (mv->sched_rounds < 0 || !mv->sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": no schedule was computed on this handle");
+    const int S = (int)mv->slot_off.size() - 1, SL = mv->slot_off[(size_t)S];
+    if (S > BL_S_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 8 states");
+    if (SL > BL_SLP_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 32 slots per row");
+    if (S > 0 && !in->state_constraints) throw_err(BLANCE_ERR_INVALID_ARG, name + ": state_constraints is NULL");
+    for (int s = 0; s < S; ++s)
+      if (in->state_constraints[s] < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": negative state constraint");
+    if (in->top_state < -1 || in->top_state >= S) throw_err(BLANCE_ERR_INVALID_ARG, name + ": top_state outside [-1, n_states)");
+    const int NU = mv->n_node_ids;
+    check_forest(name, in->n_domains, in->domain_parent, NU);
+    // a scheduled op emits at most two ancestor chains of AUDIT_DEPTH_MAX + 1 vertices; the event count is an int
+    if ((out->dom_peak || out->dom_peak_round) && 2ll * (AUDIT_DEPTH_MAX + 1) * mv->sched_moves >= (1ll << 31))
+      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": dom_peak needs 34 x moves_done < 2^31");
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    const int P = mv->n_parts, R = mv->sched_rounds;
+    const long long T = mv->total_ops, M = mv->sched_moves, R1 = (long long)R + 1;
+    const int V = NU + in->n_domains;
+    const bool dom = out->dom_peak || out->dom_peak_round;
+    ExpoArgs E{};
+    E.op_off = mv->d_off; E.op_node = mv->d_node; E.op_state = mv->d_state; E.op_kind = mv->d_kind; E.beg = mv->d_beg;
+    E.P = P; E.SL = SL; E.S = S; E.NU = NU; E.R = R; E.top = in->top_state;
+    for (int s = 0; s < S; ++s) { E.constraints[s] = in->state_constraints[s]; E.slot_off[s] = mv->slot_off[(size_t)s]; }
+    E.slot_off[S] = SL;
+    int32_t* op_round = nullptr;
+    long long* stats = nullptr;
+    int32_t* parent = nullptr;
+    unsigned long long* dom_key = nullptr;
+    long long* ev_off = nullptr;
+    size_t scan_tmp = 0;
+    void* tmp = nullptr;
+    CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const long long*)nullptr, (long long*)nullptr, P + 1, st));
+    Arena a;
+    a.add(op_round, (size_t)std::max(T, 1ll)); a.add(E.diff, (size_t)(BLANCE_EXPO_N * R1)); a.add(stats, 3 * BLANCE_EXPO_N);
+    if (out->part_min_copies) a.add(E.part_min, (size_t)P);
+    if (out->part_no_top) a.add(E.part_notop, (size_t)P);
+    if (out->part_flags) a.add(E.part_flags, (size_t)P);
+    if (dom) {
+      if (in->domain_parent) a.add(parent, (size_t)V);
+      a.add(E.dom_base, (size_t)V); a.add(dom_key, (size_t)V);
+      a.add(E.ev_count, (size_t)P + 1); a.add(ev_off, (size_t)P + 1); a.add(tmp, scan_tmp);
+    }
+    a.alloc(st, "the exposure");
+    E.op_round = op_round; E.dom_parent = parent;
+    CUDA(cudaEventRecord(dev->ev[0], st));
+    if (parent) CUDA(cudaMemcpyAsync(parent, in->domain_parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
+    CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(T, 1ll), st));
+    CUDA(cudaMemsetAsync(E.diff, 0, sizeof(long long) * (size_t)(BLANCE_EXPO_N * R1), st));
+    if (dom && V > 0) CUDA(cudaMemsetAsync(E.dom_base, 0, sizeof(long long) * (size_t)V, st));
+    if (M > 0) launch(dev, k_expo_op_round, grid_for(dev, M, 256), 256, 0, M, R, (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
+    if (P > 0) launch(dev, k_expo_walk<0>, grid_for(dev, P, 256), 256, 0, E);
+    launch(dev, k_expo_series, BLANCE_EXPO_N, 512, 0, E.diff, R, stats);
+    // fault domains: (vertex, t, +-1) events where a partition's deepest common ancestor changes, sized exactly by a
+    // counting walk, sorted by (vertex, t), merged per key, scanned per vertex; dom_key keeps each vertex's maximum
+    std::unique_ptr<Arena> ev;
+    if (dom && V > 0) {
+      launch(dev, k_expo_dom_init, grid_for(dev, V, 256), 256, 0, V, (const long long*)E.dom_base, dom_key);
+      long long n_ev = 0;
+      if (P > 0 && M > 0) {
+        CUDA(cudaMemsetAsync(E.ev_count + P, 0, sizeof(long long), st));
+        launch(dev, k_expo_walk<1>, grid_for(dev, P, 256), 256, 0, E);
+        CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, E.ev_count, ev_off, P + 1, st));
+        CUDA(cudaMemcpyAsync(&n_ev, ev_off + P, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        CUDA(cudaStreamSynchronize(st));
+        E.ev_off = ev_off;
+      }
+      if (n_ev > 0) {
+        const int NE = (int)n_ev;
+        int vbits = 1;
+        while ((1ll << vbits) < V) ++vbits;
+        unsigned long long *k2, *uk;
+        int32_t *v2, *uv, *run;
+        int* n_runs;
+        size_t sort_b = 0, red_b = 0, scan_b = 0;
+        CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                             (const int32_t*)nullptr, (int32_t*)nullptr, NE, 0, 32 + vbits, st));
+        CUDA(cub::DeviceReduce::ReduceByKey(nullptr, red_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                            (const int32_t*)nullptr, (int32_t*)nullptr, (int*)nullptr, ExpoSum(), NE, st));
+        CUDA(cub::DeviceScan::InclusiveScanByKey(nullptr, scan_b, (const unsigned long long*)nullptr, (const int32_t*)nullptr,
+                                                 (int32_t*)nullptr, ExpoSum(), NE, ExpoSameVertex(), st));
+        size_t ev_tmp_b = std::max(sort_b, std::max(red_b, scan_b));
+        void* ev_tmp = nullptr;
+        ev.reset(new Arena());
+        ev->add(E.ev_key, (size_t)NE); ev->add(E.ev_val, (size_t)NE); ev->add(k2, (size_t)NE); ev->add(v2, (size_t)NE);
+        ev->add(uk, (size_t)NE); ev->add(uv, (size_t)NE); ev->add(run, (size_t)NE); ev->add(n_runs, 1); ev->add(ev_tmp, ev_tmp_b);
+        ev->alloc(st, "the exposure's fault-domain events");
+        launch(dev, k_expo_walk<2>, grid_for(dev, P, 256), 256, 0, E);
+        size_t b = ev_tmp_b;
+        CUDA(cub::DeviceRadixSort::SortPairs(ev_tmp, b, E.ev_key, k2, E.ev_val, v2, NE, 0, 32 + vbits, st));
+        b = ev_tmp_b;
+        CUDA(cub::DeviceReduce::ReduceByKey(ev_tmp, b, k2, uk, v2, uv, n_runs, ExpoSum(), NE, st));
+        int h_runs = 0;                            // only the merged runs are scanned
+        CUDA(cudaMemcpyAsync(&h_runs, n_runs, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CUDA(cudaStreamSynchronize(st));
+        b = ev_tmp_b;
+        CUDA(cub::DeviceScan::InclusiveScanByKey(ev_tmp, b, uk, uv, run, ExpoSum(), h_runs, ExpoSameVertex(), st));
+        launch(dev, k_expo_dom_max, grid_for(dev, h_runs, 256), 256, 0, h_runs, (const unsigned long long*)uk,
+               (const int32_t*)run, (const long long*)E.dom_base, dom_key);
+      }
+    }
+    CUDA(cudaEventRecord(dev->ev[1], st));
+    std::vector<long long> h_stats(3 * BLANCE_EXPO_N);
+    std::vector<unsigned long long> h_key(dom ? (size_t)V : 0);
+    CUDA(cudaMemcpyAsync(h_stats.data(), stats, sizeof(long long) * h_stats.size(), cudaMemcpyDeviceToHost, st));
+    if (out->series) CUDA(cudaMemcpyAsync(out->series, E.diff, sizeof(long long) * (size_t)(BLANCE_EXPO_N * R1), cudaMemcpyDeviceToHost, st));
+    if (P > 0) {
+      if (out->part_min_copies) CUDA(cudaMemcpyAsync(out->part_min_copies, E.part_min, sizeof(int32_t) * (size_t)P, cudaMemcpyDeviceToHost, st));
+      if (out->part_no_top) CUDA(cudaMemcpyAsync(out->part_no_top, E.part_notop, sizeof(int32_t) * (size_t)P, cudaMemcpyDeviceToHost, st));
+      if (out->part_flags) CUDA(cudaMemcpyAsync(out->part_flags, E.part_flags, (size_t)P, cudaMemcpyDeviceToHost, st));
+    }
+    if (dom && V > 0) CUDA(cudaMemcpyAsync(h_key.data(), dom_key, sizeof(unsigned long long) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    out->kernel_ms = 0.f;
+    cudaEventElapsedTime(&out->kernel_ms, dev->ev[0], dev->ev[1]);
+    out->rounds = R;
+    for (int m = 0; m < BLANCE_EXPO_N; ++m) {
+      out->peak[m] = h_stats[(size_t)(3 * m)];
+      out->peak_round[m] = (int32_t)h_stats[(size_t)(3 * m + 1)];
+      out->area[m] = h_stats[(size_t)(3 * m + 2)];
+    }
+    for (int v = 0; v < (dom ? V : 0); ++v) {
+      if (out->dom_peak) out->dom_peak[v] = (int64_t)(h_key[(size_t)v] >> 32);
+      if (out->dom_peak_round) out->dom_peak_round[v] = (int32_t)(0xFFFFFFFFu - (uint32_t)h_key[(size_t)v]);
+    }
   });
 }
 

@@ -186,6 +186,18 @@ struct ErrorSlot {
 // reference is then non-deterministic); starting from ascending names and running
 // Go's small-slice insertion sort gives (priority, name) order whenever the
 // reference is deterministic.
+// topPriorityStateName (plan.go:126-132): the state of minimum priority.  The reference walks the model in map order,
+// so ties are random there; here the first in ascending name order wins.  "" for an empty model.
+std::string top_priority_state_name(const PartitionModel& model) {
+  Strs by_name;
+  for (const auto& kv : model) by_name.push_back(kv.first);
+  std::sort(by_name.begin(), by_name.end());
+  std::string top;
+  for (const auto& n : by_name)
+    if (top.empty() || model.at(n).Priority < model.at(top).Priority) top = n;
+  return top;
+}
+
 Strs sort_state_names(const PartitionModel& model) {
   Strs s;
   for (const auto& kv : model) s.push_back(kv.first);
@@ -343,14 +355,7 @@ static std::unique_ptr<InternedPlan> intern_plan(const PartitionMap& prevMap, co
       if (it != options.StateStickiness->end()) { ip->state_stickiness[size_t(s)] = it->second; ip->state_has_stickiness[size_t(s)] = 1; }
     }
   }
-  {
-    // plan.go:126-132 walks the model in map order; ties on the minimum priority are
-    // resolved here as "first in ascending name order" (the reference is random).
-    Strs by_name = ip->state_names;
-    std::sort(by_name.begin(), by_name.end());
-    for (const auto& n : by_name)
-      if (top_state < 0 || model.at(n).Priority < ip->state_priority[size_t(top_state)]) top_state = state_id[n];
-  }
+  if (S > 0) top_state = state_id[top_priority_state_name(model)];
   // the model has a handful of states: comparing names beats hashing them
   auto find_state = [&](const std::string& name) -> int32_t {
     for (int32_t s = 0; s < S; ++s)
@@ -1114,7 +1119,7 @@ ScenarioTables scenario_tables(const InternedPlan& ip, const PartitionModel& mod
 
 namespace {
 
-// The fault-domain forest of blance_audit_opts over ip's node ids: the node names are vertices 0 .. NU-1, every other
+// The fault-domain forest of blance_audit_opts over interned node ids: the node names are vertices 0 .. NU-1, every other
 // name of `parents` follows in byte order; a missing or "" parent is a root.
 struct Forest {
   Strs names;                          // [V]
@@ -1122,8 +1127,8 @@ struct Forest {
   blance_audit_opts opts{};
 };
 
-void build_forest(const InternedPlan& ip, const std::optional<std::unordered_map<std::string, std::string>>& parents, bool n2n, Forest* f) {
-  f->names = ip.node_names;
+void build_forest(const Strs& node_names, const std::optional<std::unordered_map<std::string, std::string>>& parents, bool n2n, Forest* f) {
+  f->names = node_names;
   f->opts = blance_audit_opts{};
   f->opts.flags = n2n ? BLANCE_AUDIT_N2N : 0;
   if (!parents) return;
@@ -1137,7 +1142,7 @@ void build_forest(const InternedPlan& ip, const std::optional<std::unordered_map
   f->parent.assign(f->names.size(), -1);
   for (const auto& kv : *parents)
     if (!kv.first.empty() && !kv.second.empty()) f->parent[size_t(id[kv.first])] = id[kv.second];
-  f->opts.n_domains = int32_t(f->names.size() - ip.node_names.size());
+  f->opts.n_domains = int32_t(f->names.size() - node_names.size());
   f->opts.domain_parent = f->parent.data();
 }
 
@@ -1195,7 +1200,7 @@ MapAudit name_audit(const InternedPlan& ip, const Forest& f, const int32_t* rule
 void AuditForest(const InternedPlan& ip, const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy,
                  Strs* names, std::vector<int32_t>* parent) {
   Forest f;
-  build_forest(ip, nodeHierarchy, false, &f);
+  build_forest(ip.node_names, nodeHierarchy, false, &f);
   *names = std::move(f.names);
   *parent = std::move(f.parent);
 }
@@ -1210,7 +1215,7 @@ MapAudit AuditMap(const PartitionMap& map, const Strs& nodesAll, const Partition
   o.HierarchyRules = options.HierarchyRules;
   auto ip = InternPlan(map, PartitionMap{}, nodesAll, std::nullopt, std::nullopt, model, o);
   Forest f;
-  build_forest(*ip, options.NodeHierarchy, failoverSpread, &f);
+  build_forest(ip->node_names, options.NodeHierarchy, failoverSpread, &f);
   const size_t R = ip->in.has_hier_rules ? size_t(ip->in.n_rules) : 0;
   AuditBuffers b(*ip, f.names.size(), R, failoverSpread);
   blance_ctx* ctx = DefaultContext();
@@ -1353,7 +1358,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     return ip->in.has_hier_rules ? ip->rule_off.data() : nullptr;
   };
   if (audit) {
-    build_forest(*ip, options.NodeHierarchy, audit->FailoverSpread, &forest);
+    build_forest(ip->node_names, options.NodeHierarchy, audit->FailoverSpread, &forest);
     for (size_t i = 0; i < n; ++i) {
       const int32_t R = (tabs[i].set & BLANCE_OPT_HIERARCHY) ? (tabs[i].has_hier_rules ? tabs[i].n_rules : 0)
                                                              : (ip->in.has_hier_rules ? ip->in.n_rules : 0);
@@ -1597,58 +1602,127 @@ std::unordered_map<std::string, std::vector<NodeStateOp>> CalcPartitionMovesMap(
   return out;
 }
 
-std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const PartitionModel& model, const OrchestratorOptions& options,
-                                                                   const Strs& nodesAll, const PartitionMap& begMap,
-                                                                   const PartitionMap& endMap) {
+namespace {
+
+// The move lists of OrchestrateMoves(model, options, nodesAll, begMap, endMap) on the device and their lock-step
+// schedule: what OrchestrateSchedule copies out and OrchestrateExposure counts over.
+struct Orchestrated {
+  MovesTables t;
+  Strs names;                                        // partitions: begMap's keys in byte order
+  blance_ctx* ctx = nullptr;
+  std::unique_ptr<blance_moves, std::function<void(blance_moves*)>> h;
+  int64_t total = 0;
+  blance_schedule_out so{};
+  void check(int st, const char* what) const {
+    if (st != BLANCE_OK) throw BlanceError(st, std::string(what) + " failed: " + blance_last_error(ctx));
+  }
+};
+
+std::unique_ptr<Orchestrated> orchestrate(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
+                                          const PartitionMap& begMap, const PartitionMap& endMap) {
   if (begMap.size() != endMap.size()) throw BlanceError(BLANCE_ERR_INVALID_ARG, "mismatched begMap and endMap");   // orchestrate.go:250-252
+  auto o = std::make_unique<Orchestrated>();
+  MovesTables& t = o->t;
   const Strs states = sort_state_names(model);
-  Strs names;                                        // orchestrate.go:273: the partitions of begMap
-  for (const auto& kv : begMap) names.push_back(kv.first);
-  std::sort(names.begin(), names.end());
+  for (const auto& kv : begMap) o->names.push_back(kv.first);   // orchestrate.go:273: the partitions of begMap
+  std::sort(o->names.begin(), o->names.end());
   std::vector<const NodesByState*> begs, ends;
-  for (const auto& n : names) {
+  for (const auto& n : o->names) {
     begs.push_back(&begMap.at(n).NodesByState);
     auto e = endMap.find(n);
     ends.push_back(e == endMap.end() ? nullptr : &e->second.NodesByState);
   }
-  MovesTables t;
   for (const auto& n : nodesAll) t.nodes.get(n);     // node ids: nodesAll first, so exactly they have a mover
   const size_t n_movers = t.nodes.names.size();
   intern_moves(states, begs, ends, &t);
-  const int32_t P = int32_t(names.size()), S = int32_t(t.state_names.size()), NN = int32_t(t.nodes.names.size());
+  const int32_t P = int32_t(o->names.size()), S = int32_t(t.state_names.size()), NN = int32_t(t.nodes.names.size());
   std::vector<uint8_t> mover(size_t(NN) + 1, 0);
   for (size_t i = 0; i < n_movers; ++i) mover[i] = 1;
-  blance_ctx* ctx = DefaultContext();
-  auto check = [&](int st, const char* what) {
-    if (st != BLANCE_OK) throw BlanceError(st, std::string(what) + " failed: " + blance_last_error(ctx));
-  };
+  o->ctx = DefaultContext();
+  blance_ctx* ctx = o->ctx;
   blance_moves* h = nullptr;
-  int64_t total = 0;
-  check(blance_moves_create(ctx, P, S, t.n_visit, t.slot_off.data(), t.beg_rows.data(), t.end_rows.data(),
-                            options.FavorMinNodes ? 1 : 0, NN, &h, &total), "blance_moves_create");
-  std::unique_ptr<blance_moves, std::function<void(blance_moves*)>> guard(h, [ctx](blance_moves* m) { blance_moves_free(ctx, m); });
-  blance_schedule_out so{};
-  check(blance_moves_schedule(ctx, h, options.MaxConcurrentPartitionMovesPerNode, mover.data(), &so), "blance_moves_schedule");
+  o->check(blance_moves_create(ctx, P, S, t.n_visit, t.slot_off.data(), t.beg_rows.data(), t.end_rows.data(),
+                               options.FavorMinNodes ? 1 : 0, NN, &h, &o->total), "blance_moves_create");
+  o->h = std::unique_ptr<blance_moves, std::function<void(blance_moves*)>>(h, [ctx](blance_moves* m) { blance_moves_free(ctx, m); });
+  o->check(blance_moves_schedule(ctx, h, options.MaxConcurrentPartitionMovesPerNode, mover.data(), &o->so), "blance_moves_schedule");
+  return o;
+}
+
+}  // namespace
+
+std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const PartitionModel& model, const OrchestratorOptions& options,
+                                                                   const Strs& nodesAll, const PartitionMap& begMap,
+                                                                   const PartitionMap& endMap) {
+  const auto o = orchestrate(model, options, nodesAll, begMap, endMap);
+  const MovesTables& t = o->t;
+  const blance_schedule_out& so = o->so;
+  const size_t P = o->names.size();
   std::vector<int64_t> round_off(size_t(so.rounds) + 1), sched(size_t(std::max<int64_t>(so.moves_done, 1)));
-  check(blance_moves_schedule_fetch(ctx, h, round_off.data(), sched.data()), "blance_moves_schedule_fetch");
-  std::vector<int64_t> op_off(size_t(P) + 1);
-  std::vector<int32_t> op_node(size_t(std::max<int64_t>(total, 1)));
+  o->check(blance_moves_schedule_fetch(o->ctx, o->h.get(), round_off.data(), sched.data()), "blance_moves_schedule_fetch");
+  std::vector<int64_t> op_off(P + 1);
+  std::vector<int32_t> op_node(size_t(std::max<int64_t>(o->total, 1)));
   std::vector<uint8_t> op_state(op_node.size()), op_kind(op_node.size());
-  check(blance_moves_fetch(ctx, h, op_off.data(), op_node.data(), op_state.data(), op_kind.data()), "blance_moves_fetch");
+  o->check(blance_moves_fetch(o->ctx, o->h.get(), op_off.data(), op_node.data(), op_state.data(), op_kind.data()), "blance_moves_fetch");
   static const char* kOps[] = {"add", "del", "promote", "demote"};
   std::vector<std::vector<AssignPartitionsCall>> out(size_t(so.rounds));
   for (size_t r = 0; r < out.size(); ++r)
     for (int64_t i = round_off[r]; i < round_off[r + 1]; ++i) {
-      const int64_t o = sched[size_t(i)];
-      const size_t p = size_t(std::upper_bound(op_off.begin(), op_off.end(), o) - op_off.begin()) - 1;
-      const auto& node = t.nodes.names[size_t(op_node[size_t(o)])];
+      const int64_t op = sched[size_t(i)];
+      const size_t p = size_t(std::upper_bound(op_off.begin(), op_off.end(), op) - op_off.begin()) - 1;
+      const auto& node = t.nodes.names[size_t(op_node[size_t(op)])];
       if (out[r].empty() || out[r].back().Node != node) out[r].push_back(AssignPartitionsCall{node, {}, {}, {}});
       auto& call = out[r].back();
-      call.Partitions.push_back(names[p]);
-      call.States.push_back(op_state[size_t(o)] == BLANCE_OP_STATE_NONE ? std::string() : t.state_names[op_state[size_t(o)]]);
-      call.Ops.push_back(kOps[op_kind[size_t(o)]]);
+      call.Partitions.push_back(o->names[p]);
+      call.States.push_back(op_state[size_t(op)] == BLANCE_OP_STATE_NONE ? std::string() : t.state_names[op_state[size_t(op)]]);
+      call.Ops.push_back(kOps[op_kind[size_t(op)]]);
     }
   return out;
+}
+
+ExposureResult OrchestrateExposure(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
+                                   const PartitionMap& begMap, const PartitionMap& endMap,
+                                   const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy) {
+  const auto o = orchestrate(model, options, nodesAll, begMap, endMap);
+  const MovesTables& t = o->t;
+  const size_t S = t.state_names.size(), P = o->names.size(), R1 = size_t(o->so.rounds) + 1;
+  std::vector<int32_t> cons(S + 1, 0);               // the model's Constraints; 0 for states outside the model
+  for (size_t s = 0; s < S; ++s) {
+    auto it = model.find(t.state_names[s]);
+    if (it != model.end()) cons[s] = it->second.Constraints;
+  }
+  const std::string top = top_priority_state_name(model);
+  int32_t top_state = -1;
+  for (size_t s = 0; s < S && !top.empty(); ++s)
+    if (t.state_names[s] == top) top_state = int32_t(s);
+  Forest f;
+  build_forest(t.nodes.names, nodeHierarchy, false, &f);
+  const size_t V = f.names.size();
+  blance_exposure_in in{cons.data(), top_state, f.opts.n_domains, f.opts.domain_parent};
+  std::vector<int64_t> series(BLANCE_EXPO_N * R1), dom_peak(V + 1);
+  std::vector<int32_t> dom_round(V + 1), min_copies(P + 1), no_top(P + 1);
+  std::vector<uint8_t> flags(P + 1);
+  blance_exposure_out out{};
+  out.series = series.data(); out.dom_peak = dom_peak.data(); out.dom_peak_round = dom_round.data();
+  out.part_min_copies = min_copies.data(); out.part_no_top = no_top.data(); out.part_flags = flags.data();
+  o->check(blance_moves_exposure(o->ctx, o->h.get(), &in, &out), "blance_moves_exposure");
+  static const char* kMetrics[BLANCE_EXPO_N] = {"NO_TOP", "MULTI_TOP", "SHORT", "ONE_COPY", "NO_COPY", "COPIES"};
+  ExposureResult r;
+  r.Rounds = out.rounds;
+  r.KernelMs = out.kernel_ms;
+  for (size_t m = 0; m < BLANCE_EXPO_N; ++m) {
+    r.Series[kMetrics[m]].assign(series.begin() + std::ptrdiff_t(m * R1), series.begin() + std::ptrdiff_t((m + 1) * R1));
+    r.Peak[kMetrics[m]] = out.peak[m];
+    r.PeakRound[kMetrics[m]] = out.peak_round[m];
+    r.Area[kMetrics[m]] = out.area[m];
+  }
+  for (size_t v = 0; v < V; ++v)
+    if (dom_peak[v]) { r.DomPeak[f.names[v]] = dom_peak[v]; r.DomPeakRound[f.names[v]] = dom_round[v]; }
+  for (size_t p = 0; p < P; ++p) {
+    if (min_copies[p]) r.PartMinCopies[o->names[p]] = min_copies[p];
+    if (no_top[p]) r.PartNoTop[o->names[p]] = no_top[p];
+    if (flags[p]) r.PartFlags[o->names[p]] = flags[p];
+  }
+  return r;
 }
 
 }  // namespace blance

@@ -251,6 +251,29 @@ std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const Partiti
                                                                    const Strs& nodesAll, const PartitionMap& begMap,
                                                                    const PartitionMap& endMap);
 
+// The exposure of that rebalance (blance_moves_exposure, include/blance_b200.h): the same move lists and schedule as
+// OrchestrateSchedule, and the maps M_0 .. M_R it passes through counted per round.  Constraints are the model's
+// Constraints (0 for state names outside the model), the top state is topPriorityStateName (plan.go:126-132; ties go
+// to the first name in ascending order), and nodeHierarchy is the fault-domain forest as AuditMap builds it from
+// NodeHierarchy (nil: every node is its own domain).  Metric-keyed fields ("NO_TOP", "MULTI_TOP", "SHORT",
+// "ONE_COPY", "NO_COPY", "COPIES") hold every metric; vertex- and partition-keyed fields hold nonzero entries only
+// (a partition absent from PartMinCopies had no copy at some round; DomPeakRound lists the vertices of DomPeak).
+// Throws BlanceError for what OrchestrateSchedule or blance_moves_exposure rejects (e.g. more than 8 state names).
+struct ExposureResult {
+  int32_t Rounds = 0;
+  std::unordered_map<std::string, std::vector<int64_t>> Series;   // [Rounds + 1] per metric
+  std::unordered_map<std::string, int64_t> Peak, Area;
+  std::unordered_map<std::string, int32_t> PeakRound;
+  std::unordered_map<std::string, int64_t> DomPeak;               // per node or NodeHierarchy name
+  std::unordered_map<std::string, int32_t> DomPeakRound;
+  std::unordered_map<std::string, int32_t> PartMinCopies, PartNoTop, PartFlags;   // per partition; flags: bit m = metric m
+  float KernelMs = 0.f;
+};
+
+ExposureResult OrchestrateExposure(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
+                                   const PartitionMap& begMap, const PartitionMap& endMap,
+                                   const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy);
+
 // ---------------------------------------------------------------------------------
 // The interning layer, exposed so that tests can drive the SAME tables through the
 // CPU oracle and compare array for array.

@@ -277,6 +277,25 @@ PYBIND11_MODULE(_host, m) {
     return out;
   });
 
+  m.def("OrchestrateExposure", [](const PyModel& model, int max_concurrent, bool favor, const Strs& nodes_all,
+                                  const PyPartitionMap& beg, const PyPartitionMap& end, const std::optional<StrMap>& nh) {
+    OrchestratorOptions o;
+    o.MaxConcurrentPartitionMovesPerNode = max_concurrent;
+    o.FavorMinNodes = favor;
+    const PartitionMap b = to_map(beg), e = to_map(end);
+    ExposureResult r;
+    {
+      py::gil_scoped_release rel;
+      r = OrchestrateExposure(to_model(model), o, nodes_all, b, e, nh);
+    }
+    py::dict d;
+    d["rounds"] = r.Rounds; d["series"] = r.Series; d["peak"] = r.Peak; d["peak_round"] = r.PeakRound; d["area"] = r.Area;
+    d["dom_peak"] = r.DomPeak; d["dom_peak_round"] = r.DomPeakRound; d["part_min_copies"] = r.PartMinCopies;
+    d["part_no_top"] = r.PartNoTop; d["part_flags"] = r.PartFlags; d["kernel_ms"] = r.KernelMs;
+    return d;
+  }, py::arg("model"), py::arg("max_concurrent"), py::arg("favor"), py::arg("nodes_all"), py::arg("beg"), py::arg("end"),
+     py::arg("node_hierarchy") = py::none());
+
   py::class_<PyInterned>(m, "InternedPlan")
       .def_property_readonly("in_ptr", [](const PyInterned& s) { return (uintptr_t)&s.ip->in; })
       .def_property_readonly("n_nodes", [](const PyInterned& s) { return s.ip->in.n_nodes; })

@@ -295,6 +295,7 @@ class Context:
         """device_ids (a list) creates a multi-GPU context: batches are sharded over those devices."""
         self.lib = api.capi()
         self.ptr = ctypes.c_void_p()
+        self._rounds = {}                     # moves handle -> R of its last moves_schedule
         if device_ids is not None:
             arr = (ctypes.c_int * len(device_ids))(*device_ids)
             st = self.lib.blance_ctx_create_multi(ctypes.byref(self.ptr), arr, len(device_ids))
@@ -560,10 +561,49 @@ class Context:
         sched_op = np.zeros(max(1, out.moves_done), np.int64)
         self._check(self.lib.blance_moves_schedule_fetch(self.ptr, h, round_off.ctypes.data, sched_op.ctypes.data),
                     "blance_moves_schedule_fetch")
+        self._rounds[h.value] = out.rounds        # sizes moves_exposure's series
         scalars = {f: getattr(out, f) for f, _ in api.ScheduleOut._fields_}
         return round_off, sched_op[:out.moves_done], scalars
 
+    def moves_exposure(self, handle, constraints, top_state, domain_parent=None, dom=True):
+        """blance_moves_exposure: the maps the handle's last moves_schedule passes through, counted per round
+        (include/blance_b200.h); its R sizes the series.  Returns a dict:
+        series [6][R + 1], peak / peak_round / area [6] (abi.EXPO_METRICS order), dom_peak / dom_peak_round [V],
+        part_min_copies / part_no_top / part_flags [n_parts], rounds and kernel_ms.  dom=False asks for no dom_peak
+        (its arrays are then zero)."""
+        h, n_parts, n_node_ids = handle
+        keep = []
+        cons = np.ascontiguousarray(constraints, np.int32)
+        e_in = api.ExposureIn(cons.ctypes.data if cons.size else None, int(top_state), 0, None)
+        V = n_node_ids
+        if domain_parent is not None:
+            par = np.ascontiguousarray(domain_parent, np.int32)
+            keep.append(par)
+            e_in.n_domains = par.size - n_node_ids
+            e_in.domain_parent = par.ctypes.data
+            V = par.size
+        rounds = self._rounds.get(h.value)
+        if rounds is None:                      # not scheduled through this context: the library refuses the handle
+            self._check(self.lib.blance_moves_exposure(self.ptr, h, ctypes.byref(e_in), ctypes.byref(api.ExposureOut())),
+                        "blance_moves_exposure")
+            raise ValueError("schedule the handle with moves_schedule before moves_exposure")
+        res = dict(series=np.zeros((6, rounds + 1), np.int64), dom_peak=np.zeros(max(1, V), np.int64),
+                   dom_peak_round=np.zeros(max(1, V), np.int32), part_min_copies=np.zeros(max(1, n_parts), np.int32),
+                   part_no_top=np.zeros(max(1, n_parts), np.int32), part_flags=np.zeros(max(1, n_parts), np.uint8))
+        out = api.ExposureOut()
+        for k, a in res.items():
+            setattr(out, k, a.ctypes.data if dom or not k.startswith("dom") else None)
+        self._check(self.lib.blance_moves_exposure(self.ptr, h, ctypes.byref(e_in), ctypes.byref(out)), "blance_moves_exposure")
+        for k in ("dom_peak", "dom_peak_round"):
+            res[k] = res[k][:V]
+        for k in ("part_min_copies", "part_no_top", "part_flags"):
+            res[k] = res[k][:n_parts]
+        res.update(rounds=out.rounds, kernel_ms=out.kernel_ms, peak=np.array(out.peak[:], np.int64),
+                   peak_round=np.array(out.peak_round[:], np.int32), area=np.array(out.area[:], np.int64))
+        return res
+
     def moves_free(self, handle):
+        self._rounds.pop(handle[0].value, None)
         self.lib.blance_moves_free(self.ptr, handle[0])
 
     def kernel_launches(self):

@@ -560,7 +560,8 @@ typedef struct blance_moves blance_moves;
 
 /* beg_rows / end_rows / state_slot_off / n_visit_states / favor_min_nodes as in blance_calc_partition_moves.
  * n_node_ids bounds the node ids that occur in the rows.  *total_ops receives the number of ops of all
- * partitions together (the size of the op_* arrays blance_moves_fetch fills). */
+ * partitions together (the size of the op_* arrays blance_moves_fetch fills).  The handle also keeps the beg rows and
+ * the slot layout on the device, for blance_moves_exposure. */
 int blance_moves_create(blance_ctx* ctx, int32_t n_parts, int32_t n_states, int32_t n_visit_states,
                         const int32_t* state_slot_off, const int32_t* beg_rows, const int32_t* end_rows,
                         int32_t favor_min_nodes, int32_t n_node_ids, blance_moves** out, int64_t* total_ops);
@@ -616,6 +617,85 @@ typedef struct blance_schedule_out {
 int blance_moves_schedule(blance_ctx* ctx, blance_moves* moves, int32_t max_concurrent_per_node,
                           const uint8_t* node_has_mover, blance_schedule_out* out);
 int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* moves, int64_t* round_off, int64_t* sched_op);
+
+/* ---- the exposure of a rebalance (blance_moves_exposure) ---------------------------------------------------
+ * Is the data safe while a rebalance runs?  favorMinNodes (moves.go:35-40) trades "the least number of nodes at any
+ * time" against "availability across multiple nodes during moves": a primary moving from a to b is del a, add b
+ * (no copy in between) with favor_min_nodes, add b, del a (two primaries in between) without.  The exposure counts
+ * that cost over the maps a rebalance passes through under the handle's LAST blance_moves_schedule (R rounds,
+ * round_off, sched_op), on the device, without copying the schedule or any map out.
+ *
+ * Maps.  For t = 0 .. R, M_t is the map after t completed rounds.  M_0 is the handle's beg rows.  Partition p's ops
+ * are applied in CSR order; op k is applied at the end of the round rho_k that scheduled it, so it is in M_t for
+ * t > rho_k.  An op that was never scheduled (a stuck partition's remaining ops) is never applied.  Applying op
+ * (node n, state s, kind) is what the reference's test app does with an AssignPartitionsFunc call
+ * (orchestrate_test.go:137-157; orchestrate.go:143-152): every entry of n leaves the partition's lists and, unless the
+ * kind is BLANCE_OP_DEL (state ""), one entry (n, s) is added.
+ * Entries.  A partition's entries are its (state, position) entries as the move lists read a row: the slots of a
+ * state before its first BLANCE_NO_NODE.  A node listed twice in a beg row counts twice until its op.  CalcPartitionMoves'
+ * seen rule (moves.go:51-58) gives a node at most one op per partition, so when its op runs a node's entries are
+ * exactly its beg entries.  rho_k strictly increases along a partition's ops, so each of its intermediate states is
+ * some M_t: per-partition results are exact over the op sequence; only the coincidence across partitions depends on
+ * the lock-step model.
+ *
+ * For partition p in M_t with c_s entries of state s and C = sum_s c_s, metric m (enum blance_expo_metric) counts:
+ *   NO_TOP     top_state >= 0 and c_top = 0 (no primary)
+ *   MULTI_TOP  top_state >= 0, state_constraints[top] > 0 and c_top > state_constraints[top]
+ *   SHORT      some s has state_constraints[s] > 0 and c_s < state_constraints[s]
+ *   ONE_COPY   C = 1
+ *   NO_COPY    C = 0
+ *   COPIES     (not a count of partitions) sum_p C
+ *
+ * Inputs: state_constraints[n_states] (0 = not constrained; use 0 for states outside the model), top_state (-1 for
+ * none), and optionally a fault-domain forest with the meaning and checks of blance_audit_opts (V = n_node_ids +
+ * n_domains; NULL: every node is its own domain).
+ * Outputs (every array may be NULL):
+ *   rounds                     R, echoed
+ *   series[m][R + 1]           metric m on M_t
+ *   peak[m], peak_round[m]     its largest value and the smallest t that reaches it;  area[m] = sum_t series[m][t]
+ *   dom_peak[V]                max over t of the partitions with C >= 1 whose every entry lies on a node under v in M_t
+ *                              (an entry on an id outside [0, n_node_ids) lies under no vertex); without a forest,
+ *                              dom_peak[q] is the most partitions node q alone held at any moment of the rebalance
+ *   dom_peak_round[V]          the smallest t at which dom_peak[v] is reached
+ *   part_min_copies[n_parts]   min over t of C;   part_no_top[n_parts]  number of t in 0 .. R at which NO_TOP holds
+ *   part_flags[n_parts]        bit m: the partition is counted in metric m at some t (bit COPIES: C > 0 at some t)
+ *   kernel_ms                  GPU time of the exposure (events around its device work)
+ * Every value equals a literal replay of the schedule; nothing depends on thread order.
+ *
+ * Errors, before any device work: a NULL ctx, moves, in or out, a handle without a schedule, NULL constraints with
+ * states, a negative constraint, top_state outside [-1, n_states), a bad forest (as blance_map_audit)
+ * (BLANCE_ERR_INVALID_ARG); more than 8 states or 32 slots, or dom_peak / dom_peak_round asked for with
+ * 2 x 17 x moves_done >= 2^31 (BLANCE_ERR_UNSUPPORTED).  The device work is bounded by the handle's sizes plus, with
+ * dom_peak, an event buffer of at most 2 x 17 entries per scheduled op (DESIGN.md section 13); BLANCE_ERR_NOMEM when
+ * that does not fit.  The C++ twin over string maps is OrchestrateExposure (blance_b200/csrc/host_api.hpp). */
+enum blance_expo_metric {
+  BLANCE_EXPO_NO_TOP = 0, BLANCE_EXPO_MULTI_TOP = 1, BLANCE_EXPO_SHORT = 2, BLANCE_EXPO_ONE_COPY = 3,
+  BLANCE_EXPO_NO_COPY = 4, BLANCE_EXPO_COPIES = 5, BLANCE_EXPO_N = 6
+};
+
+typedef struct blance_exposure_in {
+  const int32_t* state_constraints;   /* [n_states] of the handle */
+  int32_t top_state;                  /* -1: none */
+  int32_t n_domains;                  /* inner vertices of the forest; 0 when domain_parent is NULL */
+  const int32_t* domain_parent;       /* [n_node_ids + n_domains] or NULL */
+} blance_exposure_in;
+
+typedef struct blance_exposure_out {
+  int32_t rounds;
+  int64_t* series;                    /* [BLANCE_EXPO_N][rounds + 1] */
+  int64_t peak[BLANCE_EXPO_N];
+  int32_t peak_round[BLANCE_EXPO_N];
+  int64_t area[BLANCE_EXPO_N];
+  int64_t* dom_peak;                  /* [V] */
+  int32_t* dom_peak_round;            /* [V] */
+  int32_t* part_min_copies;           /* [n_parts] */
+  int32_t* part_no_top;               /* [n_parts] */
+  uint8_t* part_flags;                /* [n_parts] */
+  float kernel_ms;
+} blance_exposure_out;
+
+int blance_moves_exposure(blance_ctx* ctx, blance_moves* moves, const blance_exposure_in* in, blance_exposure_out* out);
+
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
 #ifdef __cplusplus
