@@ -107,7 +107,7 @@ def _option_kwargs(o):
 
 
 def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=None, scenarios=(), favorMinNodes=False,
-                         wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None):
+                         wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None, exposure=None):
     """What-if variants of one cluster, planned side by side on the device.  Scenario i is
     PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, sc["nodesToRemove"], sc["nodesToAdd"], model, options with
     the scenario's plan options substituted): both node-set keys are required (None = nil).  The optional keys
@@ -129,14 +129,21 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
     audit (None = no audit, exactly the results above; or a dict with the optional key "failoverSpread") adds an
     "audit" dict to every result: AuditMap of that scenario's final map (prevMap with every assigned partition
     replaced by its next row) under the scenario's own constraints and hierarchy rules, computed inside the sweep
-    without copying the map out.  The fault domains are the options' NodeHierarchy for every scenario."""
+    without copying the map out.  The fault domains are the options' NodeHierarchy for every scenario.
+
+    exposure (None = none; or a dict with the optional key "seriesCap", default 0) needs scheduleConcurrency and adds
+    an "exposures" list to every result, one dict per value, shaped as OrchestrateExposure's: the exposure of that
+    scenario's rebalance (begMap = prevMap plus an empty entry for every assigned partition it lacks, endMap = the
+    final map) under the scenario's own constraints, with the options' NodeHierarchy as the fault domains.  "series"
+    holds the first min(rounds + 1, seriesCap) values per metric; rounds, peak, peak_round and area are complete."""
     o = options or PlanNextMapOptions()
     same = prevMap is partitionsToAssign
     return _host.PlanNextMapScenarios(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                       {k: tuple(v) for k, v in model.items()}, _scenario_tuples(scenarios),
                                       bool(favorMinNodes), [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o),
                                       schedule_concurrency=[int(c) for c in scheduleConcurrency],
-                                      audit=None if audit is None else bool(audit.get("failoverSpread", False)))
+                                      audit=None if audit is None else bool(audit.get("failoverSpread", False)),
+                                      exposure_series_cap=None if exposure is None else int(exposure.get("seriesCap", 0)))
 
 
 def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None, chains=(), favorMinNodes=False,

@@ -108,7 +108,7 @@ struct blance_ctx {
   void* cub_tmp = nullptr;
   size_t cub_tmp_bytes = 0;
   std::vector<cudaEvent_t> events;   // pool for pass timing
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [4], [5]: around the audit kernels
+  cudaEvent_t ev[8] = {};            // [4], [5]: around the audit kernels; [6], [7]: around a wave's exposures
   int* d_any_active = nullptr;
   int* h_any_active = nullptr;       // pinned
   long long launches = 0;            // kernels of this library launched so far
@@ -1493,6 +1493,185 @@ static void audit_unpack(blance_ctx* ctx, const AuditBufs& b, int n_rules, const
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// The exposure of a schedule (exposure.cuh; include/blance_b200.h): one engine for a moves handle and a wave.
+
+// The exposures requested with blance_plan_scenarios_exposure: the checked forest, the series cap and the caller's
+// outputs [n][nc]; which optional outputs any of them asks for.
+struct ExpoReq {
+  int n_domains = 0;
+  const int32_t* parent = nullptr;     // host, [n_node_ids + n_domains] or NULL
+  int32_t series_cap = 0;
+  blance_exposure_out* out = nullptr;
+  bool dom = false, part_min = false, part_notop = false, part_flags = false;
+};
+
+// The device buffers of the exposures of nw scenarios x nc counts that are priced into a wave: the op table's
+// states and rounds (in w), the per-partition outputs asked for and, for dom peaks, the forest, the per-vertex
+// counts and the per-(instance, partition) event counts and offsets.  PU partitions, MO ops each, V vertices.
+struct ExpoBufs {
+  ExpoArgs E{};
+  unsigned long long* dom_key = nullptr;
+  long long* ev_off = nullptr;
+  int32_t* parent = nullptr;
+};
+
+static void expo_slices(Arena& a, ExpoBufs& b, WSched& w, const ExpoReq& er, long long nw, long long nc, long long PU,
+                        long long MO, long long V) {
+  const long long ni = nw * nc;
+  a.add(w.op_state, (size_t)std::max(1ll, nw * PU * MO)); a.add(w.op_round, (size_t)std::max(1ll, ni * PU * MO));
+  if (er.part_min) a.add(b.E.part_min, (size_t)(ni * PU));
+  if (er.part_notop) a.add(b.E.part_notop, (size_t)(ni * PU));
+  if (er.part_flags) a.add(b.E.part_flags, (size_t)(ni * PU));
+  if (er.dom) {
+    if (er.parent) a.add(b.parent, (size_t)V);
+    a.add(b.E.dom_base, (size_t)(ni * V)); a.add(b.dom_key, (size_t)(ni * V));
+    a.add(b.E.ev_count, (size_t)(ni * PU + 1)); a.add(b.ev_off, (size_t)(ni * PU + 1));
+  }
+}
+
+// What expo_run leaves: the buffers it allocated (alive until the caller has copied out), the statistics
+// [ni][BLANCE_EXPO_N] x {peak, peak round, area} and the device bytes it allocated.
+struct ExpoResult {
+  std::unique_ptr<Arena> res, ev;
+  std::vector<long long> stats;
+  size_t bytes = 0;
+};
+
+// Runs the exposures of the instances h_inst (R and constraints set by the caller, offsets set here) on E, whose op
+// source, op rounds, rows, flags, sizes, per-partition outputs and - with dom_key - forest, dom_base, ev_count and
+// ev_off the caller set.  The diff slices (E.diff then holds the series), the statistics and the fault-domain event
+// buffers are allocated here, exactly sized.  Fault-domain events are sorted in groups of consecutive instances: g
+// instances form a group when g x V < 2^32, its events number fewer than 2^31 and fit in the free memory.
+static ExpoResult expo_run(blance_ctx* dev, ExpoArgs& E, std::vector<ExpoInst>& h_inst, unsigned long long* dom_key, long long* ev_off) {
+  cudaStream_t st = dev->stream;
+  const long long ni = (long long)h_inst.size(), P = E.P, V = E.V;
+  ExpoResult out;
+  long long n_diff = 0;
+  for (ExpoInst& I : h_inst) { I.diff_off = n_diff; n_diff += BLANCE_EXPO_N * ((long long)I.R + 1); }
+  ExpoInst* d_inst = nullptr;
+  long long* stats = nullptr;
+  void* tmp = nullptr;
+  size_t scan_tmp = 0;
+  if (dom_key) CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const long long*)nullptr, (long long*)nullptr, ni * P + 1, st));
+  out.res.reset(new Arena());
+  out.res->add(d_inst, (size_t)ni); out.res->add(E.diff, (size_t)n_diff); out.res->add(stats, (size_t)(ni * 3 * BLANCE_EXPO_N));
+  if (dom_key) out.res->add(tmp, scan_tmp);
+  out.res->alloc(st, "the exposure");
+  out.bytes = out.res->bytes();
+  E.inst = d_inst;
+  CUDA(cudaMemcpyAsync(d_inst, h_inst.data(), sizeof(ExpoInst) * (size_t)ni, cudaMemcpyHostToDevice, st));
+  CUDA(cudaMemsetAsync(E.diff, 0, sizeof(long long) * (size_t)n_diff, st));
+  if (dom_key && V > 0) CUDA(cudaMemsetAsync(E.dom_base, 0, sizeof(long long) * (size_t)(ni * V), st));
+  // instances i0 .. i0 + n - 1, at most 65535 per launch (grid y)
+  auto walk = [&](void (*kernel)(const ExpoArgs), long long i0, long long n) {
+    for (long long y = 0; y < n; y += 65535) {
+      ExpoArgs A = E;
+      A.i0 = (int32_t)(i0 + y);
+      const long long ny = std::min(65535ll, n - y);
+      const int bx = (int)std::max(1ll, std::min((P + 255) / 256, std::max(1ll, (long long)dev->sm_count * 8 / ny)));
+      launch(dev, kernel, dim3((unsigned)bx, (unsigned)ny), 256, 0, A);
+    }
+  };
+  if (P > 0) walk(k_expo_walk<0>, 0, ni);
+  for (long long y = 0; y < ni; y += 65535)
+    launch(dev, k_expo_series, dim3(BLANCE_EXPO_N, (unsigned)std::min(65535ll, ni - y)), 512, 0, (const ExpoInst*)(d_inst + y), E.diff,
+           stats + y * 3 * BLANCE_EXPO_N);
+  // fault domains: (vertex, t, +-1) events where a partition's deepest common ancestor changes, sized exactly by a
+  // counting walk, sorted by (instance, vertex, t), merged per key, scanned per (instance, vertex); dom_key keeps each
+  // vertex's maximum
+  if (dom_key && V > 0) {
+    launch(dev, k_expo_dom_init, grid_for(dev, ni * V, 256), 256, 0, ni * V, (const long long*)E.dom_base, dom_key);
+    std::vector<long long> first((size_t)ni + 1, 0);     // ev_off at each instance's first partition, and the total
+    if (P > 0) {
+      CUDA(cudaMemsetAsync(E.ev_count + ni * P, 0, sizeof(long long), st));
+      walk(k_expo_walk<1>, 0, ni);
+      CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, E.ev_count, ev_off, ni * P + 1, st));
+      CUDA(cudaMemcpy2DAsync(first.data(), sizeof(long long), ev_off, sizeof(long long) * (size_t)P, sizeof(long long), (size_t)ni + 1,
+                             cudaMemcpyDeviceToHost, st));
+      CUDA(cudaStreamSynchronize(st));
+      E.ev_off = ev_off;
+    }
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
+    const size_t headroom = std::max<size_t>(1ull << 30, total_b / 16);
+    // bytes per event: keys and values in, sorted, merged, and the running sums (the sorts' scratch is extra)
+    const long long per_ev = 2 * 8 + 3 * 4 + 8 + 4, fit = std::max(1ll, (long long)((free_b > headroom ? free_b - headroom : 0) / (2 * per_ev)));
+    std::vector<std::pair<long long, long long>> groups;  // [g0, g1)
+    long long max_ne = 0;
+    for (long long g0 = 0; g0 < ni;) {
+      long long g1 = g0 + 1;
+      while (g1 < ni && (g1 + 1 - g0) * V < (1ll << 32) && first[(size_t)g1 + 1] - first[(size_t)g0] < std::min(fit, 1ll << 31)) ++g1;
+      if (first[(size_t)g1] - first[(size_t)g0] >= (1ll << 31))
+        throw_err(BLANCE_ERR_UNSUPPORTED, "the exposure: 2^31 or more fault-domain events in one instance (internal error)");
+      groups.emplace_back(g0, g1);
+      max_ne = std::max(max_ne, first[(size_t)g1] - first[(size_t)g0]);
+      g0 = g1;
+    }
+    if (max_ne > 0) {
+      const int NE = (int)max_ne;
+      long long max_key = 0;
+      for (auto& g : groups) max_key = std::max(max_key, (g.second - g.first) * V);
+      int vbits = 1;
+      while ((1ll << vbits) < max_key) ++vbits;
+      unsigned long long *k2, *uk;
+      int32_t *v2, *uv, *run;
+      int* n_runs;
+      size_t sort_b = 0, red_b = 0, scan_b = 0;
+      CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                           (const int32_t*)nullptr, (int32_t*)nullptr, NE, 0, 32 + vbits, st));
+      CUDA(cub::DeviceReduce::ReduceByKey(nullptr, red_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                          (const int32_t*)nullptr, (int32_t*)nullptr, (int*)nullptr, ExpoSum(), NE, st));
+      CUDA(cub::DeviceScan::InclusiveScanByKey(nullptr, scan_b, (const unsigned long long*)nullptr, (const int32_t*)nullptr,
+                                               (int32_t*)nullptr, ExpoSum(), NE, ExpoSameVertex(), st));
+      const size_t ev_tmp_b = std::max(sort_b, std::max(red_b, scan_b));
+      void* ev_tmp = nullptr;
+      out.ev.reset(new Arena());
+      out.ev->add(E.ev_key, (size_t)NE); out.ev->add(E.ev_val, (size_t)NE); out.ev->add(k2, (size_t)NE); out.ev->add(v2, (size_t)NE);
+      out.ev->add(uk, (size_t)NE); out.ev->add(uv, (size_t)NE); out.ev->add(run, (size_t)NE); out.ev->add(n_runs, 1); out.ev->add(ev_tmp, ev_tmp_b);
+      out.ev->alloc(st, "the exposure's fault-domain events");
+      out.bytes += out.ev->bytes();
+      for (auto& g : groups) {
+        const int ne = (int)(first[(size_t)g.second] - first[(size_t)g.first]);
+        if (ne == 0) continue;
+        E.ev0 = first[(size_t)g.first];
+        E.g0 = (int32_t)g.first;          // the keys' instance origin; walk() splits the group into launches of 65535
+        walk(k_expo_walk<2>, g.first, g.second - g.first);
+        size_t b = ev_tmp_b;
+        CUDA(cub::DeviceRadixSort::SortPairs(ev_tmp, b, E.ev_key, k2, E.ev_val, v2, ne, 0, 32 + vbits, st));
+        b = ev_tmp_b;
+        CUDA(cub::DeviceReduce::ReduceByKey(ev_tmp, b, k2, uk, v2, uv, n_runs, ExpoSum(), ne, st));
+        int h_runs = 0;                          // only the merged runs are scanned
+        CUDA(cudaMemcpyAsync(&h_runs, n_runs, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CUDA(cudaStreamSynchronize(st));
+        b = ev_tmp_b;
+        CUDA(cub::DeviceScan::InclusiveScanByKey(ev_tmp, b, uk, uv, run, ExpoSum(), h_runs, ExpoSameVertex(), st));
+        launch(dev, k_expo_dom_max, grid_for(dev, h_runs, 256), 256, 0, h_runs, (const unsigned long long*)uk, (const int32_t*)run,
+               (const long long*)(E.dom_base + g.first * V), dom_key + g.first * V);
+      }
+    }
+  }
+  out.stats.assign((size_t)(ni * 3 * BLANCE_EXPO_N), 0);
+  CUDA(cudaMemcpyAsync(out.stats.data(), stats, sizeof(long long) * out.stats.size(), cudaMemcpyDeviceToHost, st));
+  return out;
+}
+
+// The scalars of instance i of r into o, after the stream was synchronised (dom_key: the host copy of the instance's
+// [V] keys, or NULL).
+static void expo_unpack(const ExpoResult& r, long long i, int R, const unsigned long long* dom_key, int V, blance_exposure_out& o) {
+  o.rounds = R;
+  const long long* s = r.stats.data() + i * 3 * BLANCE_EXPO_N;
+  for (int m = 0; m < BLANCE_EXPO_N; ++m) {
+    o.peak[m] = s[3 * m];
+    o.peak_round[m] = (int32_t)s[3 * m + 1];
+    o.area[m] = s[3 * m + 2];
+  }
+  for (int v = 0; dom_key && v < V; ++v) {
+    if (o.dom_peak) o.dom_peak[v] = (int64_t)(dom_key[v] >> 32);
+    if (o.dom_peak_round) o.dom_peak_round[v] = (int32_t)(0xFFFFFFFFu - (uint32_t)dom_key[v]);
+  }
+}
+
 // The chains requested with blance_plan_chains: T stages per chain, stages [n][T], net [n] or NULL.
 struct ChainReq {
   int T = 1;
@@ -1558,11 +1737,63 @@ static void wave_summary(blance_ctx* ctx, blance_plan* pl, int nw, const int32_t
   else launch(ctx, k_scenario_summary<false>, grid, 256, 0, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
 }
 
+// The exposures of a wave's nw scenarios x nc counts after their schedules (scal: the instances' scalars), on the
+// op table and rounds the schedule left in W and the buffers of b; wave member j is scenario idx[j].  Copies every
+// result out into er.out; *ms and *bytes: the device time and the bytes allocated after the schedule.
+static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan* pl, int nw, int nc, const int* idx,
+                          const blance_plan_in& base, const WSched& W, ExpoBufs& b, const std::vector<unsigned long long>& scal,
+                          float* ms, size_t* bytes) {
+  cudaStream_t st = ctx->stream;
+  const int PU = base.n_parts, S = base.n_states;
+  const long long ni = (long long)nw * nc, V = (long long)base.n_node_ids + er.n_domains;
+  ExpoArgs& E = b.E;
+  E.op_off = nullptr; E.op_n = W.op_n; E.op_node = W.op_node; E.op_state = W.op_state; E.op_kind = W.op_kind; E.op_round = W.op_round;
+  E.beg = pl->prev_rows_init; E.pflags = pl->pflags_init; E.dom_parent = b.parent;
+  E.stride = pl->h_insts[0].SLP; E.P = PU; E.SL = base.n_slots; E.S = S; E.NU = base.n_node_ids; E.V = (int32_t)V;
+  E.MO = W.MO; E.top = base.top_state;
+  for (int s = 0; s <= S; ++s) E.slot_off[s] = base.state_slot_off[s];
+  std::vector<ExpoInst> inst((size_t)ni, ExpoInst{});
+  for (long long i = 0; i < ni; ++i) {
+    const long long j = i / nc;
+    const DInst& D = pl->h_insts[(size_t)j];
+    ExpoInst& I = inst[(size_t)i];
+    I.beg_off = D.rows_off; I.pf_off = D.part_off; I.gp_off = j * PU;
+    I.R = (int32_t)scal[(size_t)(4 * i)];
+    for (int s = 0; s < S; ++s) I.constraints[s] = D.state_constraints[s];
+  }
+  CUDA(cudaEventRecord(ctx->ev[6], st));
+  const ExpoResult r = expo_run(ctx, E, inst, er.dom ? b.dom_key : nullptr, b.ev_off);
+  CUDA(cudaEventRecord(ctx->ev[7], st));
+  std::vector<unsigned long long> h_key(er.dom ? (size_t)(ni * V) : 0);
+  if (!h_key.empty()) CUDA(cudaMemcpyAsync(h_key.data(), b.dom_key, sizeof(unsigned long long) * h_key.size(), cudaMemcpyDeviceToHost, st));
+  for (long long i = 0; i < ni; ++i) {
+    blance_exposure_out& o = er.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    const long long R1 = (long long)inst[(size_t)i].R + 1, w = std::min<long long>(R1, er.series_cap);
+    if (o.series && w > 0)        // [BLANCE_EXPO_N][series_cap] <- the first w of each metric's R + 1 values
+      CUDA(cudaMemcpy2DAsync(o.series, sizeof(int64_t) * (size_t)er.series_cap, E.diff + inst[(size_t)i].diff_off, sizeof(long long) * (size_t)R1,
+                             sizeof(long long) * (size_t)w, BLANCE_EXPO_N, cudaMemcpyDeviceToHost, st));
+    if (PU > 0) {
+      if (o.part_min_copies && E.part_min) CUDA(cudaMemcpyAsync(o.part_min_copies, E.part_min + i * PU, sizeof(int32_t) * (size_t)PU, cudaMemcpyDeviceToHost, st));
+      if (o.part_no_top && E.part_notop) CUDA(cudaMemcpyAsync(o.part_no_top, E.part_notop + i * PU, sizeof(int32_t) * (size_t)PU, cudaMemcpyDeviceToHost, st));
+      if (o.part_flags && E.part_flags) CUDA(cudaMemcpyAsync(o.part_flags, E.part_flags + i * PU, (size_t)PU, cudaMemcpyDeviceToHost, st));
+    }
+  }
+  CUDA(cudaStreamSynchronize(st));
+  *ms = 0.f;
+  cudaEventElapsedTime(ms, ctx->ev[6], ctx->ev[7]);
+  *bytes = r.bytes;
+  for (long long i = 0; i < ni; ++i) {
+    blance_exposure_out& o = er.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    expo_unpack(r, i, inst[(size_t)i].R, er.dom ? h_key.data() + i * V : nullptr, (int)V, o);
+    o.kernel_ms = *ms;
+  }
+}
+
 // Plans the scenarios idx (of sc / opts) on one device, in waves.  With cr each is a chain of cr->T stages, planned
 // in lock step: a stage boundary is an iteration boundary plus the next stage's node tables (DESIGN.md section 12).
 static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
                                 const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
-                                const SchedReq* sr, const AuditReq* ar, const ChainReq* cr = nullptr) {
+                                const SchedReq* sr, const AuditReq* ar, const ChainReq* cr = nullptr, const ExpoReq* er = nullptr) {
   cudaStream_t st = ctx->stream;
   const int n_dev = (int)idx.size();
   const int T = cr ? cr->T : 1;
@@ -1585,6 +1816,14 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     AuditBufs b;
     audit_slices(one, b, *ar, 1, base->n_states, max_rules, base->n_node_ids, base->n_nodes, base->n_parts, audit_flags);
     extra_bytes = one.bytes();
+  }
+  const long long V = (long long)base->n_node_ids + (er ? er->n_domains : 0);
+  if (er) {                            // one scenario's exposure buffers: op states and rounds, outputs asked for
+    Arena one;
+    ExpoBufs b;
+    WSched w{};
+    expo_slices(one, b, w, *er, 1, sr->nc, base->n_parts, scenario_ops(*base), V);
+    extra_bytes += one.bytes();
   }
   {
     cudaMemPool_t pool;                // measure free memory without this context's cached arenas
@@ -1653,6 +1892,8 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     if (!ow.empty()) wave.add(d_ow, ow.size());
     AuditBufs abuf;
     if (ar) audit_slices(wave, abuf, *ar, nw, S, max_rules, NU, base->n_nodes, PU, audit_flags);
+    ExpoBufs ebuf;
+    if (er) expo_slices(wave, ebuf, wsch, *er, nw, sr->nc, PU, scenario_ops(*base), V);
     int32_t* net_prev = nullptr;
     uint8_t* net_flags = nullptr;
     long long* d_net = nullptr;
@@ -1764,8 +2005,14 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
         o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
         if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
       }
+      float expo_ms = 0.f;
+      size_t expo_bytes = 0;
       if (sr) {
         CUDA(cudaEventRecord(ctx->ev[3], st));
+        if (er) {
+          CUDA(cudaMemsetAsync(wsch.op_round, 0xFF, sizeof(int32_t) * (size_t)nw * sr->nc * PU * scenario_ops(*base), st));
+          if (ebuf.parent) CUDA(cudaMemcpyAsync(ebuf.parent, er->parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
+        }
         if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, wsch);
         std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
         for (size_t x = 0; x < ops.size(); ++x) {
@@ -1786,6 +2033,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
         CUDA(cudaEventRecord(ctx->ev[1], st));
         CUDA(cudaEventSynchronize(ctx->ev[1]));
         cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
+        if (er) wave_exposure(ctx, *er, pl, nw, sr->nc, idx.data() + w0, *base, wsch, ebuf, scal, &expo_ms, &expo_bytes);
       }
       if (times) {
         float wave_ms = 0.f;
@@ -1793,6 +2041,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
         std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
                      w0, nw, W, per, wave_ms, sum_ms);
         if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
+        if (er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", expo_ms, expo_bytes);
         std::fprintf(stderr, "\n");
       }
     }
@@ -1830,7 +2079,7 @@ static int check_scenario(const blance_plan_in& base, const blance_scenario& sc,
 
 static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                            const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
-                           const SchedReq* sr = nullptr, const AuditReq* ar = nullptr) {
+                           const SchedReq* sr = nullptr, const AuditReq* ar = nullptr, const ExpoReq* er = nullptr) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
   if (!base || !sc || !out) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
   // every scenario is checked before the context is used, so a NULL ctx checks the scenarios without a device
@@ -1846,7 +2095,7 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
   fan_out(ctx, G, [&](int d, blance_ctx* dev) {
-    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr, ar);
+    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr, ar, nullptr, er);
   });
 }
 
@@ -1965,6 +2214,52 @@ extern "C" int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in
       }
     need_ctx(ctx);
     plan_scenarios(ctx, name.c_str(), base, n, sc, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, &ar);
+  });
+}
+
+extern "C" int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                              const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                              int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                              blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                                              const blance_audit_opts* aopts, blance_audit_out* audit,
+                                              const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo) {
+  return entry(ctx, [&](Device&) {
+    const std::string name = "blance_plan_scenarios_exposure";
+    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base is NULL");
+    AuditReq ar;
+    if (audit) ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
+    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": an exposure needs a schedule: n_move_conc must be positive");
+    const SchedReq sr = sched_req(name.c_str(), base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
+    if (!expo) throw_err(BLANCE_ERR_INVALID_ARG, name + ": expo is NULL");
+    if (series_cap < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": series_cap is negative");
+    ExpoReq er;
+    er.series_cap = series_cap;
+    er.out = expo;
+    if (eopts) {
+      if (eopts->flags) throw_err(BLANCE_ERR_INVALID_ARG, name + ": eopts.flags must be 0 (eopts carries a forest only)");
+      check_forest(name, eopts->n_domains, eopts->domain_parent, base->n_node_ids);
+      er.n_domains = eopts->n_domains;
+      er.parent = eopts->domain_parent;
+    }
+    if (audit && n > 0 && sc)
+      for (int i = 0; i < n; ++i) {
+        const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
+        check_audit_model(name + ": scenario " + std::to_string(i), &in);
+      }
+    for (long long x = 0; x < (long long)std::max(0, n) * n_move_conc; ++x) {
+      const blance_exposure_out& o = expo[x];
+      er.dom |= o.dom_peak || o.dom_peak_round;
+      er.part_min |= o.part_min_copies != nullptr;
+      er.part_notop |= o.part_no_top != nullptr;
+      er.part_flags |= o.part_flags != nullptr;
+      // a scheduled op emits at most two ancestor chains of AUDIT_DEPTH_MAX + 1 vertices and a partition has at most
+      // 2 x n_slots ops: the static form of blance_moves_exposure's event bound
+      if ((o.dom_peak || o.dom_peak_round) && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base->n_slots) * std::max(0, base->n_parts) >= (1ll << 31))
+        throw_err(BLANCE_ERR_UNSUPPORTED, name + ": scenario " + std::to_string(x / n_move_conc) + ", count " + std::to_string(x % n_move_conc) +
+                                              ": dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+    }
+    // plan_scenarios checks every scenario before it looks at the context
+    plan_scenarios(ctx, name.c_str(), base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, &er);
   });
 }
 
@@ -2293,111 +2588,47 @@ extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const bl
     const long long T = mv->total_ops, M = mv->sched_moves, R1 = (long long)R + 1;
     const int V = NU + in->n_domains;
     const bool dom = out->dom_peak || out->dom_peak_round;
-    ExpoArgs E{};
+    // the one-instance, CSR case of the engine: every partition, the handle's beg rows
+    ExpoBufs b;
+    ExpoArgs& E = b.E;
     E.op_off = mv->d_off; E.op_node = mv->d_node; E.op_state = mv->d_state; E.op_kind = mv->d_kind; E.beg = mv->d_beg;
-    E.P = P; E.SL = SL; E.S = S; E.NU = NU; E.R = R; E.top = in->top_state;
-    for (int s = 0; s < S; ++s) { E.constraints[s] = in->state_constraints[s]; E.slot_off[s] = mv->slot_off[(size_t)s]; }
+    E.stride = SL; E.P = P; E.SL = SL; E.S = S; E.NU = NU; E.V = V; E.top = in->top_state;
+    for (int s = 0; s < S; ++s) E.slot_off[s] = mv->slot_off[(size_t)s];
     E.slot_off[S] = SL;
+    std::vector<ExpoInst> inst(1, ExpoInst{});
+    inst[0].R = R;
+    for (int s = 0; s < S; ++s) inst[0].constraints[s] = in->state_constraints[s];
     int32_t* op_round = nullptr;
-    long long* stats = nullptr;
-    int32_t* parent = nullptr;
-    unsigned long long* dom_key = nullptr;
-    long long* ev_off = nullptr;
-    size_t scan_tmp = 0;
-    void* tmp = nullptr;
-    CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const long long*)nullptr, (long long*)nullptr, P + 1, st));
     Arena a;
-    a.add(op_round, (size_t)std::max(T, 1ll)); a.add(E.diff, (size_t)(BLANCE_EXPO_N * R1)); a.add(stats, 3 * BLANCE_EXPO_N);
+    a.add(op_round, (size_t)std::max(T, 1ll));
     if (out->part_min_copies) a.add(E.part_min, (size_t)P);
     if (out->part_no_top) a.add(E.part_notop, (size_t)P);
     if (out->part_flags) a.add(E.part_flags, (size_t)P);
     if (dom) {
-      if (in->domain_parent) a.add(parent, (size_t)V);
-      a.add(E.dom_base, (size_t)V); a.add(dom_key, (size_t)V);
-      a.add(E.ev_count, (size_t)P + 1); a.add(ev_off, (size_t)P + 1); a.add(tmp, scan_tmp);
+      if (in->domain_parent) a.add(b.parent, (size_t)V);
+      a.add(E.dom_base, (size_t)V); a.add(b.dom_key, (size_t)V);
+      a.add(E.ev_count, (size_t)P + 1); a.add(b.ev_off, (size_t)P + 1);
     }
     a.alloc(st, "the exposure");
-    E.op_round = op_round; E.dom_parent = parent;
+    E.op_round = op_round; E.dom_parent = b.parent;
     CUDA(cudaEventRecord(dev->ev[0], st));
-    if (parent) CUDA(cudaMemcpyAsync(parent, in->domain_parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
+    if (b.parent) CUDA(cudaMemcpyAsync(b.parent, in->domain_parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
     CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(T, 1ll), st));
-    CUDA(cudaMemsetAsync(E.diff, 0, sizeof(long long) * (size_t)(BLANCE_EXPO_N * R1), st));
-    if (dom && V > 0) CUDA(cudaMemsetAsync(E.dom_base, 0, sizeof(long long) * (size_t)V, st));
     if (M > 0) launch(dev, k_expo_op_round, grid_for(dev, M, 256), 256, 0, M, R, (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
-    if (P > 0) launch(dev, k_expo_walk<0>, grid_for(dev, P, 256), 256, 0, E);
-    launch(dev, k_expo_series, BLANCE_EXPO_N, 512, 0, E.diff, R, stats);
-    // fault domains: (vertex, t, +-1) events where a partition's deepest common ancestor changes, sized exactly by a
-    // counting walk, sorted by (vertex, t), merged per key, scanned per vertex; dom_key keeps each vertex's maximum
-    std::unique_ptr<Arena> ev;
-    if (dom && V > 0) {
-      launch(dev, k_expo_dom_init, grid_for(dev, V, 256), 256, 0, V, (const long long*)E.dom_base, dom_key);
-      long long n_ev = 0;
-      if (P > 0 && M > 0) {
-        CUDA(cudaMemsetAsync(E.ev_count + P, 0, sizeof(long long), st));
-        launch(dev, k_expo_walk<1>, grid_for(dev, P, 256), 256, 0, E);
-        CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, E.ev_count, ev_off, P + 1, st));
-        CUDA(cudaMemcpyAsync(&n_ev, ev_off + P, sizeof(long long), cudaMemcpyDeviceToHost, st));
-        CUDA(cudaStreamSynchronize(st));
-        E.ev_off = ev_off;
-      }
-      if (n_ev > 0) {
-        const int NE = (int)n_ev;
-        int vbits = 1;
-        while ((1ll << vbits) < V) ++vbits;
-        unsigned long long *k2, *uk;
-        int32_t *v2, *uv, *run;
-        int* n_runs;
-        size_t sort_b = 0, red_b = 0, scan_b = 0;
-        CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                             (const int32_t*)nullptr, (int32_t*)nullptr, NE, 0, 32 + vbits, st));
-        CUDA(cub::DeviceReduce::ReduceByKey(nullptr, red_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                            (const int32_t*)nullptr, (int32_t*)nullptr, (int*)nullptr, ExpoSum(), NE, st));
-        CUDA(cub::DeviceScan::InclusiveScanByKey(nullptr, scan_b, (const unsigned long long*)nullptr, (const int32_t*)nullptr,
-                                                 (int32_t*)nullptr, ExpoSum(), NE, ExpoSameVertex(), st));
-        size_t ev_tmp_b = std::max(sort_b, std::max(red_b, scan_b));
-        void* ev_tmp = nullptr;
-        ev.reset(new Arena());
-        ev->add(E.ev_key, (size_t)NE); ev->add(E.ev_val, (size_t)NE); ev->add(k2, (size_t)NE); ev->add(v2, (size_t)NE);
-        ev->add(uk, (size_t)NE); ev->add(uv, (size_t)NE); ev->add(run, (size_t)NE); ev->add(n_runs, 1); ev->add(ev_tmp, ev_tmp_b);
-        ev->alloc(st, "the exposure's fault-domain events");
-        launch(dev, k_expo_walk<2>, grid_for(dev, P, 256), 256, 0, E);
-        size_t b = ev_tmp_b;
-        CUDA(cub::DeviceRadixSort::SortPairs(ev_tmp, b, E.ev_key, k2, E.ev_val, v2, NE, 0, 32 + vbits, st));
-        b = ev_tmp_b;
-        CUDA(cub::DeviceReduce::ReduceByKey(ev_tmp, b, k2, uk, v2, uv, n_runs, ExpoSum(), NE, st));
-        int h_runs = 0;                            // only the merged runs are scanned
-        CUDA(cudaMemcpyAsync(&h_runs, n_runs, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CUDA(cudaStreamSynchronize(st));
-        b = ev_tmp_b;
-        CUDA(cub::DeviceScan::InclusiveScanByKey(ev_tmp, b, uk, uv, run, ExpoSum(), h_runs, ExpoSameVertex(), st));
-        launch(dev, k_expo_dom_max, grid_for(dev, h_runs, 256), 256, 0, h_runs, (const unsigned long long*)uk,
-               (const int32_t*)run, (const long long*)E.dom_base, dom_key);
-      }
-    }
+    const ExpoResult r = expo_run(dev, E, inst, dom ? b.dom_key : nullptr, b.ev_off);
     CUDA(cudaEventRecord(dev->ev[1], st));
-    std::vector<long long> h_stats(3 * BLANCE_EXPO_N);
     std::vector<unsigned long long> h_key(dom ? (size_t)V : 0);
-    CUDA(cudaMemcpyAsync(h_stats.data(), stats, sizeof(long long) * h_stats.size(), cudaMemcpyDeviceToHost, st));
     if (out->series) CUDA(cudaMemcpyAsync(out->series, E.diff, sizeof(long long) * (size_t)(BLANCE_EXPO_N * R1), cudaMemcpyDeviceToHost, st));
     if (P > 0) {
       if (out->part_min_copies) CUDA(cudaMemcpyAsync(out->part_min_copies, E.part_min, sizeof(int32_t) * (size_t)P, cudaMemcpyDeviceToHost, st));
       if (out->part_no_top) CUDA(cudaMemcpyAsync(out->part_no_top, E.part_notop, sizeof(int32_t) * (size_t)P, cudaMemcpyDeviceToHost, st));
       if (out->part_flags) CUDA(cudaMemcpyAsync(out->part_flags, E.part_flags, (size_t)P, cudaMemcpyDeviceToHost, st));
     }
-    if (dom && V > 0) CUDA(cudaMemcpyAsync(h_key.data(), dom_key, sizeof(unsigned long long) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    if (dom && V > 0) CUDA(cudaMemcpyAsync(h_key.data(), b.dom_key, sizeof(unsigned long long) * (size_t)V, cudaMemcpyDeviceToHost, st));
     CUDA(cudaStreamSynchronize(st));
     out->kernel_ms = 0.f;
     cudaEventElapsedTime(&out->kernel_ms, dev->ev[0], dev->ev[1]);
-    out->rounds = R;
-    for (int m = 0; m < BLANCE_EXPO_N; ++m) {
-      out->peak[m] = h_stats[(size_t)(3 * m)];
-      out->peak_round[m] = (int32_t)h_stats[(size_t)(3 * m + 1)];
-      out->area[m] = h_stats[(size_t)(3 * m + 2)];
-    }
-    for (int v = 0; v < (dom ? V : 0); ++v) {
-      if (out->dom_peak) out->dom_peak[v] = (int64_t)(h_key[(size_t)v] >> 32);
-      if (out->dom_peak_round) out->dom_peak_round[v] = (int32_t)(0xFFFFFFFFu - (uint32_t)h_key[(size_t)v]);
-    }
+    expo_unpack(r, 0, R, dom ? h_key.data() : nullptr, V, *out);
   });
 }
 

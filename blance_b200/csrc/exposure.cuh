@@ -1,17 +1,23 @@
-// blance_b200/csrc/exposure.cuh — the exposure of a rebalance (include/blance_b200.h, blance_moves_exposure): the
-// maps M_0 .. M_R a moves handle passes through under its last lock-step schedule, counted per round without ever
-// materialising one of them.
+// blance_b200/csrc/exposure.cuh — the exposure of a rebalance (include/blance_b200.h, blance_moves_exposure and
+// blance_plan_scenarios_exposure): the maps M_0 .. M_R a schedule passes through, counted per round without ever
+// materialising one of them.  One engine serves a moves handle (one instance, CSR ops, per-op rounds from the
+// schedule's order) and a scenario wave (grid y = instance (scenario, count); ops in the wave's fixed-stride table,
+// their rounds recorded by k_wave_pick).
 //
-//   k_expo_op_round   one thread per scheduled op: op_round[sched_op[i]] = the round whose slice of sched_op holds i
+//   k_expo_op_round   one thread per scheduled op of a handle: op_round[sched_op[i]] = the round whose slice of
+//                     sched_op holds i
 //   k_expo_walk<0>    one thread per partition: its beg row and ops read once, the per-state entry counts c_s in
 //                     registers.  Each state interval [rho_{k-1} + 1, rho_k] contributes its metric values as changes
-//                     at the interval's first round into diff[metric][R + 1] (the t = 0 values warp-reduced first);
-//                     the per-partition outputs are written directly, the t = 0 fault-domain counts with REDs
-//   k_expo_series     one CTA per metric: the scan of diff into the series, its peak, first peak round and area
+//                     at the interval's first round into its instance's diff[metric][R + 1] (the t = 0 values
+//                     warp-reduced first); the per-partition outputs are written directly, the t = 0 fault-domain
+//                     counts with REDs
+//   k_expo_series     one CTA per (instance, metric): the scan of diff into the series, its peak, first peak round
+//                     and area
 //   k_expo_walk<1|2>  (fault domains only) the same walk, counting / emitting (vertex, t, +-1) events where the
 //                     partition's deepest common ancestor changes: the chains of the old and the new ancestor below
-//                     their own common ancestor.  The emitted events are radix-sorted by (vertex, t), merged per key
-//                     and scanned per vertex by the host; k_expo_dom_max takes each vertex's running maximum.
+//                     their own common ancestor.  The events of a group of instances are keyed ((g V + vertex), t)
+//                     (g the instance within the group), radix-sorted, merged per key and scanned per key vertex by
+//                     the host; k_expo_dom_max takes each vertex's running maximum.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -24,29 +30,46 @@
 
 namespace blance_dev {
 
+// One instance: a handle's schedule, or one (scenario, count) pair of a wave.
+struct ExpoInst {
+  long long beg_off;              // its beg rows: beg + beg_off + p * stride
+  long long pf_off;               // its partitions' begMap flags: pflags + pf_off + p
+  long long gp_off;               // its partitions' ops: partition gp_off + p of the op source
+  long long diff_off;             // its [BLANCE_EXPO_N][R + 1] slice of diff
+  int32_t R;
+  int32_t constraints[BL_S_MAX];
+};
+
 struct ExpoArgs {
-  const long long* op_off;        // [P + 1] CSR ops of the handle
+  const ExpoInst* inst;           // [ni]
+  const long long* op_off;        // [P + 1] CSR ops of a handle (one instance), or NULL: the table [.][MO], op_n
+  const uint8_t* op_n;
   const int32_t* op_node;
   const uint8_t* op_state;
   const uint8_t* op_kind;
-  const int32_t* op_round;        // [total_ops] round of each op, -1 = never scheduled
-  const int32_t* beg;             // [P][SL] the handle's beg rows
+  const int32_t* op_round;        // round of each op, -1 = never scheduled: CSR [total_ops] / table [ni * P][MO]
+  const int32_t* beg;             // beg rows, `stride` apart
+  const uint8_t* pflags;          // begMap membership (PF_IN_PREV | PF_IN_ASSIGN), or NULL: every partition, its row
   const int32_t* dom_parent;      // [V] or NULL (every node its own root)
-  long long* diff;                // [BLANCE_EXPO_N][R + 1] changes, scanned in place into the series
-  int32_t* part_min;              // [P] or NULL
-  int32_t* part_notop;            // [P] or NULL
-  uint8_t* part_flags;            // [P] or NULL
-  long long* dom_base;            // [V] partitions under each vertex in M_0, or NULL (no fault domains asked for)
-  long long* ev_count;            // [P + 1] events per partition (pass 1)
-  const long long* ev_off;        // [P + 1] their exclusive scan (pass 2)
-  unsigned long long* ev_key;     // (vertex << 32) | t
+  long long* diff;                // the instances' [BLANCE_EXPO_N][R + 1] changes, scanned in place into the series
+  int32_t* part_min;              // [ni][P] or NULL
+  int32_t* part_notop;            // [ni][P] or NULL
+  uint8_t* part_flags;            // [ni][P] or NULL
+  long long* dom_base;            // [ni][V] partitions under each vertex in M_0, or NULL (no fault domains asked for)
+  long long* ev_count;            // [ni * P + 1] events per (instance, partition) (pass 1)
+  const long long* ev_off;        // [ni * P + 1] their exclusive scan (pass 2), ev0 = that of the group's first
+  unsigned long long* ev_key;     // ((g V + vertex) << 32) | t, g = instance - g0
   int32_t* ev_val;                // +1 / -1
-  int32_t P, SL, S, NU, R, top;
-  int32_t constraints[BL_S_MAX], slot_off[BL_S_MAX + 1];
+  long long stride, ev0;
+  int32_t P, SL, S, NU, V, MO, top;
+  int32_t i0;                     // the launch's first instance (grid y is at most 65535 instances)
+  int32_t g0;                     // the first instance of the event group being emitted (pass 2)
+  int32_t slot_off[BL_S_MAX + 1];
 };
 
-// the metric values of one partition with entry counts c[] (enum blance_expo_metric order)
-__device__ __forceinline__ void expo_values(const ExpoArgs& E, const int (&c)[BL_S_MAX], int (&v)[BLANCE_EXPO_N]) {
+// the metric values of one partition with entry counts c[] under constraints cons[BL_S_MAX] (enum
+// blance_expo_metric order)
+__device__ __forceinline__ void expo_values(const ExpoArgs& E, const int32_t* cons, const int (&c)[BL_S_MAX], int (&v)[BLANCE_EXPO_N]) {
   int C = 0, ctop = 0, ktop = 0;
   bool is_short = false;
 #pragma unroll
@@ -54,8 +77,8 @@ __device__ __forceinline__ void expo_values(const ExpoArgs& E, const int (&c)[BL
     C += c[s];
     const int at_top = -(int)(s == E.top);          // masks, not selects: a select folds into c[top], a local-memory load
     ctop += c[s] & at_top;
-    ktop += E.constraints[s] & at_top;
-    is_short |= s < E.S && E.constraints[s] > 0 && c[s] < E.constraints[s];
+    ktop += cons[s] & at_top;
+    is_short |= s < E.S && cons[s] > 0 && c[s] < cons[s];
   }
   const bool has_top = E.top >= 0;
   v[BLANCE_EXPO_NO_TOP] = has_top && ctop == 0;
@@ -109,27 +132,44 @@ __global__ void k_expo_op_round(long long moves_done, int32_t R, const long long
 }
 
 // MODE 0: metrics, per-partition outputs and the t = 0 domain counts; 1: count domain events; 2: emit them.
+// Grid: x strides over the partitions of instance i0 + blockIdx.y.
 template <int MODE>
 __global__ void __launch_bounds__(256) k_expo_walk(const ExpoArgs E) {
-  const long long R1 = (long long)E.R + 1;
+  __shared__ ExpoInst I;
+  const int i = E.i0 + blockIdx.y;
+  if (threadIdx.x == 0) I = E.inst[i];
+  __syncthreads();
+  const long long R1 = (long long)I.R + 1;
+  long long* diff = E.diff + I.diff_off;
   // warp-uniform trip count: every lane reaches the t = 0 reductions at the end of each pass
   for (long long p0 = blockIdx.x * (long long)blockDim.x; p0 < E.P; p0 += (long long)gridDim.x * blockDim.x) {
-    const long long p = p0 + threadIdx.x;
+    const long long p = p0 + threadIdx.x, ci = (long long)i * E.P + p;
     uint32_t base[BLANCE_EXPO_N] = {0, 0, 0, 0, 0, 0};
-    if (p < E.P) {
-      const int32_t* row = E.beg + p * E.SL;
-      const long long o0 = E.op_off[p], o1 = E.op_off[p + 1];
+    const uint8_t f = p < E.P && E.pflags ? E.pflags[I.pf_off + p] : (uint8_t)PF_IN_PREV;
+    if (p < E.P && !(f & (PF_IN_PREV | PF_IN_ASSIGN))) {     // in neither map: no partition of begMap
+      if (MODE == 0) {
+        if (E.part_min) E.part_min[ci] = -1;
+        if (E.part_notop) E.part_notop[ci] = 0;
+        if (E.part_flags) E.part_flags[ci] = 0;
+      }
+      if (MODE == 1) E.ev_count[ci] = 0;
+    } else if (p < E.P) {
+      const int32_t* row = E.beg + I.beg_off + p * E.stride;
+      const long long gp = I.gp_off + p;
+      const long long o0 = E.op_off ? E.op_off[gp] : gp * E.MO;
+      const long long o1 = E.op_off ? E.op_off[gp + 1] : o0 + E.op_n[gp];
+      const int32_t* rho = E.op_round + (E.op_off ? 0 : ci * E.MO - o0);
       int c[BL_S_MAX] = {0, 0, 0, 0, 0, 0, 0, 0};
       uint32_t live = 0, closed = 0;                 // beg slots that hold an entry whose node has not had its op yet;
-      for (int i = 0; i < E.SL; ++i) {               // states whose list already ended
-        const int si = expo_slot_state(E, i);
-        if (row[i] == BLANCE_NO_NODE || (closed >> si & 1u)) { closed |= 1u << si; continue; }
-        live |= 1u << i;
+      for (int x = 0; x < E.SL && (f & PF_IN_PREV); ++x) {   // states whose list already ended (no row: empty)
+        const int si = expo_slot_state(E, x);
+        if (row[x] == BLANCE_NO_NODE || (closed >> si & 1u)) { closed |= 1u << si; continue; }
+        live |= 1u << x;
 #pragma unroll
         for (int s = 0; s < BL_S_MAX; ++s) c[s] += s == si ? 1 : 0;
       }
       int v[BLANCE_EXPO_N];
-      expo_values(E, c, v);
+      expo_values(E, I.constraints, c, v);
       int min_c = v[BLANCE_EXPO_COPIES], notop = 0, t0 = 0;
       uint32_t flags = 0;
       if (MODE == 0) {
@@ -137,22 +177,22 @@ __global__ void __launch_bounds__(256) k_expo_walk(const ExpoArgs E) {
         for (int m = 0; m < BLANCE_EXPO_N; ++m) { base[m] += (uint32_t)v[m]; flags |= (v[m] != 0) << m; }
         if (E.dom_base) {
           const int d = expo_dca(E, row, live, o0, 0);
-          expo_chain(E, d, -1, [&](int x) { red_add64(E.dom_base + x, 1ull); });
+          expo_chain(E, d, -1, [&](int x) { red_add64(E.dom_base + (long long)i * E.V + x, 1ull); });
         }
       }
       int d_prev = MODE == 0 ? -1 : expo_dca(E, row, live, o0, 0);
-      long long n_ev = 0, w = MODE == 2 ? E.ev_off[p] : 0;
+      long long n_ev = 0, w = MODE == 2 ? E.ev_off[ci] - E.ev0 : 0;
       for (long long k = o0; k < o1; ++k) {
-        const int r = E.op_round[k];
+        const int r = rho[k];
         if (r < 0) break;                            // the partition is stuck from here on
         // apply op k: every entry of its node leaves, a non-del op adds one entry of its state (one op per node, so
         // the entries that leave are exactly the node's beg entries)
         const int32_t n = E.op_node[k];
         for (uint32_t m = live; m; m &= m - 1) {
-          const int i = __ffs(m) - 1;
-          if (row[i] != n) continue;
-          live &= ~(1u << i);
-          const int si = expo_slot_state(E, i);
+          const int x = __ffs(m) - 1;
+          if (row[x] != n) continue;
+          live &= ~(1u << x);
+          const int si = expo_slot_state(E, x);
 #pragma unroll
           for (int s = 0; s < BL_S_MAX; ++s) c[s] -= s == si ? 1 : 0;
         }
@@ -164,10 +204,10 @@ __global__ void __launch_bounds__(256) k_expo_walk(const ExpoArgs E) {
         if (MODE == 0) {
           notop += v[BLANCE_EXPO_NO_TOP] * (r + 1 - t0);       // the state before held rounds t0 .. r
           int u[BLANCE_EXPO_N];
-          expo_values(E, c, u);
+          expo_values(E, I.constraints, c, u);
 #pragma unroll
           for (int m = 0; m < BLANCE_EXPO_N; ++m) {
-            if (u[m] != v[m]) red_add64(E.diff + m * R1 + r + 1, (unsigned long long)(long long)(u[m] - v[m]));
+            if (u[m] != v[m]) red_add64(diff + m * R1 + r + 1, (unsigned long long)(long long)(u[m] - v[m]));
             flags |= (u[m] != 0) << m;
             v[m] = u[m];
           }
@@ -177,8 +217,9 @@ __global__ void __launch_bounds__(256) k_expo_walk(const ExpoArgs E) {
           if (d != d_prev) {
             const int top = d_prev >= 0 && d >= 0 ? audit_dca(E.dom_parent, d_prev, d) : -1;
             const unsigned long long t = (unsigned long long)(r + 1);
+            const unsigned long long g = (unsigned long long)(i - E.g0) * (unsigned long long)E.V;
             auto ev = [&](int x, int32_t delta) {
-              if (MODE == 2) { E.ev_key[w] = ((unsigned long long)x << 32) | t; E.ev_val[w] = delta; ++w; }
+              if (MODE == 2) { E.ev_key[w] = ((g + (unsigned long long)x) << 32) | t; E.ev_val[w] = delta; ++w; }
               else ++n_ev;
             };
             expo_chain(E, d_prev, top, [&](int x) { ev(x, -1); });
@@ -189,33 +230,37 @@ __global__ void __launch_bounds__(256) k_expo_walk(const ExpoArgs E) {
         t0 = r + 1;
       }
       if (MODE == 0) {
-        notop += v[BLANCE_EXPO_NO_TOP] * (E.R + 1 - t0);
-        if (E.part_min) E.part_min[p] = min_c;
-        if (E.part_notop) E.part_notop[p] = notop;
-        if (E.part_flags) E.part_flags[p] = (uint8_t)flags;
+        notop += v[BLANCE_EXPO_NO_TOP] * (I.R + 1 - t0);
+        if (E.part_min) E.part_min[ci] = min_c;
+        if (E.part_notop) E.part_notop[ci] = notop;
+        if (E.part_flags) E.part_flags[ci] = (uint8_t)flags;
       }
-      if (MODE == 1) E.ev_count[p] = n_ev;
+      if (MODE == 1) E.ev_count[ci] = n_ev;
     }
     if (MODE == 0) {
       // every partition's t = 0 values land on index 0: one RED per warp and metric
 #pragma unroll
       for (int m = 0; m < BLANCE_EXPO_N; ++m) {
         const uint32_t b = __reduce_add_sync(0xFFFFFFFFu, base[m]);
-        if ((threadIdx.x & 31) == 0 && b) red_add64(E.diff + m * R1, b);
+        if ((threadIdx.x & 31) == 0 && b) red_add64(diff + m * R1, b);
       }
     }
   }
 }
 
-// One CTA per metric: diff[m] scanned in place into series[m]; stats[m] = {peak, first round at the peak, area}.
-__global__ void __launch_bounds__(512) k_expo_series(long long* __restrict__ diff, int32_t R, long long* __restrict__ stats) {
+// One CTA per (metric blockIdx.x, instance blockIdx.y): the instance's diff[m] scanned in place into series[m];
+// stats[instance][m] = {peak, first round at the peak, area}.
+__global__ void __launch_bounds__(512) k_expo_series(const ExpoInst* __restrict__ inst, long long* __restrict__ diff,
+                                                     long long* __restrict__ stats) {
   typedef cub::BlockScan<long long, 512> Scan;
   typedef cub::BlockReduce<long long, 512> Reduce;
   __shared__ typename Scan::TempStorage s_scan;
   __shared__ typename Reduce::TempStorage s_red;
   __shared__ long long s_carry, s_peak;
-  const long long n = (long long)R + 1;
-  long long* x = diff + blockIdx.x * n;
+  const ExpoInst& I = inst[blockIdx.y];
+  const long long n = (long long)I.R + 1;
+  long long* x = diff + I.diff_off + blockIdx.x * n;
+  stats += ((long long)blockIdx.y * BLANCE_EXPO_N + blockIdx.x) * 3;
   long long best = LLONG_MIN, best_t = LLONG_MAX, area = 0;
   if (threadIdx.x == 0) s_carry = 0;
   __syncthreads();
@@ -240,7 +285,7 @@ __global__ void __launch_bounds__(512) k_expo_series(long long* __restrict__ dif
   __syncthreads();
   const long long sum = Reduce(s_red).Sum(area);
   if (threadIdx.x == 0) {
-    stats[blockIdx.x * 3] = s_peak; stats[blockIdx.x * 3 + 1] = first; stats[blockIdx.x * 3 + 2] = sum;
+    stats[0] = s_peak; stats[1] = first; stats[2] = sum;
   }
 }
 
@@ -252,20 +297,22 @@ struct ExpoSameVertex {
   __host__ __device__ bool operator()(unsigned long long a, unsigned long long b) const { return (a >> 32) == (b >> 32); }
 };
 
-// dom_key[v] = (partitions under v << 32) | (0xFFFFFFFF - t) at t = 0: the running maximum starts there.
-__global__ void k_expo_dom_init(int32_t V, const long long* __restrict__ dom_base, unsigned long long* __restrict__ dom_key) {
-  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < V; v += gridDim.x * blockDim.x)
+// dom_key[v] = (partitions under v << 32) | (0xFFFFFFFF - t) at t = 0, over the n = instances x V vertices: the running
+// maximum starts there.
+__global__ void k_expo_dom_init(long long n, const long long* __restrict__ dom_base, unsigned long long* __restrict__ dom_key) {
+  for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < n; v += (long long)gridDim.x * blockDim.x)
     dom_key[v] = ((unsigned long long)dom_base[v] << 32) | 0xFFFFFFFFu;
 }
 
-// Run i of the merged events: (vertex, t) and the vertex's running sum of changes up to and including t.  The count
-// at t is dom_base + that sum; the largest count, at its smallest t, wins the RED.MAX on one u64 key.
+// Run i of the merged events: (key vertex, t) and the key vertex's running sum of changes up to and including t.  The
+// count at t is dom_base + that sum; the largest count, at its smallest t, wins the RED.MAX on one u64 key.  A key
+// vertex g V + v is vertex v of the group's instance g: dom_base and dom_key are the group's [g][V] slices.
 __global__ void k_expo_dom_max(int n, const unsigned long long* __restrict__ keys,
                                const int32_t* __restrict__ running, const long long* __restrict__ dom_base,
                                unsigned long long* __restrict__ dom_key) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const unsigned long long key = keys[i];
-    const int v = (int)(key >> 32);
+    const long long v = (long long)(key >> 32);
     const uint32_t t = (uint32_t)key;
     const unsigned long long cnt = (unsigned long long)(dom_base[v] + running[i]);
     red_max64((long long*)(dom_key + v), (cnt << 32) | (0xFFFFFFFFu - t));

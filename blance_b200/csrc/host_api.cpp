@@ -1303,14 +1303,56 @@ ScenarioResult scenario_result(const InternedPlan& ip, const blance_scenario_out
   return r;
 }
 
+// Output buffers of one blance_exposure_out: series [BLANCE_EXPO_N][cap], V vertices, P partitions.
+struct ExposureBuffers {
+  std::vector<int64_t> series, dom_peak;
+  std::vector<int32_t> dom_round, min_copies, no_top;
+  std::vector<uint8_t> flags;
+  blance_exposure_out out{};
+  ExposureBuffers(size_t cap, size_t V, size_t P)
+      : series(BLANCE_EXPO_N * cap + 1), dom_peak(V + 1), dom_round(V + 1), min_copies(P + 1), no_top(P + 1), flags(P + 1) {
+    out.series = cap ? series.data() : nullptr; out.dom_peak = dom_peak.data(); out.dom_peak_round = dom_round.data();
+    out.part_min_copies = min_copies.data(); out.part_no_top = no_top.data(); out.part_flags = flags.data();
+  }
+};
+
+// One exposure by name: `cap` series values per metric were copied (the first min(R + 1, cap) are kept), vertices
+// are vnames, partitions pnames.  Vertex- and partition-keyed fields keep positive entries only (a partition outside
+// the exposed map reads -1 / 0 / 0 and is left out).
+ExposureResult name_exposure(const ExposureBuffers& b, size_t cap, const Strs& vnames, const Strs& pnames) {
+  static const char* kMetrics[BLANCE_EXPO_N] = {"NO_TOP", "MULTI_TOP", "SHORT", "ONE_COPY", "NO_COPY", "COPIES"};
+  const blance_exposure_out& o = b.out;
+  ExposureResult r;
+  r.Rounds = o.rounds;
+  r.KernelMs = o.kernel_ms;
+  const size_t n = std::min(size_t(o.rounds) + 1, cap);
+  for (size_t m = 0; m < BLANCE_EXPO_N; ++m) {
+    r.Series[kMetrics[m]].assign(b.series.begin() + std::ptrdiff_t(m * cap), b.series.begin() + std::ptrdiff_t(m * cap + n));
+    r.Peak[kMetrics[m]] = o.peak[m];
+    r.PeakRound[kMetrics[m]] = o.peak_round[m];
+    r.Area[kMetrics[m]] = o.area[m];
+  }
+  for (size_t v = 0; v < vnames.size(); ++v)
+    if (b.dom_peak[v] > 0) { r.DomPeak[vnames[v]] = b.dom_peak[v]; r.DomPeakRound[vnames[v]] = b.dom_round[v]; }
+  for (size_t p = 0; p < pnames.size(); ++p) {
+    if (b.min_copies[p] > 0) r.PartMinCopies[pnames[p]] = b.min_copies[p];
+    if (b.no_top[p] > 0) r.PartNoTop[pnames[p]] = b.no_top[p];
+    if (b.flags[p]) r.PartFlags[pnames[p]] = b.flags[p];
+  }
+  return r;
+}
+
 }  // namespace
 
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                                  const Strs& nodesAll, const PartitionModel& model,
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
                                                  bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
-                                                 const std::vector<int>& scheduleConcurrency, const ScenarioAudit* audit) {
+                                                 const std::vector<int>& scheduleConcurrency, const ScenarioAudit* audit,
+                                                 const ScenarioExposure* exposure) {
   if (scenarios.empty()) invalid("PlanNextMapScenarios: no scenarios");
+  if (exposure && scheduleConcurrency.empty()) invalid("PlanNextMapScenarios: an exposure needs scheduleConcurrency");
+  if (exposure && exposure->SeriesCap < 0) invalid("PlanNextMapScenarios: SeriesCap is negative");
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, scenarios);
   const size_t n = scenarios.size();
   PartIndex parts{*ip, {}};
@@ -1366,8 +1408,24 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
       aout.push_back(abuf.back()->out);
     }
   }
+  // the exposures: the options' NodeHierarchy as the forest, one output per (scenario, count)
+  Forest eforest;
+  std::vector<std::unique_ptr<ExposureBuffers>> ebuf;
+  std::vector<blance_exposure_out> eout;
+  const size_t cap = exposure ? size_t(exposure->SeriesCap) : 0;
+  if (exposure) {
+    build_forest(ip->node_names, options.NodeHierarchy, false, &eforest);
+    for (size_t x = 0; x < n * nc; ++x) {
+      ebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), size_t(ip->in.n_parts)));
+      eout.push_back(ebuf.back()->out);
+    }
+  }
   blance_ctx* ctx = DefaultContext();
-  const int st = audit ? blance_plan_scenarios_audit(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+  const int st = exposure ? blance_plan_scenarios_exposure(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                                           int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), sched.data(),
+                                                           audit ? &forest.opts : nullptr, audit ? aout.data() : nullptr, &eforest.opts,
+                                                           int32_t(cap), eout.data())
+                 : audit ? blance_plan_scenarios_audit(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                      int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
                                                      nc ? sched.data() : nullptr, &forest.opts, aout.data())
                  : nc ? blance_plan_scenarios_schedule(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
@@ -1394,6 +1452,11 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     if (audit) {
       abuf[i]->out = aout[i];
       r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[i], audit->FailoverSpread);
+    }
+    for (size_t k = 0; exposure && k < nc; ++k) {
+      ExposureBuffers& b = *ebuf[i * nc + k];
+      b.out = eout[i * nc + k];
+      r.Exposures.push_back(name_exposure(b, cap, eforest.names, ip->part_names));
     }
   }
   return res;
@@ -1696,33 +1759,10 @@ ExposureResult OrchestrateExposure(const PartitionModel& model, const Orchestrat
     if (t.state_names[s] == top) top_state = int32_t(s);
   Forest f;
   build_forest(t.nodes.names, nodeHierarchy, false, &f);
-  const size_t V = f.names.size();
   blance_exposure_in in{cons.data(), top_state, f.opts.n_domains, f.opts.domain_parent};
-  std::vector<int64_t> series(BLANCE_EXPO_N * R1), dom_peak(V + 1);
-  std::vector<int32_t> dom_round(V + 1), min_copies(P + 1), no_top(P + 1);
-  std::vector<uint8_t> flags(P + 1);
-  blance_exposure_out out{};
-  out.series = series.data(); out.dom_peak = dom_peak.data(); out.dom_peak_round = dom_round.data();
-  out.part_min_copies = min_copies.data(); out.part_no_top = no_top.data(); out.part_flags = flags.data();
-  o->check(blance_moves_exposure(o->ctx, o->h.get(), &in, &out), "blance_moves_exposure");
-  static const char* kMetrics[BLANCE_EXPO_N] = {"NO_TOP", "MULTI_TOP", "SHORT", "ONE_COPY", "NO_COPY", "COPIES"};
-  ExposureResult r;
-  r.Rounds = out.rounds;
-  r.KernelMs = out.kernel_ms;
-  for (size_t m = 0; m < BLANCE_EXPO_N; ++m) {
-    r.Series[kMetrics[m]].assign(series.begin() + std::ptrdiff_t(m * R1), series.begin() + std::ptrdiff_t((m + 1) * R1));
-    r.Peak[kMetrics[m]] = out.peak[m];
-    r.PeakRound[kMetrics[m]] = out.peak_round[m];
-    r.Area[kMetrics[m]] = out.area[m];
-  }
-  for (size_t v = 0; v < V; ++v)
-    if (dom_peak[v]) { r.DomPeak[f.names[v]] = dom_peak[v]; r.DomPeakRound[f.names[v]] = dom_round[v]; }
-  for (size_t p = 0; p < P; ++p) {
-    if (min_copies[p]) r.PartMinCopies[o->names[p]] = min_copies[p];
-    if (no_top[p]) r.PartNoTop[o->names[p]] = no_top[p];
-    if (flags[p]) r.PartFlags[o->names[p]] = flags[p];
-  }
-  return r;
+  ExposureBuffers b(R1, f.names.size(), P);
+  o->check(blance_moves_exposure(o->ctx, o->h.get(), &in, &b.out), "blance_moves_exposure");
+  return name_exposure(b, R1, f.names, o->names);
 }
 
 }  // namespace blance

@@ -140,6 +140,18 @@ struct MapAudit {
 MapAudit AuditMap(const PartitionMap& map, const Strs& nodesAll, const PartitionModel& model,
                   const PlanNextMapOptions& options, bool failoverSpread);
 
+// The exposure of one rebalance by name (OrchestrateExposure below, and PlanNextMapScenarios' Exposures).
+struct ExposureResult {
+  int32_t Rounds = 0;
+  std::unordered_map<std::string, std::vector<int64_t>> Series;   // [Rounds + 1] per metric
+  std::unordered_map<std::string, int64_t> Peak, Area;
+  std::unordered_map<std::string, int32_t> PeakRound;
+  std::unordered_map<std::string, int64_t> DomPeak;               // per node or NodeHierarchy name
+  std::unordered_map<std::string, int32_t> DomPeakRound;
+  std::unordered_map<std::string, int32_t> PartMinCopies, PartNoTop, PartFlags;   // per partition; flags: bit m = metric m
+  float KernelMs = 0.f;
+};
+
 struct ScenarioResult {
   int iters_run = 0, converged = 0;
   int64_t steps = 0, sticky_steps = 0, parts_moved = 0, ops_total = 0, warn_parts = 0;
@@ -153,12 +165,22 @@ struct ScenarioResult {
   Warnings NextWarnings;
   std::vector<ScenarioSchedule> Schedules;   // one per scheduleConcurrency value; empty without them
   std::optional<MapAudit> Audit;       // with `audit`: the audit of the scenario's final map
+  std::vector<ExposureResult> Exposures;   // with `exposure`: one per scheduleConcurrency value
 };
 
 // PlanNextMapScenarios' audit request: every result's Audit is AuditMap of that scenario's final map (prevMap with
 // every assigned partition replaced by its next row) under the scenario's own constraints and hierarchy rules
 // (blance_plan_scenarios_audit).  The fault-domain forest is the options' NodeHierarchy for every scenario.
 struct ScenarioAudit { bool FailoverSpread = false; };
+
+// PlanNextMapScenarios' exposure request (blance_plan_scenarios_exposure): every result's Exposures[k] is
+// OrchestrateExposure(model with the scenario's effective ModelStateConstraints, {scheduleConcurrency[k],
+// favorMinNodes}, nodesAll, begMap, finalMap, the options' NodeHierarchy), where begMap is prevMap plus an empty entry
+// for every assigned partition it lacks and finalMap is prevMap with every assigned partition replaced by its next
+// row; the top state is topPriorityStateName.  Partitions are walked in interning order, as for the schedules.
+// Series holds the first min(Rounds + 1, SeriesCap) values per metric (Rounds is not known before planning; an
+// up-front bound would cost hundreds of MB per scenario and count); Rounds, Peak, PeakRound and Area are complete.
+struct ScenarioExposure { int32_t SeriesCap = 0; };
 
 // Scenario i is PlanNextMapEx(prevMap, partitionsToAssign, nodesAll, NodesToRemove_i, NodesToAdd_i, model, options
 // with the scenario's NodeWeights, ModelStateConstraints, StateStickiness, PartitionWeights, NodeHierarchy and
@@ -178,7 +200,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
                                                  const PlanNextMapOptions& options, const std::vector<Scenario>& scenarios,
                                                  bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
                                                  const std::vector<int>& scheduleConcurrency = {},
-                                                 const ScenarioAudit* audit = nullptr);
+                                                 const ScenarioAudit* audit = nullptr, const ScenarioExposure* exposure = nullptr);
 
 // ---- chains of cluster changes (blance_plan_chains) --------------------------------------------------------------
 struct ChainStage {
@@ -259,17 +281,6 @@ std::vector<std::vector<AssignPartitionsCall>> OrchestrateSchedule(const Partiti
 // "ONE_COPY", "NO_COPY", "COPIES") hold every metric; vertex- and partition-keyed fields hold nonzero entries only
 // (a partition absent from PartMinCopies had no copy at some round; DomPeakRound lists the vertices of DomPeak).
 // Throws BlanceError for what OrchestrateSchedule or blance_moves_exposure rejects (e.g. more than 8 state names).
-struct ExposureResult {
-  int32_t Rounds = 0;
-  std::unordered_map<std::string, std::vector<int64_t>> Series;   // [Rounds + 1] per metric
-  std::unordered_map<std::string, int64_t> Peak, Area;
-  std::unordered_map<std::string, int32_t> PeakRound;
-  std::unordered_map<std::string, int64_t> DomPeak;               // per node or NodeHierarchy name
-  std::unordered_map<std::string, int32_t> DomPeakRound;
-  std::unordered_map<std::string, int32_t> PartMinCopies, PartNoTop, PartFlags;   // per partition; flags: bit m = metric m
-  float KernelMs = 0.f;
-};
-
 ExposureResult OrchestrateExposure(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
                                    const PartitionMap& begMap, const PartitionMap& endMap,
                                    const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy);

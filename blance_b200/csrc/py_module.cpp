@@ -78,6 +78,14 @@ static py::array_t<T> np_copy(const std::vector<T>& v, size_t n) {
   return a;
 }
 
+static py::dict exposure_dict(const ExposureResult& r) {
+  py::dict d;
+  d["rounds"] = r.Rounds; d["series"] = r.Series; d["peak"] = r.Peak; d["peak_round"] = r.PeakRound; d["area"] = r.Area;
+  d["dom_peak"] = r.DomPeak; d["dom_peak_round"] = r.DomPeakRound; d["part_min_copies"] = r.PartMinCopies;
+  d["part_no_top"] = r.PartNoTop; d["part_flags"] = r.PartFlags; d["kernel_ms"] = r.KernelMs;
+  return d;
+}
+
 static py::dict audit_dict(const MapAudit& a) {
   py::dict d;
   d["short_slots"] = a.ShortSlots; d["over_slots"] = a.OverSlots;
@@ -288,11 +296,7 @@ PYBIND11_MODULE(_host, m) {
       py::gil_scoped_release rel;
       r = OrchestrateExposure(to_model(model), o, nodes_all, b, e, nh);
     }
-    py::dict d;
-    d["rounds"] = r.Rounds; d["series"] = r.Series; d["peak"] = r.Peak; d["peak_round"] = r.PeakRound; d["area"] = r.Area;
-    d["dom_peak"] = r.DomPeak; d["dom_peak_round"] = r.DomPeakRound; d["part_min_copies"] = r.PartMinCopies;
-    d["part_no_top"] = r.PartNoTop; d["part_flags"] = r.PartFlags; d["kernel_ms"] = r.KernelMs;
-    return d;
+    return exposure_dict(r);
   }, py::arg("model"), py::arg("max_concurrent"), py::arg("favor"), py::arg("nodes_all"), py::arg("beg"), py::arg("end"),
      py::arg("node_hierarchy") = py::none());
 
@@ -408,7 +412,8 @@ PYBIND11_MODULE(_host, m) {
                      const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
                      const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
                      const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
-                     int engine, const std::vector<int>& schedule_concurrency, const std::optional<bool>& audit) {
+                     int engine, const std::vector<int>& schedule_concurrency, const std::optional<bool>& audit,
+                     const std::optional<int>& exposure_series_cap) {
         PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
         const PartitionMap prev_map = to_map(prev);
         const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
@@ -416,10 +421,13 @@ PYBIND11_MODULE(_host, m) {
         std::vector<ScenarioResult> res;
         ScenarioAudit aud;
         aud.FailoverSpread = audit.value_or(false);
+        ScenarioExposure expo;
+        expo.SeriesCap = exposure_series_cap.value_or(0);
         {
           py::gil_scoped_release rel;
           res = PlanNextMapScenarios(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, scs,
-                                     favor_min_nodes, want_maps, max_concurrent, schedule_concurrency, audit ? &aud : nullptr);
+                                     favor_min_nodes, want_maps, max_concurrent, schedule_concurrency, audit ? &aud : nullptr,
+                                     exposure_series_cap ? &expo : nullptr);
         }
         py::list out;
         for (const auto& r : res) {
@@ -440,6 +448,11 @@ PYBIND11_MODULE(_host, m) {
             d["schedules"] = sl;
           }
           if (r.Audit) d["audit"] = audit_dict(*r.Audit);
+          if (exposure_series_cap) {
+            py::list el;
+            for (const auto& e : r.Exposures) el.append(exposure_dict(e));
+            d["exposures"] = el;
+          }
           out.append(d);
         }
         return out;
@@ -449,7 +462,8 @@ PYBIND11_MODULE(_host, m) {
       py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
-      py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none());
+      py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none(),
+      py::arg("exposure_series_cap") = py::none());
 
   // chains: per chain (its option fields as a scenario tuple - the node sets are not read -, its stages); per stage
   // (nodes_to_remove, nodes_to_add, has_node_weights_key, node_weights, nodes_all or None for the default)

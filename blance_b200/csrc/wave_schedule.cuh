@@ -28,7 +28,8 @@
 //
 // The ops are a moves handle's CSR arrays (op_off set) or the table [nw * PU][MO] k_wave_moves fills.  With one
 // instance the segments are the nodes in ascending id, so pick x of segment s in round r is op
-// round_off[r] + poff[s] + x of the schedule's order (round, node id, pick order).
+// round_off[r] + poff[s] + x of the schedule's order (round, node id, pick order).  For an exposure of the table's
+// schedules (exposure.cuh), k_wave_moves also keeps each op's state and k_wave_pick each op's round per instance.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -60,6 +61,8 @@ struct WSched {
   int32_t* overflow;                       // more picks than the host sorted (internal error)
   long long* esum;                         // the host's reduction of len: entries left in all lists
   long long* round_off; long long* sched_op;   // one instance only: the per-op order (null: not emitted)
+  uint8_t* op_state;                       // [nw * PU][MO] the op table's states, or null (no exposure asked for)
+  int32_t* op_round;                       // [ni * PU][MO] the round of each op of the table, -1 = never; or null
 };
 
 __device__ __forceinline__ bool wave_pickable(const WSched& W, int32_t node) {
@@ -117,11 +120,14 @@ __global__ void k_wave_moves(DPool pool, const int32_t* __restrict__ prev_rows_i
     const uint8_t f = pflags_init[g];
     int32_t* on = W.op_node + gp * W.MO;
     uint8_t* ok = W.op_kind + gp * W.MO;
+    uint8_t* os = W.op_state ? W.op_state + gp * W.MO : nullptr;
     int cnt = 0;
     if (f & PF_IN_ASSIGN) {
-      auto emit = [&](int32_t node, int, int kind) {
+      auto emit = [&](int32_t node, int state, int kind) {
         for (int x = 0; x < cnt; ++x) if (on[x] == node) return;   // addMoves + seen, moves.go:51-58
-        on[cnt] = node; ok[cnt] = (uint8_t)kind; ++cnt;
+        on[cnt] = node; ok[cnt] = (uint8_t)kind;
+        if (os) os[cnt] = (uint8_t)state;
+        ++cnt;
       };
       const int32_t* next = pool.rows + D.rows_off + p * D.SLP;
       if (f & PF_IN_PREV) calc_moves_row(prev_rows_init + D.rows_off + p * D.SLP, next, D.state_slot_off, D.SL, D.S, favor_min, emit);
@@ -190,6 +196,7 @@ __global__ void __launch_bounds__(WAVE_THREADS) k_wave_pick(WSched W, int32_t r,
       const long long ci = i * W.PU + p, gp = j * W.PU + p;
       const int32_t cu = W.cur[ci];
       if (ops) ops[x] = wave_op(W, gp, cu);
+      if (W.op_round) W.op_round[ci * W.MO + cu] = r;
       W.cur[ci] = cu + 1;
       unsigned long long key = ~0ull;
       if (cu + 1 >= wave_n_ops(W, gp)) W.part_done[ci] = r + 1;

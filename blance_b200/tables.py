@@ -128,6 +128,7 @@ class ScenarioResult:
     sticky_steps = property(lambda self: self.out.sticky_steps)
     schedules = None          # blance_plan_scenarios_schedule: one ScenarioSchedule per count
     audit = None              # blance_plan_scenarios_audit: the AuditResult of the final map
+    exposures = None          # blance_plan_scenarios_exposure: one moves_exposure-shaped dict per count
     parts_moved = property(lambda self: self.out.parts_moved)
     ops_total = property(lambda self: self.out.ops_total)
     warn_parts = property(lambda self: self.out.warn_parts)
@@ -201,6 +202,41 @@ def _audit_opts(n2n, domain_parent, n_node_ids, keep):
         o.n_domains = a.size - n_node_ids
         o.domain_parent = a.ctypes.data
     return o, int(o.n_domains)
+
+
+EXPOSURE_KEYS = ("domain_parent", "series_cap", "dom", "parts")
+
+
+class _ScenarioExposure:
+    """Output buffers of one blance_exposure_out of a scenario wave: series [6][series_cap], the per-vertex arrays
+    (with dom) and the per-partition ones (with parts); result() shapes them as Context.moves_exposure does, with the
+    arrays not asked for left out."""
+
+    def __init__(self, t, V, series_cap, dom, parts):
+        self.V, self.cap = V, series_cap
+        self.a = dict(series=np.zeros((6, max(1, series_cap)), np.int64))
+        if dom:
+            self.a.update(dom_peak=np.zeros(max(1, V), np.int64), dom_peak_round=np.zeros(max(1, V), np.int32))
+        if parts:
+            self.a.update(part_min_copies=np.zeros(max(1, t.n_parts), np.int32), part_no_top=np.zeros(max(1, t.n_parts), np.int32),
+                          part_flags=np.zeros(max(1, t.n_parts), np.uint8))
+        self.n_parts = t.n_parts
+        self.out = api.ExposureOut()
+        for k, a in self.a.items():
+            setattr(self.out, k, a.ctypes.data if k != "series" or series_cap > 0 else None)
+
+    def result(self):
+        o, a = self.out, self.a
+        n = min(o.rounds + 1, self.cap)
+        r = dict(series=a["series"][:, :n].copy(), rounds=o.rounds, kernel_ms=o.kernel_ms, peak=np.array(o.peak[:], np.int64),
+                 peak_round=np.array(o.peak_round[:], np.int32), area=np.array(o.area[:], np.int64))
+        for k in ("dom_peak", "dom_peak_round"):
+            if k in a:
+                r[k] = a[k][:self.V]
+        for k in ("part_min_copies", "part_no_top", "part_flags"):
+            if k in a:
+                r[k] = a[k][:self.n_parts]
+        return r
 
 
 def _n_rules(t):
@@ -351,7 +387,7 @@ class Context:
         return r
 
     def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None,
-                       schedule=None, node_has_mover=None, audit=None):
+                       schedule=None, node_has_mover=None, audit=None, exposure=None):
         """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
         (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
         are copied out.  opts (None, or one dict of OPT_GROUPS keys per scenario) calls blance_plan_scenarios_ex
@@ -360,7 +396,18 @@ class Context:
         sets each result's `schedules` to one ScenarioSchedule per value.  Returns one ScenarioResult per
         scenario.  audit (None, or a dict with the optional keys n2n and domain_parent) calls
         blance_plan_scenarios_audit (with the schedules when `schedule` is given) and sets each result's `audit` to
-        the AuditResult of that scenario's final map."""
+        the AuditResult of that scenario's final map.  exposure (None, or a dict with the optional keys domain_parent,
+        series_cap (default 0), dom (default True) and parts (default True)) needs `schedule` and calls
+        blance_plan_scenarios_exposure; each result's `exposures` is then one dict per count, shaped as
+        moves_exposure's, with series [6][min(R + 1, series_cap)].  dom=False leaves out dom_peak / dom_peak_round (the
+        device then skips the fault-domain work), parts=False the per-partition arrays (nothing of n_parts size is
+        copied out)."""
+        if exposure is not None:
+            unknown = set(exposure) - set(EXPOSURE_KEYS)
+            if unknown:
+                raise KeyError("unknown exposure option(s) %s" % sorted(unknown))
+            if not schedule:
+                raise ValueError("an exposure needs a schedule: pass schedule=[counts]")
         n = len(scenarios)
         want = set(want_rows)
         base = base_tables.struct()
@@ -390,7 +437,30 @@ class Context:
             ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
             args = (self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent), int(counts.size),
                     counts.ctypes.data if counts.size else None, None if mover is None else mover.ctypes.data, outs, sch)
-            if audit is None:
+            if exposure is not None:
+                e_opts, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
+                V = base_tables.n_node_ids + int(e_opts.n_domains)
+                cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
+                expo = [[_ScenarioExposure(base_tables, V, max(cap, 0), dom, parts) for _ in counts] for _ in results]
+                exps = (api.ExposureOut * max(1, n * counts.size))(*[e.out for es in expo for e in es])
+                auds = None
+                if audit is not None:
+                    a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
+                    for i, r in enumerate(results):
+                        t = scenario_tables(base_tables, scenarios[i], None if opts is None else opts[i])
+                        r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
+                    auds = (api.AuditOut * max(1, n))(*[r.audit.out for r in results])
+                self._check(self.lib.blance_plan_scenarios_exposure(
+                    *args, None if audit is None else ctypes.byref(a_opts), auds,
+                    ctypes.byref(e_opts) if exposure.get("domain_parent") is not None else None, cap, exps),
+                    "blance_plan_scenarios_exposure")
+                for i, r in enumerate(results):
+                    if auds is not None:
+                        r.audit.out = auds[i]
+                    for k, e in enumerate(expo[i]):
+                        e.out = exps[i * counts.size + k]
+                    r.exposures = [e.result() for e in expo[i]]
+            elif audit is None:
                 self._check(self.lib.blance_plan_scenarios_schedule(*args), "blance_plan_scenarios_schedule")
             else:
                 a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)

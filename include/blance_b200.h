@@ -526,7 +526,8 @@ int blance_plan_audit(blance_ctx* ctx, blance_plan* plan, const blance_audit_opt
  * under scenario i's own constraints and hierarchy (blance_scenario_opts) and the shared `aopts`.  The audit runs
  * inside the wave, next to the summaries and before anything is copied out; its buffers are priced into the wave
  * size (a few KB per scenario, plus n_nodes x n_nodes x 4 bytes with BLANCE_AUDIT_N2N).
- * Errors as blance_plan_scenarios_schedule and blance_map_audit, plus a NULL audit, all before any device work. */
+ * Errors as blance_plan_scenarios_schedule and blance_map_audit, plus a NULL audit, all before any device work.
+ * blance_plan_scenarios_exposure (below, after blance_moves_exposure) adds the exposure of every scenario's schedule. */
 int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                 const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                 int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
@@ -695,6 +696,44 @@ typedef struct blance_exposure_out {
 } blance_exposure_out;
 
 int blance_moves_exposure(blance_ctx* ctx, blance_moves* moves, const blance_exposure_in* in, blance_exposure_out* out);
+
+/* ---- the exposure of every scenario's rebalance (blance_plan_scenarios_exposure) ----------------------------
+ * blance_plan_scenarios_audit, and the exposure of every (scenario, count) pair's schedule, inside the wave.
+ *
+ * Arguments up to audit mean what they mean in blance_plan_scenarios_audit, except that audit may be NULL (no audit;
+ * aopts is then not read).  out, sched and audit equal what blance_plan_scenarios_audit returns for the same
+ * arguments; with audit NULL, out and sched equal blance_plan_scenarios_schedule.
+ *
+ * expo[i * n_move_conc + k] equals blance_moves_exposure on the handle of scenario i's rebalance at move_conc[k]:
+ *   partitions   those of its begMap - part_in_prev || part_in_assign - in ascending partition index;
+ *   beg row      the prev row as passed in (model states only; an assigned partition absent from prevMap starts
+ *                from an empty row); end row: the next row for an assigned partition, the prev row otherwise;
+ *   handle       favor_min_nodes, all states visited, scheduled at move_conc[k] with node_has_mover (the schedule
+ *                sched[i * n_move_conc + k] reports);
+ *   exposure_in  scenario i's own state_constraints (BLANCE_OPT_CONSTRAINTS applies), the base's top_state and the
+ *                forest of eopts (flags must be 0; NULL = every node its own domain).
+ * The per-partition arrays are [n_parts] over all partitions: a partition in neither map is no partition of begMap,
+ * counts in no metric and gets part_min_copies = -1, part_no_top = 0 and part_flags = 0.
+ * series is [BLANCE_EXPO_N][series_cap]: the first min(R + 1, series_cap) values of each metric (R = rounds, so a
+ * caller sees when the series was cut; R is not known before planning).  peak, peak_round and area always cover all
+ * R + 1 maps.  series_cap = 0 or a NULL series asks for none.  dom_peak / dom_peak_round are computed only when some
+ * expo[] asks for one of them.  kernel_ms is the wave's exposure time, the same value in each of its members.
+ * No value depends on n, max_concurrent, the wave size, the engine, the number of devices or the other move_conc.
+ *
+ * Errors, all before any device work, naming the scenario or k: everything blance_plan_scenarios_audit rejects;
+ * n_move_conc < 1, a NULL expo, series_cap < 0, eopts with flags set or a bad forest (BLANCE_ERR_INVALID_ARG);
+ * dom_peak or dom_peak_round asked for with 2 x 17 x 2 x n_slots x n_parts >= 2^31 (BLANCE_ERR_UNSUPPORTED, the
+ * static form of blance_moves_exposure's bound).  The op states and rounds and the outputs asked for are priced
+ * into the wave size; the per-round arrays (48 bytes per round and instance) and the fault-domain events are
+ * allocated after the schedule, exactly sized, and BLANCE_ERR_NOMEM names the exposure when they do not fit
+ * (DESIGN.md section 14). */
+int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                   const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                   int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                   blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                                   const blance_audit_opts* aopts, blance_audit_out* audit /* [n] or NULL */,
+                                   const blance_audit_opts* eopts /* forest only, flags must be 0; NULL = nodes only */,
+                                   int32_t series_cap, blance_exposure_out* expo /* [n][n_move_conc] */);
 
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
