@@ -1165,8 +1165,13 @@ static void sched_slices(Arena& a, int nw, int nc, long long PU, long long NU, i
   while (w.PB < WAVE_PART_BITS && (1ll << w.PB) < PU) ++w.PB;
 }
 
-// The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit).  Scenarios differ only in
-// their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and override list of any.
+// The widest wave: the wave kernels (k_wave_moves, k_wave_first, k_scenario_summary, the audit kernels) put the
+// wave member on grid y.
+static const int kWaveMax = 65535;
+
+// The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit), at most kWaveMax.  Scenarios
+// differ only in their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and
+// override list of any.
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
                      int max_concurrent, const SchedReq* sr, size_t extra_bytes, size_t* per_scenario) {
   blance_plan probe;
@@ -1190,6 +1195,7 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   *per_scenario = per;
   if (sr)            // the first round's arrival slots (nc x n_parts per scenario) are int32 positions
     n_dev = (int)std::min<long long>(n_dev, std::max(1ll, (long long)INT32_MAX / ((long long)sr->nc * std::max(1, in0.n_parts))));
+  n_dev = std::min(n_dev, kWaveMax);
   if (max_concurrent > 0) return std::min(n_dev, max_concurrent);
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return 1; }
