@@ -108,9 +108,18 @@ class _ExposureOut(ctypes.Structure):  # struct blance_exposure_out
                 ("part_flags", ctypes.c_void_p), ("kernel_ms", ctypes.c_float)]
 
 
+class _ChainSpanOut(ctypes.Structure):  # struct blance_chain_span_out
+    _fields_ = [("rounds", ctypes.c_int64), ("moves_done", ctypes.c_int64), ("stuck_parts", ctypes.c_int64),
+                ("max_batch", ctypes.c_int32), ("node_rounds", ctypes.c_void_p), ("node_last_round", ctypes.c_void_p),
+                ("part_done_round", ctypes.c_void_p), ("peak", ctypes.c_int64 * 6), ("peak_stage", ctypes.c_int32 * 6),
+                ("peak_round", ctypes.c_int32 * 6), ("area", ctypes.c_int64 * 6), ("part_min_copies", ctypes.c_void_p),
+                ("part_no_top", ctypes.c_void_p), ("part_flags", ctypes.c_void_p), ("dom_peak", ctypes.c_void_p),
+                ("dom_peak_stage", ctypes.c_void_p), ("dom_peak_round", ctypes.c_void_p)]
+
+
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_chains", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_chains", "blance_plan_chains_exposure", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
            "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_exposure", "blance_moves_free")
 
@@ -139,6 +148,8 @@ def capi():
         lib.blance_plan_scenarios_audit.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         lib.blance_plan_scenarios_exposure.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp]
         lib.blance_plan_chains.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, vp, vp]
+        lib.blance_plan_chains_exposure.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp,
+                                                    vp, vp, vp]
         lib.blance_map_audit.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.blance_plan_audit.argtypes = [vp, vp, vp, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
@@ -174,3 +185,4 @@ AuditOpts = _AuditOpts
 AuditOut = _AuditOut
 ExposureIn = _ExposureIn
 ExposureOut = _ExposureOut
+ChainSpanOut = _ChainSpanOut

@@ -147,7 +147,7 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
 
 
 def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None, chains=(), favorMinNodes=False,
-                      wantMaps=(), maxConcurrent=0):
+                      wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None, exposure=None):
     """Chains of cluster changes, each stage planned on the map the stage before produced (blance_plan_chains).  Chain
     i runs the Go loop `next = PlanNextMapEx(prev, assign, nodesAll_t, nodesToRemove_t, nodesToAdd_t, model, options_i_t);
     prev = prev with every entry of next replaced; assign = next` over its stages.  nodesAll is the universe: a stage's
@@ -161,7 +161,16 @@ def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None
 
     Returns one dict per chain: "stages", one dict per stage with the keys of PlanNextMapScenarios' results (next_map
     and warnings for the chains in wantMaps), and "net": node_ops, ops_total and parts_moved of CalcPartitionMoves
-    from the base prevMap to the last stage's map."""
+    from the base prevMap to the last stage's map.
+
+    scheduleConcurrency, audit and exposure (as PlanNextMapScenarios; the movers are the universe) add "schedules",
+    "audit" and "exposures" to every stage's dict, with that stage's prevMap as begMap.  Then "net" also gets
+    "schedules" (and with exposure "exposures") of the direct rebalance from prevMap to the last stage's map, and each
+    chain dict a "span" list, one dict per value: the chain's stages folded on one global round axis (rounds,
+    moves_done, stuck_parts, max_batch; node_rounds / node_last_round {node: ...}; part_done_round {partition: ...,
+    -1 = stuck in some stage}; with exposure peak / peak_stage / peak_round / area {metric: ...}, part_min_copies /
+    part_no_top / part_flags {partition: ...}, dom_peak / dom_peak_stage / dom_peak_round {name: ...}), nonzero
+    entries only."""
     o = options or PlanNextMapOptions()
     same = prevMap is partitionsToAssign
     cs = []
@@ -180,7 +189,10 @@ def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None
         cs.append((_scenario_tuples([opts])[0], stages))
     return _host.PlanNextMapChains(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                    {k: tuple(v) for k, v in model.items()}, cs, bool(favorMinNodes),
-                                   [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o))
+                                   [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o),
+                                   schedule_concurrency=[int(c) for c in scheduleConcurrency],
+                                   audit=None if audit is None else bool(audit.get("failoverSpread", False)),
+                                   exposure_series_cap=None if exposure is None else int(exposure.get("seriesCap", 0)))
 
 
 def AuditMap(partitionMap, nodesAll, model, options=None, failoverSpread=False):

@@ -1678,12 +1678,33 @@ static void expo_unpack(const ExpoResult& r, long long i, int R, const unsigned 
   }
 }
 
-// The chains requested with blance_plan_chains: T stages per chain, stages [n][T], net [n] or NULL.
+// The chains requested with blance_plan_chains: T stages per chain, stages [n][T], net [n] or NULL; with
+// blance_plan_chains_exposure the net rebalance's schedules and exposures [n][nc] and the spans [n][nc], each or NULL,
+// and which span arrays any span asks for (span_parts: the per-partition exposure arrays, span_dom: the per-vertex).
 struct ChainReq {
   int T = 1;
   const blance_chain_stage* stages = nullptr;
   blance_chain_out* net = nullptr;
+  blance_scenario_schedule_out* net_sched = nullptr;
+  blance_exposure_out* net_expo = nullptr;
+  blance_chain_span_out* span = nullptr;
+  bool span_parts = false, span_dom = false;
 };
+
+// The span accumulators of nw chains x nc counts (k_chain_fold) and each instance's G_t: the schedule's always, the
+// per-partition exposure arrays with span_parts, the per-vertex ones with span_dom.
+struct SpanBufs {
+  ChainFold F{};
+  long long* G = nullptr;
+};
+
+static void span_slices(Arena& a, SpanBufs& b, const ChainReq& cr, long long nw, long long nc, long long PU, long long NU, long long V) {
+  const long long ni = nw * nc;
+  a.add(b.G, (size_t)ni);
+  a.add(b.F.a_part_done, (size_t)(ni * PU)); a.add(b.F.a_node_rounds, (size_t)(ni * NU)); a.add(b.F.a_node_last, (size_t)(ni * NU));
+  if (cr.span_parts) { a.add(b.F.a_part_min, (size_t)(ni * PU)); a.add(b.F.a_part_notop, (size_t)(ni * PU)); a.add(b.F.a_part_flags, (size_t)(ni * PU)); }
+  if (cr.span_dom) { a.add(b.F.a_dom_peak, (size_t)(ni * V)); a.add(b.F.a_dom_stage, (size_t)(ni * V)); a.add(b.F.a_dom_round, (size_t)(ni * V)); }
+}
 
 // The node fields of scenario (or chain) i at stage t.
 static const blance_scenario& nodes_of(const blance_scenario* sc, const ChainReq* cr, int i, int t) {
@@ -1743,18 +1764,19 @@ static void wave_summary(blance_ctx* ctx, blance_plan* pl, int nw, const int32_t
   else launch(ctx, k_scenario_summary<false>, grid, 256, 0, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
 }
 
-// The exposures of a wave's nw scenarios x nc counts after their schedules (scal: the instances' scalars), on the
-// op table and rounds the schedule left in W and the buffers of b; wave member j is scenario idx[j].  Copies every
-// result out into er.out; *ms and *bytes: the device time and the bytes allocated after the schedule.
-static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan* pl, int nw, int nc, const int* idx,
-                          const blance_plan_in& base, const WSched& W, ExpoBufs& b, const std::vector<unsigned long long>& scal,
-                          float* ms, size_t* bytes) {
+// The exposures of a wave's nw scenarios x nc counts after their schedules (scal: the instances' scalars), from the
+// beg rows / flags `beg` / `pflags` over the op table and rounds the schedule left in W, on the buffers of b.  Copies
+// the result of instance i out into *outs[i]; *ms and *bytes: the device time and the bytes allocated after the
+// schedule.  The per-partition outputs and fault-domain keys stay in b until the wave's next exposure.
+static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan* pl, int nw, int nc, const int32_t* beg, const uint8_t* pflags,
+                          const std::vector<blance_exposure_out*>& outs, const blance_plan_in& base, const WSched& W, ExpoBufs& b,
+                          const std::vector<unsigned long long>& scal, float* ms, size_t* bytes) {
   cudaStream_t st = ctx->stream;
   const int PU = base.n_parts, S = base.n_states;
   const long long ni = (long long)nw * nc, V = (long long)base.n_node_ids + er.n_domains;
   ExpoArgs& E = b.E;
   E.op_off = nullptr; E.op_n = W.op_n; E.op_node = W.op_node; E.op_state = W.op_state; E.op_kind = W.op_kind; E.op_round = W.op_round;
-  E.beg = pl->prev_rows_init; E.pflags = pl->pflags_init; E.dom_parent = b.parent;
+  E.beg = beg; E.pflags = pflags; E.dom_parent = b.parent;
   E.stride = pl->h_insts[0].SLP; E.P = PU; E.SL = base.n_slots; E.S = S; E.NU = base.n_node_ids; E.V = (int32_t)V;
   E.MO = W.MO; E.top = base.top_state;
   for (int s = 0; s <= S; ++s) E.slot_off[s] = base.state_slot_off[s];
@@ -1773,7 +1795,7 @@ static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan*
   std::vector<unsigned long long> h_key(er.dom ? (size_t)(ni * V) : 0);
   if (!h_key.empty()) CUDA(cudaMemcpyAsync(h_key.data(), b.dom_key, sizeof(unsigned long long) * h_key.size(), cudaMemcpyDeviceToHost, st));
   for (long long i = 0; i < ni; ++i) {
-    blance_exposure_out& o = er.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    blance_exposure_out& o = *outs[(size_t)i];
     const long long R1 = (long long)inst[(size_t)i].R + 1, w = std::min<long long>(R1, er.series_cap);
     if (o.series && w > 0)        // [BLANCE_EXPO_N][series_cap] <- the first w of each metric's R + 1 values
       CUDA(cudaMemcpy2DAsync(o.series, sizeof(int64_t) * (size_t)er.series_cap, E.diff + inst[(size_t)i].diff_off, sizeof(long long) * (size_t)R1,
@@ -1789,7 +1811,7 @@ static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan*
   cudaEventElapsedTime(ms, ctx->ev[6], ctx->ev[7]);
   *bytes = r.bytes;
   for (long long i = 0; i < ni; ++i) {
-    blance_exposure_out& o = er.out[(size_t)idx[i / nc] * nc + (size_t)(i % nc)];
+    blance_exposure_out& o = *outs[(size_t)i];
     expo_unpack(r, i, inst[(size_t)i].R, er.dom ? h_key.data() + i * V : nullptr, (int)V, o);
     o.kernel_ms = *ms;
   }
@@ -1814,7 +1836,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     max_mask = std::max(max_mask, mask_words(in));
     max_ow = std::max(max_ow, n_overrides(opts_of(opts, i)));
     max_rules = std::max(max_rules, in.has_hier_rules ? in.n_rules : 0);
-    audit_flags |= ar && ar->out[i].part_flags;
+    for (int t = 0; ar && t < T; ++t) audit_flags |= ar->out[(size_t)i * T + t].part_flags != nullptr;
   }
   size_t extra_bytes = 0;              // one scenario's audit buffers / one chain's net buffers, priced into the wave
   if (ar) {
@@ -1848,6 +1870,13 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     uint8_t* f = nullptr;
     long long* d = nullptr;
     one.add(r, (size_t)pb->RT + 4); one.add(f, (size_t)pb->PT + 1); one.add(d, (size_t)stride);
+    extra_bytes += one.bytes();
+  }
+  const bool want_span = cr && cr->span;
+  if (want_span) {                     // one chain's span accumulators
+    Arena one;
+    SpanBufs b;
+    span_slices(one, b, *cr, 1, sr->nc, base->n_parts, base->n_node_ids, V);
     extra_bytes += one.bytes();
   }
   size_t per = 0;
@@ -1904,6 +1933,8 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
     uint8_t* net_flags = nullptr;
     long long* d_net = nullptr;
     if (want_net) { wave.add(net_prev, (size_t)pl->RT + 4); wave.add(net_flags, (size_t)pl->PT + 1); wave.add(d_net, (size_t)(stride * nw)); }
+    SpanBufs sbuf;
+    if (want_span) span_slices(wave, sbuf, *cr, nw, sr->nc, PU, NU, V);
     try {
       wave.alloc(st, "a scenario wave");
     } catch (const Error&) {
@@ -1934,6 +1965,43 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
       CUDA(cudaMemcpyAsync(net_flags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
     }
     if (!lone) finish_upload(ctx, pl);
+    // the caller's outputs of wave member j (at stage t) and instance i = j * nc + k
+    auto out_index = [&](int j, int t) { return (size_t)idx[(size_t)(w0 + j)] * T + t; };
+    auto expo_outs = [&](int t, blance_exposure_out* o, int per) {
+      std::vector<blance_exposure_out*> v;
+      for (long long i = 0; i < (long long)nw * sr->nc; ++i)
+        v.push_back(o + ((size_t)idx[(size_t)(w0 + i / sr->nc)] * per + t) * sr->nc + (size_t)(i % sr->nc));
+      return v;
+    };
+    std::vector<long long> G(want_span ? (size_t)nw * sr->nc : 0, 0);    // each instance's G_t
+    // the schedules of the wave's instances from the beg rows / flags `beg` / `pflags` to the working rows, each
+    // scenario's ops per node read from its summary in `sum`; instance i's result goes to outs[(idx * per + t) * nc + k]
+    // (outs NULL: kept on the device only).  Returns the instances' scalars.
+    auto schedule = [&](const int32_t* beg, const uint8_t* pflags, const std::vector<long long>& sum, blance_scenario_schedule_out* outs,
+                        int per, int t) {
+      if (er) {
+        CUDA(cudaMemsetAsync(wsch.op_round, 0xFF, sizeof(int32_t) * (size_t)nw * sr->nc * PU * scenario_ops(*base), st));
+        if (ebuf.parent) CUDA(cudaMemcpyAsync(ebuf.parent, er->parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
+      }
+      if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, pl->pool, beg, pflags, favor_min, wsch);
+      std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
+      for (size_t x = 0; x < ops.size(); ++x) {
+        const long long* s = sum.data() + (x / NU) * stride + 4 * (x % NU);
+        ops[x] = s[0] + s[1] + s[2] + s[3];
+      }
+      std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
+      for (long long i = 0; outs && i < (long long)nw * sr->nc; ++i) {
+        blance_scenario_schedule_out& o = outs[((size_t)idx[(size_t)(w0 + i / sr->nc)] * per + t) * sr->nc + (size_t)(i % sr->nc)];
+        o.rounds = (int32_t)scal[(size_t)(4 * i)];
+        o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
+        o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
+        o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
+        if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+        if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+        if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
+      }
+      return scal;
+    };
     for (int t = 0; t < T; ++t) {
       if (t > 0) {
         // the stage boundary: what the convergence loop left in the working state is the next stage's input - the
@@ -1961,7 +2029,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
       if (want_net && t == T - 1) wave_summary(ctx, pl, nw, net_prev, net_flags, favor_min, stride, d_net);
       CUDA(cudaEventRecord(ctx->ev[2], st));
       // the output of wave member j at this stage
-      auto out_of = [&](int j) -> blance_scenario_out& { return out[(size_t)idx[(size_t)(w0 + j)] * T + t]; };
+      auto out_of = [&](int j) -> blance_scenario_out& { return out[out_index(j, t)]; };
       // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
       std::vector<AuditInst> a_insts;
       std::vector<std::vector<long long>> a_host((size_t)(ar ? nw : 0));
@@ -1977,7 +2045,7 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
           a_insts.push_back(A);
         }
         audit_run(ctx, abuf, *ar, a_insts);
-        for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
+        for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[out_index(j, t)]);
       }
       bool any_rows = false;
       for (int j = 0; j < nw; ++j) {
@@ -2009,37 +2077,53 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
         o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
         o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
         o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
-        if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[idx[(size_t)(w0 + j)]]);
+        if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[out_index(j, t)]);
       }
-      float expo_ms = 0.f;
+      float expo_ms = 0.f, fold_ms = 0.f;
       size_t expo_bytes = 0;
       if (sr) {
         CUDA(cudaEventRecord(ctx->ev[3], st));
-        if (er) {
-          CUDA(cudaMemsetAsync(wsch.op_round, 0xFF, sizeof(int32_t) * (size_t)nw * sr->nc * PU * scenario_ops(*base), st));
-          if (ebuf.parent) CUDA(cudaMemcpyAsync(ebuf.parent, er->parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
-        }
-        if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, P, pl->prev_rows_init, pl->pflags_init, favor_min, wsch);
-        std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
-        for (size_t x = 0; x < ops.size(); ++x) {
-          const long long* s = h_sum.data() + (x / NU) * stride + 4 * (x % NU);
-          ops[x] = s[0] + s[1] + s[2] + s[3];
-        }
-        const std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
-        for (long long i = 0; i < (long long)nw * sr->nc; ++i) {
-          blance_scenario_schedule_out& o = sr->out[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
-          o.rounds = (int32_t)scal[(size_t)(4 * i)];
-          o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
-          o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
-          o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
-          if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-          if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-          if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
-        }
+        const std::vector<unsigned long long> scal = schedule(pl->prev_rows_init, pl->pflags_init, h_sum, sr->out, T, t);
         CUDA(cudaEventRecord(ctx->ev[1], st));
         CUDA(cudaEventSynchronize(ctx->ev[1]));
         cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
-        if (er) wave_exposure(ctx, *er, pl, nw, sr->nc, idx.data() + w0, *base, wsch, ebuf, scal, &expo_ms, &expo_bytes);
+        const std::vector<blance_exposure_out*> eo = er ? expo_outs(t, er->out, T) : std::vector<blance_exposure_out*>();
+        if (er) wave_exposure(ctx, *er, pl, nw, sr->nc, pl->prev_rows_init, pl->pflags_init, eo, *base, wsch, ebuf, scal, &expo_ms, &expo_bytes);
+        if (want_span) {
+          // the stage folded into the span before the next stage boundary overwrites the schedule and exposure
+          CUDA(cudaEventRecord(ctx->ev[4], st));
+          ChainFold F = sbuf.F;
+          F.node_rounds = wsch.node_rounds; F.node_last = wsch.node_last; F.part_done = wsch.part_done;
+          F.part_min = ebuf.E.part_min; F.part_notop = ebuf.E.part_notop; F.part_flags = ebuf.E.part_flags;
+          F.dom_key = ebuf.dom_key; F.G = sbuf.G;
+          F.ni = (long long)nw * sr->nc; F.PU = PU; F.NU = NU; F.V = (int32_t)V; F.stage = t;
+          CUDA(cudaMemcpyAsync(sbuf.G, G.data(), sizeof(long long) * G.size(), cudaMemcpyHostToDevice, st));
+          const long long n_el = F.ni * ((long long)PU + NU + V);
+          if (n_el > 0) launch(ctx, k_chain_fold, grid_for(ctx, n_el, 256), 256, 0, F);
+          CUDA(cudaEventRecord(ctx->ev[5], st));
+          CUDA(cudaEventSynchronize(ctx->ev[5]));     // G is rewritten below
+          cudaEventElapsedTime(&fold_ms, ctx->ev[4], ctx->ev[5]);
+          for (long long i = 0; i < F.ni; ++i) {
+            blance_chain_span_out& s = cr->span[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
+            const int R = (int)scal[(size_t)(4 * i)];
+            if (t == 0) {
+              s.rounds = s.moves_done = s.stuck_parts = 0;
+              s.max_batch = 0;
+              for (int m = 0; m < BLANCE_EXPO_N; ++m) { s.peak[m] = 0; s.peak_stage[m] = 0; s.peak_round[m] = 0; s.area[m] = 0; }
+            }
+            s.rounds += R;
+            s.moves_done += (int64_t)scal[(size_t)(4 * i + 1)];
+            s.stuck_parts += (int64_t)scal[(size_t)(4 * i + 2)];
+            s.max_batch = std::max(s.max_batch, (int32_t)scal[(size_t)(4 * i + 3)]);
+            G[(size_t)i] += R;
+            if (!er) continue;
+            const blance_exposure_out& e = *eo[(size_t)i];
+            for (int m = 0; m < BLANCE_EXPO_N; ++m) {
+              if (t == 0 || e.peak[m] > s.peak[m]) { s.peak[m] = e.peak[m]; s.peak_stage[m] = t; s.peak_round[m] = e.peak_round[m]; }
+              s.area[m] += e.area[m];
+            }
+          }
+        }
       }
       if (times) {
         float wave_ms = 0.f;
@@ -2048,6 +2132,8 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
                      w0, nw, W, per, wave_ms, sum_ms);
         if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
         if (er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", expo_ms, expo_bytes);
+        if (want_span) std::fprintf(stderr, ", span fold %.3f ms", fold_ms);
+        if (cr) std::fprintf(stderr, " (stage %d)", t);
         std::fprintf(stderr, "\n");
       }
     }
@@ -2061,6 +2147,38 @@ static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, con
         if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
         o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2];
       }
+      // the direct rebalance from the base's prevMap to the last stage's final map, on the wave's schedule and
+      // exposure buffers (the last stage's were copied out and folded above)
+      if (cr->net_sched || cr->net_expo) {
+        const std::vector<unsigned long long> scal = schedule(net_prev, net_flags, h_net, cr->net_sched, 1, 0);
+        if (cr->net_expo) {
+          float ms = 0.f;
+          size_t bytes = 0;
+          wave_exposure(ctx, *er, pl, nw, sr->nc, net_prev, net_flags, expo_outs(0, cr->net_expo, 1), *base, wsch, ebuf, scal, &ms, &bytes);
+        }
+      }
+    }
+    if (want_span) {                   // the folded arrays out
+      const long long ni = (long long)nw * sr->nc;
+      const SpanBufs& b = sbuf;
+      for (long long i = 0; i < ni; ++i) {
+        blance_chain_span_out& s = cr->span[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
+        auto d2h = [&](void* dst, const void* src, size_t bytes) { if (dst && src && bytes) CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st)); };
+        d2h(s.node_rounds, b.F.a_node_rounds + i * NU, sizeof(int32_t) * NU);
+        d2h(s.node_last_round, b.F.a_node_last + i * NU, sizeof(int64_t) * NU);
+        d2h(s.part_done_round, b.F.a_part_done + i * PU, sizeof(int64_t) * PU);
+        if (cr->span_parts) {
+          d2h(s.part_min_copies, b.F.a_part_min + i * PU, sizeof(int32_t) * PU);
+          d2h(s.part_no_top, b.F.a_part_notop + i * PU, sizeof(int32_t) * PU);
+          d2h(s.part_flags, b.F.a_part_flags + i * PU, (size_t)PU);
+        }
+        if (cr->span_dom) {
+          d2h(s.dom_peak, b.F.a_dom_peak + i * V, sizeof(int64_t) * V);
+          d2h(s.dom_peak_stage, b.F.a_dom_stage + i * V, sizeof(int32_t) * V);
+          d2h(s.dom_peak_round, b.F.a_dom_round + i * V, sizeof(int32_t) * V);
+        }
+      }
+      CUDA(cudaStreamSynchronize(st));
     }
     w0 += nw;
   }
@@ -2107,10 +2225,8 @@ static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_
 
 // Chains of stages over one base (blance_plan_chains): chain i -> device i mod G, its stages planned in lock step
 // with the other chains of its wave.
-static void plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
-                        const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
-                        blance_chain_out* net) {
-  const std::string name = "blance_plan_chains";
+static void check_chains(const std::string& name, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
+                         const blance_scenario_opts* opts, blance_scenario_out* out) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
   if (n_stages < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_stages must be positive");
   if (!base || !stages || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
@@ -2128,14 +2244,18 @@ static void plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, 
         if (cs.node_in_all[q] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
       if (st != BLANCE_OK) throw_err(st, name + ": chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": " + why);
     }
+}
+
+// Plans the checked chains of cr (chain i -> device i mod G), with the schedules, audits and exposures asked for.
+static void plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const ChainReq& cr, const blance_scenario_opts* opts,
+                        int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out, const SchedReq* sr = nullptr,
+                        const AuditReq* ar = nullptr, const ExpoReq* er = nullptr) {
   if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  ChainReq cr;
-  cr.T = n_stages; cr.stages = stages; cr.net = net;
   const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
   fan_out(ctx, G, [&](int d, blance_ctx* dev) {
-    scenarios_on_device(dev, base, idx[(size_t)d], nullptr, opts, favor_min_nodes, max_concurrent, out, nullptr, nullptr, &cr);
+    scenarios_on_device(dev, base, idx[(size_t)d], nullptr, opts, favor_min_nodes, max_concurrent, out, sr, ar, &cr, er);
   });
 }
 
@@ -2143,7 +2263,89 @@ extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, i
                                   const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
                                   int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
   return entry(ctx, [&](Device&) {
-    plan_chains(ctx, base, n, n_stages, stages, opts, favor_min_nodes, max_concurrent, out, net);
+    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, out);
+    ChainReq cr;
+    cr.T = n_stages; cr.stages = stages; cr.net = net;
+    plan_chains(ctx, base, n, cr, opts, favor_min_nodes, max_concurrent, out);
+  });
+}
+
+static SchedReq sched_req(const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc, const blance_scenario_out* out,
+                          int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                          blance_scenario_schedule_out* sched);
+
+// The checked exposure request of eopts / series_cap, the flags of the outputs asked for in the [n_out] `outs` (NULL:
+// none) added to er.  `what(x)` names output x in a message.
+template <class Name>
+static void expo_flags(const std::string& name, const blance_plan_in& base, const blance_exposure_out* outs, long long n_out, Name&& what,
+                       ExpoReq& er) {
+  for (long long x = 0; outs && x < n_out; ++x) {
+    const blance_exposure_out& o = outs[x];
+    er.dom |= o.dom_peak || o.dom_peak_round;
+    er.part_min |= o.part_min_copies != nullptr;
+    er.part_notop |= o.part_no_top != nullptr;
+    er.part_flags |= o.part_flags != nullptr;
+    if ((o.dom_peak || o.dom_peak_round) && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base.n_slots) * std::max(0, base.n_parts) >= (1ll << 31))
+      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": " + what(x) + ": dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+  }
+}
+
+extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                           const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
+                                           int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
+                                           const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
+                                           blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
+                                           const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
+                                           blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo,
+                                           blance_chain_span_out* span) {
+  return entry(ctx, [&](Device&) {
+    const std::string name = "blance_plan_chains_exposure";
+    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
+    const int T = n_stages, nc = n_move_conc;
+    if ((net_sched || net_expo) && !net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_sched and net_expo need net");
+    AuditReq ar;
+    if (audit) {
+      ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
+      for (int i = 0; stages && T > 0 && i < n; ++i) {
+        const blance_plan_in in = scenario_in(*base, stages[(size_t)i * T].nodes, opts_of(opts, i));
+        check_audit_model(name + ": chain " + std::to_string(i), &in);
+      }
+    }
+    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive");
+    // sched_req reads n x nc outputs; a chain has T x nc of them, cleared here
+    SchedReq sr = sched_req(name.c_str(), base, 0, nullptr, nullptr, n_move_conc, move_conc, node_has_mover, sched);
+    for (long long x = 0; x < (long long)std::max(0, n) * std::max(0, T) * nc; ++x) { sched[x].rounds = 0; sched[x].moves_done = 0; sched[x].stuck_parts = 0; sched[x].max_batch = 0; }
+    if (series_cap < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": series_cap is negative");
+    ExpoReq er;
+    er.series_cap = series_cap;
+    er.out = expo;
+    if (eopts) {
+      if (eopts->flags) throw_err(BLANCE_ERR_INVALID_ARG, name + ": eopts.flags must be 0 (eopts carries a forest only)");
+      check_forest(name, eopts->n_domains, eopts->domain_parent, base->n_node_ids);
+      er.n_domains = eopts->n_domains;
+      er.parent = eopts->domain_parent;
+    }
+    ChainReq cr;
+    cr.T = T; cr.stages = stages; cr.net = net; cr.net_sched = net_sched; cr.net_expo = net_expo; cr.span = span;
+    for (long long x = 0; span && x < (long long)std::max(0, n) * nc; ++x) {
+      const blance_chain_span_out& s = span[x];
+      cr.span_parts |= s.part_min_copies || s.part_no_top || s.part_flags;
+      cr.span_dom |= s.dom_peak || s.dom_peak_stage || s.dom_peak_round;
+    }
+    if (!expo && (net_expo || cr.span_parts || cr.span_dom))
+      throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_expo and the span's exposure arrays need expo");
+    auto stage_name = [&](long long x) {
+      return "chain " + std::to_string(x / ((long long)T * nc)) + ", stage " + std::to_string(x / nc % T) + ", count " + std::to_string(x % nc);
+    };
+    auto pair_name = [&](long long x) { return "chain " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
+    expo_flags(name, *base, expo, (long long)std::max(0, n) * std::max(0, T) * nc, stage_name, er);
+    expo_flags(name, *base, net_expo, (long long)std::max(0, n) * nc, pair_name, er);
+    if (cr.span_dom && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base->n_slots) * std::max(0, base->n_parts) >= (1ll << 31))
+      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": span: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+    er.dom |= cr.span_dom;
+    er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
+    check_chains(name, base, n, n_stages, stages, opts, out);
+    plan_chains(ctx, base, n, cr, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, expo ? &er : nullptr);
   });
 }
 

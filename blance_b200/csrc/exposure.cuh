@@ -319,4 +319,60 @@ __global__ void k_expo_dom_max(int n, const unsigned long long* __restrict__ key
   }
 }
 
+// The span of a chain wave (blance_plan_chains_exposure): one stage's schedule summaries, per-partition exposures and
+// fault-domain maxima folded into per-instance accumulators.  Inputs are [ni][NU], [ni][PU] and [ni][V] as the
+// schedule (WSched), the exposure walk (ExpoArgs) and k_expo_dom_max leave them; a null input or accumulator is not
+// folded.  G[i] is the global round at which this stage starts for instance i.
+struct ChainFold {
+  const int32_t* node_rounds; const int32_t* node_last; const int32_t* part_done;
+  const int32_t* part_min; const int32_t* part_notop; const uint8_t* part_flags;
+  const unsigned long long* dom_key;
+  const long long* G;
+  int32_t* a_node_rounds; long long* a_node_last; long long* a_part_done;
+  int32_t* a_part_min; int32_t* a_part_notop; uint8_t* a_part_flags;
+  long long* a_dom_peak; int32_t* a_dom_stage; int32_t* a_dom_round;
+  long long ni;
+  int32_t PU, NU, V, stage;
+};
+
+// One thread per accumulator element (instance, partition | node | vertex), stages folded in launch order: no atomics.
+// Stage 0 starts every accumulator from its identity instead of reading it.
+__global__ void __launch_bounds__(256) k_chain_fold(const ChainFold F) {
+  const long long W = (long long)F.PU + F.NU + F.V, n = F.ni * W;
+  const bool first = F.stage == 0;
+  for (long long x = blockIdx.x * (long long)blockDim.x + threadIdx.x; x < n; x += (long long)gridDim.x * blockDim.x) {
+    const long long i = x / W, e = x - i * W, G = F.G[i];
+    if (e < F.PU) {
+      const long long c = i * F.PU + e;
+      if (F.a_part_done) {
+        const long long old = first ? 0 : F.a_part_done[c];
+        const int32_t d = F.part_done[c];
+        F.a_part_done[c] = old == -1 || d == -1 ? -1 : d > 0 ? G + d : old;
+      }
+      if (F.a_part_min) {
+        const int32_t old = first ? -1 : F.a_part_min[c], m = F.part_min[c];
+        F.a_part_min[c] = m < 0 ? old : old < 0 ? m : min(old, m);
+      }
+      if (F.a_part_notop) F.a_part_notop[c] = (first ? 0 : F.a_part_notop[c]) + F.part_notop[c];
+      if (F.a_part_flags) F.a_part_flags[c] = (uint8_t)((first ? 0 : F.a_part_flags[c]) | F.part_flags[c]);
+    } else if (e < F.PU + F.NU) {
+      const long long c = i * F.NU + (e - F.PU);
+      if (F.a_node_rounds) F.a_node_rounds[c] = (first ? 0 : F.a_node_rounds[c]) + F.node_rounds[c];
+      if (F.a_node_last) {
+        const int32_t l = F.node_last[c];
+        F.a_node_last[c] = l > 0 ? G + l : first ? 0 : F.a_node_last[c];
+      }
+    } else if (F.a_dom_peak) {
+      const long long c = i * F.V + (e - F.PU - F.NU);
+      const unsigned long long key = F.dom_key[c];
+      const long long cnt = (long long)(key >> 32);
+      if (first || cnt > F.a_dom_peak[c]) {
+        F.a_dom_peak[c] = cnt;
+        F.a_dom_stage[c] = F.stage;
+        F.a_dom_round[c] = (int32_t)(0xFFFFFFFFu - (uint32_t)key);
+      }
+    }
+  }
+}
+
 }  // namespace blance_dev

@@ -1342,6 +1342,78 @@ ExposureResult name_exposure(const ExposureBuffers& b, size_t cap, const Strs& v
   return r;
 }
 
+// One schedule summary by name, at MaxConcurrentPartitionMovesPerNode `count`.
+ScenarioSchedule name_schedule(const InternedPlan& ip, const blance_scenario_schedule_out& so, int count) {
+  ScenarioSchedule s;
+  s.MaxConcurrentPartitionMovesPerNode = count;
+  s.Rounds = so.rounds; s.MovesDone = so.moves_done; s.StuckParts = so.stuck_parts; s.MaxBatch = so.max_batch;
+  for (int32_t q = 0; q < ip.in.n_node_ids; ++q) {
+    if (so.node_rounds[q]) s.NodeRounds[ip.node_names[size_t(q)]] = so.node_rounds[q];
+    if (so.node_last_round[q]) s.NodeLastRound[ip.node_names[size_t(q)]] = so.node_last_round[q];
+  }
+  return s;
+}
+
+// Output buffers of n x nc blance_scenario_schedule_out (per-node arrays only, as ScenarioSchedule reports).
+struct ScheduleBuffers {
+  std::vector<blance_scenario_schedule_out> out;
+  std::vector<int32_t> node_rounds, node_last;
+  ScheduleBuffers(size_t count, size_t NU) : out(count), node_rounds(count * NU + 1), node_last(count * NU + 1) {
+    for (size_t x = 0; x < count; ++x) {
+      out[x] = blance_scenario_schedule_out{};
+      out[x].node_rounds = node_rounds.data() + x * NU;
+      out[x].node_last_round = node_last.data() + x * NU;
+    }
+  }
+};
+
+// Output buffers of one blance_chain_span_out: NU node ids, P partitions, V vertices; exposure arrays with `expo`.
+struct SpanBuffers {
+  std::vector<int32_t> node_rounds, min_copies, no_top, dom_stage, dom_round;
+  std::vector<int64_t> node_last, part_done, dom_peak;
+  std::vector<uint8_t> flags;
+  blance_chain_span_out out{};
+  SpanBuffers(size_t NU, size_t P, size_t V, bool expo)
+      : node_rounds(NU + 1), min_copies(P + 1), no_top(P + 1), dom_stage(V + 1), dom_round(V + 1), node_last(NU + 1), part_done(P + 1),
+        dom_peak(V + 1), flags(P + 1) {
+    out.node_rounds = node_rounds.data(); out.node_last_round = node_last.data(); out.part_done_round = part_done.data();
+    if (expo) {
+      out.part_min_copies = min_copies.data(); out.part_no_top = no_top.data(); out.part_flags = flags.data();
+      out.dom_peak = dom_peak.data(); out.dom_peak_stage = dom_stage.data(); out.dom_peak_round = dom_round.data();
+    }
+  }
+};
+
+ChainSpan name_span(const InternedPlan& ip, const SpanBuffers& b, int count, const Strs& vnames) {
+  static const char* kMetrics[BLANCE_EXPO_N] = {"NO_TOP", "MULTI_TOP", "SHORT", "ONE_COPY", "NO_COPY", "COPIES"};
+  const blance_chain_span_out& o = b.out;
+  ChainSpan r;
+  r.MaxConcurrentPartitionMovesPerNode = count;
+  r.Rounds = o.rounds; r.MovesDone = o.moves_done; r.StuckParts = o.stuck_parts; r.MaxBatch = o.max_batch;
+  for (int32_t q = 0; q < ip.in.n_node_ids; ++q) {
+    if (b.node_rounds[size_t(q)]) r.NodeRounds[ip.node_names[size_t(q)]] = b.node_rounds[size_t(q)];
+    if (b.node_last[size_t(q)]) r.NodeLastRound[ip.node_names[size_t(q)]] = b.node_last[size_t(q)];
+  }
+  const size_t P = ip.part_names.size();
+  for (size_t p = 0; p < P; ++p)
+    if (b.part_done[p]) r.PartDoneRound[ip.part_names[p]] = b.part_done[p];
+  if (!o.part_min_copies) return r;
+  for (size_t m = 0; m < BLANCE_EXPO_N; ++m) {
+    r.Peak[kMetrics[m]] = o.peak[m]; r.Area[kMetrics[m]] = o.area[m];
+    r.PeakStage[kMetrics[m]] = o.peak_stage[m]; r.PeakRound[kMetrics[m]] = o.peak_round[m];
+  }
+  for (size_t p = 0; p < P; ++p) {
+    if (b.min_copies[p] > 0) r.PartMinCopies[ip.part_names[p]] = b.min_copies[p];
+    if (b.no_top[p] > 0) r.PartNoTop[ip.part_names[p]] = b.no_top[p];
+    if (b.flags[p]) r.PartFlags[ip.part_names[p]] = b.flags[p];
+  }
+  for (size_t v = 0; v < vnames.size(); ++v)
+    if (b.dom_peak[v] > 0) {
+      r.DomPeak[vnames[v]] = b.dom_peak[v]; r.DomPeakStage[vnames[v]] = b.dom_stage[v]; r.DomPeakRound[vnames[v]] = b.dom_round[v];
+    }
+  return r;
+}
+
 }  // namespace
 
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
@@ -1439,15 +1511,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
     r = scenario_result(*ip, out[i], ops[i], load[i], want[i] ? maps[i].get() : nullptr, k);
     for (size_t k = 0; k < nc; ++k) {
-      const blance_scenario_schedule_out& so = sched[i * nc + k];
-      ScenarioSchedule s;
-      s.MaxConcurrentPartitionMovesPerNode = scheduleConcurrency[k];
-      s.Rounds = so.rounds; s.MovesDone = so.moves_done; s.StuckParts = so.stuck_parts; s.MaxBatch = so.max_batch;
-      for (int32_t q = 0; q < NU; ++q) {
-        if (so.node_rounds[q]) s.NodeRounds[ip->node_names[size_t(q)]] = so.node_rounds[q];
-        if (so.node_last_round[q]) s.NodeLastRound[ip->node_names[size_t(q)]] = so.node_last_round[q];
-      }
-      r.Schedules.push_back(std::move(s));
+      r.Schedules.push_back(name_schedule(*ip, sched[i * nc + k], scheduleConcurrency[k]));
     }
     if (audit) {
       abuf[i]->out = aout[i];
@@ -1465,8 +1529,12 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
 std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                            const Strs& nodesAll, const PartitionModel& model,
                                            const PlanNextMapOptions& options, const std::vector<Chain>& chains,
-                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent) {
+                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
+                                           const std::vector<int>& scheduleConcurrency, const ScenarioAudit* audit,
+                                           const ScenarioExposure* exposure) {
   if (chains.empty()) invalid("PlanNextMapChains: no chains");
+  if ((audit || exposure) && scheduleConcurrency.empty()) invalid("PlanNextMapChains: an audit or exposure needs scheduleConcurrency");
+  if (exposure && exposure->SeriesCap < 0) invalid("PlanNextMapChains: SeriesCap is negative");
   const size_t n = chains.size(), T = chains[0].Stages.size();
   if (T == 0) invalid("PlanNextMapChains: chain 0 has no stages");
   for (size_t i = 0; i < n; ++i)
@@ -1544,19 +1612,85 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     net[i] = blance_chain_out{};
     net[i].node_ops = net_ops[i].data();
   }
+  // the analyses (blance_plan_chains_exposure): per stage [n][T][nc], the net rebalance and the spans [n][nc]
+  const size_t nc = scheduleConcurrency.size(), P = size_t(ip->in.n_parts);
+  ScheduleBuffers sched(n * T * nc, size_t(NU)), net_sched(n * nc, size_t(NU));
+  Forest forest, eforest;
+  std::vector<std::unique_ptr<AuditBuffers>> abuf;
+  std::vector<blance_audit_out> aout;
+  auto rules_of = [&](size_t i) -> const int32_t* {
+    const ScenarioTables& t0 = tabs[i * T];
+    if (t0.set & BLANCE_OPT_HIERARCHY) return t0.has_hier_rules ? t0.rule_off.data() : nullptr;
+    return ip->in.has_hier_rules ? ip->rule_off.data() : nullptr;
+  };
+  if (audit) {
+    build_forest(ip->node_names, options.NodeHierarchy, audit->FailoverSpread, &forest);
+    for (size_t x = 0; x < n * T; ++x) {
+      const ScenarioTables& t0 = tabs[x - x % T];
+      const int32_t R = (t0.set & BLANCE_OPT_HIERARCHY) ? (t0.has_hier_rules ? t0.n_rules : 0) : (ip->in.has_hier_rules ? ip->in.n_rules : 0);
+      abuf.push_back(std::make_unique<AuditBuffers>(*ip, forest.names.size(), size_t(R), audit->FailoverSpread));
+      aout.push_back(abuf.back()->out);
+    }
+  }
+  const size_t cap = exposure ? size_t(exposure->SeriesCap) : 0;
+  std::vector<std::unique_ptr<ExposureBuffers>> ebuf, nebuf;
+  std::vector<blance_exposure_out> eout, neout;
+  std::vector<std::unique_ptr<SpanBuffers>> sbuf;
+  std::vector<blance_chain_span_out> sout;
+  if (nc) {
+    build_forest(ip->node_names, options.NodeHierarchy, false, &eforest);
+    for (size_t x = 0; exposure && x < n * T * nc; ++x) {
+      ebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), P));
+      eout.push_back(ebuf.back()->out);
+    }
+    for (size_t x = 0; x < n * nc; ++x) {
+      if (exposure) {
+        nebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), P));
+        neout.push_back(nebuf.back()->out);
+      }
+      sbuf.push_back(std::make_unique<SpanBuffers>(size_t(NU), P, eforest.names.size(), exposure != nullptr));
+      sout.push_back(sbuf.back()->out);
+    }
+  }
   blance_ctx* ctx = DefaultContext();
-  const int st = blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
-                                    maxConcurrent, out.data(), net.data());
+  const int st = nc ? blance_plan_chains_exposure(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+                                                  maxConcurrent, int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), net.data(),
+                                                  sched.out.data(), audit ? &forest.opts : nullptr, audit ? aout.data() : nullptr,
+                                                  &eforest.opts, int32_t(cap), exposure ? eout.data() : nullptr, net_sched.out.data(),
+                                                  exposure ? neout.data() : nullptr, sout.data())
+                    : blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+                                         maxConcurrent, out.data(), net.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_chains failed: ") + blance_last_error(ctx));
   std::vector<ChainResult> res(n);
   for (size_t i = 0; i < n; ++i) {
     const ScenarioTables& t0 = tabs[i * T];
     const int32_t* k = (t0.set & BLANCE_OPT_CONSTRAINTS) ? t0.constraints.data() : ip->state_constraints.data();
-    for (size_t t = 0; t < T; ++t)
-      res[i].Stages.push_back(scenario_result(*ip, out[i * T + t], ops[i * T + t], load[i * T + t], maps[i * T + t].get(), k));
+    for (size_t t = 0; t < T; ++t) {
+      const size_t x = i * T + t;
+      ScenarioResult r = scenario_result(*ip, out[x], ops[x], load[x], maps[x].get(), k);
+      for (size_t c = 0; c < nc; ++c) r.Schedules.push_back(name_schedule(*ip, sched.out[x * nc + c], scheduleConcurrency[c]));
+      if (audit) {
+        abuf[x]->out = aout[x];
+        r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[x], audit->FailoverSpread);
+      }
+      for (size_t c = 0; exposure && c < nc; ++c) {
+        ebuf[x * nc + c]->out = eout[x * nc + c];
+        r.Exposures.push_back(name_exposure(*ebuf[x * nc + c], cap, eforest.names, ip->part_names));
+      }
+      res[i].Stages.push_back(std::move(r));
+    }
     res[i].NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());
     res[i].NetOpsTotal = net[i].ops_total;
     res[i].NetPartsMoved = net[i].parts_moved;
+    for (size_t c = 0; c < nc; ++c) {
+      res[i].NetSchedules.push_back(name_schedule(*ip, net_sched.out[i * nc + c], scheduleConcurrency[c]));
+      if (exposure) {
+        nebuf[i * nc + c]->out = neout[i * nc + c];
+        res[i].NetExposures.push_back(name_exposure(*nebuf[i * nc + c], cap, eforest.names, ip->part_names));
+      }
+      sbuf[i * nc + c]->out = sout[i * nc + c];
+      res[i].Span.push_back(name_span(*ip, *sbuf[i * nc + c], scheduleConcurrency[c], eforest.names));
+    }
   }
   return res;
 }

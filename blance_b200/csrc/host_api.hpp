@@ -221,12 +221,33 @@ struct Chain {
   std::vector<ChainStage> Stages;
 };
 
+// One chain's stages folded at one MaxConcurrentPartitionMovesPerNode (blance_chain_span_out), by node, partition and
+// metric name, nonzero entries only.  Rounds are global: stage t's rounds follow those of the stages before it.  The
+// exposure fields are filled with PlanNextMapChains' `exposure` only.
+struct ChainSpan {
+  int MaxConcurrentPartitionMovesPerNode = 0;
+  int64_t Rounds = 0, MovesDone = 0, StuckParts = 0;
+  int MaxBatch = 0;
+  std::unordered_map<std::string, int> NodeRounds;
+  std::unordered_map<std::string, int64_t> NodeLastRound, PartDoneRound;   // PartDoneRound: -1 = stuck in some stage
+  std::unordered_map<std::string, int64_t> Peak, Area;
+  std::unordered_map<std::string, int32_t> PeakStage, PeakRound;
+  std::unordered_map<std::string, int32_t> PartMinCopies, PartNoTop, PartFlags;
+  std::unordered_map<std::string, int64_t> DomPeak;
+  std::unordered_map<std::string, int32_t> DomPeakStage, DomPeakRound;
+};
+
 struct ChainResult {
   std::vector<ScenarioResult> Stages;  // one per stage, as PlanNextMapScenarios' results; "prev row" = that stage's prevMap
   // CalcPartitionMoves from the base prevMap row (empty when absent) to the last stage's next row, every assigned
   // partition: per node and op name (nonzero only), the total and the partitions with at least one op
   std::unordered_map<std::string, std::unordered_map<std::string, int64_t>> NetNodeOps;
   int64_t NetOpsTotal = 0, NetPartsMoved = 0;
+  // with scheduleConcurrency, one per value: the schedule (and with `exposure` the exposure) of the direct rebalance
+  // from prevMap to the last stage's final map, and the chain's span
+  std::vector<ScenarioSchedule> NetSchedules;
+  std::vector<ExposureResult> NetExposures;
+  std::vector<ChainSpan> Span;
 };
 
 // Chain i is the Go loop of include/blance_b200.h over its stages: stage t is PlanNextMapEx(prev, assign, nodesAll_t,
@@ -237,10 +258,17 @@ struct ChainResult {
 // panic on (a removal in the first stage with assigned partitions absent from prevMap, plan.go:544), a NodesAll name
 // outside the universe or chains of different lengths throw BlanceError naming the chain and stage before any device
 // work.  Stage maps (NextMap / NextWarnings) are filled for the chains listed in wantMaps.
+// scheduleConcurrency, audit and exposure (blance_plan_chains_exposure) fill every stage's Schedules / Audit /
+// Exposures exactly as PlanNextMapScenarios does for one scenario, with that stage's prevMap as begMap and the chain's
+// option fields; the result's NetSchedules / NetExposures and Span as described there.  The movers are the universe.
+// A stage's ops only touch its own nodesAll when every node that leaves nodesAll was removed in an earlier stage, which
+// the default NodesAll rule guarantees; then the stage's schedule equals OrchestrateSchedule(nodesAll_t, ...).
 std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                            const Strs& nodesAll, const PartitionModel& model,
                                            const PlanNextMapOptions& options, const std::vector<Chain>& chains,
-                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent);
+                                           bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
+                                           const std::vector<int>& scheduleConcurrency = {},
+                                           const ScenarioAudit* audit = nullptr, const ScenarioExposure* exposure = nullptr);
 
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 

@@ -86,6 +86,31 @@ static py::dict exposure_dict(const ExposureResult& r) {
   return d;
 }
 
+static py::list schedules_list(const std::vector<ScenarioSchedule>& v) {
+  py::list sl;
+  for (const auto& s : v) {
+    py::dict sd;
+    sd["MaxConcurrentPartitionMovesPerNode"] = s.MaxConcurrentPartitionMovesPerNode;
+    sd["Rounds"] = s.Rounds; sd["MovesDone"] = s.MovesDone; sd["StuckParts"] = s.StuckParts;
+    sd["MaxBatch"] = s.MaxBatch; sd["NodeRounds"] = s.NodeRounds; sd["NodeLastRound"] = s.NodeLastRound;
+    sl.append(sd);
+  }
+  return sl;
+}
+
+static py::dict span_dict(const ChainSpan& s, bool expo) {
+  py::dict d;
+  d["MaxConcurrentPartitionMovesPerNode"] = s.MaxConcurrentPartitionMovesPerNode;
+  d["rounds"] = s.Rounds; d["moves_done"] = s.MovesDone; d["stuck_parts"] = s.StuckParts; d["max_batch"] = s.MaxBatch;
+  d["node_rounds"] = s.NodeRounds; d["node_last_round"] = s.NodeLastRound; d["part_done_round"] = s.PartDoneRound;
+  if (expo) {
+    d["peak"] = s.Peak; d["peak_stage"] = s.PeakStage; d["peak_round"] = s.PeakRound; d["area"] = s.Area;
+    d["part_min_copies"] = s.PartMinCopies; d["part_no_top"] = s.PartNoTop; d["part_flags"] = s.PartFlags;
+    d["dom_peak"] = s.DomPeak; d["dom_peak_stage"] = s.DomPeakStage; d["dom_peak_round"] = s.DomPeakRound;
+  }
+  return d;
+}
+
 static py::dict audit_dict(const MapAudit& a) {
   py::dict d;
   d["short_slots"] = a.ShortSlots; d["over_slots"] = a.OverSlots;
@@ -436,17 +461,7 @@ PYBIND11_MODULE(_host, m) {
           d["sticky_steps"] = r.sticky_steps; d["parts_moved"] = r.parts_moved; d["ops_total"] = r.ops_total;
           d["warn_parts"] = r.warn_parts; d["node_ops"] = r.NodeOps; d["state_node_load"] = r.StateNodeLoad;
           if (r.HasMap) { d["next_map"] = from_map(r.NextMap); d["warnings"] = r.NextWarnings; }
-          if (!schedule_concurrency.empty()) {
-            py::list sl;
-            for (const auto& s : r.Schedules) {
-              py::dict sd;
-              sd["MaxConcurrentPartitionMovesPerNode"] = s.MaxConcurrentPartitionMovesPerNode;
-              sd["Rounds"] = s.Rounds; sd["MovesDone"] = s.MovesDone; sd["StuckParts"] = s.StuckParts;
-              sd["MaxBatch"] = s.MaxBatch; sd["NodeRounds"] = s.NodeRounds; sd["NodeLastRound"] = s.NodeLastRound;
-              sl.append(sd);
-            }
-            d["schedules"] = sl;
-          }
+          if (!schedule_concurrency.empty()) d["schedules"] = schedules_list(r.Schedules);
           if (r.Audit) d["audit"] = audit_dict(*r.Audit);
           if (exposure_series_cap) {
             py::list el;
@@ -476,10 +491,15 @@ PYBIND11_MODULE(_host, m) {
                      const std::vector<int>& want_maps, int max_concurrent, const std::optional<IntMap>& msc,
                      const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
                      const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
-                     int engine) {
+                     int engine, const std::vector<int>& schedule_concurrency, const std::optional<bool>& audit,
+                     const std::optional<int>& exposure_series_cap) {
         PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
         const PartitionMap prev_map = to_map(prev);
         const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
+        ScenarioAudit aud;
+        aud.FailoverSpread = audit.value_or(false);
+        ScenarioExposure expo;
+        expo.SeriesCap = exposure_series_cap.value_or(0);
         std::vector<Chain> cs;
         for (const auto& c : chains) {
           Chain ch;
@@ -498,7 +518,8 @@ PYBIND11_MODULE(_host, m) {
         {
           py::gil_scoped_release rel;
           res = PlanNextMapChains(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, cs, favor_min_nodes,
-                                  want_maps, max_concurrent);
+                                  want_maps, max_concurrent, schedule_concurrency, audit ? &aud : nullptr,
+                                  exposure_series_cap ? &expo : nullptr);
         }
         py::list out;
         for (const auto& c : res) {
@@ -509,11 +530,29 @@ PYBIND11_MODULE(_host, m) {
             d["sticky_steps"] = r.sticky_steps; d["parts_moved"] = r.parts_moved; d["ops_total"] = r.ops_total;
             d["warn_parts"] = r.warn_parts; d["node_ops"] = r.NodeOps; d["state_node_load"] = r.StateNodeLoad;
             if (r.HasMap) { d["next_map"] = from_map(r.NextMap); d["warnings"] = r.NextWarnings; }
+            if (!schedule_concurrency.empty()) d["schedules"] = schedules_list(r.Schedules);
+            if (r.Audit) d["audit"] = audit_dict(*r.Audit);
+            if (exposure_series_cap) {
+              py::list el;
+              for (const auto& e : r.Exposures) el.append(exposure_dict(e));
+              d["exposures"] = el;
+            }
             stages.append(d);
           }
           py::dict net;
           net["node_ops"] = c.NetNodeOps; net["ops_total"] = c.NetOpsTotal; net["parts_moved"] = c.NetPartsMoved;
           py::dict d;
+          if (!schedule_concurrency.empty()) {
+            net["schedules"] = schedules_list(c.NetSchedules);
+            py::list sp;
+            for (const auto& x : c.Span) sp.append(span_dict(x, exposure_series_cap.has_value()));
+            d["span"] = sp;
+          }
+          if (exposure_series_cap) {
+            py::list el;
+            for (const auto& e : c.NetExposures) el.append(exposure_dict(e));
+            net["exposures"] = el;
+          }
           d["stages"] = stages;
           d["net"] = net;
           out.append(d);
@@ -524,7 +563,9 @@ PYBIND11_MODULE(_host, m) {
       py::arg("favor_min_nodes") = false, py::arg("want_maps") = std::vector<int>{}, py::arg("max_concurrent") = 0,
       py::arg("model_state_constraints") = py::none(), py::arg("partition_weights") = py::none(),
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
-      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0);
+      py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
+      py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none(),
+      py::arg("exposure_series_cap") = py::none());
 
   // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
   m.def(

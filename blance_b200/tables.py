@@ -144,6 +144,8 @@ class ChainNet:
 
     ops_total = property(lambda self: self.out.ops_total)
     parts_moved = property(lambda self: self.out.parts_moved)
+    schedules = None          # blance_plan_chains_exposure: the direct rebalance's ScenarioSchedule per count
+    exposures = None          # ... and its exposure dict per count
 
 
 class ScenarioSchedule:
@@ -236,6 +238,36 @@ class _ScenarioExposure:
         for k in ("part_min_copies", "part_no_top", "part_flags"):
             if k in a:
                 r[k] = a[k][:self.n_parts]
+        return r
+
+
+class _ChainSpan:
+    """Output buffers of one blance_chain_span_out: the schedule's arrays always, the per-partition exposure arrays
+    with parts and the per-vertex ones with dom; result() returns a dict, the exposure scalars only with expo."""
+
+    def __init__(self, t, V, expo, dom, parts):
+        self.expo = expo
+        self.a = dict(node_rounds=np.zeros(max(1, t.n_node_ids), np.int32), node_last_round=np.zeros(max(1, t.n_node_ids), np.int64),
+                      part_done_round=np.zeros(max(1, t.n_parts), np.int64))
+        if expo and parts:
+            self.a.update(part_min_copies=np.zeros(max(1, t.n_parts), np.int32), part_no_top=np.zeros(max(1, t.n_parts), np.int32),
+                          part_flags=np.zeros(max(1, t.n_parts), np.uint8))
+        if expo and dom:
+            self.a.update(dom_peak=np.zeros(max(1, V), np.int64), dom_peak_stage=np.zeros(max(1, V), np.int32),
+                          dom_peak_round=np.zeros(max(1, V), np.int32))
+        self.sizes = dict(node=t.n_node_ids, part=t.n_parts, dom=V)
+        self.out = api.ChainSpanOut()
+        for k, a in self.a.items():
+            setattr(self.out, k, a.ctypes.data)
+
+    def result(self):
+        o = self.out
+        r = dict(rounds=o.rounds, moves_done=o.moves_done, stuck_parts=o.stuck_parts, max_batch=o.max_batch)
+        if self.expo:
+            r.update(peak=np.array(o.peak[:], np.int64), peak_stage=np.array(o.peak_stage[:], np.int32),
+                     peak_round=np.array(o.peak_round[:], np.int32), area=np.array(o.area[:], np.int64))
+        for k, a in self.a.items():
+            r[k] = a[:self.sizes[k.split("_")[0]]]
         return r
 
 
@@ -485,12 +517,30 @@ class Context:
             r.out = o
         return results
 
-    def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True):
+    def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True,
+                    schedule=None, node_has_mover=None, audit=None, exposure=None, span=False, stage_arrays=True):
         """blance_plan_chains: chains of cluster changes, each stage planned on the map the stage before produced.
         chains is a list of chains of equal length; a stage is a dict of SCENARIO_FIELDS and node_in_all ([n_nodes],
         missing = every node; missing scenario keys keep the base's value).  want_rows lists the (chain, stage) pairs
         whose next rows, shapes and warnings are copied out.  opts: None, or one dict of OPT_GROUPS keys per chain.
-        Returns (results, nets): results[i][t] a ScenarioResult per stage, nets[i] a ChainNet (None without net)."""
+        Returns (results, nets): results[i][t] a ScenarioResult per stage, nets[i] a ChainNet (None without net).
+
+        schedule (a list of MaxConcurrentPartitionMovesPerNode values) calls blance_plan_chains_exposure: every stage's
+        result gets `schedules`, and with audit / exposure (the keys of plan_scenarios) `audit` / `exposures`, as
+        plan_scenarios sets them; with net each ChainNet gets `schedules` (and `exposures`) of the direct rebalance.
+        node_has_mover as plan_scenarios, for every stage.  span=True (needs schedule) returns (results, nets, spans):
+        spans[i][k] is chain i's stages folded at count k, a dict of blance_chain_span_out's fields (the exposure ones
+        with exposure, the per-partition ones with its parts, the per-vertex ones with its dom).  stage_arrays=False
+        asks for no per-stage array (schedules and exposures keep their scalars; no series): the span alone."""
+        if schedule is None:
+            if audit is not None or exposure is not None or span or node_has_mover is not None:
+                raise ValueError("audit, exposure, span and node_has_mover need a schedule: pass schedule=[counts]")
+        elif not len(schedule):
+            raise ValueError("schedule needs at least one count")
+        if exposure is not None:
+            unknown = set(exposure) - set(EXPOSURE_KEYS)
+            if unknown:
+                raise KeyError("unknown exposure option(s) %s" % sorted(unknown))
         n = len(chains)
         T = len(chains[0]) if n else 0
         if any(len(c) != T for c in chains):
@@ -518,14 +568,91 @@ class Context:
         nets = [ChainNet(base_tables) for _ in range(n)] if net else None
         net_arr = (api.ChainOut * max(1, n))(*[x.out for x in nets]) if net else None
         ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-        self._check(self.lib.blance_plan_chains(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
-                                                int(max_concurrent), outs, net_arr), "blance_plan_chains")
+        if schedule is None:
+            self._check(self.lib.blance_plan_chains(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
+                                                    int(max_concurrent), outs, net_arr), "blance_plan_chains")
+        else:
+            spans = self._chains_exposure(base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results,
+                                          opts, schedule, node_has_mover, audit, exposure, span, stage_arrays, keep)
         for i in range(n):
             for t in range(T):
                 results[i][t].out = outs[i * T + t]
             if net:
                 nets[i].out = net_arr[i]
-        return results, nets
+        return (results, nets, spans) if span else (results, nets)
+
+    def _chains_exposure(self, base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results, opts,
+                         schedule, node_has_mover, audit, exposure, span, stage_arrays, keep):
+        """The blance_plan_chains_exposure call of plan_chains: fills the results' and nets' schedules, audits and
+        exposures; returns the spans (or None)."""
+        counts = np.ascontiguousarray(schedule, np.int32)
+        nc = counts.size
+        mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
+        if mover is not None and mover.size != base_tables.n_node_ids:
+            raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
+        stages = [r for rs in results for r in rs]
+        for r in stages:
+            r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+            for s in r.schedules if not stage_arrays else ():
+                s.out.node_rounds = s.out.node_last_round = s.out.part_done_round = None
+        sch = (api.ScenarioScheduleOut * (n * T * nc))(*[s.out for r in stages for s in r.schedules])
+        net_sch = None
+        if nets is not None:
+            for x in nets:
+                x.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+            net_sch = (api.ScenarioScheduleOut * (n * nc))(*[s.out for x in nets for s in x.schedules])
+        a_opts, auds = None, None
+        if audit is not None:
+            a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
+            for i in range(n):
+                t = scenario_tables(base_tables, {}, None if opts is None else opts[i])
+                for r in results[i]:
+                    r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
+            auds = (api.AuditOut * (n * T))(*[r.audit.out for r in stages])
+        e_opts, exps, net_exps, expo, net_expo, cap = None, None, None, None, None, 0
+        dom = parts = False
+        V = base_tables.n_node_ids
+        if exposure is not None:
+            e_opts, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
+            V += int(e_opts.n_domains)
+            cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
+            expo = [[_ScenarioExposure(base_tables, V, max(cap, 0) if stage_arrays else 0, dom and stage_arrays, parts and stage_arrays)
+                     for _ in counts] for _ in stages]
+            exps = (api.ExposureOut * (n * T * nc))(*[e.out for es in expo for e in es])
+            if nets is not None:
+                # one series_cap serves the stages and the net rebalance: 0 without per-stage arrays
+                net_expo = [[_ScenarioExposure(base_tables, V, max(cap, 0) if stage_arrays else 0, dom, parts) for _ in counts] for _ in nets]
+                net_exps = (api.ExposureOut * (n * nc))(*[e.out for es in net_expo for e in es])
+        spans = [[_ChainSpan(base_tables, V, exposure is not None, dom, parts) for _ in counts] for _ in range(n)] if span else None
+        span_arr = (api.ChainSpanOut * (n * nc))(*[s.out for ss in spans for s in ss]) if span else None
+        self._check(self.lib.blance_plan_chains_exposure(
+            self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)), int(max_concurrent), nc, counts.ctypes.data,
+            None if mover is None else mover.ctypes.data, outs, net_arr, sch, None if audit is None else ctypes.byref(a_opts), auds,
+            ctypes.byref(e_opts) if exposure is not None and exposure.get("domain_parent") is not None else None,
+            cap if stage_arrays else 0, exps,
+            net_sch, net_exps, span_arr), "blance_plan_chains_exposure")
+        for x, r in enumerate(stages):
+            for k, s in enumerate(r.schedules):
+                s.out = sch[x * nc + k]
+            if auds is not None:
+                r.audit.out = auds[x]
+            if exps is not None:
+                for k, e in enumerate(expo[x]):
+                    e.out = exps[x * nc + k]
+                r.exposures = [e.result() for e in expo[x]]
+        for i, x in enumerate(nets or ()):
+            for k, s in enumerate(x.schedules):
+                s.out = net_sch[i * nc + k]
+            if net_exps is not None:
+                for k, e in enumerate(net_expo[i]):
+                    e.out = net_exps[i * nc + k]
+                x.exposures = [e.result() for e in net_expo[i]]
+        if not span:
+            return None
+        for i in range(n):
+            for k, s in enumerate(spans[i]):
+                s.out = span_arr[i * nc + k]
+        return [[s.result() for s in ss] for ss in spans]
 
     def prepare_batch(self, tables_list, results=None):
         """Builds the blance_plan_in / blance_plan_out arrays of a batch once; run_batch() is then only the

@@ -331,7 +331,7 @@ int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_
  * partition is absent from prevMap) to the LAST stage's next row, for every assigned partition: node_ops, ops_total,
  * parts_moved as in blance_scenario_out.  sum_t out[i * n_stages + t].ops_total - net[i].ops_total is what the
  * sequence moves beyond one direct plan.  Nothing depends on n, max_concurrent, the engine or the number of devices.
- * No schedules or audits per stage: blance_map_audit audits a copied-out row table.
+ * Schedules, audits and exposures per stage: blance_plan_chains_exposure (below, after blance_plan_scenarios_exposure).
  *
  * Errors, all before any device work: n <= 0, n_stages < 1, a NULL base / stages / out; n_stages > 1 with
  * max_iters < 1 (a stage that plans nothing leaves no next map); a stage that blance_plan_scenarios_ex would reject,
@@ -734,6 +734,83 @@ int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan_in* base, 
                                    const blance_audit_opts* aopts, blance_audit_out* audit /* [n] or NULL */,
                                    const blance_audit_opts* eopts /* forest only, flags must be 0; NULL = nodes only */,
                                    int32_t series_cap, blance_exposure_out* expo /* [n][n_move_conc] */);
+
+/* ---- schedules, audits and exposures of every chain stage (blance_plan_chains_exposure) ---------------------
+ * blance_plan_chains, and for every stage of every chain what blance_plan_scenarios_exposure gives for one scenario:
+ * how many rounds each step of a rolling upgrade takes, whether a step leaves partitions without a primary or on one
+ * node, and whether the map after each step meets its constraints and hierarchy rules.  T = n_stages, nc = n_move_conc.
+ *
+ * Plans are unchanged: out and net equal blance_plan_chains for the same arguments, byte for byte.
+ *
+ * Per stage.  sched[(i * T + t) * nc + k], audit[i * T + t] and expo[(i * T + t) * nc + k] are what
+ * blance_plan_scenarios_exposure defines for one scenario, where "prevMap" is STAGE t's prevMap: begMap = stage t's
+ * prevMap plus an empty entry for every assigned partition it lacks, the end map is stage t's final map, the
+ * constraints and hierarchy are chain i's own (opts[i]), the top state the base's and the forest that of eopts.  With
+ * T = 1 and every node_in_all set the result equals blance_plan_scenarios_exposure field for field.
+ *
+ * Net.  net_sched[i * nc + k] and net_expo[i * nc + k] are the schedule and exposure of the direct rebalance from the
+ * BASE's prevMap to the last stage's final map - the moves net[i] counts: the chain against one direct jump.
+ *
+ * Movers.  One node_has_mover [n_node_ids] serves every stage and the net rebalance; NULL means the ids < n_nodes,
+ * the universe, as OrchestrateSchedule has them.  A stage's ops only touch nodes in that stage's nodesAll when every
+ * node that leaves nodesAll was removed in an earlier stage (removal strips a node from every assigned row).  The
+ * string twin's default NodesAll rule guarantees that, and the result then equals OrchestrateSchedule(nodesAll_t, ...).
+ * Per-chain, per-stage mover sets are not supported.
+ *
+ * Span.  span[i * nc + k] folds chain i's stages at move_conc[k] into one record, on the device.  R_t is stage t's
+ * rounds and G_t = sum_{u < t} R_u the global round at which stage t starts.  Every span array may be NULL; nothing in
+ * the span depends on whether the per-stage arrays were asked for (they may all be NULL while the span is complete).
+ * Schedule fields (from sched):
+ *   rounds = sum_t R_t;  moves_done, stuck_parts: sums;  max_batch: max;  node_rounds[q] = sum_t;
+ *   node_last_round[q]   G_t + stage t's node_last_round[q] for the last stage t with a batch on q; 0 if none;
+ *   part_done_round[p]   -1 if p is stuck in any stage; else G_t + stage t's part_done_round[p] for the last stage t
+ *                        where p has ops; 0 if it never has ops.
+ * Exposure fields (need expo; zero without it):
+ *   peak[m] = max_t;  peak_stage[m], peak_round[m]: the first stage that reaches the peak and that stage's peak round;
+ *   area[m] = sum_t - a map that ends stage t and begins stage t + 1 is counted in both;
+ *   part_min_copies[p]   min over the stages whose begMap holds p; -1 if none;
+ *   part_no_top[p] = sum_t;  part_flags[p]: OR over the stages;
+ *   dom_peak[v] = max_t;  dom_peak_stage[v], dom_peak_round[v]: the first stage that reaches it and that stage's round.
+ *
+ * No value depends on n, max_concurrent, the wave size, the engine, the number of devices or the other move_conc.
+ *
+ * Errors, all before any device work, naming "chain i, stage t" or the index k: everything blance_plan_chains and
+ * blance_plan_scenarios_exposure reject (with audit and expo optional as there: audit NULL = no audit, expo NULL = no
+ * exposure); net_sched or net_expo without net, net_expo or a span exposure array without expo
+ * (BLANCE_ERR_INVALID_ARG); a dom_peak / dom_peak_round of expo, net_expo or span with 2 x 17 x 2 x n_slots x n_parts
+ * >= 2^31 (BLANCE_ERR_UNSUPPORTED; every stage shares the layout, so the bound is the same for each).  A NULL ctx
+ * checks everything and then returns BLANCE_ERR_INVALID_ARG.  The span accumulators are priced into the wave size
+ * next to the audit, exposure and net buffers (DESIGN.md section 15). */
+typedef struct blance_chain_span_out {
+  int64_t  rounds, moves_done, stuck_parts;
+  int32_t  max_batch;
+  int32_t* node_rounds;              /* [n_node_ids] */
+  int64_t* node_last_round;          /* [n_node_ids] */
+  int64_t* part_done_round;          /* [n_parts] */
+  int64_t  peak[BLANCE_EXPO_N];
+  int32_t  peak_stage[BLANCE_EXPO_N];
+  int32_t  peak_round[BLANCE_EXPO_N];
+  int64_t  area[BLANCE_EXPO_N];
+  int32_t* part_min_copies;          /* [n_parts] */
+  int32_t* part_no_top;              /* [n_parts] */
+  uint8_t* part_flags;               /* [n_parts] */
+  int64_t* dom_peak;                 /* [V] */
+  int32_t* dom_peak_stage;           /* [V] */
+  int32_t* dom_peak_round;           /* [V] */
+} blance_chain_span_out;
+
+int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                const blance_chain_stage* stages /* [n][n_stages] */, const blance_scenario_opts* opts /* [n] or NULL */,
+                                int32_t favor_min_nodes, int32_t max_concurrent,
+                                int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                blance_scenario_out* out /* [n][n_stages] */, blance_chain_out* net /* [n] or NULL */,
+                                blance_scenario_schedule_out* sched /* [n][n_stages][n_move_conc] */,
+                                const blance_audit_opts* aopts, blance_audit_out* audit /* [n][n_stages] or NULL */,
+                                const blance_audit_opts* eopts /* forest only, flags must be 0; NULL = nodes only */,
+                                int32_t series_cap, blance_exposure_out* expo /* [n][n_stages][n_move_conc] or NULL */,
+                                blance_scenario_schedule_out* net_sched /* [n][n_move_conc] or NULL, needs net */,
+                                blance_exposure_out* net_expo /* [n][n_move_conc] or NULL, needs net and expo */,
+                                blance_chain_span_out* span /* [n][n_move_conc] or NULL */);
 
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
