@@ -1706,23 +1706,36 @@ static void span_slices(Arena& a, SpanBufs& b, const ChainReq& cr, long long nw,
   if (cr.span_dom) { a.add(b.F.a_dom_peak, (size_t)(ni * V)); a.add(b.F.a_dom_stage, (size_t)(ni * V)); a.add(b.F.a_dom_round, (size_t)(ni * V)); }
 }
 
+// What a scenario wave plans and analyses: the base and its scenarios sc / opts (with cr: its chains, sc NULL), the
+// plan options, the caller's outputs, and the schedules, audits and exposures asked for (each NULL: none).
+struct WaveReq {
+  const blance_plan_in* base = nullptr;
+  const blance_scenario* sc = nullptr;
+  const blance_scenario_opts* opts = nullptr;
+  int favor_min = 0, max_concurrent = 0;
+  blance_scenario_out* out = nullptr;
+  const SchedReq* sr = nullptr;
+  const AuditReq* ar = nullptr;
+  const ChainReq* cr = nullptr;
+  const ExpoReq* er = nullptr;
+};
+
 // The node fields of scenario (or chain) i at stage t.
-static const blance_scenario& nodes_of(const blance_scenario* sc, const ChainReq* cr, int i, int t) {
-  return cr ? cr->stages[(size_t)i * cr->T + t].nodes : sc[i];
+static const blance_scenario& nodes_of(const WaveReq& q, int i, int t) {
+  return q.cr ? q.cr->stages[(size_t)i * q.cr->T + t].nodes : q.sc[i];
 }
 
 // The substituted instance of scenario / chain i at stage t.  A chain stage's node_removed is written in the device
 // code into `code` (NR_OUTSIDE for the ids below n_nodes that its node_in_all leaves out), and from stage 2 on the
 // non-model counts of iteration 1 are those of the later iterations: the assigned partitions' prevMap entries are
 // the previous stage's next rows, which hold model states only.
-static blance_plan_in stage_in(const blance_plan_in& base, const blance_scenario* sc, const blance_scenario_opts* opts,
-                               const ChainReq* cr, int i, int t, std::vector<uint8_t>& code) {
-  blance_plan_in in = scenario_in(base, nodes_of(sc, cr, i, t), opts_of(opts, i));
-  if (!cr) return in;
-  const blance_chain_stage& st = cr->stages[(size_t)i * cr->T + t];
-  code.assign((size_t)std::max(1, base.n_node_ids), 0);
-  for (int q = 0; q < base.n_node_ids; ++q)
-    code[(size_t)q] = (uint8_t)((st.nodes.node_removed[q] ? NR_REMOVE : 0) | (q < base.n_nodes && !st.node_in_all[q] ? NR_OUTSIDE : 0));
+static blance_plan_in stage_in(const WaveReq& q, int i, int t, std::vector<uint8_t>& code) {
+  blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q.opts, i));
+  if (!q.cr) return in;
+  const blance_chain_stage& st = q.cr->stages[(size_t)i * q.cr->T + t];
+  code.assign((size_t)std::max(1, in.n_node_ids), 0);
+  for (int k = 0; k < in.n_node_ids; ++k)
+    code[(size_t)k] = (uint8_t)((st.nodes.node_removed[k] ? NR_REMOVE : 0) | (k < in.n_nodes && !st.node_in_all[k] ? NR_OUTSIDE : 0));
   in.node_removed = code.data();
   if (t > 0) in.extra_tot_first = in.extra_tot_rest;
   return in;
@@ -1749,57 +1762,101 @@ static void upload_nodes(blance_ctx* ctx, blance_plan* pl, const std::vector<bla
   CUDA(cudaStreamSynchronize(st));          // the host vectors die here
 }
 
-// Scenario summaries (node_ops | state_node_load | 3 scalars per instance, `stride` int64 words) of the wave's plans
-// from the beg rows / flags `prev_rows` / `pflags` to the working rows.
-static void wave_summary(blance_ctx* ctx, blance_plan* pl, int nw, const int32_t* prev_rows, const uint8_t* pflags, int favor_min,
-                         long long stride, long long* d_sum) {
-  const DInst& D0 = pl->h_insts[0];
-  const int PU = D0.PU, NU = D0.NU, S = D0.S;
-  CUDA(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(stride * nw), ctx->stream));
-  if (PU <= 0) return;
-  const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)S * NU;
-  const int bx = std::max(1, std::min((PU + 255) / 256, std::max(1, ctx->sm_count * 8 / nw)));
-  const dim3 grid((unsigned)bx, (unsigned)nw);
-  if (smem <= 48 * 1024) launch(ctx, k_scenario_summary<true>, grid, 256, smem, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
-  else launch(ctx, k_scenario_summary<false>, grid, 256, 0, pl->pool, prev_rows, pflags, favor_min, stride, d_sum);
+// What every wave of one device's items idx of q shares, computed once: the base upload pb, the sizes of the
+// analyses, and the wave size W (halved when a wave does not fit) with the device bytes `per` one member is priced at.
+struct Sweep {
+  blance_ctx* ctx;
+  const WaveReq& q;
+  const std::vector<int>& idx;
+  const int T, nc, MO;                 // stages per item, counts per schedule, ops per partition
+  const long long V, stride;           // exposure vertices, int64 words of one summary
+  int max_rules = 0, W = 0;
+  int n_prev_later = 0;                // len(prevMap) from stage 2 on: the base's prevMap plus every assigned partition
+  bool audit_flags = false;            // any caller wants the per-partition flags
+  PlanPtr pb;
+  size_t per = 0;
+  Sweep(blance_ctx* c, const std::vector<int>& items, const WaveReq& r)
+      : ctx(c), q(r), idx(items), T(r.cr ? r.cr->T : 1), nc(r.sr ? r.sr->nc : 0), MO(scenario_ops(*r.base)),
+        V((long long)r.base->n_node_ids + (r.er ? r.er->n_domains : 0)), stride(summary_stride(*r.base)) {}
+};
+
+// The buffers of a wave's analyses: audits, exposures, span accumulators, a chain's net prev rows, flags and summaries.
+struct AnalysisBufs {
+  AuditBufs audit;
+  ExpoBufs expo;
+  SpanBufs span;
+  int32_t* net_prev = nullptr;
+  uint8_t* net_flags = nullptr;
+  long long* net_sum = nullptr;
+};
+
+// One wave of a sweep: members idx[w0, w0 + nw) (instances ins at the current stage, node codes `code`), the plan (lone:
+// the base upload), the wave's one arena and its slices, each chain instance's G_t, the stage's BLANCE_SCENARIO_TIMES.
+struct Wave {
+  Wave(int first, int n) : w0(first), nw(n), ins((size_t)n), code((size_t)n) {}
+  const int w0, nw;
+  bool lone = false;
+  blance_plan plan;
+  blance_plan* pl = nullptr;
+  std::vector<blance_plan_in> ins;
+  std::vector<std::vector<uint8_t>> code;
+  std::vector<int> seg_off;
+  std::vector<int32_t> ow;             // the weight overrides: index[k] | weight[k] | presence[k]
+  Arena arena;
+  long long* d_sum = nullptr;
+  WSched sched{};
+  void* wtmp = nullptr;
+  size_t wtmp_bytes = 0;
+  int32_t* d_ow = nullptr;
+  AnalysisBufs an;
+  std::vector<long long> G;
+  float sum_ms = 0.f, sched_ms = 0.f, expo_ms = 0.f, fold_ms = 0.f;
+  size_t expo_bytes = 0;
+};
+
+// Where the caller keeps the output of instance i of wave w (member i / n, its count i % n) at stage t, in an array of
+// `per` stages per item and n counts per stage.
+static size_t out_at(const Sweep& s, const Wave& w, long long i, int n, int per, int t) {
+  return ((size_t)s.idx[(size_t)(w.w0 + i / n)] * per + t) * n + (size_t)(i % n);
 }
 
-// The exposures of a wave's nw scenarios x nc counts after their schedules (scal: the instances' scalars), from the
-// beg rows / flags `beg` / `pflags` over the op table and rounds the schedule left in W, on the buffers of b.  Copies
-// the result of instance i out into *outs[i]; *ms and *bytes: the device time and the bytes allocated after the
-// schedule.  The per-partition outputs and fault-domain keys stay in b until the wave's next exposure.
-static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan* pl, int nw, int nc, const int32_t* beg, const uint8_t* pflags,
-                          const std::vector<blance_exposure_out*>& outs, const blance_plan_in& base, const WSched& W, ExpoBufs& b,
-                          const std::vector<unsigned long long>& scal, float* ms, size_t* bytes) {
-  cudaStream_t st = ctx->stream;
-  const int PU = base.n_parts, S = base.n_states;
-  const long long ni = (long long)nw * nc, V = (long long)base.n_node_ids + er.n_domains;
-  ExpoArgs& E = b.E;
+// The exposures of wave w's instances after their schedules (scal: the instances' scalars), from the beg rows / flags
+// `beg` / `pflags` over the op table and rounds the schedule left in w.sched; instance i's result goes to
+// outs[out_at(i, nc, per, t)].  The per-partition outputs and fault-domain keys stay in w.an.expo until the next one.
+static void wave_exposure(const Sweep& s, Wave& w, const int32_t* beg, const uint8_t* pflags, blance_exposure_out* outs, int per, int t,
+                          const std::vector<unsigned long long>& scal) {
+  cudaStream_t st = s.ctx->stream;
+  const blance_plan_in& base = *s.q.base;
+  const ExpoReq& er = *s.q.er;
+  const int PU = base.n_parts;
+  const long long ni = (long long)w.nw * s.nc;
+  const WSched& W = w.sched;
+  ExpoArgs& E = w.an.expo.E;
   E.op_off = nullptr; E.op_n = W.op_n; E.op_node = W.op_node; E.op_state = W.op_state; E.op_kind = W.op_kind; E.op_round = W.op_round;
-  E.beg = beg; E.pflags = pflags; E.dom_parent = b.parent;
-  E.stride = pl->h_insts[0].SLP; E.P = PU; E.SL = base.n_slots; E.S = S; E.NU = base.n_node_ids; E.V = (int32_t)V;
+  E.beg = beg; E.pflags = pflags; E.dom_parent = w.an.expo.parent;
+  E.stride = w.pl->h_insts[0].SLP; E.P = PU; E.SL = base.n_slots; E.S = base.n_states; E.NU = base.n_node_ids; E.V = (int32_t)s.V;
   E.MO = W.MO; E.top = base.top_state;
-  for (int s = 0; s <= S; ++s) E.slot_off[s] = base.state_slot_off[s];
+  for (int k = 0; k <= base.n_states; ++k) E.slot_off[k] = base.state_slot_off[k];
   std::vector<ExpoInst> inst((size_t)ni, ExpoInst{});
   for (long long i = 0; i < ni; ++i) {
-    const long long j = i / nc;
-    const DInst& D = pl->h_insts[(size_t)j];
+    const long long j = i / s.nc;
+    const DInst& D = w.pl->h_insts[(size_t)j];
     ExpoInst& I = inst[(size_t)i];
     I.beg_off = D.rows_off; I.pf_off = D.part_off; I.gp_off = j * PU;
     I.R = (int32_t)scal[(size_t)(4 * i)];
-    for (int s = 0; s < S; ++s) I.constraints[s] = D.state_constraints[s];
+    for (int k = 0; k < base.n_states; ++k) I.constraints[k] = D.state_constraints[k];
   }
-  CUDA(cudaEventRecord(ctx->ev[6], st));
-  const ExpoResult r = expo_run(ctx, E, inst, er.dom ? b.dom_key : nullptr, b.ev_off);
-  CUDA(cudaEventRecord(ctx->ev[7], st));
-  std::vector<unsigned long long> h_key(er.dom ? (size_t)(ni * V) : 0);
-  if (!h_key.empty()) CUDA(cudaMemcpyAsync(h_key.data(), b.dom_key, sizeof(unsigned long long) * h_key.size(), cudaMemcpyDeviceToHost, st));
+  CUDA(cudaEventRecord(s.ctx->ev[6], st));
+  const ExpoResult r = expo_run(s.ctx, E, inst, er.dom ? w.an.expo.dom_key : nullptr, w.an.expo.ev_off);
+  CUDA(cudaEventRecord(s.ctx->ev[7], st));
+  std::vector<unsigned long long> h_key(er.dom ? (size_t)(ni * s.V) : 0);
+  if (!h_key.empty()) CUDA(cudaMemcpyAsync(h_key.data(), w.an.expo.dom_key, sizeof(unsigned long long) * h_key.size(), cudaMemcpyDeviceToHost, st));
   for (long long i = 0; i < ni; ++i) {
-    blance_exposure_out& o = *outs[(size_t)i];
-    const long long R1 = (long long)inst[(size_t)i].R + 1, w = std::min<long long>(R1, er.series_cap);
-    if (o.series && w > 0)        // [BLANCE_EXPO_N][series_cap] <- the first w of each metric's R + 1 values
+    blance_exposure_out& o = outs[out_at(s, w, i, s.nc, per, t)];
+    const long long R1 = (long long)inst[(size_t)i].R + 1, n = std::min<long long>(R1, er.series_cap);
+    if (o.series && n > 0)        // [BLANCE_EXPO_N][series_cap] <- the first n of each metric's R + 1 values
       CUDA(cudaMemcpy2DAsync(o.series, sizeof(int64_t) * (size_t)er.series_cap, E.diff + inst[(size_t)i].diff_off, sizeof(long long) * (size_t)R1,
-                             sizeof(long long) * (size_t)w, BLANCE_EXPO_N, cudaMemcpyDeviceToHost, st));
+                             sizeof(long long) * (size_t)n, BLANCE_EXPO_N, cudaMemcpyDeviceToHost, st));
     if (PU > 0) {
       if (o.part_min_copies && E.part_min) CUDA(cudaMemcpyAsync(o.part_min_copies, E.part_min + i * PU, sizeof(int32_t) * (size_t)PU, cudaMemcpyDeviceToHost, st));
       if (o.part_no_top && E.part_notop) CUDA(cudaMemcpyAsync(o.part_no_top, E.part_notop + i * PU, sizeof(int32_t) * (size_t)PU, cudaMemcpyDeviceToHost, st));
@@ -1807,382 +1864,385 @@ static void wave_exposure(blance_ctx* ctx, const ExpoReq& er, const blance_plan*
     }
   }
   CUDA(cudaStreamSynchronize(st));
-  *ms = 0.f;
-  cudaEventElapsedTime(ms, ctx->ev[6], ctx->ev[7]);
-  *bytes = r.bytes;
+  w.expo_ms = 0.f;
+  cudaEventElapsedTime(&w.expo_ms, s.ctx->ev[6], s.ctx->ev[7]);
+  w.expo_bytes = r.bytes;
   for (long long i = 0; i < ni; ++i) {
-    blance_exposure_out& o = *outs[(size_t)i];
-    expo_unpack(r, i, inst[(size_t)i].R, er.dom ? h_key.data() + i * V : nullptr, (int)V, o);
-    o.kernel_ms = *ms;
+    blance_exposure_out& o = outs[out_at(s, w, i, s.nc, per, t)];
+    expo_unpack(r, i, inst[(size_t)i].R, er.dom ? h_key.data() + i * s.V : nullptr, (int)s.V, o);
+    o.kernel_ms = w.expo_ms;
   }
 }
 
-// Plans the scenarios idx (of sc / opts) on one device, in waves.  With cr each is a chain of cr->T stages, planned
-// in lock step: a stage boundary is an iteration boundary plus the next stage's node tables (DESIGN.md section 12).
-static void scenarios_on_device(blance_ctx* ctx, const blance_plan_in* base, const std::vector<int>& idx, const blance_scenario* sc,
-                                const blance_scenario_opts* opts, int favor_min, int max_concurrent, blance_scenario_out* out,
-                                const SchedReq* sr, const AuditReq* ar, const ChainReq* cr = nullptr, const ExpoReq* er = nullptr) {
+// The slices of the analyses of nw members laid out as pl into b (the exposures' op states and rounds into sched).
+// One member's are what it adds to the price wave_size makes of its plan, summaries and schedule state.
+static void analysis_slices(const Sweep& s, Arena& a, AnalysisBufs& b, WSched& sched, int nw, const blance_plan* pl) {
+  const blance_plan_in& base = *s.q.base;
+  if (s.q.ar) audit_slices(a, b.audit, *s.q.ar, nw, base.n_states, s.max_rules, base.n_node_ids, base.n_nodes, base.n_parts, s.audit_flags);
+  if (s.q.er) expo_slices(a, b.expo, sched, *s.q.er, nw, s.nc, base.n_parts, s.MO, s.V);
+  if (s.q.cr && s.q.cr->net) {
+    a.add(b.net_prev, (size_t)pl->RT + 4);
+    a.add(b.net_flags, (size_t)pl->PT + 1);
+    a.add(b.net_sum, (size_t)(s.stride * nw));
+  }
+  if (s.q.cr && s.q.cr->span) span_slices(a, b.span, *s.q.cr, nw, s.nc, base.n_parts, base.n_node_ids, s.V);
+}
+
+// Lays out wave w at its first stage and allocates it in one arena, so that a plan is never lost for want of its
+// summaries or analyses: the plan (lone: the base upload), summaries, schedule state, weight overrides and analyses.
+// Returns false when the wave is to be halved: 2^29 or more partitions, or the free memory moved under an automatic size.
+static bool wave_alloc(const Sweep& s, Wave& w) {
+  const WaveReq& q = s.q;
+  const int nw = w.nw, PU = q.base->n_parts;
+  for (int j = 0; j < nw; ++j) w.ins[(size_t)j] = stage_in(q, s.idx[(size_t)(w.w0 + j)], 0, w.code[(size_t)j]);
+  // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
+  w.lone = s.idx.size() == 1;
+  blance_plan* pl = w.pl = w.lone ? s.pb.get() : &w.plan;
+  if (!w.lone) layout(pl, nw, w.ins.data(), w.seg_off, q.cr != nullptr);
+  if (!w.lone && pl->PT >= (1LL << 29)) {
+    if (nw > 1) return false;
+    throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
+  }
+  // the wave's partition-weight overrides over its replicated slices (lone: over the base upload), as wave-global
+  // partition indices
+  for (int pass = 0; pass < 3; ++pass)
+    for (int j = 0; j < nw; ++j) {
+      const blance_scenario_opts* o = opts_of(q.opts, s.idx[(size_t)(w.w0 + j)]);
+      for (int k = 0; k < n_overrides(o); ++k)
+        w.ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
+    }
+  if (!w.lone) plan_slices(w.arena, pl, nw);
+  w.arena.add(w.d_sum, (size_t)(s.stride * nw));
+  if (q.sr) sched_slices(w.arena, nw, s.nc, PU, q.base->n_node_ids, s.MO, (long long)PU * s.MO, w.sched, w.wtmp, w.wtmp_bytes, s.ctx->stream);
+  if (!w.ow.empty()) w.arena.add(w.d_ow, w.ow.size());
+  analysis_slices(s, w.arena, w.an, w.sched, nw, pl);
+  try {
+    w.arena.alloc(s.ctx->stream, "a scenario wave");
+  } catch (const Error&) {
+    if (q.max_concurrent <= 0 && nw > 1) return false;      // the free memory moved
+    throw;
+  }
+  w.G.assign(q.cr && q.cr->span ? (size_t)nw * s.nc : 0, 0);
+  return true;
+}
+
+// The node tables of wave w's members (small host copies; the hierarchy masks and extra counts of the base), the base
+// replicated into every member's slices, the weight overrides, and the chains' copy of the base's prev rows and flags.
+static void wave_upload(const Sweep& s, Wave& w) {
+  blance_ctx* ctx = s.ctx;
   cudaStream_t st = ctx->stream;
+  blance_plan* pl = w.pl;
+  const blance_plan* pb = s.pb.get();
+  DPool& P = pl->pool;
+  if (!w.lone) {
+    upload_nodes(ctx, pl, w.ins, s.q.cr != nullptr);
+    CUDA(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(w.nw + 1), cudaMemcpyHostToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(w.nw + 1), cudaMemcpyHostToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->d_seg_off, w.seg_off.data(), sizeof(int) * (size_t)(w.nw + 1), cudaMemcpyHostToDevice, st));
+    CUDA(cudaStreamSynchronize(st));          // the upload completes before the wave's first kernel is enqueued
+  }
+  if (!w.lone && pl->PT > 0)
+    launch(ctx, k_scenario_replicate, grid_for(ctx, pl->PT, 256), 256, 0, pl->rows_init, pl->prev_rows_init, pl->pmeta_init,
+           pl->prev_meta_init, pl->pflags_init, const_cast<int32_t*>(P.pweight), const_cast<int32_t*>(P.name_rank),
+           const_cast<int32_t*>(P.part_inst), pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init,
+           pb->pflags_init, pb->pool.pweight, pb->pool.name_rank, s.q.base->n_parts, pl->h_insts[0].SLP, pl->PT);
+  if (!w.ow.empty()) {
+    const int k = (int)(w.ow.size() / 3);
+    CUDA(cudaMemcpyAsync(w.d_ow, w.ow.data(), sizeof(int32_t) * w.ow.size(), cudaMemcpyHostToDevice, st));
+    launch(ctx, k_scenario_weights, grid_for(ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, w.d_ow, k);
+  }
+  if (s.q.cr && s.q.cr->net && pl->PT > 0) {   // the stage boundary overwrites these (in the lone path, the base upload's own)
+    CUDA(cudaMemcpyAsync(w.an.net_prev, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(w.an.net_flags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+  }
+  if (!w.lone) finish_upload(ctx, pl);
+}
+
+// The stage boundary before stage t: what the convergence loop left in the working state is the next stage's input -
+// the assigned partitions' prev and cur rows are their next rows, committed by k_commit (or equal to them when the
+// stage converged) with their flags - then the next stage's node tables and a fresh loop state.
+static void stage_boundary(const Sweep& s, Wave& w, int t) {
+  cudaStream_t st = s.ctx->stream;
+  blance_plan* pl = w.pl;
+  if (pl->PT > 0) {
+    CUDA(cudaMemcpyAsync(pl->rows_init, pl->pool.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_rows_init, pl->pool.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->pmeta_init, pl->pool.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_meta_init, pl->pool.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->pflags_init, pl->pool.pflags, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+  }
+  for (int j = 0; j < w.nw; ++j) {
+    w.ins[(size_t)j] = stage_in(s.q, s.idx[(size_t)(w.w0 + j)], t, w.code[(size_t)j]);
+    node_state(pl->h_insts[(size_t)j], w.ins[(size_t)j], s.q.cr != nullptr, s.n_prev_later);
+  }
+  upload_nodes(s.ctx, pl, w.ins, s.q.cr != nullptr);
+}
+
+// Summaries (node_ops | state_node_load | 3 scalars per member, s.stride int64 words) of wave w's plans from the beg
+// rows / flags `prev_rows` / `pflags` to the working rows, into d_sum.
+static void wave_summary(const Sweep& s, const Wave& w, const int32_t* prev_rows, const uint8_t* pflags, long long* d_sum) {
+  const int PU = s.q.base->n_parts, NU = s.q.base->n_node_ids, nw = w.nw;
+  CUDA(cudaMemsetAsync(d_sum, 0, sizeof(long long) * (size_t)(s.stride * nw), s.ctx->stream));
+  if (PU <= 0) return;
+  const size_t smem = align_up(sizeof(uint32_t) * 4 * (size_t)NU, 8) + sizeof(long long) * (size_t)s.q.base->n_states * NU;
+  const dim3 grid((unsigned)std::max(1, std::min((PU + 255) / 256, std::max(1, s.ctx->sm_count * 8 / nw))), (unsigned)nw);
+  if (smem <= 48 * 1024) launch(s.ctx, k_scenario_summary<true>, grid, 256, smem, w.pl->pool, prev_rows, pflags, s.q.favor_min, s.stride, d_sum);
+  else launch(s.ctx, k_scenario_summary<false>, grid, 256, 0, w.pl->pool, prev_rows, pflags, s.q.favor_min, s.stride, d_sum);
+}
+
+// Plans stage t of wave w and hands its results to the caller: the summaries (at a chain's last stage also the net
+// summaries), the audits of the final maps, the requested rows and the loop's counters.  Returns the summaries.
+static std::vector<long long> stage_results(const Sweep& s, Wave& w, int t) {
+  blance_ctx* ctx = s.ctx;
+  cudaStream_t st = ctx->stream;
+  const WaveReq& q = s.q;
+  blance_plan* pl = w.pl;
+  DPool& P = pl->pool;
+  const int nw = w.nw, NU = q.base->n_node_ids, PU = q.base->n_parts, S = q.base->n_states;
+  CUDA(cudaEventRecord(ctx->ev[0], st));
+  run(ctx, pl);
+  // summaries, then the requested rows
+  CUDA(cudaEventRecord(ctx->ev[1], st));
+  wave_summary(s, w, pl->prev_rows_init, pl->pflags_init, w.d_sum);
+  if (q.cr && q.cr->net && t == s.T - 1) wave_summary(s, w, w.an.net_prev, w.an.net_flags, w.an.net_sum);
+  CUDA(cudaEventRecord(ctx->ev[2], st));
+  auto out_of = [&](int j) -> blance_scenario_out& { return q.out[out_at(s, w, j, 1, s.T, t)]; };
+  // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
+  std::vector<AuditInst> a_insts;
+  std::vector<std::vector<long long>> a_host((size_t)(q.ar ? nw : 0));
+  if (q.ar) {
+    for (int j = 0; j < nw; ++j) {
+      const DInst& D = pl->h_insts[(size_t)j];
+      AuditInst A = audit_inst(D);
+      A.rows = P.rows + D.rows_off; A.alt_rows = pl->prev_rows_init + D.rows_off;
+      A.meta = P.pmeta + D.part_off; A.alt_meta = pl->prev_meta_init + D.part_off;
+      A.pflags = pl->pflags_init + D.part_off;
+      A.ie_mask = P.ie_mask + D.mask_off;
+      A.stride = D.SLP;
+      a_insts.push_back(A);
+    }
+    audit_run(ctx, w.an.audit, *q.ar, a_insts);
+    for (int j = 0; j < nw; ++j) audit_fetch(ctx, w.an.audit, j, a_host[(size_t)j], q.ar->out[out_at(s, w, j, 1, s.T, t)]);
+  }
+  bool any_rows = false;
+  for (int j = 0; j < nw; ++j) {
+    const blance_scenario_out& o = out_of(j);
+    any_rows |= o.next_rows || o.next_shape || o.warn;
+  }
+  if (any_rows && pl->PT > 0)
+    launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
+           pl->d_raw_shape_off, pl->PT);
+  std::vector<long long> h_sum((size_t)(s.stride * nw));
+  std::vector<DInst> fin((size_t)nw);
+  CUDA(cudaMemcpyAsync(h_sum.data(), w.d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st));
+  CUDA(cudaMemcpyAsync(fin.data(), P.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st));
+  const size_t rr = (size_t)PU * q.base->n_slots, rs = (size_t)PU * S;
+  for (int j = 0; j < nw; ++j) {
+    blance_scenario_out& o = out_of(j);
+    if (rr && o.next_rows) CUDA(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st));
+    if (rs && o.next_shape) CUDA(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+    if (rs && o.warn) CUDA(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
+  }
+  CUDA(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&w.sum_ms, ctx->ev[1], ctx->ev[2]);
+  for (int j = 0; j < nw; ++j) {
+    if (fin[(size_t)j].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
+    blance_scenario_out& o = out_of(j);
+    const long long* h = h_sum.data() + (size_t)j * (size_t)s.stride;
+    if (o.node_ops) std::memcpy(o.node_ops, h, sizeof(int64_t) * 4 * (size_t)NU);
+    if (o.state_node_load) std::memcpy(o.state_node_load, h + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
+    o.parts_moved = h[s.stride - 3]; o.ops_total = h[s.stride - 2]; o.warn_parts = h[s.stride - 1];
+    o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
+    o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
+    if (q.ar) audit_unpack(ctx, w.an.audit, a_insts[(size_t)j].n_rules, a_host[(size_t)j], q.ar->out[out_at(s, w, j, 1, s.T, t)]);
+  }
+  return h_sum;
+}
+
+// The schedules of wave w's instances from the beg rows / flags `beg` / `pflags` to the working rows, each member's ops
+// per node from its summary in `sum`, into outs (NULL: kept on the device only).  Returns the instances' scalars.
+static std::vector<unsigned long long> stage_schedule(const Sweep& s, Wave& w, const int32_t* beg, const uint8_t* pflags,
+                                                      const std::vector<long long>& sum, blance_scenario_schedule_out* outs, int per, int t) {
+  cudaStream_t st = s.ctx->stream;
+  const int NU = s.q.base->n_node_ids, PU = s.q.base->n_parts;
+  const WSched& W = w.sched;
+  if (s.q.er) {
+    CUDA(cudaMemsetAsync(W.op_round, 0xFF, sizeof(int32_t) * (size_t)w.nw * s.nc * PU * s.MO, st));
+    if (w.an.expo.parent) CUDA(cudaMemcpyAsync(w.an.expo.parent, s.q.er->parent, sizeof(int32_t) * (size_t)s.V, cudaMemcpyHostToDevice, st));
+  }
+  if (PU > 0) launch(s.ctx, k_wave_moves, wave_grid(s.ctx, PU, w.nw), 256, 0, w.pl->pool, beg, pflags, s.q.favor_min, W);
+  std::vector<long long> ops((size_t)w.nw * NU);        // each member's ops per node: its node_ops summed over the kinds
+  for (size_t x = 0; x < ops.size(); ++x) {
+    const long long* h = sum.data() + (x / NU) * s.stride + 4 * (x % NU);
+    ops[x] = h[0] + h[1] + h[2] + h[3];
+  }
+  std::vector<unsigned long long> scal = wave_schedule(s.ctx, "blance_plan_scenarios_schedule", *s.q.sr, W, w.wtmp, w.wtmp_bytes, ops.data());
+  for (long long i = 0; outs && i < (long long)w.nw * s.nc; ++i) {
+    blance_scenario_schedule_out& o = outs[out_at(s, w, i, s.nc, per, t)];
+    o.rounds = (int32_t)scal[(size_t)(4 * i)];
+    o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
+    o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
+    o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
+    if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, W.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+    if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, W.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
+    if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, W.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
+  }
+  return scal;
+}
+
+// Folds stage t of wave w (scal: its schedules' scalars) into the chains' spans, before the next stage boundary
+// overwrites the schedule and exposure: the arrays on the device (k_chain_fold), the scalars here.
+static void span_fold(const Sweep& s, Wave& w, int t, const std::vector<unsigned long long>& scal) {
+  blance_ctx* ctx = s.ctx;
+  const int PU = s.q.base->n_parts, NU = s.q.base->n_node_ids;
+  CUDA(cudaEventRecord(ctx->ev[4], ctx->stream));
+  ChainFold F = w.an.span.F;
+  F.node_rounds = w.sched.node_rounds; F.node_last = w.sched.node_last; F.part_done = w.sched.part_done;
+  F.part_min = w.an.expo.E.part_min; F.part_notop = w.an.expo.E.part_notop; F.part_flags = w.an.expo.E.part_flags;
+  F.dom_key = w.an.expo.dom_key; F.G = w.an.span.G;
+  F.ni = (long long)w.nw * s.nc; F.PU = PU; F.NU = NU; F.V = (int32_t)s.V; F.stage = t;
+  CUDA(cudaMemcpyAsync(w.an.span.G, w.G.data(), sizeof(long long) * w.G.size(), cudaMemcpyHostToDevice, ctx->stream));
+  const long long n_el = F.ni * ((long long)PU + NU + s.V);
+  if (n_el > 0) launch(ctx, k_chain_fold, grid_for(ctx, n_el, 256), 256, 0, F);
+  CUDA(cudaEventRecord(ctx->ev[5], ctx->stream));
+  CUDA(cudaEventSynchronize(ctx->ev[5]));     // G is rewritten below
+  cudaEventElapsedTime(&w.fold_ms, ctx->ev[4], ctx->ev[5]);
+  for (long long i = 0; i < F.ni; ++i) {
+    blance_chain_span_out& sp = s.q.cr->span[out_at(s, w, i, s.nc, 1, 0)];
+    const int R = (int)scal[(size_t)(4 * i)];
+    if (t == 0) {
+      sp.rounds = sp.moves_done = sp.stuck_parts = 0;
+      sp.max_batch = 0;
+      for (int m = 0; m < BLANCE_EXPO_N; ++m) { sp.peak[m] = 0; sp.peak_stage[m] = 0; sp.peak_round[m] = 0; sp.area[m] = 0; }
+    }
+    sp.rounds += R;
+    sp.moves_done += (int64_t)scal[(size_t)(4 * i + 1)];
+    sp.stuck_parts += (int64_t)scal[(size_t)(4 * i + 2)];
+    sp.max_batch = std::max(sp.max_batch, (int32_t)scal[(size_t)(4 * i + 3)]);
+    w.G[(size_t)i] += R;
+    if (!s.q.er) continue;
+    const blance_exposure_out& e = s.q.er->out[out_at(s, w, i, s.nc, s.T, t)];
+    for (int m = 0; m < BLANCE_EXPO_N; ++m) {
+      if (t == 0 || e.peak[m] > sp.peak[m]) { sp.peak[m] = e.peak[m]; sp.peak_stage[m] = t; sp.peak_round[m] = e.peak_round[m]; }
+      sp.area[m] += e.area[m];
+    }
+  }
+}
+
+// The chains' net results of wave w: the summaries of the direct rebalance from the base's prevMap to the last stage's
+// final map, then its schedules and exposures on the wave's buffers (the last stage's were copied out and folded).
+static void net_results(const Sweep& s, Wave& w) {
+  const ChainReq& cr = *s.q.cr;
+  std::vector<long long> h_net((size_t)(s.stride * w.nw));
+  CUDA(cudaMemcpyAsync(h_net.data(), w.an.net_sum, sizeof(long long) * h_net.size(), cudaMemcpyDeviceToHost, s.ctx->stream));
+  CUDA(cudaStreamSynchronize(s.ctx->stream));
+  for (int j = 0; j < w.nw; ++j) {
+    blance_chain_out& o = cr.net[s.idx[(size_t)(w.w0 + j)]];
+    const long long* h = h_net.data() + (size_t)j * (size_t)s.stride;
+    if (o.node_ops) std::memcpy(o.node_ops, h, sizeof(int64_t) * 4 * (size_t)s.q.base->n_node_ids);
+    o.parts_moved = h[s.stride - 3]; o.ops_total = h[s.stride - 2];
+  }
+  if (!cr.net_sched && !cr.net_expo) return;
+  const std::vector<unsigned long long> scal = stage_schedule(s, w, w.an.net_prev, w.an.net_flags, h_net, cr.net_sched, 1, 0);
+  if (cr.net_expo) wave_exposure(s, w, w.an.net_prev, w.an.net_flags, cr.net_expo, 1, 0, scal);
+}
+
+// The folded span arrays of wave w out to the caller.
+static void span_out(const Sweep& s, const Wave& w) {
+  const ChainReq& cr = *s.q.cr;
+  const ChainFold& F = w.an.span.F;
+  const long long PU = s.q.base->n_parts, NU = s.q.base->n_node_ids, V = s.V;
+  auto d2h = [&](void* dst, const void* src, size_t bytes) { if (dst && src && bytes) CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s.ctx->stream)); };
+  for (long long i = 0; i < (long long)w.nw * s.nc; ++i) {
+    blance_chain_span_out& sp = cr.span[out_at(s, w, i, s.nc, 1, 0)];
+    d2h(sp.node_rounds, F.a_node_rounds + i * NU, sizeof(int32_t) * NU);
+    d2h(sp.node_last_round, F.a_node_last + i * NU, sizeof(int64_t) * NU);
+    d2h(sp.part_done_round, F.a_part_done + i * PU, sizeof(int64_t) * PU);
+    if (cr.span_parts) {
+      d2h(sp.part_min_copies, F.a_part_min + i * PU, sizeof(int32_t) * PU);
+      d2h(sp.part_no_top, F.a_part_notop + i * PU, sizeof(int32_t) * PU);
+      d2h(sp.part_flags, F.a_part_flags + i * PU, (size_t)PU);
+    }
+    if (cr.span_dom) {
+      d2h(sp.dom_peak, F.a_dom_peak + i * V, sizeof(int64_t) * V);
+      d2h(sp.dom_peak_stage, F.a_dom_stage + i * V, sizeof(int32_t) * V);
+      d2h(sp.dom_peak_round, F.a_dom_round + i * V, sizeof(int32_t) * V);
+    }
+  }
+  CUDA(cudaStreamSynchronize(s.ctx->stream));
+}
+
+// The BLANCE_SCENARIO_TIMES line of stage t of wave w.
+static void report(const Sweep& s, const Wave& w, int t) {
+  float wave_ms = 0.f;
+  cudaEventElapsedTime(&wave_ms, s.ctx->ev[0], s.ctx->ev[2]);
+  std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
+               w.w0, w.nw, s.W, s.per, wave_ms, w.sum_ms);
+  if (s.q.sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", w.sched_ms, s.nc);
+  if (s.q.er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", w.expo_ms, w.expo_bytes);
+  if (s.q.cr && s.q.cr->span) std::fprintf(stderr, ", span fold %.3f ms", w.fold_ms);
+  if (s.q.cr) std::fprintf(stderr, " (stage %d)", t);
+  std::fprintf(stderr, "\n");
+}
+
+// Plans the items idx of q on one device, in waves.  With q.cr each item is a chain of cr->T stages, planned in lock
+// step: a stage boundary is an iteration boundary plus the next stage's node tables (DESIGN.md section 12).
+static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, const WaveReq& q) {
+  Sweep s(ctx, idx, q);
   const int n_dev = (int)idx.size();
-  const int T = cr ? cr->T : 1;
-  const bool coded = cr != nullptr;
   std::vector<uint8_t> code0;
-  const blance_plan_in in0 = stage_in(*base, sc, opts, cr, idx[0], 0, code0);
+  const blance_plan_in in0 = stage_in(q, idx[0], 0, code0);
   long long max_mask = 0;
-  int max_ow = 0, max_rules = 0;
-  bool audit_flags = false;            // any caller wants the per-partition flags
+  int max_ow = 0;
   for (int i : idx) {
-    const blance_plan_in in = scenario_in(*base, nodes_of(sc, cr, i, 0), opts_of(opts, i));
+    const blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, 0), opts_of(q.opts, i));
     max_mask = std::max(max_mask, mask_words(in));
-    max_ow = std::max(max_ow, n_overrides(opts_of(opts, i)));
-    max_rules = std::max(max_rules, in.has_hier_rules ? in.n_rules : 0);
-    for (int t = 0; ar && t < T; ++t) audit_flags |= ar->out[(size_t)i * T + t].part_flags != nullptr;
-  }
-  size_t extra_bytes = 0;              // one scenario's audit buffers / one chain's net buffers, priced into the wave
-  if (ar) {
-    Arena one;
-    AuditBufs b;
-    audit_slices(one, b, *ar, 1, base->n_states, max_rules, base->n_node_ids, base->n_nodes, base->n_parts, audit_flags);
-    extra_bytes = one.bytes();
-  }
-  const long long V = (long long)base->n_node_ids + (er ? er->n_domains : 0);
-  if (er) {                            // one scenario's exposure buffers: op states and rounds, outputs asked for
-    Arena one;
-    ExpoBufs b;
-    WSched w{};
-    expo_slices(one, b, w, *er, 1, sr->nc, base->n_parts, scenario_ops(*base), V);
-    extra_bytes += one.bytes();
+    max_ow = std::max(max_ow, n_overrides(opts_of(q.opts, i)));
+    s.max_rules = std::max(s.max_rules, in.has_hier_rules ? in.n_rules : 0);
+    for (int t = 0; q.ar && t < s.T; ++t) s.audit_flags |= q.ar->out[(size_t)i * s.T + t].part_flags != nullptr;
   }
   {
     cudaMemPool_t pool;                // measure free memory without this context's cached arenas
-    if (max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
-      cudaStreamSynchronize(st);
+    if (q.max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
+      cudaStreamSynchronize(ctx->stream);
       cudaMemPoolTrimTo(pool, 0);
     }
   }
   // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
-  const PlanPtr pb = upload(ctx, 1, &in0, coded);
-  const long long stride = summary_stride(*base);
-  const bool want_net = cr && cr->net;
-  if (want_net) {                      // the base's prev rows and flags, kept for the net summary, and its result
-    Arena one;
-    int32_t* r = nullptr;
-    uint8_t* f = nullptr;
-    long long* d = nullptr;
-    one.add(r, (size_t)pb->RT + 4); one.add(f, (size_t)pb->PT + 1); one.add(d, (size_t)stride);
-    extra_bytes += one.bytes();
-  }
-  const bool want_span = cr && cr->span;
-  if (want_span) {                     // one chain's span accumulators
-    Arena one;
-    SpanBufs b;
-    span_slices(one, b, *cr, 1, sr->nc, base->n_parts, base->n_node_ids, V);
-    extra_bytes += one.bytes();
-  }
-  size_t per = 0;
-  int W = wave_size(ctx, in0, max_mask, max_ow, n_dev, max_concurrent, sr, extra_bytes, &per);
-  if (W < 1)
-    throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(per >> 20) + " MiB, more than the free device memory");
-  const bool auto_wave = max_concurrent <= 0;
-  const bool times = getenv("BLANCE_SCENARIO_TIMES") != nullptr;
-  const int PU = base->n_parts, NU = base->n_node_ids, S = base->n_states;
-  int n_prev_later = 0;                // len(prevMap) from stage 2 on: the base's prevMap plus every assigned partition
-  for (int p = 0; cr && p < PU; ++p) n_prev_later += (base->part_in_prev[p] || base->part_in_assign[p]) ? 1 : 0;
+  s.pb = upload(ctx, 1, &in0, q.cr != nullptr);
+  Arena one;                           // one member's analysis buffers, priced into the wave
+  AnalysisBufs one_bufs;
+  WSched one_sched{};
+  analysis_slices(s, one, one_bufs, one_sched, 1, s.pb.get());
+  s.W = wave_size(ctx, in0, max_mask, max_ow, n_dev, q.max_concurrent, q.sr, one.bytes(), &s.per);
+  if (s.W < 1)
+    throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(s.per >> 20) + " MiB, more than the free device memory");
+  for (int p = 0; q.cr && p < q.base->n_parts; ++p) s.n_prev_later += (q.base->part_in_prev[p] || q.base->part_in_assign[p]) ? 1 : 0;
   for (int w0 = 0; w0 < n_dev;) {
-    const int nw = std::min(W, n_dev - w0);
-    std::vector<blance_plan_in> ins((size_t)nw);
-    std::vector<std::vector<uint8_t>> code((size_t)nw);
-    for (int j = 0; j < nw; ++j) ins[(size_t)j] = stage_in(*base, sc, opts, cr, idx[(size_t)(w0 + j)], 0, code[(size_t)j]);
-    // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
-    const bool lone = n_dev == 1;
-    blance_plan wave_plan;
-    blance_plan* pl = lone ? pb.get() : &wave_plan;
-    std::vector<int> seg_off;
-    if (!lone) layout(pl, nw, ins.data(), seg_off, coded);
-    if (!lone && pl->PT >= (1LL << 29)) {
-      if (nw > 1) { W = nw / 2; continue; }
-      throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
-    }
-    // the wave's partition-weight overrides over its replicated slices (lone: over the base upload), as
-    // wave-global partition indices: ow = index[k] | weight[k] | presence[k]
-    std::vector<int32_t> ow;
-    for (int pass = 0; pass < 3; ++pass)
-      for (int j = 0; j < nw; ++j) {
-        const blance_scenario_opts* o = opts_of(opts, idx[(size_t)(w0 + j)]);
-        for (int k = 0; k < n_overrides(o); ++k)
-          ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
-      }
-    // one allocation per wave, so that a plan is never lost for want of its summaries or schedule state: the
-    // wave's plan (lone: the base upload is the plan), the summaries, the schedule state, the weight overrides,
-    // the chains' net buffers
-    Arena wave;
-    if (!lone) plan_slices(wave, pl, nw);
-    long long* d_sum = nullptr;
-    wave.add(d_sum, (size_t)(stride * nw));
-    WSched wsch{};
-    void* wtmp = nullptr;
-    size_t wtmp_bytes = 0;
-    if (sr) sched_slices(wave, nw, sr->nc, PU, NU, scenario_ops(*base), (long long)PU * scenario_ops(*base), wsch, wtmp, wtmp_bytes, st);
-    int32_t* d_ow = nullptr;
-    if (!ow.empty()) wave.add(d_ow, ow.size());
-    AuditBufs abuf;
-    if (ar) audit_slices(wave, abuf, *ar, nw, S, max_rules, NU, base->n_nodes, PU, audit_flags);
-    ExpoBufs ebuf;
-    if (er) expo_slices(wave, ebuf, wsch, *er, nw, sr->nc, PU, scenario_ops(*base), V);
-    int32_t* net_prev = nullptr;
-    uint8_t* net_flags = nullptr;
-    long long* d_net = nullptr;
-    if (want_net) { wave.add(net_prev, (size_t)pl->RT + 4); wave.add(net_flags, (size_t)pl->PT + 1); wave.add(d_net, (size_t)(stride * nw)); }
-    SpanBufs sbuf;
-    if (want_span) span_slices(wave, sbuf, *cr, nw, sr->nc, PU, NU, V);
-    try {
-      wave.alloc(st, "a scenario wave");
-    } catch (const Error&) {
-      if (auto_wave && nw > 1) { W = nw / 2; continue; }      // the free memory moved
-      throw;
-    }
-    DPool& P = pl->pool;
-    // the node tables of the wave's scenarios (small host copies); the hierarchy masks and extra counts of the base
-    if (!lone) {
-      upload_nodes(ctx, pl, ins, coded);
-      CUDA(cudaMemcpyAsync(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaMemcpyAsync(pl->d_seg_off, seg_off.data(), sizeof(int) * (size_t)(nw + 1), cudaMemcpyHostToDevice, st));
-      CUDA(cudaStreamSynchronize(st));          // the host vectors die at the end of this block
-    }
-    if (!lone && pl->PT > 0)
-      launch(ctx, k_scenario_replicate, grid_for(ctx, pl->PT, 256), 256, 0, pl->rows_init, pl->prev_rows_init, pl->pmeta_init,
-             pl->prev_meta_init, pl->pflags_init, const_cast<int32_t*>(P.pweight), const_cast<int32_t*>(P.name_rank),
-             const_cast<int32_t*>(P.part_inst), pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init,
-             pb->pflags_init, pb->pool.pweight, pb->pool.name_rank, PU, pl->h_insts[0].SLP, pl->PT);
-    if (!ow.empty()) {
-      const int k = (int)(ow.size() / 3);
-      CUDA(cudaMemcpyAsync(d_ow, ow.data(), sizeof(int32_t) * ow.size(), cudaMemcpyHostToDevice, st));
-      launch(ctx, k_scenario_weights, grid_for(ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, d_ow, k);
-    }
-    if (want_net && pl->PT > 0) {      // the stage boundary overwrites these (in the lone path, the base upload's own)
-      CUDA(cudaMemcpyAsync(net_prev, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-      CUDA(cudaMemcpyAsync(net_flags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-    }
-    if (!lone) finish_upload(ctx, pl);
-    // the caller's outputs of wave member j (at stage t) and instance i = j * nc + k
-    auto out_index = [&](int j, int t) { return (size_t)idx[(size_t)(w0 + j)] * T + t; };
-    auto expo_outs = [&](int t, blance_exposure_out* o, int per) {
-      std::vector<blance_exposure_out*> v;
-      for (long long i = 0; i < (long long)nw * sr->nc; ++i)
-        v.push_back(o + ((size_t)idx[(size_t)(w0 + i / sr->nc)] * per + t) * sr->nc + (size_t)(i % sr->nc));
-      return v;
-    };
-    std::vector<long long> G(want_span ? (size_t)nw * sr->nc : 0, 0);    // each instance's G_t
-    // the schedules of the wave's instances from the beg rows / flags `beg` / `pflags` to the working rows, each
-    // scenario's ops per node read from its summary in `sum`; instance i's result goes to outs[(idx * per + t) * nc + k]
-    // (outs NULL: kept on the device only).  Returns the instances' scalars.
-    auto schedule = [&](const int32_t* beg, const uint8_t* pflags, const std::vector<long long>& sum, blance_scenario_schedule_out* outs,
-                        int per, int t) {
-      if (er) {
-        CUDA(cudaMemsetAsync(wsch.op_round, 0xFF, sizeof(int32_t) * (size_t)nw * sr->nc * PU * scenario_ops(*base), st));
-        if (ebuf.parent) CUDA(cudaMemcpyAsync(ebuf.parent, er->parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
-      }
-      if (PU > 0) launch(ctx, k_wave_moves, wave_grid(ctx, PU, nw), 256, 0, pl->pool, beg, pflags, favor_min, wsch);
-      std::vector<long long> ops((size_t)nw * NU);        // each scenario's ops per node: its node_ops summed over the kinds
-      for (size_t x = 0; x < ops.size(); ++x) {
-        const long long* s = sum.data() + (x / NU) * stride + 4 * (x % NU);
-        ops[x] = s[0] + s[1] + s[2] + s[3];
-      }
-      std::vector<unsigned long long> scal = wave_schedule(ctx, "blance_plan_scenarios_schedule", *sr, wsch, wtmp, wtmp_bytes, ops.data());
-      for (long long i = 0; outs && i < (long long)nw * sr->nc; ++i) {
-        blance_scenario_schedule_out& o = outs[((size_t)idx[(size_t)(w0 + i / sr->nc)] * per + t) * sr->nc + (size_t)(i % sr->nc)];
-        o.rounds = (int32_t)scal[(size_t)(4 * i)];
-        o.moves_done = (int64_t)scal[(size_t)(4 * i + 1)];
-        o.stuck_parts = (int64_t)scal[(size_t)(4 * i + 2)];
-        o.max_batch = (int32_t)scal[(size_t)(4 * i + 3)];
-        if (o.node_rounds && NU) CUDA(cudaMemcpyAsync(o.node_rounds, wsch.node_rounds + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-        if (o.node_last_round && NU) CUDA(cudaMemcpyAsync(o.node_last_round, wsch.node_last + i * NU, sizeof(int32_t) * NU, cudaMemcpyDeviceToHost, st));
-        if (o.part_done_round && PU) CUDA(cudaMemcpyAsync(o.part_done_round, wsch.part_done + i * PU, sizeof(int32_t) * PU, cudaMemcpyDeviceToHost, st));
-      }
-      return scal;
-    };
-    for (int t = 0; t < T; ++t) {
-      if (t > 0) {
-        // the stage boundary: what the convergence loop left in the working state is the next stage's input - the
-        // assigned partitions' prev and cur rows are their next rows, committed by k_commit (or equal to them when the
-        // stage converged) with their flags - then the next stage's node tables and a fresh loop state
-        if (pl->PT > 0) {
-          CUDA(cudaMemcpyAsync(pl->rows_init, P.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-          CUDA(cudaMemcpyAsync(pl->prev_rows_init, P.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-          CUDA(cudaMemcpyAsync(pl->pmeta_init, P.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-          CUDA(cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-          CUDA(cudaMemcpyAsync(pl->pflags_init, P.pflags, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-        }
-        for (int j = 0; j < nw; ++j) {
-          ins[(size_t)j] = stage_in(*base, sc, opts, cr, idx[(size_t)(w0 + j)], t, code[(size_t)j]);
-          node_state(pl->h_insts[(size_t)j], ins[(size_t)j], coded, n_prev_later);
-        }
-        upload_nodes(ctx, pl, ins, coded);
-      }
-      CUDA(cudaEventRecord(ctx->ev[0], st));
-      run(ctx, pl);
-      // summaries, then the requested rows
-      float sum_ms = 0.f, sched_ms = 0.f;
-      CUDA(cudaEventRecord(ctx->ev[1], st));
-      wave_summary(ctx, pl, nw, pl->prev_rows_init, pl->pflags_init, favor_min, stride, d_sum);
-      if (want_net && t == T - 1) wave_summary(ctx, pl, nw, net_prev, net_flags, favor_min, stride, d_net);
-      CUDA(cudaEventRecord(ctx->ev[2], st));
-      // the output of wave member j at this stage
-      auto out_of = [&](int j) -> blance_scenario_out& { return out[out_index(j, t)]; };
-      // the audits of the wave's final maps: assigned partitions from the next rows, the others from prevMap as uploaded
-      std::vector<AuditInst> a_insts;
-      std::vector<std::vector<long long>> a_host((size_t)(ar ? nw : 0));
-      if (ar) {
-        for (int j = 0; j < nw; ++j) {
-          const DInst& D = pl->h_insts[(size_t)j];
-          AuditInst A = audit_inst(D);
-          A.rows = P.rows + D.rows_off; A.alt_rows = pl->prev_rows_init + D.rows_off;
-          A.meta = P.pmeta + D.part_off; A.alt_meta = pl->prev_meta_init + D.part_off;
-          A.pflags = pl->pflags_init + D.part_off;
-          A.ie_mask = P.ie_mask + D.mask_off;
-          A.stride = D.SLP;
-          a_insts.push_back(A);
-        }
-        audit_run(ctx, abuf, *ar, a_insts);
-        for (int j = 0; j < nw; ++j) audit_fetch(ctx, abuf, j, a_host[(size_t)j], ar->out[out_index(j, t)]);
-      }
-      bool any_rows = false;
-      for (int j = 0; j < nw; ++j) {
-        const blance_scenario_out& o = out_of(j);
-        any_rows |= o.next_rows || o.next_shape || o.warn;
-      }
-      if (any_rows && pl->PT > 0)
-        launch(ctx, k_pack, grid_for(ctx, pl->PT, 256), 256, 0, P, pl->raw_a, pl->rawsh_a, pl->rawsh_b, pl->d_raw_rows_off,
-               pl->d_raw_shape_off, pl->PT);
-      std::vector<long long> h_sum((size_t)(stride * nw));
-      std::vector<DInst> fin((size_t)nw);
-      CUDA(cudaMemcpyAsync(h_sum.data(), d_sum, sizeof(long long) * h_sum.size(), cudaMemcpyDeviceToHost, st));
-      CUDA(cudaMemcpyAsync(fin.data(), P.insts, sizeof(DInst) * (size_t)nw, cudaMemcpyDeviceToHost, st));
-      for (int j = 0; j < nw; ++j) {
-        blance_scenario_out& o = out_of(j);
-        const size_t rr = (size_t)PU * base->n_slots, rs = (size_t)PU * S;
-        if (rr && o.next_rows) CUDA(cudaMemcpyAsync(o.next_rows, pl->raw_a + pl->raw_rows_off[(size_t)j], sizeof(int32_t) * rr, cudaMemcpyDeviceToHost, st));
-        if (rs && o.next_shape) CUDA(cudaMemcpyAsync(o.next_shape, pl->rawsh_a + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
-        if (rs && o.warn) CUDA(cudaMemcpyAsync(o.warn, pl->rawsh_b + pl->raw_shape_off[(size_t)j], rs, cudaMemcpyDeviceToHost, st));
-      }
-      CUDA(cudaStreamSynchronize(st));
-      cudaEventElapsedTime(&sum_ms, ctx->ev[1], ctx->ev[2]);
-      for (int j = 0; j < nw; ++j) {
-        if (fin[(size_t)j].spec_abort) throw_err(BLANCE_ERR_CUDA, "the speculative pass kernel gave up waiting (internal error; see stderr of the device printf)");
-        blance_scenario_out& o = out_of(j);
-        const long long* s = h_sum.data() + (size_t)j * (size_t)stride;
-        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
-        if (o.state_node_load) std::memcpy(o.state_node_load, s + 4ll * NU, sizeof(int64_t) * (size_t)S * NU);
-        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2]; o.warn_parts = s[stride - 1];
-        o.iters_run = fin[(size_t)j].iters_run; o.converged = fin[(size_t)j].converged;
-        o.steps = fin[(size_t)j].steps; o.sticky_steps = fin[(size_t)j].fast_steps;
-        if (ar) audit_unpack(ctx, abuf, a_insts[(size_t)j].n_rules, a_host[(size_t)j], ar->out[out_index(j, t)]);
-      }
-      float expo_ms = 0.f, fold_ms = 0.f;
-      size_t expo_bytes = 0;
-      if (sr) {
-        CUDA(cudaEventRecord(ctx->ev[3], st));
-        const std::vector<unsigned long long> scal = schedule(pl->prev_rows_init, pl->pflags_init, h_sum, sr->out, T, t);
-        CUDA(cudaEventRecord(ctx->ev[1], st));
+    Wave w(w0, std::min(s.W, n_dev - w0));
+    if (!wave_alloc(s, w)) { s.W = w.nw / 2; continue; }
+    wave_upload(s, w);
+    for (int t = 0; t < s.T; ++t) {
+      w.sum_ms = w.sched_ms = w.expo_ms = w.fold_ms = 0.f;
+      w.expo_bytes = 0;
+      if (t > 0) stage_boundary(s, w, t);
+      const std::vector<long long> h_sum = stage_results(s, w, t);
+      if (q.sr) {                      // the schedules, exposures and span fold of the stage
+        CUDA(cudaEventRecord(ctx->ev[3], ctx->stream));
+        const auto scal = stage_schedule(s, w, w.pl->prev_rows_init, w.pl->pflags_init, h_sum, q.sr->out, s.T, t);
+        CUDA(cudaEventRecord(ctx->ev[1], ctx->stream));
         CUDA(cudaEventSynchronize(ctx->ev[1]));
-        cudaEventElapsedTime(&sched_ms, ctx->ev[3], ctx->ev[1]);
-        const std::vector<blance_exposure_out*> eo = er ? expo_outs(t, er->out, T) : std::vector<blance_exposure_out*>();
-        if (er) wave_exposure(ctx, *er, pl, nw, sr->nc, pl->prev_rows_init, pl->pflags_init, eo, *base, wsch, ebuf, scal, &expo_ms, &expo_bytes);
-        if (want_span) {
-          // the stage folded into the span before the next stage boundary overwrites the schedule and exposure
-          CUDA(cudaEventRecord(ctx->ev[4], st));
-          ChainFold F = sbuf.F;
-          F.node_rounds = wsch.node_rounds; F.node_last = wsch.node_last; F.part_done = wsch.part_done;
-          F.part_min = ebuf.E.part_min; F.part_notop = ebuf.E.part_notop; F.part_flags = ebuf.E.part_flags;
-          F.dom_key = ebuf.dom_key; F.G = sbuf.G;
-          F.ni = (long long)nw * sr->nc; F.PU = PU; F.NU = NU; F.V = (int32_t)V; F.stage = t;
-          CUDA(cudaMemcpyAsync(sbuf.G, G.data(), sizeof(long long) * G.size(), cudaMemcpyHostToDevice, st));
-          const long long n_el = F.ni * ((long long)PU + NU + V);
-          if (n_el > 0) launch(ctx, k_chain_fold, grid_for(ctx, n_el, 256), 256, 0, F);
-          CUDA(cudaEventRecord(ctx->ev[5], st));
-          CUDA(cudaEventSynchronize(ctx->ev[5]));     // G is rewritten below
-          cudaEventElapsedTime(&fold_ms, ctx->ev[4], ctx->ev[5]);
-          for (long long i = 0; i < F.ni; ++i) {
-            blance_chain_span_out& s = cr->span[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
-            const int R = (int)scal[(size_t)(4 * i)];
-            if (t == 0) {
-              s.rounds = s.moves_done = s.stuck_parts = 0;
-              s.max_batch = 0;
-              for (int m = 0; m < BLANCE_EXPO_N; ++m) { s.peak[m] = 0; s.peak_stage[m] = 0; s.peak_round[m] = 0; s.area[m] = 0; }
-            }
-            s.rounds += R;
-            s.moves_done += (int64_t)scal[(size_t)(4 * i + 1)];
-            s.stuck_parts += (int64_t)scal[(size_t)(4 * i + 2)];
-            s.max_batch = std::max(s.max_batch, (int32_t)scal[(size_t)(4 * i + 3)]);
-            G[(size_t)i] += R;
-            if (!er) continue;
-            const blance_exposure_out& e = *eo[(size_t)i];
-            for (int m = 0; m < BLANCE_EXPO_N; ++m) {
-              if (t == 0 || e.peak[m] > s.peak[m]) { s.peak[m] = e.peak[m]; s.peak_stage[m] = t; s.peak_round[m] = e.peak_round[m]; }
-              s.area[m] += e.area[m];
-            }
-          }
-        }
+        cudaEventElapsedTime(&w.sched_ms, ctx->ev[3], ctx->ev[1]);
+        if (q.er) wave_exposure(s, w, w.pl->prev_rows_init, w.pl->pflags_init, q.er->out, s.T, t, scal);
+        if (q.cr && q.cr->span) span_fold(s, w, t, scal);
       }
-      if (times) {
-        float wave_ms = 0.f;
-        cudaEventElapsedTime(&wave_ms, ctx->ev[0], ctx->ev[2]);
-        std::fprintf(stderr, "[blance] scenario wave at %d: %d scenarios (wave size %d, %zu device bytes each), %.3f ms, summary %.3f ms",
-                     w0, nw, W, per, wave_ms, sum_ms);
-        if (sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", sched_ms, sr->nc);
-        if (er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", expo_ms, expo_bytes);
-        if (want_span) std::fprintf(stderr, ", span fold %.3f ms", fold_ms);
-        if (cr) std::fprintf(stderr, " (stage %d)", t);
-        std::fprintf(stderr, "\n");
-      }
+      if (getenv("BLANCE_SCENARIO_TIMES")) report(s, w, t);
     }
-    if (want_net) {
-      std::vector<long long> h_net((size_t)(stride * nw));
-      CUDA(cudaMemcpyAsync(h_net.data(), d_net, sizeof(long long) * h_net.size(), cudaMemcpyDeviceToHost, st));
-      CUDA(cudaStreamSynchronize(st));
-      for (int j = 0; j < nw; ++j) {
-        blance_chain_out& o = cr->net[idx[(size_t)(w0 + j)]];
-        const long long* s = h_net.data() + (size_t)j * (size_t)stride;
-        if (o.node_ops) std::memcpy(o.node_ops, s, sizeof(int64_t) * 4 * (size_t)NU);
-        o.parts_moved = s[stride - 3]; o.ops_total = s[stride - 2];
-      }
-      // the direct rebalance from the base's prevMap to the last stage's final map, on the wave's schedule and
-      // exposure buffers (the last stage's were copied out and folded above)
-      if (cr->net_sched || cr->net_expo) {
-        const std::vector<unsigned long long> scal = schedule(net_prev, net_flags, h_net, cr->net_sched, 1, 0);
-        if (cr->net_expo) {
-          float ms = 0.f;
-          size_t bytes = 0;
-          wave_exposure(ctx, *er, pl, nw, sr->nc, net_prev, net_flags, expo_outs(0, cr->net_expo, 1), *base, wsch, ebuf, scal, &ms, &bytes);
-        }
-      }
-    }
-    if (want_span) {                   // the folded arrays out
-      const long long ni = (long long)nw * sr->nc;
-      const SpanBufs& b = sbuf;
-      for (long long i = 0; i < ni; ++i) {
-        blance_chain_span_out& s = cr->span[(size_t)idx[(size_t)(w0 + i / sr->nc)] * sr->nc + (size_t)(i % sr->nc)];
-        auto d2h = [&](void* dst, const void* src, size_t bytes) { if (dst && src && bytes) CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st)); };
-        d2h(s.node_rounds, b.F.a_node_rounds + i * NU, sizeof(int32_t) * NU);
-        d2h(s.node_last_round, b.F.a_node_last + i * NU, sizeof(int64_t) * NU);
-        d2h(s.part_done_round, b.F.a_part_done + i * PU, sizeof(int64_t) * PU);
-        if (cr->span_parts) {
-          d2h(s.part_min_copies, b.F.a_part_min + i * PU, sizeof(int32_t) * PU);
-          d2h(s.part_no_top, b.F.a_part_notop + i * PU, sizeof(int32_t) * PU);
-          d2h(s.part_flags, b.F.a_part_flags + i * PU, (size_t)PU);
-        }
-        if (cr->span_dom) {
-          d2h(s.dom_peak, b.F.a_dom_peak + i * V, sizeof(int64_t) * V);
-          d2h(s.dom_peak_stage, b.F.a_dom_stage + i * V, sizeof(int32_t) * V);
-          d2h(s.dom_peak_round, b.F.a_dom_round + i * V, sizeof(int32_t) * V);
-        }
-      }
-      CUDA(cudaStreamSynchronize(st));
-    }
-    w0 += nw;
+    if (q.cr && q.cr->net) net_results(s, w);
+    if (q.cr && q.cr->span) span_out(s, w);
+    w0 += w.nw;
   }
-  cudaStreamSynchronize(st);
+  cudaStreamSynchronize(ctx->stream);
 }
 
 // The checks of one scenario's substituted instance (base_sum: see check_counts).  Returns a status, `why` the reason.
@@ -2201,30 +2261,29 @@ static int check_scenario(const blance_plan_in& base, const blance_scenario& sc,
   return st;
 }
 
-static void plan_scenarios(blance_ctx* ctx, const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
-                           const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out,
-                           const SchedReq* sr = nullptr, const AuditReq* ar = nullptr, const ExpoReq* er = nullptr) {
-  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n must be positive");
-  if (!base || !sc || !out) throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": base, sc or out is NULL");
-  // every scenario is checked before the context is used, so a NULL ctx checks the scenarios without a device
-  long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
-  for (int i = 0; i < n; ++i) {
-    std::string why;
-    const int st = check_scenario(*base, sc[i], opts_of(opts, i), base_sum, why);
-    if (st != BLANCE_OK) throw_err(st, std::string(name) + ": scenario " + std::to_string(i) + ": " + why);
-  }
+// Plans the n items of q, item i on device i mod G: one host thread per device, each with its own copy of the base.
+static void plan_wave(blance_ctx* ctx, int32_t n, const WaveReq& q) {
   if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  // several GPUs: scenario i -> device i mod G, one host thread per device, each with its own copy of the base
   const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
   std::vector<std::vector<int>> idx((size_t)G);
   for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
-  fan_out(ctx, G, [&](int d, blance_ctx* dev) {
-    scenarios_on_device(dev, base, idx[(size_t)d], sc, opts, favor_min_nodes, max_concurrent, out, sr, ar, nullptr, er);
-  });
+  fan_out(ctx, G, [&](int d, blance_ctx* dev) { scenarios_on_device(dev, idx[(size_t)d], q); });
 }
 
-// Chains of stages over one base (blance_plan_chains): chain i -> device i mod G, its stages planned in lock step
-// with the other chains of its wave.
+// Plans the n scenarios of q, each checked before the context is used: a NULL ctx checks them without a device.
+static void plan_scenarios(blance_ctx* ctx, const std::string& name, int32_t n, const WaveReq& q) {
+  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
+  if (!q.base || !q.sc || !q.out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, sc or out is NULL");
+  long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
+  for (int i = 0; i < n; ++i) {
+    std::string why;
+    const int st = check_scenario(*q.base, q.sc[i], opts_of(q.opts, i), base_sum, why);
+    if (st != BLANCE_OK) throw_err(st, name + ": scenario " + std::to_string(i) + ": " + why);
+  }
+  plan_wave(ctx, n, q);
+}
+
+// The checks of the chains of stages over one base that blance_plan_chains and blance_plan_chains_exposure plan.
 static void check_chains(const std::string& name, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
                          const blance_scenario_opts* opts, blance_scenario_out* out) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
@@ -2246,36 +2305,54 @@ static void check_chains(const std::string& name, const blance_plan_in* base, in
     }
 }
 
-// Plans the checked chains of cr (chain i -> device i mod G), with the schedules, audits and exposures asked for.
-static void plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const ChainReq& cr, const blance_scenario_opts* opts,
-                        int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out, const SchedReq* sr = nullptr,
-                        const AuditReq* ar = nullptr, const ExpoReq* er = nullptr) {
-  if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-  const int G = (int)std::min<size_t>((size_t)blance_ctx_device_count(ctx), (size_t)n);
-  std::vector<std::vector<int>> idx((size_t)G);
-  for (int i = 0; i < n; ++i) idx[(size_t)(i % G)].push_back(i);
-  fan_out(ctx, G, [&](int d, blance_ctx* dev) {
-    scenarios_on_device(dev, base, idx[(size_t)d], nullptr, opts, favor_min_nodes, max_concurrent, out, sr, ar, &cr, er);
-  });
+// The checked schedule request of n_move_conc / move_conc / node_has_mover over base; the scalars of the first n_clear
+// outputs of sched (none when n_clear <= 0) are cleared.
+static SchedReq sched_req(const std::string& name, const blance_plan_in* base, long long n_clear, int32_t n_move_conc, const int32_t* move_conc,
+                          const uint8_t* node_has_mover, blance_scenario_schedule_out* sched) {
+  if (n_move_conc < 1 || !move_conc || !sched)
+    throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive and move_conc and sched not NULL");
+  if (base && base->n_parts >= (1 << WAVE_PART_BITS))
+    throw_err(BLANCE_ERR_UNSUPPORTED, name + ": 2^29 or more partitions");
+  if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
+    throw_err(BLANCE_ERR_UNSUPPORTED, name + ": n_move_conc x n_parts exceeds 2^31 - 1");
+  SchedReq sr{n_move_conc, {}, {}, sched};
+  for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
+  if (base && base->n_node_ids > 0) {
+    sr.mover.assign((size_t)base->n_node_ids, 0);
+    for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
+  }
+  for (long long x = 0; x < n_clear; ++x) { sched[x].rounds = 0; sched[x].moves_done = 0; sched[x].stuck_parts = 0; sched[x].max_batch = 0; }
+  return sr;
 }
 
-extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
-                                  const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
-                                  int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
-  return entry(ctx, [&](Device&) {
-    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, out);
-    ChainReq cr;
-    cr.T = n_stages; cr.stages = stages; cr.net = net;
-    plan_chains(ctx, base, n, cr, opts, favor_min_nodes, max_concurrent, out);
-  });
+// check_audit_model over the first stages of the n scenarios sc, or of the n chains `stages` (none while NULL).
+static void check_audit_models(const std::string& name, const blance_plan_in& base, int32_t n, const blance_scenario* sc,
+                               const blance_chain_stage* stages, int32_t T, const blance_scenario_opts* opts) {
+  if (stages ? T < 1 : !sc) return;
+  for (int i = 0; i < n; ++i) {
+    const blance_plan_in in = scenario_in(base, stages ? stages[(size_t)i * T].nodes : sc[i], opts_of(opts, i));
+    check_audit_model(name + (stages ? ": chain " : ": scenario ") + std::to_string(i), &in);
+  }
 }
 
-static SchedReq sched_req(const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc, const blance_scenario_out* out,
-                          int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
-                          blance_scenario_schedule_out* sched);
+// A scheduled op emits at most two ancestor chains of AUDIT_DEPTH_MAX + 1 vertices and a partition has at most
+// 2 x n_slots ops: the static form of blance_moves_exposure's event bound, for the dom peaks asked for at `where`.
+static void check_event_bound(const std::string& name, const std::string& where, const blance_plan_in& base) {
+  if (2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base.n_slots) * std::max(0, base.n_parts) >= (1ll << 31))
+    throw_err(BLANCE_ERR_UNSUPPORTED, name + ": " + where + ": dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+}
 
-// The checked exposure request of eopts / series_cap, the flags of the outputs asked for in the [n_out] `outs` (NULL:
-// none) added to er.  `what(x)` names output x in a message.
+// The checked exposure request of series_cap and eopts (a forest only) over base, for the outputs expo.
+static ExpoReq expo_req(const std::string& name, const blance_plan_in& base, const blance_audit_opts* eopts, int32_t series_cap,
+                        blance_exposure_out* expo) {
+  if (series_cap < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": series_cap is negative");
+  if (eopts && eopts->flags) throw_err(BLANCE_ERR_INVALID_ARG, name + ": eopts.flags must be 0 (eopts carries a forest only)");
+  if (eopts) check_forest(name, eopts->n_domains, eopts->domain_parent, base.n_node_ids);
+  return ExpoReq{eopts ? eopts->n_domains : 0, eopts ? eopts->domain_parent : nullptr, series_cap, expo};
+}
+
+// The flags of the outputs asked for in the [n_out] `outs` (NULL: none) added to er, the event bound checked for each
+// that asks for dom peaks.  `what(x)` names output x in a message.
 template <class Name>
 static void expo_flags(const std::string& name, const blance_plan_in& base, const blance_exposure_out* outs, long long n_out, Name&& what,
                        ExpoReq& er) {
@@ -2285,9 +2362,19 @@ static void expo_flags(const std::string& name, const blance_plan_in& base, cons
     er.part_min |= o.part_min_copies != nullptr;
     er.part_notop |= o.part_no_top != nullptr;
     er.part_flags |= o.part_flags != nullptr;
-    if ((o.dom_peak || o.dom_peak_round) && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base.n_slots) * std::max(0, base.n_parts) >= (1ll << 31))
-      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": " + what(x) + ": dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+    if (o.dom_peak || o.dom_peak_round) check_event_bound(name, what(x), base);
   }
+}
+
+extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                  const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
+                                  int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
+  return entry(ctx, [&](Device&) {
+    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, out);
+    ChainReq cr;
+    cr.T = n_stages; cr.stages = stages; cr.net = net;
+    plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, nullptr, nullptr, &cr});
+  });
 }
 
 extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
@@ -2306,25 +2393,11 @@ extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in
     AuditReq ar;
     if (audit) {
       ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
-      for (int i = 0; stages && T > 0 && i < n; ++i) {
-        const blance_plan_in in = scenario_in(*base, stages[(size_t)i * T].nodes, opts_of(opts, i));
-        check_audit_model(name + ": chain " + std::to_string(i), &in);
-      }
+      check_audit_models(name, *base, n, nullptr, stages, T, opts);
     }
     if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive");
-    // sched_req reads n x nc outputs; a chain has T x nc of them, cleared here
-    SchedReq sr = sched_req(name.c_str(), base, 0, nullptr, nullptr, n_move_conc, move_conc, node_has_mover, sched);
-    for (long long x = 0; x < (long long)std::max(0, n) * std::max(0, T) * nc; ++x) { sched[x].rounds = 0; sched[x].moves_done = 0; sched[x].stuck_parts = 0; sched[x].max_batch = 0; }
-    if (series_cap < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": series_cap is negative");
-    ExpoReq er;
-    er.series_cap = series_cap;
-    er.out = expo;
-    if (eopts) {
-      if (eopts->flags) throw_err(BLANCE_ERR_INVALID_ARG, name + ": eopts.flags must be 0 (eopts carries a forest only)");
-      check_forest(name, eopts->n_domains, eopts->domain_parent, base->n_node_ids);
-      er.n_domains = eopts->n_domains;
-      er.parent = eopts->domain_parent;
-    }
+    const SchedReq sr = sched_req(name, base, (long long)std::max(0, n) * std::max(0, T) * nc, n_move_conc, move_conc, node_has_mover, sched);
+    ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
     ChainReq cr;
     cr.T = T; cr.stages = stages; cr.net = net; cr.net_sched = net_sched; cr.net_expo = net_expo; cr.span = span;
     for (long long x = 0; span && x < (long long)std::max(0, n) * nc; ++x) {
@@ -2340,19 +2413,18 @@ extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in
     auto pair_name = [&](long long x) { return "chain " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
     expo_flags(name, *base, expo, (long long)std::max(0, n) * std::max(0, T) * nc, stage_name, er);
     expo_flags(name, *base, net_expo, (long long)std::max(0, n) * nc, pair_name, er);
-    if (cr.span_dom && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base->n_slots) * std::max(0, base->n_parts) >= (1ll << 31))
-      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": span: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
+    if (cr.span_dom) check_event_bound(name, "span", *base);
     er.dom |= cr.span_dom;
     er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
     check_chains(name, base, n, n_stages, stages, opts, out);
-    plan_chains(ctx, base, n, cr, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, expo ? &er : nullptr);
+    plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, &cr, expo ? &er : nullptr});
   });
 }
 
 extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                      int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
   return entry(ctx, [&](Device&) {
-    plan_scenarios(ctx, "blance_plan_scenarios", base, n, sc, nullptr, favor_min_nodes, max_concurrent, out);
+    plan_scenarios(ctx, "blance_plan_scenarios", n, WaveReq{base, sc, nullptr, favor_min_nodes, max_concurrent, out});
   });
 }
 
@@ -2360,35 +2432,8 @@ extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* b
                                         const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                         blance_scenario_out* out) {
   return entry(ctx, [&](Device&) {
-    plan_scenarios(ctx, "blance_plan_scenarios_ex", base, n, sc, opts, favor_min_nodes, max_concurrent, out);
+    plan_scenarios(ctx, "blance_plan_scenarios_ex", n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out});
   });
-}
-
-// The checked schedule request of blance_plan_scenarios_schedule's arguments; the scalars of sched are cleared.
-static SchedReq sched_req(const char* name, const blance_plan_in* base, int32_t n, const blance_scenario* sc, const blance_scenario_out* out,
-                          int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
-                          blance_scenario_schedule_out* sched) {
-  if (n_move_conc < 1 || !move_conc || !sched)
-    throw_err(BLANCE_ERR_INVALID_ARG, std::string(name) + ": n_move_conc must be positive and move_conc and sched not NULL");
-  if (base && base->n_parts >= (1 << WAVE_PART_BITS))
-    throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": 2^29 or more partitions");
-  if (base && (long long)n_move_conc * std::max(0, base->n_parts) > INT32_MAX)
-    throw_err(BLANCE_ERR_UNSUPPORTED, std::string(name) + ": n_move_conc x n_parts exceeds 2^31 - 1");
-  SchedReq sr;
-  sr.nc = n_move_conc;
-  sr.out = sched;
-  for (int k = 0; k < n_move_conc; ++k) sr.count.push_back(move_conc[k] <= 0 ? 1 : move_conc[k]);   // orchestrate.go:484-487
-  if (base && base->n_node_ids > 0) {
-    sr.mover.assign((size_t)base->n_node_ids, 0);
-    for (int q = 0; q < base->n_node_ids; ++q) sr.mover[(size_t)q] = node_has_mover ? (node_has_mover[q] != 0) : (q < base->n_nodes);
-  }
-  if (n > 0 && sc && out)
-    for (int i = 0; i < n; ++i)
-      for (int k = 0; k < n_move_conc; ++k) {
-        blance_scenario_schedule_out& o = sched[(size_t)i * n_move_conc + k];
-        o.rounds = 0; o.moves_done = 0; o.stuck_parts = 0; o.max_batch = 0;
-      }
-  return sr;
 }
 
 extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
@@ -2396,10 +2441,10 @@ extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan
                                               int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
                                               blance_scenario_out* out, blance_scenario_schedule_out* sched) {
   return entry(ctx, [&](Device&) {
-    const char* name = "blance_plan_scenarios_schedule";
+    const std::string name = "blance_plan_scenarios_schedule";
     if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-    const SchedReq sr = sched_req(name, base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
-    plan_scenarios(ctx, name, base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr);
+    const SchedReq sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
+    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, &sr});
   });
 }
 
@@ -2414,14 +2459,10 @@ extern "C" int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in
     const AuditReq ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
     const bool no_sched = n_move_conc == 0 && !move_conc && !sched;
     SchedReq sr;
-    if (!no_sched) sr = sched_req(name.c_str(), base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
-    if (n > 0 && sc)
-      for (int i = 0; i < n; ++i) {
-        const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
-        check_audit_model(name + ": scenario " + std::to_string(i), &in);
-      }
+    if (!no_sched) sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
+    check_audit_models(name, *base, n, sc, nullptr, 0, opts);
     need_ctx(ctx);
-    plan_scenarios(ctx, name.c_str(), base, n, sc, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, &ar);
+    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, &ar});
   });
 }
 
@@ -2437,37 +2478,14 @@ extern "C" int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan
     AuditReq ar;
     if (audit) ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
     if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": an exposure needs a schedule: n_move_conc must be positive");
-    const SchedReq sr = sched_req(name.c_str(), base, n, sc, out, n_move_conc, move_conc, node_has_mover, sched);
+    const SchedReq sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
     if (!expo) throw_err(BLANCE_ERR_INVALID_ARG, name + ": expo is NULL");
-    if (series_cap < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": series_cap is negative");
-    ExpoReq er;
-    er.series_cap = series_cap;
-    er.out = expo;
-    if (eopts) {
-      if (eopts->flags) throw_err(BLANCE_ERR_INVALID_ARG, name + ": eopts.flags must be 0 (eopts carries a forest only)");
-      check_forest(name, eopts->n_domains, eopts->domain_parent, base->n_node_ids);
-      er.n_domains = eopts->n_domains;
-      er.parent = eopts->domain_parent;
-    }
-    if (audit && n > 0 && sc)
-      for (int i = 0; i < n; ++i) {
-        const blance_plan_in in = scenario_in(*base, sc[i], opts_of(opts, i));
-        check_audit_model(name + ": scenario " + std::to_string(i), &in);
-      }
-    for (long long x = 0; x < (long long)std::max(0, n) * n_move_conc; ++x) {
-      const blance_exposure_out& o = expo[x];
-      er.dom |= o.dom_peak || o.dom_peak_round;
-      er.part_min |= o.part_min_copies != nullptr;
-      er.part_notop |= o.part_no_top != nullptr;
-      er.part_flags |= o.part_flags != nullptr;
-      // a scheduled op emits at most two ancestor chains of AUDIT_DEPTH_MAX + 1 vertices and a partition has at most
-      // 2 x n_slots ops: the static form of blance_moves_exposure's event bound
-      if ((o.dom_peak || o.dom_peak_round) && 2ll * (AUDIT_DEPTH_MAX + 1) * 2 * std::max(0, base->n_slots) * std::max(0, base->n_parts) >= (1ll << 31))
-        throw_err(BLANCE_ERR_UNSUPPORTED, name + ": scenario " + std::to_string(x / n_move_conc) + ", count " + std::to_string(x % n_move_conc) +
-                                              ": dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31");
-    }
+    ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
+    if (audit) check_audit_models(name, *base, n, sc, nullptr, 0, opts);
+    auto pair_name = [&](long long x) { return "scenario " + std::to_string(x / n_move_conc) + ", count " + std::to_string(x % n_move_conc); };
+    expo_flags(name, *base, expo, (long long)std::max(0, n) * n_move_conc, pair_name, er);
     // plan_scenarios checks every scenario before it looks at the context
-    plan_scenarios(ctx, name.c_str(), base, n, sc, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, &er);
+    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, nullptr, &er});
   });
 }
 

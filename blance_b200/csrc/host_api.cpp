@@ -1414,6 +1414,75 @@ ChainSpan name_span(const InternedPlan& ip, const SpanBuffers& b, int count, con
   return r;
 }
 
+// The rule offsets and count a scenario audits with: its own when its options set the hierarchy, else the base's.
+struct AuditRules {
+  const int32_t* off = nullptr;
+  int32_t n = 0;
+};
+
+AuditRules audit_rules(const ScenarioTables& t, const InternedPlan& ip) {
+  if (t.set & BLANCE_OPT_HIERARCHY) return t.has_hier_rules ? AuditRules{t.rule_off.data(), t.n_rules} : AuditRules{};
+  return ip.in.has_hier_rules ? AuditRules{ip.rule_off.data(), ip.in.n_rules} : AuditRules{};
+}
+
+// A blance_scenario_out into ops and load and, when the map is wanted, into map's rows, shape and warnings.
+blance_scenario_out scenario_out(std::vector<int64_t>& ops, std::vector<int64_t>& load, PlanOutBuffers* map) {
+  blance_scenario_out o{};
+  o.node_ops = ops.data();
+  o.state_node_load = load.data();
+  if (map) {
+    o.next_rows = map->next_rows.data();
+    o.next_shape = map->next_shape.data();
+    o.warn = map->warn.data();
+  }
+  return o;
+}
+
+// The schedule, audit and exposure outputs of n_out planned maps at nc counts each: schedules [n_out][nc], with audit
+// audits [n_out] (map x audits with rules(x)), with exposure exposures [n_out][nc].  The exposures' forest is the
+// options' NodeHierarchy, built also without exposure when `eforest_always` (a chain's spans are keyed by it).
+struct AnalysisOutputs {
+  const ScenarioAudit* audit;
+  const bool exposure;
+  const size_t cap;
+  ScheduleBuffers sched;
+  Forest forest, eforest;
+  std::vector<std::unique_ptr<AuditBuffers>> abuf;
+  std::vector<blance_audit_out> aout;
+  std::vector<std::unique_ptr<ExposureBuffers>> ebuf;
+  std::vector<blance_exposure_out> eout;
+  template <class Rules>
+  AnalysisOutputs(const InternedPlan& ip, const PlanNextMapOptions& options, size_t n_out, size_t nc, const ScenarioAudit* a,
+                  const ScenarioExposure* e, bool eforest_always, Rules&& rules)
+      : audit(a), exposure(e != nullptr), cap(e ? size_t(e->SeriesCap) : 0), sched(n_out * nc, size_t(ip.in.n_node_ids)) {
+    if (audit) {
+      build_forest(ip.node_names, options.NodeHierarchy, audit->FailoverSpread, &forest);
+      for (size_t x = 0; x < n_out; ++x) {
+        abuf.push_back(std::make_unique<AuditBuffers>(ip, forest.names.size(), size_t(rules(x).n), audit->FailoverSpread));
+        aout.push_back(abuf.back()->out);
+      }
+    }
+    if (exposure || eforest_always) build_forest(ip.node_names, options.NodeHierarchy, false, &eforest);
+    for (size_t x = 0; exposure && x < n_out * nc; ++x) {
+      ebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), size_t(ip.in.n_parts)));
+      eout.push_back(ebuf.back()->out);
+    }
+  }
+  // Map x's schedules at `counts`, audit (with the rule offsets rule_off) and exposures, into r.
+  void name(const InternedPlan& ip, size_t x, const std::vector<int>& counts, const int32_t* rule_off, ScenarioResult& r) {
+    const size_t nc = counts.size();
+    for (size_t k = 0; k < nc; ++k) r.Schedules.push_back(name_schedule(ip, sched.out[x * nc + k], counts[k]));
+    if (audit) {
+      abuf[x]->out = aout[x];
+      r.Audit = name_audit(ip, forest, rule_off, *abuf[x], audit->FailoverSpread);
+    }
+    for (size_t k = 0; exposure && k < nc; ++k) {
+      ebuf[x * nc + k]->out = eout[x * nc + k];
+      r.Exposures.push_back(name_exposure(*ebuf[x * nc + k], cap, eforest.names, ip.part_names));
+    }
+  }
+};
+
 }  // namespace
 
 std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
@@ -1445,63 +1514,22 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     sc[i] = blance_scenario{tabs[i].removed.data(), tabs[i].added.data(), tabs[i].add_is_nil, tabs[i].has_node_weights,
                             tabs[i].weight.data(), tabs[i].has_weight.data()};
     opts[i] = scenario_opts(tabs[i]);
-    out[i] = blance_scenario_out{};
-    out[i].node_ops = ops[i].data();
-    out[i].state_node_load = load[i].data();
-    if (want[i]) {
-      maps[i] = std::make_unique<PlanOutBuffers>(*ip);
-      out[i].next_rows = maps[i]->next_rows.data();
-      out[i].next_shape = maps[i]->next_shape.data();
-      out[i].warn = maps[i]->warn.data();
-    }
+    if (want[i]) maps[i] = std::make_unique<PlanOutBuffers>(*ip);
+    out[i] = scenario_out(ops[i], load[i], maps[i].get());
   }
   const size_t nc = scheduleConcurrency.size();
-  std::vector<blance_scenario_schedule_out> sched(n * nc);
-  std::vector<int32_t> node_rounds(n * nc * size_t(NU) + 1), node_last(n * nc * size_t(NU) + 1);
-  for (size_t x = 0; x < sched.size(); ++x) {
-    sched[x] = blance_scenario_schedule_out{};
-    sched[x].node_rounds = node_rounds.data() + x * size_t(NU);
-    sched[x].node_last_round = node_last.data() + x * size_t(NU);
-  }
   // the audits: one forest for all scenarios, each scenario's own rules
-  Forest forest;
-  std::vector<std::unique_ptr<AuditBuffers>> abuf;
-  std::vector<blance_audit_out> aout;
-  auto rules_of = [&](size_t i) -> const int32_t* {
-    if (tabs[i].set & BLANCE_OPT_HIERARCHY) return tabs[i].has_hier_rules ? tabs[i].rule_off.data() : nullptr;
-    return ip->in.has_hier_rules ? ip->rule_off.data() : nullptr;
-  };
-  if (audit) {
-    build_forest(ip->node_names, options.NodeHierarchy, audit->FailoverSpread, &forest);
-    for (size_t i = 0; i < n; ++i) {
-      const int32_t R = (tabs[i].set & BLANCE_OPT_HIERARCHY) ? (tabs[i].has_hier_rules ? tabs[i].n_rules : 0)
-                                                             : (ip->in.has_hier_rules ? ip->in.n_rules : 0);
-      abuf.push_back(std::make_unique<AuditBuffers>(*ip, forest.names.size(), size_t(R), audit->FailoverSpread));
-      aout.push_back(abuf.back()->out);
-    }
-  }
-  // the exposures: the options' NodeHierarchy as the forest, one output per (scenario, count)
-  Forest eforest;
-  std::vector<std::unique_ptr<ExposureBuffers>> ebuf;
-  std::vector<blance_exposure_out> eout;
-  const size_t cap = exposure ? size_t(exposure->SeriesCap) : 0;
-  if (exposure) {
-    build_forest(ip->node_names, options.NodeHierarchy, false, &eforest);
-    for (size_t x = 0; x < n * nc; ++x) {
-      ebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), size_t(ip->in.n_parts)));
-      eout.push_back(ebuf.back()->out);
-    }
-  }
+  AnalysisOutputs an(*ip, options, n, nc, audit, exposure, false, [&](size_t i) { return audit_rules(tabs[i], *ip); });
   blance_ctx* ctx = DefaultContext();
   const int st = exposure ? blance_plan_scenarios_exposure(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
-                                                           int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), sched.data(),
-                                                           audit ? &forest.opts : nullptr, audit ? aout.data() : nullptr, &eforest.opts,
-                                                           int32_t(cap), eout.data())
+                                                           int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), an.sched.out.data(),
+                                                           audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr, &an.eforest.opts,
+                                                           int32_t(an.cap), an.eout.data())
                  : audit ? blance_plan_scenarios_audit(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                      int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
-                                                     nc ? sched.data() : nullptr, &forest.opts, aout.data())
+                                                     nc ? an.sched.out.data() : nullptr, &an.forest.opts, an.aout.data())
                  : nc ? blance_plan_scenarios_schedule(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
-                                                     int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), sched.data())
+                                                     int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), an.sched.out.data())
                     : blance_plan_scenarios_ex(ctx, &ip->in, int32_t(n), sc.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                                                out.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_scenarios failed: ") + blance_last_error(ctx));
@@ -1510,18 +1538,7 @@ std::vector<ScenarioResult> PlanNextMapScenarios(const PartitionMap& prevMap, co
     ScenarioResult& r = res[i];
     const int32_t* k = (tabs[i].set & BLANCE_OPT_CONSTRAINTS) ? tabs[i].constraints.data() : ip->state_constraints.data();
     r = scenario_result(*ip, out[i], ops[i], load[i], want[i] ? maps[i].get() : nullptr, k);
-    for (size_t k = 0; k < nc; ++k) {
-      r.Schedules.push_back(name_schedule(*ip, sched[i * nc + k], scheduleConcurrency[k]));
-    }
-    if (audit) {
-      abuf[i]->out = aout[i];
-      r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[i], audit->FailoverSpread);
-    }
-    for (size_t k = 0; exposure && k < nc; ++k) {
-      ExposureBuffers& b = *ebuf[i * nc + k];
-      b.out = eout[i * nc + k];
-      r.Exposures.push_back(name_exposure(b, cap, eforest.names, ip->part_names));
-    }
+    an.name(*ip, i, scheduleConcurrency, audit_rules(tabs[i], *ip).off, r);
   }
   return res;
 }
@@ -1597,15 +1614,8 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     stages[x] = blance_chain_stage{blance_scenario{tb.removed.data(), tb.added.data(), tb.add_is_nil, tb.has_node_weights,
                                                    tb.weight.data(), tb.has_weight.data()},
                                    member[x].data()};
-    out[x] = blance_scenario_out{};
-    out[x].node_ops = ops[x].data();
-    out[x].state_node_load = load[x].data();
-    if (want[x / T]) {
-      maps[x] = std::make_unique<PlanOutBuffers>(*ip);
-      out[x].next_rows = maps[x]->next_rows.data();
-      out[x].next_shape = maps[x]->next_shape.data();
-      out[x].warn = maps[x]->warn.data();
-    }
+    if (want[x / T]) maps[x] = std::make_unique<PlanOutBuffers>(*ip);
+    out[x] = scenario_out(ops[x], load[x], maps[x].get());
   }
   for (size_t i = 0; i < n; ++i) {
     opts[i] = scenario_opts(tabs[i * T]);     // the chain's option groups (its stages differ in node fields only)
@@ -1614,49 +1624,26 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
   }
   // the analyses (blance_plan_chains_exposure): per stage [n][T][nc], the net rebalance and the spans [n][nc]
   const size_t nc = scheduleConcurrency.size(), P = size_t(ip->in.n_parts);
-  ScheduleBuffers sched(n * T * nc, size_t(NU)), net_sched(n * nc, size_t(NU));
-  Forest forest, eforest;
-  std::vector<std::unique_ptr<AuditBuffers>> abuf;
-  std::vector<blance_audit_out> aout;
-  auto rules_of = [&](size_t i) -> const int32_t* {
-    const ScenarioTables& t0 = tabs[i * T];
-    if (t0.set & BLANCE_OPT_HIERARCHY) return t0.has_hier_rules ? t0.rule_off.data() : nullptr;
-    return ip->in.has_hier_rules ? ip->rule_off.data() : nullptr;
-  };
-  if (audit) {
-    build_forest(ip->node_names, options.NodeHierarchy, audit->FailoverSpread, &forest);
-    for (size_t x = 0; x < n * T; ++x) {
-      const ScenarioTables& t0 = tabs[x - x % T];
-      const int32_t R = (t0.set & BLANCE_OPT_HIERARCHY) ? (t0.has_hier_rules ? t0.n_rules : 0) : (ip->in.has_hier_rules ? ip->in.n_rules : 0);
-      abuf.push_back(std::make_unique<AuditBuffers>(*ip, forest.names.size(), size_t(R), audit->FailoverSpread));
-      aout.push_back(abuf.back()->out);
-    }
-  }
-  const size_t cap = exposure ? size_t(exposure->SeriesCap) : 0;
-  std::vector<std::unique_ptr<ExposureBuffers>> ebuf, nebuf;
-  std::vector<blance_exposure_out> eout, neout;
+  // a chain audits with its first stage's rules
+  AnalysisOutputs an(*ip, options, n * T, nc, audit, exposure, nc > 0, [&](size_t x) { return audit_rules(tabs[x - x % T], *ip); });
+  ScheduleBuffers net_sched(n * nc, size_t(NU));
+  std::vector<std::unique_ptr<ExposureBuffers>> nebuf;
+  std::vector<blance_exposure_out> neout;
   std::vector<std::unique_ptr<SpanBuffers>> sbuf;
   std::vector<blance_chain_span_out> sout;
-  if (nc) {
-    build_forest(ip->node_names, options.NodeHierarchy, false, &eforest);
-    for (size_t x = 0; exposure && x < n * T * nc; ++x) {
-      ebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), P));
-      eout.push_back(ebuf.back()->out);
+  for (size_t x = 0; x < n * nc; ++x) {
+    if (exposure) {
+      nebuf.push_back(std::make_unique<ExposureBuffers>(an.cap, an.eforest.names.size(), P));
+      neout.push_back(nebuf.back()->out);
     }
-    for (size_t x = 0; x < n * nc; ++x) {
-      if (exposure) {
-        nebuf.push_back(std::make_unique<ExposureBuffers>(cap, eforest.names.size(), P));
-        neout.push_back(nebuf.back()->out);
-      }
-      sbuf.push_back(std::make_unique<SpanBuffers>(size_t(NU), P, eforest.names.size(), exposure != nullptr));
-      sout.push_back(sbuf.back()->out);
-    }
+    sbuf.push_back(std::make_unique<SpanBuffers>(size_t(NU), P, an.eforest.names.size(), exposure != nullptr));
+    sout.push_back(sbuf.back()->out);
   }
   blance_ctx* ctx = DefaultContext();
   const int st = nc ? blance_plan_chains_exposure(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
                                                   maxConcurrent, int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), net.data(),
-                                                  sched.out.data(), audit ? &forest.opts : nullptr, audit ? aout.data() : nullptr,
-                                                  &eforest.opts, int32_t(cap), exposure ? eout.data() : nullptr, net_sched.out.data(),
+                                                  an.sched.out.data(), audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr,
+                                                  &an.eforest.opts, int32_t(an.cap), exposure ? an.eout.data() : nullptr, net_sched.out.data(),
                                                   exposure ? neout.data() : nullptr, sout.data())
                     : blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
                                          maxConcurrent, out.data(), net.data());
@@ -1668,15 +1655,7 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     for (size_t t = 0; t < T; ++t) {
       const size_t x = i * T + t;
       ScenarioResult r = scenario_result(*ip, out[x], ops[x], load[x], maps[x].get(), k);
-      for (size_t c = 0; c < nc; ++c) r.Schedules.push_back(name_schedule(*ip, sched.out[x * nc + c], scheduleConcurrency[c]));
-      if (audit) {
-        abuf[x]->out = aout[x];
-        r.Audit = name_audit(*ip, forest, rules_of(i), *abuf[x], audit->FailoverSpread);
-      }
-      for (size_t c = 0; exposure && c < nc; ++c) {
-        ebuf[x * nc + c]->out = eout[x * nc + c];
-        r.Exposures.push_back(name_exposure(*ebuf[x * nc + c], cap, eforest.names, ip->part_names));
-      }
+      an.name(*ip, x, scheduleConcurrency, audit_rules(t0, *ip).off, r);
       res[i].Stages.push_back(std::move(r));
     }
     res[i].NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());
@@ -1686,10 +1665,10 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
       res[i].NetSchedules.push_back(name_schedule(*ip, net_sched.out[i * nc + c], scheduleConcurrency[c]));
       if (exposure) {
         nebuf[i * nc + c]->out = neout[i * nc + c];
-        res[i].NetExposures.push_back(name_exposure(*nebuf[i * nc + c], cap, eforest.names, ip->part_names));
+        res[i].NetExposures.push_back(name_exposure(*nebuf[i * nc + c], an.cap, an.eforest.names, ip->part_names));
       }
       sbuf[i * nc + c]->out = sout[i * nc + c];
-      res[i].Span.push_back(name_span(*ip, *sbuf[i * nc + c], scheduleConcurrency[c], eforest.names));
+      res[i].Span.push_back(name_span(*ip, *sbuf[i * nc + c], scheduleConcurrency[c], an.eforest.names));
     }
   }
   return res;
