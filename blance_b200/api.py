@@ -155,9 +155,10 @@ def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None
     keys of PlanNextMapScenarios' scenarios ("nodeWeights", "modelStateConstraints", "stateStickiness",
     "partitionWeights", "nodeHierarchy", "hierarchyRules": missing inherits the options, None means nil), shared by
     its stages.  A stage is a dict with "nodesToRemove" and "nodesToAdd" (required, None = nil), an optional
-    "nodeWeights" and an optional "nodesAll"; without it, the previous stage's members minus its nodesToRemove plus
-    this stage's nodesToAdd (the first stage: the whole universe).  Every chain has the same number of stages.  The
-    caller's maps are NOT mutated.
+    "nodesAll" and the same optional option keys: a stage's own value replaces the chain's for that stage only (the
+    next stage starts from the chain's again).  Without "nodesAll", the previous stage's members minus its
+    nodesToRemove plus this stage's nodesToAdd (the first stage: the whole universe).  Every chain has the same number
+    of stages.  The caller's maps are NOT mutated.
 
     Returns one dict per chain: "stages", one dict per stage with the keys of PlanNextMapScenarios' results (next_map
     and warnings for the chains in wantMaps), and "net": node_ops, ops_total and parts_moved of CalcPartitionMoves
@@ -182,10 +183,8 @@ def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None
             missing = {"nodesToRemove", "nodesToAdd"} - set(st)
             if missing:
                 raise ValueError("chain %d, stage %d lacks %s" % (i, t, ", ".join(sorted(missing))))
-            rm, ad, na = st["nodesToRemove"], st["nodesToAdd"], st.get("nodesAll")
-            nw = st.get("nodeWeights")
-            stages.append((None if rm is None else list(rm), None if ad is None else list(ad), "nodeWeights" in st,
-                           None if nw is None else dict(nw), None if na is None else list(na)))
+            na = st.get("nodesAll")
+            stages.append((_scenario_tuples([st])[0], None if na is None else list(na)))
         cs.append((_scenario_tuples([opts])[0], stages))
     return _host.PlanNextMapChains(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                    {k: tuple(v) for k, v in model.items()}, cs, bool(favorMinNodes),

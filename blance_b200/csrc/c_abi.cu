@@ -492,8 +492,26 @@ static void node_state(DInst& D, const blance_plan_in& in, bool coded, int n_pre
   D.iters_run = 0; D.converged = 0; D.mismatch = 0;
 }
 
-// Host side of a batch: the per-instance descriptors, their offsets into the pooled arrays and the totals.
-static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off, bool coded = false) {
+// The fields of a descriptor that plan options set (blance_scenario_opts): constraints, stickiness, the partition-weight
+// and hierarchy flags, the rule offsets and the mask size.  A chain stage with options of its own (blance_plan_chains_ex)
+// sets them again at its boundary; the mask slice keeps its offset and size.
+static void option_state(DInst& D, const blance_plan_in& in) {
+  D.HW = in.has_hier_rules ? (in.n_hier_bits + 31) / 32 : 0;
+  D.n_rules = in.has_hier_rules ? in.n_rules : 0;
+  D.has_part_weights = in.has_part_weights; D.has_hier_rules = in.has_hier_rules;
+  for (int s = 0; s < in.n_states; ++s) {
+    D.state_constraints[s] = in.state_constraints[s];
+    D.state_stickiness[s] = in.state_stickiness[s];
+    D.state_has_stickiness[s] = in.state_has_stickiness[s];
+    D.rule_off[s] = in.has_hier_rules ? in.rule_off[s] : 0;
+  }
+  D.rule_off[in.n_states] = in.has_hier_rules ? in.rule_off[in.n_states] : 0;
+}
+
+// Host side of a batch: the per-instance descriptors, their offsets into the pooled arrays and the totals.  mask_cap
+// (NULL: none) gives instance i a hierarchy-mask slice of at least mask_cap[i] words, for later stages with more rules.
+static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vector<int>& seg_off, bool coded = false,
+                   const long long* mask_cap = nullptr) {
   pl->n_inst = n;
   pl->h_insts.resize(n);
   pl->raw_rows_off.resize(n + 1);
@@ -506,23 +524,17 @@ static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vecto
     std::memset(&D, 0, sizeof D);
     D.N = in.n_nodes; D.NU = in.n_node_ids; D.S = in.n_states; D.PU = in.n_parts; D.SL = in.n_slots;
     D.SLP = std::max(4, (int)align_up((size_t)in.n_slots, 4));
-    D.HW = in.has_hier_rules ? (in.n_hier_bits + 31) / 32 : 0;
-    D.n_rules = in.has_hier_rules ? in.n_rules : 0;
+    option_state(D, in);
     D.top_state = in.top_state; D.booster = in.booster_kind;
-    D.has_part_weights = in.has_part_weights; D.has_node_weights = in.has_node_weights;
-    D.has_hier_rules = in.has_hier_rules; D.max_iters = in.max_iters; D.engine = in.engine;
+    D.has_node_weights = in.has_node_weights;
+    D.max_iters = in.max_iters; D.engine = in.engine;
     D.debug = getenv("BLANCE_SPEC_STATS") ? 1 : 0;
     for (int s = 0; s < in.n_states; ++s) {
       D.state_priority[s] = in.state_priority[s];
-      D.state_constraints[s] = in.state_constraints[s];
       D.state_slot_off[s] = in.state_slot_off[s];
-      D.state_stickiness[s] = in.state_stickiness[s];
-      D.state_has_stickiness[s] = in.state_has_stickiness[s];
-      D.rule_off[s] = in.has_hier_rules ? in.rule_off[s] : 0;
       if (in.state_constraints[s] > 0) pl->any_state_active[s] = true;
     }
     D.state_slot_off[in.n_states] = in.n_slots;
-    D.rule_off[in.n_states] = in.has_hier_rules ? in.rule_off[in.n_states] : 0;
     // (the instances of a scenario wave share their partition tables: counted once)
     const bool same_parts = i > 0 && in.n_parts == ins[i - 1].n_parts && in.part_in_prev == ins[i - 1].part_in_prev &&
                             in.part_in_assign == ins[i - 1].part_in_assign;
@@ -539,7 +551,7 @@ static void layout(blance_plan* pl, int n, const blance_plan_in* ins, std::vecto
     pl->ST += (long long)D.PU * (D.SLP + 8);
     pl->PT += D.PU; pl->RT += (long long)D.PU * D.SLP; pl->NT += D.N; pl->NUT += D.NU;
     pl->CT += (long long)D.S * D.N; pl->N2T += (long long)(D.NU + 1) * D.N;
-    pl->MT += (long long)D.n_rules * (D.NU + 1) * D.HW;
+    pl->MT += std::max((long long)D.n_rules * (D.NU + 1) * D.HW, mask_cap ? mask_cap[i] : 0ll);
     pl->RRT += (long long)D.PU * D.SL; pl->RST += (long long)D.PU * D.S;
     pl->max_N = std::max(pl->max_N, D.N); pl->max_S = std::max(pl->max_S, D.S); pl->max_NU = std::max(pl->max_NU, D.NU);
   }
@@ -629,12 +641,13 @@ static uint8_t part_flags(const blance_plan_in& in, int p) {
                    (in.part_in_assign[p] ? PF_IN_ASSIGN : 0) | (in.part_has_weight[p] ? PF_HAS_WEIGHT : 0));
 }
 
-static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins, bool coded = false) {
+// Uploads a batch; mask_cap as layout() (the slices beyond an instance's own masks are left unwritten).
+static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins, bool coded = false, const long long* mask_cap = nullptr) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, "batch size must be positive");
   for (int i = 0; i < n; ++i) validate(&ins[i], i);
   PlanPtr pl(new blance_plan());
   std::vector<int> seg_off;
-  layout(pl.get(), n, ins, seg_off, coded);
+  layout(pl.get(), n, ins, seg_off, coded, mask_cap);
   if (pl->PT >= (1LL << 29)) throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one batch");
   plan_slices(pl->arena, pl.get(), n);
   pl->arena.alloc(ctx->stream, "the plan arena");
@@ -646,8 +659,11 @@ static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins, bool co
   const int32_t *h_nw = nullptr, *h_ef = nullptr, *h_er = nullptr;
   const uint8_t *h_csh = nullptr, *h_psh = nullptr, *h_flags = nullptr, *h_rm = nullptr, *h_ad = nullptr, *h_hw = nullptr;
   const uint32_t* h_mask = nullptr;
+  size_t mask_words_up = (size_t)pl->MT;
   std::vector<uint8_t> v_flags, v_rm;
   if (direct(pl.get())) {
+    const DInst& D = pl->h_insts[0];
+    mask_words_up = (size_t)D.n_rules * (D.NU + 1) * D.HW;      // the caller's array; a wider mask_cap slice stays unwritten
     const blance_plan_in& in = ins[0];
     v_flags.resize((size_t)in.n_parts + 1);
     for (int p = 0; p < in.n_parts; ++p) v_flags[(size_t)p] = part_flags(in, p);
@@ -720,7 +736,7 @@ static PlanPtr upload(blance_ctx* ctx, int n, const blance_plan_in* ins, bool co
   h2d(P.node_removed, h_rm, (size_t)pl->NUT); h2d(P.node_added, h_ad, (size_t)pl->NUT);
   h2d(P.node_weight, h_nw, sizeof(int32_t) * (size_t)pl->NT); h2d(P.node_has_weight, h_hw, (size_t)pl->NT);
   h2d(P.extra_first, h_ef, sizeof(int32_t) * (size_t)pl->NT); h2d(P.extra_rest, h_er, sizeof(int32_t) * (size_t)pl->NT);
-  h2d(P.ie_mask, h_mask, sizeof(uint32_t) * (size_t)pl->MT);
+  h2d(P.ie_mask, h_mask, sizeof(uint32_t) * mask_words_up);
   h2d(P.insts, pl->h_insts.data(), sizeof(DInst) * (size_t)n);
   h2d(pl->d_raw_rows_off, pl->raw_rows_off.data(), sizeof(long long) * (size_t)(n + 1));
   h2d(pl->d_raw_shape_off, pl->raw_shape_off.data(), sizeof(long long) * (size_t)(n + 1));
@@ -1060,7 +1076,11 @@ static blance_plan_in scenario_in(const blance_plan_in& base, const blance_scena
   return in;
 }
 
-static const blance_scenario_opts* opts_of(const blance_scenario_opts* opts, int i) { return opts ? &opts[i] : nullptr; }
+// The options of item i at stage t (NULL opts: none).  per_stage = T: opts is [n][T], one per chain stage
+// (blance_plan_chains_ex); per_stage = 0: opts is [n], one per scenario or chain for all its stages.
+static const blance_scenario_opts* opts_at(const blance_scenario_opts* opts, int per_stage, int i, int t) {
+  return opts ? &opts[per_stage ? (size_t)i * per_stage + t : (size_t)i] : nullptr;
+}
 
 static int n_overrides(const blance_scenario_opts* o) {
   return o && (o->set & BLANCE_OPT_PART_WEIGHTS) ? o->n_weight_overrides : 0;
@@ -1171,7 +1191,7 @@ static const int kWaveMax = 65535;
 
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit), at most kWaveMax.  Scenarios
 // differ only in their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and
-// override list of any.
+// override list of any (of any stage of a chain: its mask slice and weight changes at the stage that needs the most).
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
                      int max_concurrent, const SchedReq* sr, size_t extra_bytes, size_t* per_scenario) {
   blance_plan probe;
@@ -1681,8 +1701,10 @@ static void expo_unpack(const ExpoResult& r, long long i, int R, const unsigned 
 // The chains requested with blance_plan_chains: T stages per chain, stages [n][T], net [n] or NULL; with
 // blance_plan_chains_exposure the net rebalance's schedules and exposures [n][nc] and the spans [n][nc], each or NULL,
 // and which span arrays any span asks for (span_parts: the per-partition exposure arrays, span_dom: the per-vertex).
+// stage_opts: the request's opts are [n][T], one per stage (blance_plan_chains_ex), else [n].
 struct ChainReq {
   int T = 1;
+  bool stage_opts = false;
   const blance_chain_stage* stages = nullptr;
   blance_chain_out* net = nullptr;
   blance_scenario_schedule_out* net_sched = nullptr;
@@ -1725,12 +1747,17 @@ static const blance_scenario& nodes_of(const WaveReq& q, int i, int t) {
   return q.cr ? q.cr->stages[(size_t)i * q.cr->T + t].nodes : q.sc[i];
 }
 
+// The plan options of scenario (or chain) i at stage t.
+static const blance_scenario_opts* opts_of(const WaveReq& q, int i, int t) {
+  return opts_at(q.opts, q.cr && q.cr->stage_opts ? q.cr->T : 0, i, t);
+}
+
 // The substituted instance of scenario / chain i at stage t.  A chain stage's node_removed is written in the device
 // code into `code` (NR_OUTSIDE for the ids below n_nodes that its node_in_all leaves out), and from stage 2 on the
 // non-model counts of iteration 1 are those of the later iterations: the assigned partitions' prevMap entries are
-// the previous stage's next rows, which hold model states only.
+// the previous stage's next rows, which hold model states only (with a stage's own weight options, its extra_tot_rest).
 static blance_plan_in stage_in(const WaveReq& q, int i, int t, std::vector<uint8_t>& code) {
-  blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q.opts, i));
+  blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q, i, t));
   if (!q.cr) return in;
   const blance_chain_stage& st = q.cr->stages[(size_t)i * q.cr->T + t];
   code.assign((size_t)std::max(1, in.n_node_ids), 0);
@@ -1739,6 +1766,40 @@ static blance_plan_in stage_in(const WaveReq& q, int i, int t, std::vector<uint8
   in.node_removed = code.data();
   if (t > 0) in.extra_tot_first = in.extra_tot_rest;
   return in;
+}
+
+// A partition-weight change (k_scenario_weights): the partition, its new weight and presence.
+struct WeightSet { int32_t part, weight, has; };
+
+// The weight changes that item i's partition weights go through before stage t, appended to d.  Stage 0: its overrides
+// over the base's, as given.  Stage t > 0: the difference from stage t-1's weights to stage t's, each the base's with
+// that stage's own overrides applied - an index stage t-1 overrode and stage t leaves alone returns to the base's
+// weight and presence - in ascending partition order, without the entries that do not change.  Scenarios and chains
+// whose options hold for every stage change nothing after stage 0.
+static void weight_delta(const WaveReq& q, int i, int t, std::vector<WeightSet>& d) {
+  const blance_scenario_opts* b = opts_of(q, i, t);
+  if (t == 0) {
+    for (int k = 0; k < n_overrides(b); ++k) d.push_back(WeightSet{b->ow_part[k], b->ow_weight[k], b->ow_has[k]});
+    return;
+  }
+  const blance_scenario_opts* a = opts_of(q, i, t - 1);
+  if (a == b || (n_overrides(a) == 0 && n_overrides(b) == 0)) return;
+  auto sorted = [](const blance_scenario_opts* o) {
+    std::vector<WeightSet> v;
+    for (int k = 0; k < n_overrides(o); ++k) v.push_back(WeightSet{o->ow_part[k], o->ow_weight[k], o->ow_has[k]});
+    std::sort(v.begin(), v.end(), [](const WeightSet& x, const WeightSet& y) { return x.part < y.part; });
+    return v;
+  };
+  const std::vector<WeightSet> va = sorted(a), vb = sorted(b);
+  const blance_plan_in& base = *q.base;
+  auto at_base = [&](int32_t p) { return WeightSet{p, base.part_weight[p], base.part_has_weight[p] ? 1 : 0}; };
+  size_t x = 0, y = 0;
+  while (x < va.size() || y < vb.size()) {
+    const int32_t p = y == vb.size() || (x < va.size() && va[x].part < vb[y].part) ? va[x].part : vb[y].part;
+    const WeightSet was = x < va.size() && va[x].part == p ? va[x++] : at_base(p);
+    const WeightSet now = y < vb.size() && vb[y].part == p ? vb[y++] : at_base(p);
+    if (was.weight != now.weight || was.has != now.has) d.push_back(now);
+  }
 }
 
 // Uploads the node tables (node flags, weights, non-model counts, hierarchy masks) of the wave's instances `ins`
@@ -1770,7 +1831,8 @@ struct Sweep {
   const std::vector<int>& idx;
   const int T, nc, MO;                 // stages per item, counts per schedule, ops per partition
   const long long V, stride;           // exposure vertices, int64 words of one summary
-  int max_rules = 0, W = 0;
+  int max_rules = 0, W = 0;            // max_rules: over every stage of every item
+  std::vector<long long> mask_cap;     // per item of idx: the mask words of its stage with the largest hierarchy masks
   int n_prev_later = 0;                // len(prevMap) from stage 2 on: the base's prevMap plus every assigned partition
   bool audit_flags = false;            // any caller wants the per-partition flags
   PlanPtr pb;
@@ -1801,7 +1863,7 @@ struct Wave {
   std::vector<blance_plan_in> ins;
   std::vector<std::vector<uint8_t>> code;
   std::vector<int> seg_off;
-  std::vector<int32_t> ow;             // the weight overrides: index[k] | weight[k] | presence[k]
+  std::vector<int32_t> ow;             // the stage's weight changes: index[k] | weight[k] | presence[k]
   Arena arena;
   long long* d_sum = nullptr;
   WSched sched{};
@@ -1888,9 +1950,25 @@ static void analysis_slices(const Sweep& s, Arena& a, AnalysisBufs& b, WSched& s
   if (s.q.cr && s.q.cr->span) span_slices(a, b.span, *s.q.cr, nw, s.nc, base.n_parts, base.n_node_ids, s.V);
 }
 
+// The partition-weight changes of wave w's members before stage t (weight_delta) into w.ow, as wave-global partition
+// indices over the members' replicated slices (lone: over the base upload).
+static void wave_weights(const Sweep& s, Wave& w, int t) {
+  std::vector<WeightSet> d;
+  std::vector<long long> off;          // the wave-global index of each change's member's first partition
+  for (int j = 0; j < w.nw; ++j) {
+    weight_delta(s.q, s.idx[(size_t)(w.w0 + j)], t, d);
+    off.resize(d.size(), w.pl->h_insts[(size_t)j].part_off);
+  }
+  w.ow.clear();
+  for (size_t k = 0; k < d.size(); ++k) w.ow.push_back((int32_t)(off[k] + d[k].part));
+  for (const WeightSet& x : d) w.ow.push_back(x.weight);
+  for (const WeightSet& x : d) w.ow.push_back(x.has);
+}
+
 // Lays out wave w at its first stage and allocates it in one arena, so that a plan is never lost for want of its
-// summaries or analyses: the plan (lone: the base upload), summaries, schedule state, weight overrides and analyses.
-// Returns false when the wave is to be halved: 2^29 or more partitions, or the free memory moved under an automatic size.
+// summaries or analyses: the plan (lone: the base upload), summaries, schedule state, weight changes (room for the
+// stage that changes the most) and analyses.  Returns false when the wave is to be halved: 2^29 or more partitions,
+// or the free memory moved under an automatic size.
 static bool wave_alloc(const Sweep& s, Wave& w) {
   const WaveReq& q = s.q;
   const int nw = w.nw, PU = q.base->n_parts;
@@ -1898,23 +1976,20 @@ static bool wave_alloc(const Sweep& s, Wave& w) {
   // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
   w.lone = s.idx.size() == 1;
   blance_plan* pl = w.pl = w.lone ? s.pb.get() : &w.plan;
-  if (!w.lone) layout(pl, nw, w.ins.data(), w.seg_off, q.cr != nullptr);
+  if (!w.lone) layout(pl, nw, w.ins.data(), w.seg_off, q.cr != nullptr, s.mask_cap.data() + w.w0);
   if (!w.lone && pl->PT >= (1LL << 29)) {
     if (nw > 1) return false;
     throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
   }
-  // the wave's partition-weight overrides over its replicated slices (lone: over the base upload), as wave-global
-  // partition indices
-  for (int pass = 0; pass < 3; ++pass)
-    for (int j = 0; j < nw; ++j) {
-      const blance_scenario_opts* o = opts_of(q.opts, s.idx[(size_t)(w.w0 + j)]);
-      for (int k = 0; k < n_overrides(o); ++k)
-        w.ow.push_back(pass == 0 ? (int32_t)(pl->h_insts[(size_t)j].part_off + o->ow_part[k]) : pass == 1 ? o->ow_weight[k] : (int32_t)o->ow_has[k]);
-    }
+  size_t ow_cap = 0;
+  for (int t = s.T - 1; t >= 0; --t) {   // ends with stage 0's changes in w.ow
+    wave_weights(s, w, t);
+    ow_cap = std::max(ow_cap, w.ow.size());
+  }
   if (!w.lone) plan_slices(w.arena, pl, nw);
   w.arena.add(w.d_sum, (size_t)(s.stride * nw));
   if (q.sr) sched_slices(w.arena, nw, s.nc, PU, q.base->n_node_ids, s.MO, (long long)PU * s.MO, w.sched, w.wtmp, w.wtmp_bytes, s.ctx->stream);
-  if (!w.ow.empty()) w.arena.add(w.d_ow, w.ow.size());
+  if (ow_cap) w.arena.add(w.d_ow, ow_cap);
   analysis_slices(s, w.arena, w.an, w.sched, nw, pl);
   try {
     w.arena.alloc(s.ctx->stream, "a scenario wave");
@@ -1960,22 +2035,34 @@ static void wave_upload(const Sweep& s, Wave& w) {
 
 // The stage boundary before stage t: what the convergence loop left in the working state is the next stage's input -
 // the assigned partitions' prev and cur rows are their next rows, committed by k_commit (or equal to them when the
-// stage converged) with their flags - then the next stage's node tables and a fresh loop state.
+// stage converged) with their flags - then the next stage's options, node tables and a fresh loop state, and the
+// partition-weight changes from the previous stage's weights to this stage's (none when the options hold for every
+// stage: nothing is launched then).
 static void stage_boundary(const Sweep& s, Wave& w, int t) {
   cudaStream_t st = s.ctx->stream;
   blance_plan* pl = w.pl;
+  DPool& P = pl->pool;
   if (pl->PT > 0) {
-    CUDA(cudaMemcpyAsync(pl->rows_init, pl->pool.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-    CUDA(cudaMemcpyAsync(pl->prev_rows_init, pl->pool.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
-    CUDA(cudaMemcpyAsync(pl->pmeta_init, pl->pool.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-    CUDA(cudaMemcpyAsync(pl->prev_meta_init, pl->pool.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
-    CUDA(cudaMemcpyAsync(pl->pflags_init, pl->pool.pflags, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->rows_init, P.rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_rows_init, P.prev_rows, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->pmeta_init, P.pmeta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->prev_meta_init, P.prev_meta, sizeof(uint32_t) * (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+    CUDA(cudaMemcpyAsync(pl->pflags_init, P.pflags, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
   }
+  std::fill(pl->any_state_active, pl->any_state_active + BL_S_MAX, false);
   for (int j = 0; j < w.nw; ++j) {
-    w.ins[(size_t)j] = stage_in(s.q, s.idx[(size_t)(w.w0 + j)], t, w.code[(size_t)j]);
-    node_state(pl->h_insts[(size_t)j], w.ins[(size_t)j], s.q.cr != nullptr, s.n_prev_later);
+    const blance_plan_in& in = w.ins[(size_t)j] = stage_in(s.q, s.idx[(size_t)(w.w0 + j)], t, w.code[(size_t)j]);
+    option_state(pl->h_insts[(size_t)j], in);
+    node_state(pl->h_insts[(size_t)j], in, s.q.cr != nullptr, s.n_prev_later);
+    for (int k = 0; k < in.n_states; ++k) pl->any_state_active[k] |= in.state_constraints[k] > 0;
   }
   upload_nodes(s.ctx, pl, w.ins, s.q.cr != nullptr);
+  wave_weights(s, w, t);
+  if (!w.ow.empty()) {                 // after the copy into pflags_init above, which carries the previous stage's presence
+    const int k = (int)(w.ow.size() / 3);
+    CUDA(cudaMemcpyAsync(w.d_ow, w.ow.data(), sizeof(int32_t) * w.ow.size(), cudaMemcpyHostToDevice, st));
+    launch(s.ctx, k_scenario_weights, grid_for(s.ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, w.d_ow, k);
+  }
 }
 
 // Summaries (node_ops | state_node_load | 3 scalars per member, s.stride int64 words) of wave w's plans from the beg
@@ -2192,13 +2279,23 @@ static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, co
   const int n_dev = (int)idx.size();
   std::vector<uint8_t> code0;
   const blance_plan_in in0 = stage_in(q, idx[0], 0, code0);
+  // a member is priced and laid out by the largest of its stages: hierarchy masks, rules and weight changes
   long long max_mask = 0;
   int max_ow = 0;
-  for (int i : idx) {
-    const blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, 0), opts_of(q.opts, i));
-    max_mask = std::max(max_mask, mask_words(in));
-    max_ow = std::max(max_ow, n_overrides(opts_of(q.opts, i)));
-    s.max_rules = std::max(s.max_rules, in.has_hier_rules ? in.n_rules : 0);
+  s.mask_cap.assign(idx.size(), 0);
+  std::vector<WeightSet> delta;
+  for (size_t x = 0; x < idx.size(); ++x) {
+    const int i = idx[x];
+    for (int t = 0; t < s.T; ++t) {
+      if (t > 0 && !(q.cr && q.cr->stage_opts)) break;    // the same options at every stage
+      const blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q, i, t));
+      s.mask_cap[x] = std::max(s.mask_cap[x], mask_words(in));
+      s.max_rules = std::max(s.max_rules, in.has_hier_rules ? in.n_rules : 0);
+      delta.clear();
+      weight_delta(q, i, t, delta);
+      max_ow = std::max(max_ow, (int)delta.size());
+    }
+    max_mask = std::max(max_mask, s.mask_cap[x]);
     for (int t = 0; q.ar && t < s.T; ++t) s.audit_flags |= q.ar->out[(size_t)i * s.T + t].part_flags != nullptr;
   }
   {
@@ -2209,7 +2306,7 @@ static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, co
     }
   }
   // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
-  s.pb = upload(ctx, 1, &in0, q.cr != nullptr);
+  s.pb = upload(ctx, 1, &in0, q.cr != nullptr, n_dev == 1 ? s.mask_cap.data() : nullptr);   // lone: the wave's own plan
   Arena one;                           // one member's analysis buffers, priced into the wave
   AnalysisBufs one_bufs;
   WSched one_sched{};
@@ -2277,15 +2374,16 @@ static void plan_scenarios(blance_ctx* ctx, const std::string& name, int32_t n, 
   long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
   for (int i = 0; i < n; ++i) {
     std::string why;
-    const int st = check_scenario(*q.base, q.sc[i], opts_of(q.opts, i), base_sum, why);
+    const int st = check_scenario(*q.base, q.sc[i], opts_of(q, i, 0), base_sum, why);
     if (st != BLANCE_OK) throw_err(st, name + ": scenario " + std::to_string(i) + ": " + why);
   }
   plan_wave(ctx, n, q);
 }
 
-// The checks of the chains of stages over one base that blance_plan_chains and blance_plan_chains_exposure plan.
+// The checks of the chains of stages over one base that blance_plan_chains, blance_plan_chains_exposure and
+// blance_plan_chains_ex plan; opts as opts_at() with per_stage (0, or n_stages for options per stage).
 static void check_chains(const std::string& name, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
-                         const blance_scenario_opts* opts, blance_scenario_out* out) {
+                         const blance_scenario_opts* opts, int per_stage, blance_scenario_out* out) {
   if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
   if (n_stages < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_stages must be positive");
   if (!base || !stages || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
@@ -2297,7 +2395,7 @@ static void check_chains(const std::string& name, const blance_plan_in* base, in
     for (int t = 0; t < n_stages; ++t) {
       const blance_chain_stage& cs = stages[(size_t)i * n_stages + t];
       std::string why;
-      int st = check_scenario(*base, cs.nodes, opts_of(opts, i), base_sum, why);
+      int st = check_scenario(*base, cs.nodes, opts_at(opts, per_stage, i, t), base_sum, why);
       if (st == BLANCE_OK && base->n_nodes > 0 && !cs.node_in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
       for (int q = 0; st == BLANCE_OK && q < base->n_nodes; ++q)
         if (cs.node_in_all[q] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
@@ -2325,14 +2423,16 @@ static SchedReq sched_req(const std::string& name, const blance_plan_in* base, l
   return sr;
 }
 
-// check_audit_model over the first stages of the n scenarios sc, or of the n chains `stages` (none while NULL).
+// check_audit_model over the first stages of the n scenarios sc, or of the n chains `stages` (none while NULL); with
+// per_stage (opts [n][T], as opts_at) over every stage of every chain, naming "chain i, stage t".
 static void check_audit_models(const std::string& name, const blance_plan_in& base, int32_t n, const blance_scenario* sc,
-                               const blance_chain_stage* stages, int32_t T, const blance_scenario_opts* opts) {
+                               const blance_chain_stage* stages, int32_t T, const blance_scenario_opts* opts, int per_stage = 0) {
   if (stages ? T < 1 : !sc) return;
-  for (int i = 0; i < n; ++i) {
-    const blance_plan_in in = scenario_in(base, stages ? stages[(size_t)i * T].nodes : sc[i], opts_of(opts, i));
-    check_audit_model(name + (stages ? ": chain " : ": scenario ") + std::to_string(i), &in);
-  }
+  for (int i = 0; i < n; ++i)
+    for (int t = 0; t < (per_stage ? T : 1); ++t) {
+      const blance_plan_in in = scenario_in(base, stages ? stages[(size_t)i * T + t].nodes : sc[i], opts_at(opts, per_stage, i, t));
+      check_audit_model(name + (stages ? ": chain " : ": scenario ") + std::to_string(i) + (per_stage ? ", stage " + std::to_string(t) : ""), &in);
+    }
 }
 
 // A scheduled op emits at most two ancestor chains of AUDIT_DEPTH_MAX + 1 vertices and a partition has at most
@@ -2370,11 +2470,60 @@ extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, i
                                   const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
                                   int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
   return entry(ctx, [&](Device&) {
-    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, out);
+    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, 0, out);
     ChainReq cr;
     cr.T = n_stages; cr.stages = stages; cr.net = net;
     plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, nullptr, nullptr, &cr});
   });
+}
+
+// blance_plan_chains_exposure (opts [n]) and blance_plan_chains_ex (stage_opts: opts [n][n_stages], and the schedule
+// may be left out: n_move_conc 0 with move_conc and sched NULL plans and audits without one).
+static void plan_chains_analysed(blance_ctx* ctx, const std::string& name, bool stage_opts, const blance_plan_in* base, int32_t n,
+                                 int32_t n_stages, const blance_chain_stage* stages, const blance_scenario_opts* opts,
+                                 int32_t favor_min_nodes, int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
+                                 const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
+                                 blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
+                                 const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
+                                 blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span) {
+  if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
+  const int T = n_stages, nc = n_move_conc, per_stage = stage_opts ? T : 0;
+  if ((net_sched || net_expo) && !net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_sched and net_expo need net");
+  AuditReq ar;
+  if (audit) {
+    ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
+    check_audit_models(name, *base, n, nullptr, stages, T, opts, per_stage);
+  }
+  const bool no_sched = stage_opts && n_move_conc == 0 && !move_conc && !sched;
+  if (no_sched && (expo || net_sched || net_expo || span))
+    throw_err(BLANCE_ERR_INVALID_ARG, name + ": expo, net_sched, net_expo and span need a schedule");
+  SchedReq sr;
+  if (!no_sched) {
+    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive");
+    sr = sched_req(name, base, (long long)std::max(0, n) * std::max(0, T) * nc, n_move_conc, move_conc, node_has_mover, sched);
+  }
+  ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
+  ChainReq cr;
+  cr.T = T; cr.stage_opts = stage_opts; cr.stages = stages; cr.net = net; cr.net_sched = net_sched; cr.net_expo = net_expo; cr.span = span;
+  for (long long x = 0; span && x < (long long)std::max(0, n) * nc; ++x) {
+    const blance_chain_span_out& s = span[x];
+    cr.span_parts |= s.part_min_copies || s.part_no_top || s.part_flags;
+    cr.span_dom |= s.dom_peak || s.dom_peak_stage || s.dom_peak_round;
+  }
+  if (!expo && (net_expo || cr.span_parts || cr.span_dom))
+    throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_expo and the span's exposure arrays need expo");
+  auto stage_name = [&](long long x) {
+    return "chain " + std::to_string(x / ((long long)T * nc)) + ", stage " + std::to_string(x / nc % T) + ", count " + std::to_string(x % nc);
+  };
+  auto pair_name = [&](long long x) { return "chain " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
+  expo_flags(name, *base, expo, (long long)std::max(0, n) * std::max(0, T) * nc, stage_name, er);
+  expo_flags(name, *base, net_expo, (long long)std::max(0, n) * nc, pair_name, er);
+  if (cr.span_dom) check_event_bound(name, "span", *base);
+  er.dom |= cr.span_dom;
+  er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
+  check_chains(name, base, n, n_stages, stages, opts, per_stage, out);
+  plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, audit ? &ar : nullptr, &cr,
+                            expo ? &er : nullptr});
 }
 
 extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
@@ -2386,38 +2535,23 @@ extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in
                                            blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo,
                                            blance_chain_span_out* span) {
   return entry(ctx, [&](Device&) {
-    const std::string name = "blance_plan_chains_exposure";
-    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
-    const int T = n_stages, nc = n_move_conc;
-    if ((net_sched || net_expo) && !net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_sched and net_expo need net");
-    AuditReq ar;
-    if (audit) {
-      ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
-      check_audit_models(name, *base, n, nullptr, stages, T, opts);
-    }
-    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive");
-    const SchedReq sr = sched_req(name, base, (long long)std::max(0, n) * std::max(0, T) * nc, n_move_conc, move_conc, node_has_mover, sched);
-    ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
-    ChainReq cr;
-    cr.T = T; cr.stages = stages; cr.net = net; cr.net_sched = net_sched; cr.net_expo = net_expo; cr.span = span;
-    for (long long x = 0; span && x < (long long)std::max(0, n) * nc; ++x) {
-      const blance_chain_span_out& s = span[x];
-      cr.span_parts |= s.part_min_copies || s.part_no_top || s.part_flags;
-      cr.span_dom |= s.dom_peak || s.dom_peak_stage || s.dom_peak_round;
-    }
-    if (!expo && (net_expo || cr.span_parts || cr.span_dom))
-      throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_expo and the span's exposure arrays need expo");
-    auto stage_name = [&](long long x) {
-      return "chain " + std::to_string(x / ((long long)T * nc)) + ", stage " + std::to_string(x / nc % T) + ", count " + std::to_string(x % nc);
-    };
-    auto pair_name = [&](long long x) { return "chain " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
-    expo_flags(name, *base, expo, (long long)std::max(0, n) * std::max(0, T) * nc, stage_name, er);
-    expo_flags(name, *base, net_expo, (long long)std::max(0, n) * nc, pair_name, er);
-    if (cr.span_dom) check_event_bound(name, "span", *base);
-    er.dom |= cr.span_dom;
-    er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
-    check_chains(name, base, n, n_stages, stages, opts, out);
-    plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, &cr, expo ? &er : nullptr});
+    plan_chains_analysed(ctx, "blance_plan_chains_exposure", false, base, n, n_stages, stages, opts, favor_min_nodes, max_concurrent,
+                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
+                         net_expo, span);
+  });
+}
+
+extern "C" int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                     const blance_chain_stage* stages, const blance_scenario_opts* stage_opts, int32_t favor_min_nodes,
+                                     int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
+                                     const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
+                                     blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
+                                     const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
+                                     blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span) {
+  return entry(ctx, [&](Device&) {
+    plan_chains_analysed(ctx, "blance_plan_chains_ex", true, base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent,
+                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
+                         net_expo, span);
   });
 }
 

@@ -1558,8 +1558,9 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     if (chains[i].Stages.size() != T)
       invalid("PlanNextMapChains: chain " + std::to_string(i) + " has " + std::to_string(chains[i].Stages.size()) +
               " stages, chain 0 has " + std::to_string(T) + " (chains of different lengths go in separate calls)");
-  // every stage as a scenario: its node sets and weights, the chain's option fields
+  // every stage as a scenario: its node sets and weights, the chain's option fields and the stage's own
   std::vector<Scenario> flat(n * T);
+  bool stage_opts = false;             // some stage sets an option of its own: blance_plan_chains_ex
   for (size_t i = 0; i < n; ++i)
     for (size_t t = 0; t < T; ++t) {
       const ChainStage& cs = chains[i].Stages[t];
@@ -1568,6 +1569,12 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
       sc.NodesToRemove = cs.NodesToRemove;
       sc.NodesToAdd = cs.NodesToAdd;
       if (cs.NodeWeights) sc.NodeWeights = cs.NodeWeights;
+      if (cs.ModelStateConstraints) sc.ModelStateConstraints = cs.ModelStateConstraints;
+      if (cs.StateStickiness) sc.StateStickiness = cs.StateStickiness;
+      if (cs.PartitionWeights) sc.PartitionWeights = cs.PartitionWeights;
+      if (cs.NodeHierarchy) sc.NodeHierarchy = cs.NodeHierarchy;
+      if (cs.HierarchyRules) sc.HierarchyRules = cs.HierarchyRules;
+      stage_opts |= cs.ModelStateConstraints || cs.StateStickiness || cs.PartitionWeights || cs.NodeHierarchy || cs.HierarchyRules;
     }
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, flat);
   const int32_t N = ip->in.n_nodes, NU = ip->in.n_node_ids, S = ip->in.n_states;
@@ -1603,7 +1610,7 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     want[size_t(i)] = true;
   }
   std::vector<blance_chain_stage> stages(n * T);
-  std::vector<blance_scenario_opts> opts(n);
+  std::vector<blance_scenario_opts> opts(stage_opts ? n * T : n);
   std::vector<blance_scenario_out> out(n * T);
   std::vector<blance_chain_out> net(n);
   std::vector<std::vector<int64_t>> ops(n * T, std::vector<int64_t>(size_t(NU) * 4 + 1)),
@@ -1617,15 +1624,16 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     if (want[x / T]) maps[x] = std::make_unique<PlanOutBuffers>(*ip);
     out[x] = scenario_out(ops[x], load[x], maps[x].get());
   }
+  // each stage's option groups, or the chain's when no stage sets its own (its stages then differ in node fields only)
+  for (size_t x = 0; x < opts.size(); ++x) opts[x] = scenario_opts(tabs[stage_opts ? x : x * T]);
   for (size_t i = 0; i < n; ++i) {
-    opts[i] = scenario_opts(tabs[i * T]);     // the chain's option groups (its stages differ in node fields only)
     net[i] = blance_chain_out{};
     net[i].node_ops = net_ops[i].data();
   }
   // the analyses (blance_plan_chains_exposure): per stage [n][T][nc], the net rebalance and the spans [n][nc]
   const size_t nc = scheduleConcurrency.size(), P = size_t(ip->in.n_parts);
-  // a chain audits with its first stage's rules
-  AnalysisOutputs an(*ip, options, n * T, nc, audit, exposure, nc > 0, [&](size_t x) { return audit_rules(tabs[x - x % T], *ip); });
+  // every stage audits with its own rules
+  AnalysisOutputs an(*ip, options, n * T, nc, audit, exposure, nc > 0, [&](size_t x) { return audit_rules(tabs[x], *ip); });
   ScheduleBuffers net_sched(n * nc, size_t(NU));
   std::vector<std::unique_ptr<ExposureBuffers>> nebuf;
   std::vector<blance_exposure_out> neout;
@@ -1640,7 +1648,14 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     sout.push_back(sbuf.back()->out);
   }
   blance_ctx* ctx = DefaultContext();
-  const int st = nc ? blance_plan_chains_exposure(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+  const int st = stage_opts
+                     ? blance_plan_chains_ex(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+                                             maxConcurrent, int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
+                                             net.data(), nc ? an.sched.out.data() : nullptr, audit ? &an.forest.opts : nullptr,
+                                             audit ? an.aout.data() : nullptr, &an.eforest.opts, int32_t(an.cap),
+                                             exposure ? an.eout.data() : nullptr, nc ? net_sched.out.data() : nullptr,
+                                             exposure ? neout.data() : nullptr, nc ? sout.data() : nullptr)
+                 : nc ? blance_plan_chains_exposure(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
                                                   maxConcurrent, int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), net.data(),
                                                   an.sched.out.data(), audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr,
                                                   &an.eforest.opts, int32_t(an.cap), exposure ? an.eout.data() : nullptr, net_sched.out.data(),
@@ -1650,12 +1665,11 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_chains failed: ") + blance_last_error(ctx));
   std::vector<ChainResult> res(n);
   for (size_t i = 0; i < n; ++i) {
-    const ScenarioTables& t0 = tabs[i * T];
-    const int32_t* k = (t0.set & BLANCE_OPT_CONSTRAINTS) ? t0.constraints.data() : ip->state_constraints.data();
     for (size_t t = 0; t < T; ++t) {
       const size_t x = i * T + t;
+      const int32_t* k = (tabs[x].set & BLANCE_OPT_CONSTRAINTS) ? tabs[x].constraints.data() : ip->state_constraints.data();
       ScenarioResult r = scenario_result(*ip, out[x], ops[x], load[x], maps[x].get(), k);
-      an.name(*ip, x, scheduleConcurrency, audit_rules(t0, *ip).off, r);
+      an.name(*ip, x, scheduleConcurrency, audit_rules(tabs[x], *ip).off, r);
       res[i].Stages.push_back(std::move(r));
     }
     res[i].NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());

@@ -211,11 +211,19 @@ struct ChainStage {
   // nullopt: the previous stage's members minus its NodesToRemove, plus this stage's NodesToAdd that are in the
   // universe; the first stage's default is the whole universe.
   OptStrs NodesAll;
+  // This stage's plan options (blance_plan_chains_ex), each with the meaning it has in Scenario.  Outer nullopt: the
+  // chain's value (Chain::Options, and where that is unset the options').  A stage's options do not carry over to the
+  // next stage: each stage starts from the chain's.
+  ScenarioOpt<std::unordered_map<std::string, int>> ModelStateConstraints;
+  ScenarioOpt<std::unordered_map<std::string, int>> StateStickiness;
+  ScenarioOpt<std::unordered_map<std::string, int>> PartitionWeights;
+  ScenarioOpt<std::unordered_map<std::string, std::string>> NodeHierarchy;
+  ScenarioOpt<::blance::HierarchyRules> HierarchyRules;
 };
 
 struct Chain {
   // The plan options of every stage of the chain: the option fields of a Scenario (ModelStateConstraints,
-  // StateStickiness, PartitionWeights, NodeHierarchy, HierarchyRules, and NodeWeights unless a stage sets its own).
+  // StateStickiness, PartitionWeights, NodeHierarchy, HierarchyRules, and NodeWeights), unless a stage sets its own.
   // Its NodesToRemove / NodesToAdd are not read.
   Scenario Options;
   std::vector<ChainStage> Stages;
@@ -251,7 +259,8 @@ struct ChainResult {
 };
 
 // Chain i is the Go loop of include/blance_b200.h over its stages: stage t is PlanNextMapEx(prev, assign, nodesAll_t,
-// NodesToRemove_t, NodesToAdd_t, model, options with chain i's option fields and stage t's NodeWeights), then prev =
+// NodesToRemove_t, NodesToAdd_t, model, options with chain i's option fields, those stage t sets of its own and stage t's
+// NodeWeights), then prev =
 // prev with every entry of next replaced and assign = next.  nodesAll is the UNIVERSE: every stage's nodesAll is a
 // subset of it in its order, so a node that leaves and comes back keeps its position.  The caller's maps are NOT
 // mutated; they are interned once.  Every chain has the same number of stages (>= 1).  A stage the reference would
@@ -259,8 +268,10 @@ struct ChainResult {
 // outside the universe or chains of different lengths throw BlanceError naming the chain and stage before any device
 // work.  Stage maps (NextMap / NextWarnings) are filled for the chains listed in wantMaps.
 // scheduleConcurrency, audit and exposure (blance_plan_chains_exposure) fill every stage's Schedules / Audit /
-// Exposures exactly as PlanNextMapScenarios does for one scenario, with that stage's prevMap as begMap and the chain's
-// option fields; the result's NetSchedules / NetExposures and Span as described there.  The movers are the universe.
+// Exposures exactly as PlanNextMapScenarios does for one scenario, with that stage's prevMap as begMap and that stage's
+// option fields; the result's NetSchedules / NetExposures and Span as described there (the net rebalance under the last
+// stage's constraints).  The movers are the universe.  Each state's slot range is as wide as the largest constraint
+// of any stage of any chain; when some stage sets an option of its own the call is blance_plan_chains_ex.
 // A stage's ops only touch its own nodesAll when every node that leaves nodesAll was removed in an earlier stage, which
 // the default NodesAll rule guarantees; then the stage's schedule equals OrchestrateSchedule(nodesAll_t, ...).
 std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,

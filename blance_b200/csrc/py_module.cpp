@@ -481,8 +481,8 @@ PYBIND11_MODULE(_host, m) {
       py::arg("exposure_series_cap") = py::none());
 
   // chains: per chain (its option fields as a scenario tuple - the node sets are not read -, its stages); per stage
-  // (nodes_to_remove, nodes_to_add, has_node_weights_key, node_weights, nodes_all or None for the default)
-  using PyStage = std::tuple<OptStrs, OptStrs, bool, std::optional<IntMap>, OptStrs>;
+  // (a scenario tuple: its node sets, node weights and plan options of its own; nodes_all or None for the default)
+  using PyStage = std::tuple<PyScenario, OptStrs>;
   using PyChain = std::tuple<PyScenario, std::vector<PyStage>>;
   m.def(
       "PlanNextMapChains",
@@ -505,11 +505,17 @@ PYBIND11_MODULE(_host, m) {
           Chain ch;
           ch.Options = to_scenarios({std::get<0>(c)})[0];
           for (const auto& st : std::get<1>(c)) {
+            Scenario sc = to_scenarios({std::get<0>(st)})[0];
             ChainStage s;
-            s.NodesToRemove = std::get<0>(st);
-            s.NodesToAdd = std::get<1>(st);
-            if (std::get<2>(st)) s.NodeWeights = std::get<3>(st);
-            s.NodesAll = std::get<4>(st);
+            s.NodesToRemove = std::move(sc.NodesToRemove);
+            s.NodesToAdd = std::move(sc.NodesToAdd);
+            s.NodeWeights = std::move(sc.NodeWeights);
+            s.ModelStateConstraints = std::move(sc.ModelStateConstraints);
+            s.StateStickiness = std::move(sc.StateStickiness);
+            s.PartitionWeights = std::move(sc.PartitionWeights);
+            s.NodeHierarchy = std::move(sc.NodeHierarchy);
+            s.HierarchyRules = std::move(sc.HierarchyRules);
+            s.NodesAll = std::get<1>(st);
             ch.Stages.push_back(std::move(s));
           }
           cs.push_back(std::move(ch));

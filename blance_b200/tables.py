@@ -518,7 +518,7 @@ class Context:
         return results
 
     def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True,
-                    schedule=None, node_has_mover=None, audit=None, exposure=None, span=False, stage_arrays=True):
+                    schedule=None, node_has_mover=None, audit=None, exposure=None, span=False, stage_arrays=True, stage_opts=None):
         """blance_plan_chains: chains of cluster changes, each stage planned on the map the stage before produced.
         chains is a list of chains of equal length; a stage is a dict of SCENARIO_FIELDS and node_in_all ([n_nodes],
         missing = every node; missing scenario keys keep the base's value).  want_rows lists the (chain, stage) pairs
@@ -531,7 +531,13 @@ class Context:
         node_has_mover as plan_scenarios, for every stage.  span=True (needs schedule) returns (results, nets, spans):
         spans[i][k] is chain i's stages folded at count k, a dict of blance_chain_span_out's fields (the exposure ones
         with exposure, the per-partition ones with its parts, the per-vertex ones with its dom).  stage_arrays=False
-        asks for no per-stage array (schedules and exposures keep their scalars; no series): the span alone."""
+        asks for no per-stage array (schedules and exposures keep their scalars; no series): the span alone.
+
+        stage_opts (instead of opts: None, or an [n][T] nested list of the option dicts plan_scenarios takes per
+        scenario) calls blance_plan_chains_ex: stage t of chain i plans with the base's options and the groups of
+        stage_opts[i][t], and its audit and exposure use them; with or without a schedule."""
+        if opts is not None and stage_opts is not None:
+            raise ValueError("pass opts (per chain) or stage_opts (per stage), not both")
         if schedule is None:
             if audit is not None or exposure is not None or span or node_has_mover is not None:
                 raise ValueError("audit, exposure, span and node_has_mover need a schedule: pass schedule=[counts]")
@@ -567,13 +573,27 @@ class Context:
         outs = (api.ScenarioOut * max(1, n * T))(*[r.out for rs in results for r in rs])
         nets = [ChainNet(base_tables) for _ in range(n)] if net else None
         net_arr = (api.ChainOut * max(1, n))(*[x.out for x in nets]) if net else None
-        ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-        if schedule is None:
+        if stage_opts is not None:
+            if len(stage_opts) != n or any(len(so) != T for so in stage_opts):
+                raise ValueError("stage_opts must hold one option dict per stage of every chain")
+            ops = (api.ScenarioOpts * max(1, n * T))(*[_opts_struct(base_tables, o, keep) for so in stage_opts for o in so])
+        else:
+            ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
+        if schedule is None and stage_opts is not None:
+            self._check(self.lib.blance_plan_chains_ex(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
+                                                       int(max_concurrent), 0, None, None, outs, net_arr, None, None, None, None, 0,
+                                                       None, None, None, None), "blance_plan_chains_ex")
+        elif schedule is None:
             self._check(self.lib.blance_plan_chains(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
                                                     int(max_concurrent), outs, net_arr), "blance_plan_chains")
         else:
+            if stage_opts is not None:
+                opt_of = lambda i, t: stage_opts[i][t]                    # noqa: E731
+            else:
+                opt_of = lambda i, t: None if opts is None else opts[i]  # noqa: E731
             spans = self._chains_exposure(base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results,
-                                          opts, schedule, node_has_mover, audit, exposure, span, stage_arrays, keep)
+                                          opt_of, stage_opts is not None, schedule, node_has_mover, audit, exposure, span,
+                                          stage_arrays, keep)
         for i in range(n):
             for t in range(T):
                 results[i][t].out = outs[i * T + t]
@@ -581,10 +601,11 @@ class Context:
                 nets[i].out = net_arr[i]
         return (results, nets, spans) if span else (results, nets)
 
-    def _chains_exposure(self, base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results, opts,
-                         schedule, node_has_mover, audit, exposure, span, stage_arrays, keep):
-        """The blance_plan_chains_exposure call of plan_chains: fills the results' and nets' schedules, audits and
-        exposures; returns the spans (or None)."""
+    def _chains_exposure(self, base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results, opt_of,
+                         per_stage, schedule, node_has_mover, audit, exposure, span, stage_arrays, keep):
+        """The blance_plan_chains_exposure call of plan_chains (per_stage: blance_plan_chains_ex; opt_of(i, t) is the
+        option dict of chain i's stage t): fills the results' and nets' schedules, audits and exposures; returns the
+        spans (or None)."""
         counts = np.ascontiguousarray(schedule, np.int32)
         nc = counts.size
         mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
@@ -605,9 +626,9 @@ class Context:
         if audit is not None:
             a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
             for i in range(n):
-                t = scenario_tables(base_tables, {}, None if opts is None else opts[i])
-                for r in results[i]:
-                    r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
+                for t, r in enumerate(results[i]):
+                    x = scenario_tables(base_tables, {}, opt_of(i, t))
+                    r.audit = AuditResult(base_tables, _n_rules(x), n_dom, audit.get("n2n", False))
             auds = (api.AuditOut * (n * T))(*[r.audit.out for r in stages])
         e_opts, exps, net_exps, expo, net_expo, cap = None, None, None, None, None, 0
         dom = parts = False
@@ -625,12 +646,14 @@ class Context:
                 net_exps = (api.ExposureOut * (n * nc))(*[e.out for es in net_expo for e in es])
         spans = [[_ChainSpan(base_tables, V, exposure is not None, dom, parts) for _ in counts] for _ in range(n)] if span else None
         span_arr = (api.ChainSpanOut * (n * nc))(*[s.out for ss in spans for s in ss]) if span else None
-        self._check(self.lib.blance_plan_chains_exposure(
+        fn, what = (self.lib.blance_plan_chains_ex, "blance_plan_chains_ex") if per_stage else \
+            (self.lib.blance_plan_chains_exposure, "blance_plan_chains_exposure")
+        self._check(fn(
             self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)), int(max_concurrent), nc, counts.ctypes.data,
             None if mover is None else mover.ctypes.data, outs, net_arr, sch, None if audit is None else ctypes.byref(a_opts), auds,
             ctypes.byref(e_opts) if exposure is not None and exposure.get("domain_parent") is not None else None,
             cap if stage_arrays else 0, exps,
-            net_sch, net_exps, span_arr), "blance_plan_chains_exposure")
+            net_sch, net_exps, span_arr), what)
         for x, r in enumerate(stages):
             for k, s in enumerate(r.schedules):
                 s.out = sch[x * nc + k]

@@ -812,6 +812,47 @@ int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int
                                 blance_exposure_out* net_expo /* [n][n_move_conc] or NULL, needs net and expo */,
                                 blance_chain_span_out* span /* [n][n_move_conc] or NULL */);
 
+/* ---- plan options per chain stage (blance_plan_chains_ex) ---------------------------------------------------
+ * blance_plan_chains_exposure where every STAGE has its own plan options: "add two nodes, then raise the replica
+ * count", "bring in the new rack, then switch on the different-rack rule", "lose a node while the partition weights
+ * change".  T = n_stages.  Stage t of chain i is
+ *
+ *     PlanNextMapEx(prev, assign, nodesAll_t, nodesToRemove_t, nodesToAdd_t, model, options_i_t)
+ *
+ * in the Go loop of blance_plan_chains, where options_i_t is the BASE's options with the groups of
+ * stage_opts[i * T + t] substituted (as blance_plan_scenarios_ex does for one scenario) and stage t's NodeWeights.
+ * The options are absolute, not cumulative: a group whose bit is clear at stage t is the base's, whatever an earlier
+ * stage set; the partition weights of stage t are the base's with stage t's overrides applied.  From stage 2 on
+ * extra_tot_first = extra_tot_rest as in blance_plan_chains, with the stage's own extra_tot_rest when its weight group
+ * gives one.  stage_opts NULL: no options vary.  Every group keeps the rules of blance_plan_scenarios_ex (a
+ * constraint within the base's slot range of its state, distinct override indices, weights <= 999999999, the count
+ * bound), checked per stage.
+ *
+ * Per stage, the audit uses stage t's constraints and hierarchy rules and the exposure stage t's constraints.  The
+ * net schedule and exposure (base prevMap -> the last stage's final map) use the LAST stage's constraints.  The span
+ * folds the per-stage results as in blance_plan_chains_exposure.
+ *
+ * Arguments and outputs are those of blance_plan_chains_exposure, with opts [n] replaced by stage_opts [n][n_stages].
+ * With stage_opts[i * T + t] = opts[i] for every t the outputs equal blance_plan_chains_exposure's byte for byte.  The
+ * schedule may be left out: n_move_conc = 0 with move_conc and sched NULL plans (and audits, with audit) without one,
+ * and then expo, net_sched, net_expo and span must be NULL.
+ *
+ * Errors, all before any device work: everything blance_plan_chains_exposure rejects, an option group's error
+ * naming "chain i, stage t" (the audit model check too); expo, net_sched, net_expo or span without a schedule
+ * (BLANCE_ERR_INVALID_ARG).  A member of a wave is laid out and priced by the largest of its stages (hierarchy masks,
+ * rules and weight changes), so the automatic wave size holds at every stage (DESIGN.md section 16). */
+int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                          const blance_chain_stage* stages /* [n][n_stages] */,
+                          const blance_scenario_opts* stage_opts /* [n][n_stages] or NULL */, int32_t favor_min_nodes,
+                          int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                          blance_scenario_out* out /* [n][n_stages] */, blance_chain_out* net /* [n] or NULL */,
+                          blance_scenario_schedule_out* sched /* [n][n_stages][n_move_conc], or NULL without a schedule */,
+                          const blance_audit_opts* aopts, blance_audit_out* audit /* [n][n_stages] or NULL */,
+                          const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo /* [n][n_stages][n_move_conc] or NULL */,
+                          blance_scenario_schedule_out* net_sched /* [n][n_move_conc] or NULL, needs net */,
+                          blance_exposure_out* net_expo /* [n][n_move_conc] or NULL, needs net and expo */,
+                          blance_chain_span_out* span /* [n][n_move_conc] or NULL */);
+
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
 #ifdef __cplusplus
