@@ -65,6 +65,11 @@ class _ChainOut(ctypes.Structure):     # struct blance_chain_out
     _fields_ = [("node_ops", ctypes.c_void_p), ("ops_total", ctypes.c_int64), ("parts_moved", ctypes.c_int64)]
 
 
+class _ChainBranch(ctypes.Structure):  # struct blance_chain_branch
+    _fields_ = [("chain", ctypes.c_int32), ("after_stage", ctypes.c_int32), ("stages", ctypes.c_void_p),
+                ("stage_opts", ctypes.c_void_p)]
+
+
 OPT_CONSTRAINTS, OPT_STICKINESS, OPT_PART_WEIGHTS, OPT_HIERARCHY = 1, 2, 4, 8   # enum blance_scenario_opt_set
 
 
@@ -119,7 +124,7 @@ class _ChainSpanOut(ctypes.Structure):  # struct blance_chain_span_out
 
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_chains", "blance_plan_chains_exposure", "blance_plan_chains_ex", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_chains", "blance_plan_chains_exposure", "blance_plan_chains_ex", "blance_plan_chain_branches", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
            "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_exposure", "blance_moves_free")
 
@@ -152,6 +157,7 @@ def capi():
                                                     vp, vp, vp]
         lib.blance_plan_chains_ex.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp,
                                               vp, vp, vp]
+        lib.blance_plan_chain_branches.argtypes = lib.blance_plan_chains_ex.argtypes + [i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.blance_map_audit.argtypes = [vp, vp, vp, vp, vp, vp]
         lib.blance_plan_audit.argtypes = [vp, vp, vp, vp]
         lib.blance_plan_upload.argtypes = [vp, vp, ctypes.POINTER(vp)]
@@ -182,6 +188,7 @@ ScenarioOut = _ScenarioOut
 ScheduleOut = _ScheduleOut
 ChainStage = _ChainStage
 ChainOut = _ChainOut
+ChainBranch = _ChainBranch
 ScenarioScheduleOut = _ScenarioScheduleOut
 AuditOpts = _AuditOpts
 AuditOut = _AuditOut

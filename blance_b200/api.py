@@ -147,7 +147,7 @@ def PlanNextMapScenarios(prevMap, partitionsToAssign, nodesAll, model, options=N
 
 
 def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None, chains=(), favorMinNodes=False,
-                      wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None, exposure=None):
+                      wantMaps=(), maxConcurrent=0, scheduleConcurrency=(), audit=None, exposure=None, branches=None):
     """Chains of cluster changes, each stage planned on the map the stage before produced (blance_plan_chains).  Chain
     i runs the Go loop `next = PlanNextMapEx(prev, assign, nodesAll_t, nodesToRemove_t, nodesToAdd_t, model, options_i_t);
     prev = prev with every entry of next replaced; assign = next` over its stages.  nodesAll is the universe: a stage's
@@ -171,27 +171,42 @@ def PlanNextMapChains(prevMap, partitionsToAssign, nodesAll, model, options=None
     moves_done, stuck_parts, max_batch; node_rounds / node_last_round {node: ...}; part_done_round {partition: ...,
     -1 = stuck in some stage}; with exposure peak / peak_stage / peak_round / area {metric: ...}, part_min_copies /
     part_no_top / part_flags {partition: ...}, dom_peak / dom_peak_stage / dom_peak_round {name: ...}), nonzero
-    entries only."""
+    entries only.
+
+    branches (blance_plan_chain_branches): a list of dicts with "chain" (the index of the chain it leaves),
+    "afterStage" (the stage after which it leaves, -1 for the base map), "stages" (stage dicts as above, the same number
+    in every branch) and an optional "wantMaps" (bool).  A branch is planned as stages afterStage + 1, ... of its
+    equivalent chain: the chain's options and stages 0..afterStage followed by the branch's stages (so a branch stage
+    without "nodesAll" starts from trunk stage afterStage's members).  The return is then (chains, branches): one dict
+    per branch shaped like a chain's, without "span"."""
     o = options or PlanNextMapOptions()
     same = prevMap is partitionsToAssign
+
+    def stage_tuples(where, stages):
+        out = []
+        for t, st in enumerate(stages):
+            missing = {"nodesToRemove", "nodesToAdd"} - set(st)
+            if missing:
+                raise ValueError("%s, stage %d lacks %s" % (where, t, ", ".join(sorted(missing))))
+            na = st.get("nodesAll")
+            out.append((_scenario_tuples([st])[0], None if na is None else list(na)))
+        return out
+
     cs = []
     for i, c in enumerate(chains):
         opts = {k: v for k, v in c.items() if k != "stages"}
         opts.update(nodesToRemove=None, nodesToAdd=None)
-        stages = []
-        for t, st in enumerate(c["stages"]):
-            missing = {"nodesToRemove", "nodesToAdd"} - set(st)
-            if missing:
-                raise ValueError("chain %d, stage %d lacks %s" % (i, t, ", ".join(sorted(missing))))
-            na = st.get("nodesAll")
-            stages.append((_scenario_tuples([st])[0], None if na is None else list(na)))
-        cs.append((_scenario_tuples([opts])[0], stages))
+        cs.append((_scenario_tuples([opts])[0], stage_tuples("chain %d" % i, c["stages"])))
+    bs = None if branches is None else [
+        (int(b["chain"]), int(b["afterStage"]), stage_tuples("branch %d" % x, b["stages"]), bool(b.get("wantMaps", False)))
+        for x, b in enumerate(branches)]
     return _host.PlanNextMapChains(prevMap, None if same else partitionsToAssign, list(nodesAll),
                                    {k: tuple(v) for k, v in model.items()}, cs, bool(favorMinNodes),
                                    [int(i) for i in wantMaps], int(maxConcurrent), **_option_kwargs(o),
                                    schedule_concurrency=[int(c) for c in scheduleConcurrency],
                                    audit=None if audit is None else bool(audit.get("failoverSpread", False)),
-                                   exposure_series_cap=None if exposure is None else int(exposure.get("seriesCap", 0)))
+                                   exposure_series_cap=None if exposure is None else int(exposure.get("seriesCap", 0)),
+                                   branches=bs)
 
 
 def AuditMap(partitionMap, nodesAll, model, options=None, failoverSpread=False):

@@ -1192,8 +1192,9 @@ static const int kWaveMax = 65535;
 // The wave size of `n_dev` scenarios on one device (0 = one scenario does not fit), at most kWaveMax.  Scenarios
 // differ only in their hierarchy masks and weight overrides, so one is priced as in0 with the largest mask and
 // override list of any (of any stage of a chain: its mask slice and weight changes at the stage that needs the most).
+// `reserve` bytes of the free memory are left to what runs beside the wave (a chain's branch waves).
 static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_mask_words, int max_overrides, int n_dev,
-                     int max_concurrent, const SchedReq* sr, size_t extra_bytes, size_t* per_scenario) {
+                     int max_concurrent, const SchedReq* sr, size_t extra_bytes, size_t reserve, size_t* per_scenario) {
   blance_plan probe;
   std::vector<int> seg;
   layout(&probe, 1, &in0, seg);
@@ -1219,7 +1220,7 @@ static int wave_size(blance_ctx* ctx, const blance_plan_in& in0, long long max_m
   if (max_concurrent > 0) return std::min(n_dev, max_concurrent);
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return 1; }
-  const size_t headroom = std::max<size_t>(1ull << 30, total_b / 16);     // the device is shared: leave room
+  const size_t headroom = std::max<size_t>(1ull << 30, total_b / 16) + reserve;     // the device is shared: leave room
   const long long fit = free_b > headroom ? (long long)((free_b - headroom) / std::max<size_t>(per, 1)) : 0;
   int w = (int)std::min<long long>(n_dev, fit);
   // above the 3-scout speculative kernel's node limit a wide batch would drop to lock-step (run(): 2n <= sm_count)
@@ -1728,8 +1729,11 @@ static void span_slices(Arena& a, SpanBufs& b, const ChainReq& cr, long long nw,
   if (cr.span_dom) { a.add(b.F.a_dom_peak, (size_t)(ni * V)); a.add(b.F.a_dom_stage, (size_t)(ni * V)); a.add(b.F.a_dom_round, (size_t)(ni * V)); }
 }
 
+struct BranchReq;
+
 // What a scenario wave plans and analyses: the base and its scenarios sc / opts (with cr: its chains, sc NULL), the
-// plan options, the caller's outputs, and the schedules, audits and exposures asked for (each NULL: none).
+// plan options, the caller's outputs, and the schedules, audits and exposures asked for (each NULL: none).  forks: the
+// branches that leave the chains (blance_plan_chain_branches); br: the items are those branches, not chains.
 struct WaveReq {
   const blance_plan_in* base = nullptr;
   const blance_scenario* sc = nullptr;
@@ -1740,15 +1744,39 @@ struct WaveReq {
   const AuditReq* ar = nullptr;
   const ChainReq* cr = nullptr;
   const ExpoReq* er = nullptr;
+  const BranchReq* forks = nullptr;
+  const BranchReq* br = nullptr;
 };
+
+// The branches of a chain request: n branches of cr.T stages each, the trunk request they leave, and the request
+// that plans them (its items are the branches; its outputs the br_* ones).
+struct BranchReq {
+  int n = 0;
+  const blance_chain_branch* br = nullptr;
+  const WaveReq* trunk = nullptr;
+  WaveReq q;
+  ChainReq cr;
+  SchedReq sr;
+  AuditReq ar;
+  ExpoReq er;
+};
+
+// The chain stage of chain (or branch) i at its stage t.
+static const blance_chain_stage& chain_stage(const WaveReq& q, int i, int t) {
+  return q.br ? q.br->br[i].stages[t] : q.cr->stages[(size_t)i * q.cr->T + t];
+}
+
+// Stage t of item i as a stage of its (equivalent) chain: a branch's stage t follows its trunk's stage after_stage.
+static int chain_at(const WaveReq& q, int i, int t) { return q.br ? q.br->br[i].after_stage + 1 + t : t; }
 
 // The node fields of scenario (or chain) i at stage t.
 static const blance_scenario& nodes_of(const WaveReq& q, int i, int t) {
-  return q.cr ? q.cr->stages[(size_t)i * q.cr->T + t].nodes : q.sc[i];
+  return q.cr ? chain_stage(q, i, t).nodes : q.sc[i];
 }
 
 // The plan options of scenario (or chain) i at stage t.
 static const blance_scenario_opts* opts_of(const WaveReq& q, int i, int t) {
+  if (q.br) return q.br->br[i].stage_opts ? &q.br->br[i].stage_opts[t] : nullptr;
   return opts_at(q.opts, q.cr && q.cr->stage_opts ? q.cr->T : 0, i, t);
 }
 
@@ -1759,12 +1787,12 @@ static const blance_scenario_opts* opts_of(const WaveReq& q, int i, int t) {
 static blance_plan_in stage_in(const WaveReq& q, int i, int t, std::vector<uint8_t>& code) {
   blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q, i, t));
   if (!q.cr) return in;
-  const blance_chain_stage& st = q.cr->stages[(size_t)i * q.cr->T + t];
+  const blance_chain_stage& st = chain_stage(q, i, t);
   code.assign((size_t)std::max(1, in.n_node_ids), 0);
   for (int k = 0; k < in.n_node_ids; ++k)
     code[(size_t)k] = (uint8_t)((st.nodes.node_removed[k] ? NR_REMOVE : 0) | (k < in.n_nodes && !st.node_in_all[k] ? NR_OUTSIDE : 0));
   in.node_removed = code.data();
-  if (t > 0) in.extra_tot_first = in.extra_tot_rest;
+  if (chain_at(q, i, t) > 0) in.extra_tot_first = in.extra_tot_rest;
   return in;
 }
 
@@ -1775,14 +1803,15 @@ struct WeightSet { int32_t part, weight, has; };
 // over the base's, as given.  Stage t > 0: the difference from stage t-1's weights to stage t's, each the base's with
 // that stage's own overrides applied - an index stage t-1 overrode and stage t leaves alone returns to the base's
 // weight and presence - in ascending partition order, without the entries that do not change.  Scenarios and chains
-// whose options hold for every stage change nothing after stage 0.
+// whose options hold for every stage change nothing after stage 0.  A branch's stage 0 changes from the weights of
+// the trunk stage it forks from.
 static void weight_delta(const WaveReq& q, int i, int t, std::vector<WeightSet>& d) {
   const blance_scenario_opts* b = opts_of(q, i, t);
-  if (t == 0) {
+  if (chain_at(q, i, t) == 0) {
     for (int k = 0; k < n_overrides(b); ++k) d.push_back(WeightSet{b->ow_part[k], b->ow_weight[k], b->ow_has[k]});
     return;
   }
-  const blance_scenario_opts* a = opts_of(q, i, t - 1);
+  const blance_scenario_opts* a = t > 0 ? opts_of(q, i, t - 1) : opts_of(*q.br->trunk, q.br->br[i].chain, q.br->br[i].after_stage);
   if (a == b || (n_overrides(a) == 0 && n_overrides(b) == 0)) return;
   auto sorted = [](const blance_scenario_opts* o) {
     std::vector<WeightSet> v;
@@ -1825,6 +1854,7 @@ static void upload_nodes(blance_ctx* ctx, blance_plan* pl, const std::vector<bla
 
 // What every wave of one device's items idx of q shares, computed once: the base upload pb, the sizes of the
 // analyses, and the wave size W (halved when a wave does not fit) with the device bytes `per` one member is priced at.
+// A sweep of branches (q.br) forks its items from the members src of a trunk wave (trunk NULL: from the base).
 struct Sweep {
   blance_ctx* ctx;
   const WaveReq& q;
@@ -1833,9 +1863,17 @@ struct Sweep {
   const long long V, stride;           // exposure vertices, int64 words of one summary
   int max_rules = 0, W = 0;            // max_rules: over every stage of every item
   std::vector<long long> mask_cap;     // per item of idx: the mask words of its stage with the largest hierarchy masks
+  long long max_mask = 0;              // over the items: the largest mask_cap
+  int max_ow = 0;                      // over the items and stages: the most weight changes
   int n_prev_later = 0;                // len(prevMap) from stage 2 on: the base's prevMap plus every assigned partition
   bool audit_flags = false;            // any caller wants the per-partition flags
-  PlanPtr pb;
+  bool lone_ok = false;                // the only item may plan on the base upload (no branch replicates it later)
+  std::vector<int> branches;           // the branches that leave this device's chains (q.forks)
+  std::vector<uint8_t> code0;
+  blance_plan_in in0{};                // the first item's first stage, which prices a member
+  blance_plan* pb = nullptr;
+  const blance_plan* trunk = nullptr;  // the trunk wave's plan
+  std::vector<int> src;                // per item of idx: its chain's member in `trunk`
   size_t per = 0;
   Sweep(blance_ctx* c, const std::vector<int>& items, const WaveReq& r)
       : ctx(c), q(r), idx(items), T(r.cr ? r.cr->T : 1), nc(r.sr ? r.sr->nc : 0), MO(scenario_ops(*r.base)),
@@ -1951,12 +1989,15 @@ static void analysis_slices(const Sweep& s, Arena& a, AnalysisBufs& b, WSched& s
 }
 
 // The partition-weight changes of wave w's members before stage t (weight_delta) into w.ow, as wave-global partition
-// indices over the members' replicated slices (lone: over the base upload).
+// indices over the members' replicated slices (lone: over the base upload).  t = -1, for branches: their trunk
+// chains' stage-0 changes over the base.
 static void wave_weights(const Sweep& s, Wave& w, int t) {
   std::vector<WeightSet> d;
   std::vector<long long> off;          // the wave-global index of each change's member's first partition
   for (int j = 0; j < w.nw; ++j) {
-    weight_delta(s.q, s.idx[(size_t)(w.w0 + j)], t, d);
+    const int i = s.idx[(size_t)(w.w0 + j)];
+    if (t < 0) weight_delta(*s.q.br->trunk, s.q.br->br[i].chain, 0, d);
+    else weight_delta(s.q, i, t, d);
     off.resize(d.size(), w.pl->h_insts[(size_t)j].part_off);
   }
   w.ow.clear();
@@ -1974,15 +2015,19 @@ static bool wave_alloc(const Sweep& s, Wave& w) {
   const int nw = w.nw, PU = q.base->n_parts;
   for (int j = 0; j < nw; ++j) w.ins[(size_t)j] = stage_in(q, s.idx[(size_t)(w.w0 + j)], 0, w.code[(size_t)j]);
   // a device's only scenario is the base upload itself: nothing to replicate (its weight overrides still apply)
-  w.lone = s.idx.size() == 1;
-  blance_plan* pl = w.pl = w.lone ? s.pb.get() : &w.plan;
+  w.lone = s.lone_ok;
+  blance_plan* pl = w.pl = w.lone ? s.pb : &w.plan;
   if (!w.lone) layout(pl, nw, w.ins.data(), w.seg_off, q.cr != nullptr, s.mask_cap.data() + w.w0);
   if (!w.lone && pl->PT >= (1LL << 29)) {
     if (nw > 1) return false;
     throw_err(BLANCE_ERR_UNSUPPORTED, "2^29 or more partitions in one scenario");
   }
+  // a branch forked after trunk stage t starts at the loop state of a chain's later stages (stage_boundary)
+  for (int j = 0; j < nw; ++j)
+    if (chain_at(q, s.idx[(size_t)(w.w0 + j)], 0) > 0) node_state(pl->h_insts[(size_t)j], w.ins[(size_t)j], true, s.n_prev_later);
   size_t ow_cap = 0;
-  for (int t = s.T - 1; t >= 0; --t) {   // ends with stage 0's changes in w.ow
+  // ends with stage 0's changes in w.ow (a fork's wave_upload sets its own: its trunk's stage-0 changes come first)
+  for (int t = s.T - 1; t >= (s.trunk ? -1 : 0); --t) {
     wave_weights(s, w, t);
     ow_cap = std::max(ow_cap, w.ow.size());
   }
@@ -2001,13 +2046,44 @@ static bool wave_alloc(const Sweep& s, Wave& w) {
   return true;
 }
 
+// The partition-weight changes in w.ow applied to wave w's working weights and presence flags (none: nothing launched).
+static void apply_weights(const Sweep& s, Wave& w) {
+  if (w.ow.empty()) return;
+  const int k = (int)(w.ow.size() / 3);
+  CUDA(cudaMemcpyAsync(w.d_ow, w.ow.data(), sizeof(int32_t) * w.ow.size(), cudaMemcpyHostToDevice, s.ctx->stream));
+  launch(s.ctx, k_scenario_weights, grid_for(s.ctx, k, 256), 256, 0, const_cast<int32_t*>(w.pl->pool.pweight), w.pl->pflags_init, w.d_ow, k);
+}
+
+// The fork of branch wave w: each member's map, loop state and partition weights are its trunk member's after trunk
+// stage t - what stage_boundary carries into stage t + 1 - copied on the device.  Both waves share the base's layout.
+static void fork_copy(const Sweep& s, Wave& w) {
+  cudaStream_t st = s.ctx->stream;
+  const blance_plan* tp = s.trunk;
+  blance_plan* pl = w.pl;
+  auto d2d = [&](void* dst, const void* src, size_t bytes) { if (bytes) CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st)); };
+  for (int j = 0; j < w.nw; ++j) {
+    const DInst& D = pl->h_insts[(size_t)j];
+    const DInst& F = tp->h_insts[(size_t)s.src[(size_t)(w.w0 + j)]];
+    const size_t rows = (size_t)D.PU * D.SLP, parts = (size_t)D.PU;
+    d2d(pl->rows_init + D.rows_off, tp->pool.rows + F.rows_off, sizeof(int32_t) * rows);
+    d2d(pl->prev_rows_init + D.rows_off, tp->pool.prev_rows + F.rows_off, sizeof(int32_t) * rows);
+    d2d(pl->pmeta_init + D.part_off, tp->pool.pmeta + F.part_off, sizeof(uint32_t) * parts);
+    d2d(pl->prev_meta_init + D.part_off, tp->pool.prev_meta + F.part_off, sizeof(uint32_t) * parts);
+    d2d(pl->pflags_init + D.part_off, tp->pool.pflags + F.part_off, parts);
+    d2d(const_cast<int32_t*>(pl->pool.pweight) + D.part_off, tp->pool.pweight + F.part_off, sizeof(int32_t) * parts);
+  }
+}
+
 // The node tables of wave w's members (small host copies; the hierarchy masks and extra counts of the base), the base
 // replicated into every member's slices, the weight overrides, and the chains' copy of the base's prev rows and flags.
+// A branch wave forked from a trunk wave first applies its trunk chains' stage-0 weight changes, so that its nets
+// start from the base exactly as the equivalent chains' do, then forks and changes the weights from the trunk stage's
+// to its first stage's.
 static void wave_upload(const Sweep& s, Wave& w) {
   blance_ctx* ctx = s.ctx;
   cudaStream_t st = ctx->stream;
   blance_plan* pl = w.pl;
-  const blance_plan* pb = s.pb.get();
+  const blance_plan* pb = s.pb;
   DPool& P = pl->pool;
   if (!w.lone) {
     upload_nodes(ctx, pl, w.ins, s.q.cr != nullptr);
@@ -2021,14 +2097,16 @@ static void wave_upload(const Sweep& s, Wave& w) {
            pl->prev_meta_init, pl->pflags_init, const_cast<int32_t*>(P.pweight), const_cast<int32_t*>(P.name_rank),
            const_cast<int32_t*>(P.part_inst), pb->rows_init, pb->prev_rows_init, pb->pmeta_init, pb->prev_meta_init,
            pb->pflags_init, pb->pool.pweight, pb->pool.name_rank, s.q.base->n_parts, pl->h_insts[0].SLP, pl->PT);
-  if (!w.ow.empty()) {
-    const int k = (int)(w.ow.size() / 3);
-    CUDA(cudaMemcpyAsync(w.d_ow, w.ow.data(), sizeof(int32_t) * w.ow.size(), cudaMemcpyHostToDevice, st));
-    launch(ctx, k_scenario_weights, grid_for(ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, w.d_ow, k);
-  }
+  if (s.trunk) wave_weights(s, w, -1); // the base as its trunk chain's stage 0 saw it: the nets' prev rows and flags
+  apply_weights(s, w);
   if (s.q.cr && s.q.cr->net && pl->PT > 0) {   // the stage boundary overwrites these (in the lone path, the base upload's own)
     CUDA(cudaMemcpyAsync(w.an.net_prev, pl->prev_rows_init, sizeof(int32_t) * (size_t)pl->RT, cudaMemcpyDeviceToDevice, st));
     CUDA(cudaMemcpyAsync(w.an.net_flags, pl->pflags_init, (size_t)pl->PT, cudaMemcpyDeviceToDevice, st));
+  }
+  if (s.trunk) {
+    fork_copy(s, w);
+    wave_weights(s, w, 0);
+    apply_weights(s, w);
   }
   if (!w.lone) finish_upload(ctx, pl);
 }
@@ -2058,11 +2136,7 @@ static void stage_boundary(const Sweep& s, Wave& w, int t) {
   }
   upload_nodes(s.ctx, pl, w.ins, s.q.cr != nullptr);
   wave_weights(s, w, t);
-  if (!w.ow.empty()) {                 // after the copy into pflags_init above, which carries the previous stage's presence
-    const int k = (int)(w.ow.size() / 3);
-    CUDA(cudaMemcpyAsync(w.d_ow, w.ow.data(), sizeof(int32_t) * w.ow.size(), cudaMemcpyHostToDevice, st));
-    launch(s.ctx, k_scenario_weights, grid_for(s.ctx, k, 256), 256, 0, const_cast<int32_t*>(P.pweight), pl->pflags_init, w.d_ow, k);
-  }
+  apply_weights(s, w);                 // after the copy into pflags_init above, which carries the previous stage's presence
 }
 
 // Summaries (node_ops | state_node_load | 3 scalars per member, s.stride int64 words) of wave w's plans from the beg
@@ -2268,24 +2342,20 @@ static void report(const Sweep& s, const Wave& w, int t) {
   if (s.q.sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", w.sched_ms, s.nc);
   if (s.q.er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", w.expo_ms, w.expo_bytes);
   if (s.q.cr && s.q.cr->span) std::fprintf(stderr, ", span fold %.3f ms", w.fold_ms);
-  if (s.q.cr) std::fprintf(stderr, " (stage %d)", t);
+  if (s.q.br) std::fprintf(stderr, " (branches after trunk stage %d, stage %d)", chain_at(s.q, s.idx[0], 0) - 1, t);
+  else if (s.q.cr) std::fprintf(stderr, " (stage %d)", t);
   std::fprintf(stderr, "\n");
 }
 
-// Plans the items idx of q on one device, in waves.  With q.cr each item is a chain of cr->T stages, planned in lock
-// step: a stage boundary is an iteration boundary plus the next stage's node tables (DESIGN.md section 12).
-static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, const WaveReq& q) {
-  Sweep s(ctx, idx, q);
-  const int n_dev = (int)idx.size();
-  std::vector<uint8_t> code0;
-  const blance_plan_in in0 = stage_in(q, idx[0], 0, code0);
-  // a member is priced and laid out by the largest of its stages: hierarchy masks, rules and weight changes
-  long long max_mask = 0;
-  int max_ow = 0;
-  s.mask_cap.assign(idx.size(), 0);
+// Prices one member of sweep s and its largest stage: the mask slices, rules, weight changes and audit flags of every
+// stage of every item, and s.in0.
+static void price_items(Sweep& s) {
+  const WaveReq& q = s.q;
+  s.in0 = stage_in(q, s.idx[0], 0, s.code0);
+  s.mask_cap.assign(s.idx.size(), 0);
   std::vector<WeightSet> delta;
-  for (size_t x = 0; x < idx.size(); ++x) {
-    const int i = idx[x];
+  for (size_t x = 0; x < s.idx.size(); ++x) {
+    const int i = s.idx[x];
     for (int t = 0; t < s.T; ++t) {
       if (t > 0 && !(q.cr && q.cr->stage_opts)) break;    // the same options at every stage
       const blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q, i, t));
@@ -2293,28 +2363,71 @@ static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, co
       s.max_rules = std::max(s.max_rules, in.has_hier_rules ? in.n_rules : 0);
       delta.clear();
       weight_delta(q, i, t, delta);
-      max_ow = std::max(max_ow, (int)delta.size());
+      s.max_ow = std::max(s.max_ow, (int)delta.size());
     }
-    max_mask = std::max(max_mask, s.mask_cap[x]);
+    if (q.br && chain_at(q, i, 0) > 0) {  // a fork applies its trunk chain's stage-0 changes first (wave_upload)
+      delta.clear();
+      weight_delta(*q.br->trunk, q.br->br[i].chain, 0, delta);
+      s.max_ow = std::max(s.max_ow, (int)delta.size());
+    }
+    s.max_mask = std::max(s.max_mask, s.mask_cap[x]);
     for (int t = 0; q.ar && t < s.T; ++t) s.audit_flags |= q.ar->out[(size_t)i * s.T + t].part_flags != nullptr;
   }
-  {
-    cudaMemPool_t pool;                // measure free memory without this context's cached arenas
-    if (q.max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaMemPoolTrimTo(pool, 0);
-    }
+  for (int p = 0; q.cr && p < q.base->n_parts; ++p) s.n_prev_later += (q.base->part_in_prev[p] || q.base->part_in_assign[p]) ? 1 : 0;
+}
+
+// Releases the device memory this context's pool caches, so that free memory is measured without it (automatic
+// wave sizes only).
+static void trim_pool(const Sweep& s) {
+  cudaMemPool_t pool;
+  if (s.q.max_concurrent <= 0 && cudaDeviceGetDefaultMemPool(&pool, s.ctx->device) == cudaSuccess) {
+    cudaStreamSynchronize(s.ctx->stream);
+    cudaMemPoolTrimTo(pool, 0);
   }
-  // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
-  s.pb = upload(ctx, 1, &in0, q.cr != nullptr, n_dev == 1 ? s.mask_cap.data() : nullptr);   // lone: the wave's own plan
+}
+
+// The wave size of sweep s over n items with max_concurrent (its price in s.per), leaving `reserve` bytes free.
+static int size_waves(Sweep& s, int n, int max_concurrent, size_t reserve) {
   Arena one;                           // one member's analysis buffers, priced into the wave
   AnalysisBufs one_bufs;
   WSched one_sched{};
-  analysis_slices(s, one, one_bufs, one_sched, 1, s.pb.get());
-  s.W = wave_size(ctx, in0, max_mask, max_ow, n_dev, q.max_concurrent, q.sr, one.bytes(), &s.per);
+  analysis_slices(s, one, one_bufs, one_sched, 1, s.pb);
+  return wave_size(s.ctx, s.in0, s.max_mask, s.max_ow, n, max_concurrent, s.q.sr, one.bytes(), reserve, &s.per);
+}
+
+static void sweep_waves(Sweep& s);
+
+// Plans the branches `items` of the trunk sweep ts that leave the members src of the trunk wave planned on `trunk`
+// (NULL: from the base), in waves sized by the free memory now.
+static void branch_sweep(const Sweep& ts, const std::vector<int>& items, const blance_plan* trunk, std::vector<int> src) {
+  Sweep s(ts.ctx, items, ts.q.forks->q);
+  s.pb = ts.pb; s.trunk = trunk; s.src = std::move(src);
+  price_items(s);
+  trim_pool(s);                        // the arenas of earlier branch waves
+  s.W = size_waves(s, (int)items.size(), s.q.max_concurrent, 0);
   if (s.W < 1)
-    throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(s.per >> 20) + " MiB, more than the free device memory");
-  for (int p = 0; q.cr && p < q.base->n_parts; ++p) s.n_prev_later += (q.base->part_in_prev[p] || q.base->part_in_assign[p]) ? 1 : 0;
+    throw_err(BLANCE_ERR_NOMEM, "blance_plan_chain_branches: one branch needs " + std::to_string(s.per >> 20) + " MiB, more than the free device memory");
+  sweep_waves(s);
+}
+
+// After stage t of trunk wave w: the branches of the device that leave the wave's members there.
+static void fork_branches(const Sweep& s, const Wave& w, int t) {
+  std::vector<int> items, src;
+  for (int b : s.branches) {
+    const blance_chain_branch& x = s.q.forks->br[b];
+    if (x.after_stage != t) continue;
+    for (int j = 0; j < w.nw; ++j)
+      if (s.idx[(size_t)(w.w0 + j)] == x.chain) { items.push_back(b); src.push_back(j); }
+  }
+  if (!items.empty()) branch_sweep(s, items, w.pl, std::move(src));
+}
+
+// The waves of sweep s, each planned stage by stage in lock step (a stage boundary is an iteration boundary plus the
+// next stage's node tables, DESIGN.md section 12), with the branches that fork off them (section 17).
+static void sweep_waves(Sweep& s) {
+  blance_ctx* ctx = s.ctx;
+  const WaveReq& q = s.q;
+  const int n_dev = (int)s.idx.size();
   for (int w0 = 0; w0 < n_dev;) {
     Wave w(w0, std::min(s.W, n_dev - w0));
     if (!wave_alloc(s, w)) { s.W = w.nw / 2; continue; }
@@ -2334,11 +2447,50 @@ static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, co
         if (q.cr && q.cr->span) span_fold(s, w, t, scal);
       }
       if (getenv("BLANCE_SCENARIO_TIMES")) report(s, w, t);
+      if (!s.branches.empty()) fork_branches(s, w, t);
     }
     if (q.cr && q.cr->net) net_results(s, w);
     if (q.cr && q.cr->span) span_out(s, w);
     w0 += w.nw;
   }
+}
+
+// Plans the items idx of q on one device, in waves (sweep_waves).  With q.cr each item is a chain of cr->T stages;
+// with q.forks the branches that leave these chains are planned with them: those from the base first, the others
+// forked off the trunk waves.  A device with branches keeps the base upload pristine (no lone path), and its trunk's
+// automatic wave size leaves room for a branch wave of one member beside the live trunk wave.
+static void scenarios_on_device(blance_ctx* ctx, const std::vector<int>& idx, const WaveReq& q) {
+  Sweep s(ctx, idx, q);
+  const int n_dev = (int)idx.size();
+  if (q.forks) {
+    std::vector<char> mine;
+    for (int i : idx) { mine.resize(std::max(mine.size(), (size_t)i + 1), 0); mine[(size_t)i] = 1; }
+    for (int b = 0; b < q.forks->n; ++b)
+      if ((size_t)q.forks->br[b].chain < mine.size() && mine[(size_t)q.forks->br[b].chain]) s.branches.push_back(b);
+  }
+  s.lone_ok = n_dev == 1 && s.branches.empty();
+  // a member is priced and laid out by the largest of its stages: hierarchy masks, rules and weight changes
+  price_items(s);
+  trim_pool(s);                        // measure free memory without this context's cached arenas
+  // the base: one H2D of the caller's layout, then k_unpack (into its *_init slices)
+  const PlanPtr pb = upload(ctx, 1, &s.in0, q.cr != nullptr, s.lone_ok ? s.mask_cap.data() : nullptr);   // lone: the wave's own plan
+  s.pb = pb.get();
+  size_t reserve = 0;                  // one branch member, the largest of the device's
+  if (!s.branches.empty()) {
+    Sweep sb(ctx, s.branches, q.forks->q);
+    sb.pb = s.pb;
+    price_items(sb);
+    size_waves(sb, 1, 1, 0);
+    reserve = sb.per;
+  }
+  s.W = size_waves(s, n_dev, q.max_concurrent, reserve);
+  if (s.W < 1)
+    throw_err(BLANCE_ERR_NOMEM, "blance_plan_scenarios: one scenario needs " + std::to_string(s.per >> 20) + " MiB, more than the free device memory");
+  std::vector<int> from_base;
+  for (int b : s.branches)
+    if (q.forks->br[b].after_stage < 0) from_base.push_back(b);
+  if (!from_base.empty()) branch_sweep(s, from_base, nullptr, {});
+  sweep_waves(s);
   cudaStreamSynchronize(ctx->stream);
 }
 
@@ -2477,15 +2629,96 @@ extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, i
   });
 }
 
+// The branch arguments of blance_plan_chain_branches.
+struct BranchArgs {
+  int32_t n = 0, T = 0;
+  const blance_chain_branch* br = nullptr;
+  blance_scenario_out* out = nullptr;
+  blance_chain_out* net = nullptr;
+  blance_scenario_schedule_out* sched = nullptr;
+  blance_audit_out* audit = nullptr;
+  blance_exposure_out* expo = nullptr;
+  blance_scenario_schedule_out* net_sched = nullptr;
+  blance_exposure_out* net_expo = nullptr;
+};
+
+// The checks of the branches a of the trunk request q (its n chains of n_stages stages, checked), run on each
+// equivalent chain's branch stages, and their request in b (q.forks set to it).  aopts as the trunk's.
+static void check_branches(const std::string& name, WaveReq& q, int32_t n, int32_t n_stages, const blance_audit_opts* aopts,
+                           const BranchArgs& a, BranchReq& b) {
+  const blance_plan_in& base = *q.base;
+  if (a.n < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_branches is negative");
+  if (a.n == 0) return;
+  if (a.T < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_branch_stages must be positive");
+  if (!a.br || !a.out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br or br_out is NULL");
+  if ((a.net_sched || a.net_expo) && !a.net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_net_sched and br_net_expo need br_net");
+  if (!q.sr && (a.sched || a.expo || a.net_sched || a.net_expo))
+    throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_sched, br_expo, br_net_sched and br_net_expo need a schedule");
+  if (q.sr && !a.sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_sched is NULL with a schedule");
+  if ((a.expo && !q.er) || (a.net_expo && !a.expo)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_expo needs expo and br_net_expo needs br_expo");
+  long long base_sum = -1;
+  for (int x = 0; x < a.n; ++x) {
+    const blance_chain_branch& br = a.br[x];
+    const std::string at = name + ": branch " + std::to_string(x);
+    if (!br.stages) throw_err(BLANCE_ERR_INVALID_ARG, at + ": stages is NULL");
+    if (br.chain < 0 || br.chain >= n) throw_err(BLANCE_ERR_INVALID_ARG, at + ": chain outside [0, n)");
+    if (br.after_stage < -1 || br.after_stage >= n_stages) throw_err(BLANCE_ERR_INVALID_ARG, at + ": after_stage outside [-1, n_stages)");
+    if (br.after_stage + 1 + a.T > 1 && base.max_iters < 1)
+      throw_err(BLANCE_ERR_INVALID_ARG, at + ": a chain of several stages needs max_iters >= 1");
+    for (int u = 0; u < a.T; ++u) {     // the checks check_chains makes of a chain stage
+      const blance_chain_stage& cs = br.stages[u];
+      std::string why;
+      int st = check_scenario(base, cs.nodes, br.stage_opts ? &br.stage_opts[u] : nullptr, base_sum, why);
+      if (st == BLANCE_OK && base.n_nodes > 0 && !cs.node_in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
+      for (int k = 0; st == BLANCE_OK && k < base.n_nodes; ++k)
+        if (cs.node_in_all[k] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
+      if (st != BLANCE_OK) throw_err(st, at + ", stage " + std::to_string(u) + ": " + why);
+    }
+  }
+  b.n = a.n; b.br = a.br; b.trunk = &q;
+  b.cr.T = a.T; b.cr.stage_opts = true; b.cr.net = a.net; b.cr.net_sched = a.net_sched; b.cr.net_expo = a.net_expo;
+  b.q = WaveReq{q.base, nullptr, nullptr, q.favor_min, q.max_concurrent, a.out, nullptr, nullptr, &b.cr};
+  b.q.br = &b;
+  if (a.audit) {
+    b.ar = check_audit_opts(name, aopts, base.n_node_ids, a.audit);
+    for (int x = 0; x < a.n; ++x)
+      for (int u = 0; u < a.T; ++u) {
+        const blance_plan_in in = scenario_in(base, a.br[x].stages[u].nodes, opts_of(b.q, x, u));
+        check_audit_model(name + ": branch " + std::to_string(x) + ", stage " + std::to_string(u), &in);
+      }
+    b.q.ar = &b.ar;
+  }
+  const int nc = q.sr ? q.sr->nc : 0;
+  if (q.sr) {
+    b.sr = *q.sr;
+    b.sr.out = a.sched;
+    for (long long x = 0; x < (long long)a.n * a.T * nc; ++x) { a.sched[x].rounds = 0; a.sched[x].moves_done = 0; a.sched[x].stuck_parts = 0; a.sched[x].max_batch = 0; }
+    b.q.sr = &b.sr;
+  }
+  if (a.expo) {
+    b.er = ExpoReq{q.er->n_domains, q.er->parent, q.er->series_cap, a.expo};
+    auto stage_name = [&](long long x) {
+      return "branch " + std::to_string(x / ((long long)a.T * nc)) + ", stage " + std::to_string(x / nc % a.T) + ", count " + std::to_string(x % nc);
+    };
+    auto pair_name = [&](long long x) { return "branch " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
+    expo_flags(name, base, a.expo, (long long)a.n * a.T * nc, stage_name, b.er);
+    expo_flags(name, base, a.net_expo, (long long)a.n * nc, pair_name, b.er);
+    b.q.er = &b.er;
+  }
+  q.forks = &b;
+}
+
 // blance_plan_chains_exposure (opts [n]) and blance_plan_chains_ex (stage_opts: opts [n][n_stages], and the schedule
-// may be left out: n_move_conc 0 with move_conc and sched NULL plans and audits without one).
+// may be left out: n_move_conc 0 with move_conc and sched NULL plans and audits without one); with ba the branches of
+// blance_plan_chain_branches.
 static void plan_chains_analysed(blance_ctx* ctx, const std::string& name, bool stage_opts, const blance_plan_in* base, int32_t n,
                                  int32_t n_stages, const blance_chain_stage* stages, const blance_scenario_opts* opts,
                                  int32_t favor_min_nodes, int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
                                  const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
                                  blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
                                  const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
-                                 blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span) {
+                                 blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span,
+                                 const BranchArgs* ba = nullptr) {
   if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
   const int T = n_stages, nc = n_move_conc, per_stage = stage_opts ? T : 0;
   if ((net_sched || net_expo) && !net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_sched and net_expo need net");
@@ -2522,8 +2755,10 @@ static void plan_chains_analysed(blance_ctx* ctx, const std::string& name, bool 
   er.dom |= cr.span_dom;
   er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
   check_chains(name, base, n, n_stages, stages, opts, per_stage, out);
-  plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, audit ? &ar : nullptr, &cr,
-                            expo ? &er : nullptr});
+  WaveReq q{base, nullptr, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, audit ? &ar : nullptr, &cr, expo ? &er : nullptr};
+  BranchReq br;
+  if (ba) check_branches(name, q, n, n_stages, aopts, *ba, br);
+  plan_wave(ctx, n, q);
 }
 
 extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
@@ -2552,6 +2787,25 @@ extern "C" int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base
     plan_chains_analysed(ctx, "blance_plan_chains_ex", true, base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent,
                          n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
                          net_expo, span);
+  });
+}
+
+extern "C" int blance_plan_chain_branches(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                          const blance_chain_stage* stages, const blance_scenario_opts* stage_opts, int32_t favor_min_nodes,
+                                          int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
+                                          const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
+                                          blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
+                                          const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
+                                          blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span,
+                                          int32_t n_branches, int32_t n_branch_stages, const blance_chain_branch* br,
+                                          blance_scenario_out* br_out, blance_chain_out* br_net, blance_scenario_schedule_out* br_sched,
+                                          blance_audit_out* br_audit, blance_exposure_out* br_expo,
+                                          blance_scenario_schedule_out* br_net_sched, blance_exposure_out* br_net_expo) {
+  return entry(ctx, [&](Device&) {
+    const BranchArgs ba{n_branches, n_branch_stages, br, br_out, br_net, br_sched, br_audit, br_expo, br_net_sched, br_net_expo};
+    plan_chains_analysed(ctx, "blance_plan_chain_branches", true, base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent,
+                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
+                         net_expo, span, &ba);
   });
 }
 

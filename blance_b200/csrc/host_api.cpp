@@ -1548,7 +1548,8 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
                                            const PlanNextMapOptions& options, const std::vector<Chain>& chains,
                                            bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
                                            const std::vector<int>& scheduleConcurrency, const ScenarioAudit* audit,
-                                           const ScenarioExposure* exposure) {
+                                           const ScenarioExposure* exposure, const std::vector<ChainBranch>* branches,
+                                           std::vector<ChainResult>* branchResults) {
   if (chains.empty()) invalid("PlanNextMapChains: no chains");
   if ((audit || exposure) && scheduleConcurrency.empty()) invalid("PlanNextMapChains: an audit or exposure needs scheduleConcurrency");
   if (exposure && exposure->SeriesCap < 0) invalid("PlanNextMapChains: SeriesCap is negative");
@@ -1558,97 +1559,139 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
     if (chains[i].Stages.size() != T)
       invalid("PlanNextMapChains: chain " + std::to_string(i) + " has " + std::to_string(chains[i].Stages.size()) +
               " stages, chain 0 has " + std::to_string(T) + " (chains of different lengths go in separate calls)");
-  // every stage as a scenario: its node sets and weights, the chain's option fields and the stage's own
-  std::vector<Scenario> flat(n * T);
-  bool stage_opts = false;             // some stage sets an option of its own: blance_plan_chains_ex
+  const size_t nb = branches ? branches->size() : 0, TB = nb ? (*branches)[0].Stages.size() : 0;
+  if (nb && !branchResults) invalid("PlanNextMapChains: branches need branchResults");
+  for (size_t b = 0; b < nb; ++b) {
+    const ChainBranch& br = (*branches)[b];
+    const std::string who = "PlanNextMapChains: branch " + std::to_string(b);
+    if (br.Stages.size() != TB || TB == 0)
+      invalid(who + " has " + std::to_string(br.Stages.size()) + " stages, branch 0 has " + std::to_string(TB) +
+              " (every branch of one call has the same number of stages, at least one)");
+    if (br.Chain < 0 || size_t(br.Chain) >= n) invalid(who + ": Chain outside [0, len(chains))");
+    if (br.AfterStage < -1 || br.AfterStage >= int(T)) invalid(who + ": AfterStage outside [-1, stages)");
+  }
+  // every stage as a scenario: its node sets and weights, its chain's option fields and the stage's own; the trunk's
+  // n x T stages first, then the branches' nb x TB
+  auto stage_scenario = [](const Chain& ch, const ChainStage& cs, bool& own_opts) {
+    Scenario sc = ch.Options;
+    sc.NodesToRemove = cs.NodesToRemove;
+    sc.NodesToAdd = cs.NodesToAdd;
+    if (cs.NodeWeights) sc.NodeWeights = cs.NodeWeights;
+    if (cs.ModelStateConstraints) sc.ModelStateConstraints = cs.ModelStateConstraints;
+    if (cs.StateStickiness) sc.StateStickiness = cs.StateStickiness;
+    if (cs.PartitionWeights) sc.PartitionWeights = cs.PartitionWeights;
+    if (cs.NodeHierarchy) sc.NodeHierarchy = cs.NodeHierarchy;
+    if (cs.HierarchyRules) sc.HierarchyRules = cs.HierarchyRules;
+    own_opts |= cs.ModelStateConstraints || cs.StateStickiness || cs.PartitionWeights || cs.NodeHierarchy || cs.HierarchyRules;
+    return sc;
+  };
+  const size_t NS = n * T + nb * TB;   // stages of the trunk and the branches
+  std::vector<Scenario> flat(NS);
+  bool stage_opts = nb > 0;            // some stage sets an option of its own (or branches): options per stage
   for (size_t i = 0; i < n; ++i)
-    for (size_t t = 0; t < T; ++t) {
-      const ChainStage& cs = chains[i].Stages[t];
-      Scenario& sc = flat[i * T + t];
-      sc = chains[i].Options;
-      sc.NodesToRemove = cs.NodesToRemove;
-      sc.NodesToAdd = cs.NodesToAdd;
-      if (cs.NodeWeights) sc.NodeWeights = cs.NodeWeights;
-      if (cs.ModelStateConstraints) sc.ModelStateConstraints = cs.ModelStateConstraints;
-      if (cs.StateStickiness) sc.StateStickiness = cs.StateStickiness;
-      if (cs.PartitionWeights) sc.PartitionWeights = cs.PartitionWeights;
-      if (cs.NodeHierarchy) sc.NodeHierarchy = cs.NodeHierarchy;
-      if (cs.HierarchyRules) sc.HierarchyRules = cs.HierarchyRules;
-      stage_opts |= cs.ModelStateConstraints || cs.StateStickiness || cs.PartitionWeights || cs.NodeHierarchy || cs.HierarchyRules;
-    }
+    for (size_t t = 0; t < T; ++t) flat[i * T + t] = stage_scenario(chains[i], chains[i].Stages[t], stage_opts);
+  for (size_t b = 0; b < nb; ++b)
+    for (size_t u = 0; u < TB; ++u)
+      flat[n * T + b * TB + u] = stage_scenario(chains[size_t((*branches)[b].Chain)], (*branches)[b].Stages[u], stage_opts);
   auto ip = intern_scenario_base(prevMap, partitionsToAssign, nodesAll, model, options, flat);
   const int32_t N = ip->in.n_nodes, NU = ip->in.n_node_ids, S = ip->in.n_states;
   std::unordered_map<std::string, int32_t> universe;
   for (int32_t q = 0; q < N; ++q) universe.emplace(ip->node_names[size_t(q)], q);
   PartIndex parts{*ip, {}};
-  std::vector<ScenarioTables> tabs(n * T);
-  std::vector<std::vector<uint8_t>> member(n * T);
-  for (size_t i = 0; i < n; ++i)
-    for (size_t t = 0; t < T; ++t) {
-      const std::string who = "chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": ";
-      tabs[i * T + t] = scenario_tables(*ip, model, flat[i * T + t], options, who, parts, t == 0);
-      const ChainStage& cs = chains[i].Stages[t];
-      std::vector<uint8_t>& m = member[i * T + t];
-      m.assign(size_t(N) + 1, 0);
-      if (cs.NodesAll) {
-        for (const auto& name : *cs.NodesAll) {
-          auto it = universe.find(name);
-          if (it == universe.end()) throw BlanceError(BLANCE_ERR_INVALID_ARG, "blance: " + who + "NodesAll name '" + name + "' is not in nodesAll");
-          m[size_t(it->second)] = 1;
-        }
-      } else if (t == 0) {
-        std::fill(m.begin(), m.begin() + N, uint8_t(1));
-      } else {                         // (previous members - previous NodesToRemove) U NodesToAdd
-        const std::vector<uint8_t>& pm = member[i * T + t - 1];
-        const ScenarioTables& pt = tabs[i * T + t - 1];
-        for (int32_t q = 0; q < N; ++q) m[size_t(q)] = (pm[size_t(q)] && !pt.removed[size_t(q)]) || tabs[i * T + t].added[size_t(q)];
+  std::vector<ScenarioTables> tabs(NS);
+  std::vector<std::vector<uint8_t>> member(NS);
+  // the tables and members of stage x (chain stage g of its equivalent chain; prev: the stage before it, or NS)
+  auto stage_tables = [&](size_t x, const ChainStage& cs, size_t g, size_t prev, const std::string& who) {
+    tabs[x] = scenario_tables(*ip, model, flat[x], options, who, parts, g == 0);
+    std::vector<uint8_t>& m = member[x];
+    m.assign(size_t(N) + 1, 0);
+    if (cs.NodesAll) {
+      for (const auto& name : *cs.NodesAll) {
+        auto it = universe.find(name);
+        if (it == universe.end()) throw BlanceError(BLANCE_ERR_INVALID_ARG, "blance: " + who + "NodesAll name '" + name + "' is not in nodesAll");
+        m[size_t(it->second)] = 1;
       }
+    } else if (g == 0) {
+      std::fill(m.begin(), m.begin() + N, uint8_t(1));
+    } else {                           // (previous members - previous NodesToRemove) U NodesToAdd
+      const std::vector<uint8_t>& pm = member[prev];
+      const ScenarioTables& pt = tabs[prev];
+      for (int32_t q = 0; q < N; ++q) m[size_t(q)] = (pm[size_t(q)] && !pt.removed[size_t(q)]) || tabs[x].added[size_t(q)];
     }
-  std::vector<bool> want(n, false);
+  };
+  for (size_t i = 0; i < n; ++i)
+    for (size_t t = 0; t < T; ++t)
+      stage_tables(i * T + t, chains[i].Stages[t], t, i * T + t - 1, "chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": ");
+  for (size_t b = 0; b < nb; ++b) {
+    const ChainBranch& br = (*branches)[b];
+    for (size_t u = 0; u < TB; ++u) {
+      const size_t x = n * T + b * TB + u, g = size_t(br.AfterStage + 1) + u;
+      const size_t prev = u > 0 ? x - 1 : br.AfterStage >= 0 ? size_t(br.Chain) * T + size_t(br.AfterStage) : NS;
+      stage_tables(x, br.Stages[u], g, prev, "branch " + std::to_string(b) + ", stage " + std::to_string(u) + ": ");
+    }
+  }
+  std::vector<bool> want(NS, false);
   for (int i : wantMaps) {
     if (i < 0 || size_t(i) >= n) invalid("PlanNextMapChains: wantMaps index " + std::to_string(i) + " out of range");
-    want[size_t(i)] = true;
+    for (size_t t = 0; t < T; ++t) want[size_t(i) * T + t] = true;
   }
-  std::vector<blance_chain_stage> stages(n * T);
-  std::vector<blance_scenario_opts> opts(stage_opts ? n * T : n);
-  std::vector<blance_scenario_out> out(n * T);
-  std::vector<blance_chain_out> net(n);
-  std::vector<std::vector<int64_t>> ops(n * T, std::vector<int64_t>(size_t(NU) * 4 + 1)),
-      load(n * T, std::vector<int64_t>(size_t(S) * size_t(NU) + 1)), net_ops(n, std::vector<int64_t>(size_t(NU) * 4 + 1));
-  std::vector<std::unique_ptr<PlanOutBuffers>> maps(n * T);
-  for (size_t x = 0; x < n * T; ++x) {
+  for (size_t b = 0; b < nb; ++b)
+    for (size_t u = 0; u < TB; ++u) want[n * T + b * TB + u] = (*branches)[b].WantMaps;
+  std::vector<blance_chain_stage> stages(NS);
+  std::vector<blance_scenario_opts> opts(stage_opts ? NS : n);
+  std::vector<blance_scenario_out> out(NS);
+  std::vector<blance_chain_out> net(n + nb);
+  std::vector<std::vector<int64_t>> ops(NS, std::vector<int64_t>(size_t(NU) * 4 + 1)),
+      load(NS, std::vector<int64_t>(size_t(S) * size_t(NU) + 1)), net_ops(n + nb, std::vector<int64_t>(size_t(NU) * 4 + 1));
+  std::vector<std::unique_ptr<PlanOutBuffers>> maps(NS);
+  for (size_t x = 0; x < NS; ++x) {
     const ScenarioTables& tb = tabs[x];
     stages[x] = blance_chain_stage{blance_scenario{tb.removed.data(), tb.added.data(), tb.add_is_nil, tb.has_node_weights,
                                                    tb.weight.data(), tb.has_weight.data()},
                                    member[x].data()};
-    if (want[x / T]) maps[x] = std::make_unique<PlanOutBuffers>(*ip);
+    if (want[x]) maps[x] = std::make_unique<PlanOutBuffers>(*ip);
     out[x] = scenario_out(ops[x], load[x], maps[x].get());
   }
   // each stage's option groups, or the chain's when no stage sets its own (its stages then differ in node fields only)
   for (size_t x = 0; x < opts.size(); ++x) opts[x] = scenario_opts(tabs[stage_opts ? x : x * T]);
-  for (size_t i = 0; i < n; ++i) {
+  for (size_t i = 0; i < n + nb; ++i) {
     net[i] = blance_chain_out{};
     net[i].node_ops = net_ops[i].data();
   }
-  // the analyses (blance_plan_chains_exposure): per stage [n][T][nc], the net rebalance and the spans [n][nc]
+  // the analyses (blance_plan_chains_exposure): per stage [n][T][nc], the net rebalance and the spans [n][nc]; the
+  // branches' per stage [nb][TB][nc] and their nets [nb][nc] after them
   const size_t nc = scheduleConcurrency.size(), P = size_t(ip->in.n_parts);
   // every stage audits with its own rules
   AnalysisOutputs an(*ip, options, n * T, nc, audit, exposure, nc > 0, [&](size_t x) { return audit_rules(tabs[x], *ip); });
-  ScheduleBuffers net_sched(n * nc, size_t(NU));
+  AnalysisOutputs ban(*ip, options, nb * TB, nc, audit, exposure, false, [&](size_t x) { return audit_rules(tabs[n * T + x], *ip); });
+  ScheduleBuffers net_sched((n + nb) * nc, size_t(NU));
   std::vector<std::unique_ptr<ExposureBuffers>> nebuf;
   std::vector<blance_exposure_out> neout;
   std::vector<std::unique_ptr<SpanBuffers>> sbuf;
   std::vector<blance_chain_span_out> sout;
-  for (size_t x = 0; x < n * nc; ++x) {
+  for (size_t x = 0; x < (n + nb) * nc; ++x) {
     if (exposure) {
       nebuf.push_back(std::make_unique<ExposureBuffers>(an.cap, an.eforest.names.size(), P));
       neout.push_back(nebuf.back()->out);
     }
+    if (x >= n * nc) continue;
     sbuf.push_back(std::make_unique<SpanBuffers>(size_t(NU), P, an.eforest.names.size(), exposure != nullptr));
     sout.push_back(sbuf.back()->out);
   }
+  std::vector<blance_chain_branch> br(nb);
+  for (size_t b = 0; b < nb; ++b)
+    br[b] = blance_chain_branch{(*branches)[b].Chain, (*branches)[b].AfterStage, stages.data() + n * T + b * TB, opts.data() + n * T + b * TB};
   blance_ctx* ctx = DefaultContext();
-  const int st = stage_opts
+  const int st = nb ? blance_plan_chain_branches(
+                          ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                          int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(), net.data(),
+                          nc ? an.sched.out.data() : nullptr, audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr,
+                          &an.eforest.opts, int32_t(an.cap), exposure ? an.eout.data() : nullptr, nc ? net_sched.out.data() : nullptr,
+                          exposure ? neout.data() : nullptr, nc ? sout.data() : nullptr, int32_t(nb), int32_t(TB), br.data(),
+                          out.data() + n * T, net.data() + n, nc ? ban.sched.out.data() : nullptr, audit ? ban.aout.data() : nullptr,
+                          exposure ? ban.eout.data() : nullptr, nc ? net_sched.out.data() + n * nc : nullptr,
+                          exposure ? neout.data() + n * nc : nullptr)
+                 : stage_opts
                      ? blance_plan_chains_ex(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
                                              maxConcurrent, int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
                                              net.data(), nc ? an.sched.out.data() : nullptr, audit ? &an.forest.opts : nullptr,
@@ -1663,28 +1706,35 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
                     : blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
                                          maxConcurrent, out.data(), net.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_chains failed: ") + blance_last_error(ctx));
-  std::vector<ChainResult> res(n);
-  for (size_t i = 0; i < n; ++i) {
-    for (size_t t = 0; t < T; ++t) {
-      const size_t x = i * T + t;
+  // chain (or branch) i of n + nb: its stages' results from x0 on, its net and, for a chain, its span
+  auto result = [&](size_t i, size_t x0, size_t len, AnalysisOutputs& a) {
+    ChainResult c;
+    for (size_t t = 0; t < len; ++t) {
+      const size_t x = x0 + t;
       const int32_t* k = (tabs[x].set & BLANCE_OPT_CONSTRAINTS) ? tabs[x].constraints.data() : ip->state_constraints.data();
       ScenarioResult r = scenario_result(*ip, out[x], ops[x], load[x], maps[x].get(), k);
-      an.name(*ip, x, scheduleConcurrency, audit_rules(tabs[x], *ip).off, r);
-      res[i].Stages.push_back(std::move(r));
+      a.name(*ip, i < n ? x : x - n * T, scheduleConcurrency, audit_rules(tabs[x], *ip).off, r);
+      c.Stages.push_back(std::move(r));
     }
-    res[i].NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());
-    res[i].NetOpsTotal = net[i].ops_total;
-    res[i].NetPartsMoved = net[i].parts_moved;
-    for (size_t c = 0; c < nc; ++c) {
-      res[i].NetSchedules.push_back(name_schedule(*ip, net_sched.out[i * nc + c], scheduleConcurrency[c]));
+    c.NetNodeOps = node_ops_by_name(*ip, net_ops[i].data());
+    c.NetOpsTotal = net[i].ops_total;
+    c.NetPartsMoved = net[i].parts_moved;
+    for (size_t k = 0; k < nc; ++k) {
+      c.NetSchedules.push_back(name_schedule(*ip, net_sched.out[i * nc + k], scheduleConcurrency[k]));
       if (exposure) {
-        nebuf[i * nc + c]->out = neout[i * nc + c];
-        res[i].NetExposures.push_back(name_exposure(*nebuf[i * nc + c], an.cap, an.eforest.names, ip->part_names));
+        nebuf[i * nc + k]->out = neout[i * nc + k];
+        c.NetExposures.push_back(name_exposure(*nebuf[i * nc + k], an.cap, an.eforest.names, ip->part_names));
       }
-      sbuf[i * nc + c]->out = sout[i * nc + c];
-      res[i].Span.push_back(name_span(*ip, *sbuf[i * nc + c], scheduleConcurrency[c], an.eforest.names));
+      if (i >= n) continue;
+      sbuf[i * nc + k]->out = sout[i * nc + k];
+      c.Span.push_back(name_span(*ip, *sbuf[i * nc + k], scheduleConcurrency[k], an.eforest.names));
     }
-  }
+    return c;
+  };
+  std::vector<ChainResult> res;
+  for (size_t i = 0; i < n; ++i) res.push_back(result(i, i * T, T, an));
+  if (branchResults) branchResults->clear();
+  for (size_t b = 0; b < nb; ++b) branchResults->push_back(result(n + b, n * T + b * TB, TB, ban));
   return res;
 }
 

@@ -229,6 +229,18 @@ struct Chain {
   std::vector<ChainStage> Stages;
 };
 
+// A what-if branch off a chain (blance_plan_chain_branches): it leaves chain `Chain` after its stage AfterStage (-1:
+// from the base map) and plans its own Stages there.  It is planned as stages AfterStage + 1, ... of its EQUIVALENT
+// CHAIN: chain Chain's Options and stages 0..AfterStage followed by Stages, so its option fields and default NodesAll
+// follow ChainStage's rules on that chain (stage 0's default starts from trunk stage AfterStage's members, or from the
+// universe when AfterStage is -1).  WantMaps: fill its stages' NextMap / NextWarnings.
+struct ChainBranch {
+  int Chain = 0;
+  int AfterStage = -1;
+  std::vector<ChainStage> Stages;
+  bool WantMaps = false;
+};
+
 // One chain's stages folded at one MaxConcurrentPartitionMovesPerNode (blance_chain_span_out), by node, partition and
 // metric name, nonzero entries only.  Rounds are global: stage t's rounds follow those of the stages before it.  The
 // exposure fields are filled with PlanNextMapChains' `exposure` only.
@@ -274,12 +286,18 @@ struct ChainResult {
 // of any stage of any chain; when some stage sets an option of its own the call is blance_plan_chains_ex.
 // A stage's ops only touch its own nodesAll when every node that leaves nodesAll was removed in an earlier stage, which
 // the default NodesAll rule guarantees; then the stage's schedule equals OrchestrateSchedule(nodesAll_t, ...).
+// branches (blance_plan_chain_branches; every branch has the same number of stages, >= 1): each branch's result goes
+// to (*branchResults)[b], shaped like a chain's (its Stages, the net of its equivalent chain; no Span), equal to the
+// matching stages of its equivalent chain planned as a chain of its own.  The slot ranges cover every branch stage's
+// constraints too; errors name "branch b, stage u".
 std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const PartitionMap& partitionsToAssign,
                                            const Strs& nodesAll, const PartitionModel& model,
                                            const PlanNextMapOptions& options, const std::vector<Chain>& chains,
                                            bool favorMinNodes, const std::vector<int>& wantMaps, int maxConcurrent,
                                            const std::vector<int>& scheduleConcurrency = {},
-                                           const ScenarioAudit* audit = nullptr, const ScenarioExposure* exposure = nullptr);
+                                           const ScenarioAudit* audit = nullptr, const ScenarioExposure* exposure = nullptr,
+                                           const std::vector<ChainBranch>* branches = nullptr,
+                                           std::vector<ChainResult>* branchResults = nullptr);
 
 struct NodeStateOp { std::string Node, State, Op; };   // moves.go:17-21
 

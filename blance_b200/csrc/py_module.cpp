@@ -484,6 +484,8 @@ PYBIND11_MODULE(_host, m) {
   // (a scenario tuple: its node sets, node weights and plan options of its own; nodes_all or None for the default)
   using PyStage = std::tuple<PyScenario, OptStrs>;
   using PyChain = std::tuple<PyScenario, std::vector<PyStage>>;
+  // branches: per branch (the chain it leaves, the stage after which it leaves (-1: the base), its stages, want maps)
+  using PyBranch = std::tuple<int, int, std::vector<PyStage>, bool>;
   m.def(
       "PlanNextMapChains",
       [to_scenarios](const PyPartitionMap& prev, const std::optional<PyPartitionMap>& assign, const Strs& nodes_all,
@@ -492,7 +494,7 @@ PYBIND11_MODULE(_host, m) {
                      const std::optional<IntMap>& pw, const std::optional<IntMap>& ss, const std::optional<IntMap>& nw,
                      const std::optional<StrMap>& nh, const std::optional<PyRules>& hr, int booster, int max_iterations,
                      int engine, const std::vector<int>& schedule_concurrency, const std::optional<bool>& audit,
-                     const std::optional<int>& exposure_series_cap) {
+                     const std::optional<int>& exposure_series_cap, const std::optional<std::vector<PyBranch>>& branches) {
         PlanNextMapOptions o = to_options(msc, pw, ss, nw, nh, hr, booster, max_iterations, engine);
         const PartitionMap prev_map = to_map(prev);
         const PartitionMap assign_map = assign ? to_map(*assign) : PartitionMap{};
@@ -500,11 +502,9 @@ PYBIND11_MODULE(_host, m) {
         aud.FailoverSpread = audit.value_or(false);
         ScenarioExposure expo;
         expo.SeriesCap = exposure_series_cap.value_or(0);
-        std::vector<Chain> cs;
-        for (const auto& c : chains) {
-          Chain ch;
-          ch.Options = to_scenarios({std::get<0>(c)})[0];
-          for (const auto& st : std::get<1>(c)) {
+        auto to_stages = [&](const std::vector<PyStage>& py_stages) {
+          std::vector<ChainStage> out;
+          for (const auto& st : py_stages) {
             Scenario sc = to_scenarios({std::get<0>(st)})[0];
             ChainStage s;
             s.NodesToRemove = std::move(sc.NodesToRemove);
@@ -516,19 +516,29 @@ PYBIND11_MODULE(_host, m) {
             s.NodeHierarchy = std::move(sc.NodeHierarchy);
             s.HierarchyRules = std::move(sc.HierarchyRules);
             s.NodesAll = std::get<1>(st);
-            ch.Stages.push_back(std::move(s));
+            out.push_back(std::move(s));
           }
+          return out;
+        };
+        std::vector<Chain> cs;
+        for (const auto& c : chains) {
+          Chain ch;
+          ch.Options = to_scenarios({std::get<0>(c)})[0];
+          ch.Stages = to_stages(std::get<1>(c));
           cs.push_back(std::move(ch));
         }
-        std::vector<ChainResult> res;
+        std::vector<ChainBranch> bs;
+        for (const auto& b : branches.value_or(std::vector<PyBranch>{}))
+          bs.push_back(ChainBranch{std::get<0>(b), std::get<1>(b), to_stages(std::get<2>(b)), std::get<3>(b)});
+        std::vector<ChainResult> res, bres;
         {
           py::gil_scoped_release rel;
           res = PlanNextMapChains(prev_map, assign ? assign_map : prev_map, nodes_all, to_model(model), o, cs, favor_min_nodes,
                                   want_maps, max_concurrent, schedule_concurrency, audit ? &aud : nullptr,
-                                  exposure_series_cap ? &expo : nullptr);
+                                  exposure_series_cap ? &expo : nullptr, branches ? &bs : nullptr, branches ? &bres : nullptr);
         }
-        py::list out;
-        for (const auto& c : res) {
+        // one chain's (or branch's) dict: its stages, its net and (a chain's, with a schedule) its span
+        auto chain_dict = [&](const ChainResult& c, bool with_span) {
           py::list stages;
           for (const auto& r : c.Stages) {
             py::dict d;
@@ -550,9 +560,11 @@ PYBIND11_MODULE(_host, m) {
           py::dict d;
           if (!schedule_concurrency.empty()) {
             net["schedules"] = schedules_list(c.NetSchedules);
-            py::list sp;
-            for (const auto& x : c.Span) sp.append(span_dict(x, exposure_series_cap.has_value()));
-            d["span"] = sp;
+            if (with_span) {
+              py::list sp;
+              for (const auto& x : c.Span) sp.append(span_dict(x, exposure_series_cap.has_value()));
+              d["span"] = sp;
+            }
           }
           if (exposure_series_cap) {
             py::list el;
@@ -561,9 +573,14 @@ PYBIND11_MODULE(_host, m) {
           }
           d["stages"] = stages;
           d["net"] = net;
-          out.append(d);
-        }
-        return out;
+          return d;
+        };
+        py::list out;
+        for (const auto& c : res) out.append(chain_dict(c, true));
+        if (!branches) return py::object(out);
+        py::list bout;
+        for (const auto& c : bres) bout.append(chain_dict(c, false));
+        return py::object(py::make_tuple(out, bout));
       },
       py::arg("prev_map"), py::arg("partitions_to_assign"), py::arg("nodes_all"), py::arg("model"), py::arg("chains"),
       py::arg("favor_min_nodes") = false, py::arg("want_maps") = std::vector<int>{}, py::arg("max_concurrent") = 0,
@@ -571,7 +588,7 @@ PYBIND11_MODULE(_host, m) {
       py::arg("state_stickiness") = py::none(), py::arg("node_weights") = py::none(), py::arg("node_hierarchy") = py::none(),
       py::arg("hierarchy_rules") = py::none(), py::arg("booster") = 0, py::arg("max_iterations") = 10, py::arg("engine") = 0,
       py::arg("schedule_concurrency") = std::vector<int>{}, py::arg("audit") = py::none(),
-      py::arg("exposure_series_cap") = py::none());
+      py::arg("exposure_series_cap") = py::none(), py::arg("branches") = py::none());
 
   // test hook: the blance_plan_in of scenario `index`, as an interned plan the CPU oracle can run
   m.def(

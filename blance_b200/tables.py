@@ -356,6 +356,75 @@ def _opts_struct(base, o, keep):
     return s
 
 
+def _chain_stage(base_tables, stage, st, keep):
+    """Fills the blance_chain_stage st from a stage dict of plan_chains."""
+    sc = scenario_tables(base_tables, {k: v for k, v in stage.items() if k != "node_in_all"})
+    for f in SCENARIO_FIELDS:
+        v = getattr(sc, f)
+        if f in ("add_is_nil", "has_node_weights"):
+            setattr(st.nodes, f, int(v))
+            continue
+        a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
+        keep.append(a)
+        setattr(st.nodes, f, a.ctypes.data if a.size else None)
+    m = np.ascontiguousarray(stage.get("node_in_all", np.ones(base_tables.n_nodes)), np.uint8)
+    keep.append(m)
+    st.node_in_all = m.ctypes.data if m.size else None
+
+
+class _ChainAnalysis:
+    """The schedule, audit and exposure outputs of the stages results[i][t] (option dicts opt_of(i, t)) and nets of one
+    chain call's items (its chains, or its branches); fill() hands the filled outputs back to the results and nets."""
+
+    def __init__(self, base_tables, results, nets, opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts):
+        nc = counts.size
+        self.results, self.nets, self.nc = results, nets, nc
+        self.stages = stages = [r for rs in results for r in rs]
+        for r in stages:
+            r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+            for s in r.schedules if not stage_arrays else ():
+                s.out.node_rounds = s.out.node_last_round = s.out.part_done_round = None
+        self.sch = (api.ScenarioScheduleOut * (len(stages) * nc))(*[s.out for r in stages for s in r.schedules])
+        self.net_sch = self.auds = self.exps = self.net_exps = self.expo = self.net_expo = None
+        if nets is not None:
+            for x in nets:
+                x.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+            self.net_sch = (api.ScenarioScheduleOut * (len(nets) * nc))(*[s.out for x in nets for s in x.schedules])
+        if audit is not None:
+            for i, rs in enumerate(results):
+                for t, r in enumerate(rs):
+                    x = scenario_tables(base_tables, {}, opt_of(i, t))
+                    r.audit = AuditResult(base_tables, _n_rules(x), n_dom, audit.get("n2n", False))
+            self.auds = (api.AuditOut * len(stages))(*[r.audit.out for r in stages])
+        if exposure is not None:
+            c = max(cap, 0) if stage_arrays else 0
+            self.expo = [[_ScenarioExposure(base_tables, V, c, dom and stage_arrays, parts and stage_arrays) for _ in counts] for _ in stages]
+            self.exps = (api.ExposureOut * (len(stages) * nc))(*[e.out for es in self.expo for e in es])
+            if nets is not None:
+                # one series_cap serves the stages and the net rebalance: 0 without per-stage arrays
+                self.net_expo = [[_ScenarioExposure(base_tables, V, c, dom, parts) for _ in counts] for _ in nets]
+                self.net_exps = (api.ExposureOut * (len(nets) * nc))(*[e.out for es in self.net_expo for e in es])
+
+    def fill(self):
+        nc = self.nc
+        for x, r in enumerate(self.stages):
+            for k, s in enumerate(r.schedules):
+                s.out = self.sch[x * nc + k]
+            if self.auds is not None:
+                r.audit.out = self.auds[x]
+            if self.exps is not None:
+                for k, e in enumerate(self.expo[x]):
+                    e.out = self.exps[x * nc + k]
+                r.exposures = [e.result() for e in self.expo[x]]
+        for i, x in enumerate(self.nets or ()):
+            for k, s in enumerate(x.schedules):
+                s.out = self.net_sch[i * nc + k]
+            if self.net_exps is not None:
+                for k, e in enumerate(self.net_expo[i]):
+                    e.out = self.net_exps[i * nc + k]
+                x.exposures = [e.result() for e in self.net_expo[i]]
+
+
 class Context:
     """A blance_ctx* (one per process/GPU)."""
 
@@ -518,7 +587,8 @@ class Context:
         return results
 
     def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True,
-                    schedule=None, node_has_mover=None, audit=None, exposure=None, span=False, stage_arrays=True, stage_opts=None):
+                    schedule=None, node_has_mover=None, audit=None, exposure=None, span=False, stage_arrays=True, stage_opts=None,
+                    branches=None):
         """blance_plan_chains: chains of cluster changes, each stage planned on the map the stage before produced.
         chains is a list of chains of equal length; a stage is a dict of SCENARIO_FIELDS and node_in_all ([n_nodes],
         missing = every node; missing scenario keys keep the base's value).  want_rows lists the (chain, stage) pairs
@@ -535,7 +605,14 @@ class Context:
 
         stage_opts (instead of opts: None, or an [n][T] nested list of the option dicts plan_scenarios takes per
         scenario) calls blance_plan_chains_ex: stage t of chain i plans with the base's options and the groups of
-        stage_opts[i][t], and its audit and exposure use them; with or without a schedule."""
+        stage_opts[i][t], and its audit and exposure use them; with or without a schedule.
+
+        branches (a list of dicts: "chain", "after_stage" (-1: from the base), "stages" (stage dicts as above, the same
+        number in every branch), "stage_opts" (None, or one option dict per stage) and "want_rows" (bool)) calls
+        blance_plan_chain_branches: each branch plans its stages on trunk chain `chain`'s map after stage after_stage,
+        as stages after_stage + 1, ... of that chain's stages 0..after_stage followed by the branch's would.  The return
+        then ends with (branch_results, branch_nets): branch_results[b][u] a ScenarioResult with the schedules, audit and
+        exposures the trunk's stages get, branch_nets[b] a ChainNet (None without net)."""
         if opts is not None and stage_opts is not None:
             raise ValueError("pass opts (per chain) or stage_opts (per stage), not both")
         if schedule is None:
@@ -556,30 +633,29 @@ class Context:
         keep, sts = [], (api.ChainStage * max(1, n * T))()
         for i, chain in enumerate(chains):
             for t, stage in enumerate(chain):
-                st = sts[i * T + t]
-                sc = scenario_tables(base_tables, {k: v for k, v in stage.items() if k != "node_in_all"})
-                for f in SCENARIO_FIELDS:
-                    v = getattr(sc, f)
-                    if f in ("add_is_nil", "has_node_weights"):
-                        setattr(st.nodes, f, int(v))
-                        continue
-                    a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
-                    keep.append(a)
-                    setattr(st.nodes, f, a.ctypes.data if a.size else None)
-                m = np.ascontiguousarray(stage.get("node_in_all", np.ones(base_tables.n_nodes)), np.uint8)
-                keep.append(m)
-                st.node_in_all = m.ctypes.data if m.size else None
+                _chain_stage(base_tables, stage, sts[i * T + t], keep)
         results = [[ScenarioResult(base_tables, (i, t) in want) for t in range(T)] for i in range(n)]
         outs = (api.ScenarioOut * max(1, n * T))(*[r.out for rs in results for r in rs])
         nets = [ChainNet(base_tables) for _ in range(n)] if net else None
         net_arr = (api.ChainOut * max(1, n))(*[x.out for x in nets]) if net else None
+        if branches is not None and opts is not None:     # the branch entry takes options per stage
+            stage_opts, opts = [[opts[i]] * T for i in range(n)], None
         if stage_opts is not None:
             if len(stage_opts) != n or any(len(so) != T for so in stage_opts):
                 raise ValueError("stage_opts must hold one option dict per stage of every chain")
             ops = (api.ScenarioOpts * max(1, n * T))(*[_opts_struct(base_tables, o, keep) for so in stage_opts for o in so])
         else:
             ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-        if schedule is None and stage_opts is not None:
+        b = None
+        if branches is not None:
+            b = self._branch_args(base_tables, branches, net, keep)
+            b_args, b_results, b_nets, _ = b
+        if schedule is None and branches is not None:
+            self._check(self.lib.blance_plan_chain_branches(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
+                                                            int(max_concurrent), 0, None, None, outs, net_arr, None, None, None, None, 0,
+                                                            None, None, None, None, *b_args, None, None, None, None, None),
+                        "blance_plan_chain_branches")
+        elif schedule is None and stage_opts is not None:
             self._check(self.lib.blance_plan_chains_ex(self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)),
                                                        int(max_concurrent), 0, None, None, outs, net_arr, None, None, None, None, 0,
                                                        None, None, None, None), "blance_plan_chains_ex")
@@ -593,83 +669,88 @@ class Context:
                 opt_of = lambda i, t: None if opts is None else opts[i]  # noqa: E731
             spans = self._chains_exposure(base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results,
                                           opt_of, stage_opts is not None, schedule, node_has_mover, audit, exposure, span,
-                                          stage_arrays, keep)
+                                          stage_arrays, keep, b)
         for i in range(n):
             for t in range(T):
                 results[i][t].out = outs[i * T + t]
             if net:
                 nets[i].out = net_arr[i]
-        return (results, nets, spans) if span else (results, nets)
+        ret = (results, nets, spans) if span else (results, nets)
+        if branches is None:
+            return ret
+        b_outs, b_net_arr = b_args[3], b_args[4]
+        TB = b_args[1]
+        for x, rs in enumerate(b_results):
+            for u, r in enumerate(rs):
+                r.out = b_outs[x * TB + u]
+            if net:
+                b_nets[x].out = b_net_arr[x]
+        return ret + (b_results, b_nets)
+
+    def _branch_args(self, base_tables, branches, net, keep):
+        """The branch arguments of blance_plan_chain_branches for plan_chains(branches=...): ([n_branches,
+        n_branch_stages, br, br_out, br_net], results [b][u], nets [b] or None, opt_of(b, u))."""
+        nb = len(branches)
+        TB = len(branches[0]["stages"]) if nb else 0
+        if any(len(x["stages"]) != TB for x in branches):
+            raise ValueError("every branch of one call has the same number of stages")
+        br = (api.ChainBranch * max(1, nb))()
+        for x, d in enumerate(branches):
+            sts = (api.ChainStage * max(1, TB))()
+            for u, stage in enumerate(d["stages"]):
+                _chain_stage(base_tables, stage, sts[u], keep)
+            keep.append(sts)
+            br[x].chain, br[x].after_stage, br[x].stages = int(d["chain"]), int(d["after_stage"]), ctypes.addressof(sts)
+            so = d.get("stage_opts")
+            if so is not None:
+                if len(so) != TB:
+                    raise ValueError("a branch's stage_opts must hold one option dict per stage")
+                ops = (api.ScenarioOpts * max(1, TB))(*[_opts_struct(base_tables, o, keep) for o in so])
+                keep.append(ops)
+                br[x].stage_opts = ctypes.addressof(ops)
+        results = [[ScenarioResult(base_tables, bool(d.get("want_rows"))) for _ in range(TB)] for d in branches]
+        outs = (api.ScenarioOut * max(1, nb * TB))(*[r.out for rs in results for r in rs])
+        nets = [ChainNet(base_tables) for _ in range(nb)] if net else None
+        net_arr = (api.ChainOut * max(1, nb))(*[x.out for x in nets]) if net else None
+        opt_of = lambda x, u: None if branches[x].get("stage_opts") is None else branches[x]["stage_opts"][u]  # noqa: E731
+        return [nb, TB, br, outs, net_arr], results, nets, opt_of
 
     def _chains_exposure(self, base_tables, base, n, T, sts, ops, favor_min_nodes, max_concurrent, outs, nets, net_arr, results, opt_of,
-                         per_stage, schedule, node_has_mover, audit, exposure, span, stage_arrays, keep):
+                         per_stage, schedule, node_has_mover, audit, exposure, span, stage_arrays, keep, branches=None):
         """The blance_plan_chains_exposure call of plan_chains (per_stage: blance_plan_chains_ex; opt_of(i, t) is the
-        option dict of chain i's stage t): fills the results' and nets' schedules, audits and exposures; returns the
-        spans (or None)."""
+        option dict of chain i's stage t; branches: the (args, results, nets, opt_of) of blance_plan_chain_branches):
+        fills the results' and nets' schedules, audits and exposures; returns the spans (or None)."""
         counts = np.ascontiguousarray(schedule, np.int32)
         nc = counts.size
         mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
         if mover is not None and mover.size != base_tables.n_node_ids:
             raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
-        stages = [r for rs in results for r in rs]
-        for r in stages:
-            r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
-            for s in r.schedules if not stage_arrays else ():
-                s.out.node_rounds = s.out.node_last_round = s.out.part_done_round = None
-        sch = (api.ScenarioScheduleOut * (n * T * nc))(*[s.out for r in stages for s in r.schedules])
-        net_sch = None
-        if nets is not None:
-            for x in nets:
-                x.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
-            net_sch = (api.ScenarioScheduleOut * (n * nc))(*[s.out for x in nets for s in x.schedules])
-        a_opts, auds = None, None
+        a_opts, n_dom, e_opts, cap, dom, parts, V = None, 0, None, 0, False, False, base_tables.n_node_ids
         if audit is not None:
             a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
-            for i in range(n):
-                for t, r in enumerate(results[i]):
-                    x = scenario_tables(base_tables, {}, opt_of(i, t))
-                    r.audit = AuditResult(base_tables, _n_rules(x), n_dom, audit.get("n2n", False))
-            auds = (api.AuditOut * (n * T))(*[r.audit.out for r in stages])
-        e_opts, exps, net_exps, expo, net_expo, cap = None, None, None, None, None, 0
-        dom = parts = False
-        V = base_tables.n_node_ids
         if exposure is not None:
             e_opts, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
             V += int(e_opts.n_domains)
             cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
-            expo = [[_ScenarioExposure(base_tables, V, max(cap, 0) if stage_arrays else 0, dom and stage_arrays, parts and stage_arrays)
-                     for _ in counts] for _ in stages]
-            exps = (api.ExposureOut * (n * T * nc))(*[e.out for es in expo for e in es])
-            if nets is not None:
-                # one series_cap serves the stages and the net rebalance: 0 without per-stage arrays
-                net_expo = [[_ScenarioExposure(base_tables, V, max(cap, 0) if stage_arrays else 0, dom, parts) for _ in counts] for _ in nets]
-                net_exps = (api.ExposureOut * (n * nc))(*[e.out for es in net_expo for e in es])
+        trunk = _ChainAnalysis(base_tables, results, nets, opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts)
         spans = [[_ChainSpan(base_tables, V, exposure is not None, dom, parts) for _ in counts] for _ in range(n)] if span else None
         span_arr = (api.ChainSpanOut * (n * nc))(*[s.out for ss in spans for s in ss]) if span else None
-        fn, what = (self.lib.blance_plan_chains_ex, "blance_plan_chains_ex") if per_stage else \
-            (self.lib.blance_plan_chains_exposure, "blance_plan_chains_exposure")
-        self._check(fn(
-            self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)), int(max_concurrent), nc, counts.ctypes.data,
-            None if mover is None else mover.ctypes.data, outs, net_arr, sch, None if audit is None else ctypes.byref(a_opts), auds,
-            ctypes.byref(e_opts) if exposure is not None and exposure.get("domain_parent") is not None else None,
-            cap if stage_arrays else 0, exps,
-            net_sch, net_exps, span_arr), what)
-        for x, r in enumerate(stages):
-            for k, s in enumerate(r.schedules):
-                s.out = sch[x * nc + k]
-            if auds is not None:
-                r.audit.out = auds[x]
-            if exps is not None:
-                for k, e in enumerate(expo[x]):
-                    e.out = exps[x * nc + k]
-                r.exposures = [e.result() for e in expo[x]]
-        for i, x in enumerate(nets or ()):
-            for k, s in enumerate(x.schedules):
-                s.out = net_sch[i * nc + k]
-            if net_exps is not None:
-                for k, e in enumerate(net_expo[i]):
-                    e.out = net_exps[i * nc + k]
-                x.exposures = [e.result() for e in net_expo[i]]
+        args = [self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)), int(max_concurrent), nc, counts.ctypes.data,
+                None if mover is None else mover.ctypes.data, outs, net_arr, trunk.sch,
+                None if audit is None else ctypes.byref(a_opts), trunk.auds,
+                ctypes.byref(e_opts) if exposure is not None and exposure.get("domain_parent") is not None else None,
+                cap if stage_arrays else 0, trunk.exps, trunk.net_sch, trunk.net_exps, span_arr]
+        if branches is not None:
+            b_args, b_results, b_nets, b_opt_of = branches
+            br = _ChainAnalysis(base_tables, b_results, b_nets, b_opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts)
+            self._check(self.lib.blance_plan_chain_branches(*args, *b_args, br.sch, br.auds, br.exps, br.net_sch, br.net_exps),
+                        "blance_plan_chain_branches")
+            br.fill()
+        else:
+            fn, what = (self.lib.blance_plan_chains_ex, "blance_plan_chains_ex") if per_stage else \
+                (self.lib.blance_plan_chains_exposure, "blance_plan_chains_exposure")
+            self._check(fn(*args), what)
+        trunk.fill()
         if not span:
             return None
         for i in range(n):

@@ -853,6 +853,61 @@ int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n
                           blance_exposure_out* net_expo /* [n][n_move_conc] or NULL, needs net and expo */,
                           blance_chain_span_out* span /* [n][n_move_conc] or NULL */);
 
+/* ---- what-if branches off the stages of a chain (blance_plan_chain_branches) ---------------------------------
+ * "What if node X fails after stage 2 of the rolling upgrade?" for every candidate failure and every stage, in one
+ * call: blance_plan_chains_ex for the trunk chains, plus branches that leave trunk chain `chain` after its stage
+ * `after_stage` and plan n_branch_stages stages of their own on that stage's final map.
+ *
+ * Branch b's EQUIVALENT CHAIN is trunk chain br[b].chain's stages 0..after_stage with their stage_opts, followed by
+ * the branch's stages and stage_opts.  br_out[b * n_branch_stages + u] and the matching br_sched / br_audit / br_expo
+ * entries equal stage after_stage + 1 + u of blance_plan_chains_ex on the equivalent chain, byte for byte; br_net,
+ * br_net_sched and br_net_expo equal that call's net, net_sched and net_expo.  after_stage = -1 branches from the base
+ * map (the branch is then a chain of its own).  Options are absolute, as in blance_plan_chains_ex: a branch stage with
+ * NULL options plans with the base's options, not the trunk stage's.  The trunk outputs equal blance_plan_chains_ex
+ * with the same trunk arguments byte for byte, and n_branches = 0 is that call.  One node_has_mover, move_conc,
+ * aopts, eopts and series_cap serve trunk and branches.  Nothing depends on n, max_concurrent, the wave size, the
+ * engine or the number of devices.
+ *
+ * The trunk prefix is planned once: after stage t of a trunk wave, the branches that leave its members there are
+ * forked from the wave's working map on the device (DESIGN.md section 17).  For T trunk stages and N one-stage branches
+ * after every stage that is T + N.T stage plans, against N.T(T+3)/2 when each equivalent chain is its own call.
+ *
+ * Errors, all before any device work: everything blance_plan_chains_ex rejects, with the checks of its stages run on
+ * each equivalent chain's branch stages and named "branch b, stage u"; n_branches < 0; n_branches > 0 with
+ * n_branch_stages < 1 or a NULL br, br_out or stages; chain outside [0, n) or after_stage outside [-1, n_stages);
+ * br_sched NULL with a schedule or given without one; br_expo without a schedule or without expo; br_net_expo without
+ * br_expo; br_net_sched or br_net_expo without br_net (BLANCE_ERR_INVALID_ARG).  With ctx NULL the call returns the
+ * first error, or BLANCE_ERR_INVALID_ARG for the NULL ctx.
+ *
+ * Not provided: spans for branches (the trunk's span is unchanged), branches of branches, and a mover set or
+ * favor_min_nodes of a branch's own. */
+typedef struct blance_chain_branch {
+  int32_t chain;                           /* the trunk chain it leaves, in [0, n) */
+  int32_t after_stage;                     /* -1: from the base map; t in [0, n_stages): from trunk stage t's final map */
+  const blance_chain_stage* stages;        /* [n_branch_stages] */
+  const blance_scenario_opts* stage_opts;  /* [n_branch_stages] or NULL (no option group set) */
+} blance_chain_branch;
+
+int blance_plan_chain_branches(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                               const blance_chain_stage* stages /* [n][n_stages] */,
+                               const blance_scenario_opts* stage_opts /* [n][n_stages] or NULL */, int32_t favor_min_nodes,
+                               int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                               blance_scenario_out* out /* [n][n_stages] */, blance_chain_out* net /* [n] or NULL */,
+                               blance_scenario_schedule_out* sched /* [n][n_stages][n_move_conc], or NULL without a schedule */,
+                               const blance_audit_opts* aopts, blance_audit_out* audit /* [n][n_stages] or NULL */,
+                               const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo /* [n][n_stages][n_move_conc] or NULL */,
+                               blance_scenario_schedule_out* net_sched /* [n][n_move_conc] or NULL, needs net */,
+                               blance_exposure_out* net_expo /* [n][n_move_conc] or NULL, needs net and expo */,
+                               blance_chain_span_out* span /* [n][n_move_conc] or NULL */,
+                               int32_t n_branches, int32_t n_branch_stages, const blance_chain_branch* br /* [n_branches] */,
+                               blance_scenario_out* br_out /* [n_branches][n_branch_stages] */,
+                               blance_chain_out* br_net /* [n_branches] or NULL */,
+                               blance_scenario_schedule_out* br_sched /* [n_branches][n_branch_stages][n_move_conc], or NULL without a schedule */,
+                               blance_audit_out* br_audit /* [n_branches][n_branch_stages] or NULL */,
+                               blance_exposure_out* br_expo /* [n_branches][n_branch_stages][n_move_conc] or NULL, needs expo */,
+                               blance_scenario_schedule_out* br_net_sched /* [n_branches][n_move_conc] or NULL, needs br_net */,
+                               blance_exposure_out* br_net_expo /* [n_branches][n_move_conc] or NULL, needs br_net and br_expo */);
+
 void blance_moves_free(blance_ctx* ctx, blance_moves* moves);
 
 #ifdef __cplusplus
