@@ -1076,12 +1076,6 @@ static blance_plan_in scenario_in(const blance_plan_in& base, const blance_scena
   return in;
 }
 
-// The options of item i at stage t (NULL opts: none).  per_stage = T: opts is [n][T], one per chain stage
-// (blance_plan_chains_ex); per_stage = 0: opts is [n], one per scenario or chain for all its stages.
-static const blance_scenario_opts* opts_at(const blance_scenario_opts* opts, int per_stage, int i, int t) {
-  return opts ? &opts[per_stage ? (size_t)i * per_stage + t : (size_t)i] : nullptr;
-}
-
 static int n_overrides(const blance_scenario_opts* o) {
   return o && (o->set & BLANCE_OPT_PART_WEIGHTS) ? o->n_weight_overrides : 0;
 }
@@ -1774,10 +1768,12 @@ static const blance_scenario& nodes_of(const WaveReq& q, int i, int t) {
   return q.cr ? chain_stage(q, i, t).nodes : q.sc[i];
 }
 
-// The plan options of scenario (or chain) i at stage t.
+// The plan options of scenario (or chain) i at stage t (NULL: none): opts is [n][T], one per chain stage, with
+// cr->stage_opts (blance_plan_chains_ex), else [n], one per scenario or chain for all its stages.
 static const blance_scenario_opts* opts_of(const WaveReq& q, int i, int t) {
   if (q.br) return q.br->br[i].stage_opts ? &q.br->br[i].stage_opts[t] : nullptr;
-  return opts_at(q.opts, q.cr && q.cr->stage_opts ? q.cr->T : 0, i, t);
+  if (!q.opts) return nullptr;
+  return &q.opts[q.cr && q.cr->stage_opts ? (size_t)i * q.cr->T + t : (size_t)i];
 }
 
 // The substituted instance of scenario / chain i at stage t.  A chain stage's node_removed is written in the device
@@ -2519,40 +2515,24 @@ static void plan_wave(blance_ctx* ctx, int32_t n, const WaveReq& q) {
   fan_out(ctx, G, [&](int d, blance_ctx* dev) { scenarios_on_device(dev, idx[(size_t)d], q); });
 }
 
-// Plans the n scenarios of q, each checked before the context is used: a NULL ctx checks them without a device.
-static void plan_scenarios(blance_ctx* ctx, const std::string& name, int32_t n, const WaveReq& q) {
-  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
-  if (!q.base || !q.sc || !q.out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, sc or out is NULL");
-  long long base_sum = -1;                // sum |w_p| of the base (1 without a weight), for the int32 bound
-  for (int i = 0; i < n; ++i) {
-    std::string why;
-    const int st = check_scenario(*q.base, q.sc[i], opts_of(q, i, 0), base_sum, why);
-    if (st != BLANCE_OK) throw_err(st, name + ": scenario " + std::to_string(i) + ": " + why);
-  }
-  plan_wave(ctx, n, q);
+// Item i of q in a message, with its stage t when t >= 0: "scenario i", "chain i, stage t" or "branch i, stage t".
+static std::string item_name(const WaveReq& q, long long i, int t = -1) {
+  return std::string(q.br ? "branch " : q.cr ? "chain " : "scenario ") + std::to_string(i) + (t >= 0 ? ", stage " + std::to_string(t) : "");
 }
 
-// The checks of the chains of stages over one base that blance_plan_chains, blance_plan_chains_exposure and
-// blance_plan_chains_ex plan; opts as opts_at() with per_stage (0, or n_stages for options per stage).
-static void check_chains(const std::string& name, const blance_plan_in* base, int32_t n, int32_t n_stages, const blance_chain_stage* stages,
-                         const blance_scenario_opts* opts, int per_stage, blance_scenario_out* out) {
-  if (n <= 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n must be positive");
-  if (n_stages < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_stages must be positive");
-  if (!base || !stages || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
-  if (n_stages > 1 && base->max_iters < 1)      // the stage would assign nothing and leave no next map to plan on
-    throw_err(BLANCE_ERR_INVALID_ARG, name + ": a chain of several stages needs max_iters >= 1");
-  // every stage is checked before the context is used, so a NULL ctx checks the chains without a device
-  long long base_sum = -1;
-  for (int i = 0; i < n; ++i)
-    for (int t = 0; t < n_stages; ++t) {
-      const blance_chain_stage& cs = stages[(size_t)i * n_stages + t];
-      std::string why;
-      int st = check_scenario(*base, cs.nodes, opts_at(opts, per_stage, i, t), base_sum, why);
-      if (st == BLANCE_OK && base->n_nodes > 0 && !cs.node_in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
-      for (int q = 0; st == BLANCE_OK && q < base->n_nodes; ++q)
-        if (cs.node_in_all[q] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
-      if (st != BLANCE_OK) throw_err(st, name + ": chain " + std::to_string(i) + ", stage " + std::to_string(t) + ": " + why);
-    }
+// The checks of stage t of item i of q (base_sum: see check_counts): its substituted instance and, for a chain or
+// branch stage, its node_in_all.
+static void check_stage(const std::string& name, const WaveReq& q, int i, int t, long long& base_sum) {
+  const blance_plan_in& base = *q.base;
+  std::string why;
+  int st = check_scenario(base, nodes_of(q, i, t), opts_of(q, i, t), base_sum, why);
+  if (q.cr) {
+    const uint8_t* in_all = chain_stage(q, i, t).node_in_all;
+    if (st == BLANCE_OK && base.n_nodes > 0 && !in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
+    for (int k = 0; st == BLANCE_OK && k < base.n_nodes; ++k)
+      if (in_all[k] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
+  }
+  if (st != BLANCE_OK) throw_err(st, name + ": " + item_name(q, i, q.cr ? t : -1) + ": " + why);
 }
 
 // The checked schedule request of n_move_conc / move_conc / node_has_mover over base; the scalars of the first n_clear
@@ -2575,15 +2555,14 @@ static SchedReq sched_req(const std::string& name, const blance_plan_in* base, l
   return sr;
 }
 
-// check_audit_model over the first stages of the n scenarios sc, or of the n chains `stages` (none while NULL); with
-// per_stage (opts [n][T], as opts_at) over every stage of every chain, naming "chain i, stage t".
-static void check_audit_models(const std::string& name, const blance_plan_in& base, int32_t n, const blance_scenario* sc,
-                               const blance_chain_stage* stages, int32_t T, const blance_scenario_opts* opts, int per_stage = 0) {
-  if (stages ? T < 1 : !sc) return;
+// check_audit_model over the stages of q's n items whose options can differ: every stage of a request with options
+// per stage, else the first.
+static void check_audit_models(const std::string& name, const WaveReq& q, int32_t n) {
+  const bool per_stage = q.cr && q.cr->stage_opts;
   for (int i = 0; i < n; ++i)
-    for (int t = 0; t < (per_stage ? T : 1); ++t) {
-      const blance_plan_in in = scenario_in(base, stages ? stages[(size_t)i * T + t].nodes : sc[i], opts_at(opts, per_stage, i, t));
-      check_audit_model(name + (stages ? ": chain " : ": scenario ") + std::to_string(i) + (per_stage ? ", stage " + std::to_string(t) : ""), &in);
+    for (int t = 0; t < (per_stage ? q.cr->T : 1); ++t) {
+      const blance_plan_in in = scenario_in(*q.base, nodes_of(q, i, t), opts_of(q, i, t));
+      check_audit_model(name + ": " + item_name(q, i, per_stage ? t : -1), &in);
     }
 }
 
@@ -2603,10 +2582,10 @@ static ExpoReq expo_req(const std::string& name, const blance_plan_in& base, con
   return ExpoReq{eopts ? eopts->n_domains : 0, eopts ? eopts->domain_parent : nullptr, series_cap, expo};
 }
 
-// The flags of the outputs asked for in the [n_out] `outs` (NULL: none) added to er, the event bound checked for each
-// that asks for dom peaks.  `what(x)` names output x in a message.
-template <class Name>
-static void expo_flags(const std::string& name, const blance_plan_in& base, const blance_exposure_out* outs, long long n_out, Name&& what,
+// The flags of the exposure outputs `outs` (NULL: none) of q's items added to er, the event bound checked for each that
+// asks for dom peaks.  outs holds n_out outputs [n][T][nc], or [n][nc] with T = 0 (a scenario's, or a chain's net
+// rebalance).
+static void expo_flags(const std::string& name, const WaveReq& q, const blance_exposure_out* outs, long long n_out, int T, int nc,
                        ExpoReq& er) {
   for (long long x = 0; outs && x < n_out; ++x) {
     const blance_exposure_out& o = outs[x];
@@ -2614,151 +2593,188 @@ static void expo_flags(const std::string& name, const blance_plan_in& base, cons
     er.part_min |= o.part_min_copies != nullptr;
     er.part_notop |= o.part_no_top != nullptr;
     er.part_flags |= o.part_flags != nullptr;
-    if (o.dom_peak || o.dom_peak_round) check_event_bound(name, what(x), base);
+    if (!o.dom_peak && !o.dom_peak_round) continue;
+    const std::string at = item_name(q, x / ((long long)std::max(T, 1) * nc), T > 0 ? (int)(x / nc % T) : -1);
+    check_event_bound(name, at + ", count " + std::to_string(x % nc), *q.base);
   }
 }
 
-extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
-                                  const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
-                                  int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
-  return entry(ctx, [&](Device&) {
-    check_chains("blance_plan_chains", base, n, n_stages, stages, opts, 0, out);
-    ChainReq cr;
-    cr.T = n_stages; cr.stages = stages; cr.net = net;
-    plan_wave(ctx, n, WaveReq{base, nullptr, opts, favor_min_nodes, max_concurrent, out, nullptr, nullptr, &cr});
-  });
-}
-
-// The branch arguments of blance_plan_chain_branches.
-struct BranchArgs {
-  int32_t n = 0, T = 0;
-  const blance_chain_branch* br = nullptr;
+// The arguments of a scenario or chain entry point: those of blance_plan_chain_branches, in its order, and the
+// scenarios sc.  A NULL pointer or a zero count is an argument the entry point does not take or the caller left out.
+struct WaveArgs {
+  const blance_plan_in* base = nullptr;
+  int32_t n = 0, n_stages = 0;
+  const blance_chain_stage* stages = nullptr;
+  const blance_scenario_opts* opts = nullptr;
+  int32_t favor_min = 0, max_concurrent = 0, n_move_conc = 0;
+  const int32_t* move_conc = nullptr;
+  const uint8_t* node_has_mover = nullptr;
   blance_scenario_out* out = nullptr;
   blance_chain_out* net = nullptr;
   blance_scenario_schedule_out* sched = nullptr;
+  const blance_audit_opts* aopts = nullptr;
   blance_audit_out* audit = nullptr;
+  const blance_audit_opts* eopts = nullptr;
+  int32_t series_cap = 0;
   blance_exposure_out* expo = nullptr;
   blance_scenario_schedule_out* net_sched = nullptr;
   blance_exposure_out* net_expo = nullptr;
+  blance_chain_span_out* span = nullptr;
+  int32_t n_branches = 0, n_branch_stages = 0;
+  const blance_chain_branch* br = nullptr;
+  blance_scenario_out* br_out = nullptr;
+  blance_chain_out* br_net = nullptr;
+  blance_scenario_schedule_out* br_sched = nullptr;
+  blance_audit_out* br_audit = nullptr;
+  blance_exposure_out* br_expo = nullptr;
+  blance_scenario_schedule_out* br_net_sched = nullptr;
+  blance_exposure_out* br_net_expo = nullptr;
+  const blance_scenario* sc = nullptr;
 };
 
-// The checks of the branches a of the trunk request q (its n chains of n_stages stages, checked), run on each
-// equivalent chain's branch stages, and their request in b (q.forks set to it).  aopts as the trunk's.
-static void check_branches(const std::string& name, WaveReq& q, int32_t n, int32_t n_stages, const blance_audit_opts* aopts,
-                           const BranchArgs& a, BranchReq& b) {
+// Whether an entry point takes an analysis: never, always, or when the caller asks for it (an audit or an exposure
+// with its output; a schedule unless n_move_conc is 0 and move_conc and sched are NULL).
+enum Takes { NEVER, ALWAYS, MAY };
+
+// When an entry point reports a NULL context: before any other check, through need_ctx after the checks of its
+// analyses, or at the fan-out after every check.
+enum NullCtx { CTX_FIRST, CTX_NEED, CTX_FAN_OUT };
+
+// How one scenario or chain entry point differs from the others.
+struct Entry {
+  const char* name;
+  bool chains;                         // the items are chains of n_stages stages, not scenarios
+  bool stage_opts;                     // opts is [n][n_stages], one per stage, not [n]
+  Takes sched, audit, expo;
+  bool branches;
+  NullCtx null_ctx;
+};
+
+// The branches of the chain request q (its chains checked) in b, and q.forks set to them: the branch arguments' own
+// checks, each branch's stages checked as a chain's, and its schedule, audit and exposure requests built as the
+// trunk's, with the trunk's counts, movers, audit options and forest.
+static void check_branches(const std::string& name, const WaveArgs& a, WaveReq& q, BranchReq& b) {
+  auto bad = [&](const std::string& what) { throw_err(BLANCE_ERR_INVALID_ARG, name + ": " + what); };
   const blance_plan_in& base = *q.base;
-  if (a.n < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_branches is negative");
-  if (a.n == 0) return;
-  if (a.T < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_branch_stages must be positive");
-  if (!a.br || !a.out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br or br_out is NULL");
-  if ((a.net_sched || a.net_expo) && !a.net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_net_sched and br_net_expo need br_net");
-  if (!q.sr && (a.sched || a.expo || a.net_sched || a.net_expo))
-    throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_sched, br_expo, br_net_sched and br_net_expo need a schedule");
-  if (q.sr && !a.sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_sched is NULL with a schedule");
-  if ((a.expo && !q.er) || (a.net_expo && !a.expo)) throw_err(BLANCE_ERR_INVALID_ARG, name + ": br_expo needs expo and br_net_expo needs br_expo");
-  long long base_sum = -1;
-  for (int x = 0; x < a.n; ++x) {
-    const blance_chain_branch& br = a.br[x];
-    const std::string at = name + ": branch " + std::to_string(x);
-    if (!br.stages) throw_err(BLANCE_ERR_INVALID_ARG, at + ": stages is NULL");
-    if (br.chain < 0 || br.chain >= n) throw_err(BLANCE_ERR_INVALID_ARG, at + ": chain outside [0, n)");
-    if (br.after_stage < -1 || br.after_stage >= n_stages) throw_err(BLANCE_ERR_INVALID_ARG, at + ": after_stage outside [-1, n_stages)");
-    if (br.after_stage + 1 + a.T > 1 && base.max_iters < 1)
-      throw_err(BLANCE_ERR_INVALID_ARG, at + ": a chain of several stages needs max_iters >= 1");
-    for (int u = 0; u < a.T; ++u) {     // the checks check_chains makes of a chain stage
-      const blance_chain_stage& cs = br.stages[u];
-      std::string why;
-      int st = check_scenario(base, cs.nodes, br.stage_opts ? &br.stage_opts[u] : nullptr, base_sum, why);
-      if (st == BLANCE_OK && base.n_nodes > 0 && !cs.node_in_all) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is NULL"; }
-      for (int k = 0; st == BLANCE_OK && k < base.n_nodes; ++k)
-        if (cs.node_in_all[k] > 1) { st = BLANCE_ERR_INVALID_ARG; why = "node_in_all is neither 0 nor 1"; }
-      if (st != BLANCE_OK) throw_err(st, at + ", stage " + std::to_string(u) + ": " + why);
-    }
-  }
-  b.n = a.n; b.br = a.br; b.trunk = &q;
-  b.cr.T = a.T; b.cr.stage_opts = true; b.cr.net = a.net; b.cr.net_sched = a.net_sched; b.cr.net_expo = a.net_expo;
-  b.q = WaveReq{q.base, nullptr, nullptr, q.favor_min, q.max_concurrent, a.out, nullptr, nullptr, &b.cr};
+  const int TB = a.n_branch_stages, nc = a.n_move_conc;
+  if (a.n_branches < 0) bad("n_branches is negative");
+  if (a.n_branches == 0) return;
+  if (TB < 1) bad("n_branch_stages must be positive");
+  if (!a.br || !a.br_out) bad("br or br_out is NULL");
+  if ((a.br_net_sched || a.br_net_expo) && !a.br_net) bad("br_net_sched and br_net_expo need br_net");
+  if (!q.sr && (a.br_sched || a.br_expo || a.br_net_sched || a.br_net_expo))
+    bad("br_sched, br_expo, br_net_sched and br_net_expo need a schedule");
+  if (q.sr && !a.br_sched) bad("br_sched is NULL with a schedule");
+  if ((a.br_expo && !q.er) || (a.br_net_expo && !a.br_expo)) bad("br_expo needs expo and br_net_expo needs br_expo");
+  b.n = a.n_branches; b.br = a.br; b.trunk = &q;
+  b.cr = ChainReq{TB, true, nullptr, a.br_net, a.br_net_sched, a.br_net_expo};
+  b.q = WaveReq{q.base, nullptr, nullptr, q.favor_min, q.max_concurrent, a.br_out, nullptr, nullptr, &b.cr};
   b.q.br = &b;
-  if (a.audit) {
-    b.ar = check_audit_opts(name, aopts, base.n_node_ids, a.audit);
-    for (int x = 0; x < a.n; ++x)
-      for (int u = 0; u < a.T; ++u) {
-        const blance_plan_in in = scenario_in(base, a.br[x].stages[u].nodes, opts_of(b.q, x, u));
-        check_audit_model(name + ": branch " + std::to_string(x) + ", stage " + std::to_string(u), &in);
-      }
-    b.q.ar = &b.ar;
+  long long base_sum = -1;
+  for (int x = 0; x < b.n; ++x) {
+    const blance_chain_branch& br = a.br[x];
+    const std::string at = item_name(b.q, x) + ": ";
+    if (!br.stages) bad(at + "stages is NULL");
+    if (br.chain < 0 || br.chain >= a.n) bad(at + "chain outside [0, n)");
+    if (br.after_stage < -1 || br.after_stage >= a.n_stages) bad(at + "after_stage outside [-1, n_stages)");
+    if (br.after_stage + 1 + TB > 1 && base.max_iters < 1) bad(at + "a chain of several stages needs max_iters >= 1");
+    for (int u = 0; u < TB; ++u) check_stage(name, b.q, x, u, base_sum);
   }
-  const int nc = q.sr ? q.sr->nc : 0;
+  if (a.br_audit) {
+    b.ar = check_audit_opts(name, a.aopts, base.n_node_ids, a.br_audit);
+    b.q.ar = &b.ar;
+    check_audit_models(name, b.q, b.n);
+  }
   if (q.sr) {
-    b.sr = *q.sr;
-    b.sr.out = a.sched;
-    for (long long x = 0; x < (long long)a.n * a.T * nc; ++x) { a.sched[x].rounds = 0; a.sched[x].moves_done = 0; a.sched[x].stuck_parts = 0; a.sched[x].max_batch = 0; }
+    b.sr = sched_req(name, &base, (long long)b.n * TB * nc, nc, a.move_conc, a.node_has_mover, a.br_sched);
     b.q.sr = &b.sr;
   }
-  if (a.expo) {
-    b.er = ExpoReq{q.er->n_domains, q.er->parent, q.er->series_cap, a.expo};
-    auto stage_name = [&](long long x) {
-      return "branch " + std::to_string(x / ((long long)a.T * nc)) + ", stage " + std::to_string(x / nc % a.T) + ", count " + std::to_string(x % nc);
-    };
-    auto pair_name = [&](long long x) { return "branch " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
-    expo_flags(name, base, a.expo, (long long)a.n * a.T * nc, stage_name, b.er);
-    expo_flags(name, base, a.net_expo, (long long)a.n * nc, pair_name, b.er);
+  if (a.br_expo) {
+    b.er = expo_req(name, base, a.eopts, a.series_cap, a.br_expo);
+    expo_flags(name, b.q, a.br_expo, (long long)b.n * TB * nc, TB, nc, b.er);
+    expo_flags(name, b.q, a.br_net_expo, (long long)b.n * nc, 0, nc, b.er);
     b.q.er = &b.er;
   }
   q.forks = &b;
 }
 
-// blance_plan_chains_exposure (opts [n]) and blance_plan_chains_ex (stage_opts: opts [n][n_stages], and the schedule
-// may be left out: n_move_conc 0 with move_conc and sched NULL plans and audits without one); with ba the branches of
-// blance_plan_chain_branches.
-static void plan_chains_analysed(blance_ctx* ctx, const std::string& name, bool stage_opts, const blance_plan_in* base, int32_t n,
-                                 int32_t n_stages, const blance_chain_stage* stages, const blance_scenario_opts* opts,
-                                 int32_t favor_min_nodes, int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
-                                 const uint8_t* node_has_mover, blance_scenario_out* out, blance_chain_out* net,
-                                 blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
-                                 const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
-                                 blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span,
-                                 const BranchArgs* ba = nullptr) {
-  if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base, stages or out is NULL");
-  const int T = n_stages, nc = n_move_conc, per_stage = stage_opts ? T : 0;
-  if ((net_sched || net_expo) && !net) throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_sched and net_expo need net");
-  AuditReq ar;
-  if (audit) {
-    ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
-    check_audit_models(name, *base, n, nullptr, stages, T, opts, per_stage);
-  }
-  const bool no_sched = stage_opts && n_move_conc == 0 && !move_conc && !sched;
-  if (no_sched && (expo || net_sched || net_expo || span))
-    throw_err(BLANCE_ERR_INVALID_ARG, name + ": expo, net_sched, net_expo and span need a schedule");
-  SchedReq sr;
-  if (!no_sched) {
-    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": n_move_conc must be positive");
-    sr = sched_req(name, base, (long long)std::max(0, n) * std::max(0, T) * nc, n_move_conc, move_conc, node_has_mover, sched);
-  }
-  ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
-  ChainReq cr;
-  cr.T = T; cr.stage_opts = stage_opts; cr.stages = stages; cr.net = net; cr.net_sched = net_sched; cr.net_expo = net_expo; cr.span = span;
-  for (long long x = 0; span && x < (long long)std::max(0, n) * nc; ++x) {
-    const blance_chain_span_out& s = span[x];
-    cr.span_parts |= s.part_min_copies || s.part_no_top || s.part_flags;
-    cr.span_dom |= s.dom_peak || s.dom_peak_stage || s.dom_peak_round;
-  }
-  if (!expo && (net_expo || cr.span_parts || cr.span_dom))
-    throw_err(BLANCE_ERR_INVALID_ARG, name + ": net_expo and the span's exposure arrays need expo");
-  auto stage_name = [&](long long x) {
-    return "chain " + std::to_string(x / ((long long)T * nc)) + ", stage " + std::to_string(x / nc % T) + ", count " + std::to_string(x % nc);
-  };
-  auto pair_name = [&](long long x) { return "chain " + std::to_string(x / nc) + ", count " + std::to_string(x % nc); };
-  expo_flags(name, *base, expo, (long long)std::max(0, n) * std::max(0, T) * nc, stage_name, er);
-  expo_flags(name, *base, net_expo, (long long)std::max(0, n) * nc, pair_name, er);
-  if (cr.span_dom) check_event_bound(name, "span", *base);
-  er.dom |= cr.span_dom;
-  er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
-  check_chains(name, base, n, n_stages, stages, opts, per_stage, out);
-  WaveReq q{base, nullptr, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, audit ? &ar : nullptr, &cr, expo ? &er : nullptr};
-  BranchReq br;
-  if (ba) check_branches(name, q, n, n_stages, aopts, *ba, br);
-  plan_wave(ctx, n, q);
+// Entry point e on the arguments a: every check, in one order for all entry points, then the wave.  Only e decides
+// which checks run and when a NULL ctx is reported; every other check runs before the context is used, so a NULL
+// ctx checks a call without a device.
+static int plan_request(blance_ctx* ctx, const Entry& e, const WaveArgs& a) {
+  return entry(ctx, [&](Device&) {
+    const std::string name = e.name;
+    auto bad = [&](const std::string& what) { throw_err(BLANCE_ERR_INVALID_ARG, name + ": " + what); };
+    if (e.null_ctx == CTX_FIRST && !ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
+    // the checks of an audit or an exposure read the base
+    if ((e.audit != NEVER || e.expo != NEVER) && !a.base) bad(e.chains ? "base, stages or out is NULL" : "base is NULL");
+    if ((a.net_sched || a.net_expo) && !a.net) bad("net_sched and net_expo need net");
+    const int T = e.chains ? a.n_stages : 1;
+    const long long n = std::max(0, a.n), nc = a.n_move_conc;
+    ChainReq cr{T, e.stage_opts, a.stages, a.net, a.net_sched, a.net_expo, a.span};
+    WaveReq q{a.base, a.sc, a.opts, a.favor_min, a.max_concurrent, a.out};
+    if (e.chains) q.cr = &cr;
+    AuditReq ar;
+    if (e.audit == ALWAYS || (e.audit == MAY && a.audit)) {
+      ar = check_audit_opts(name, a.aopts, a.base->n_node_ids, a.audit);
+      q.ar = &ar;
+    }
+    // a chain's audit models are checked before its schedule request, a scenario's after its exposure request
+    auto audit_models = [&] { if (q.ar && (e.chains ? a.stages && T >= 1 : a.sc != nullptr)) check_audit_models(name, q, a.n); };
+    if (e.chains) audit_models();
+    SchedReq sr;
+    const bool no_sched = e.sched == MAY && a.n_move_conc == 0 && !a.move_conc && !a.sched;
+    if (no_sched && (a.expo || a.net_sched || a.net_expo || a.span)) bad("expo, net_sched, net_expo and span need a schedule");
+    if (e.sched != NEVER && !no_sched) {
+      if (e.expo != NEVER && a.n_move_conc < 1)
+        bad(std::string(e.expo == ALWAYS ? "an exposure needs a schedule: " : "") + "n_move_conc must be positive");
+      sr = sched_req(name, a.base, e.chains || (a.sc && a.out) ? n * std::max(0, T) * nc : 0, a.n_move_conc, a.move_conc, a.node_has_mover,
+                     a.sched);
+      q.sr = &sr;
+    }
+    ExpoReq er;
+    if (e.expo != NEVER) {
+      if (e.expo == ALWAYS && !a.expo) bad("expo is NULL");
+      er = expo_req(name, *a.base, a.eopts, a.series_cap, a.expo);
+    }
+    if (!e.chains) audit_models();
+    if (e.expo != NEVER) {
+      for (long long x = 0; a.span && x < n * nc; ++x) {
+        const blance_chain_span_out& s = a.span[x];
+        cr.span_parts |= s.part_min_copies || s.part_no_top || s.part_flags;
+        cr.span_dom |= s.dom_peak || s.dom_peak_stage || s.dom_peak_round;
+      }
+      if (!a.expo && (a.net_expo || cr.span_parts || cr.span_dom)) bad("net_expo and the span's exposure arrays need expo");
+      expo_flags(name, q, a.expo, n * std::max(0, T) * nc, e.chains ? T : 0, (int)nc, er);
+      expo_flags(name, q, a.net_expo, n * nc, 0, (int)nc, er);
+      if (cr.span_dom) check_event_bound(name, "span", *a.base);
+      er.dom |= cr.span_dom;
+      er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
+      if (a.expo) q.er = &er;
+    }
+    if (e.null_ctx == CTX_NEED) need_ctx(ctx);
+    if (a.n <= 0) bad("n must be positive");
+    if (e.chains && a.n_stages < 1) bad("n_stages must be positive");
+    if (!a.base || !(e.chains ? (const void*)a.stages : a.sc) || !a.out)
+      bad(e.chains ? "base, stages or out is NULL" : "base, sc or out is NULL");
+    if (T > 1 && a.base->max_iters < 1)      // the stage would assign nothing and leave no next map to plan on
+      bad("a chain of several stages needs max_iters >= 1");
+    long long base_sum = -1;                 // sum |w_p| of the base (1 without a weight), for the int32 bound
+    for (int i = 0; i < a.n; ++i)
+      for (int t = 0; t < T; ++t) check_stage(name, q, i, t, base_sum);
+    BranchReq b;
+    if (e.branches) check_branches(name, a, q, b);
+    plan_wave(ctx, a.n, q);
+  });
+}
+
+extern "C" int blance_plan_chains(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
+                                  const blance_chain_stage* stages, const blance_scenario_opts* opts, int32_t favor_min_nodes,
+                                  int32_t max_concurrent, blance_scenario_out* out, blance_chain_out* net) {
+  WaveArgs a;
+  a.base = base; a.n = n; a.n_stages = n_stages; a.stages = stages; a.opts = opts;
+  a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent; a.out = out; a.net = net;
+  return plan_request(ctx, Entry{"blance_plan_chains", true, false, NEVER, NEVER, NEVER, false, CTX_FAN_OUT}, a);
 }
 
 extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
@@ -2769,13 +2785,12 @@ extern "C" int blance_plan_chains_exposure(blance_ctx* ctx, const blance_plan_in
                                            const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
                                            blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo,
                                            blance_chain_span_out* span) {
-  return entry(ctx, [&](Device&) {
-    plan_chains_analysed(ctx, "blance_plan_chains_exposure", false, base, n, n_stages, stages, opts, favor_min_nodes, max_concurrent,
-                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
-                         net_expo, span);
-  });
+  const WaveArgs a{base, n, n_stages, stages, opts, favor_min_nodes, max_concurrent, n_move_conc, move_conc, node_has_mover, out,
+                   net, sched, aopts, audit, eopts, series_cap, expo, net_sched, net_expo, span};
+  return plan_request(ctx, Entry{"blance_plan_chains_exposure", true, false, ALWAYS, MAY, MAY, false, CTX_FAN_OUT}, a);
 }
 
+// the schedule may be left out: n_move_conc 0 with move_conc and sched NULL plans and audits without one
 extern "C" int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
                                      const blance_chain_stage* stages, const blance_scenario_opts* stage_opts, int32_t favor_min_nodes,
                                      int32_t max_concurrent, int32_t n_move_conc, const int32_t* move_conc,
@@ -2783,11 +2798,9 @@ extern "C" int blance_plan_chains_ex(blance_ctx* ctx, const blance_plan_in* base
                                      blance_scenario_schedule_out* sched, const blance_audit_opts* aopts, blance_audit_out* audit,
                                      const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
                                      blance_scenario_schedule_out* net_sched, blance_exposure_out* net_expo, blance_chain_span_out* span) {
-  return entry(ctx, [&](Device&) {
-    plan_chains_analysed(ctx, "blance_plan_chains_ex", true, base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent,
-                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
-                         net_expo, span);
-  });
+  const WaveArgs a{base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent, n_move_conc, move_conc, node_has_mover,
+                   out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched, net_expo, span};
+  return plan_request(ctx, Entry{"blance_plan_chains_ex", true, true, MAY, MAY, MAY, false, CTX_FAN_OUT}, a);
 }
 
 extern "C" int blance_plan_chain_branches(blance_ctx* ctx, const blance_plan_in* base, int32_t n, int32_t n_stages,
@@ -2801,39 +2814,35 @@ extern "C" int blance_plan_chain_branches(blance_ctx* ctx, const blance_plan_in*
                                           blance_scenario_out* br_out, blance_chain_out* br_net, blance_scenario_schedule_out* br_sched,
                                           blance_audit_out* br_audit, blance_exposure_out* br_expo,
                                           blance_scenario_schedule_out* br_net_sched, blance_exposure_out* br_net_expo) {
-  return entry(ctx, [&](Device&) {
-    const BranchArgs ba{n_branches, n_branch_stages, br, br_out, br_net, br_sched, br_audit, br_expo, br_net_sched, br_net_expo};
-    plan_chains_analysed(ctx, "blance_plan_chain_branches", true, base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent,
-                         n_move_conc, move_conc, node_has_mover, out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched,
-                         net_expo, span, &ba);
-  });
+  const WaveArgs a{base, n, n_stages, stages, stage_opts, favor_min_nodes, max_concurrent, n_move_conc, move_conc, node_has_mover,
+                   out, net, sched, aopts, audit, eopts, series_cap, expo, net_sched, net_expo, span, n_branches, n_branch_stages,
+                   br, br_out, br_net, br_sched, br_audit, br_expo, br_net_sched, br_net_expo};
+  return plan_request(ctx, Entry{"blance_plan_chain_branches", true, true, MAY, MAY, MAY, true, CTX_FAN_OUT}, a);
 }
 
 extern "C" int blance_plan_scenarios(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                      int32_t favor_min_nodes, int32_t max_concurrent, blance_scenario_out* out) {
-  return entry(ctx, [&](Device&) {
-    plan_scenarios(ctx, "blance_plan_scenarios", n, WaveReq{base, sc, nullptr, favor_min_nodes, max_concurrent, out});
-  });
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent; a.out = out;
+  return plan_request(ctx, Entry{"blance_plan_scenarios", false, false, NEVER, NEVER, NEVER, false, CTX_FAN_OUT}, a);
 }
 
 extern "C" int blance_plan_scenarios_ex(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                         const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                         blance_scenario_out* out) {
-  return entry(ctx, [&](Device&) {
-    plan_scenarios(ctx, "blance_plan_scenarios_ex", n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out});
-  });
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.opts = opts; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent; a.out = out;
+  return plan_request(ctx, Entry{"blance_plan_scenarios_ex", false, false, NEVER, NEVER, NEVER, false, CTX_FAN_OUT}, a);
 }
 
 extern "C" int blance_plan_scenarios_schedule(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
                                               const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
                                               int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
                                               blance_scenario_out* out, blance_scenario_schedule_out* sched) {
-  return entry(ctx, [&](Device&) {
-    const std::string name = "blance_plan_scenarios_schedule";
-    if (!ctx) throw_err(BLANCE_ERR_INVALID_ARG, "ctx is NULL");
-    const SchedReq sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
-    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, &sr});
-  });
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.opts = opts; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent;
+  a.n_move_conc = n_move_conc; a.move_conc = move_conc; a.node_has_mover = node_has_mover; a.out = out; a.sched = sched;
+  return plan_request(ctx, Entry{"blance_plan_scenarios_schedule", false, false, ALWAYS, NEVER, NEVER, false, CTX_FIRST}, a);
 }
 
 extern "C" int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
@@ -2841,17 +2850,11 @@ extern "C" int blance_plan_scenarios_audit(blance_ctx* ctx, const blance_plan_in
                                            int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
                                            blance_scenario_out* out, blance_scenario_schedule_out* sched,
                                            const blance_audit_opts* aopts, blance_audit_out* audit) {
-  return entry(ctx, [&](Device&) {
-    const std::string name = "blance_plan_scenarios_audit";
-    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base is NULL");
-    const AuditReq ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
-    const bool no_sched = n_move_conc == 0 && !move_conc && !sched;
-    SchedReq sr;
-    if (!no_sched) sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
-    check_audit_models(name, *base, n, sc, nullptr, 0, opts);
-    need_ctx(ctx);
-    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, no_sched ? nullptr : &sr, &ar});
-  });
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.opts = opts; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent;
+  a.n_move_conc = n_move_conc; a.move_conc = move_conc; a.node_has_mover = node_has_mover; a.out = out; a.sched = sched;
+  a.aopts = aopts; a.audit = audit;
+  return plan_request(ctx, Entry{"blance_plan_scenarios_audit", false, false, MAY, ALWAYS, NEVER, false, CTX_NEED}, a);
 }
 
 extern "C" int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
@@ -2860,21 +2863,11 @@ extern "C" int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan
                                               blance_scenario_out* out, blance_scenario_schedule_out* sched,
                                               const blance_audit_opts* aopts, blance_audit_out* audit,
                                               const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo) {
-  return entry(ctx, [&](Device&) {
-    const std::string name = "blance_plan_scenarios_exposure";
-    if (!base) throw_err(BLANCE_ERR_INVALID_ARG, name + ": base is NULL");
-    AuditReq ar;
-    if (audit) ar = check_audit_opts(name, aopts, base->n_node_ids, audit);
-    if (n_move_conc < 1) throw_err(BLANCE_ERR_INVALID_ARG, name + ": an exposure needs a schedule: n_move_conc must be positive");
-    const SchedReq sr = sched_req(name, base, sc && out ? (long long)n * n_move_conc : 0, n_move_conc, move_conc, node_has_mover, sched);
-    if (!expo) throw_err(BLANCE_ERR_INVALID_ARG, name + ": expo is NULL");
-    ExpoReq er = expo_req(name, *base, eopts, series_cap, expo);
-    if (audit) check_audit_models(name, *base, n, sc, nullptr, 0, opts);
-    auto pair_name = [&](long long x) { return "scenario " + std::to_string(x / n_move_conc) + ", count " + std::to_string(x % n_move_conc); };
-    expo_flags(name, *base, expo, (long long)std::max(0, n) * n_move_conc, pair_name, er);
-    // plan_scenarios checks every scenario before it looks at the context
-    plan_scenarios(ctx, name, n, WaveReq{base, sc, opts, favor_min_nodes, max_concurrent, out, &sr, audit ? &ar : nullptr, nullptr, &er});
-  });
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.opts = opts; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent;
+  a.n_move_conc = n_move_conc; a.move_conc = move_conc; a.node_has_mover = node_has_mover; a.out = out; a.sched = sched;
+  a.aopts = aopts; a.audit = audit; a.eopts = eopts; a.series_cap = series_cap; a.expo = expo;
+  return plan_request(ctx, Entry{"blance_plan_scenarios_exposure", false, false, ALWAYS, MAY, ALWAYS, false, CTX_FAN_OUT}, a);
 }
 
 // blance_map_audit / blance_plan_audit: one audit on buffers of its own.

@@ -1682,6 +1682,8 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
   for (size_t b = 0; b < nb; ++b)
     br[b] = blance_chain_branch{(*branches)[b].Chain, (*branches)[b].AfterStage, stages.data() + n * T + b * TB, opts.data() + n * T + b * TB};
   blance_ctx* ctx = DefaultContext();
+  // options per stage, or a schedule with options per chain: the two entry points take the same arguments
+  auto* const analysed = stage_opts ? blance_plan_chains_ex : blance_plan_chains_exposure;
   const int st = nb ? blance_plan_chain_branches(
                           ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
                           int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(), net.data(),
@@ -1691,20 +1693,14 @@ std::vector<ChainResult> PlanNextMapChains(const PartitionMap& prevMap, const Pa
                           out.data() + n * T, net.data() + n, nc ? ban.sched.out.data() : nullptr, audit ? ban.aout.data() : nullptr,
                           exposure ? ban.eout.data() : nullptr, nc ? net_sched.out.data() + n * nc : nullptr,
                           exposure ? neout.data() + n * nc : nullptr)
-                 : stage_opts
-                     ? blance_plan_chains_ex(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
-                                             maxConcurrent, int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(),
-                                             net.data(), nc ? an.sched.out.data() : nullptr, audit ? &an.forest.opts : nullptr,
-                                             audit ? an.aout.data() : nullptr, &an.eforest.opts, int32_t(an.cap),
-                                             exposure ? an.eout.data() : nullptr, nc ? net_sched.out.data() : nullptr,
-                                             exposure ? neout.data() : nullptr, nc ? sout.data() : nullptr)
-                 : nc ? blance_plan_chains_exposure(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
-                                                  maxConcurrent, int32_t(nc), scheduleConcurrency.data(), nullptr, out.data(), net.data(),
-                                                  an.sched.out.data(), audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr,
-                                                  &an.eforest.opts, int32_t(an.cap), exposure ? an.eout.data() : nullptr, net_sched.out.data(),
-                                                  exposure ? neout.data() : nullptr, sout.data())
-                    : blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
-                                         maxConcurrent, out.data(), net.data());
+                 : stage_opts || nc
+                     ? analysed(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0, maxConcurrent,
+                                int32_t(nc), nc ? scheduleConcurrency.data() : nullptr, nullptr, out.data(), net.data(),
+                                nc ? an.sched.out.data() : nullptr, audit ? &an.forest.opts : nullptr, audit ? an.aout.data() : nullptr,
+                                &an.eforest.opts, int32_t(an.cap), exposure ? an.eout.data() : nullptr, nc ? net_sched.out.data() : nullptr,
+                                exposure ? neout.data() : nullptr, nc ? sout.data() : nullptr)
+                     : blance_plan_chains(ctx, &ip->in, int32_t(n), int32_t(T), stages.data(), opts.data(), favorMinNodes ? 1 : 0,
+                                          maxConcurrent, out.data(), net.data());
   if (st != BLANCE_OK) throw BlanceError(st, std::string("blance_plan_chains failed: ") + blance_last_error(ctx));
   // chain (or branch) i of n + nb: its stages' results from x0 on, its net and, for a chain, its span
   auto result = [&](size_t i, size_t x0, size_t len, AnalysisOutputs& a) {

@@ -356,36 +356,67 @@ def _opts_struct(base, o, keep):
     return s
 
 
-def _chain_stage(base_tables, stage, st, keep):
-    """Fills the blance_chain_stage st from a stage dict of plan_chains."""
-    sc = scenario_tables(base_tables, {k: v for k, v in stage.items() if k != "node_in_all"})
+def _scenario_struct(base_tables, scenario, st, keep):
+    """Fills the blance_scenario st from a scenario dict (missing keys keep the base's value)."""
+    sc = scenario_tables(base_tables, scenario)
     for f in SCENARIO_FIELDS:
         v = getattr(sc, f)
         if f in ("add_is_nil", "has_node_weights"):
-            setattr(st.nodes, f, int(v))
+            setattr(st, f, int(v))
             continue
         a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
         keep.append(a)
-        setattr(st.nodes, f, a.ctypes.data if a.size else None)
+        setattr(st, f, a.ctypes.data if a.size else None)
+
+
+def _chain_stage(base_tables, stage, st, keep):
+    """Fills the blance_chain_stage st from a stage dict of plan_chains."""
+    _scenario_struct(base_tables, {k: v for k, v in stage.items() if k != "node_in_all"}, st.nodes, keep)
     m = np.ascontiguousarray(stage.get("node_in_all", np.ones(base_tables.n_nodes)), np.uint8)
     keep.append(m)
     st.node_in_all = m.ctypes.data if m.size else None
 
 
+def _analysis_opts(base_tables, schedule, node_has_mover, audit, exposure, keep):
+    """The analysis arguments of plan_scenarios and plan_chains: (counts, the node_has_mover pointer, the audit options
+    pointer and n_domains, the exposure options pointer, V, series_cap, dom, parts); counts is empty without a
+    schedule, each pointer None when not given."""
+    counts = np.ascontiguousarray([] if schedule is None else schedule, np.int32)
+    mover = None
+    if node_has_mover is not None:
+        m = np.ascontiguousarray(node_has_mover, np.uint8)
+        if m.size != base_tables.n_node_ids:
+            raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
+        keep.append(m)
+        mover = m.ctypes.data
+    a_opts, n_dom, e_opts, cap, dom, parts, V = None, 0, None, 0, False, False, base_tables.n_node_ids
+    if audit is not None:
+        a, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
+        a_opts = ctypes.byref(a)
+    if exposure is not None:
+        e, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
+        V += int(e.n_domains)
+        e_opts = ctypes.byref(e) if exposure.get("domain_parent") is not None else None
+        cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
+    return counts, mover, a_opts, n_dom, e_opts, V, cap, dom, parts
+
+
 class _ChainAnalysis:
     """The schedule, audit and exposure outputs of the stages results[i][t] (option dicts opt_of(i, t)) and nets of one
-    chain call's items (its chains, or its branches); fill() hands the filled outputs back to the results and nets."""
+    call's items (its scenarios as one-stage items without nets, its chains, or its branches; counts None: no
+    schedule); fill() hands the filled outputs back to the results and nets."""
 
     def __init__(self, base_tables, results, nets, opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts):
-        nc = counts.size
+        nc = 0 if counts is None else counts.size
         self.results, self.nets, self.nc = results, nets, nc
         self.stages = stages = [r for rs in results for r in rs]
-        for r in stages:
-            r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
-            for s in r.schedules if not stage_arrays else ():
-                s.out.node_rounds = s.out.node_last_round = s.out.part_done_round = None
-        self.sch = (api.ScenarioScheduleOut * (len(stages) * nc))(*[s.out for r in stages for s in r.schedules])
-        self.net_sch = self.auds = self.exps = self.net_exps = self.expo = self.net_expo = None
+        self.sch = self.net_sch = self.auds = self.exps = self.net_exps = self.expo = self.net_expo = None
+        if counts is not None:
+            for r in stages:
+                r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
+                for s in r.schedules if not stage_arrays else ():
+                    s.out.node_rounds = s.out.node_last_round = s.out.part_done_round = None
+            self.sch = (api.ScenarioScheduleOut * (len(stages) * nc))(*[s.out for r in stages for s in r.schedules])
         if nets is not None:
             for x in nets:
                 x.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
@@ -408,7 +439,7 @@ class _ChainAnalysis:
     def fill(self):
         nc = self.nc
         for x, r in enumerate(self.stages):
-            for k, s in enumerate(r.schedules):
+            for k, s in enumerate(r.schedules or ()):
                 s.out = self.sch[x * nc + k]
             if self.auds is not None:
                 r.audit.out = self.auds[x]
@@ -514,74 +545,28 @@ class Context:
         base = base_tables.struct()
         keep, scs = [], (api.Scenario * max(1, n))()
         for i, sc in enumerate(scenarios):
-            t = scenario_tables(base_tables, sc)
-            for f in SCENARIO_FIELDS:
-                v = getattr(t, f)
-                if f in ("add_is_nil", "has_node_weights"):
-                    setattr(scs[i], f, int(v))
-                    continue
-                a = np.ascontiguousarray(v, dtype=np.int32 if f == "node_weight" else np.uint8)
-                keep.append(a)
-                setattr(scs[i], f, a.ctypes.data if a.size else None)
+            _scenario_struct(base_tables, sc, scs[i], keep)
         results = [ScenarioResult(base_tables, i in want) for i in range(n)]
         outs = (api.ScenarioOut * max(1, n))(*[r.out for r in results])
-        if schedule is not None or audit is not None:
-            counts = np.ascontiguousarray([] if schedule is None else schedule, np.int32)
-            mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
-            if mover is not None and mover.size != base_tables.n_node_ids:
-                raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
-            sch = None
-            if schedule is not None:
-                for r in results:
-                    r.schedules = [ScenarioSchedule(base_tables, int(c)) for c in counts]
-                sch = (api.ScenarioScheduleOut * max(1, n * counts.size))(*[s.out for r in results for s in r.schedules])
-            ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-            args = (self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent), int(counts.size),
-                    counts.ctypes.data if counts.size else None, None if mover is None else mover.ctypes.data, outs, sch)
-            if exposure is not None:
-                e_opts, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
-                V = base_tables.n_node_ids + int(e_opts.n_domains)
-                cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
-                expo = [[_ScenarioExposure(base_tables, V, max(cap, 0), dom, parts) for _ in counts] for _ in results]
-                exps = (api.ExposureOut * max(1, n * counts.size))(*[e.out for es in expo for e in es])
-                auds = None
-                if audit is not None:
-                    a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
-                    for i, r in enumerate(results):
-                        t = scenario_tables(base_tables, scenarios[i], None if opts is None else opts[i])
-                        r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
-                    auds = (api.AuditOut * max(1, n))(*[r.audit.out for r in results])
-                self._check(self.lib.blance_plan_scenarios_exposure(
-                    *args, None if audit is None else ctypes.byref(a_opts), auds,
-                    ctypes.byref(e_opts) if exposure.get("domain_parent") is not None else None, cap, exps),
-                    "blance_plan_scenarios_exposure")
-                for i, r in enumerate(results):
-                    if auds is not None:
-                        r.audit.out = auds[i]
-                    for k, e in enumerate(expo[i]):
-                        e.out = exps[i * counts.size + k]
-                    r.exposures = [e.result() for e in expo[i]]
-            elif audit is None:
-                self._check(self.lib.blance_plan_scenarios_schedule(*args), "blance_plan_scenarios_schedule")
-            else:
-                a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
-                for i, r in enumerate(results):
-                    t = scenario_tables(base_tables, scenarios[i], None if opts is None else opts[i])
-                    r.audit = AuditResult(base_tables, _n_rules(t), n_dom, audit.get("n2n", False))
-                auds = (api.AuditOut * max(1, n))(*[r.audit.out for r in results])
-                self._check(self.lib.blance_plan_scenarios_audit(*args, ctypes.byref(a_opts), auds), "blance_plan_scenarios_audit")
-                for r, a in zip(results, auds):
-                    r.audit.out = a
-            for i, r in enumerate(results):
-                for k, s in enumerate(r.schedules or ()):
-                    s.out = sch[i * counts.size + k]
-        elif opts is None:
-            self._check(self.lib.blance_plan_scenarios(self.ptr, ctypes.byref(base), n, scs, int(bool(favor_min_nodes)),
-                                                       int(max_concurrent), outs), "blance_plan_scenarios")
+        ops = None if opts is None else (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
+        args = (self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)), int(max_concurrent))
+        an = None
+        if schedule is None and audit is None:
+            what = "blance_plan_scenarios" if opts is None else "blance_plan_scenarios_ex"
+            args = args[:4] + args[5:] + (outs,) if opts is None else args + (outs,)
         else:
-            ops = (api.ScenarioOpts * max(1, n))(*[_opts_struct(base_tables, o, keep) for o in opts])
-            self._check(self.lib.blance_plan_scenarios_ex(self.ptr, ctypes.byref(base), n, scs, ops, int(bool(favor_min_nodes)),
-                                                          int(max_concurrent), outs), "blance_plan_scenarios_ex")
+            counts, mover, a_opts, n_dom, e_opts, V, cap, dom, parts = _analysis_opts(base_tables, schedule, node_has_mover, audit, exposure,
+                                                                                        keep)
+            an = _ChainAnalysis(base_tables, [[r] for r in results], None, lambda i, t: None if opts is None else opts[i],
+                                None if schedule is None else counts, audit, n_dom, exposure, True, V, cap, dom, parts)
+            # each scenario entry point with an analysis takes a prefix of blance_plan_scenarios_exposure's arguments
+            what, k = (("blance_plan_scenarios_exposure", 17) if exposure is not None else
+                       ("blance_plan_scenarios_audit", 14) if audit is not None else ("blance_plan_scenarios_schedule", 12))
+            args = (args + (counts.size, counts.ctypes.data if counts.size else None, mover, outs, an.sch, a_opts, an.auds, e_opts, cap,
+                            an.exps))[:k]
+        self._check(getattr(self.lib, what)(*args), what)
+        if an is not None:
+            an.fill()
         for r, o in zip(results, outs):
             r.out = o
         return results
@@ -720,26 +705,14 @@ class Context:
         """The blance_plan_chains_exposure call of plan_chains (per_stage: blance_plan_chains_ex; opt_of(i, t) is the
         option dict of chain i's stage t; branches: the (args, results, nets, opt_of) of blance_plan_chain_branches):
         fills the results' and nets' schedules, audits and exposures; returns the spans (or None)."""
-        counts = np.ascontiguousarray(schedule, np.int32)
+        counts, mover, a_opts, n_dom, e_opts, V, cap, dom, parts = _analysis_opts(base_tables, schedule, node_has_mover, audit, exposure, keep)
         nc = counts.size
-        mover = None if node_has_mover is None else np.ascontiguousarray(node_has_mover, np.uint8)
-        if mover is not None and mover.size != base_tables.n_node_ids:
-            raise ValueError("node_has_mover must have n_node_ids = %d entries" % base_tables.n_node_ids)
-        a_opts, n_dom, e_opts, cap, dom, parts, V = None, 0, None, 0, False, False, base_tables.n_node_ids
-        if audit is not None:
-            a_opts, n_dom = _audit_opts(audit.get("n2n", False), audit.get("domain_parent"), base_tables.n_node_ids, keep)
-        if exposure is not None:
-            e_opts, _ = _audit_opts(False, exposure.get("domain_parent"), base_tables.n_node_ids, keep)
-            V += int(e_opts.n_domains)
-            cap, dom, parts = int(exposure.get("series_cap", 0)), bool(exposure.get("dom", True)), bool(exposure.get("parts", True))
         trunk = _ChainAnalysis(base_tables, results, nets, opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts)
         spans = [[_ChainSpan(base_tables, V, exposure is not None, dom, parts) for _ in counts] for _ in range(n)] if span else None
         span_arr = (api.ChainSpanOut * (n * nc))(*[s.out for ss in spans for s in ss]) if span else None
         args = [self.ptr, ctypes.byref(base), n, T, sts, ops, int(bool(favor_min_nodes)), int(max_concurrent), nc, counts.ctypes.data,
-                None if mover is None else mover.ctypes.data, outs, net_arr, trunk.sch,
-                None if audit is None else ctypes.byref(a_opts), trunk.auds,
-                ctypes.byref(e_opts) if exposure is not None and exposure.get("domain_parent") is not None else None,
-                cap if stage_arrays else 0, trunk.exps, trunk.net_sch, trunk.net_exps, span_arr]
+                mover, outs, net_arr, trunk.sch, a_opts, trunk.auds, e_opts, cap if stage_arrays else 0, trunk.exps, trunk.net_sch,
+                trunk.net_exps, span_arr]
         if branches is not None:
             b_args, b_results, b_nets, b_opt_of = branches
             br = _ChainAnalysis(base_tables, b_results, b_nets, b_opt_of, counts, audit, n_dom, exposure, stage_arrays, V, cap, dom, parts)

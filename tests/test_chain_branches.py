@@ -162,6 +162,15 @@ ROWS = [
      _at("rule_off is NULL")),
     ("branch event bound", dict(br_expo=True, br_dom=True),
      (UNSUPPORTED, NAME + ": branch 1, stage 0, count 1: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31")),
+    # without a trunk audit, the audit options are first checked for br_audit
+    ("branch audit flags", dict(audit=False, aflags=0x80, br_audit=True), (INVALID, NAME + ": audit flags hold an unknown bit")),
+    # two bad arguments: which check fires first
+    ("chain before branch stage", dict(chain=-1, bscen=dict(add_is_nil=2)), _br("chain outside [0, n)")),
+    ("branch stage before audit flags", dict(audit=False, aflags=0x80, br_audit=True, bscen=dict(add_is_nil=2)),
+     _at("add_is_nil is neither 0 nor 1")),
+    ("branch audit model before branch event bound",
+     dict(br_audit=True, br_expo=True, br_dom=True, bopts=dict(set=api.OPT_HIERARCHY, has_hier_rules=1, n_hier_bits=4)),
+     _at("rule_off is NULL")),
 ]
 
 

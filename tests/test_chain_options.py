@@ -142,6 +142,8 @@ ROWS = [
     # two bad arguments: which check fires first
     ("stage before options", dict(BAD_SCEN, stage_opts=dict(set=0x100)), _stage("add_is_nil is neither 0 nor 1"), 8),
     ("schedule before options", dict(nmc=0, stage_opts=dict(set=0x100)), (INVALID, NAME + ": n_move_conc must be positive"), 0),
+    ("audit flags before no schedule, expo", dict(NO_SCHED, expo=True, aflags=0x80), (INVALID, NAME + ": audit flags hold an unknown bit"), 0),
+    ("audit model before no schedule, expo", dict(NO_SCHED, expo=True, stage_opts=dict(set=H_, has_hier_rules=1)), _stage("rule_off is NULL"), 0),
 ]
 
 

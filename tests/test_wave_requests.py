@@ -339,6 +339,23 @@ ROWS = [
      (INVALID, "blance_plan_chains_exposure: n_move_conc must be positive"), 0),
     ("chains_exposure", "event bound before stage", dict(dom=True, n_parts=EVENTS_OVER, **BAD_SCEN, audit=False),
      (UNSUPPORTED, "blance_plan_chains_exposure: chain 1, stage 1, count 1: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31"), 8),
+    ("exposure", "n_move_conc before expo", dict(nmc=0, expo=False),
+     (INVALID, "blance_plan_scenarios_exposure: an exposure needs a schedule: n_move_conc must be positive"), 0),
+    ("exposure", "expo before audit model", dict(BAD_RULES, expo=False),
+     (INVALID, "blance_plan_scenarios_exposure: expo is NULL"), 4),
+    ("exposure", "audit model before event bound", dict(BAD_RULES, dom=True, n_parts=EVENTS_OVER),
+     (INVALID, "blance_plan_scenarios_exposure: scenario 0: state_slot_off does not span [0, n_slots]"), 4),
+    ("chains_exposure", "base before net", dict(base=False, net=False, net_sched=True),
+     (INVALID, "blance_plan_chains_exposure: base, stages or out is NULL"), 0),
+    ("chains_exposure", "audit model before n_move_conc", dict(BAD_RULES, nmc=0),
+     (INVALID, "blance_plan_chains_exposure: chain 1: rule_off is NULL"), 0),
+    ("chains_exposure", "series_cap before span without expo", dict(expo=False, span="part_flags", series_cap=-1),
+     (INVALID, "blance_plan_chains_exposure: series_cap is negative"), 8),
+    ("chains_exposure", "event bound before net event bound", dict(dom=True, net_expo=True, net_dom=True, n_parts=EVENTS_OVER, audit=False),
+     (UNSUPPORTED, "blance_plan_chains_exposure: chain 1, stage 1, count 1: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31"), 8),
+    ("chains_exposure", "net event bound before span event bound",
+     dict(net_expo=True, net_dom=True, span="dom_peak_stage", n_parts=EVENTS_OVER, audit=False),
+     (UNSUPPORTED, "blance_plan_chains_exposure: chain 1, count 1: dom_peak needs 2 x 17 x 2 x n_slots x n_parts < 2^31"), 8),
 ]
 
 
