@@ -18,10 +18,10 @@ from . import build as _build
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
 _API_NAMES = ("AuditMap", "BOOSTER_CBGT_MAX", "BOOSTER_NONE", "BlanceError", "CalcPartitionMoves", "CalcPartitionMovesMap",
-              "NodeStateOp", "OrchestrateExposure", "OrchestrateSchedule", "OrchestratorOptions", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions",
+              "NodeStateOp", "OrchestrateExposure", "OrchestrateLoad", "OrchestrateSchedule", "OrchestratorOptions", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions",
               "PlanNextMapChains", "PlanNextMapScenarios", "capi")
 __all__ = ["AuditMap", "PlanNextMap", "PlanNextMapEx", "PlanNextMapOptions", "PlanNextMapScenarios", "PlanNextMapChains", "CalcPartitionMoves", "CalcPartitionMovesMap",
-           "NodeStateOp", "OrchestrateExposure", "OrchestrateSchedule", "OrchestratorOptions", "BlanceError", "BOOSTER_NONE", "BOOSTER_CBGT_MAX", "capi"]
+           "NodeStateOp", "OrchestrateExposure", "OrchestrateLoad", "OrchestrateSchedule", "OrchestratorOptions", "BlanceError", "BOOSTER_NONE", "BOOSTER_CBGT_MAX", "capi"]
 
 
 def __getattr__(name):

@@ -113,6 +113,16 @@ class _ExposureOut(ctypes.Structure):  # struct blance_exposure_out
                 ("part_flags", ctypes.c_void_p), ("kernel_ms", ctypes.c_float)]
 
 
+class _LoadIn(ctypes.Structure):       # struct blance_load_in
+    _fields_ = [("part_weight", ctypes.c_void_p), ("part_has_weight", ctypes.c_void_p)]
+
+
+class _LoadOut(ctypes.Structure):      # struct blance_load_out
+    _fields_ = [("rounds", ctypes.c_int32), ("node_beg", ctypes.c_void_p), ("node_end", ctypes.c_void_p),
+                ("node_peak", ctypes.c_void_p), ("node_peak_round", ctypes.c_void_p), ("over_max", ctypes.c_int64),
+                ("over_node", ctypes.c_int32), ("kernel_ms", ctypes.c_float)]
+
+
 class _ChainSpanOut(ctypes.Structure):  # struct blance_chain_span_out
     _fields_ = [("rounds", ctypes.c_int64), ("moves_done", ctypes.c_int64), ("stuck_parts", ctypes.c_int64),
                 ("max_batch", ctypes.c_int32), ("node_rounds", ctypes.c_void_p), ("node_last_round", ctypes.c_void_p),
@@ -124,9 +134,9 @@ class _ChainSpanOut(ctypes.Structure):  # struct blance_chain_span_out
 
 _CAPI = None
 EXPORTS = ("blance_ctx_create", "blance_ctx_create_multi", "blance_ctx_device_count", "blance_ctx_destroy", "blance_last_error", "blance_version", "blance_ctx_kernel_launches", "blance_plan_in_check", "blance_plan_next_map",
-           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_chains", "blance_plan_chains_exposure", "blance_plan_chains_ex", "blance_plan_chain_branches", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
+           "blance_plan_next_map_batch", "blance_plan_scenarios", "blance_plan_scenarios_ex", "blance_plan_scenarios_schedule", "blance_plan_scenarios_audit", "blance_plan_scenarios_exposure", "blance_plan_scenarios_load", "blance_plan_chains", "blance_plan_chains_exposure", "blance_plan_chains_ex", "blance_plan_chain_branches", "blance_map_audit", "blance_plan_audit", "blance_plan_upload", "blance_plan_run", "blance_plan_fetch", "blance_plan_free", "blance_plan_timing",
            "blance_calc_partition_moves", "blance_moves_create", "blance_moves_fetch", "blance_moves_available",
-           "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_exposure", "blance_moves_free")
+           "blance_moves_schedule", "blance_moves_schedule_fetch", "blance_moves_exposure", "blance_moves_load", "blance_moves_free")
 
 
 def capi():
@@ -152,6 +162,7 @@ def capi():
         lib.blance_plan_scenarios_schedule.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]
         lib.blance_plan_scenarios_audit.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         lib.blance_plan_scenarios_exposure.argtypes = [vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+        lib.blance_plan_scenarios_load.argtypes = lib.blance_plan_scenarios_exposure.argtypes + [vp]
         lib.blance_plan_chains.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, vp, vp]
         lib.blance_plan_chains_exposure.argtypes = [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp,
                                                     vp, vp, vp]
@@ -174,6 +185,7 @@ def capi():
         lib.blance_moves_schedule.argtypes = [vp, vp, i32, vp, vp]
         lib.blance_moves_schedule_fetch.argtypes = [vp, vp, vp, vp]
         lib.blance_moves_exposure.argtypes = [vp, vp, vp, vp]
+        lib.blance_moves_load.argtypes = [vp, vp, vp, vp]
         lib.blance_moves_free.argtypes = [vp, vp]
         lib.blance_moves_free.restype = None
         _CAPI = lib
@@ -195,3 +207,5 @@ AuditOut = _AuditOut
 ExposureIn = _ExposureIn
 ExposureOut = _ExposureOut
 ChainSpanOut = _ChainSpanOut
+LoadIn = _LoadIn
+LoadOut = _LoadOut

@@ -9,6 +9,8 @@
         (the lock-step model of OrchestrateMoves, orchestrate.go:240-591; include/blance_b200.h)
     OrchestrateExposure(model, options, nodesAll, begMap, endMap, nodeHierarchy) -> the maps those rounds pass
         through, counted per round (blance_moves_exposure)
+    OrchestrateLoad(model, options, nodesAll, begMap, endMap, partitionWeights) -> each node's load on those maps:
+        start, end and peak (blance_moves_load)
 
 A PartitionMap is {partitionName: {stateName: [nodeName, ...] | None}}; a
 PartitionModel is {stateName: (priority, constraints)}; HierarchyRules is
@@ -284,6 +286,21 @@ def OrchestrateExposure(model, options, nodesAll, begMap, endMap, nodeHierarchy=
     return _host.OrchestrateExposure({k: tuple(v) for k, v in model.items()}, int(o.MaxConcurrentPartitionMovesPerNode),
                                      bool(o.FavorMinNodes), list(nodesAll), begMap, endMap,
                                      None if nodeHierarchy is None else dict(nodeHierarchy))
+
+
+def OrchestrateLoad(model, options, nodesAll, begMap, endMap, partitionWeights=None):
+    """Does a node run out of room while the rebalance of OrchestrateSchedule(model, options, nodesAll, begMap, endMap)
+    runs?  Each node's load on the maps M_0 .. M_R it passes through under the lock-step model, counted on the device
+    (blance_moves_load, include/blance_b200.h).  A partition weighs partitionWeights[name] ({partition: weight}, as
+    PartitionWeights), 1 when it has none.  Returns a dict:
+      rounds R;  states {state: {node: {beg, end, peak, peak_round}}} and nodes {node: {...}} over all states (nonzero
+        entries only): the load on M_0, on M_R, its largest value and the first round at it;
+      over_max / over_node: the largest peak over both ends of one node (all states) and that node ("" without nodes);
+      kernel_ms."""
+    o = options or OrchestratorOptions()
+    return _host.OrchestrateLoad({k: tuple(v) for k, v in model.items()}, int(o.MaxConcurrentPartitionMovesPerNode),
+                                 bool(o.FavorMinNodes), list(nodesAll), begMap, endMap,
+                                 None if partitionWeights is None else {k: int(v) for k, v in partitionWeights.items()})
 
 
 # ---- the raw C ABI (ctypes) lives in abi.py; re-exported here for callers of the Python face -----------

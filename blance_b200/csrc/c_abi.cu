@@ -30,6 +30,7 @@
 #include "count_bound.hpp"
 #include "device_types.cuh"
 #include "exposure.cuh"
+#include "node_load.h"
 #include "wave_schedule.cuh"
 
 using namespace blance_dev;
@@ -111,7 +112,8 @@ struct blance_ctx {
   cudaEvent_t ev[8] = {};            // [4], [5]: around the audit kernels; [6], [7]: around a wave's exposures
   int* d_any_active = nullptr;
   int* h_any_active = nullptr;       // pinned
-  long long launches = 0;            // kernels of this library launched so far
+  long long launches = 0;            // kernels launched so far by this library's own launches and by the node-load
+                                     // launchers of libblance_b200_load.so (CUB's launches are not counted)
   void* h_stage = nullptr;           // pinned staging of a batch (kept between calls, grow-only)
   size_t h_stage_bytes = 0;
   std::vector<blance_ctx*> children; // blance_ctx_create_multi: one single-device context per GPU
@@ -1740,6 +1742,7 @@ struct WaveReq {
   const ExpoReq* er = nullptr;
   const BranchReq* forks = nullptr;
   const BranchReq* br = nullptr;
+  blance_load_out* load = nullptr;     // [n][nc] each node's load over every schedule (blance_plan_scenarios_load)
 };
 
 // The branches of a chain request: n branches of cr.T stages each, the trunk request they leave, and the request
@@ -1876,10 +1879,31 @@ struct Sweep {
         V((long long)r.base->n_node_ids + (r.er ? r.er->n_domains : 0)), stride(summary_stride(*r.base)) {}
 };
 
-// The buffers of a wave's analyses: audits, exposures, span accumulators, a chain's net prev rows, flags and summaries.
+// The per-instance buffers of the node loads of nw scenarios x nc counts that are priced into a wave: [ni][(S + 1) NU]
+// loads, peaks and packed maxima, one packed overshoot each, and [ni][PU + 1] event counts and offsets.  The op states
+// and rounds are the exposure's (expo_slices), laid out here when no exposure is asked for.
+struct LoadBufs {
+  long long *node_beg = nullptr, *node_end = nullptr, *node_peak = nullptr;
+  int32_t* node_peak_round = nullptr;
+  unsigned long long *peak_key = nullptr, *over_key = nullptr;
+  long long *ev_count = nullptr, *ev_off = nullptr;
+};
+
+static void load_slices(Arena& a, LoadBufs& b, WSched& w, bool expo, long long nw, long long nc, long long PU, long long MO,
+                        long long K) {
+  const long long ni = nw * nc;
+  if (!expo) { a.add(w.op_state, (size_t)std::max(1ll, nw * PU * MO)); a.add(w.op_round, (size_t)std::max(1ll, ni * PU * MO)); }
+  a.add(b.node_beg, (size_t)(ni * K)); a.add(b.node_end, (size_t)(ni * K)); a.add(b.node_peak, (size_t)(ni * K));
+  a.add(b.node_peak_round, (size_t)(ni * K)); a.add(b.peak_key, (size_t)(ni * K)); a.add(b.over_key, (size_t)ni);
+  a.add(b.ev_count, (size_t)(ni * (PU + 1))); a.add(b.ev_off, (size_t)(ni * (PU + 1)));
+}
+
+// The buffers of a wave's analyses: audits, exposures, loads, span accumulators, a chain's net prev rows, flags and
+// summaries.
 struct AnalysisBufs {
   AuditBufs audit;
   ExpoBufs expo;
+  LoadBufs load;
   SpanBufs span;
   int32_t* net_prev = nullptr;
   uint8_t* net_flags = nullptr;
@@ -1906,8 +1930,8 @@ struct Wave {
   int32_t* d_ow = nullptr;
   AnalysisBufs an;
   std::vector<long long> G;
-  float sum_ms = 0.f, sched_ms = 0.f, expo_ms = 0.f, fold_ms = 0.f;
-  size_t expo_bytes = 0;
+  float sum_ms = 0.f, sched_ms = 0.f, expo_ms = 0.f, fold_ms = 0.f, load_ms = 0.f;
+  size_t expo_bytes = 0, load_bytes = 0;
 };
 
 // Where the caller keeps the output of instance i of wave w (member i / n, its count i % n) at stage t, in an array of
@@ -1970,12 +1994,99 @@ static void wave_exposure(const Sweep& s, Wave& w, const int32_t* beg, const uin
   }
 }
 
+// The node loads of wave w's instances after their schedules (scal: the instances' scalars), from the beg rows / flags
+// `beg` / `pflags` and the members' partition weights over the op table and rounds the schedule left in w.sched;
+// instance i's result goes to outs[out_at(i, nc, per, t)].  Every instance is counted first; the event buffers are
+// then allocated once, exactly sized for the instance with the most events, and the instances run one by one on them.
+static void wave_load(const Sweep& s, Wave& w, const int32_t* beg, const uint8_t* pflags, blance_load_out* outs, int per, int t,
+                      const std::vector<unsigned long long>& scal) {
+  blance_ctx* dev = s.ctx;
+  cudaStream_t st = dev->stream;
+  const blance_plan_in& base = *s.q.base;
+  const int PU = base.n_parts, S = base.n_states, NU = base.n_node_ids;
+  const long long ni = (long long)w.nw * s.nc, K = (long long)(S + 1) * NU;
+  const WSched& W = w.sched;
+  const LoadBufs& b = w.an.load;
+  std::vector<blance_load::LoadArgs> args((size_t)ni);
+  Arena scan;
+  void* scan_tmp = nullptr;
+  size_t scan_bytes = 0;
+  CUDA(blance_load::load_scan_bytes(PU, &scan_bytes, st));
+  scan.add(scan_tmp, scan_bytes);
+  scan.alloc(st, "the load");
+  CUDA(cudaEventRecord(dev->ev[6], st));
+  for (long long i = 0; i < ni; ++i) {
+    const long long j = i / s.nc;
+    const DInst& D = w.pl->h_insts[(size_t)j];
+    blance_load::LoadArgs& A = args[(size_t)i];
+    A.beg = beg + D.rows_off; A.stride = D.SLP;
+    A.op_n = W.op_n + j * PU; A.op_node = W.op_node + j * PU * s.MO; A.op_state = W.op_state + j * PU * s.MO;
+    A.op_kind = W.op_kind + j * PU * s.MO; A.op_round = W.op_round + i * PU * s.MO; A.MO = s.MO;
+    A.weight = w.pl->pool.pweight + D.part_off; A.pflags = pflags + D.part_off; A.has_part_weights = D.has_part_weights;
+    A.P = PU; A.S = S; A.SL = base.n_slots; A.NU = NU;
+    for (int k = 0; k <= S; ++k) A.slot_off[k] = base.state_slot_off[k];
+    A.node_beg = b.node_beg + i * K; A.node_end = b.node_end + i * K; A.node_peak = b.node_peak + i * K;
+    A.node_peak_round = b.node_peak_round + i * K; A.peak_key = b.peak_key + i * K; A.over_key = b.over_key + i;
+    A.ev_count = b.ev_count + i * (PU + 1); A.ev_off = b.ev_off + i * (PU + 1);
+    A.scan_tmp = scan_tmp; A.scan_tmp_bytes = scan_bytes;
+    CUDA(blance_load::load_count(A, dev->sm_count, st, &dev->launches));
+  }
+  std::vector<long long> ne((size_t)ni, 0);   // each instance's event count: ev_off[P]
+  if (ni > 0)
+    CUDA(cudaMemcpy2DAsync(ne.data(), sizeof(long long), b.ev_off + PU, sizeof(long long) * (size_t)(PU + 1), sizeof(long long), (size_t)ni,
+                           cudaMemcpyDeviceToHost, st));
+  CUDA(cudaStreamSynchronize(st));
+  const long long max_ne = ni > 0 ? *std::max_element(ne.begin(), ne.end()) : 0;
+  int key_bits = 1;
+  while ((1ll << key_bits) < K) ++key_bits;
+  blance_load::LoadArgs E{};
+  Arena ev;
+  if (max_ne > 0) {
+    CUDA(blance_load::load_event_bytes(max_ne, key_bits, &E.ev_tmp_bytes, st));
+    const size_t n = (size_t)max_ne;
+    ev.add(E.ev_key, n); ev.add(E.ev_key2, n); ev.add(E.run_key, n); ev.add(E.ev_val, n); ev.add(E.ev_val2, n);
+    ev.add(E.run_val, n); ev.add(E.run_sum, n); ev.add(E.n_runs, 1); ev.add(E.ev_tmp, E.ev_tmp_bytes);
+    ev.alloc(st, "the load's events");
+  }
+  w.load_bytes = scan.bytes() + ev.bytes();
+  for (long long i = 0; i < ni; ++i) {
+    blance_load::LoadArgs& A = args[(size_t)i];
+    A.ev_key = E.ev_key; A.ev_key2 = E.ev_key2; A.run_key = E.run_key; A.ev_val = E.ev_val; A.ev_val2 = E.ev_val2;
+    A.run_val = E.run_val; A.run_sum = E.run_sum; A.n_runs = E.n_runs; A.ev_tmp = E.ev_tmp; A.ev_tmp_bytes = E.ev_tmp_bytes;
+    CUDA(blance_load::load_peaks(A, ne[(size_t)i], key_bits, dev->sm_count, st, &dev->launches));
+  }
+  CUDA(cudaEventRecord(dev->ev[7], st));
+  std::vector<unsigned long long> over((size_t)ni, 0);
+  if (ni > 0) CUDA(cudaMemcpyAsync(over.data(), b.over_key, sizeof(unsigned long long) * (size_t)ni, cudaMemcpyDeviceToHost, st));
+  const size_t kb = sizeof(int64_t) * (size_t)K;
+  for (long long i = 0; i < ni && K > 0; ++i) {
+    blance_load_out& o = outs[out_at(s, w, i, s.nc, per, t)];
+    if (o.node_beg) CUDA(cudaMemcpyAsync(o.node_beg, b.node_beg + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_end) CUDA(cudaMemcpyAsync(o.node_end, b.node_end + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_peak) CUDA(cudaMemcpyAsync(o.node_peak, b.node_peak + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_peak_round)
+      CUDA(cudaMemcpyAsync(o.node_peak_round, b.node_peak_round + i * K, sizeof(int32_t) * (size_t)K, cudaMemcpyDeviceToHost, st));
+  }
+  CUDA(cudaStreamSynchronize(st));
+  w.load_ms = 0.f;
+  cudaEventElapsedTime(&w.load_ms, dev->ev[6], dev->ev[7]);
+  for (long long i = 0; i < ni; ++i) {
+    blance_load_out& o = outs[out_at(s, w, i, s.nc, per, t)];
+    o.rounds = (int32_t)scal[(size_t)(4 * i)];
+    o.over_max = NU > 0 ? (int64_t)(over[(size_t)i] >> 32) : 0;
+    o.over_node = NU > 0 ? (int32_t)(0xFFFFFFFFu - (uint32_t)over[(size_t)i]) : -1;
+    o.kernel_ms = w.load_ms;
+  }
+}
+
 // The slices of the analyses of nw members laid out as pl into b (the exposures' op states and rounds into sched).
 // One member's are what it adds to the price wave_size makes of its plan, summaries and schedule state.
 static void analysis_slices(const Sweep& s, Arena& a, AnalysisBufs& b, WSched& sched, int nw, const blance_plan* pl) {
   const blance_plan_in& base = *s.q.base;
   if (s.q.ar) audit_slices(a, b.audit, *s.q.ar, nw, base.n_states, s.max_rules, base.n_node_ids, base.n_nodes, base.n_parts, s.audit_flags);
   if (s.q.er) expo_slices(a, b.expo, sched, *s.q.er, nw, s.nc, base.n_parts, s.MO, s.V);
+  if (s.q.load)
+    load_slices(a, b.load, sched, s.q.er != nullptr, nw, s.nc, base.n_parts, s.MO, (long long)(base.n_states + 1) * base.n_node_ids);
   if (s.q.cr && s.q.cr->net) {
     a.add(b.net_prev, (size_t)pl->RT + 4);
     a.add(b.net_flags, (size_t)pl->PT + 1);
@@ -2223,8 +2334,8 @@ static std::vector<unsigned long long> stage_schedule(const Sweep& s, Wave& w, c
   cudaStream_t st = s.ctx->stream;
   const int NU = s.q.base->n_node_ids, PU = s.q.base->n_parts;
   const WSched& W = w.sched;
+  if (W.op_round) CUDA(cudaMemsetAsync(W.op_round, 0xFF, sizeof(int32_t) * (size_t)w.nw * s.nc * PU * s.MO, st));
   if (s.q.er) {
-    CUDA(cudaMemsetAsync(W.op_round, 0xFF, sizeof(int32_t) * (size_t)w.nw * s.nc * PU * s.MO, st));
     if (w.an.expo.parent) CUDA(cudaMemcpyAsync(w.an.expo.parent, s.q.er->parent, sizeof(int32_t) * (size_t)s.V, cudaMemcpyHostToDevice, st));
   }
   if (PU > 0) launch(s.ctx, k_wave_moves, wave_grid(s.ctx, PU, w.nw), 256, 0, w.pl->pool, beg, pflags, s.q.favor_min, W);
@@ -2337,6 +2448,7 @@ static void report(const Sweep& s, const Wave& w, int t) {
                w.w0, w.nw, s.W, s.per, wave_ms, w.sum_ms);
   if (s.q.sr) std::fprintf(stderr, ", schedule %.3f ms (%d counts)", w.sched_ms, s.nc);
   if (s.q.er) std::fprintf(stderr, ", exposure %.3f ms (%zu device bytes)", w.expo_ms, w.expo_bytes);
+  if (s.q.load) std::fprintf(stderr, ", load %.3f ms (%zu device bytes)", w.load_ms, w.load_bytes);
   if (s.q.cr && s.q.cr->span) std::fprintf(stderr, ", span fold %.3f ms", w.fold_ms);
   if (s.q.br) std::fprintf(stderr, " (branches after trunk stage %d, stage %d)", chain_at(s.q, s.idx[0], 0) - 1, t);
   else if (s.q.cr) std::fprintf(stderr, " (stage %d)", t);
@@ -2429,8 +2541,8 @@ static void sweep_waves(Sweep& s) {
     if (!wave_alloc(s, w)) { s.W = w.nw / 2; continue; }
     wave_upload(s, w);
     for (int t = 0; t < s.T; ++t) {
-      w.sum_ms = w.sched_ms = w.expo_ms = w.fold_ms = 0.f;
-      w.expo_bytes = 0;
+      w.sum_ms = w.sched_ms = w.expo_ms = w.fold_ms = w.load_ms = 0.f;
+      w.expo_bytes = w.load_bytes = 0;
       if (t > 0) stage_boundary(s, w, t);
       const std::vector<long long> h_sum = stage_results(s, w, t);
       if (q.sr) {                      // the schedules, exposures and span fold of the stage
@@ -2440,6 +2552,7 @@ static void sweep_waves(Sweep& s) {
         CUDA(cudaEventSynchronize(ctx->ev[1]));
         cudaEventElapsedTime(&w.sched_ms, ctx->ev[3], ctx->ev[1]);
         if (q.er) wave_exposure(s, w, w.pl->prev_rows_init, w.pl->pflags_init, q.er->out, s.T, t, scal);
+        if (q.load) wave_load(s, w, w.pl->prev_rows_init, w.pl->pflags_init, q.load, s.T, t, scal);
         if (q.cr && q.cr->span) span_fold(s, w, t, scal);
       }
       if (getenv("BLANCE_SCENARIO_TIMES")) report(s, w, t);
@@ -2630,6 +2743,7 @@ struct WaveArgs {
   blance_scenario_schedule_out* br_net_sched = nullptr;
   blance_exposure_out* br_net_expo = nullptr;
   const blance_scenario* sc = nullptr;
+  blance_load_out* load = nullptr;
 };
 
 // Whether an entry point takes an analysis: never, always, or when the caller asks for it (an audit or an exposure
@@ -2648,6 +2762,7 @@ struct Entry {
   Takes sched, audit, expo;
   bool branches;
   NullCtx null_ctx;
+  Takes load = NEVER;
 };
 
 // The branches of the chain request q (its chains checked) in b, and q.forks set to them: the branch arguments' own
@@ -2726,6 +2841,7 @@ static int plan_request(blance_ctx* ctx, const Entry& e, const WaveArgs& a) {
     const bool no_sched = e.sched == MAY && a.n_move_conc == 0 && !a.move_conc && !a.sched;
     if (no_sched && (a.expo || a.net_sched || a.net_expo || a.span)) bad("expo, net_sched, net_expo and span need a schedule");
     if (e.sched != NEVER && !no_sched) {
+      if (e.load == ALWAYS && a.n_move_conc < 1) bad("the load needs a schedule: n_move_conc must be positive");
       if (e.expo != NEVER && a.n_move_conc < 1)
         bad(std::string(e.expo == ALWAYS ? "an exposure needs a schedule: " : "") + "n_move_conc must be positive");
       sr = sched_req(name, a.base, e.chains || (a.sc && a.out) ? n * std::max(0, T) * nc : 0, a.n_move_conc, a.move_conc, a.node_has_mover,
@@ -2751,6 +2867,15 @@ static int plan_request(blance_ctx* ctx, const Entry& e, const WaveArgs& a) {
       er.dom |= cr.span_dom;
       er.part_min |= cr.span_parts; er.part_notop |= cr.span_parts; er.part_flags |= cr.span_parts;
       if (a.expo) q.er = &er;
+    }
+    if (e.load == ALWAYS) {
+      if (!a.load) bad("load is NULL");
+      const long long SL = std::max(0, a.base->n_slots), K = (long long)(a.base->n_states + 1) * std::max(0, a.base->n_node_ids);
+      // a partition has at most 2 x n_slots ops, each emitting at most n_slots + 1 load changes
+      if ((SL + 1) * 2 * SL * std::max(0, a.base->n_parts) >= (1ll << 31))
+        throw_err(BLANCE_ERR_UNSUPPORTED, name + ": the load needs (n_slots + 1) x 2 x n_slots x n_parts < 2^31");
+      if (K >= (1ll << 32)) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": the load needs (n_states + 1) x n_node_ids < 2^32");
+      q.load = a.load;
     }
     if (e.null_ctx == CTX_NEED) need_ctx(ctx);
     if (a.n <= 0) bad("n must be positive");
@@ -2868,6 +2993,20 @@ extern "C" int blance_plan_scenarios_exposure(blance_ctx* ctx, const blance_plan
   a.n_move_conc = n_move_conc; a.move_conc = move_conc; a.node_has_mover = node_has_mover; a.out = out; a.sched = sched;
   a.aopts = aopts; a.audit = audit; a.eopts = eopts; a.series_cap = series_cap; a.expo = expo;
   return plan_request(ctx, Entry{"blance_plan_scenarios_exposure", false, false, ALWAYS, MAY, ALWAYS, false, CTX_FAN_OUT}, a);
+}
+
+extern "C" int blance_plan_scenarios_load(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                                          const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                                          int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                                          blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                                          const blance_audit_opts* aopts, blance_audit_out* audit,
+                                          const blance_audit_opts* eopts, int32_t series_cap, blance_exposure_out* expo,
+                                          blance_load_out* load) {
+  WaveArgs a;
+  a.base = base; a.n = n; a.sc = sc; a.opts = opts; a.favor_min = favor_min_nodes; a.max_concurrent = max_concurrent;
+  a.n_move_conc = n_move_conc; a.move_conc = move_conc; a.node_has_mover = node_has_mover; a.out = out; a.sched = sched;
+  a.aopts = aopts; a.audit = audit; a.eopts = eopts; a.series_cap = series_cap; a.expo = expo; a.load = load;
+  return plan_request(ctx, Entry{"blance_plan_scenarios_load", false, false, ALWAYS, MAY, MAY, false, CTX_FAN_OUT, ALWAYS}, a);
 }
 
 // blance_map_audit / blance_plan_audit: one audit on buffers of its own.
@@ -3236,6 +3375,86 @@ extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const bl
     out->kernel_ms = 0.f;
     cudaEventElapsedTime(&out->kernel_ms, dev->ev[0], dev->ev[1]);
     expo_unpack(r, 0, R, dom ? h_key.data() : nullptr, V, *out);
+  });
+}
+
+// Each node's load over the handle's last schedule (node_load.cu in libblance_b200_load.so; include/blance_b200.h).
+extern "C" int blance_moves_load(blance_ctx* ctx, blance_moves* mv, const blance_load_in* in, blance_load_out* out) {
+  return entry(ctx, [&](Device& device) {
+    const std::string name = "blance_moves_load";
+    if (!ctx || !mv || !in || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": ctx, moves, in or out is NULL");
+    if (mv->sched_rounds < 0 || !mv->sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": no schedule was computed on this handle");
+    const int S = (int)mv->slot_off.size() - 1, SL = mv->slot_off[(size_t)S];
+    if (S > BL_S_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 8 states");
+    if (SL > BL_SLP_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 32 slots per row");
+    const int P = mv->n_parts, NU = mv->n_node_ids, R = mv->sched_rounds;
+    const long long T = mv->total_ops, M = mv->sched_moves;
+    std::vector<int32_t> weight(in->part_weight ? (size_t)P : 0);
+    long long total_w = in->part_weight ? 0 : P;
+    for (int p = 0; p < (int)weight.size(); ++p) {
+      const bool has = !in->part_has_weight || in->part_has_weight[p];
+      weight[(size_t)p] = has ? in->part_weight[p] : 1;
+      if (weight[(size_t)p] < 0 || weight[(size_t)p] > 999999999)
+        throw_err(BLANCE_ERR_INVALID_ARG, name + ": the weight of partition " + std::to_string(p) + " is outside [0, 999999999]");
+      total_w = std::min(total_w + weight[(size_t)p], 1ll << 31);   // saturated: the product below cannot overflow
+    }
+    if (total_w * std::max(SL, 1) >= (1ll << 31))
+      throw_err(BLANCE_ERR_UNSUPPORTED, name + ": a node's load can reach 2^31 (sum of weights x max(n_slots, 1))");
+    if ((long long)(SL + 1) * M >= (1ll << 31)) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": (n_slots + 1) x moves_done reaches 2^31");
+    const long long nk = (long long)(S + 1) * NU;
+    if (nk >= (1ll << 32)) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": (n_states + 1) x n_node_ids reaches 2^32");
+    blance_ctx* dev = device();
+    cudaStream_t st = dev->stream;
+    blance_load::LoadArgs A{};
+    A.beg = mv->d_beg; A.op_off = mv->d_off; A.op_node = mv->d_node; A.op_state = mv->d_state; A.op_kind = mv->d_kind;
+    A.stride = SL; A.P = P; A.S = S; A.SL = SL; A.NU = NU;
+    for (int s = 0; s <= S; ++s) A.slot_off[s] = mv->slot_off[(size_t)s];
+    int32_t *op_round = nullptr, *d_weight = nullptr;
+    const size_t K = (size_t)std::max(nk, 1ll);
+    CUDA(blance_load::load_scan_bytes(P, &A.scan_tmp_bytes, st));
+    Arena a;
+    a.add(op_round, (size_t)std::max(T, 1ll));
+    if (!weight.empty()) a.add(d_weight, (size_t)P);
+    a.add(A.node_beg, K); a.add(A.node_end, K); a.add(A.node_peak, K); a.add(A.node_peak_round, K); a.add(A.peak_key, K);
+    a.add(A.over_key, 1); a.add(A.ev_count, (size_t)P + 1); a.add(A.ev_off, (size_t)P + 1); a.add(A.scan_tmp, A.scan_tmp_bytes);
+    a.alloc(st, "the load");
+    A.op_round = op_round; A.weight = d_weight;
+    CUDA(cudaEventRecord(dev->ev[0], st));
+    if (d_weight) CUDA(cudaMemcpyAsync(d_weight, weight.data(), sizeof(int32_t) * (size_t)P, cudaMemcpyHostToDevice, st));
+    CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(T, 1ll), st));
+    if (M > 0) launch(dev, k_expo_op_round, grid_for(dev, M, 256), 256, 0, M, R, (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
+    CUDA(blance_load::load_count(A, dev->sm_count, st, &dev->launches));
+    long long NE = 0;
+    CUDA(cudaMemcpyAsync(&NE, A.ev_off + P, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    // the events, sized exactly; keys ((n (S + 1) + s) << 32) | t
+    int key_bits = 1;
+    while ((1ll << key_bits) < nk) ++key_bits;
+    Arena ev;
+    if (NE > 0) {
+      CUDA(blance_load::load_event_bytes(NE, key_bits, &A.ev_tmp_bytes, st));
+      const size_t n = (size_t)NE;
+      ev.add(A.ev_key, n); ev.add(A.ev_key2, n); ev.add(A.run_key, n); ev.add(A.ev_val, n); ev.add(A.ev_val2, n);
+      ev.add(A.run_val, n); ev.add(A.run_sum, n); ev.add(A.n_runs, 1); ev.add(A.ev_tmp, A.ev_tmp_bytes);
+      ev.alloc(st, "the load's events");
+    }
+    CUDA(blance_load::load_peaks(A, NE, key_bits, dev->sm_count, st, &dev->launches));
+    CUDA(cudaEventRecord(dev->ev[1], st));
+    unsigned long long over = 0;
+    const size_t kb = sizeof(int64_t) * (size_t)nk;
+    if (nk > 0) {
+      if (out->node_beg) CUDA(cudaMemcpyAsync(out->node_beg, A.node_beg, kb, cudaMemcpyDeviceToHost, st));
+      if (out->node_end) CUDA(cudaMemcpyAsync(out->node_end, A.node_end, kb, cudaMemcpyDeviceToHost, st));
+      if (out->node_peak) CUDA(cudaMemcpyAsync(out->node_peak, A.node_peak, kb, cudaMemcpyDeviceToHost, st));
+      if (out->node_peak_round) CUDA(cudaMemcpyAsync(out->node_peak_round, A.node_peak_round, sizeof(int32_t) * (size_t)nk, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA(cudaMemcpyAsync(&over, A.over_key, sizeof over, cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    out->rounds = R;
+    out->over_max = NU > 0 ? (int64_t)(over >> 32) : 0;
+    out->over_node = NU > 0 ? (int32_t)(0xFFFFFFFFu - (uint32_t)over) : -1;
+    out->kernel_ms = 0.f;
+    cudaEventElapsedTime(&out->kernel_ms, dev->ev[0], dev->ev[1]);
   });
 }
 

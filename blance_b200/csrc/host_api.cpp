@@ -1938,4 +1938,37 @@ ExposureResult OrchestrateExposure(const PartitionModel& model, const Orchestrat
   return name_exposure(b, R1, f.names, o->names);
 }
 
+LoadResult OrchestrateLoad(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
+                           const PartitionMap& begMap, const PartitionMap& endMap,
+                           const std::optional<std::unordered_map<std::string, int>>& partitionWeights) {
+  const auto o = orchestrate(model, options, nodesAll, begMap, endMap);
+  const MovesTables& t = o->t;
+  const size_t S = t.state_names.size(), P = o->names.size(), NN = t.nodes.names.size(), K = (S + 1) * NN;
+  std::vector<int32_t> weight(partitionWeights ? P : 0, 1);
+  for (size_t p = 0; p < weight.size(); ++p) {
+    auto it = partitionWeights->find(o->names[p]);
+    if (it != partitionWeights->end()) weight[p] = it->second;
+  }
+  std::vector<int64_t> beg(std::max<size_t>(K, 1)), end(beg.size()), peak(beg.size());
+  std::vector<int32_t> peak_round(beg.size());
+  blance_load_in in{weight.empty() ? nullptr : weight.data(), nullptr};
+  blance_load_out out{};
+  out.node_beg = beg.data(); out.node_end = end.data(); out.node_peak = peak.data(); out.node_peak_round = peak_round.data();
+  o->check(blance_moves_load(o->ctx, o->h.get(), &in, &out), "blance_moves_load");
+  LoadResult r;
+  r.Rounds = out.rounds;
+  for (size_t s = 0; s <= S; ++s)
+    for (size_t q = 0; q < NN; ++q) {
+      const size_t i = s * NN + q;
+      if (peak[i] == 0) continue;                    // the peak bounds both ends
+      const NodeLoad l{beg[i], end[i], peak[i], peak_round[i]};
+      if (s < S) r.States[t.state_names[s]][t.nodes.names[q]] = l;
+      else r.Nodes[t.nodes.names[q]] = l;
+    }
+  r.OverMax = out.over_max;
+  r.OverNode = out.over_node >= 0 ? t.nodes.names[size_t(out.over_node)] : std::string();
+  r.KernelMs = out.kernel_ms;
+  return r;
+}
+
 }  // namespace blance

@@ -342,6 +342,30 @@ ExposureResult OrchestrateExposure(const PartitionModel& model, const Orchestrat
                                    const PartitionMap& begMap, const PartitionMap& endMap,
                                    const std::optional<std::unordered_map<std::string, std::string>>& nodeHierarchy);
 
+// One node's load in one state or in all (blance_moves_load): on the first map, on the last, and its peak over every
+// map of the rebalance with the first round that reaches it.
+struct NodeLoad {
+  int64_t Beg = 0, End = 0, Peak = 0;
+  int32_t PeakRound = 0;
+};
+
+struct LoadResult {
+  int32_t Rounds = 0;
+  std::unordered_map<std::string, std::unordered_map<std::string, NodeLoad>> States;   // state -> node; nonzero only
+  std::unordered_map<std::string, NodeLoad> Nodes;                                     // node, over all states; nonzero only
+  int64_t OverMax = 0;          // the largest Nodes[q].Peak - max(Beg, End)
+  std::string OverNode;         // the node that reaches it first in node-id order (nodesAll first); "" without nodes
+  float KernelMs = 0.f;
+};
+
+// Each node's load while that rebalance runs (blance_moves_load, include/blance_b200.h): the same move lists and
+// schedule as OrchestrateSchedule, and the maps M_0 .. M_R it passes through.  A partition weighs its entry of
+// partitionWeights, 1 when it has none (the rule of countStateNodes, plan.go:374-399).  Throws BlanceError for what
+// OrchestrateSchedule or blance_moves_load rejects (e.g. a weight outside [0, 999999999]).
+LoadResult OrchestrateLoad(const PartitionModel& model, const OrchestratorOptions& options, const Strs& nodesAll,
+                           const PartitionMap& begMap, const PartitionMap& endMap,
+                           const std::optional<std::unordered_map<std::string, int>>& partitionWeights);
+
 // ---------------------------------------------------------------------------------
 // The interning layer, exposed so that tests can drive the SAME tables through the
 // CPU oracle and compare array for array.

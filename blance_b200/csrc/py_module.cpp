@@ -325,6 +325,36 @@ PYBIND11_MODULE(_host, m) {
   }, py::arg("model"), py::arg("max_concurrent"), py::arg("favor"), py::arg("nodes_all"), py::arg("beg"), py::arg("end"),
      py::arg("node_hierarchy") = py::none());
 
+  m.def("OrchestrateLoad", [](const PyModel& model, int max_concurrent, bool favor, const Strs& nodes_all,
+                              const PyPartitionMap& beg, const PyPartitionMap& end,
+                              const std::optional<std::unordered_map<std::string, int>>& weights) {
+    OrchestratorOptions o;
+    o.MaxConcurrentPartitionMovesPerNode = max_concurrent;
+    o.FavorMinNodes = favor;
+    const PartitionMap b = to_map(beg), e = to_map(end);
+    LoadResult r;
+    {
+      py::gil_scoped_release rel;
+      r = OrchestrateLoad(to_model(model), o, nodes_all, b, e, weights);
+    }
+    auto one = [](const NodeLoad& l) {
+      py::dict d;
+      d["beg"] = l.Beg; d["end"] = l.End; d["peak"] = l.Peak; d["peak_round"] = l.PeakRound;
+      return d;
+    };
+    py::dict states, nodes, d;
+    for (const auto& s : r.States) {
+      py::dict sd;
+      for (const auto& q : s.second) sd[py::str(q.first)] = one(q.second);
+      states[py::str(s.first)] = sd;
+    }
+    for (const auto& q : r.Nodes) nodes[py::str(q.first)] = one(q.second);
+    d["rounds"] = r.Rounds; d["states"] = states; d["nodes"] = nodes; d["over_max"] = r.OverMax; d["over_node"] = r.OverNode;
+    d["kernel_ms"] = r.KernelMs;
+    return d;
+  }, py::arg("model"), py::arg("max_concurrent"), py::arg("favor"), py::arg("nodes_all"), py::arg("beg"), py::arg("end"),
+     py::arg("partition_weights") = py::none());
+
   py::class_<PyInterned>(m, "InternedPlan")
       .def_property_readonly("in_ptr", [](const PyInterned& s) { return (uintptr_t)&s.ip->in; })
       .def_property_readonly("n_nodes", [](const PyInterned& s) { return s.ip->in.n_nodes; })

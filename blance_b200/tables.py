@@ -456,6 +456,20 @@ class _ChainAnalysis:
                 x.exposures = [e.result() for e in self.net_expo[i]]
 
 
+def _load_buffers(S, NU):
+    """The arrays of one blance_load_out ([S + 1][NU] each) and the struct pointing at them."""
+    res = dict(node_beg=np.zeros((S + 1, NU), np.int64), node_end=np.zeros((S + 1, NU), np.int64),
+               node_peak=np.zeros((S + 1, NU), np.int64), node_peak_round=np.zeros((S + 1, NU), np.int32))
+    out = api.LoadOut()
+    for k, a in res.items():
+        setattr(out, k, a.ctypes.data if a.size else None)
+    return res, out
+
+
+def _load_result(res, out):
+    return dict(res, rounds=out.rounds, over_max=out.over_max, over_node=out.over_node, kernel_ms=out.kernel_ms)
+
+
 class Context:
     """A blance_ctx* (one per process/GPU)."""
 
@@ -464,6 +478,7 @@ class Context:
         self.lib = api.capi()
         self.ptr = ctypes.c_void_p()
         self._rounds = {}                     # moves handle -> R of its last moves_schedule
+        self._states = {}                     # moves handle -> its n_states (sizes moves_load's arrays)
         if device_ids is not None:
             arr = (ctypes.c_int * len(device_ids))(*device_ids)
             st = self.lib.blance_ctx_create_multi(ctypes.byref(self.ptr), arr, len(device_ids))
@@ -519,7 +534,7 @@ class Context:
         return r
 
     def plan_scenarios(self, base_tables, scenarios, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None,
-                       schedule=None, node_has_mover=None, audit=None, exposure=None):
+                       schedule=None, node_has_mover=None, audit=None, exposure=None, load=False):
         """blance_plan_scenarios: what-if variants of one cluster.  A scenario is a dict of SCENARIO_FIELDS
         (missing keys keep the base's value); want_rows lists the scenarios whose next rows, shapes and warnings
         are copied out.  opts (None, or one dict of OPT_GROUPS keys per scenario) calls blance_plan_scenarios_ex
@@ -533,7 +548,10 @@ class Context:
         blance_plan_scenarios_exposure; each result's `exposures` is then one dict per count, shaped as
         moves_exposure's, with series [6][min(R + 1, series_cap)].  dom=False leaves out dom_peak / dom_peak_round (the
         device then skips the fault-domain work), parts=False the per-partition arrays (nothing of n_parts size is
-        copied out)."""
+        copied out).  load=True needs `schedule` and calls blance_plan_scenarios_load (with the audit and exposure
+        asked for); each result's `loads` is then one dict per count, shaped as moves_load's."""
+        if load and not schedule:
+            raise ValueError("the load needs a schedule: pass schedule=[counts]")
         if exposure is not None:
             unknown = set(exposure) - set(EXPOSURE_KEYS)
             if unknown:
@@ -559,16 +577,20 @@ class Context:
                                                                                         keep)
             an = _ChainAnalysis(base_tables, [[r] for r in results], None, lambda i, t: None if opts is None else opts[i],
                                 None if schedule is None else counts, audit, n_dom, exposure, True, V, cap, dom, parts)
-            # each scenario entry point with an analysis takes a prefix of blance_plan_scenarios_exposure's arguments
-            what, k = (("blance_plan_scenarios_exposure", 17) if exposure is not None else
+            # each scenario entry point with an analysis takes a prefix of blance_plan_scenarios_load's arguments
+            what, k = (("blance_plan_scenarios_load", 18) if load else ("blance_plan_scenarios_exposure", 17) if exposure is not None else
                        ("blance_plan_scenarios_audit", 14) if audit is not None else ("blance_plan_scenarios_schedule", 12))
+            loads = [[_load_buffers(base_tables.n_states, base_tables.n_node_ids) for _ in range(counts.size)] for _ in range(n)] if load else []
+            l_outs = (api.LoadOut * max(1, n * counts.size))(*[o for row in loads for _, o in row]) if load else None
             args = (args + (counts.size, counts.ctypes.data if counts.size else None, mover, outs, an.sch, a_opts, an.auds, e_opts, cap,
-                            an.exps))[:k]
+                            an.exps, l_outs))[:k]
         self._check(getattr(self.lib, what)(*args), what)
         if an is not None:
             an.fill()
-        for r, o in zip(results, outs):
+        for i, (r, o) in enumerate(zip(results, outs)):
             r.out = o
+            if load:
+                r.loads = [_load_result(res, l_outs[i * counts.size + k]) for k, (res, _) in enumerate(loads[i])]
         return results
 
     def plan_chains(self, base_tables, chains, favor_min_nodes, max_concurrent=0, want_rows=(), opts=None, net=True,
@@ -799,6 +821,7 @@ class Context:
                                           slot_off.ctypes.data, beg.ctypes.data, end.ctypes.data, int(bool(favor_min_nodes)),
                                           int(n_node_ids), ctypes.byref(h), ctypes.byref(tot))
         self._check(st, "blance_moves_create")
+        self._states[h.value] = n_states
         return (h, beg.shape[0], int(n_node_ids)), int(tot.value)
 
     def moves_fetch(self, handle, total_ops):
@@ -876,8 +899,32 @@ class Context:
                    peak_round=np.array(out.peak_round[:], np.int32), area=np.array(out.area[:], np.int64))
         return res
 
+    def moves_load(self, handle, part_weight=None, part_has_weight=None):
+        """blance_moves_load: each node's load over the maps the handle's last moves_schedule passes through
+        (include/blance_b200.h).  part_weight [n_parts] (None: every partition weighs 1) and part_has_weight [n_parts]
+        (None: every partition has its weight).  Returns a dict: node_beg / node_end / node_peak / node_peak_round
+        [n_states + 1][n_node_ids] (row n_states: every state), over_max, over_node, rounds and kernel_ms."""
+        h, n_parts, n_node_ids = handle
+        keep = []
+        l_in = api.LoadIn(None, None)
+        for name, arr, dt in (("part_weight", part_weight, np.int32), ("part_has_weight", part_has_weight, np.uint8)):
+            if arr is not None:
+                a = np.ascontiguousarray(arr, dt)
+                if a.size != n_parts:
+                    raise ValueError("%s must have n_parts = %d entries" % (name, n_parts))
+                keep.append(a)
+                setattr(l_in, name, a.ctypes.data if a.size else None)
+        S = self._states.get(h.value)
+        if S is None or h.value not in self._rounds:     # the library reports what is missing
+            self._check(self.lib.blance_moves_load(self.ptr, h, ctypes.byref(l_in), ctypes.byref(api.LoadOut())), "blance_moves_load")
+            raise ValueError("create the handle with moves_create and schedule it with moves_schedule before moves_load")
+        res, out = _load_buffers(S, n_node_ids)
+        self._check(self.lib.blance_moves_load(self.ptr, h, ctypes.byref(l_in), ctypes.byref(out)), "blance_moves_load")
+        return _load_result(res, out)
+
     def moves_free(self, handle):
         self._rounds.pop(handle[0].value, None)
+        self._states.pop(handle[0].value, None)
         self.lib.blance_moves_free(self.ptr, handle[0])
 
     def kernel_launches(self):

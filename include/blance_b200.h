@@ -697,6 +697,89 @@ typedef struct blance_exposure_out {
 
 int blance_moves_exposure(blance_ctx* ctx, blance_moves* moves, const blance_exposure_in* in, blance_exposure_out* out);
 
+/* ---- each node's load while a rebalance runs (blance_moves_load) ---------------------------------------------
+ * Does a node run out of room while the rebalance runs?  Without favor_min_nodes every move adds the new copy before
+ * it deletes the old one (moves.go:35-40), so a node that gains copies early and loses its own late holds more, at
+ * some round in between, than both its start and its end load.  The load counts that over the maps a rebalance passes
+ * through under the handle's LAST blance_moves_schedule, on the device, without copying the schedule or any map out.
+ *
+ * Maps and entries are exactly those of blance_moves_exposure: M_0 .. M_R, M_0 the handle's beg rows, op k applied
+ * at the end of its round rho_k, an op that was never scheduled never applied.
+ * Weight.  Partition p weighs w_p: part_weight[p] when it has one, else 1 (the rule of countStateNodes,
+ * plan.go:374-399, and of state_node_load).  part_weight NULL: every partition weighs 1; part_has_weight NULL with a
+ * part_weight: every partition has its weight.
+ * Load.  load_t[s][q] is the sum of w_p over the entries (q, s) of M_t; row s = n_states is the sum over all states.
+ * An entry on an id outside [0, n_node_ids) counts nowhere.
+ * Outputs (every array may be NULL; arrays are [n_states + 1][n_node_ids]):
+ *   rounds                     R, echoed
+ *   node_beg, node_end         the load on M_0 and on M_R (node_end is not the end rows' load when partitions are stuck)
+ *   node_peak                  max over t of load_t
+ *   node_peak_round            the smallest t that reaches it
+ *   over_max, over_node        the largest node_peak[S][q] - max(node_beg[S][q], node_end[S][q]) and the lowest q
+ *                              that reaches it (over_node = -1 without node ids): how far the busiest node overshoots
+ *                              both ends of the rebalance
+ *   kernel_ms                  time of the load on the stream: events around its device work, which also span the
+ *                              host's two waits for the stream (the event count, then the merged runs) and the
+ *                              allocation of the event buffer between them
+ * Every value equals a literal replay of the schedule; nothing depends on thread order.  No output is sized by
+ * nodes x rounds: there is no per-node series.
+ *
+ * Bounds.  On any M_t node q holds, for partition p, either its beg entries or at most one entry, so its load is at
+ * most sum_p w_p x max(n_slots, 1); the call refuses that reaching 2^31, and below it every load is exact.
+ * Errors, before any device work: a NULL ctx, moves, in or out, a handle without a schedule, a weight below 0 or
+ * above 999999999 (BLANCE_ERR_INVALID_ARG); more than 8 states or 32 slots, the load bound above, (n_slots + 1) x
+ * moves_done >= 2^31 (each scheduled op emits at most n_slots + 1 load changes) or (n_states + 1) x n_node_ids >= 2^32
+ * (BLANCE_ERR_UNSUPPORTED).  The device work is bounded by the handle's sizes plus an event buffer sized exactly by a
+ * counting pass (DESIGN.md section 18); BLANCE_ERR_NOMEM names the load when that does not fit. */
+typedef struct blance_load_in {
+  const int32_t* part_weight;         /* [n_parts] or NULL */
+  const uint8_t* part_has_weight;     /* [n_parts] or NULL */
+} blance_load_in;
+
+typedef struct blance_load_out {
+  int32_t rounds;
+  int64_t* node_beg;                  /* [n_states + 1][n_node_ids] */
+  int64_t* node_end;                  /* [n_states + 1][n_node_ids] */
+  int64_t* node_peak;                 /* [n_states + 1][n_node_ids] */
+  int32_t* node_peak_round;           /* [n_states + 1][n_node_ids] */
+  int64_t over_max;
+  int32_t over_node;
+  float kernel_ms;
+} blance_load_out;
+
+int blance_moves_load(blance_ctx* ctx, blance_moves* moves, const blance_load_in* in, blance_load_out* out);
+
+/* ---- each node's load while every scenario's rebalance runs (blance_plan_scenarios_load) -----------------------
+ * blance_plan_scenarios_exposure with the exposure optional (expo NULL: none; eopts and series_cap are then only
+ * checked), and the node load of every (scenario, count) pair's schedule inside the wave.  out, sched, audit and expo
+ * equal what blance_plan_scenarios_exposure returns for the same arguments (with expo NULL: blance_plan_scenarios_audit,
+ * or blance_plan_scenarios_schedule with audit NULL too).
+ *
+ * load[i * n_move_conc + k] equals blance_moves_load on the handle of scenario i's rebalance at move_conc[k], the
+ * handle and its schedule as blance_plan_scenarios_exposure defines them for expo, with scenario i's own partition
+ * weights (its BLANCE_OPT_PART_WEIGHTS overrides applied; weight 1 where has_part_weights is 0 or a partition has
+ * none): the rule of state_node_load, so with no stuck partition node_end's state rows equal out[i].state_node_load.
+ * A partition in neither map is no partition of begMap and counts nowhere.  The count bound every scenario passes
+ * (sum of |weight| x max(n_slots, 1) < 2^31) bounds every node's load on every map, so the loads are exact; a weight
+ * may be negative where the planner allows one.  kernel_ms is the wave's load time (as blance_moves_load measures it,
+ * over all its members), the same value in each of its members.  No value depends on n, max_concurrent, the wave
+ * size, the engine, the number of devices or the other move_conc.
+ *
+ * Errors, all before any device work: everything blance_plan_scenarios_exposure rejects except a NULL expo; a NULL
+ * load (BLANCE_ERR_INVALID_ARG); (n_slots + 1) x 2 x n_slots x n_parts >= 2^31 or (n_states + 1) x n_node_ids >= 2^32
+ * (BLANCE_ERR_UNSUPPORTED, the static forms of blance_moves_load's event and key bounds).  The per-instance outputs
+ * (36 bytes per (state, node) and 16 per partition) are priced into the wave size; the event buffers are allocated
+ * after the schedules, exactly sized for the wave's instance with the most events, and BLANCE_ERR_NOMEM names the
+ * load when they do not fit (DESIGN.md section 18). */
+int blance_plan_scenarios_load(blance_ctx* ctx, const blance_plan_in* base, int32_t n, const blance_scenario* sc,
+                               const blance_scenario_opts* opts, int32_t favor_min_nodes, int32_t max_concurrent,
+                               int32_t n_move_conc, const int32_t* move_conc, const uint8_t* node_has_mover,
+                               blance_scenario_out* out, blance_scenario_schedule_out* sched,
+                               const blance_audit_opts* aopts, blance_audit_out* audit /* [n] or NULL */,
+                               const blance_audit_opts* eopts, int32_t series_cap,
+                               blance_exposure_out* expo /* [n][n_move_conc] or NULL */,
+                               blance_load_out* load /* [n][n_move_conc] */);
+
 /* ---- the exposure of every scenario's rebalance (blance_plan_scenarios_exposure) ----------------------------
  * blance_plan_scenarios_audit, and the exposure of every (scenario, count) pair's schedule, inside the wave.
  *
