@@ -1,10 +1,7 @@
 """In-tree build of the native pieces (no JIT cache: the .so files live in the source tree, so that a
 copy of the built tree runs on another machine without compiling again).
 
-    libblance_b200_load.so  nvcc, sm_90a: the node-load kernels (csrc/node_load.cu), hidden visibility: only the
-                        launchers of csrc/node_load.h are exported
-    libblance_b200.so   nvcc, sm_90a (H100) only: the CUDA kernels + the C ABI (include/blance_b200.h), linked
-                        against libblance_b200_load.so
+    libblance_b200.so   nvcc, sm_90a (H100) only: the CUDA kernels + the C ABI (include/blance_b200.h)
     _host*.so           g++: the C++ host mirror of blance's api.go (pybind11 face), linked
                         against libblance_b200.so
 
@@ -43,39 +40,22 @@ def lib_path():
     return os.path.join(LIBDIR, "libblance_b200.so")
 
 
-def load_lib_path():
-    return os.path.join(LIBDIR, "libblance_b200_load.so")
-
-
 def host_module_path():
     return os.path.join(HERE, "_host" + sysconfig.get_config_var("EXT_SUFFIX"))
-
-
-def _nvcc(srcs, deps, out, extra, force, verbose):
-    if force or _newer(deps, out):
-        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-I" + INCLUDE, "-I" + CSRC] + srcs + extra + ["-o", out]
-        log = _run(cmd)
-        if verbose:
-            print(log)
-    return out
-
-
-def build_load_lib(force=False, verbose=False):
-    """The node-load kernels in a library of their own: both libraries link cudart statically and instantiate CUB,
-    so with hidden visibility neither can bind a kernel stub of the other."""
-    os.makedirs(LIBDIR, exist_ok=True)
-    srcs = [os.path.join(CSRC, "node_load.cu")]
-    deps = srcs + [os.path.join(CSRC, "node_load.h"), os.path.join(CSRC, "device_types.cuh"), os.path.join(INCLUDE, "blance_b200.h")]
-    return _nvcc(srcs, deps, load_lib_path(), ["-Xcompiler", "-fvisibility=hidden"], force, verbose)
 
 
 def build_cuda_lib(force=False, verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     srcs = [os.path.join(CSRC, "c_abi.cu")]
-    deps = srcs + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(CSRC, "count_bound.hpp"), os.path.join(INCLUDE, "blance_b200.h"),
-                                                            os.path.join(CSRC, "node_load.cu"), os.path.join(CSRC, "node_load.h"), load_lib_path()]
-    return _nvcc(srcs, deps, lib_path(), ["-L" + LIBDIR, "-lblance_b200_load", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"], force, verbose)
+    deps = srcs + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(CSRC, "count_bound.hpp"), os.path.join(INCLUDE, "blance_b200.h")]
+    out = lib_path()
+    if force or _newer(deps, out):
+        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-I" + INCLUDE, "-I" + CSRC] + srcs + ["-o", out]
+        log = _run(cmd)
+        if verbose:
+            print(log)
+    return out
 
 
 def build_host_module(force=False):
@@ -93,7 +73,6 @@ def build_host_module(force=False):
 
 
 def build_all(force=False, verbose=False):
-    build_load_lib(force, verbose)
     build_cuda_lib(force, verbose)
     build_host_module(force)
 
@@ -101,6 +80,5 @@ def build_all(force=False, verbose=False):
 if __name__ == "__main__":
     import sys
     build_all(force="--force" in sys.argv, verbose="-v" in sys.argv)
-    print(load_lib_path())
     print(lib_path())
     print(host_module_path())

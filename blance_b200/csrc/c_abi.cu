@@ -30,7 +30,7 @@
 #include "count_bound.hpp"
 #include "device_types.cuh"
 #include "exposure.cuh"
-#include "node_load.h"
+#include "node_load.cuh"
 #include "wave_schedule.cuh"
 
 using namespace blance_dev;
@@ -112,8 +112,7 @@ struct blance_ctx {
   cudaEvent_t ev[8] = {};            // [4], [5]: around the audit kernels; [6], [7]: around a wave's exposures
   int* d_any_active = nullptr;
   int* h_any_active = nullptr;       // pinned
-  long long launches = 0;            // kernels launched so far by this library's own launches and by the node-load
-                                     // launchers of libblance_b200_load.so (CUB's launches are not counted)
+  long long launches = 0;            // kernels of this library launched so far
   void* h_stage = nullptr;           // pinned staging of a batch (kept between calls, grow-only)
   size_t h_stage_bytes = 0;
   std::vector<blance_ctx*> children; // blance_ctx_create_multi: one single-device context per GPU
@@ -1879,9 +1878,14 @@ struct Sweep {
         V((long long)r.base->n_node_ids + (r.er ? r.er->n_domains : 0)), stride(summary_stride(*r.base)) {}
 };
 
-// The per-instance buffers of the node loads of nw scenarios x nc counts that are priced into a wave: [ni][(S + 1) NU]
-// loads, peaks and packed maxima, one packed overshoot each, and [ni][PU + 1] event counts and offsets.  The op states
-// and rounds are the exposure's (expo_slices), laid out here when no exposure is asked for.
+// ---------------------------------------------------------------------------------------
+// Each node's load over the maps of a schedule (node_load.cuh; include/blance_b200.h): one engine for a moves handle
+// and a wave.
+
+// The per-instance buffers of the node loads of ni instances (a moves handle's one, or the nw scenarios x nc counts
+// priced into a wave): [ni][(S + 1) NU] loads, peaks and packed maxima, one packed overshoot each, and [ni][P + 1]
+// event counts and offsets.  A wave's op states and rounds are the exposure's (expo_slices), laid out here when no
+// exposure is asked for.
 struct LoadBufs {
   long long *node_beg = nullptr, *node_end = nullptr, *node_peak = nullptr;
   int32_t* node_peak_round = nullptr;
@@ -1896,6 +1900,132 @@ static void load_slices(Arena& a, LoadBufs& b, WSched& w, bool expo, long long n
   a.add(b.node_beg, (size_t)(ni * K)); a.add(b.node_end, (size_t)(ni * K)); a.add(b.node_peak, (size_t)(ni * K));
   a.add(b.node_peak_round, (size_t)(ni * K)); a.add(b.peak_key, (size_t)(ni * K)); a.add(b.over_key, (size_t)ni);
   a.add(b.ev_count, (size_t)(ni * (PU + 1))); a.add(b.ev_off, (size_t)(ni * (PU + 1)));
+}
+
+// Scratch bytes of the event-count scan over P partitions.
+static size_t load_scan_bytes(int32_t P, cudaStream_t st) {
+  size_t bytes = 0;
+  CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const long long*)nullptr, (long long*)nullptr, P + 1, st));
+  return bytes;
+}
+
+// Scratch bytes of the sort, merge and scan of NE events whose keys use the low 32 + key_bits bits.
+static size_t load_event_bytes(long long NE, int key_bits, cudaStream_t st) {
+  const int ne = (int)NE;
+  size_t sort_b = 0, red_b = 0, scan_b = 0;
+  CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                       (const int32_t*)nullptr, (int32_t*)nullptr, ne, 0, 32 + key_bits, st));
+  CUDA(cub::DeviceReduce::ReduceByKey(nullptr, red_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                      (const int32_t*)nullptr, (int32_t*)nullptr, (int*)nullptr, blance_load::Sum(), ne, st));
+  CUDA(cub::DeviceScan::InclusiveScanByKey(nullptr, scan_b, (const unsigned long long*)nullptr, (const int32_t*)nullptr,
+                                           (int32_t*)nullptr, blance_load::Sum(), ne, blance_load::SameKey(), st));
+  return std::max(sort_b, std::max(red_b, scan_b));
+}
+
+// node_beg (the load on M_0) and the exact event count: ev_off[p] is partition p's first event, ev_off[P] the total.
+static void load_count(blance_ctx* dev, const blance_load::LoadArgs& A) {
+  cudaStream_t st = dev->stream;
+  const long long nk = (long long)(A.S + 1) * A.NU;
+  CUDA(cudaMemsetAsync(A.node_beg, 0, sizeof(long long) * (size_t)std::max(nk, 1ll), st));
+  CUDA(cudaMemsetAsync(A.ev_count + A.P, 0, sizeof(long long), st));
+  if (A.P == 0) {
+    CUDA(cudaMemsetAsync(A.ev_off, 0, sizeof(long long), st));
+    return;
+  }
+  launch(dev, blance_load::k_load_walk<0>, grid_for(dev, A.P, 256), 256, 0, A);
+  size_t b = A.scan_tmp_bytes;
+  CUDA(cub::DeviceScan::ExclusiveSum(A.scan_tmp, b, A.ev_count, A.ev_off, A.P + 1, st));
+}
+
+// Emits the NE events, merges them per (node, state, t), scans them per (node, state) and takes each key's peak;
+// fills node_end, node_peak, node_peak_round and over_key.  Waits for the stream once (the number of merged runs).
+static void load_peaks(blance_ctx* dev, const blance_load::LoadArgs& A, long long NE, int key_bits) {
+  cudaStream_t st = dev->stream;
+  const long long nk = (long long)(A.S + 1) * A.NU;
+  if (nk == 0) {
+    CUDA(cudaMemsetAsync(A.over_key, 0, sizeof(unsigned long long), st));
+    return;
+  }
+  launch(dev, blance_load::k_load_init, grid_for(dev, nk, 256), 256, 0, nk, A.node_beg, A.node_end, A.peak_key);
+  CUDA(cudaMemsetAsync(A.over_key, 0, sizeof(unsigned long long), st));
+  if (NE > 0) {
+    const int ne = (int)NE;
+    launch(dev, blance_load::k_load_walk<1>, grid_for(dev, A.P, 256), 256, 0, A);
+    size_t b = A.ev_tmp_bytes;
+    CUDA(cub::DeviceRadixSort::SortPairs(A.ev_tmp, b, A.ev_key, A.ev_key2, A.ev_val, A.ev_val2, ne, 0, 32 + key_bits, st));
+    b = A.ev_tmp_bytes;
+    CUDA(cub::DeviceReduce::ReduceByKey(A.ev_tmp, b, A.ev_key2, A.run_key, A.ev_val2, A.run_val, A.n_runs, blance_load::Sum(), ne, st));
+    int h_runs = 0;                                // only the merged runs are scanned
+    CUDA(cudaMemcpyAsync(&h_runs, A.n_runs, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA(cudaStreamSynchronize(st));
+    b = A.ev_tmp_bytes;
+    CUDA(cub::DeviceScan::InclusiveScanByKey(A.ev_tmp, b, A.run_key, A.run_val, A.run_sum, blance_load::Sum(), h_runs,
+                                             blance_load::SameKey(), st));
+    if (h_runs > 0)
+      launch(dev, blance_load::k_load_peak, grid_for(dev, h_runs, 256), 256, 0, h_runs, A.S, A.NU, A.run_key, A.run_sum, A.node_beg,
+             A.node_end, A.peak_key);
+  }
+  launch(dev, blance_load::k_load_final, grid_for(dev, nk, 256), 256, 0, A.S, A.NU, A.peak_key, A.node_beg, A.node_end, A.node_peak,
+         A.node_peak_round, A.over_key);
+}
+
+// Runs the node loads of the instances `args` (one at least; inputs and scan scratch set by the caller, results
+// pointed into b here).  Every instance is counted first; the event buffers are then allocated once, exactly sized for
+// the instance with the most events, and the instances run one by one on them.  Records `stop` after the last one,
+// then copies instance i's arrays that *outs[i] asks for and its overshoot into *outs[i].  Returns the event buffers'
+// bytes.
+static size_t load_run(blance_ctx* dev, std::vector<blance_load::LoadArgs>& args, const LoadBufs& b,
+                       const std::vector<blance_load_out*>& outs, cudaEvent_t stop) {
+  cudaStream_t st = dev->stream;
+  const long long ni = (long long)args.size(), P = args[0].P, NU = args[0].NU, K = (long long)(args[0].S + 1) * NU;
+  for (long long i = 0; i < ni; ++i) {
+    blance_load::LoadArgs& A = args[(size_t)i];
+    A.node_beg = b.node_beg + i * K; A.node_end = b.node_end + i * K; A.node_peak = b.node_peak + i * K;
+    A.node_peak_round = b.node_peak_round + i * K; A.peak_key = b.peak_key + i * K; A.over_key = b.over_key + i;
+    A.ev_count = b.ev_count + i * (P + 1); A.ev_off = b.ev_off + i * (P + 1);
+    load_count(dev, A);
+  }
+  std::vector<long long> ne((size_t)ni, 0);   // each instance's event count: ev_off[P]
+  CUDA(cudaMemcpy2DAsync(ne.data(), sizeof(long long), b.ev_off + P, sizeof(long long) * (size_t)(P + 1), sizeof(long long), (size_t)ni,
+                         cudaMemcpyDeviceToHost, st));
+  CUDA(cudaStreamSynchronize(st));
+  const long long max_ne = *std::max_element(ne.begin(), ne.end());
+  int key_bits = 1;                           // the events' keys: ((n (S + 1) + s) << 32) | t
+  while ((1ll << key_bits) < K) ++key_bits;
+  blance_load::LoadArgs E{};
+  Arena ev;
+  if (max_ne > 0) {
+    E.ev_tmp_bytes = load_event_bytes(max_ne, key_bits, st);
+    const size_t n = (size_t)max_ne;
+    ev.add(E.ev_key, n); ev.add(E.ev_key2, n); ev.add(E.run_key, n); ev.add(E.ev_val, n); ev.add(E.ev_val2, n);
+    ev.add(E.run_val, n); ev.add(E.run_sum, n); ev.add(E.n_runs, 1); ev.add(E.ev_tmp, E.ev_tmp_bytes);
+    ev.alloc(st, "the load's events");
+  }
+  for (long long i = 0; i < ni; ++i) {
+    blance_load::LoadArgs& A = args[(size_t)i];
+    A.ev_key = E.ev_key; A.ev_key2 = E.ev_key2; A.run_key = E.run_key; A.ev_val = E.ev_val; A.ev_val2 = E.ev_val2;
+    A.run_val = E.run_val; A.run_sum = E.run_sum; A.n_runs = E.n_runs; A.ev_tmp = E.ev_tmp; A.ev_tmp_bytes = E.ev_tmp_bytes;
+    load_peaks(dev, A, ne[(size_t)i], key_bits);
+  }
+  CUDA(cudaEventRecord(stop, st));
+  std::vector<unsigned long long> over((size_t)ni, 0);
+  CUDA(cudaMemcpyAsync(over.data(), b.over_key, sizeof(unsigned long long) * (size_t)ni, cudaMemcpyDeviceToHost, st));
+  const size_t kb = sizeof(int64_t) * (size_t)K;
+  for (long long i = 0; i < ni && K > 0; ++i) {
+    const blance_load_out& o = *outs[(size_t)i];
+    if (o.node_beg) CUDA(cudaMemcpyAsync(o.node_beg, b.node_beg + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_end) CUDA(cudaMemcpyAsync(o.node_end, b.node_end + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_peak) CUDA(cudaMemcpyAsync(o.node_peak, b.node_peak + i * K, kb, cudaMemcpyDeviceToHost, st));
+    if (o.node_peak_round)
+      CUDA(cudaMemcpyAsync(o.node_peak_round, b.node_peak_round + i * K, sizeof(int32_t) * (size_t)K, cudaMemcpyDeviceToHost, st));
+  }
+  CUDA(cudaStreamSynchronize(st));
+  for (long long i = 0; i < ni; ++i) {
+    blance_load_out& o = *outs[(size_t)i];
+    o.over_max = NU > 0 ? (int64_t)(over[(size_t)i] >> 32) : 0;
+    o.over_node = NU > 0 ? (int32_t)(0xFFFFFFFFu - (uint32_t)over[(size_t)i]) : -1;
+  }
+  return ev.bytes();
 }
 
 // The buffers of a wave's analyses: audits, exposures, loads, span accumulators, a chain's net prev rows, flags and
@@ -1996,25 +2126,22 @@ static void wave_exposure(const Sweep& s, Wave& w, const int32_t* beg, const uin
 
 // The node loads of wave w's instances after their schedules (scal: the instances' scalars), from the beg rows / flags
 // `beg` / `pflags` and the members' partition weights over the op table and rounds the schedule left in w.sched;
-// instance i's result goes to outs[out_at(i, nc, per, t)].  Every instance is counted first; the event buffers are
-// then allocated once, exactly sized for the instance with the most events, and the instances run one by one on them.
+// instance i's result goes to outs[out_at(i, nc, per, t)].
 static void wave_load(const Sweep& s, Wave& w, const int32_t* beg, const uint8_t* pflags, blance_load_out* outs, int per, int t,
                       const std::vector<unsigned long long>& scal) {
   blance_ctx* dev = s.ctx;
   cudaStream_t st = dev->stream;
   const blance_plan_in& base = *s.q.base;
-  const int PU = base.n_parts, S = base.n_states, NU = base.n_node_ids;
-  const long long ni = (long long)w.nw * s.nc, K = (long long)(S + 1) * NU;
+  const int PU = base.n_parts, S = base.n_states;
+  const long long ni = (long long)w.nw * s.nc;
   const WSched& W = w.sched;
-  const LoadBufs& b = w.an.load;
   std::vector<blance_load::LoadArgs> args((size_t)ni);
+  std::vector<blance_load_out*> o((size_t)ni);
   Arena scan;
   void* scan_tmp = nullptr;
-  size_t scan_bytes = 0;
-  CUDA(blance_load::load_scan_bytes(PU, &scan_bytes, st));
+  const size_t scan_bytes = load_scan_bytes(PU, st);
   scan.add(scan_tmp, scan_bytes);
   scan.alloc(st, "the load");
-  CUDA(cudaEventRecord(dev->ev[6], st));
   for (long long i = 0; i < ni; ++i) {
     const long long j = i / s.nc;
     const DInst& D = w.pl->h_insts[(size_t)j];
@@ -2023,59 +2150,18 @@ static void wave_load(const Sweep& s, Wave& w, const int32_t* beg, const uint8_t
     A.op_n = W.op_n + j * PU; A.op_node = W.op_node + j * PU * s.MO; A.op_state = W.op_state + j * PU * s.MO;
     A.op_kind = W.op_kind + j * PU * s.MO; A.op_round = W.op_round + i * PU * s.MO; A.MO = s.MO;
     A.weight = w.pl->pool.pweight + D.part_off; A.pflags = pflags + D.part_off; A.has_part_weights = D.has_part_weights;
-    A.P = PU; A.S = S; A.SL = base.n_slots; A.NU = NU;
+    A.P = PU; A.S = S; A.SL = base.n_slots; A.NU = base.n_node_ids;
     for (int k = 0; k <= S; ++k) A.slot_off[k] = base.state_slot_off[k];
-    A.node_beg = b.node_beg + i * K; A.node_end = b.node_end + i * K; A.node_peak = b.node_peak + i * K;
-    A.node_peak_round = b.node_peak_round + i * K; A.peak_key = b.peak_key + i * K; A.over_key = b.over_key + i;
-    A.ev_count = b.ev_count + i * (PU + 1); A.ev_off = b.ev_off + i * (PU + 1);
     A.scan_tmp = scan_tmp; A.scan_tmp_bytes = scan_bytes;
-    CUDA(blance_load::load_count(A, dev->sm_count, st, &dev->launches));
+    o[(size_t)i] = &outs[out_at(s, w, i, s.nc, per, t)];
   }
-  std::vector<long long> ne((size_t)ni, 0);   // each instance's event count: ev_off[P]
-  if (ni > 0)
-    CUDA(cudaMemcpy2DAsync(ne.data(), sizeof(long long), b.ev_off + PU, sizeof(long long) * (size_t)(PU + 1), sizeof(long long), (size_t)ni,
-                           cudaMemcpyDeviceToHost, st));
-  CUDA(cudaStreamSynchronize(st));
-  const long long max_ne = ni > 0 ? *std::max_element(ne.begin(), ne.end()) : 0;
-  int key_bits = 1;
-  while ((1ll << key_bits) < K) ++key_bits;
-  blance_load::LoadArgs E{};
-  Arena ev;
-  if (max_ne > 0) {
-    CUDA(blance_load::load_event_bytes(max_ne, key_bits, &E.ev_tmp_bytes, st));
-    const size_t n = (size_t)max_ne;
-    ev.add(E.ev_key, n); ev.add(E.ev_key2, n); ev.add(E.run_key, n); ev.add(E.ev_val, n); ev.add(E.ev_val2, n);
-    ev.add(E.run_val, n); ev.add(E.run_sum, n); ev.add(E.n_runs, 1); ev.add(E.ev_tmp, E.ev_tmp_bytes);
-    ev.alloc(st, "the load's events");
-  }
-  w.load_bytes = scan.bytes() + ev.bytes();
-  for (long long i = 0; i < ni; ++i) {
-    blance_load::LoadArgs& A = args[(size_t)i];
-    A.ev_key = E.ev_key; A.ev_key2 = E.ev_key2; A.run_key = E.run_key; A.ev_val = E.ev_val; A.ev_val2 = E.ev_val2;
-    A.run_val = E.run_val; A.run_sum = E.run_sum; A.n_runs = E.n_runs; A.ev_tmp = E.ev_tmp; A.ev_tmp_bytes = E.ev_tmp_bytes;
-    CUDA(blance_load::load_peaks(A, ne[(size_t)i], key_bits, dev->sm_count, st, &dev->launches));
-  }
-  CUDA(cudaEventRecord(dev->ev[7], st));
-  std::vector<unsigned long long> over((size_t)ni, 0);
-  if (ni > 0) CUDA(cudaMemcpyAsync(over.data(), b.over_key, sizeof(unsigned long long) * (size_t)ni, cudaMemcpyDeviceToHost, st));
-  const size_t kb = sizeof(int64_t) * (size_t)K;
-  for (long long i = 0; i < ni && K > 0; ++i) {
-    blance_load_out& o = outs[out_at(s, w, i, s.nc, per, t)];
-    if (o.node_beg) CUDA(cudaMemcpyAsync(o.node_beg, b.node_beg + i * K, kb, cudaMemcpyDeviceToHost, st));
-    if (o.node_end) CUDA(cudaMemcpyAsync(o.node_end, b.node_end + i * K, kb, cudaMemcpyDeviceToHost, st));
-    if (o.node_peak) CUDA(cudaMemcpyAsync(o.node_peak, b.node_peak + i * K, kb, cudaMemcpyDeviceToHost, st));
-    if (o.node_peak_round)
-      CUDA(cudaMemcpyAsync(o.node_peak_round, b.node_peak_round + i * K, sizeof(int32_t) * (size_t)K, cudaMemcpyDeviceToHost, st));
-  }
-  CUDA(cudaStreamSynchronize(st));
+  CUDA(cudaEventRecord(dev->ev[6], st));
+  w.load_bytes = scan.bytes() + load_run(dev, args, w.an.load, o, dev->ev[7]);
   w.load_ms = 0.f;
   cudaEventElapsedTime(&w.load_ms, dev->ev[6], dev->ev[7]);
   for (long long i = 0; i < ni; ++i) {
-    blance_load_out& o = outs[out_at(s, w, i, s.nc, per, t)];
-    o.rounds = (int32_t)scal[(size_t)(4 * i)];
-    o.over_max = NU > 0 ? (int64_t)(over[(size_t)i] >> 32) : 0;
-    o.over_node = NU > 0 ? (int32_t)(0xFFFFFFFFu - (uint32_t)over[(size_t)i]) : -1;
-    o.kernel_ms = w.load_ms;
+    o[(size_t)i]->rounds = (int32_t)scal[(size_t)(4 * i)];
+    o[(size_t)i]->kernel_ms = w.load_ms;
   }
 }
 
@@ -3310,15 +3396,31 @@ extern "C" int blance_moves_schedule_fetch(blance_ctx* ctx, blance_moves* mv, in
   });
 }
 
+// The checks of an analysis of the handle's last schedule that the entry point `name` makes first: no NULL argument,
+// a schedule, and at most 8 states and 32 slots (the kernels' limits).
+static void check_moves_sched(const std::string& name, const blance_ctx* ctx, const blance_moves* mv, const void* in, const void* out) {
+  if (!ctx || !mv || !in || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": ctx, moves, in or out is NULL");
+  if (mv->sched_rounds < 0 || !mv->sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": no schedule was computed on this handle");
+  const int S = (int)mv->slot_off.size() - 1;
+  if (S > BL_S_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 8 states");
+  if (mv->slot_off[(size_t)S] > BL_SLP_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 32 slots per row");
+}
+
+// op_round [max(total_ops, 1)]: the round of the handle's last schedule that applies each op, -1 for an op it never
+// scheduled.
+static void moves_op_round(blance_ctx* dev, const blance_moves* mv, int32_t* op_round) {
+  CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(mv->total_ops, 1ll), dev->stream));
+  if (mv->sched_moves > 0)
+    launch(dev, k_expo_op_round, grid_for(dev, mv->sched_moves, 256), 256, 0, mv->sched_moves, mv->sched_rounds,
+           (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
+}
+
 // The exposure of the handle's last schedule (exposure.cuh; include/blance_b200.h).
 extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const blance_exposure_in* in, blance_exposure_out* out) {
   return entry(ctx, [&](Device& device) {
     const std::string name = "blance_moves_exposure";
-    if (!ctx || !mv || !in || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": ctx, moves, in or out is NULL");
-    if (mv->sched_rounds < 0 || !mv->sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": no schedule was computed on this handle");
+    check_moves_sched(name, ctx, mv, in, out);
     const int S = (int)mv->slot_off.size() - 1, SL = mv->slot_off[(size_t)S];
-    if (S > BL_S_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 8 states");
-    if (SL > BL_SLP_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 32 slots per row");
     if (S > 0 && !in->state_constraints) throw_err(BLANCE_ERR_INVALID_ARG, name + ": state_constraints is NULL");
     for (int s = 0; s < S; ++s)
       if (in->state_constraints[s] < 0) throw_err(BLANCE_ERR_INVALID_ARG, name + ": negative state constraint");
@@ -3331,7 +3433,7 @@ extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const bl
     blance_ctx* dev = device();
     cudaStream_t st = dev->stream;
     const int P = mv->n_parts, R = mv->sched_rounds;
-    const long long T = mv->total_ops, M = mv->sched_moves, R1 = (long long)R + 1;
+    const long long T = mv->total_ops, R1 = (long long)R + 1;
     const int V = NU + in->n_domains;
     const bool dom = out->dom_peak || out->dom_peak_round;
     // the one-instance, CSR case of the engine: every partition, the handle's beg rows
@@ -3359,8 +3461,7 @@ extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const bl
     E.op_round = op_round; E.dom_parent = b.parent;
     CUDA(cudaEventRecord(dev->ev[0], st));
     if (b.parent) CUDA(cudaMemcpyAsync(b.parent, in->domain_parent, sizeof(int32_t) * (size_t)V, cudaMemcpyHostToDevice, st));
-    CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(T, 1ll), st));
-    if (M > 0) launch(dev, k_expo_op_round, grid_for(dev, M, 256), 256, 0, M, R, (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
+    moves_op_round(dev, mv, op_round);
     const ExpoResult r = expo_run(dev, E, inst, dom ? b.dom_key : nullptr, b.ev_off);
     CUDA(cudaEventRecord(dev->ev[1], st));
     std::vector<unsigned long long> h_key(dom ? (size_t)V : 0);
@@ -3378,15 +3479,12 @@ extern "C" int blance_moves_exposure(blance_ctx* ctx, blance_moves* mv, const bl
   });
 }
 
-// Each node's load over the handle's last schedule (node_load.cu in libblance_b200_load.so; include/blance_b200.h).
+// Each node's load over the handle's last schedule (node_load.cuh; include/blance_b200.h).
 extern "C" int blance_moves_load(blance_ctx* ctx, blance_moves* mv, const blance_load_in* in, blance_load_out* out) {
   return entry(ctx, [&](Device& device) {
     const std::string name = "blance_moves_load";
-    if (!ctx || !mv || !in || !out) throw_err(BLANCE_ERR_INVALID_ARG, name + ": ctx, moves, in or out is NULL");
-    if (mv->sched_rounds < 0 || !mv->sched) throw_err(BLANCE_ERR_INVALID_ARG, name + ": no schedule was computed on this handle");
+    check_moves_sched(name, ctx, mv, in, out);
     const int S = (int)mv->slot_off.size() - 1, SL = mv->slot_off[(size_t)S];
-    if (S > BL_S_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 8 states");
-    if (SL > BL_SLP_MAX) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": more than 32 slots per row");
     const int P = mv->n_parts, NU = mv->n_node_ids, R = mv->sched_rounds;
     const long long T = mv->total_ops, M = mv->sched_moves;
     std::vector<int32_t> weight(in->part_weight ? (size_t)P : 0);
@@ -3405,54 +3503,28 @@ extern "C" int blance_moves_load(blance_ctx* ctx, blance_moves* mv, const blance
     if (nk >= (1ll << 32)) throw_err(BLANCE_ERR_UNSUPPORTED, name + ": (n_states + 1) x n_node_ids reaches 2^32");
     blance_ctx* dev = device();
     cudaStream_t st = dev->stream;
-    blance_load::LoadArgs A{};
+    // the one-instance, CSR case of the engine: every partition, the handle's beg rows
+    std::vector<blance_load::LoadArgs> args(1, blance_load::LoadArgs{});
+    blance_load::LoadArgs& A = args[0];
     A.beg = mv->d_beg; A.op_off = mv->d_off; A.op_node = mv->d_node; A.op_state = mv->d_state; A.op_kind = mv->d_kind;
     A.stride = SL; A.P = P; A.S = S; A.SL = SL; A.NU = NU;
     for (int s = 0; s <= S; ++s) A.slot_off[s] = mv->slot_off[(size_t)s];
     int32_t *op_round = nullptr, *d_weight = nullptr;
     const size_t K = (size_t)std::max(nk, 1ll);
-    CUDA(blance_load::load_scan_bytes(P, &A.scan_tmp_bytes, st));
+    A.scan_tmp_bytes = load_scan_bytes(P, st);
+    LoadBufs b;
     Arena a;
     a.add(op_round, (size_t)std::max(T, 1ll));
     if (!weight.empty()) a.add(d_weight, (size_t)P);
-    a.add(A.node_beg, K); a.add(A.node_end, K); a.add(A.node_peak, K); a.add(A.node_peak_round, K); a.add(A.peak_key, K);
-    a.add(A.over_key, 1); a.add(A.ev_count, (size_t)P + 1); a.add(A.ev_off, (size_t)P + 1); a.add(A.scan_tmp, A.scan_tmp_bytes);
+    a.add(b.node_beg, K); a.add(b.node_end, K); a.add(b.node_peak, K); a.add(b.node_peak_round, K); a.add(b.peak_key, K);
+    a.add(b.over_key, 1); a.add(b.ev_count, (size_t)P + 1); a.add(b.ev_off, (size_t)P + 1); a.add(A.scan_tmp, A.scan_tmp_bytes);
     a.alloc(st, "the load");
     A.op_round = op_round; A.weight = d_weight;
     CUDA(cudaEventRecord(dev->ev[0], st));
     if (d_weight) CUDA(cudaMemcpyAsync(d_weight, weight.data(), sizeof(int32_t) * (size_t)P, cudaMemcpyHostToDevice, st));
-    CUDA(cudaMemsetAsync(op_round, 0xFF, sizeof(int32_t) * (size_t)std::max(T, 1ll), st));
-    if (M > 0) launch(dev, k_expo_op_round, grid_for(dev, M, 256), 256, 0, M, R, (const long long*)mv->round_off, (const long long*)mv->sched_op, op_round);
-    CUDA(blance_load::load_count(A, dev->sm_count, st, &dev->launches));
-    long long NE = 0;
-    CUDA(cudaMemcpyAsync(&NE, A.ev_off + P, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    CUDA(cudaStreamSynchronize(st));
-    // the events, sized exactly; keys ((n (S + 1) + s) << 32) | t
-    int key_bits = 1;
-    while ((1ll << key_bits) < nk) ++key_bits;
-    Arena ev;
-    if (NE > 0) {
-      CUDA(blance_load::load_event_bytes(NE, key_bits, &A.ev_tmp_bytes, st));
-      const size_t n = (size_t)NE;
-      ev.add(A.ev_key, n); ev.add(A.ev_key2, n); ev.add(A.run_key, n); ev.add(A.ev_val, n); ev.add(A.ev_val2, n);
-      ev.add(A.run_val, n); ev.add(A.run_sum, n); ev.add(A.n_runs, 1); ev.add(A.ev_tmp, A.ev_tmp_bytes);
-      ev.alloc(st, "the load's events");
-    }
-    CUDA(blance_load::load_peaks(A, NE, key_bits, dev->sm_count, st, &dev->launches));
-    CUDA(cudaEventRecord(dev->ev[1], st));
-    unsigned long long over = 0;
-    const size_t kb = sizeof(int64_t) * (size_t)nk;
-    if (nk > 0) {
-      if (out->node_beg) CUDA(cudaMemcpyAsync(out->node_beg, A.node_beg, kb, cudaMemcpyDeviceToHost, st));
-      if (out->node_end) CUDA(cudaMemcpyAsync(out->node_end, A.node_end, kb, cudaMemcpyDeviceToHost, st));
-      if (out->node_peak) CUDA(cudaMemcpyAsync(out->node_peak, A.node_peak, kb, cudaMemcpyDeviceToHost, st));
-      if (out->node_peak_round) CUDA(cudaMemcpyAsync(out->node_peak_round, A.node_peak_round, sizeof(int32_t) * (size_t)nk, cudaMemcpyDeviceToHost, st));
-    }
-    CUDA(cudaMemcpyAsync(&over, A.over_key, sizeof over, cudaMemcpyDeviceToHost, st));
-    CUDA(cudaStreamSynchronize(st));
+    moves_op_round(dev, mv, op_round);
+    load_run(dev, args, b, {out}, dev->ev[1]);
     out->rounds = R;
-    out->over_max = NU > 0 ? (int64_t)(over >> 32) : 0;
-    out->over_node = NU > 0 ? (int32_t)(0xFFFFFFFFu - (uint32_t)over) : -1;
     out->kernel_ms = 0.f;
     cudaEventElapsedTime(&out->kernel_ms, dev->ev[0], dev->ev[1]);
   });

@@ -1,12 +1,12 @@
 """blance_moves_load on the device: equal, field for field, to the literal replay on random move lists (with and
 without weights), to the vectorised oracle on the synthetic configurations and on the full-size headline rebalance,
-countStateNodes of the beg and end maps at both ends, the argument errors, and the launch counts of the schedule and
-the exposure unchanged by it.  The first launches of libblance_b200_load.so's kernels on the ctx stream happen
-here.  Needs an H100; run with -m gpu."""
+countStateNodes of the beg and end maps at both ends, the argument errors, the load's own launch count, and the
+launch counts of the schedule and the exposure unchanged by it.  Needs an H100; run with -m gpu."""
 import numpy as np
 import pytest
 
 import load_oracle as LO
+from exposure_oracle import beg_entries
 from test_exposure_gpu import SCHEDULE_LAUNCHES
 from test_exposure_oracle import random_case
 from test_load_oracle import random_weights
@@ -147,19 +147,48 @@ def test_edges(ctx):
     ctx.moves_free(h)
 
 
+def has_events(slot_off, beg, op_off, op_node, op_state, op_kind, sched_op, NN):
+    """Whether the load of unit weights has an event: an op scheduled before its partition's first unscheduled one, on
+    a node in range, that changes the node's entries of some state."""
+    S = len(slot_off) - 1
+    done = np.zeros(len(op_node), bool)
+    done[np.asarray(sched_op, np.int64)] = True
+    for p in range(len(op_off) - 1):
+        live = beg_entries(slot_off, beg[p])
+        for k in range(op_off[p], op_off[p + 1]):
+            if not done[k]:
+                break
+            n = int(op_node[k])
+            before = [live.count((n, s)) for s in range(S)]
+            live = [e for e in live if e[0] != n]
+            after = [int(op_kind[k] != LO.DEL and s == op_state[k]) for s in range(S)]
+            if 0 <= n < NN and before != after:
+                return True
+    return False
+
+
 @pytest.mark.parametrize("case", sorted(SCHEDULE_LAUNCHES))
 def test_schedule_and_exposure_launches_are_unchanged(ctx, case):
     seed, P, NN, c = case
     slot_off, beg, end, cons, top, _ = random_case(np.random.default_rng(seed), P=P, NN=NN)
-    h, _ = ctx.moves_create(slot_off, beg, end, False, NN)
-    expo = []
+    h, total = ctx.moves_create(slot_off, beg, end, False, NN)
+    expo, load = [], []
     for _ in range(2):                       # before and after a load on the handle
         n0 = ctx.kernel_launches()
-        ctx.moves_schedule(h, c)
+        _, so, sc = ctx.moves_schedule(h, c)
         assert ctx.kernel_launches() - n0 == SCHEDULE_LAUNCHES[case]
         n0 = ctx.kernel_launches()
         ctx.moves_exposure(h, cons, top)
         expo.append(ctx.kernel_launches() - n0)
+        n0 = ctx.kernel_launches()
         ctx.moves_load(h)
+        load.append(ctx.kernel_launches() - n0)
     assert expo[0] == expo[1]
+    # the load's own kernels (CUB's are not counted): the op rounds when the schedule moved anything, walk<0> over the
+    # partitions, init and final over the (state, node) keys, walk<1> when there are events and peak when there are
+    # merged runs, which every event starts or joins
+    M = sc["moves_done"]
+    ev = has_events(slot_off, beg, *ctx.moves_fetch(h, total), so[:M], NN)
+    want = (M > 0) + (P > 0) + (len(slot_off) * NN > 0) * (2 + 2 * ev)
+    assert ev and load == [want, want], (ev, load, want)
     ctx.moves_free(h)

@@ -1,12 +1,10 @@
 """Each node's load while a rebalance runs (blance_moves_load), CPU side: the literal replay against the vectorised
 oracle on random move lists scheduled by tests/schedule_oracle.c, hand-derived cases, the reference's
 CalcPartitionMoves goldens replayed as one-partition rebalances, the argument errors that need no device, and what
-libblance_b200_load.so exports and compiles to."""
+the load kernels compile to."""
 import ctypes
 import json
 import os
-import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -15,6 +13,7 @@ import pytest
 import load_oracle as LO
 import schedule_oracle as SO
 from test_exposure_oracle import ADD, DEL, DEMOTE, NONE, PROMOTE, calc_moves, random_case
+from test_sass_guard import kernels  # noqa: F401  (the parsed SASS, a module-scoped fixture)
 
 from blance_b200 import abi, build
 
@@ -192,45 +191,13 @@ def test_struct_layout_matches_header(tmp_path):
                    abi.LoadOut.over_max.offset, abi.LoadOut.over_node.offset, abi.LoadOut.kernel_ms.offset]
 
 
-def test_load_library_exports_only_its_launchers():
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm is not available")
-    syms = subprocess.run([nm, "-D", "--defined-only", build.load_lib_path()], stdout=subprocess.PIPE, text=True, check=True).stdout
-    names = sorted(l.split()[-1] for l in syms.splitlines() if l.strip())
-    launchers = ("10load_count", "10load_peaks", "15load_scan_bytes", "16load_event_bytes")   # mangled blance_load::...
-    assert len(names) == 4 and all(n.startswith("_ZN11blance_load") for n in names), names
-    assert sorted(next(x for x in launchers if x in n) for n in names) == sorted(launchers), names
+def test_the_library_needs_no_second_native_library():
+    out = subprocess.run(["readelf", "-d", build.lib_path()], stdout=subprocess.PIPE, text=True, check=True).stdout
+    assert "NEEDED" in out and "libblance_b200_load.so" not in out
 
 
-def test_main_library_links_the_load_library():
-    out = subprocess.run(["readelf", "-d", build.lib_path()], stdout=subprocess.PIPE, text=True).stdout
-    assert "libblance_b200_load.so" in out and "$ORIGIN" in out
-
-
-@pytest.fixture(scope="module")
-def load_kernels():
-    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    try:
-        txt = subprocess.run([cuobjdump, "-sass", build.load_lib_path()], stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True,
-                             timeout=300).stdout
-    except (OSError, subprocess.TimeoutExpired):
-        pytest.skip("cuobjdump is not available")
-    if "Function :" not in txt:
-        pytest.skip("cuobjdump printed no SASS")
-    out, name = {}, None
-    for line in txt.split("\n"):
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            out[name] = []
-        elif name and re.match(r"\s*/\*[0-9a-f]{4,6}\*/", line):
-            out[name].append(line)
-    return {k: "\n".join(v) for k, v in out.items()}
-
-
-def test_load_kernels_use_reductions_and_no_atomics(load_kernels):
-    own = {k: b for k, b in load_kernels.items() if "k_load_" in k}
+def test_load_kernels_in_the_library_use_reductions_and_no_atomics(kernels):  # noqa: F811
+    own = {k: "\n".join(b) for k, b in kernels.items() if "k_load_" in k}
     assert len(own) == 5, sorted(own)          # walk<0|1>, init, peak, final
     for k, body in own.items():
         assert "ATOMG" not in body, k
